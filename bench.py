@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Benchmark of the THA4 poser hot path on B200 (contract: see the task's bench.py section).
+"""Benchmark of the THA4 poser hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W [--impl reference|torch_cuda] [--workload ...] [--no-extras]
+                    [--dump-outputs DIR]
 
 A "step" is one poser forward over one batch of synthetic input.  The headline workload is BASELINE.json configs[1]:
 the full five-network poser (mode_07), batch 1 per GPU, the lambda_00 character image, one random pose per step,
@@ -16,7 +17,7 @@ frames/sec.  Rank 0 prints ONE JSON line:
                (HBM bound), the kernel BASELINE.json's metric names;
   cpu_baseline the CPU oracle (a PyTorch-CPU port of the reference path, oracle/) on this box's host cores.
 
-and -- so that every BASELINE config is on the driver's record -- sub-objects measured in the same run:
+and -- so that every BASELINE config is in the record -- sub-objects measured in the same run:
 
   torch_cuda_eager  configs[1] executed by PyTorch-CUDA eager (the oracle's ops on the GPU = what the reference's own
                     CUDA path dispatches): the denominator of BASELINE's ">= 30x" target;
@@ -26,6 +27,8 @@ and -- so that every BASELINE config is on the driver's record -- sub-objects me
                     the 1.33 MB flat gradient + Adam), per-GPU batch 1, 1000 steps at N = 8, with the final weights
                     compared against a single-process run of the same global batch.
 `--impl reference` times the CPU port alone, as the reference arm.
+`--dump-outputs DIR` writes what the timed path returned in its last timed step as DIR/<name>.npy (float32; inputs are
+seeded, so two builds run with the same arguments can be compared output for output).
 """
 import argparse
 import json
@@ -52,7 +55,7 @@ WORKLOADS = {
 }
 TEACHER_GFLOP_PER_FRAME = 625.9   # cache-hot (SURVEY.md section 8a)
 DISTILL_W, DISTILL_LR = [0.0, 1.0, 1.0, 0.0], 1e-4        # phase 1 of the body schedule: warp + grid-change terms (distiller_config.py:178-186)
-L2_NOTE = 'packed weights (657 MB teacher) and activations exceed the 126 MB L2; no explicit flush'
+L2_NOTE = 'packed weights (657 MB teacher) and activations exceed the 50 MB L2; no explicit flush'
 
 
 def config_for(workload, batch_per_gpu, world):
@@ -69,7 +72,7 @@ def load_peaks():
     if os.path.exists(path):
         p = json.load(open(path))
         return dict(hbm_gbs=p['hbm_gbs'], tflops=p['bf16_tflops'], tflops_sustained=p.get('bf16_tflops_sustained'), source='measured (MEASURED_PEAKS.json)')
-    return dict(hbm_gbs=6650.0, tflops=1590.0, tflops_sustained=1400.0, source='fallback (B200_PROFILING.md)')
+    return dict(hbm_gbs=3350.0, tflops=989.0, tflops_sustained=None, source='H100 SXM data sheet (HBM3, dense FP16/BF16), not measured')
 
 
 def load_ncu_traffic():
@@ -178,14 +181,11 @@ def run_reference(args, rank, world):
         if wl['mode'] == 'mode_07':     # eyebrow cache hot, as in the GPU arm (mode_07.py:56-68)
             dec = tha4_oracle.eyebrow_decomposer(sds['eyebrow_decomposer'], img_b[:, :, 64:192, 192:320])
             kw = dict(cached_decomposer_output=dec)
-        t_start = time.perf_counter()
         for i in range(args.warmup + args.steps):
             t0 = time.perf_counter()
             fn(sds, img_b, poses[(i * b) % 32:(i * b) % 32 + b], **kw)
             if i >= args.warmup:
                 times.append((time.perf_counter() - t0) / b)
-            if times and time.perf_counter() - t_start > 150.0:     # bounded sample: keep the arm within minutes
-                break
     spf = sum(times) / len(times)
     B = wl.get('batch', max(1, wl.get('total', 1) // world))
     line = {
@@ -194,8 +194,8 @@ def run_reference(args, rank, world):
         'scaling': 'strong' if 'total' in wl else 'weak', 'vs_baseline': None, 'dtype': 'f32', 'data': 'synthetic',
         'config': config_for(args.workload, B, world),
         'cpu_baseline': {'value': 1.0 / spf, 'unit': 'frames/s', 'cores': threads, 'kind': 'port',
-                         'sample': '%d timed steps (of %d requested) of %d frame(s) each of the same workload (PyTorch-CPU port of the reference path, '
-                                   '%d of %d host threads)' % (len(times), args.steps, per_step_frames, threads, os.cpu_count() or 1)},
+                         'sample': '%d timed steps of %d frame(s) each of the same workload (PyTorch-CPU port of the reference path, '
+                                   '%d of %d host threads)' % (len(times), per_step_frames, threads, os.cpu_count() or 1)},
         'e2e': {'value': 1.0 / spf, 'unit': 'frames/s', 'h2d_bytes_per_step': 0, 'd2h_bytes_per_step': 0},
         'gpu_launches': 0,
     }
@@ -321,9 +321,9 @@ def roofline_objects(prof, steps, peaks, traffic):
     if prof.get('conv', {}).get('us', 0) > 0:
         c = prof['conv']
         ach = c['flops'] / (c['us'] * 1e-6) / 1e12
-        out['roofline'] = {'kernel': 'conv_tc_kernel (implicit-GEMM conv: TMA + tcgen05.mma kind::f16/tf32, TMEM accumulator; all conv launches of the step)', 'bound': 'tensor', 'achieved': ach,
+        out['roofline'] = {'kernel': 'implicit-GEMM conv kernels (TMA + wgmma on f16 / tf32 operands, register accumulator; all conv launches of the step)', 'bound': 'tensor', 'achieved': ach,
                            'peak': peaks['tflops'], 'unit': 'TFLOP/s', 'frac': ach / peaks['tflops'], 'traffic': traffic.get('conv', {}).get('dram_bytes_per_launch'),
-                           'peak_source': peaks['source'] + ' dense bf16 burst (= the f16 operand rate; kind::tf32 layers peak at half of it)',
+                           'peak_source': peaks['source'] + '; dense f16 rate (tf32 layers peak at half of it)',
                            'avg_launch_us': c['us'] / max(1, c['launches']), 'launches_per_step': c['launches'] / steps,
                            'share_of_profiled_kernel_time': c['us'] / max(1.0, sum(v['us'] for v in prof.values()))}
     if prof.get('tail', {}).get('us', 0) > 0:
@@ -351,7 +351,13 @@ def main():
     ap.add_argument('--no-extras', action='store_true', help='skip the student / pose-sweep / distill / torch-eager sub-objects')
     ap.add_argument('--distill-steps', type=int, default=0, help='0: 1000 at N = 8 (BASELINE configs[4]), 200 otherwise')
     ap.add_argument('--option', action='append', default=[], help='library option name=value (developer A/B runs)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed step as DIR/<name>.npy (float32, at most 64 MB in all)')
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be at least 1')
+    if args.dump_outputs and args.impl != 'tha4_b200':
+        ap.error('--dump-outputs writes the outputs of the tha4_b200 path only')
     args.warmup = max(args.warmup, 3)
 
     rank = int(os.environ.get('RANK', '0'))
@@ -424,11 +430,16 @@ def main():
         l0 = ctx.counter('kernel_launches')
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
+        last = None
         for i in range(args.steps):
-            step_resident(args.warmup + i)
+            last = step_resident(args.warmup + i)
         e1.record()
         timer.barrier()
         ms = e0.elapsed_time(e1)
+        if args.dump_outputs and rank == 0:
+            # a training step returns nothing when losses are not requested: what it computed is the updated student
+            dump_outputs(args.dump_outputs, {'student_params': distiller.flat} if distiller is not None else
+                         {'out%02d' % k: t for k, t in enumerate(last)})
         launches = ctx.counter('kernel_launches') - l0
         clocks = sampler.stop()
 
@@ -539,10 +550,28 @@ def main():
         fps, nfr, dt = cpu_port_fps(wl['mode'], ssds if student_mode else tsds, image, poses, B, budget, threads)
         line['cpu_baseline'] = {'value': fps, 'unit': 'frames/s', 'cores': threads, 'kind': 'port',
                                 'sample': '%d frames of the same workload in %.1f s (PyTorch-CPU port of the reference path in oracle/, '
-                                          '%d of %d host threads; /root/reference itself is pure Python and does not exist on the GPU box)' % (nfr, dt, threads, os.cpu_count() or 1)}
+                                          '%d of %d host threads)' % (nfr, dt, threads, os.cpu_count() or 1)}
     emit(line)
     if world > 1:
         dist.destroy_process_group()
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, tensors):
+    """Writes each tensor as <out_dir>/<name>.npy in float32.  When everything would exceed DUMP_LIMIT_BYTES, a tensor gets
+    an equal share of the budget: a fixed, seeded sample of its flattened elements (sorted indices, seed 0), so that two
+    runs with the same arguments write the same elements."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    sample = sum(t.numel() for t in tensors.values()) * 4 > DUMP_LIMIT_BYTES
+    share = max(1, DUMP_LIMIT_BYTES // 4 // max(1, len(tensors)))
+    for name, t in tensors.items():
+        a = t.detach().float().cpu().numpy()
+        if sample and a.size > share:
+            a = a.reshape(-1)[np.sort(np.random.default_rng(0).choice(a.size, share, replace=False))]
+        np.save(os.path.join(out_dir, name + '.npy'), np.ascontiguousarray(a, dtype=np.float32))
 
 
 def run_extras(args, timer, rank, world, device, teacher, ctx, tsds, ssds, image, peaks, traffic):

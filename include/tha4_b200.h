@@ -1,4 +1,4 @@
-/* tha4_b200 -- C ABI of the B200-native THA4 poser hot path.
+/* tha4_b200 -- C ABI of the H100-native (sm_90a) THA4 poser hot path.
  *
  * The reference (pkhungurn/talking-head-anime-4-demo) is pure Python on PyTorch and has no FFI of its own
  * (SURVEY.md F1, section 8b): the seam it offers is Python duck-typing -- the `Poser` protocol
@@ -54,14 +54,13 @@ const char* tha4_last_error(const tha4_ctx* ctx);
  *                         pointers -- repeats is captured once and replayed as one graph launch, writing the caller's
  *                         tensors directly; the pose is staged, so its address may change),
  *          developer switches, default = the measured-best setting:
- *          "tcgen05" (1: convs on the tcgen05/TMA/TMEM kernels; 0: everything on mma.sync),
+ *          "tcgen05" (1: convs on the wgmma/TMA kernels; 0: everything on mma.sync; the name is historical),
  *          "half_operands" (1: f16 conv operands, normalisations fused into the consumer conv's operand path),
  *          "halo_conv" (1: 3x3 stride-1 convs on the halo-reuse kernel), "tma_store" (1: unsplit conv epilogue through TMA stores),
  *          "cluster_splitk" (1: K-split convs reduce through a thread-block cluster / DSMEM; 0: workspace + reduce kernel),
- *          "pdl" (1: programmatic dependent launch), "tc_stride2" (1: 4x4 stride-2 convs on tcgen05),
- *          "small_bn" (1: narrower N tiles for small unsplit launches), "siren_tc" (1: students on tcgen05; 0: mma.sync kernels),
+ *          "pdl" (1: programmatic dependent launch), "tc_stride2" (1: 4x4 stride-2 convs on the wgmma kernel),
+ *          "small_bn" (1: narrower N tiles for small unsplit launches), "siren_tc" (1: students on the wgmma kernels; 0: mma.sync kernels),
  *          "attn_split16", "attn_mma" (1: default-mode attention on mma.sync with f16 operands; 0: the fp32 kernel everywhere),
- *          "tail_persist" (1: persistent software-pipelined decoder tail; 0: one tile per CTA),
  *          "profile" (1: time every kernel class with CUDA events on the launching stream, 2: same + reset, 0: off).
  * "strict", "microbatch", "cuda_graphs" and "half_operands" belong to the context.  The other developer switches select
  * kernels PROCESS-WIDE (they are statics of the kernel translation units): changing one on any context changes it for all
@@ -184,7 +183,7 @@ int tha4_base_grid(int size, float* host_out);
 int tha4_test_conv(tha4_ctx* ctx, int kind, const float* x, const float* w, const float* bias, const float* res,
                    int res_mode, int in_up, float* y, int N, int Cin, int H, int W, int Cout, int strict, int ksplit,
                    void* stream);
-/* conv(act(norm(x))) with the normalisation FUSED into the tcgen05 conv's operand path (default mode of the networks):
+/* conv(act(norm(x))) with the normalisation FUSED into the wgmma conv's operand path (default mode of the networks):
  * x [N,Cin,H,W] is the raw tensor; its first norm_C channels are normalised (groups 0: InstanceNorm2d, else GroupNorm;
  * FiLM vectors film0 [2*norm_C] / film1 [N,2*norm_C] optional; act 0 none / 1 relu / 2 silu), the remaining channels
  * pass through.  y: fp32 output [N,Cout,Ho,Wo]; y_from_f16 (optional): the f16 copy the kernel writes, widened. */

@@ -1,7 +1,7 @@
 """How much does rounding conv operands to a 10-bit mantissa (what TF32 / f16 tensor-core operands carry) move the
 teacher's outputs on the seeded weights used by tests and bench?  Pure CPU experiment on the oracle: every
 conv2d / conv_transpose2d input and weight is rounded through float16, everything else stays fp32.
-Result committed as profiles/r02_cpu_10bit_sensitivity.txt (context for DESIGN.md section 4)."""
+Context for the default-mode tolerances (DESIGN.md)."""
 import os
 import sys
 

@@ -1,4 +1,4 @@
-"""Developer diagnostics for the tcgen05 conv kernel (not a pytest file): structured inputs that expose layout bugs."""
+"""Developer diagnostics for the wgmma conv kernel (option "tcgen05") (not a pytest file): structured inputs that expose layout bugs."""
 import math
 import sys
 import os

@@ -10,7 +10,7 @@ for _p in (ROOT, os.path.join(ROOT, 'tests')):
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a real B200 (run with -m gpu on the GPU box)')
+    config.addinivalue_line('markers', 'gpu: needs an H100 (run with -m gpu)')
 
 
 @pytest.fixture(scope='session')

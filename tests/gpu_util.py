@@ -36,7 +36,7 @@ def conv(kind, x, w, bias=None, res=None, res_mode=0, in_up=0, strict=1, ksplit=
 
 
 def conv_norm(kind, x, norm_C, groups, gamma, beta, film0, film1, act, w, bias=None, res=None, res_mode=0, ksplit=0):
-    """conv(act(norm(x))) through the fused-input-normalisation tcgen05 kernel; returns (fp32 output, f16 copy widened)."""
+    """conv(act(norm(x))) through the fused-input-normalisation wgmma kernel; returns (fp32 output, f16 copy widened)."""
     c = ctx()
     N, Cin, H, W = x.shape
     Cout = w.shape[1] if kind == 2 else w.shape[0]

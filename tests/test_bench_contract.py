@@ -1,7 +1,5 @@
 """bench.py contract checks that need no GPU: the reference arm runs here (CPU port of the reference path) and prints
-exactly one JSON line with the agreed keys; the bench lines committed under profiles/ carry every key the round-end
-driver reads (roofline / cpu_baseline / e2e / clocks / gpu_launches)."""
-import glob
+exactly one JSON line with the agreed keys; --dump-outputs writes float32 arrays within its size budget."""
 import json
 import os
 import subprocess
@@ -26,54 +24,20 @@ def test_reference_arm_prints_one_json_line():
     assert d['e2e'] == {'value': d['value'], 'unit': 'frames/s', 'h2d_bytes_per_step': 0, 'd2h_bytes_per_step': 0}
 
 
-def test_round2_default_bench_line_has_the_sub_objects():
-    """The round-2 default line (BASELINE configs[1]) carries the other configs as sub-objects and the >= 30x denominator."""
-    f = os.path.join(ROOT, 'profiles', 'r02_final_bench_default.json')
-    d = json.load(open(f))
-    assert BASE_KEYS <= set(d) and d['n_gpus'] == 1 and d['gpu_launches'] > 0
-    assert d['e2e']['value'] > 0 and d['e2e']['d2h_bytes_per_step'] == 512 * 512 * 4       # the uint8 frame
-    assert d['cpu_baseline']['kind'] == 'port' and d['cpu_baseline']['value'] > 0
-    for key in ('pose_sweep_512', 'distill', 'student_b64', 'torch_cuda_eager'):
-        assert key in d, key
-    assert d['pose_sweep_512']['scaling'] == 'strong' and d['pose_sweep_512']['frames_total'] == 512
-    assert d['distill']['steps_per_s'] > 0 and d['torch_cuda_eager_fps'] > 0
-    assert d['cuda_graphs']['replays'] > 0 and d['cuda_graphs']['failures'] == 0
-    for r in (d['roofline'], d['roofline_tail']):
-        assert r['bound'] in ('hbm', 'tensor') and abs(r['frac'] - r['achieved'] / r['peak']) < 1e-9
-    ref = json.load(open(os.path.join(ROOT, 'profiles', 'r02_final_bench_reference_arm.json')))
-    assert ref['impl'] == 'reference' and ref['config'] == d['config'], 'the two arms must print the same config'
-
-
-def test_round2_final_bench_line_if_committed():
-    """The bench line of the end of round 2 (second half), when its evidence run made it into profiles/."""
-    f = os.path.join(ROOT, 'profiles', 'r02b_final_bench_default.json')
-    if not os.path.exists(f):
-        return
-    d = json.load(open(f))
-    assert BASE_KEYS <= set(d) and d['n_gpus'] == 1 and d['gpu_launches'] > 0 and d['value'] > 0
-    assert d['e2e']['value'] > 0 and d['e2e']['d2h_bytes_per_step'] == 512 * 512 * 4
-    for key in ('pose_sweep_512', 'distill', 'student_b64', 'torch_cuda_eager', 'roofline', 'roofline_tail', 'cpu_baseline', 'clocks'):
-        assert key in d, key
-    assert not set(d['clocks']['reasons']) & {'hw_slowdown', 'hw_thermal_slowdown', 'sw_thermal_slowdown'}
-
-
-def test_committed_bench_lines_are_complete():
-    files = sorted(glob.glob(os.path.join(ROOT, 'profiles', 'r01_final_bench_*.json')))
-    assert files, 'round-1 bench lines missing from profiles/'
-    seen_default = False
-    for f in files:
-        d = json.load(open(f))
-        if d.get('impl') in ('reference', 'torch_cuda_eager'):
-            continue
-        assert BASE_KEYS <= set(d), (f, BASE_KEYS - set(d))
-        assert d['gpu_launches'] > 0 and d['e2e']['value'] > 0 and d['e2e']['h2d_bytes_per_step'] > 0, f
-        assert d['clocks']['sm_mhz'] and not set(d['clocks']['reasons']) & {'hw_slowdown', 'hw_thermal_slowdown', 'sw_thermal_slowdown'}, f
-        r = d['roofline']
-        assert r['bound'] in ('hbm', 'tensor') and r['unit'] in ('GB/s', 'TFLOP/s') and r['peak'] > 0, f
-        if r['achieved'] is not None:
-            assert abs(r['frac'] - r['achieved'] / r['peak']) < 1e-9, f
-        if os.path.basename(f) == 'r01_final_bench_teacher_b1.json':
-            seen_default = True
-            assert d['n_gpus'] == 1 and d['cpu_baseline']['value'] > 0 and d['cpu_baseline']['kind'] == 'port'
-            assert d['roofline_tail']['bound'] == 'hbm'
-    assert seen_default
+def test_dump_outputs_writes_float32_within_budget(tmp_path):
+    sys.path.insert(0, ROOT)
+    import numpy as np
+    import torch
+    import bench
+    big = {'a': torch.arange(3 * 1024 * 1024 * 4, dtype=torch.float32).reshape(4, -1), 'b': torch.ones(2, 3, dtype=torch.float64)}
+    limit = bench.DUMP_LIMIT_BYTES
+    bench.DUMP_LIMIT_BYTES = 1 << 20
+    try:
+        bench.dump_outputs(str(tmp_path / 'x'), big)
+        bench.dump_outputs(str(tmp_path / 'y'), big)
+    finally:
+        bench.DUMP_LIMIT_BYTES = limit
+    a, b = np.load(tmp_path / 'x' / 'a.npy'), np.load(tmp_path / 'x' / 'b.npy')
+    assert a.dtype == np.float32 and b.dtype == np.float32 and a.nbytes + b.nbytes <= 1 << 20
+    assert np.array_equal(a, np.load(tmp_path / 'y' / 'a.npy'))           # the same seeded sample every run
+    assert np.all(np.diff(a) > 0) and b.shape == (2, 3)                    # sorted indices of arange; small tensors stay whole

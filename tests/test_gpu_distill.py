@@ -1,4 +1,4 @@
-"""Distillation inner loop on the B200 (-m gpu): losses, flat gradient and post-Adam weights of the CUDA step against
+"""Distillation inner loop on the H100 (-m gpu): losses, flat gradient and post-Adam weights of the CUDA step against
 CPU autograd on the oracle (same student weights, same targets).
 
 Tolerances: the dense layers run TF32 products (as the reference's own CUDA path would for 1x1 convs) and L1 has a

@@ -1,4 +1,4 @@
-"""Kernel-level parity on the B200 (-m gpu): every CUDA kernel family against a plain fp32 PyTorch reference of the
+"""Kernel-level parity on the H100 (-m gpu): every CUDA kernel family against a plain fp32 PyTorch reference of the
 same op (CPU), and the grid_sample / interpolate index math bit-exactly against the C oracle."""
 import ctypes
 import math
@@ -104,7 +104,7 @@ CONV_CASES = [
     (0, 1, 528, 16, 512, False, 0, 0, 0),        # pose-concat bottleneck as the f16 path sees it (pose padded to 16)
     (0, 1, 544, 24, 512, False, 0, 0, 3),
     (3, 1, 512, 16, 1536, True, 0, 0, 0),        # attention qkv
-    (0, 1, 32, 512, 32, True, 1, 0, 0),          # > 444 tiles: persistent streaming kernel (ring + TMEM double buffer across tiles)
+    (0, 1, 32, 512, 32, True, 1, 0, 0),          # many tiles: several CTAs per SM
     (0, 2, 64, 256, 64, True, 1, 0, 0),
     (0, 3, 128, 200, 128, True, 0, 0, 0),        # streaming kernel with partial tiles in both directions
     (4, 1, 64, 128, 64, True, 2, 0, 0),          # 4 phases x 128 tiles
@@ -116,7 +116,7 @@ CONV_CASES = [
 @pytest.mark.parametrize('case', CONV_CASES)
 @pytest.mark.parametrize('path', ['strict_mma', 'tf32_tcgen05', 'f16_tcgen05', 'tf32_mma'])
 def test_conv_vs_torch(case, path):
-    """strict_mma: 3xTF32 mma.sync (== fp32); tf32_tcgen05: TMA + tcgen05.mma kind::tf32 where the configuration is
+    """strict_mma: 3xTF32 mma.sync (== fp32); tf32_tcgen05: TMA + wgmma on tf32 operands where the configuration is
     supported (stride-1 taps, no fused upsample), else mma.sync; f16_tcgen05: the same kernel with f16 operands
     (kind::f16, 128- or 64-byte rows) where Cin % 8 == 0, as the networks run it behind a normalisation layer;
     tf32_mma: single-TF32 mma.sync everywhere."""
@@ -184,7 +184,7 @@ CONV_NORM_CASES = [
 @pytest.mark.parametrize('halo', [1, 0])
 def test_conv_with_fused_input_norm(case, halo):
     """The default mode's conv: the pending normalisation (+FiLM, +activation) of the RAW f16 input is applied to the
-    operand tiles in shared memory between TMA and tcgen05.mma.  Reference: conv(act(norm(x))) in fp32.  Tolerance:
+    operand tiles in shared memory between TMA and wgmma.  Reference: conv(act(norm(x))) in fp32.  Tolerance:
     two f16 roundings of O(1) operands (raw value, normalised value) + tanh.approx SiLU, over a K-term dot product:
     6e-3 of the output's scale (same class as the separate-pass f16 path)."""
     kind, N, Cin, nC, H, Cout, groups, act, film, has_bias, res_mode, ksplit = case

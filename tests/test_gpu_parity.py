@@ -1,15 +1,15 @@
-"""Network- and poser-level parity on the B200 (-m gpu): the CUDA path, called through the reference-shaped Python
+"""Network- and poser-level parity on the H100 (-m gpu): the CUDA path, called through the reference-shaped Python
 API (which goes through the C ABI), against the CPU oracle on the same seeded weights / inputs, and against the
 committed golden fixtures produced by the unmodified reference.
 
 Tolerances (outputs live in [-1, 1]; stated per precision mode).  The seeded teacher weights are conditioned like
 trained ones (tha4_b200/synthetic.py), so the fp32 oracle is a well-conditioned yardstick: rounding every conv operand of
 the CPU oracle to a 10-bit mantissa moves each mode_07 output by <= 3e-4 mean / 1.4e-2 max
-(profiles/r02_cpu_10bit_sensitivity.txt).
+(scripts/dev/cpu_10bit_sensitivity.py).
   strict (3xTF32 products == fp32 convolution): single network: max-abs 2e-3, mean-abs 1e-4 over every output;
       whole poser (up to five chained networks, each warping the previous one's output): max-abs 3e-2, mean-abs 3e-4
       -- the max is set by isolated edge pixels where a ~5e-5 difference of a warp offset moves the sampling point.
-  default (the BENCHMARKED mode: tcgen05 convs on f16 / TF32 operands with a 10-bit mantissa, fp32 accumulation,
+  default (the BENCHMARKED mode: wgmma convs on f16 / TF32 operands with a 10-bit mantissa, fp32 accumulation,
       fast-math SiLU -- the class of PyTorch's own CUDA path with TF32 convs): every output of every network and of the
       whole poser: mean-abs <= 2e-3, max-abs <= 5e-2.
   student (fp16 tensor-core products, fp32 accumulation): mean-abs 4e-3 on images, 1e-3 on grid_change.
@@ -318,7 +318,7 @@ def test_student_modules_standalone(student_sds):
 
 
 def test_student_tcgen05_and_mma_paths_agree(lambda00_sds):
-    """The student runs on TMA + tcgen05 + TMEM by default (siren_tc.cu); the mma.sync kernels (siren.cu, option
+    """The student runs on TMA + wgmma by default (siren_tc.cu); the mma.sync kernels (siren.cu, option
     "siren_tc" = 0) are the same math in the same precision class (fp16 operands, fp32 accumulate): both must satisfy the
     student tolerances against the oracle and agree with each other."""
     poser = mode_14.create_poser(DEV, state_dicts=lambda00_sds)

@@ -103,7 +103,7 @@ __global__ void __launch_bounds__(QPB * KSPLIT) attention_kernel(const float* __
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Default-mode attention on the tensor cores (mma.sync m16n8k16, f16 operands, fp32 accumulate).  The kernel above is one
-// dependent 32-FMA chain per (query, key) with two warps per scheduler: 23 us per launch, 12 launches per frame, for
+// dependent 32-FMA chain per (query, key) with two warps per scheduler, 12 launches per frame for
 // 0.07 GFLOP each.  Here a warp owns 16 queries of one (sample, head): S = Q K^T for all 256 keys stays in registers as
 // 32 accumulator tiles, the softmax runs on the fragments (row max / sum over the 4 lanes of a quad), and the accumulator
 // layout of two adjacent S tiles IS the A-fragment layout of P for the P V product (the FlashAttention-2 register identity).

@@ -58,8 +58,8 @@ struct tha4_ctx {
     }
     std::string err;
     int strict = 0;
-    int microbatch = 32;                   // frames per internal pass (measured: 4 -> 276, 8 -> 325, 16 -> 363-366, 32 -> 384 frames/s)
-    int half_operands = 1;                 // f16 conv operands between normalisation and tcgen05 conv (non-strict mode)
+    int microbatch = 32;                   // frames per internal pass
+    int half_operands = 1;                 // f16 conv operands between normalisation and wgmma conv (non-strict mode)
     Pool persist, scratch;
     int* flag = nullptr;
     double* loss_acc = nullptr;            // 4 doubles: L1 sums of the distillation step
@@ -202,7 +202,7 @@ int tha4_ctx_create(int device, tha4_ctx** out) {
         THA4_CUDA_CHECK(cudaSetDevice(device));
         cudaDeviceProp prop;
         THA4_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
-        THA4_REQUIRE(prop.major == 10, "tha4_b200 is built for sm_100a (B200) only; found sm_" + std::to_string(prop.major) + std::to_string(prop.minor));
+        THA4_REQUIRE(prop.major == 9 && prop.minor == 0, "tha4_b200 is built for sm_90a (H100) only; found sm_" + std::to_string(prop.major) + std::to_string(prop.minor));
         auto* ctx = new tha4_ctx();
         ctx->device = device;
         THA4_CUDA_CHECK(cudaMalloc(&ctx->flag, sizeof(int)));
@@ -738,7 +738,7 @@ int tha4_test_norm(tha4_ctx* ctx, const float* x, int N, int C, int H, int W, in
         View yo = xin; yo.stats = nullptr;
         if (pool) { yo.H = H / 2; yo.W = W / 2; }
         yo.p = P->alloc((size_t)N * yo.H * yo.W * C);
-        if (out_f16) {     // the variant the default mode runs: f16 output (operand of a tcgen05 conv), fast-math SiLU
+        if (out_f16) {     // the variant the default mode runs: f16 output (operand of a wgmma conv), fast-math SiLU
             View y16 = yo; y16.f16 = 1; y16.p = P->alloc(((size_t)N * yo.H * yo.W * C + 1) / 2);
             norm_apply_fused(xin, groups, gamma, beta, film0, film1, 2 * C, act == ACT_SILU ? ACT_SILU_FAST : act, pool, nullptr, y16, s, 1);
             convert_f32(y16, yo, s);
@@ -780,7 +780,7 @@ int tha4_test_tail(tha4_ctx* ctx, int kind, const float* feature, int N, int C, 
         const int a = (act == ACT_SILU && !strict) ? ACT_SILU_FAST : act;
         const ImgView i0 = make_img(image0, N, 4, S, S);
         const ImgView i1 = image1 ? make_img(image1, N, 4, S, S) : ImgView{};
-        if (!strict && rt.f16) {      // the default mode's kernel: raw f16 feature map + statistics -> tcgen05 tail
+        if (!strict && rt.f16) {      // the default mode's kernel: raw f16 feature map + statistics -> wgmma tail
             { SinkScope own(&sink); tail_make_half(tw, s); }
             View f16v = f; f16v.f16 = 1; f16v.p = P->alloc(((size_t)N * S * S * C + 1) / 2);
             convert_f16(f, f16v, s);

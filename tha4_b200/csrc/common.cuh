@@ -1,4 +1,4 @@
-// Shared declarations for the tha4_b200 CUDA library (sm_100a only).
+// Shared declarations for the tha4_b200 CUDA library (sm_90a: H100).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -21,7 +21,7 @@ struct View {
     float* p = nullptr;
     int N = 0, H = 0, W = 0, C = 0, ld = 0;
     // f16 == 1: `p` really addresses __half elements (ld still counts elements).  Only the normalisation kernels write
-    // such tensors and only the tcgen05 conv reads them (kind::f16 operands: same 10-bit mantissa as TF32, half the
+    // such tensors and only the wgmma conv reads them (kind::f16 operands: same 10-bit mantissa as TF32, half the
     // operand bytes); everything else requires f16 == 0.
     int f16 = 0;
     // Optional per-(n,c) statistics of this tensor: stats[(n * stats_ld + c) * 2 + {0: sum, 1: sum of squares}] (doubles),
@@ -75,6 +75,13 @@ struct CudaError : std::runtime_error { using std::runtime_error::runtime_error;
 // configured per device (a process may hold contexts on several GPUs), not per process.
 constexpr int THA4_MAX_DEVICES = 64;
 inline int current_device() { int d = 0; cudaGetDevice(&d); return d < 0 || d >= THA4_MAX_DEVICES ? 0 : d; }
+// streaming multiprocessors of the current device (132 on an H100 SXM): launch plans size their grids by it
+inline int num_sms() {
+    static int sms[THA4_MAX_DEVICES] = {};
+    const int d = current_device();
+    if (!sms[d]) { cudaDeviceGetAttribute(&sms[d], cudaDevAttrMultiProcessorCount, d); if (sms[d] <= 0) sms[d] = 132; }
+    return sms[d];
+}
 #define THA4_ENSURE_SMEM(kernel, bytes)                                                           \
     do {                                                                                          \
         static size_t _cfg[tha4::THA4_MAX_DEVICES] = {};                                          \
@@ -94,7 +101,7 @@ inline int current_device() { int d = 0; cudaGetDevice(&d); return d < 0 || d >=
 // Programmatic dependent launch: a kernel launched through launch_pdl may start while its predecessor in the stream is
 // still running; it must execute pdl_wait() before touching global memory (blocks until every earlier grid has
 // completed and flushed) and should execute pdl_trigger() once it holds its resources (so that the NEXT kernel's
-// prologue -- barrier init, TMEM allocation, descriptor prefetch, launch latency -- overlaps this one's body).
+// prologue -- barrier init, descriptor prefetch, launch latency -- overlaps this one's body).
 #ifdef __CUDACC__
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;\n" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;\n" ::: "memory"); }
@@ -150,7 +157,7 @@ __device__ __forceinline__ float act_apply(float v, int act) {
     if (act == ACT_SILU_FAST) return __fdividef(v, 1.0f + __expf(-v));
     return v;
 }
-// round-to-nearest TF32 (10-bit mantissa) as the tensor cores would ideally see it; tcgen05 kind::tf32 truncates the
+// round-to-nearest TF32 (10-bit mantissa) as the tensor cores would ideally see it; wgmma kind::tf32 truncates the
 // low mantissa bits of what it reads, so producers of conv operands round once when they write (non-strict mode).
 __device__ __forceinline__ float round_tf32(float v) {
     unsigned r;
@@ -159,8 +166,8 @@ __device__ __forceinline__ float round_tf32(float v) {
 }
 __device__ __forceinline__ float sigmoid_f(float v) { return 1.0f / (1.0f + expf(-v)); }
 // (sum, sum of squares) of one channel folded over the statistics replicas.  The loads are issued eight at a time before
-// any of them is consumed: a dependent chain of up to 16 L2 round trips (~0.4 us each) per channel was the single
-// largest item in the prologue of every kernel that rebuilds a normalisation affine (profiles/r02_ncu_tail_tc_v1.txt).
+// any of them is consumed: a dependent chain of up to 16 L2 round trips per channel was the single
+// largest item in the prologue of every kernel that rebuilds a normalisation affine.
 __device__ __forceinline__ double2 fold_stat_replicas(const double* __restrict__ p, long rep_stride, int rep) {
     double su = 0.0, sq = 0.0;
     for (int r0 = 0; r0 < rep; r0 += 8) {

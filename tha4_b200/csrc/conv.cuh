@@ -49,7 +49,7 @@ void conv_pack(const ConvWeights& cw, ConvKind kind, const float* w_ref, int w_c
 void conv_set_pack_rounding(bool round_tf32);   // applies to subsequent conv_pack calls (set from the context's strict option)
 bool conv_pack_rounding();
 
-// Pending normalisation of the conv's INPUT, applied by the tcgen05 kernel to its f16 operand tiles in shared memory
+// Pending normalisation of the conv's INPUT, applied by the wgmma kernel to its f16 operand tiles in shared memory
 // (conv_tc.cu, XF kernels): y = act(A_c x + B_c) with (A, B) built per CTA from the statistics the producing conv
 // accumulated -- InstanceNorm2d (groups == 0) / GroupNorm(groups), eps 1e-5, affine, up to two FiLM scale-shifts.
 // Replaces a separate normalisation pass (one launch + one read and one write of the tensor) per conv.
@@ -67,7 +67,7 @@ struct ConvArgs {
     int in_up = 0;              // nearest-neighbour x2 upsample fused into the gather (unet.py:46)
     View out;                   // geometry + statistics slot of the output; out.p may be null when only the f16 copy is wanted
     View out16;                 // optional f16 copy of the output (out16.p == nullptr: none)
-    ConvNormIn nin;             // fused normalisation of the input (tcgen05 kernel, f16 input only)
+    ConvNormIn nin;             // fused normalisation of the input (wgmma kernel, f16 input only)
     View res;                   // residual added in the epilogue (res.p == nullptr: none)
     int res_mode = RES_NONE;    // RES_UP2: res stored at half resolution; RES_DOWN2: res at double resolution (2x2 mean)
     int strict = 0;             // 1: 3xTF32 error-compensated products (fp32-equivalent); 0: single TF32
@@ -76,16 +76,16 @@ struct ConvArgs {
     size_t ws_floats = 0;
 };
 
-// Floats of workspace the tcgen05 kernel wants for this call (0: none needed / not the tcgen05 path).
+// Floats of workspace the wgmma kernel wants for this call (0: none needed / not the wgmma path).
 size_t conv_workspace_floats(const ConvWeights& cw, const ConvArgs& a);
 
 // out = conv(in) + bias (+ res).  When the launch splits K, `out` is zeroed first on the same stream.
-// Dispatches to the tcgen05 kernel (conv_tc.cu) when it supports the configuration, else to the mma.sync kernel.
+// Dispatches to the wgmma kernel (conv_tc.cu) when it supports the configuration, else to the mma.sync kernel.
 void conv_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s);
 void conv_mma_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s);     // conv.cu (general shapes, strict mode)
 bool conv_tc_supported(const ConvWeights& cw, const ConvArgs& a);
-void conv_tc_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s);      // conv_tc.cu (tcgen05 + TMA + TMEM)
-// True when conv_forward(cw, a) will itself accumulate a.out.stats (tcgen05 epilogue / split-K reduction); otherwise
+void conv_tc_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s);      // conv_tc.cu (wgmma + TMA)
+// True when conv_forward(cw, a) will itself accumulate a.out.stats (wgmma epilogue / split-K reduction); otherwise
 // the caller runs norm_stats on the output.
 bool conv_fuses_stats(const ConvWeights& cw, const ConvArgs& a);
 bool conv_tc_fuses_stats(const ConvWeights& cw, const ConvArgs& a);
@@ -101,6 +101,6 @@ bool conv_tc_enabled();
 void conv_make_half(const ConvWeights& cw, cudaStream_t s);   // f16 copy of the packed weights (cw.w16), recorded in the active AllocSink
 void conv_tc_enable_cluster(bool on);
 void conv_tc_enable_small_bn(bool on);  // narrower N tiles for tiny unsplit GEMMs
-void conv_tc_enable_stride2(bool on);   // stride-2 4x4 convs on the tcgen05 kernel (element-strided TMA) instead of mma.sync
+void conv_tc_enable_stride2(bool on);   // stride-2 4x4 convs on the wgmma kernel (element-strided TMA) instead of mma.sync
 
 }  // namespace tha4

@@ -1,15 +1,15 @@
-// 3x3 (stride 1, pad 1) convolution on tcgen05 with HALO REUSE -- the kernel behind most of the teacher's FLOPs in the
+// 3x3 (stride 1, pad 1) convolution on wgmma with HALO REUSE -- the kernel behind most of the teacher's FLOPs in the
 // default mode (both 3x3 convs of every U-Net ResBlock, the eleven 512 -> 512 bottleneck convs of the encoder-decoder nets).
 //
 // conv_tc.cu fetches one 128-pixel x 64-channel activation box PER TAP (9 boxes per channel chunk) and, with the fused
 // input normalisation, transforms each of them.  Here the CTA tile is 8 x 16 pixels and one TMA box {64 ch, 10 w, 18 h}
 // brings in the tile's 10 x 18 HALO once per channel chunk; the nine taps are nine VIEWS of that shared-memory image:
-// the UMMA A-descriptor start address is shifted by ((dy + 1) * 10 + (dx + 1)) pixel rows and the stride between 8-row
+// the wgmma A-descriptor start address is shifted by ((dy + 1) * 10 + (dx + 1)) pixel rows and the stride between 8-row
 // groups (SBO) is the halo pitch (10 rows) -- the tensor core applies the 128-/64-byte swizzle on absolute shared-memory
-// addresses, so row-shifted views of a TMA-written image are legal (profiles/r02_umma_row_shift_probe.txt).
+// addresses, so row-shifted views of a TMA-written image are legal.
 //   * activation traffic L2 -> shared memory per channel chunk: 180 rows instead of 9 x 128 (6.4x less);
 //   * the pending normalisation (XF: GroupNorm / InstanceNorm affine + FiLM + SiLU / ReLU of the RAW f16 input) is
-//     applied to 180 rows once instead of 1152 rows, by the four warps that later drain the accumulator;
+//     applied to 180 rows once instead of 1152 rows, by the consumer warpgroup that issues the MMAs;
 //   * weights stream per (chunk, tap) through their own TMA ring, pre-issued ahead of the programmatic-dependency wait;
 //   * K (channel chunks) can be split over a thread-block cluster, partials meeting in distributed shared memory
 //     (same epilogues as conv_tc.cu: conv_tc_device.cuh).
@@ -33,12 +33,6 @@ using namespace tcdev;
 constexpr int HT_W = 8, HT_H = 16;                 // CTA tile: 8 x 16 = 128 output pixels
 constexpr int HALO_W = HT_W + 2, HALO_H = HT_H + 2, HALO_ROWS = HALO_W * HALO_H;     // 10 x 18 = 180 pixel rows
 
-__device__ __forceinline__ uint64_t make_desc_sbo(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t layout) {
-    const uint32_t lo = ((smem_addr & 0x3FFFF) >> 4) | (1u << 16);
-    const uint32_t hi = (sbo_bytes >> 4) | (1u << 14) | (layout << 29);
-    return ((uint64_t)hi << 32) | lo;
-}
-
 __host__ __device__ constexpr int halo_a_bytes(int rowb) { return ((HALO_ROWS * rowb + 1023) / 1024) * 1024; }
 
 // SA / SB: stages of the activation-halo ring / of the weight-tile ring.  OP: OP_F16 (64 channels per chunk, 128-byte rows)
@@ -46,31 +40,28 @@ __host__ __device__ constexpr int halo_a_bytes(int rowb) { return ((HALO_ROWS * 
 // MINB: resident CTAs per SM the register allocation must allow (4 for the single-chunk unsplit variants, whose small
 // rings fit four times: the layers at 256x256 / 512x512 are chains of dependent latencies, more CTAs = more overlap)
 __host__ __device__ constexpr int halo_min_ctas(int bn, int sa, int cs, int op) {
-    return cs > 1 ? 1 : ((sa == (op == OP_F16N ? 2 : 1) && bn <= 64) ? 4 : (bn >= 128 ? 2 : 3));
+    return cs > 1 || bn >= 128 ? 1 : ((sa == (op == OP_F16N ? 2 : 1) && bn <= 32) ? 4 : 2);
 }
 template <int BN, int SA, int SB, int CS, int OP, int XF>
 __global__ void __launch_bounds__(TC_THREADS, halo_min_ctas(BN, SA, CS, OP)) conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                                                                 const __grid_constant__ CUtensorMap tmO32, const __grid_constant__ CUtensorMap tmO16,
                                                                 const __grid_constant__ CUtensorMap tmR, const TcParams p) {
     static_assert(OP != OP_TF32, "halo kernel: f16 operands");
+    static_assert(BN <= 128, "the accumulator of one warpgroup: BN registers per thread");
     constexpr int ROWB = op_row_bytes(OP);
     constexpr int KCE = op_kch(OP);
     constexpr int A_BYTES = halo_a_bytes(ROWB);
     constexpr int B_BYTES = BN * ROWB;
-    constexpr int TMEM_COLS = BN < 32 ? 32 : BN;
-    constexpr uint32_t LAYOUT = ROWB == 128 ? 2u : 4u;
     constexpr int NSLOT = CS == 1 ? epi_nslot(BN, (size_t)SA * A_BYTES + (size_t)SB * B_BYTES) : 0;     // TMA-store staging slots of the unsplit epilogue
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);      // pointer arithmetic (not an integer round trip) keeps the shared address space: LDS / STS, not generic LD / ST
     uint8_t* smA = smem;
     uint8_t* smB = smem + SA * A_BYTES;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smB + SB * B_BYTES);
-    uint64_t* a_full = bars, *a_empty = bars + SA, *a_xf = bars + 2 * SA;
-    uint64_t* b_full = bars + 3 * SA, *b_empty = b_full + SB;
-    uint64_t* t_full = b_empty + SB;
-    uint64_t* res_bars = t_full + 1;                                     // [4]: residual tiles of the unsplit epilogue (epi_direct)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_bars + 4);
-    float* xf_A = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(tmem_slot + 4) + ((16u - (tc::smem_u32(tmem_slot + 4) & 15u)) & 15u));
+    uint64_t* a_full = bars, *a_empty = bars + SA;
+    uint64_t* b_full = bars + 2 * SA, *b_empty = b_full + SB;
+    uint64_t* res_bars = b_empty + SB;                                   // [4]: residual tiles of the unsplit epilogue (epi_direct)
+    float* xf_A = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(res_bars + 4) + ((16u - (tc::smem_u32(res_bars + 4) & 15u)) & 15u));
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // developer timing: CTA `slot` of every 97 records clock64 at its phase boundaries (8 stamps per role: dbg[slot][role][8])
@@ -91,27 +82,20 @@ __global__ void __launch_bounds__(TC_THREADS, halo_min_ctas(BN, SA, CS, OP)) con
     const int nb = nc * 9;                                               // weight tiles of this CTA
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < SA; ++s) { mbar_init(smem_u32(a_full + s), 1); mbar_init(smem_u32(a_empty + s), 1); mbar_init(smem_u32(a_xf + s), 128); }
-        for (int s = 0; s < SB; ++s) { mbar_init(smem_u32(b_full + s), 1); mbar_init(smem_u32(b_empty + s), 1); }
-        mbar_init(smem_u32(t_full), 1);
+        // the empty barriers take one arrival per consumer thread: every thread arrives once its own wgmma wait has returned
+        for (int s = 0; s < SA; ++s) { mbar_init(smem_u32(a_full + s), 1); mbar_init(smem_u32(a_empty + s), 128); }
+        for (int s = 0; s < SB; ++s) { mbar_init(smem_u32(b_full + s), 1); mbar_init(smem_u32(b_empty + s), 128); }
         for (int s = 0; s < 4; ++s) mbar_init(smem_u32(res_bars + s), 1);
         asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
         asm volatile("prefetch.tensormap [%0];\n" :: "l"(&tmA) : "memory");
         asm volatile("prefetch.tensormap [%0];\n" :: "l"(&tmB) : "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" :: "r"(smem_u32(tmem_slot)), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
     if (threadIdx.x == 0) HSTAMP(0, 1);
     pdl_trigger();
     // weight tiles of the first ring pass do not depend on the previous kernel: fetch them ahead of the dependency wait
     const int npre = p.pre_b ? min(nb, SB) : 0;
-    if (warp == 0 && lane == 0) {
+    if (warp == TC_PRODUCER_WARP && lane == 0) {
         for (int i = 0; i < npre; ++i) {
             const uint32_t full = smem_u32(b_full + i);
             mbar_expect_tx(full, B_BYTES);
@@ -121,8 +105,9 @@ __global__ void __launch_bounds__(TC_THREADS, halo_min_ctas(BN, SA, CS, OP)) con
     pdl_wait();
     if (threadIdx.x == 0) HSTAMP(0, 2);
 
+    Acc<BN> acc;
     if (nc > 0) {
-        if (warp == 0) {
+        if (warp == TC_PRODUCER_WARP) {
             if (lane == 0) {   // ===== TMA producer: one halo box per chunk, nine weight tiles per chunk =====
                 int bi = 0;
                 for (int ci = 0; ci < nc; ++ci) {
@@ -139,49 +124,26 @@ __global__ void __launch_bounds__(TC_THREADS, halo_min_ctas(BN, SA, CS, OP)) con
                     }
                 }
             }
-        } else if (warp == 1) {
-            if (lane == 0) {   // ===== MMA issuer: 9 taps = 9 row-shifted views of the halo =====
-                constexpr uint32_t idesc = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((128u >> 4) << 24);     // f16 x f16 -> f32, K-major, M = 128
-                int bi = 0;
-                for (int ci = 0; ci < nc; ++ci) {
-                    const int sa = ci % SA;
-                    mbar_wait(smem_u32((XF ? a_xf : a_full) + sa), (ci / SA) & 1);
-                    if (ci == 0) HSTAMP(1, 0);
-                    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-                    const uint32_t a_base = smem_u32(smA + sa * A_BYTES);
-                    for (int tap = 0; tap < 9; ++tap, ++bi) {
-                        const int sb = bi % SB;
-                        mbar_wait(smem_u32(b_full + sb), (bi / SB) & 1);
-                        asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-                        const int shift = (p.dy[0][tap] + 1) * HALO_W + (p.dx[0][tap] + 1);
-                        const uint64_t adesc = make_desc_sbo(a_base + shift * ROWB, HALO_W * ROWB, LAYOUT);
-                        const uint64_t bdesc = make_smem_desc_sw<ROWB>(smem_u32(smB + sb * B_BYTES));
-#pragma unroll
-                        for (int k = 0; k < ROWB / 32; ++k)
-                            umma_f16(tmem_base, adesc + 2 * k, bdesc + 2 * k, idesc, (ci > 0 || tap > 0 || k > 0) ? 1u : 0u);
-                        umma_commit(smem_u32(b_empty + sb));
-                    }
-                    umma_commit(smem_u32(a_empty + sa));                  // the halo of this chunk is free when its 9 taps retire
-                }
-                umma_commit(smem_u32(t_full));
-                HSTAMP(1, 1);
-            }
         } else {
-            if (XF) {          // ===== warps 2-5: normalise each chunk's halo ONCE, in place; then they are the epilogue =====
-                const int te = threadIdx.x - 64;
-                __half* hA = reinterpret_cast<__half*>(xf_A);
-                __half* hB = hA + p.xf_C;
+            // ===== consumer warpgroup: normalise each chunk's halo ONCE, in place (XF); 9 taps = 9 row-shifted views of the
+            // halo through wgmma; then the epilogue =====
+            const int te = threadIdx.x;
+            __half* hA = reinterpret_cast<__half*>(xf_A);
+            __half* hB = hA + p.xf_C;
+            const bool silu = p.xf_act == ACT_SILU || p.xf_act == ACT_SILU_FAST;
+            if (XF) {
                 double2* chs = reinterpret_cast<double2*>(xf_A + 2 * p.xf_C);
                 xf_build_coef(p, n, te, hA, hB, chs, cb0 * KCE, (cb0 + nc) * KCE);
                 if (te == 0) HSTAMP(2, 0);
-                const bool silu = p.xf_act == ACT_SILU || p.xf_act == ACT_SILU_FAST;
-                for (int ci = 0; ci < nc; ++ci) {
-                    const int sa = ci % SA;
-                    mbar_wait(smem_u32(a_full + sa), (ci / SA) & 1);
-                    if (te == 0 && ci == 0) HSTAMP(2, 1);
+            }
+            int bi = 0;
+            for (int ci = 0; ci < nc; ++ci) {
+                const int sa = ci % SA;
+                mbar_wait(smem_u32(a_full + sa), (ci / SA) & 1);
+                if (te == 0 && ci == 0) HSTAMP(2, 1);
+                if (XF) {
                     const int c0 = (cb0 + ci) * KCE;
-                    // items = (halo row, half row): 360 items over 128 threads (3 at most) instead of 180 whole rows (2 at most:
-                    // 52 threads did twice the work of the others and set the length of the stage)
+                    // items = (halo row, half row): 360 items over 128 threads
                     constexpr int HC = ROWB / 32;                                             // chunks per half row
                     for (int it = te; it < 2 * HALO_ROWS; it += 128) {
                         const int row = it >> 1, half = it & 1;
@@ -191,35 +153,61 @@ __global__ void __launch_bounds__(TC_THREADS, halo_min_ctas(BN, SA, CS, OP)) con
                         const int swz = ROWB == 128 ? (row & 7) : ((row >> 1) & 3);
                         xf_chunks<HC>(smA + sa * A_BYTES + row * ROWB, swz, half * HC, c0, p, hA, hB, silu);
                     }
-                    asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
-                    mbar_arrive(smem_u32(a_xf + sa));
+                    asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");   // generic-proxy writes -> wgmma's async-proxy reads
+                    asm volatile("bar.sync 1, 128;\n" ::: "memory");
                     if (te == 0 && ci == nc - 1) HSTAMP(2, 2);
                 }
+                const uint32_t a_base = smem_u32(smA + sa * A_BYTES);
+                // unrolled: the wait depth and the arrivals below depend on the tap only, so no branch separates wgmma issue
+                // from its wait (a data-dependent one makes ptxas serialise the wgmma)
+#pragma unroll
+                for (int tap = 0; tap < 9; ++tap, ++bi) {
+                    const int sb = bi % SB;
+                    mbar_wait(smem_u32(b_full + sb), (bi / SB) & 1);
+                    const int shift = (p.dy[0][tap] + 1) * HALO_W + (p.dx[0][tap] + 1);
+                    // rows 0-63 of the tile are tile rows 0-7 (halo rows from `shift`), rows 64-127 tile rows 8-15 (8 halo pitches on)
+                    const uint32_t a0 = a_base + shift * ROWB, a1 = a0 + 8 * HALO_W * ROWB;
+                    const uint32_t b_addr = smem_u32(smB + sb * B_BYTES);
+                    wg_fence();
+#pragma unroll
+                    for (int k = 0; k < ROWB / 32; ++k) {
+                        const uint64_t bd = make_smem_desc_sw<ROWB>(b_addr + 32 * k);
+                        const uint32_t accum = (ci > 0 || tap > 0 || k > 0) ? 1u : 0u;
+                        Wgmma<BN>::f16(acc.d[0], make_desc_sbo<ROWB>(a0 + 32 * k, HALO_W * ROWB), bd, accum);
+                        Wgmma<BN>::f16(acc.d[1], make_desc_sbo<ROWB>(a1 + 32 * k, HALO_W * ROWB), bd, accum);
+                    }
+                    wg_commit();
+                    if (tap < 8) {
+                        wg_wait<1>();                                           // the previous tap's weight tile has been read
+                        if (tap > 0) mbar_arrive(smem_u32(b_empty + (bi - 1) % SB));
+                    } else {
+                        wg_wait<0>();                                           // the chunk's halo and its last two weight tiles are free
+                        mbar_arrive(smem_u32(b_empty + (bi - 1) % SB));
+                        mbar_arrive(smem_u32(b_empty + bi % SB));
+                        mbar_arrive(smem_u32(a_empty + sa));
+                    }
+                }
             }
-            if (threadIdx.x == 64) { mbar_wait(smem_u32(t_full), 0); HSTAMP(2, 3); }
-            if (CS > 1) { mbar_wait(smem_u32(t_full), 0); asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }   // own accumulator complete
-            else epi_direct<BN, HT_W, NSLOT>(p, tmem_base, smem, smem_u32(t_full), n, y0, x0, n0, 0, 0, warp, lane, &tmO32, &tmO16, &tmR, res_bars);
-            if (threadIdx.x == 64) HSTAMP(2, 4);
+            wg_fence_acc(acc.d[0]); wg_fence_acc(acc.d[1]);
+            if (te == 0) { HSTAMP(1, 1); HSTAMP(2, 3); }
+            if (CS == 1) epi_direct<BN, HT_W, NSLOT>(p, acc, smem, n, y0, x0, n0, 0, 0, warp, lane, &tmO32, &tmO16, &tmR, res_bars);
+            if (te == 0) HSTAMP(2, 4);
         }
     }
     if (CS > 1) {
         // barrier A: every CTA of the cluster has its accumulator and idle pipeline buffers -> peers may write into them
         asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
         asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
-        if (threadIdx.x == 64) HSTAMP(2, 5);
-        if (warp >= 2 && nc > 0) epi_push_partial<BN, CS>(tmem_base, smem, split, warp, lane);
+        if (threadIdx.x == 0) HSTAMP(2, 5);
+        if (warp < TC_PRODUCER_WARP && nc > 0) epi_push_partial<BN, CS>(acc, smem, split, warp, lane);
         // barrier B: the pushed slices are visible to their owners; nobody touches a peer's memory afterwards
         asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
         asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
-        if (threadIdx.x == 64) HSTAMP(2, 7);
-        if (warp >= 2) epi_cluster_reduce<BN, CS, HT_W>(p, smem, n, y0, x0, n0, 0, split, warp, dbg);
-        if (threadIdx.x == 64) HSTAMP(2, 6);
+        if (threadIdx.x == 0) HSTAMP(2, 7);
+        if (warp < TC_PRODUCER_WARP) epi_cluster_reduce<BN, CS, HT_W>(p, smem, n, y0, x0, n0, 0, split, warp, dbg);
+        if (threadIdx.x == 0) HSTAMP(2, 6);
     }
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
     __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" :: "r"(tmem_base), "r"(TMEM_COLS) : "memory");
-    }
     if (threadIdx.x == 0) HSTAMP(0, 3);
 #undef HSTAMP
 }
@@ -309,19 +297,20 @@ HaloPlan halo_plan(const ConvWeights& cw, const ConvArgs& a, int op) {
     pl.tiles_x = ceil_div(a.out.W, HT_W); pl.tiles_y = ceil_div(a.out.H, HT_H);
     pl.tiles_m = pl.tiles_x * pl.tiles_y * a.in.N;
     pl.chunks = cw.cin_pad / op_kch(op);
-    pl.bn = (cw.cout_pad % 256 == 0) ? 256 : (cw.cout_pad % 128 == 0 ? 128 : (cw.cout_pad % 64 == 0 ? 64 : 32));
+    // N tile: at most 128 columns, the accumulator of one consumer warpgroup (BN fp32 registers per thread)
+    pl.bn = (cw.cout_pad % 128 == 0) ? 128 : (cw.cout_pad % 64 == 0 ? 64 : 32);
+    const int sms = num_sms();
     pl.cs = 1;
     long ctas = (long)pl.tiles_m * (cw.cout_pad / pl.bn);
     if (a.ksplit > 1) {
         while (pl.cs * 2 <= std::min(8, a.ksplit)) pl.cs *= 2;
-    } else if (a.ksplit <= 0 && ctas < 120) {
+    } else if (a.ksplit <= 0 && ctas < sms * 13 / 16) {
         // Too few tiles to fill the GPU.  Narrow the N tiles first (down to 64 columns: more CTAs and nothing to exchange),
         // then split the channel chunks over a cluster.  The DSMEM exchange moves 128 x bn x 4 x (cs-1)/cs bytes per CTA at
-        // ~11 B/clk: at bn = 256, cs = 4..8 it took twice as long as the MMA phase it parallelised (10 000 vs 4 700 cycles,
-        // profiles/r02_halo_phase_stamps.txt).
-        while (pl.bn > 64 && (long)pl.tiles_m * (cw.cout_pad / pl.bn) < 148 && cw.cout_pad % (pl.bn / 2) == 0) pl.bn /= 2;
+        // a few bytes per clock, so a wide split of a wide tile costs more than the MMA phase it parallelises.
+        while (pl.bn > 64 && (long)pl.tiles_m * (cw.cout_pad / pl.bn) < sms && cw.cout_pad % (pl.bn / 2) == 0) pl.bn /= 2;
         ctas = (long)pl.tiles_m * (cw.cout_pad / pl.bn);
-        const int want = std::max(2, (int)((222 + ctas - 1) / ctas));       // >= 2: the cluster variants carry the deep weight ring
+        const int want = std::max(2, (int)((3 * sms / 2 + ctas - 1) / ctas));       // >= 2: the cluster variants carry the deep weight ring
         while (pl.cs < 8 && pl.cs * 2 <= want && pl.cs * 2 <= pl.chunks) pl.cs *= 2;
         while (pl.bn > 32 && (long)pl.tiles_m * (cw.cout_pad / pl.bn) * pl.cs < 96 && cw.cout_pad % (pl.bn / 2) == 0) pl.bn /= 2;
     }
@@ -334,7 +323,7 @@ template <int OP, int BN, int SA, int SB, int CS, int XF>
 void launch_halo(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo32, const CUtensorMap& mo16, const CUtensorMap& mr, const TcParams& p, dim3 grid, cudaStream_t s) {
     constexpr int ROWB = op_row_bytes(OP);
     constexpr size_t ring = (size_t)SA * halo_a_bytes(ROWB) + (size_t)SB * BN * ROWB;
-    constexpr size_t smem0 = 1024 + ring + (3 * SA + 2 * SB + 1 + 4) * 8 + 16;
+    constexpr size_t smem0 = 1024 + ring + (2 * SA + 2 * SB + 4) * 8 + 16;
     static_assert(smem0 <= 227 * 1024, "shared memory budget");
     static_assert(ring >= (size_t)4 * 32 * 33 * 4 + 4 * BN * 8, "epilogue scratch must fit in the pipeline buffers");
     static_assert(CS == 1 || ring >= (size_t)128 * BN * 4 + 128 * 8 * 4 + 128 * 4 * 4, "partial tile + statistics scratch must fit");
@@ -343,13 +332,6 @@ void launch_halo(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap
     THA4_ENSURE_SMEM((conv_halo_kernel<BN, SA, SB, CS, OP, XF>), smem);
     launch_pdl(conv_halo_kernel<BN, SA, SB, CS, OP, XF>, grid, dim3(TC_THREADS), smem, s, CS, ma, mb, mo32, mo16, mr, p);
     THA4_LAUNCH_CHECK();
-}
-
-int halo_num_sms() {
-    static int sms[THA4_MAX_DEVICES] = {};
-    const int d = current_device();
-    if (!sms[d]) THA4_CUDA_CHECK(cudaDeviceGetAttribute(&sms[d], cudaDevAttrMultiProcessorCount, d));
-    return sms[d];
 }
 
 // SBD: weight-ring depth of the cluster split-K launches (few CTAs per SM, the ring is what hides the DRAM latency of weights
@@ -366,10 +348,9 @@ void launch_halo_cs(int cs, const CUtensorMap& ma, const CUtensorMap& mb, const 
     if (cs == 8) launch_halo<OP, BN, SA, SBD, 8, XF>(ma, mb, mo32, mo16, mr, p, grid, s);
     else if (cs == 4) launch_halo<OP, BN, SA, SBD, 4, XF>(ma, mb, mo32, mo16, mr, p, grid, s);
     else if (cs == 2) launch_halo<OP, BN, SA, SBD, 2, XF>(ma, mb, mo32, mo16, mr, p, grid, s);
-    else if ((long)grid.x * grid.y * grid.z <= halo_num_sms())
+    else if ((long)grid.x * grid.y * grid.z <= num_sms())
         // unsplit and at most one CTA per SM (e.g. 256 -> 256 channels at 128 x 128: 128 tiles): nothing shares the SM, so the
-        // CTA takes the deep weight ring.  With two 32 KB stages the MMA phase of that layer ran at 294 cycles per 128 x 256 x 16
-        // MMA (28 B/clk/SM of weights from L2; the tensor pipe needs 128 cycles): profiles/r02_halo_phase_stamps.txt, section F
+        // CTA takes the deep weight ring: with a two-stage ring the MMAs wait on weight tiles streaming from L2
         launch_halo<OP, BN, SA, SBD, 1, XF>(ma, mb, mo32, mo16, mr, p, grid, s);
     else launch_halo<OP, BN, SA, SBS, 1, XF>(ma, mb, mo32, mo16, mr, p, grid, s);
 }
@@ -377,10 +358,9 @@ void launch_halo_cs(int cs, const CUtensorMap& ma, const CUtensorMap& mb, const 
 template <int OP, int XF>
 void launch_halo_bn(int bn, int cs, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo32, const CUtensorMap& mo16, const CUtensorMap& mr, const TcParams& p, dim3 grid, cudaStream_t s) {
     constexpr int M = OP == OP_F16N ? 2 : 1;        // 64-byte rows: twice the stages for the same bytes in flight
-    if (bn == 256) launch_halo_cs<OP, 256, 2 * M, 4 * M, 2 * M, XF>(cs, ma, mb, mo32, mo16, mr, p, grid, s);        // unsplit: 111 KB -> 2 CTAs / SM
-    else if (bn == 128) launch_halo_cs<OP, 128, 2 * M, 6 * M, 3 * M, XF>(cs, ma, mb, mo32, mo16, mr, p, grid, s);   // unsplit:  95 KB -> 2 CTAs / SM
-    else if (bn == 64) launch_halo_cs<OP, 64, 2 * M, 8 * M, 3 * M, XF>(cs, ma, mb, mo32, mo16, mr, p, grid, s);     // unsplit:  71 KB -> 3 CTAs / SM
-    else launch_halo_cs<OP, 32, 2 * M, 9 * M, 5 * M, XF>(cs, ma, mb, mo32, mo16, mr, p, grid, s);                    // unsplit:  67 KB -> 3 CTAs / SM
+    if (bn == 128) launch_halo_cs<OP, 128, 2 * M, 6 * M, 3 * M, XF>(cs, ma, mb, mo32, mo16, mr, p, grid, s);        // unsplit:  95 KB
+    else if (bn == 64) launch_halo_cs<OP, 64, 2 * M, 8 * M, 3 * M, XF>(cs, ma, mb, mo32, mo16, mr, p, grid, s);     // unsplit:  71 KB
+    else launch_halo_cs<OP, 32, 2 * M, 9 * M, 5 * M, XF>(cs, ma, mb, mo32, mo16, mr, p, grid, s);                    // unsplit:  67 KB
 }
 
 bool g_use_halo = true;
@@ -486,7 +466,7 @@ void conv_halo_debug_dump() {
         const long long* d = h.data() + c * 32;
         if (!d[0]) continue;
         auto rel = [&](long long v) { return v ? (long)(v - d[0]) : -1L; };
-        fprintf(stderr, "halo slot %2d: tmem %ld pdl %ld | coef %ld a_full %ld xf_done %ld | mma_first %ld mma_commit %ld | t_full %ld epi_done %ld | bar_A %ld pushed+bar_B %ld (loads issued %ld stored %ld) reduce_done %ld | end %ld\n",
+        fprintf(stderr, "halo slot %2d: init %ld pdl %ld | coef %ld a_full %ld xf_done %ld | mma_first %ld mma_commit %ld | t_full %ld epi_done %ld | bar_A %ld pushed+bar_B %ld (loads issued %ld stored %ld) reduce_done %ld | end %ld\n",
                 c, rel(d[1]), rel(d[2]), rel(d[16]), rel(d[17]), rel(d[18]), rel(d[8]), rel(d[9]), rel(d[19]), rel(d[20]), rel(d[21]), rel(d[23]), rel(d[25]), rel(d[24]), rel(d[22]), rel(d[3]));
     }
 }

@@ -1,17 +1,16 @@
-// Implicit-GEMM convolution on the 5th-generation tensor cores: TMA-staged operands, tcgen05.mma (kind::f16 on f16
-// operands, kind::tf32 on fp32 operands) with the accumulator in TMEM, warp-specialised producer / MMA-issuer /
-// epilogue roles.
+// Implicit-GEMM convolution on the Hopper tensor cores: TMA-staged operands, wgmma (f16 operands at K = 16, fp32 operands
+// as TF32 at K = 8) with the accumulator in the registers of one consumer warpgroup, and a TMA producer warp.
 //
 // GEMM view per CTA: D[128 pixels x BN couts] += A[128 x KC] * B[BN x KC]^T per k-block, k-blocks = taps x (Cin/KC),
 // KC = 64 f16 / 32 f16 / 32 fp32 channels (128- or 64-byte rows, see OP_* below).
 //  * A (activations, NHWC): one 4-D TMA box {KC ch, 16 w, 8 h, 1 n} per (tap, channel chunk).  The box lands in shared
-//    memory as 128 rows with the 128-byte (64-byte) swizzle, which is exactly the canonical K-major UMMA layout; the
+//    memory as 128 rows with the 128-byte (64-byte) swizzle, which is exactly the K-major wgmma operand layout; the
 //    tap offset (dy,dx) is just a shift of the box origin, and TMA's out-of-bounds zero fill *is* the convolution's
 //    zero padding (and the channel / edge-tile padding).  No im2col buffer, no index arithmetic.  The 4x4 stride-2
 //    conv uses the same box with element strides {1,2,2,1} (a {KC, 32 w, 16 h} window sampled every other pixel).
 //  * B (weights, packed [phase*tap][cout_pad][cin_pad]): 3-D TMA box {KC cin, BN cout, 1 tap}, same layout.
-//  * D: fp32 accumulator in tensor memory (BN columns x 128 lanes), drained by 4 epilogue warps with tcgen05.ld,
-//    bias / residual fused, NHWC stores + per-channel statistics for the normalisation that follows.
+//  * D: fp32 accumulator, 128 x BN (BN <= 128: BN registers per thread), two m64 wgmmas per K step; bias / residual fused
+//    into the epilogue, NHWC stores + per-channel statistics for the normalisation that follows.
 //  * K can be split over a thread-block cluster (partials meet in distributed shared memory), launches use
 //    programmatic dependent launch with the weight tiles fetched ahead of the dependency wait.
 // Handles every tap table of conv.cuh (3x3, 1x1, 4x4 stride 2, the four phases of the transposed 4x4 and of the
@@ -36,20 +35,18 @@ using namespace tcdev;
 template <int BN, int STAGES_, int CS, int OP, int XF>
 __global__ void __launch_bounds__(TC_THREADS) conv_tc_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                const __grid_constant__ CUtensorMap tmB, const TcParams p) {
+    static_assert(BN <= 128, "the accumulator of one warpgroup: BN registers per thread");
     constexpr int STAGES = op_stages(OP, STAGES_);
     constexpr int ROWB = op_row_bytes(OP);
     constexpr int KCE = op_kch(OP);
-    constexpr int A_BYTES1 = 128 * ROWB;
+    constexpr int A_BYTES = 128 * ROWB;
     constexpr int B_BYTES = BN * ROWB;
-    constexpr int A_BYTES = A_BYTES1;
-    constexpr int TMEM_COLS = BN < 32 ? 32 : BN;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);      // pointer arithmetic (not an integer round trip) keeps the shared address space: LDS / STS, not generic LD / ST
     uint8_t* smA = smem;
     uint8_t* smB = smem + STAGES * A_BYTES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smB + STAGES * B_BYTES);   // full[STAGES], empty[STAGES], tmem_full, xf[STAGES]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * STAGES + 1);
-    float* xf_A = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(tmem_slot + 4) + ((16u - (tc::smem_u32(tmem_slot + 4) & 15u)) & 15u));   // XF: per-channel affine y = act(A * x + B), [xf_C] each
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smB + STAGES * B_BYTES);   // full[STAGES], empty[STAGES]
+    float* xf_A = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars + 2 * STAGES) + ((16u - (tc::smem_u32(bars + 2 * STAGES) & 15u)) & 15u));   // XF: per-channel affine y = act(A * x + B), [xf_C] each
     static_assert(XF == 0 || OP != OP_TF32, "the fused input normalisation works on f16 operands");
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -68,27 +65,17 @@ __global__ void __launch_bounds__(TC_THREADS) conv_tc_kernel(const __grid_consta
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; ++s) { mbar_init(smem_u32(bars + s), 1); mbar_init(smem_u32(bars + STAGES + s), 1); }
-        mbar_init(smem_u32(bars + 2 * STAGES), 1);
-        if (XF) for (int s = 0; s < STAGES; ++s) mbar_init(smem_u32(bars + 2 * STAGES + 1 + s), 128);   // all transform threads arrive
         asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
         asm volatile("prefetch.tensormap [%0];\n" :: "l"(&tmA) : "memory");
         asm volatile("prefetch.tensormap [%0];\n" :: "l"(&tmB) : "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" :: "r"(smem_u32(tmem_slot)), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
     // resources are held: let the next kernel of the stream start its prologue, then wait for our own producers.
     // The WEIGHT tiles of the first ring pass do not depend on the previous kernel: their TMA loads are issued before
-    // the dependency wait, so the DRAM round trip of the weights (they do not fit in L2 at B=1) overlaps the
-    // predecessor's tail instead of following it.
+    // the dependency wait, so the DRAM round trip of the weights overlaps the predecessor's tail instead of following it.
     pdl_trigger();
     const int npre = p.pre_b ? min(nk, STAGES) : 0;
-    if (warp == 0 && lane == 0) {
+    if (warp == TC_PRODUCER_WARP && lane == 0) {
         for (int i = 0; i < npre; ++i) {
             const uint32_t full = smem_u32(bars + i);
             mbar_expect_tx(full, A_BYTES + B_BYTES);
@@ -99,8 +86,9 @@ __global__ void __launch_bounds__(TC_THREADS) conv_tc_kernel(const __grid_consta
     }
     pdl_wait();
 
+    Acc<BN> acc;
     if (nk > 0) {
-        if (warp == 0) {
+        if (warp == TC_PRODUCER_WARP) {
             if (lane == 0) {   // ===== TMA producer =====
                 for (int i = 0; i < nk; ++i) {
                     const int s = i % STAGES;
@@ -116,62 +104,51 @@ __global__ void __launch_bounds__(TC_THREADS) conv_tc_kernel(const __grid_consta
                     tma_load_4d(smem_u32(smA + s * A_BYTES), &tmA, c0, x0 * p.in_mul + p.dx[phase][tap], y0 * p.in_mul + p.dy[phase][tap], n, full);
                 }
             }
-        } else if (warp == 1) {
-            if (lane == 0) {   // ===== MMA issuer (single thread) =====
-                // instruction descriptor: D=f32, A=B=tf32 (format 2) or f16 (format 0), both K-major, N = BN, M = 128
-                constexpr uint32_t fmt = OP == OP_TF32 ? 2u : 0u;
-                constexpr uint32_t idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(BN >> 3) << 17) | ((128u >> 4) << 24);
-                for (int i = 0; i < nk; ++i) {
-                    const int s = i % STAGES;
-                    mbar_wait(smem_u32(bars + (XF ? 2 * STAGES + 1 + s : s)), (i / STAGES) & 1);     // XF: operands are ready once transformed
-                    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-                    const uint64_t adesc = make_smem_desc_sw<ROWB>(smem_u32(smA + s * A_BYTES));
-                    const uint64_t bdesc = make_smem_desc_sw<ROWB>(smem_u32(smB + s * B_BYTES));
-#pragma unroll
-                        for (int k = 0; k < ROWB / 32; ++k) {  // one MMA consumes 32 bytes of K per row (8 tf32 / 16 f16): advance the start address by 2 (>>4)
-                            if (OP == OP_TF32)
-                                umma_tf32(tmem_base, adesc + 2 * k, bdesc + 2 * k, idesc,
-                                          (i > 0 || k > 0) ? 1u : 0u);
-                            else
-                                umma_f16(tmem_base, adesc + 2 * k, bdesc + 2 * k, idesc,
-                                         (i > 0 || k > 0) ? 1u : 0u);
-                        }
-                    umma_commit(smem_u32(bars + STAGES + s));          // frees the smem slot when these MMAs retire
-                }
-                umma_commit(smem_u32(bars + 2 * STAGES));              // accumulator complete -> epilogue
-            }
         } else {
-          if (XF) {      // ===== warps 2-5 first normalise the A operand of every k-block in place, then become the epilogue =====
-            const int te = threadIdx.x - 64;                              // 0..127 = tile row (pixel) this thread owns
-            // the affine is applied with packed half2 arithmetic (HFMA2, tanh.approx.f16x2): the operand is f16 anyway, the
-            // in-place pass costs a third of the fp32 version's issue slots and half its MUFU slots
+            // ===== consumer warpgroup: (XF: normalise the A operand of the k-block in place), wgmma, then the epilogue =====
+            const int te = threadIdx.x;                                   // 0..127 = tile row (pixel) this thread owns
             __half* hA = reinterpret_cast<__half*>(xf_A);
             __half* hB = hA + p.xf_C;
-            double2* chs = reinterpret_cast<double2*>(xf_A + 2 * p.xf_C); // per-channel (sum, sum of squares) folded over the replicas
-            int c_lo = 0, c_hi = p.xf_C;
-            { const int f = kb % p.cpt; if (f + nk <= p.cpt) { c_lo = f * KCE; c_hi = (f + nk) * KCE; } }   // k-blocks of one tap: a chunk range
-            xf_build_coef(p, n, te, hA, hB, chs, c_lo, c_hi);
             const bool silu = p.xf_act == ACT_SILU || p.xf_act == ACT_SILU_FAST;
             const int ry = te / TILE_W, rx = te % TILE_W;
-            constexpr int NCH = ROWB / 16;                               // 16-byte chunks (8 channels) per operand row
-            const int swz = ROWB == 128 ? (te & 7) : ((te >> 1) & 3);    // the row's XOR term of the TMA / UMMA swizzle (stage bases are 1024-aligned)
+            const int swz = ROWB == 128 ? (te & 7) : ((te >> 1) & 3);    // the row's XOR term of the TMA swizzle (stage bases are 1024-aligned)
+            if (XF) {
+                // the affine is applied with packed half2 arithmetic (HFMA2, tanh.approx.f16x2): the operand is f16 anyway
+                double2* chs = reinterpret_cast<double2*>(xf_A + 2 * p.xf_C); // per-channel (sum, sum of squares) folded over the replicas
+                int c_lo = 0, c_hi = p.xf_C;
+                { const int f = kb % p.cpt; if (f + nk <= p.cpt) { c_lo = f * KCE; c_hi = (f + nk) * KCE; } }   // k-blocks of one tap: a chunk range
+                xf_build_coef(p, n, te, hA, hB, chs, c_lo, c_hi);
+            }
             for (int i = 0; i < nk; ++i) {
                 const int s = i % STAGES;
                 mbar_wait(smem_u32(bars + s), (i / STAGES) & 1);          // TMA bytes of this stage have landed
-                const int kt = kb + i;
-                const int tap = kt / p.cpt;
-                const int c0 = (kt - tap * p.cpt) * KCE;
-                const int iy = (y0 + ry) * p.in_mul + p.dy[phase][tap], ix = (x0 + rx) * p.in_mul + p.dx[phase][tap];
-                // rows outside the image are the convolution's zero padding (TMA filled them with zeros): they stay zero
-                if (iy >= 0 && iy < p.inH && ix >= 0 && ix < p.inW) {
-                    xf_row<ROWB>(smA + s * A_BYTES + te * ROWB, swz, c0, p, hA, hB, silu);
+                if (XF) {
+                    const int kt = kb + i;
+                    const int tap = kt / p.cpt;
+                    const int c0 = (kt - tap * p.cpt) * KCE;
+                    const int iy = (y0 + ry) * p.in_mul + p.dy[phase][tap], ix = (x0 + rx) * p.in_mul + p.dx[phase][tap];
+                    // rows outside the image are the convolution's zero padding (TMA filled them with zeros): they stay zero
+                    if (iy >= 0 && iy < p.inH && ix >= 0 && ix < p.inW) xf_row<ROWB>(smA + s * A_BYTES + te * ROWB, swz, c0, p, hA, hB, silu);
+                    asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");   // generic-proxy writes -> visible to wgmma's async-proxy reads
+                    asm volatile("bar.sync 1, 128;\n" ::: "memory");
                 }
-                asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");   // generic-proxy writes -> visible to the tensor core's async-proxy reads
-                mbar_arrive(smem_u32(bars + 2 * STAGES + 1 + s));
+                const uint32_t a_addr = smem_u32(smA + s * A_BYTES), b_addr = smem_u32(smB + s * B_BYTES);
+                wg_fence();
+#pragma unroll
+                for (int k = 0; k < ROWB / 32; ++k) {   // one wgmma consumes 32 bytes of K per row (8 tf32 / 16 f16): advance the start address by 32
+                    const uint64_t a0 = make_smem_desc_sw<ROWB>(a_addr + 32 * k), a1 = make_smem_desc_sw<ROWB>(a_addr + 64 * ROWB + 32 * k);
+                    const uint64_t bd = make_smem_desc_sw<ROWB>(b_addr + 32 * k);
+                    const uint32_t accum = (i > 0 || k > 0) ? 1u : 0u;
+                    if (OP == OP_TF32) { Wgmma<BN>::tf32(acc.d[0], a0, bd, accum); Wgmma<BN>::tf32(acc.d[1], a1, bd, accum); }
+                    else { Wgmma<BN>::f16(acc.d[0], a0, bd, accum); Wgmma<BN>::f16(acc.d[1], a1, bd, accum); }
+                }
+                wg_commit();
+                wg_wait<1>();                                              // the k-block before this one has been read
+                if (i > 0 && te == 0) mbar_arrive(smem_u32(bars + STAGES + (i - 1) % STAGES));
             }
-          }
-          if (CS > 1) { mbar_wait(smem_u32(bars + 2 * STAGES), 0); asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }   // own accumulator complete
-          else epi_direct<BN, TILE_W>(p, tmem_base, smem, smem_u32(bars + 2 * STAGES), n, y0, x0, n0, phase, split, warp, lane);
+            wg_wait<0>();
+            wg_fence_acc(acc.d[0]); wg_fence_acc(acc.d[1]);
+            if (CS == 1) epi_direct<BN, TILE_W>(p, acc, smem, n, y0, x0, n0, phase, split, warp, lane);
         }
     }
     if (CS > 1) {
@@ -179,16 +156,11 @@ __global__ void __launch_bounds__(TC_THREADS) conv_tc_kernel(const __grid_consta
         // barrier A: every CTA of the cluster has its accumulator and idle pipeline buffers -> peers may write into them
         asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
         asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
-        if (warp >= 2 && nk > 0) epi_push_partial<BN, CS>(tmem_base, smem, split, warp, lane);
+        if (warp < TC_PRODUCER_WARP && nk > 0) epi_push_partial<BN, CS>(acc, smem, split, warp, lane);
         // barrier B: the pushed slices are visible to their owners; nobody touches a peer's memory afterwards
         asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
         asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
-        if (warp >= 2) epi_cluster_reduce<BN, CS, TILE_W>(p, smem, n, y0, x0, n0, phase, split, warp);
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" :: "r"(tmem_base), "r"(TMEM_COLS) : "memory");
+        if (warp < TC_PRODUCER_WARP) epi_cluster_reduce<BN, CS, TILE_W>(p, smem, n, y0, x0, n0, phase, split, warp);
     }
 }
 
@@ -327,7 +299,7 @@ template <int OP, int BN, int STAGES_, int CS = 1, int XF = 0>
 void launch_tc(const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& p, dim3 grid, cudaStream_t s) {
     constexpr int STAGES = op_stages(OP, STAGES_);
     constexpr int STAGE_BYTES = (128 + BN) * op_row_bytes(OP);
-    constexpr size_t smem0 = 1024 + (size_t)STAGES * STAGE_BYTES + (3 * STAGES + 1) * 8 + 16;
+    constexpr size_t smem0 = 1024 + (size_t)STAGES * STAGE_BYTES + 2 * STAGES * 8 + 16;
     static_assert(smem0 <= 227 * 1024, "shared memory budget");
     // XF: per-channel affine (2 floats) + folded statistics (1 double2) of the normalised input channels
     const size_t smem = smem0 + (XF ? (size_t)24 * p.xf_C + 32 : 0);
@@ -351,23 +323,19 @@ template <int OP, int XF>
 void launch_variants(bool cluster, int stages_mode, int bn, int ksplit, const CUtensorMap& ma, const CUtensorMap& mb,
                      const TcParams& p, dim3 grid, cudaStream_t s) {
     if (cluster) {
-        if (bn == 256) launch_tc_cluster<OP, 256, 4, XF>(ksplit, ma, mb, p, grid, s);
-        else if (bn == 128) launch_tc_cluster<OP, 128, 6, XF>(ksplit, ma, mb, p, grid, s);
+        if (bn == 128) launch_tc_cluster<OP, 128, 6, XF>(ksplit, ma, mb, p, grid, s);
         else if (bn == 64) launch_tc_cluster<OP, 64, 8, XF>(ksplit, ma, mb, p, grid, s);
         else launch_tc_cluster<OP, 32, 8, XF>(ksplit, ma, mb, p, grid, s);
     } else if (stages_mode == 0) {
-        if (bn == 256) launch_tc<OP, 256, 4, 1, XF>(ma, mb, p, grid, s);
-        else if (bn == 128) launch_tc<OP, 128, 6, 1, XF>(ma, mb, p, grid, s);
+        if (bn == 128) launch_tc<OP, 128, 6, 1, XF>(ma, mb, p, grid, s);
         else if (bn == 64) launch_tc<OP, 64, 8, 1, XF>(ma, mb, p, grid, s);
         else launch_tc<OP, 32, 8, 1, XF>(ma, mb, p, grid, s);
     } else if (stages_mode == 1) {
-        if (bn == 256) launch_tc<OP, 256, 2, 1, XF>(ma, mb, p, grid, s);
-        else if (bn == 128) launch_tc<OP, 128, 3, 1, XF>(ma, mb, p, grid, s);
+        if (bn == 128) launch_tc<OP, 128, 3, 1, XF>(ma, mb, p, grid, s);
         else if (bn == 64) launch_tc<OP, 64, 4, 1, XF>(ma, mb, p, grid, s);
         else launch_tc<OP, 32, 5, 1, XF>(ma, mb, p, grid, s);
     } else {
-        if (bn == 256) launch_tc<OP, 256, 2, 1, XF>(ma, mb, p, grid, s);
-        else if (bn == 128) launch_tc<OP, 128, 2, 1, XF>(ma, mb, p, grid, s);
+        if (bn == 128) launch_tc<OP, 128, 2, 1, XF>(ma, mb, p, grid, s);
         else if (bn == 64) launch_tc<OP, 64, 2, 1, XF>(ma, mb, p, grid, s);
         else launch_tc<OP, 32, 3, 1, XF>(ma, mb, p, grid, s);
     }
@@ -396,13 +364,15 @@ int op_for(const ConvWeights& cw, const ConvArgs& a) {
 namespace {
 struct TcPlan { int bn, tiles_x, tiles_y, tiles_m, tiles_n, ksplit, MH, MW; bool cluster; };
 bool g_use_cluster = true;
-bool g_small_bn = true;    // narrower N tiles for unsplit launches with < 64 CTAs (option "small_bn"): 161.8 -> 167.5 frames/s at B=1
+bool g_small_bn = true;    // narrower N tiles for unsplit launches with < 64 CTAs (option "small_bn")
 bool g_use_s2 = true;      // 4x4 stride-2 convs through element-strided TMA boxes (option "tc_stride2")
 TcPlan tc_plan(const ConvWeights& cw, const ConvArgs& a) {
     TcPlan pl;
     pl.MH = a.out.H / cw.out_mul; pl.MW = a.out.W / cw.out_mul;
     pl.tiles_x = ceil_div(pl.MW, TILE_W); pl.tiles_y = ceil_div(pl.MH, TILE_H);
-    pl.bn = (cw.cout_pad % 256 == 0) ? 256 : (cw.cout_pad % 128 == 0 ? 128 : (cw.cout_pad % 64 == 0 ? 64 : 32));
+    // N tile: at most 128 columns, the accumulator of one consumer warpgroup (BN fp32 registers per thread)
+    pl.bn = (cw.cout_pad % 128 == 0) ? 128 : (cw.cout_pad % 64 == 0 ? 64 : 32);
+    const int sms = num_sms();
     pl.tiles_m = pl.tiles_x * pl.tiles_y * a.in.N;
     pl.tiles_n = cw.cout_pad / pl.bn;
     const int KT = cw.ntaps * (cw.cin_pad / op_kch(op_for(cw, a)));
@@ -410,12 +380,12 @@ TcPlan tc_plan(const ConvWeights& cw, const ConvArgs& a) {
     if (ksplit <= 0) {
         // few tiles: narrow the N tiles first (nothing to exchange), split K only for what is still missing -- the DSMEM
         // exchange of a cluster split grows with bn (conv_halo.cu, halo_plan)
-        while (pl.bn > 64 && (long)pl.tiles_m * (cw.cout_pad / pl.bn) * cw.nphase < 148 && cw.cout_pad % (pl.bn / 2) == 0) pl.bn /= 2;
+        while (pl.bn > 64 && (long)pl.tiles_m * (cw.cout_pad / pl.bn) * cw.nphase < sms && cw.cout_pad % (pl.bn / 2) == 0) pl.bn /= 2;
         pl.tiles_n = cw.cout_pad / pl.bn;
         const long ctas = (long)pl.tiles_m * pl.tiles_n * cw.nphase;
         ksplit = 1;
-        if (ctas < 120) {
-            ksplit = (int)((148 + ctas - 1) / ctas);
+        if (ctas < sms * 13 / 16) {
+            ksplit = (int)((sms + ctas - 1) / ctas);
             ksplit = std::min(ksplit, std::max(1, KT / 4));
             ksplit = std::min(ksplit, 32);
         }
@@ -424,7 +394,7 @@ TcPlan tc_plan(const ConvWeights& cw, const ConvArgs& a) {
     const int k_per = (KT + ksplit - 1) / ksplit;
     pl.ksplit = (KT + k_per - 1) / k_per;          // every split owns at least one k-block
     if (g_small_bn && a.ksplit <= 0 && pl.ksplit == 1) {
-        // tiny GEMMs whose K is too short to split (the 1x1 qkv / proj convs at 16^2: 6 CTAs with BN = 256): narrower N
+        // tiny GEMMs whose K is too short to split (the 1x1 qkv / proj convs at 16^2: 12 CTAs with BN = 128): narrower N
         // tiles put more SMs to work and shorten each CTA's weight fetch and epilogue
         while (pl.bn > 32 && (long)pl.tiles_m * (cw.cout_pad / pl.bn) * cw.nphase < 64 && cw.cout_pad % (pl.bn / 2) == 0) pl.bn /= 2;
         pl.tiles_n = cw.cout_pad / pl.bn;

@@ -1,6 +1,7 @@
-// Device-side pieces shared by the tcgen05 convolution kernels (conv_tc.cu: one TMA box per tap; conv_halo.cu: one halo box
-// per channel chunk, taps as row-shifted descriptors): launch parameters, operand formats, and the three epilogues
-// (direct TMEM -> global; cluster split-K: TMEM -> own shared-memory partial, then the DSMEM reduction).
+// Device-side pieces shared by the wgmma convolution kernels (conv_tc.cu: one TMA box per tap; conv_halo.cu: one halo box
+// per channel chunk, taps as row-shifted descriptors): launch parameters, operand formats, the register accumulator of the
+// consumer warpgroup, and the three epilogues (direct accumulator -> global; cluster split-K: accumulator -> the owners'
+// shared-memory partials, then the DSMEM reduction).
 // TW: pixels per tile row of the 128-pixel CTA tile (16 x 8 tiles: 16; 8 x 16 tiles: 8); row r of the accumulator is
 // pixel (y0 + r / TW, x0 + r % TW).
 #pragma once
@@ -15,7 +16,32 @@ using namespace tc;
 
 
 constexpr int TILE_W = 16, TILE_H = 8;          // 128 output pixels per CTA
-constexpr int TC_THREADS = 192;                  // warp 0: TMA producer, warp 1: MMA issuer + TMEM owner, warps 2-5: epilogue
+constexpr int TC_THREADS = 160;                  // warps 0-3: the consumer warpgroup (operand transform, wgmma, epilogue), warp 4: TMA producer
+constexpr int TC_PRODUCER_WARP = 4;
+
+// The 128 x BN fp32 accumulator of a CTA tile, in the registers of the consumer warpgroup: two m64 halves (rows 0-63, 64-127).
+template <int BN> struct Acc { float d[2][BN / 2]; };
+
+// Columns [c0, c0 + 32) of the accumulator, transposed through `stage` ([128][33] floats) so that thread t receives the 32
+// values of tile row t (the row-per-thread layout the epilogues are written for).  Called by all 128 consumer threads with
+// the same c0 (a constant after unrolling: the accumulator stays in registers).
+template <int BN>
+__device__ __forceinline__ void acc_rows32(const Acc<BN>& acc, int c0, float* stage, uint32_t (&r)[32]) {
+    const int t = threadIdx.x, w = t >> 5, l = t & 31;
+    asm volatile("bar.sync 1, 128;\n" ::: "memory");            // earlier readers of the stage are done
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int g = c0 / 8 + j;
+            const int col = 8 * j + 2 * (l & 3), row = h * 64 + w * 16 + (l >> 2);
+            stage[row * 33 + col] = acc.d[h][4 * g];             stage[row * 33 + col + 1] = acc.d[h][4 * g + 1];
+            stage[(row + 8) * 33 + col] = acc.d[h][4 * g + 2];   stage[(row + 8) * 33 + col + 1] = acc.d[h][4 * g + 3];
+        }
+    asm volatile("bar.sync 1, 128;\n" ::: "memory");
+#pragma unroll
+    for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(stage[t * 33 + j]);
+}
 
 struct TcParams {
     float* out; int outH, outW, outC, out_ld;
@@ -32,7 +58,7 @@ struct TcParams {
     int vec4;                                      // bias / residual rows may be read as float4 (16-byte aligned, ld % 4 == 0)
     __half* out16; int out16_ld;                   // optional f16 copy of the output (the operand format of a consumer conv); out may be null then
     // ---- fused input normalisation (XF kernels): the A operand is the RAW f16 output of the producing conv; its pending
-    // InstanceNorm / GroupNorm (+FiLM) affine and activation are applied in shared memory between TMA and tcgen05.mma
+    // InstanceNorm / GroupNorm (+FiLM) affine and activation are applied in shared memory between TMA and wgmma
     const double* in_stats; int in_stats_ld, in_stats_rep; long in_stats_rep_stride;
     int inH, inW, inC;                             // geometry of the input tensor (zero padding must stay zero; statistics count)
     int xf_C;                                      // channels [0, xf_C) are normalised, the rest (pose planes, padding) pass through
@@ -61,16 +87,16 @@ __host__ __device__ constexpr int op_stages(int op, int stages) { return op == O
 
 // ===== fused input normalisation (XF kernels) =====
 // Per-channel affine of sample n's pending normalisation, as packed halves (the operand is f16; HFMA2 / tanh.approx.f16x2
-// keep the in-place pass cheap).  Called by the 128 threads of warps 2-5 (te = 0..127); chs: scratch [xf_C] double2.
+// keep the in-place pass cheap).  Called by the 128 consumer threads (te = 0..127); chs: scratch [xf_C] double2.
 // [c_lo, c_hi): the channels this CTA will transform (its K chunks); widened to whole normalisation groups.  A cluster
-// split-K CTA builds 1 / CS of the table (the fold of the statistic replicas is the expensive part: 4.8 us for 512 channels).
+// split-K CTA builds 1 / CS of the table (the fold of the statistic replicas is the expensive part).
 __device__ __forceinline__ void xf_build_coef(const TcParams& p, int n, int te, __half* hA, __half* hB, double2* chs, int c_lo, int c_hi) {
     const int cpg = p.xf_groups == 0 ? 1 : p.xf_C / p.xf_groups;
     c_lo = (c_lo / cpg) * cpg;
     c_hi = min(p.xf_C, ((c_hi + cpg - 1) / cpg) * cpg);
     // The layer constants of this thread's first channel are requested BEFORE the statistics: with the loads behind the
-    // barrier below, the table cost three dependent L2 round trips (replicas 0-7, replicas 8-15, constants) = 3 900 cycles of
-    // every XF CTA's start-up (profiles/r02_halo_phase_stamps.txt, pdl -> coef); now one.
+    // barrier below, the table cost three dependent L2 round trips (replicas 0-7, replicas 8-15, constants) in every XF
+    // CTA's start-up; now one.
     const int c1 = c_lo + te;
     const bool h1 = c1 < c_hi;
     const float* f1p = p.xf_film1 ? p.xf_film1 + (long)n * p.xf_film1_ld : nullptr;
@@ -107,7 +133,7 @@ __device__ __forceinline__ void xf_build_coef(const TcParams& p, int n, int te, 
 // ALL chunks are loaded before the first is transformed and stored after the last: with one load -> transform -> store per
 // chunk the compiler must keep the shared-memory accesses in program order (it cannot prove that the store of chunk j and the
 // load of chunk j + 1 do not alias), which made the stage one dependent ~200-cycle chain per chunk on a single warp per
-// scheduler (profiles/r02_halo_phase_stamps.txt: a_full -> xf_done 3 300 cycles for 2 rows x 8 chunks).
+// scheduler .
 template <int NC>
 __device__ __forceinline__ void xf_chunks(uint8_t* rowp, int swz, int j0, int c0, const TcParams& p, const __half* hA, const __half* hB, bool silu) {
     uint4 d[NC];
@@ -145,45 +171,44 @@ __device__ __forceinline__ void xf_row(uint8_t* rowp, int swz, int c0, const TcP
     xf_chunks<ROWB / 16>(rowp, swz, 0, c0, p, hA, hB, silu);
 }
 
-// ===== cluster split-K, step 1 (epilogue warps, after a cluster barrier that says every peer's accumulator is complete and
-// its pipeline buffers are idle): TMEM -> the OWNER's shared memory.  Rank r of the cluster finishes columns
+// ===== cluster split-K, step 1 (consumer warpgroup, after a cluster barrier that says every peer's accumulator is complete
+// and its pipeline buffers are idle): registers -> the OWNER's shared memory.  Rank r of the cluster finishes columns
 // [r * SL, (r + 1) * SL); every CTA PUSHES the slice of its partial that belongs to rank r into slot [sender] of rank r's
-// buffer with st.shared::cluster (posted stores).  The pull version (ld.shared::cluster after staging locally) ran one remote
-// load per warp at a time: 16 KB took 6 500 cycles (profiles/r02_halo_phase_stamps.txt).
+// buffer with st.shared::cluster (posted stores).
 // Buffer of a CTA: [CS slots][128 rows x SC 16-byte chunks], chunk index L = row * SC + cc stored at L ^ ((L >> 3) & 7)
-// (writers -- lanes = rows -- and readers -- lanes = consecutive L -- both spread over the banks).
+// (readers -- lanes = consecutive L -- spread over the banks).
 template <int BN, int CS>
-__device__ __forceinline__ void epi_push_partial(uint32_t tmem_base, uint8_t* smem, int split, int warp, int lane) {
+__device__ __forceinline__ void epi_push_partial(const Acc<BN>& acc, uint8_t* smem, int split, int warp, int lane) {
     constexpr int SL = BN / CS, SC = SL / 4;
     constexpr uint32_t SLOT_BYTES = 128u * SL * 4u;
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
     const uint32_t base = smem_u32(smem) + (uint32_t)split * SLOT_BYTES;       // slot [sender = this rank] in every owner's buffer
-#pragma unroll 1
-    for (int c0 = 0; c0 < BN; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, r);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int chunk = (c0 >> 2) + j;
-            const int owner = chunk / SC, cc = chunk - owner * SC;
-            const uint32_t L = (uint32_t)(row * SC + cc);
-            const uint32_t addr = base + ((L ^ ((L >> 3) & 7u)) << 4);
-            if (owner == split) {
-                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};\n" :: "r"(addr), "r"(r[4 * j]), "r"(r[4 * j + 1]), "r"(r[4 * j + 2]), "r"(r[4 * j + 3]) : "memory");
-            } else {
-                uint32_t remote;
-                asm volatile("mapa.shared::cluster.u32 %0, %1, %2;\n" : "=r"(remote) : "r"(addr), "r"(owner));
-                asm volatile("st.shared::cluster.v4.b32 [%0], {%1, %2, %3, %4};\n" :: "r"(remote), "r"(r[4 * j]), "r"(r[4 * j + 1]), "r"(r[4 * j + 2]), "r"(r[4 * j + 3]) : "memory");
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int g = 0; g < BN / 8; ++g)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int row = h * 64 + warp * 16 + (lane >> 2) + 8 * e;
+                const int col = 8 * g + 2 * (lane & 3);
+                const int chunk = col >> 2;
+                const int owner = chunk / SC, cc = chunk - owner * SC;
+                const uint32_t L = (uint32_t)(row * SC + cc);
+                const uint32_t addr = base + ((L ^ ((L >> 3) & 7u)) << 4) + (uint32_t)(col & 3) * 4u;
+                const float v0 = acc.d[h][4 * g + 2 * e], v1 = acc.d[h][4 * g + 2 * e + 1];
+                if (owner == split) {
+                    asm volatile("st.shared.v2.f32 [%0], {%1, %2};\n" :: "r"(addr), "f"(v0), "f"(v1) : "memory");
+                } else {
+                    uint32_t remote;
+                    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;\n" : "=r"(remote) : "r"(addr), "r"(owner));
+                    asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};\n" :: "r"(remote), "f"(v0), "f"(v1) : "memory");
+                }
             }
-        }
-    }
 }
 
-// ===== unsplit / workspace split-K epilogue (epilogue warps): TMEM -> registers -> global (+ statistics) =====
+// ===== unsplit / workspace split-K epilogue (consumer warpgroup): registers -> global (+ statistics) =====
 // NSLOT > 0 (and p.st_tma): the finished 128 x 32 tile of each column step is staged in shared memory in the swizzled box
 // layout and written by ONE TMA store per output (fp32 / f16) instead of 12 warp-wide stores whose 32 lanes hit 32 different
-// lines (32 L1 wavefronts per instruction: the store phase was ~1500 LSU cycles per tile, a third of the epilogue).  TMA
+// lines (32 L1 wavefronts per instruction).  TMA
 // clips what lies outside the tensor (partial tiles, channel tails).  Slots live behind the statistics scratch in the idle
 // pipeline buffers; a slot is rewritten only after its store has read it (bulk-group wait).
 constexpr int EPI_SLOT_BYTES = 128 * 128 + 128 * 64;           // fp32 stage (128-byte rows) + f16 stage (64-byte rows)
@@ -198,23 +223,16 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, uint32_t sr
 }
 
 template <int BN, int TW, int NSLOT = 0>
-__device__ __forceinline__ void epi_direct(const TcParams& p, uint32_t tmem_base, uint8_t* smem, uint32_t tmem_full_bar, int n, int y0, int x0,
+__device__ __forceinline__ void epi_direct(const TcParams& p, const Acc<BN>& acc, uint8_t* smem, int n, int y0, int x0,
                                            int n0, int phase, int split, int warp, int lane,
                                            const CUtensorMap* tm32 = nullptr, const CUtensorMap* tm16 = nullptr,
                                            const CUtensorMap* tmR = nullptr, uint64_t* res_bars = nullptr) {
-    const int q = warp & 3;                                    // TMEM lane quadrant this warp may access
-    // the bias lines of this tile's columns are pulled into L1 while the MMAs still run: the float4 reads below found them
-    // in L2 at best, one exposed round trip per 32-column step
-    if (p.bias && q == 0 && lane * 32 < BN && n0 + lane * 32 < p.outC)
-        asm volatile("prefetch.global.L1 [%0];\n" :: "l"(p.bias + n0 + lane * 32) : "memory");
-    mbar_wait(tmem_full_bar, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
+    const int q = warp & 3;
     // p.st_tma bit 2: the residual tile (same geometry as the fp32 output) ARRIVES by TMA as well, into the fp32 stage of
     // the slot it will leave from: 8 conflict-free LDS.128 per thread instead of 8 LDG.128 whose lanes hit 32 different lines
-    // (phase stamps: the epilogue of a 64-channel conv with residual took 16 700 cycles, 6 800 without).
     const bool res_tma = NSLOT > 0 && (p.st_tma & 4) != 0;
     const int nsteps = min(BN / 32, (p.outC - n0 + 31) / 32);
-    if (res_tma && threadIdx.x == 64) {
+    if (res_tma && threadIdx.x == 0) {
         for (int s = 0; s < NSLOT && s < nsteps; ++s) {
             const uint32_t bar = smem_u32(res_bars + s);
             mbar_expect_tx(bar, 128 * 128);
@@ -223,7 +241,7 @@ __device__ __forceinline__ void epi_direct(const TcParams& p, uint32_t tmem_base
     }
     const int row = q * 32 + lane;
     const bool lead = (split == 0);
-    float* scratch = reinterpret_cast<float*>(smem) + q * (32 * 33);   // pipeline smem is idle once tmem_full fired
+    float* scratch = reinterpret_cast<float*>(smem) + q * (32 * 33);   // pipeline smem is idle once the last wgmma retired
     const int my = y0 + row / TW, mx = x0 + row % TW;
     const bool valid = my < p.MH && mx < p.MW;
     const int oy = my * p.out_mul + p.ph_oy[phase], ox = mx * p.out_mul + p.ph_ox[phase];
@@ -231,10 +249,10 @@ __device__ __forceinline__ void epi_direct(const TcParams& p, uint32_t tmem_base
     float* orow = p.out + opix * p.out_ld;
     const int st_tma = NSLOT > 0 ? p.st_tma : 0;
     int step = 0;
-#pragma unroll 1
+#pragma unroll
     for (int c0 = 0; c0 < BN; c0 += 32) {
         uint32_t r[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, r);
+        acc_rows32<BN>(acc, c0, reinterpret_cast<float*>(smem), r);    // the stage is the statistics scratch: row t at t * 33
         const int cbase = n0 + c0;
         if (cbase >= p.outC) continue;                         // warp-uniform
         float v[32];
@@ -320,7 +338,7 @@ __device__ __forceinline__ void epi_direct(const TcParams& p, uint32_t tmem_base
         if (NSLOT > 0 && st_tma) {
             // every row is staged (rows outside the image hold values of zero-padded inputs; the store clips them)
             if (step >= NSLOT && !res_tma) {
-                if (threadIdx.x == 64) asm volatile("cp.async.bulk.wait_group.read %0;\n" :: "n"(NSLOT > 0 ? NSLOT - 1 : 0) : "memory");
+                if (threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group.read %0;\n" :: "n"(NSLOT > 0 ? NSLOT - 1 : 0) : "memory");
                 asm volatile("bar.sync 1, 128;\n" ::: "memory");
             }
             uint8_t* slot = smem + epi_slot0(BN) + (NSLOT > 0 ? step % NSLOT : 0) * EPI_SLOT_BYTES;
@@ -353,7 +371,7 @@ __device__ __forceinline__ void epi_direct(const TcParams& p, uint32_t tmem_base
             }
             asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
             asm volatile("bar.sync 1, 128;\n" ::: "memory");
-            if (threadIdx.x == 64) {
+            if (threadIdx.x == 0) {
                 if (st_tma & 1) tma_store_4d(tm32, smem_u32(slot), cbase, x0, y0, n);
                 if (st_tma & 2) tma_store_4d(tm16, smem_u32(slot + 128 * 128), cbase, x0, y0, n);
                 asm volatile("cp.async.bulk.commit_group;\n" ::: "memory");
@@ -385,24 +403,24 @@ __device__ __forceinline__ void epi_direct(const TcParams& p, uint32_t tmem_base
         asm volatile("bar.sync 1, 128;\n" ::: "memory");
         const float2* part = reinterpret_cast<const float2*>(reinterpret_cast<float*>(smem) + 4 * 32 * 33);
         double* base = p.stats + (long)(blockIdx.x % p.stats_rep) * p.stats_rep_stride + ((long)n * p.stats_ld + n0) * 2;
-        for (int c = (warp - 2) * 32 + lane; c < BN; c += 128) {
+        for (int c = (int)threadIdx.x; c < BN; c += 128) {
             if (n0 + c >= p.outC) break;
             const float2 a = part[c], b = part[BN + c], cc = part[2 * BN + c], d = part[3 * BN + c];
             atomicAdd(base + 2 * c, (double)a.x + (double)b.x + (double)cc.x + (double)d.x);
             atomicAdd(base + 2 * c + 1, (double)a.y + (double)b.y + (double)cc.y + (double)d.y);
         }
     }
-    if (NSLOT > 0 && st_tma && threadIdx.x == 64) asm volatile("cp.async.bulk.wait_group.read 0;\n" ::: "memory");   // the staging slots have been read before the CTA retires (the writes themselves complete with the grid)
+    if (NSLOT > 0 && st_tma && threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group.read 0;\n" ::: "memory");   // the staging slots have been read before the CTA retires (the writes themselves complete with the grid)
 }
 
-// ===== cluster split-K, step 2 (epilogue warps, after the cluster barrier that publishes the pushes): sum the CS slots of this
+// ===== cluster split-K, step 2 (consumer warpgroup, after the cluster barrier that publishes the pushes): sum the CS slots of this
 // CTA's column slice from its own shared memory, finish the columns =====
 template <int BN, int CS, int TW>
 __device__ __forceinline__ void epi_cluster_reduce(const TcParams& p, uint8_t* smem, int n, int y0, int x0, int n0, int phase, int split, int warp,
                                                    long long* dbg = nullptr) {
     constexpr int SL = BN / CS, SC = SL / 4;                   // columns / 16-byte chunks finished by this CTA
     static_assert(SL >= 4 && 128 % SC == 0, "cluster slice");
-    const int te = threadIdx.x - 64;                           // 0..127
+    const int te = threadIdx.x;                                // 0..127
     const int cc = te % SC;
     const int chunk = split * SC + cc;                         // split == rank in the cluster
     const int col = n0 + chunk * 4;
@@ -434,10 +452,10 @@ __device__ __forceinline__ void epi_cluster_reduce(const TcParams& p, uint8_t* s
                              : "=f"(part[u][pr].x), "=f"(part[u][pr].y), "=f"(part[u][pr].z), "=f"(part[u][pr].w)
                              : "r"(p_local + (uint32_t)pr * (128u * SL * 4u) + off));
         }
-        if (dbg && threadIdx.x == 64 && rb == 0) dbg[3 * 8 + 1] = clock64();
+        if (dbg && threadIdx.x == 0 && rb == 0) dbg[3 * 8 + 1] = clock64();
         // the residual rows of the batch are requested up front as well (L2 round trips).  Index arithmetic stays in 32 bits up
         // to the one widening multiply by the row stride: with 64-bit products throughout, this loop was ~250 dependent
-        // instructions per row on one warp per scheduler -- 6 500 cycles, the longest phase of the kernel (phase stamps).
+        // instructions per row on one warp per scheduler.
         float rres[U][4];
         int opix[U];
         bool ok[U];
@@ -501,7 +519,7 @@ __device__ __forceinline__ void epi_cluster_reduce(const TcParams& p, uint8_t* s
         for (int j = 0; j < cn; ++j) { su[j] += v[j]; sq[j] += v[j] * v[j]; }
       }
     }
-    if (dbg && threadIdx.x == 64) dbg[3 * 8 + 0] = clock64();
+    if (dbg && threadIdx.x == 0) dbg[3 * 8 + 0] = clock64();
     if (p.stats) {
         // per-column sums of this CTA's slice: thread te holds partials of chunk te % SC; fold the 128 / SC row
         // threads of each chunk in two short steps (8 floats per thread, then <= 16 doubles per output)

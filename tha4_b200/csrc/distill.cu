@@ -7,7 +7,7 @@
 // Layout: parameters / gradients / Adam moments are flat fp32 buffers in the reference's state_dict order
 // (siren_layers.l.j.linear.{weight,bias} ..., last_linear.{weight,bias}); activations are fp32 NHWC with channel
 // counts padded to multiples of 4 (360, 180, 92; level inputs 48 / 228 / 140), pad channels are exactly zero.
-// The dense layers are GEMMs over all pixels of the micro-batch and run on the same tcgen05 conv kernel as the
+// The dense layers are GEMMs over all pixels of the micro-batch and run on the same wgmma conv kernel as the
 // teacher (1x1 taps); weight gradients use a dedicated pixel-reduction GEMM (mma.sync TF32).
 #include "distill.cuh"
 #include "gridsample.cuh"
@@ -328,7 +328,7 @@ View mk(Pool* pool, int N, int R, int C) {
     return v;
 }
 
-// y = x * W^T (+ bias): 1x1 conv through the shared conv dispatcher (tcgen05 when available)
+// y = x * W^T (+ bias): 1x1 conv through the shared conv dispatcher (wgmma when available)
 void dense_gemm(Runtime& rt, const float* W, int nreal, int kreal, bool transpose, const float* bias_padded,
                 const View& x, const View& y) {
     ConvWeights cw;

@@ -161,7 +161,7 @@ void run_conv(Runtime& rt, const ConvWeights& cw, const View& in, const View& ou
 // ---- default (tensor-core) mode: activations in up to two precisions, normalisations fused into the consumer conv ----
 // An activation tensor as the default mode stores it: `f` always carries the geometry and the statistics slot; f.p is the
 // fp32 copy (residual streams, inputs of the few remaining normalisation passes) or null; h is the f16 copy (the operand
-// a tcgen05 conv loads by TMA) or empty.  RAW conv outputs whose only consumer is a conv with a pending normalisation
+// a wgmma conv loads by TMA) or empty.  RAW conv outputs whose only consumer is a conv with a pending normalisation
 // exist in f16 only.
 struct Tens { View f; View h; };
 
@@ -202,7 +202,7 @@ ConvNormIn norm_in(const View& src_stats, const NormW& nw, int groups, int act, 
     return n;
 }
 
-// conv on the tcgen05 kernel: `in` is an f16 operand view (or fp32 for the first layer of a network), `nin` its pending
+// conv on the wgmma kernel: `in` is an f16 operand view (or fp32 for the first layer of a network), `nin` its pending
 // normalisation (nullptr: none), `out` receives the fp32 and / or f16 copies it has storage for, plus statistics
 void run_conv_tc(Runtime& rt, const ConvWeights& cw, const View& in, const ConvNormIn* nin, const Tens& out,
                  const View* res = nullptr, int res_mode = RES_NONE) {
@@ -262,7 +262,7 @@ void EncDecNet::load(const StateDict& sd, cudaStream_t s) {
         tail_add_head(tail_, sd, "eye_color_change.0", true, s);
         tail_add_head(tail_, sd, "eye_alpha.0", true, s);
     }
-    if (conv_pack_rounding()) tail_make_half(tail_, s);       // default mode: the tcgen05 tail's f16 head weights
+    if (conv_pack_rounding()) tail_make_half(tail_, s);       // default mode: the wgmma tail's f16 head weights
     THA4_CUDA_CHECK(cudaStreamSynchronize(s));
     loaded_ = true;
 }
@@ -285,7 +285,7 @@ void EncDecNet::forward(Runtime& rt, const ImgView& image0, const ImgView& image
     }
     if (rt.f16) { forward_fused(rt, x0, image0, image1, pose, pose_ld, outputs); return; }
     // conv -> InstanceNorm -> ReLU; the activated tensor goes to `dst`, or to a fresh f16 tensor when its only consumer is
-    // a tcgen05 conv (to16), or back in place
+    // a wgmma conv (to16), or back in place
     const bool h16 = false;
     auto conv_in_relu = [&](const ConvWeights& cw, const NormW& nw, const View& in, int oh, const View* dst, bool to16) -> View {
         View raw = make_view(P, B, oh, oh, cw.cout, &rt);
@@ -518,7 +518,7 @@ void UNetNet::load(const StateDict& sd, cudaStream_t s) {
         THA4_CUDA_CHECK(cudaMemcpyAsync(film1_b_ + w->film1_off, sd_get(sd, e.second + ".cond1_layers.1.bias").p,
                                         2 * w->cout * sizeof(float), cudaMemcpyDeviceToDevice, s));
     }
-    if (conv_pack_rounding()) tail_make_half(tail_, s);       // default mode: the tcgen05 tail's f16 head weights
+    if (conv_pack_rounding()) tail_make_half(tail_, s);       // default mode: the wgmma tail's f16 head weights
     THA4_CUDA_CHECK(cudaStreamSynchronize(s));
     cudaFree(d_t0); cudaFree(d_t1); cudaFree(d_t2);
     loaded_ = true;
@@ -687,7 +687,7 @@ struct UNetFused {
         Tens h0 = make_act(rt.scratch, rt, B, out.f.H, out.f.W, w.cout, false, true);
         Tens sk;
         if (w.has_skip) {
-            // skip(x) depends on x only: it runs on the side stream next to norm0 -> conv0 (15 us of a latency-bound chain,
+            // skip(x) depends on x only: it runs on the side stream next to norm0 -> conv0 (a latency-bound chain,
             // ~30 times per frame) and is joined in front of conv1, which adds it as the residual
             sk = make_act(rt.scratch, rt, B, x.f.H, x.f.W, w.cout, true, false, false);
             if (rt.side) {

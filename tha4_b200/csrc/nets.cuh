@@ -38,7 +38,7 @@ struct Runtime {                      // per-call execution context
     Pool* scratch;
     cudaStream_t stream;
     int strict;
-    int f16 = 0;                      // normalisation layers hand f16 tensors to the tcgen05 convs (non-strict, tcgen05 on)
+    int f16 = 0;                      // normalisation layers hand f16 tensors to the wgmma convs (non-strict, wgmma on)
     // optional second stream + fork / join events: independent branches of the DAG (the 1x1 skip conv of a ResBlock next to
     // its norm0 -> conv0 chain) run beside the main chain -- also inside a captured graph, where they become parallel branches
     cudaStream_t side = nullptr;

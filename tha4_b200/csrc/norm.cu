@@ -223,7 +223,7 @@ __global__ void __launch_bounds__(256) norm_apply_kernel(const float* __restrict
         if (xpool) {
             // 2x2 mean of the RAW input as well (AvgPool2d(2) of the block's skip path, unet.py:58,164), in the order the conv
             // epilogue's RES_DOWN2 used: the consumer then adds it as a same-resolution residual (one TMA tile instead of
-            // 128 scalar loads per thread: the unsplit RES_DOWN2 epilogues cost 28 - 37 us each, profiles/r02_halo_phase_stamps.txt)
+            // 128 scalar loads per thread: slow unsplit RES_DOWN2 epilogues)
             float4 m;
             m.x = 0.25f * ((raw[0].x + raw[1].x) + (raw[2].x + raw[3].x)); m.y = 0.25f * ((raw[0].y + raw[1].y) + (raw[2].y + raw[3].y));
             m.z = 0.25f * ((raw[0].z + raw[1].z) + (raw[2].z + raw[3].z)); m.w = 0.25f * ((raw[0].w + raw[1].w) + (raw[2].w + raw[3].w));

@@ -7,7 +7,7 @@ namespace tha4 {
 
 // ---------------------------------------------------------------- normalisation (norm.cu)
 // Accumulates per-(n,c) sum / sum of squares of x into x.stats (must be zero on entry).  Only needed for tensors whose
-// producer did not already do it (the tcgen05 conv epilogue and the split-K reduction accumulate them for free).
+// producer did not already do it (the wgmma conv epilogue and the split-K reduction accumulate them for free).
 void norm_stats(const View& x, cudaStream_t s);
 
 // Turns the statistics into a per-(n,c) affine  y = x * A + B  that folds InstanceNorm2d / GroupNorm (eps 1e-5,
@@ -76,10 +76,10 @@ struct TailWeights {
     float* w = nullptr;      // [9][C][CO_PAD] fp32
     float* bias = nullptr;   // [CO_PAD]
     int C = 0, CO = 0;
-    __half* w16 = nullptr;   // [9][16][C] f16, K-major B operand of the tcgen05 tail (tail_make_half), scaled by w16_scale
+    __half* w16 = nullptr;   // [9][16][C] f16, K-major B operand of the wgmma tail (tail_make_half), scaled by w16_scale
     float w16_scale = 1.0f;
 };
-// pending normalisation of the tail's feature map (applied inside the tcgen05 tail from the feature view's statistics)
+// pending normalisation of the tail's feature map (applied inside the wgmma tail from the feature view's statistics)
 struct NormSpecTail { int groups = 0; int act = ACT_NONE; const float* gamma = nullptr; const float* beta = nullptr; };
 constexpr int TAIL_CO_PAD = 12;
 // Head weights: tail_init allocates zeroed storage (recorded in the active AllocSink), tail_add appends one reference
@@ -91,10 +91,10 @@ void tail_add(TailWeights& tw, const float* w_ref, const float* b_ref, int cout,
 // outputs: NCHW contiguous, order/meaning per kind (see tail.cu).
 void tail_forward(TailKind kind, const TailWeights& tw, const View& feature, const float* coef, int act,
                   const ImgView& image0, const ImgView& image1, float* const* outputs, cudaStream_t s, int strict);
-// tcgen05 variant (tail_tc.cu): `feature` is the RAW f16 feature map with the statistics its producer accumulated
+// wgmma variant (tail_tc.cu): `feature` is the RAW f16 feature map with the statistics its producer accumulated
 void tail_make_half(TailWeights& tw, cudaStream_t s);     // f16 B-operand copy of the head weights (recorded in the active AllocSink)
 bool tail_tc_supported(const TailWeights& tw, const View& feature);
-void tail_tc_enable_persist(bool on);      // option "tail_persist": persistent pipelined tcgen05 tail (default on)
+void tail_tc_enable_persist(bool on);      // option "tail_persist": persistent pipelined tensor-core tail (default on)
 // gather0 / gather1: optional fp32 NHWC copies of image0 / image1 (4-channel slices, 16-byte aligned pixels), e.g. the
 // network's own input tensor: the persistent kernel then reads a pixel's RGBA with one 16-byte load (same values, same results)
 void tail_tc_forward(TailKind kind, const TailWeights& tw, const View& feature, const NormSpecTail& ns, const ImgView& image0,

@@ -489,9 +489,9 @@ void SirenFaceNet::forward(Runtime& rt, const float* pose, int pose_ld, int B, f
     THA4_REQUIRE(loaded_, "network weights not loaded");
     const int R = 128;
     float* pb = pose_bias(rt, layers_[0], pose, pose_ld, B);
-    if (siren_tc_enabled()) {       // TMA + tcgen05 + TMEM path (siren_tc.cu)
+    if (siren_tc_enabled()) {       // TMA + wgmma path (siren_tc.cu)
         SirenTcPlan plan;
-        for (int i = 1; i < 8; ++i) plan.add(layers_[i], 128, 1, 0);
+        for (int i = 1; i < 8; ++i) plan.add(layers_[i], 64, 1, 0);
         plan.add(head_, 16, 0, 0);
         SirenTcLevel lv;
         lv.R = R; lv.B = B; lv.e_npad = layers_[0].NPAD; lv.e_pb = pb; lv.e_pb_ld = layers_[0].NPAD; lv.e_wxy = layers_[0].wxy;
@@ -538,10 +538,10 @@ void SirenBodyNet::forward(Runtime& rt, const ImgView& image, const float* pose,
     float* pb2 = pose_bias(rt, l_[2][0], pose, pose_ld, B);
     __half* f0 = reinterpret_cast<__half*>(rt.persist->alloc((size_t)B * 128 * 128 * 192 / 2));
     __half* f1 = reinterpret_cast<__half*>(rt.persist->alloc((size_t)B * 256 * 256 * 96 / 2));
-    if (siren_tc_enabled()) {       // TMA + tcgen05 + TMEM path (siren_tc.cu): one persistent kernel per level
+    if (siren_tc_enabled()) {       // TMA + wgmma path (siren_tc.cu): one persistent kernel per level
         {
             SirenTcPlan plan;
-            plan.add(l_[0][1], 192, 1, 0); plan.add(l_[0][2], 192, 1, 0);
+            plan.add(l_[0][1], 96, 1, 0); plan.add(l_[0][2], 96, 1, 0);
             SirenTcLevel lv;
             lv.R = 128; lv.B = B; lv.e_npad = 384; lv.e_pb = pb0; lv.e_pb_ld = 384; lv.e_wxy = l_[0][0].wxy;
             lv.out = f0; lv.out_c = 192;
@@ -567,7 +567,7 @@ void SirenBodyNet::forward(Runtime& rt, const ImgView& image, const float* pose,
         }
         return;
     }
-    THA4_REQUIRE(!outputs_f16, "siren body: f16 outputs need the tcgen05 path (option siren_tc)");
+    THA4_REQUIRE(!outputs_f16, "siren body: f16 outputs need the tensor-core path (option siren_tc)");
     using SM0 = Smem<384, 384, 2>;
     using SM1 = Smem<192, 192, 3>;
     using SM2 = Smem<96, 96, 3>;

@@ -13,7 +13,7 @@ struct SirenLayer {
     void load(const StateDict& sd, const std::string& prefix, int feat, int pose, int kpad, int npad, float scale, cudaStream_t s);
 };
 
-// ---- tcgen05 path (siren_tc.cu): a level = a chain of GEMM layers on 128-pixel tiles, weights streamed by TMA ----
+// ---- wgmma path (siren_tc.cu): a level = a chain of GEMM layers on 128-pixel tiles, weights streamed by TMA ----
 struct SirenTcPlan {          // the GEMM layers of one kernel, in order
     int nl = 0;
     int kpad[8], npad[8], nb[8], sine[8], first[8], rows[8];
@@ -48,7 +48,7 @@ class SirenBodyNet {
 public:
     void load(const StateDict& sd, cudaStream_t s);
     // image: [B,4,512,512]; pose: [B,45]; outputs: blended(4) alpha(1) colour(4) warped(4) grid_change(2), fp32 NCHW
-    // outputs_f16: the five output planes are __half (io_dtype = f16 of tha4_student_forward_io; tcgen05 path only)
+    // outputs_f16: the five output planes are __half (io_dtype = f16 of tha4_student_forward_io; wgmma path only)
     void forward(Runtime& rt, const ImgView& image, const float* pose, int pose_ld, float* const* outputs, bool outputs_f16 = false);
     bool loaded() const { return loaded_; }
 private:

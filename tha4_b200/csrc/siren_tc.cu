@@ -1,15 +1,17 @@
-// Distilled student networks on the Blackwell paths: SirenFaceMorpher00 (siren_face_morpher_00.py:28-51) and the three
-// levels of SirenMorpher03 (siren_morpher_03.py:107-139) as persistent fused-MLP kernels on TMA + tcgen05 + TMEM.
+// Distilled student networks on the tensor cores: SirenFaceMorpher00 (siren_face_morpher_00.py:28-51) and the three
+// levels of SirenMorpher03 (siren_morpher_03.py:107-139) as persistent fused-MLP kernels on TMA + wgmma.
 //
 // A CTA walks 128-pixel tiles (128 consecutive pixels of one image row).  The activations of a tile live in shared
-// memory as the K-major SWIZZLE_128B A operand ([K / 64 chunks][128 rows][128 B]); every sine layer is
+// memory as the K-major SWIZZLE_128B A operand ([K / 64 chunks][128 rows][128 B]), in two buffers that swap roles per
+// layer (a layer reads one and writes the other); every sine layer is
 //   TMA     weight tiles W[NB rows x 64 k] (fp16, pre-scaled by omega_0 = 30) stream through a ring that runs ahead of
-//           the math across layers and tiles (the weight sequence of a tile is fixed);
-//   UMMA    D[128 x N] (fp32, TMEM) = A[128 x K] . W^T: one elected thread, N in slices of NB <= 256 columns;
-//   drain   the four compute warps (thread = pixel = TMEM lane) read the accumulator with tcgen05.ld, add the bias
-//           (+ the per-sample pose bias and the two xy terms on a level's first layer: the tiled pose / position
-//           planes of siren_morpher_03.py:92-105 are never materialised), take sin(.) and write the result back INTO the
-//           A operand as fp16 -- the layer's output is the next layer's operand, it never leaves the SM.
+//           the math across layers and tiles (the weight sequence of a tile is fixed; warp 4 issues them);
+//   wgmma   D[128 x NB] (fp32, registers of the consumer warpgroup, two m64 halves) = A[128 x K] . W^T, N in slices of
+//           NB <= 96 columns;
+//   drain   each thread adds the bias to its accumulator fragment (+ the per-sample pose bias and the two xy terms on a
+//           level's first layer: the tiled pose / position planes of siren_morpher_03.py:92-105 are never materialised),
+//           takes sin(.) and writes the result into the other A buffer as fp16 -- the layer's output is the next layer's
+//           operand, it never leaves the SM.
 // Level hand-off (bilinear x2, :121) goes through fp16 NHWC tensors in HBM (it needs a cross-tile halo); level 2 ends in
 // the fused tail: 1x1 head (a 16-column MMA) -> grid_sample -> blend -> five NCHW outputs (thread = pixel: the 32 lanes
 // of a warp write 32 consecutive pixels = full 128-byte lines).  The mma.sync kernels of siren.cu remain as the
@@ -28,7 +30,7 @@ namespace {
 
 using namespace tc;
 
-constexpr int ST_THREADS = 192;            // warp 0: TMA producer, warp 1: MMA issuer + TMEM owner, warps 2-5: compute
+constexpr int ST_THREADS = 160;            // warps 0-3: the consumer warpgroup (prologue, wgmma, drain), warp 4: TMA producer
 constexpr int ST_TILE = 128;
 constexpr int ST_MAXL = 8;                 // GEMM layers per kernel (face: 7 sine + head)
 enum { SM_BODY0 = 0, SM_BODY1 = 1, SM_BODY2 = 2, SM_FACE = 3 };
@@ -59,7 +61,7 @@ struct StParams {
 
 // sin(x) WITHOUT the transcendental unit.  The mma.sync student kernels (siren.cu) and the first version of this file used
 // rintf + MUFU.SIN: two XU-pipe operations per output -- and ncu showed the XU pipe, not the tensor pipe, bounding every
-// level (profiles/r02_ncu_siren_tc_v1.txt: both implementations ran at ~1.8 sin / clk / SM).  Here: k = round(x / pi) by
+// level.  Here: k = round(x / pi) by
 // the magic-number trick (FMA pipe), r = x - k pi (two-constant Cody-Waite), sin(r) on [-pi/2, pi/2] as the degree-9
 // Taylor polynomial (|error| <= 3.6e-6, far below the fp16 the result is stored in), sign (-1)^k from the parity bit.
 // 13 FMA / ALU-pipe instructions, 128 lanes / clk / SM.
@@ -82,18 +84,44 @@ __device__ __forceinline__ uint32_t a_off(int row, int c8) {
     return (uint32_t)(chunk * (ST_TILE * 128) + row * 128 + ((j ^ (row & 7)) << 4));
 }
 
-template <int ACH, int NBMAX, int SB, int TMEM_COLS, int MODE>
+// D (+)= A . W^T for one N slice of width nb (a runtime choice among the widths the plans use), K steps of 16 up to ksteps
+template <int NBMAX>
+__device__ __forceinline__ void st_slice_mma(float (&d)[2][NBMAX / 2], int nb, uint32_t a_addr, uint32_t b_addr, int ksteps, bool acc_in) {
+    wg_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        if (k >= ksteps) break;
+        const uint64_t a0 = make_smem_desc_sw<128>(a_addr + 32 * k), a1 = make_smem_desc_sw<128>(a_addr + 64 * 128 + 32 * k);
+        const uint64_t bd = make_smem_desc_sw<128>(b_addr + 32 * k);
+        const uint32_t accum = (acc_in || k > 0) ? 1u : 0u;
+        if (nb == 16) {
+            Wgmma<16>::f16(*reinterpret_cast<float(*)[8]>(&d[0][0]), a0, bd, accum);
+            Wgmma<16>::f16(*reinterpret_cast<float(*)[8]>(&d[1][0]), a1, bd, accum);
+        } else if (nb == 64 && NBMAX >= 64) {
+            Wgmma<(NBMAX >= 64 ? 64 : 16)>::f16(*reinterpret_cast<float(*)[NBMAX >= 64 ? 32 : 8]>(&d[0][0]), a0, bd, accum);
+            Wgmma<(NBMAX >= 64 ? 64 : 16)>::f16(*reinterpret_cast<float(*)[NBMAX >= 64 ? 32 : 8]>(&d[1][0]), a1, bd, accum);
+        } else if (NBMAX >= 96) {
+            Wgmma<(NBMAX >= 96 ? 96 : 16)>::f16(*reinterpret_cast<float(*)[NBMAX >= 96 ? 48 : 8]>(&d[0][0]), a0, bd, accum);
+            Wgmma<(NBMAX >= 96 ? 96 : 16)>::f16(*reinterpret_cast<float(*)[NBMAX >= 96 ? 48 : 8]>(&d[1][0]), a1, bd, accum);
+        }
+    }
+    wg_commit();
+    wg_wait<0>();
+#pragma unroll
+    for (int h = 0; h < 2; ++h) wg_fence_acc(d[h]);
+}
+
+template <int ACH, int NBMAX, int SB, int MODE>
 __global__ void __launch_bounds__(ST_THREADS) siren_tc_kernel(const __grid_constant__ StMaps maps, const StParams p) {
     constexpr int A_BYTES = ACH * ST_TILE * 128;
     constexpr int B_STAGE = NBMAX * 128;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);      // pointer arithmetic (not an integer round trip) keeps the shared address space: LDS / STS, not generic LD / ST
-    uint8_t* smA = smem;
-    uint8_t* smB = smem + A_BYTES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smB + SB * B_STAGE);      // b_full[SB], b_empty[SB], a_ready, acc_full
-    uint64_t* b_full = bars, *b_empty = bars + SB, *a_ready = bars + 2 * SB, *acc_full = a_ready + 1;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
-    float* sbias = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(tmem_slot + 4) + ((16u - (tc::smem_u32(tmem_slot + 4) & 15u)) & 15u));   // [bias_floats]
+    uint8_t* smAbuf[2] = {smem, smem + A_BYTES};
+    uint8_t* smB = smem + 2 * A_BYTES;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smB + SB * B_STAGE);      // b_full[SB], b_empty[SB]
+    uint64_t* b_full = bars, *b_empty = bars + SB;
+    float* sbias = reinterpret_cast<float*>(bars + 2 * SB);                // [bias_floats]
     float* sfirst = sbias + ((p.bias_floats + 3) & ~3);                    // per-tile first-layer bias [npad] + wxy [2 * npad]
     float* sx = sfirst + 3 * 384;                                          // x coordinate of every tile pixel [128]
 
@@ -103,21 +131,13 @@ __global__ void __launch_bounds__(ST_THREADS) siren_tc_kernel(const __grid_const
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < SB; ++s) { mbar_init(smem_u32(b_full + s), 1); mbar_init(smem_u32(b_empty + s), 1); }
-        mbar_init(smem_u32(a_ready), 128); mbar_init(smem_u32(acc_full), 1);
         asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
         for (int l = 0; l < p.nl; ++l) asm volatile("prefetch.tensormap [%0];\n" :: "l"(&maps.w[l]) : "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" :: "r"(smem_u32(tmem_slot)), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-    }
     for (int i = threadIdx.x; i < p.bias_floats; i += ST_THREADS) sbias[i] = __ldg(p.bias_table + i);
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == 4) {
         if (lane == 0) {       // ===== TMA producer: the weight tiles of every layer of every tile, in order =====
             uint32_t it = 0;
             for (long tile = blockIdx.x; tile < ntiles; tile += gridDim.x)
@@ -134,36 +154,11 @@ __global__ void __launch_bounds__(ST_THREADS) siren_tc_kernel(const __grid_const
                         }
                 }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {       // ===== MMA issuer =====
-            uint32_t it = 0, ar = 0;
-            for (long tile = blockIdx.x; tile < ntiles; tile += gridDim.x)
-                for (int l = 0; l < p.nl; ++l, ++ar) {
-                    const StLayer& L = p.L[l];
-                    const int nsl = L.npad / L.nb, nkc = (L.kpad + 63) >> 6;
-                    mbar_wait(smem_u32(a_ready), ar & 1);                  // operand written, previous accumulator drained
-                    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-                    const uint32_t idesc = (1u << 4) | ((uint32_t)(L.nb >> 3) << 17) | ((128u >> 4) << 24);
-                    for (int ns = 0; ns < nsl; ++ns)
-                        for (int kc = 0; kc < nkc; ++kc, ++it) {
-                            const int s = it % SB;
-                            mbar_wait(smem_u32(b_full + s), (it / SB) & 1);
-                            asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-                            const uint64_t adesc = make_smem_desc_sw<128>(smem_u32(smA + kc * (ST_TILE * 128)));
-                            const uint64_t bdesc = make_smem_desc_sw<128>(smem_u32(smB + s * B_STAGE));
-                            const int ksteps = min(4, (L.kpad - kc * 64) >> 4);       // K tail: columns beyond kpad hold stale operand data
-                            for (int k = 0; k < ksteps; ++k)
-                                umma_f16(tmem_base + (uint32_t)(ns * L.nb), adesc + 2 * k, bdesc + 2 * k, idesc, (kc > 0 || k > 0) ? 1u : 0u);
-                            umma_commit(smem_u32(b_empty + s));
-                        }
-                    umma_commit(smem_u32(acc_full));
-                }
-        }
-    } else {                   // ===== compute warps: thread = pixel (tile row) = TMEM lane =====
-        const int q = warp & 3;
-        const int row = q * 32 + lane;
-        const int te = threadIdx.x - 64;                                   // 0..127, for cooperative loops
-        uint32_t af = 0;
+    } else {                   // ===== consumer warpgroup: thread te = pixel (tile row) of the prologue / head; fragments for the MMAs =====
+        const int te = threadIdx.x;                                        // 0..127
+        const int fr = warp * 16 + (lane >> 2);                            // first accumulator row of this thread (+8, +64, +72)
+        uint32_t it = 0;
+        int cur = 0;                                                       // A buffer holding the current layer's operand
         for (long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
             const int n = (int)(tile / ((long)p.R * tiles_per_row));
             const int rem = (int)(tile - (long)n * p.R * tiles_per_row);
@@ -182,6 +177,7 @@ __global__ void __launch_bounds__(ST_THREADS) siren_tc_kernel(const __grid_const
             }
             asm volatile("bar.sync 1, 128;\n" ::: "memory");
             // ---- prologue: the tile's first operand ----
+            uint8_t* smA = smAbuf[cur];
             if (MODE == SM_BODY0 || MODE == SM_FACE) {
                 const int groups = p.e_npad >> 3;
                 for (int i = te; i < ST_TILE * groups; i += 128) {
@@ -201,10 +197,7 @@ __global__ void __launch_bounds__(ST_THREADS) siren_tc_kernel(const __grid_const
             } else {
                 // bilinear x2 of the previous level (align_corners = False).  Thread = tile pixel: ONE horizontal tap pair, four corner
                 // row pointers and four packed-half weights per thread and tile, then per 8-channel group four 16-byte loads,
-                // 1 HMUL2 + 3 HFMA2 per channel pair, one 16-byte store into the swizzled operand.  The first version walked
-                // (pixel, group) items: an integer division, a lerp_locate, four 64-bit addresses and 32 half->float conversions
-                // per item made this prologue 25 % of the level's instructions and -- with its three exposed L2 round trips --
-                // 41 % of the compute warps' time, more than the sine layers (ncu source page, profiles/r02_siren_tc_notes.txt).
+                // 1 HMUL2 + 3 HFMA2 per channel pair, one 16-byte store into the swizzled operand.
                 // The taps 0 / 0.25 / 0.75 / 1 and their products are exact in fp16; the weighted sum is rounded per operation
                 // (<= 2 ulp of the fp16 operand it becomes) instead of once.
                 const int Rh = p.R >> 1, CP = p.prev_c, groups = CP >> 3;
@@ -239,105 +232,116 @@ __global__ void __launch_bounds__(ST_THREADS) siren_tc_kernel(const __grid_const
                     }
                 }
             }
-            asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
-            asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-            mbar_arrive(smem_u32(a_ready));
+            asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");     // generic-proxy writes -> wgmma's async-proxy reads
+            asm volatile("bar.sync 1, 128;\n" ::: "memory");
             // ---- the layer chain ----
-            for (int l = 0; l < p.nl; ++l, ++af) {
+            for (int l = 0; l < p.nl; ++l) {
                 const StLayer& L = p.L[l];
-                mbar_wait(smem_u32(acc_full), af & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-                if (L.sine) {
-                    const float* lb = sbias + L.bias_off;
-                    const float xv = sx[row];
-#pragma unroll 1
-                    for (int c0 = 0; c0 < L.npad; c0 += 32) {
-                        uint32_t acc[32];
-                        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, acc);
+                const int nsl = L.npad / L.nb, nkc = (L.kpad + 63) >> 6;
+                const uint8_t* src = smAbuf[cur];
+                uint8_t* dst = smAbuf[cur ^ 1];
+                const float* lb = sbias + L.bias_off;
+                for (int ns = 0; ns < nsl; ++ns) {
+                    float d[2][NBMAX / 2];
+                    for (int kc = 0; kc < nkc; ++kc, ++it) {
+                        const int s = it % SB;
+                        mbar_wait(smem_u32(b_full + s), (it / SB) & 1);
+                        const int ksteps = min(4, (L.kpad - kc * 64) >> 4);       // K tail: columns beyond kpad hold stale operand data
+                        st_slice_mma<NBMAX>(d, L.nb, smem_u32(src + kc * (ST_TILE * 128)), smem_u32(smB + s * B_STAGE), ksteps, kc > 0);
+                        if (te == 0) mbar_arrive(smem_u32(b_empty + s));
+                    }
+                    if (L.sine) {
+                        // fragment (row, column pair) -> bias / first-layer terms -> sin -> the other A buffer (fp16)
 #pragma unroll
-                        for (int g8 = 0; g8 < 4; ++g8) {
-                            uint4 pk;
-                            __half2* h2 = reinterpret_cast<__half2*>(&pk);
+                        for (int g = 0; g < NBMAX / 8; ++g) {
+                            if (g * 8 >= L.nb) break;
 #pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                const int c = c0 + g8 * 8 + 2 * e;
-                                float v0 = __uint_as_float(acc[g8 * 8 + 2 * e]), v1 = __uint_as_float(acc[g8 * 8 + 2 * e + 1]);
-                                if (L.first) {
-                                    v0 += sfirst[c] + sfirst[384 + 2 * c] * xv + sfirst[384 + 2 * c + 1] * yv;
-                                    v1 += sfirst[c + 1] + sfirst[384 + 2 * c + 2] * xv + sfirst[384 + 2 * c + 3] * yv;
-                                } else {
-                                    v0 += lb[c]; v1 += lb[c + 1];
+                            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                                for (int e = 0; e < 2; ++e) {
+                                    const int row = h * 64 + fr + 8 * e;
+                                    const int c = ns * L.nb + 8 * g + 2 * (lane & 3);
+                                    float v0 = d[h][4 * g + 2 * e], v1 = d[h][4 * g + 2 * e + 1];
+                                    if (L.first) {
+                                        const float xv = sx[row];
+                                        v0 += sfirst[c] + sfirst[384 + 2 * c] * xv + sfirst[384 + 2 * c + 1] * yv;
+                                        v1 += sfirst[c + 1] + sfirst[384 + 2 * c + 2] * xv + sfirst[384 + 2 * c + 3] * yv;
+                                    } else {
+                                        v0 += lb[c]; v1 += lb[c + 1];
+                                    }
+                                    *reinterpret_cast<__half2*>(dst + a_off(row, c & ~7) + (c & 7) * 2) = __floats2half2_rn(st_sin(v0), st_sin(v1));
                                 }
-                                h2[e] = __floats2half2_rn(st_sin(v0), st_sin(v1));
+                        }
+                    } else {
+                        // linear head: 16 accumulator columns, transposed through the idle A buffer so that thread = pixel
+                        float* stage = reinterpret_cast<float*>(dst);              // [128][17]
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+#pragma unroll
+                            for (int j = 0; j < 2; ++j) {
+                                const int col = 8 * j + 2 * (lane & 3), row = h * 64 + fr;
+                                stage[row * 17 + col] = d[h][4 * j];           stage[row * 17 + col + 1] = d[h][4 * j + 1];
+                                stage[(row + 8) * 17 + col] = d[h][4 * j + 2]; stage[(row + 8) * 17 + col + 1] = d[h][4 * j + 3];
                             }
-                            *reinterpret_cast<uint4*>(smA + a_off(row, c0 + g8 * 8)) = pk;
+                        asm volatile("bar.sync 1, 128;\n" ::: "memory");
+                        const float* acc = stage + te * 17;
+                        const int x = x0 + te;
+                        if (MODE == SM_FACE) {
+#pragma unroll
+                            for (int c = 0; c < 4; ++c)
+                                p.face_out[(((size_t)n * 4 + c) * p.R + y) * p.R + x] = acc[c] + __ldg(p.head_bias + c);
+                        } else {
+                            float o[7];
+#pragma unroll
+                            for (int c = 0; c < 7; ++c) o[c] = acc[c] + __ldg(p.head_bias + c);   // grid_change(0,1) alpha(2) colour(3..6)
+                            const GsTap t = gs_locate(sx[te], yv, o[0], o[1], p.R, p.R);
+                            float w[4];
+                            gs_sample<4>(p.image.p + n * p.image.sn, p.image.sc, p.image.sh, p.R, p.R, t, w);
+                            const size_t plane = (size_t)p.R * p.R, pix = (size_t)y * p.R + x;
+                            const float alpha = o[2];
+                            if (p.o_f16) {
+                                __half* const* oh = reinterpret_cast<__half* const*>(p.o);
+#pragma unroll
+                                for (int c = 0; c < 4; ++c) {
+                                    oh[0][((size_t)n * 4 + c) * plane + pix] = __float2half_rn((1.0f - alpha) * w[c] + alpha * o[3 + c]);
+                                    oh[2][((size_t)n * 4 + c) * plane + pix] = __float2half_rn(o[3 + c]);
+                                    oh[3][((size_t)n * 4 + c) * plane + pix] = __float2half_rn(w[c]);
+                                }
+                                oh[1][(size_t)n * plane + pix] = __float2half_rn(alpha);
+                                oh[4][((size_t)n * 2) * plane + pix] = __float2half_rn(o[0]);
+                                oh[4][((size_t)n * 2 + 1) * plane + pix] = __float2half_rn(o[1]);
+                            } else {
+#pragma unroll
+                                for (int c = 0; c < 4; ++c) {
+                                    p.o[0][((size_t)n * 4 + c) * plane + pix] = (1.0f - alpha) * w[c] + alpha * o[3 + c];
+                                    p.o[2][((size_t)n * 4 + c) * plane + pix] = o[3 + c];
+                                    p.o[3][((size_t)n * 4 + c) * plane + pix] = w[c];
+                                }
+                                p.o[1][(size_t)n * plane + pix] = alpha;
+                                p.o[4][((size_t)n * 2) * plane + pix] = o[0];
+                                p.o[4][((size_t)n * 2 + 1) * plane + pix] = o[1];
+                            }
                         }
                     }
-                    const bool last = (l == p.nl - 1);
-                    if (!last) {
-                        asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
-                        asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-                        mbar_arrive(smem_u32(a_ready));
-                    } else {
+                }
+                if (L.sine) {
+                    asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
+                    asm volatile("bar.sync 1, 128;\n" ::: "memory");             // the whole output is written before anyone reads it
+                    cur ^= 1;
+                    if (l == p.nl - 1) {
                         // levels 0 / 1: the last sine layer's output is the level's output tensor (fp16 NHWC)
-                        asm volatile("bar.sync 1, 128;\n" ::: "memory");
                         const int groups = p.out_c >> 3;
-                        __half* dst = p.out + (((size_t)n * p.R + y) * p.R + x0) * p.out_c;
+                        __half* dstg = p.out + (((size_t)n * p.R + y) * p.R + x0) * p.out_c;
                         for (int i = te; i < ST_TILE * groups; i += 128) {
                             const int r = i / groups, cg = i - r * groups;
-                            *reinterpret_cast<uint4*>(dst + (size_t)r * p.out_c + cg * 8) = *reinterpret_cast<const uint4*>(smA + a_off(r, cg * 8));
-                        }
-                        asm volatile("bar.sync 1, 128;\n" ::: "memory");      // the next tile's prologue overwrites the operand
-                    }
-                } else {
-                    // linear head: 16 accumulator columns, thread = pixel
-                    uint32_t acc[32];
-                    tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16), acc);
-                    const int x = x0 + row;
-                    if (MODE == SM_FACE) {
-#pragma unroll
-                        for (int c = 0; c < 4; ++c)
-                            p.face_out[(((size_t)n * 4 + c) * p.R + y) * p.R + x] = __uint_as_float(acc[c]) + __ldg(p.head_bias + c);
-                    } else {
-                        float o[7];
-#pragma unroll
-                        for (int c = 0; c < 7; ++c) o[c] = __uint_as_float(acc[c]) + __ldg(p.head_bias + c);   // grid_change(0,1) alpha(2) colour(3..6)
-                        const GsTap t = gs_locate(sx[row], yv, o[0], o[1], p.R, p.R);
-                        float w[4];
-                        gs_sample<4>(p.image.p + n * p.image.sn, p.image.sc, p.image.sh, p.R, p.R, t, w);
-                        const size_t plane = (size_t)p.R * p.R, pix = (size_t)y * p.R + x;
-                        const float alpha = o[2];
-                        if (p.o_f16) {
-                            __half* const* oh = reinterpret_cast<__half* const*>(p.o);
-#pragma unroll
-                            for (int c = 0; c < 4; ++c) {
-                                oh[0][((size_t)n * 4 + c) * plane + pix] = __float2half_rn((1.0f - alpha) * w[c] + alpha * o[3 + c]);
-                                oh[2][((size_t)n * 4 + c) * plane + pix] = __float2half_rn(o[3 + c]);
-                                oh[3][((size_t)n * 4 + c) * plane + pix] = __float2half_rn(w[c]);
-                            }
-                            oh[1][(size_t)n * plane + pix] = __float2half_rn(alpha);
-                            oh[4][((size_t)n * 2) * plane + pix] = __float2half_rn(o[0]);
-                            oh[4][((size_t)n * 2 + 1) * plane + pix] = __float2half_rn(o[1]);
-                        } else {
-#pragma unroll
-                            for (int c = 0; c < 4; ++c) {
-                                p.o[0][((size_t)n * 4 + c) * plane + pix] = (1.0f - alpha) * w[c] + alpha * o[3 + c];
-                                p.o[2][((size_t)n * 4 + c) * plane + pix] = o[3 + c];
-                                p.o[3][((size_t)n * 4 + c) * plane + pix] = w[c];
-                            }
-                            p.o[1][(size_t)n * plane + pix] = alpha;
-                            p.o[4][((size_t)n * 2) * plane + pix] = o[0];
-                            p.o[4][((size_t)n * 2 + 1) * plane + pix] = o[1];
+                            *reinterpret_cast<uint4*>(dstg + (size_t)r * p.out_c + cg * 8) = *reinterpret_cast<const uint4*>(smAbuf[cur] + a_off(r, cg * 8));
                         }
                     }
-                    asm volatile("bar.sync 1, 128;\n" ::: "memory");          // sx / sfirst / the operand are rewritten by the next tile
                 }
             }
+            asm volatile("bar.sync 1, 128;\n" ::: "memory");          // sx / sfirst / the operands are rewritten by the next tile
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" :: "r"(tmem_base), "r"(TMEM_COLS) : "memory");
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -369,15 +373,17 @@ CUtensorMap weight_tile_map(const void* W, int rows, int kpad, int nb) {
     return m;
 }
 
-template <int ACH, int NBMAX, int SB, int TMEM_COLS, int MODE>
+template <int ACH, int NBMAX, int SB, int MODE>
 void launch_siren_tc(const StMaps& maps, const StParams& p, int ctas_per_sm, cudaStream_t s) {
-    const size_t smem = 1024 + (size_t)ACH * ST_TILE * 128 + (size_t)SB * NBMAX * 128 + (2 * SB + 2) * 8 + 16 + 16 +
+    const size_t smem = 1024 + 2 * (size_t)ACH * ST_TILE * 128 + (size_t)SB * NBMAX * 128 + 2 * SB * 8 +
                         ((size_t)((p.bias_floats + 3) & ~3) + 3 * 384 + 128) * sizeof(float);
     THA4_REQUIRE(smem <= 227 * 1024, "siren_tc: shared memory budget");
-    THA4_ENSURE_SMEM((siren_tc_kernel<ACH, NBMAX, SB, TMEM_COLS, MODE>), smem);
+    for (int l = 0; l < p.nl; ++l)        // st_slice_mma issues the slice widths up to NBMAX only
+        THA4_REQUIRE(p.L[l].nb <= NBMAX && p.L[l].npad % p.L[l].nb == 0, "siren_tc: N slice width of layer " + std::to_string(l));
+    THA4_ENSURE_SMEM((siren_tc_kernel<ACH, NBMAX, SB, MODE>), smem);
     const long ntiles = (long)p.B * p.R * (p.R / ST_TILE);
-    const int grid = (int)std::min<long>(ntiles, 148L * ctas_per_sm);
-    siren_tc_kernel<ACH, NBMAX, SB, TMEM_COLS, MODE><<<grid, ST_THREADS, smem, s>>>(maps, p);
+    const int grid = (int)std::min<long>(ntiles, (long)num_sms() * ctas_per_sm);
+    siren_tc_kernel<ACH, NBMAX, SB, MODE><<<grid, ST_THREADS, smem, s>>>(maps, p);
     THA4_LAUNCH_CHECK();
 }
 
@@ -390,6 +396,7 @@ bool siren_tc_enabled() { return g_siren_tc; }
 
 void SirenTcPlan::add(const SirenLayer& l, int nb, int sine, int first) {
     THA4_REQUIRE(nl < 8, "siren_tc: too many layers");
+    THA4_REQUIRE(nb == 16 || nb == 64 || nb == 96, "siren_tc: N slice width");
     kpad[nl] = l.KPAD; npad[nl] = sine ? l.NPAD : 16; this->nb[nl] = nb; this->sine[nl] = sine; this->first[nl] = first;
     W[nl] = l.W; rows[nl] = l.NPAD; bias[nl] = l.bias;
     ++nl;
@@ -423,11 +430,11 @@ void siren_tc_run(Runtime& rt, int mode, const SirenTcPlan& plan, const SirenTcL
     p.face_out = lv.face_out; p.head_bias = lv.head_bias;
     cudaStream_t s = rt.stream;
     ProfScope prof(PROF_SIREN, s);
-    //                         A chunks, widest weight tile, ring, TMEM columns
-    if (mode == SM_BODY0) launch_siren_tc<6, 192, 4, 512, SM_BODY0>(maps, p, 1, s);
-    else if (mode == SM_BODY1) launch_siren_tc<3, 96, 4, 256, SM_BODY1>(maps, p, 2, s);
-    else if (mode == SM_BODY2) launch_siren_tc<2, 96, 2, 128, SM_BODY2>(maps, p, 4, s);      // 56 KB per CTA: four tiles in flight per SM
-    else launch_siren_tc<2, 128, 2, 128, SM_FACE>(maps, p, 3, s);
+    //                         A chunks, widest weight tile, ring
+    if (mode == SM_BODY0) launch_siren_tc<6, 96, 2, SM_BODY0>(maps, p, 1, s);          // two 96 KB operand buffers
+    else if (mode == SM_BODY1) launch_siren_tc<3, 96, 4, SM_BODY1>(maps, p, 1, s);
+    else if (mode == SM_BODY2) launch_siren_tc<2, 96, 2, SM_BODY2>(maps, p, 2, s);
+    else launch_siren_tc<2, 64, 2, SM_FACE>(maps, p, 2, s);
 }
 
 }  // namespace tha4

@@ -1,4 +1,4 @@
-// Per-pixel epilogue of the fused decoder tails, shared by the fp32 (mma.sync, strict-capable) and the tcgen05 kernels:
+// Per-pixel epilogue of the fused decoder tails, shared by the fp32 (mma.sync, strict-capable) and the wgmma kernels:
 // head outputs of ONE pixel -> sigmoid / tanh -> affine_grid + grid_sample of the RGBA image -> alpha blends -> planar
 // NCHW stores of every tensor the network returns.  Reference: eyebrow_decomposer_00.py:49-64,
 // eyebrow_morphing_combiner_00.py:51-72, face_morpher_08.py:170-193, morpher_00.py:53-66, upscaler_02.py:84-96.

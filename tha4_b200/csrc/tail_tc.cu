@@ -1,5 +1,4 @@
-// Fused decoder tail on the Blackwell paths (default precision mode) -- SURVEY.md section 8 a-T, the kernel BASELINE.json's
-// "grid_sample + decoder %HBM-roofline" names.  From the RAW last feature map of a network (f16, NHWC, written by the
+// Fused decoder tail on the tensor cores (default precision mode) -- SURVEY.md section 8 a-T.  From the RAW last feature map of a network (f16, NHWC, written by the
 // producing conv's epilogue) to every tensor the network returns, one pass, HBM-bound by design:
 //
 //   TMA     one 4-D box {C ch, 130 w, TR+2 h, 1 n} = the (TR+2) x 130 pixel HALO of a 128 x TR pixel tile lands in shared
@@ -7,12 +6,12 @@
 //           zero-filled = the head conv's zero padding.  The nine 16 x C head-weight tiles come in with one more box.
 //   warps   apply the pending GroupNorm / InstanceNorm affine + SiLU / ReLU to the halo IN PLACE (the affine is rebuilt
 //           per CTA from the statistics the producing conv accumulated: no finalize kernel, no coefficient tensor).
-//   UMMA    the 3x3 head conv is 9 taps x C/16 tcgen05.mma (M = 128 pixels of one tile row, N = 16 head channels, K = 16)
-//           per tile row, straight from the halo: the A descriptor of tap (dy, dx) is the SAME shared-memory image with
-//           its start address shifted by (dy * 130 + dx) rows -- the tensor core applies the swizzle on absolute
-//           addresses, so any row shift is legal (profiles/r02_umma_row_shift_probe.txt).  Accumulators: TR x 16 TMEM columns.
-//   drain   tcgen05.ld gives every thread the 16 head outputs of ITS pixel (lane = pixel): no shared-memory transpose;
-//           sigmoid / tanh, affine_grid + grid_sample (4-tap gather from the planar image), blends, and planar NCHW stores
+//   wgmma   the 3x3 head conv is 9 taps x C/16 x 2 wgmma (M = 128 pixels of one tile row as two m64 halves, N = 16 head
+//           channels, K = 16) per tile row, straight from the halo: the A descriptor of tap (dy, dx) is the SAME shared-memory
+//           image with its start address shifted by (dy * 130 + dx) rows -- the tensor core applies the swizzle on absolute
+//           addresses, so any row shift is legal.  Accumulators: TR x 16 columns in registers.
+//   drain   the accumulator goes through shared memory (the halo is free by then) so that every thread gets the 16 head
+//           outputs of ITS pixel; sigmoid / tanh, affine_grid + grid_sample (4-tap gather from the planar image), blends, and planar NCHW stores
 //           where the 32 lanes of a warp write 32 consecutive pixels = one full 128-byte line per channel.
 // Reference: morpher_00.py:53-66, upscaler_02.py:84-96, face_morpher_08.py:170-193, eyebrow_morphing_combiner_00.py:51-72,
 // eyebrow_decomposer_00.py:49-64.  The fp32 / strict variant is tail.cu.
@@ -54,7 +53,6 @@ template <int C> struct TailCfg {
     static constexpr int HROWS = (TR + 2) * TT_HW;    // halo pixels
     static constexpr int A_BYTES = ((HROWS * ROWB + 1023) / 1024) * 1024;
     static constexpr int B_BYTES = 9 * TT_N * ROWB;
-    static constexpr int TMEM_COLS = TR * TT_N < 32 ? 32 : TR * TT_N;
     static constexpr size_t SMEM = 1024 + A_BYTES + B_BYTES + 2 * C * sizeof(float) + 2 * C * sizeof(double) + 16 * sizeof(float) + 64;
 };
 
@@ -71,26 +69,18 @@ __global__ void __launch_bounds__(TT_THREADS) tail_tc_kernel(const __grid_consta
     float* cA = reinterpret_cast<float*>(chs + 2 * C);                   // [C] affine
     float* cB = cA + C;
     float* sbias = cB + C;                                               // [16]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sbias + 16);            // tma_full, mma_done
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sbias + 16);            // tma_full
 
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int n = blockIdx.z, x0 = blockIdx.x * TT_W, y0 = blockIdx.y * TR;
 
     if (tid == 0) {
-        mbar_init(smem_u32(bars), 1); mbar_init(smem_u32(bars + 1), 1);
+        mbar_init(smem_u32(bars), 1);
         asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
         asm volatile("prefetch.tensormap [%0];\n" :: "l"(&tmF) : "memory");
         asm volatile("prefetch.tensormap [%0];\n" :: "l"(&tmW) : "memory");
     }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" :: "r"(smem_u32(tmem_slot)), "r"(Cfg::TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
     pdl_trigger();
     if (tid == 0) {        // the head weights do not depend on the previous kernel: fetch them ahead of the dependency wait
         mbar_expect_tx(smem_u32(bars), Cfg::HROWS * ROWB + Cfg::B_BYTES);
@@ -159,90 +149,88 @@ __global__ void __launch_bounds__(TT_THREADS) tail_tc_kernel(const __grid_consta
     asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");          // generic-proxy writes -> the tensor core's async-proxy reads
     __syncthreads();
 
-    // ---- 3x3 head conv: one elected thread issues TR x 9 x C/16 MMAs on row-shifted views of the halo ----
-    if (tid == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-        constexpr uint32_t idesc = (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(TT_N >> 3) << 17) | ((128u >> 4) << 24);
-#pragma unroll 1
-        for (int r = 0; r < TR; ++r)
-#pragma unroll 1
-            for (int tap = 0; tap < 9; ++tap) {
-                const int dy = tap / 3, dx = tap - 3 * dy;
-                const uint64_t adesc = make_smem_desc_sw<ROWB>(smem_u32(smA + ((r + dy) * TT_HW + dx) * ROWB));
-                const uint64_t bdesc = make_smem_desc_sw<ROWB>(smem_u32(smB + tap * TT_N * ROWB));
+    // ---- 3x3 head conv: the warpgroup issues TR x 9 x C/16 x 2 wgmma on row-shifted views of the halo ----
+    float acc[TR][2][8];
+    wg_fence();
 #pragma unroll
-                for (int k = 0; k < C / 16; ++k)
-                    umma_f16(tmem_base + (uint32_t)(r * TT_N), adesc + 2 * k, bdesc + 2 * k, idesc, (tap > 0 || k > 0) ? 1u : 0u);
-            }
-        umma_commit(smem_u32(bars + 1));
-    }
-    mbar_wait(smem_u32(bars + 1), 0);
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-
-    // ---- drain: thread = pixel column x0 + tid; its 16 head outputs per tile row come straight out of TMEM ----
-    const int x = x0 + tid;
-#pragma unroll 1
-    for (int r0 = 0; r0 < TR; r0 += 2) {
-        uint32_t acc[32];
-        tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(r0 * TT_N), acc);     // two tile rows x 16 columns
-        if (x < p.S) {
+    for (int r = 0; r < TR; ++r)
 #pragma unroll
-            for (int rr = 0; rr < 2; ++rr) {
-                float o[TAIL_CO_PAD];
+        for (int tap = 0; tap < 9; ++tap) {
+            const int dy = tap / 3, dx = tap - 3 * dy;
+            const uint32_t a = smem_u32(smA + ((r + dy) * TT_HW + dx) * ROWB), b = smem_u32(smB + tap * TT_N * ROWB);
 #pragma unroll
-                for (int j = 0; j < TAIL_CO_PAD; ++j) o[j] = fmaf(__uint_as_float(acc[rr * TT_N + j]), p.acc_scale, sbias[j]);
-                tail_epilogue<KIND>(o, n, y0 + r0 + rr, x, p.S, p.img0, p.img1, p.base, p.o[0], p.o[1], p.o[2], p.o[3], p.o[4], p.o[5], p.o[6], p.o[7]);
+            for (int k = 0; k < C / 16; ++k) {
+                const uint64_t bd = make_smem_desc_sw<ROWB>(b + 32 * k);
+                Wgmma<TT_N>::f16(acc[r][0], make_smem_desc_sw<ROWB>(a + 32 * k), bd, (tap > 0 || k > 0) ? 1u : 0u);
+                Wgmma<TT_N>::f16(acc[r][1], make_smem_desc_sw<ROWB>(a + 64 * ROWB + 32 * k), bd, (tap > 0 || k > 0) ? 1u : 0u);
             }
         }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" :: "r"(tmem_base), "r"(Cfg::TMEM_COLS) : "memory");
-}
+    wg_commit();
+    wg_wait<0>();
+#pragma unroll
+    for (int r = 0; r < TR; ++r) { wg_fence_acc(acc[r][0]); wg_fence_acc(acc[r][1]); }
 
+    // ---- drain: thread = pixel column x0 + tid; its 16 head outputs per tile row, transposed through the (now idle) halo ----
+    float* stage = reinterpret_cast<float*>(smA);                        // [128][17]
+    const int x = x0 + tid;
+#pragma unroll
+    for (int r = 0; r < TR; ++r) {
+        __syncthreads();                                                 // every wgmma has read the halo / the previous row is drained
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+                const int col = 8 * j + 2 * (lane & 3), row = h * 64 + warp * 16 + (lane >> 2);
+                stage[row * 17 + col] = acc[r][h][4 * j];           stage[row * 17 + col + 1] = acc[r][h][4 * j + 1];
+                stage[(row + 8) * 17 + col] = acc[r][h][4 * j + 2]; stage[(row + 8) * 17 + col + 1] = acc[r][h][4 * j + 3];
+            }
+        __syncthreads();
+        if (x < p.S) {
+            float o[TAIL_CO_PAD];
+#pragma unroll
+            for (int j = 0; j < TAIL_CO_PAD; ++j) o[j] = fmaf(stage[tid * 17 + j], p.acc_scale, sbias[j]);
+            tail_epilogue<KIND>(o, n, y0 + r, x, p.S, p.img0, p.img1, p.base, p.o[0], p.o[1], p.o[2], p.o[3], p.o[4], p.o[5], p.o[6], p.o[7]);
+        }
+    }
+}
 
 // ---------------------------------------------------------------------------------------------------------------------
 // PERSISTENT, software-pipelined version (the default).  The kernel above runs one tile per CTA and its phases -- statistics
 // fold, halo TMA, in-place normalisation, MMAs, gather / blend / store drain -- are a serial chain, co-resident CTAs all start
-// together, so nothing overlaps (ncu at B=1, Upscaler02 site: 46 us, every unit < 16 % busy).  Here ONE CTA per SM walks a
-// contiguous range of tiles with the phases on different warps and different tiles:
-//   warp 0      TMA producer: halo boxes into an NS-deep ring (the head weights once)
-//   warp 1      MMA issuer: TR x 9 x C/16 tcgen05.mma per tile into one of TWO accumulator slots in TMEM
-//   warps 2..   workers (4 * TR warps), two stages on the same warps, two tiles apart, the drain split around the transform:
-//               drain A(i):       tcgen05.ld of the pixel's grid_change outputs -> gs_locate -> the four corner pixels requested;
+// together, so nothing overlaps.  Here ONE CTA per SM walks a contiguous range of tiles with the phases on different warps
+// and different tiles:
+//   warps 0-3   MMA warpgroup: per tile row 9 x C/16 x 2 wgmma (register accumulator, 16 columns), then the 16 head outputs
+//               of every pixel go to one of TWO accumulator slots in shared memory
+//   warp 4      TMA producer: halo boxes into an NS-deep ring (the head weights once)
+//   warps 5..   workers (4 * TR warps), two stages on the same warps, two tiles apart, the drain split around the transform:
+//               drain A(i):       the pixel's grid_change outputs from the slot -> gs_locate -> the four corner pixels requested;
 //               transform(i + 2): normalise + activate the landed halo in place (the per-channel affine is rebuilt once per
 //                                 SAMPLE, not per tile), every worker thread;
-//               drain B(i):       tcgen05.ld again -> tail_epilogue with the corners that arrived meanwhile (thread = pixel).
-// (profiles/r02_tail_persist_notes.txt: the seven versions on the way here and what the ncu source page showed for each)
-// mbarriers: h_full (TMA -> transform), h_xf (transform -> MMA, one arrival per worker thread), h_empty (MMA commit -> TMA),
-// acc_full (MMA commit -> drain), acc_empty (drain -> MMA, one arrival per drain warp once its tcgen05.ld has completed).
+//               drain B(i):       the slot again -> tail_epilogue with the corners that arrived meanwhile (thread = pixel).
+// mbarriers: h_full (TMA -> transform), h_xf (transform -> MMA, one arrival per worker thread), h_empty (MMA -> TMA, one
+// arrival per MMA thread once its wgmma have completed), acc_full (MMA -> drain, one arrival per MMA thread after its slot
+// stores), acc_empty (drain -> MMA, one arrival per drain thread once it has read the slot).
 template <int C, int TR> struct TailPCfg {
     static constexpr int ROWB = 2 * C;
     static constexpr int HROWS = (TR + 2) * TT_HW;
     static constexpr int A_BYTES = ((HROWS * ROWB + 1023) / 1024) * 1024;
-    static constexpr int NS = 3;                                            // halo ring depth (the transform runs two tiles ahead of the drain)
-    static_assert(C == 32 || TR == 2, "64-channel sites: TR = 2 (three 66 KB halo slots fit, three 100 KB slots do not)");
+    static constexpr int NS = C == 32 ? 3 : 2;                              // halo ring depth (32 channels: the transform runs two tiles
+                                                                            // ahead of the drain; three 66 KB slots of 64 channels do not fit)
     static constexpr int B_BYTES = 9 * TT_N * ROWB;
-    static constexpr int ACC_COLS = TR * TT_N;                              // TMEM columns of one accumulator slot
-    static constexpr int TMEM_COLS = 2 * ACC_COLS < 32 ? 32 : 2 * ACC_COLS; // 64 / 128: a power of two
+    static constexpr int SLOT_FLOATS = TR * TT_W * TT_N;                    // one accumulator slot: [TR rows][128 pixels][16 outputs]
     static constexpr int DRAIN_WARPS = 4 * TR;                              // one thread per output pixel of a tile
-    static constexpr int WORKER_WARPS = DRAIN_WARPS;                        // every worker warp transforms AND drains (18 / 10 warps per CTA: the
-                                                                            // register cap stays above what the split drain keeps live)
-    static constexpr int THREADS = (2 + WORKER_WARPS) * 32;
+    static constexpr int WORKER_WARPS = DRAIN_WARPS;                        // every worker warp transforms AND drains
+    static constexpr int THREADS = (5 + WORKER_WARPS) * 32;
     static constexpr int NBARS = 3 * NS + 5;
     static constexpr int MAX_S = 512;                                       // base-grid copy in shared memory
-    static constexpr size_t SMEM = 1024 + (size_t)NS * A_BYTES + B_BYTES + 2 * C * sizeof(double) + 2 * C * sizeof(float) + 16 * sizeof(float) +
-                                   MAX_S * sizeof(float) + NBARS * sizeof(uint64_t) + 16;
+    static constexpr size_t SMEM = 1024 + (size_t)NS * A_BYTES + B_BYTES + 2 * (size_t)SLOT_FLOATS * sizeof(float) + 2 * C * sizeof(double) +
+                                   2 * C * sizeof(float) + 16 * sizeof(float) + MAX_S * sizeof(float) + NBARS * sizeof(uint64_t) + 16;
+    static_assert(SMEM <= 227 * 1024, "tail_tc: shared memory budget");
 };
 
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-}
+// position of head output `col` of pixel `px` in a slot row: 16-byte chunks XOR-swizzled so that eight consecutive pixels
+// reading the same chunk (LDS.128) hit eight different bank groups
+__device__ __forceinline__ int tp_slot_off(int px, int col) { return px * TT_N + (((col >> 2) ^ ((px >> 1) & 3)) << 2) + (col & 3); }
 
 template <int KIND, int C, int TR>
 __global__ void __launch_bounds__(TailPCfg<C, TR>::THREADS, 1) tail_tc_persist_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constant__ CUtensorMap tmW,
@@ -253,7 +241,8 @@ __global__ void __launch_bounds__(TailPCfg<C, TR>::THREADS, 1) tail_tc_persist_k
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* smA = smem;
     uint8_t* smB = smem + NS * Cfg::A_BYTES;
-    double* chs = reinterpret_cast<double*>(smB + Cfg::B_BYTES);         // [C][2] folded statistics
+    float* slots = reinterpret_cast<float*>(smB + Cfg::B_BYTES);          // [2][SLOT_FLOATS] accumulator slots
+    double* chs = reinterpret_cast<double*>(slots + 2 * Cfg::SLOT_FLOATS); // [C][2] folded statistics
     float* cA = reinterpret_cast<float*>(chs + 2 * C);                   // [C] affine
     float* cB = cA + C;
     float* sbias = cB + C;                                               // [16]
@@ -261,7 +250,6 @@ __global__ void __launch_bounds__(TailPCfg<C, TR>::THREADS, 1) tail_tc_persist_k
     uint64_t* bars = reinterpret_cast<uint64_t*>(sbase + Cfg::MAX_S);
     uint64_t* h_full = bars, *h_xf = bars + NS, *h_empty = bars + 2 * NS;
     uint64_t* acc_full = bars + 3 * NS, *acc_empty = acc_full + 2, *w_full = acc_empty + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(w_full + 1);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int tiles_x = (p.S + TT_W - 1) / TT_W, tiles_y = p.S / TR, per_n = tiles_x * tiles_y;
@@ -270,31 +258,24 @@ __global__ void __launch_bounds__(TailPCfg<C, TR>::THREADS, 1) tail_tc_persist_k
     const int nt = (int)((long)(blockIdx.x + 1) * total / gridDim.x) - t_begin;       // contiguous tiles of this CTA (>= 1: grid <= total)
 
     if (tid == 0) {
-        for (int s = 0; s < NS; ++s) { mbar_init(smem_u32(h_full + s), 1); mbar_init(smem_u32(h_xf + s), Cfg::WORKER_WARPS * 32); mbar_init(smem_u32(h_empty + s), 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(smem_u32(acc_full + a), 1); mbar_init(smem_u32(acc_empty + a), Cfg::DRAIN_WARPS); }
+        for (int s = 0; s < NS; ++s) { mbar_init(smem_u32(h_full + s), 1); mbar_init(smem_u32(h_xf + s), Cfg::WORKER_WARPS * 32); mbar_init(smem_u32(h_empty + s), 128); }
+        for (int a = 0; a < 2; ++a) { mbar_init(smem_u32(acc_full + a), 128); mbar_init(smem_u32(acc_empty + a), Cfg::DRAIN_WARPS * 32); }
         mbar_init(smem_u32(w_full), 1);
         asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
         asm volatile("prefetch.tensormap [%0];\n" :: "l"(&tmF) : "memory");
         asm volatile("prefetch.tensormap [%0];\n" :: "l"(&tmW) : "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" :: "r"(smem_u32(tmem_slot)), "r"(Cfg::TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-    }
     if (tid >= 64 && tid < 80) sbias[tid - 64] = (tid - 64) < TAIL_CO_PAD ? __ldg(p.bias + (tid - 64)) : 0.0f;     // weights: independent of the previous kernel
     for (int i = tid; i < p.S; i += Cfg::THREADS) sbase[i] = __ldg(p.base + i);                                     // constant table
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
     pdl_trigger();
-    if (tid == 0) {        // the head weights do not depend on the previous kernel: fetch them ahead of the dependency wait
+    if (tid == 128) {      // the head weights do not depend on the previous kernel: fetch them ahead of the dependency wait
         mbar_expect_tx(smem_u32(w_full), Cfg::B_BYTES);
         tma_load_3d(smem_u32(smB), &tmW, 0, 0, 0, smem_u32(w_full));
     }
     pdl_wait();
 
-    if (warp == 0) {
+    if (warp == 4) {
         if (lane == 0) {   // ===== TMA producer =====
             for (int i = 0; i < nt; ++i) {
                 const int s = i % NS;
@@ -306,49 +287,63 @@ __global__ void __launch_bounds__(TailPCfg<C, TR>::THREADS, 1) tail_tc_persist_k
                 tma_load_4d(smem_u32(smA + s * Cfg::A_BYTES), &tmF, 0, tx * TT_W - 1, ty * TR - 1, n, smem_u32(h_full + s));
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {   // ===== MMA issuer: TR tile rows x 9 taps = row-shifted views of the halo =====
-            constexpr uint32_t idesc = (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(TT_N >> 3) << 17) | ((128u >> 4) << 24);
-            mbar_wait(smem_u32(w_full), 0);
-            for (int i = 0; i < nt; ++i) {
-                const int s = i % NS, a = i & 1;
-                mbar_wait(smem_u32(acc_empty + a), ((i >> 1) & 1) ^ 1);
-                mbar_wait(smem_u32(h_xf + s), (i / NS) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-                const uint8_t* hA = smA + s * Cfg::A_BYTES;
+    } else if (warp < 4) {
+        // ===== MMA warpgroup: TR tile rows x 9 taps = row-shifted views of the halo; accumulator -> slot =====
+        mbar_wait(smem_u32(w_full), 0);
+        for (int i = 0; i < nt; ++i) {
+            const int s = i % NS, a = i & 1;
+            mbar_wait(smem_u32(acc_empty + a), ((i >> 1) & 1) ^ 1);
+            mbar_wait(smem_u32(h_xf + s), (i / NS) & 1);
+            const uint8_t* hA = smA + s * Cfg::A_BYTES;
+            float* slot = slots + a * Cfg::SLOT_FLOATS;
 #pragma unroll 1
-                for (int r = 0; r < TR; ++r)
-#pragma unroll 1
-                    for (int tap = 0; tap < 9; ++tap) {
-                        const int dy = tap / 3, dx = tap - 3 * dy;
-                        const uint64_t adesc = make_smem_desc_sw<ROWB>(smem_u32(hA + ((r + dy) * TT_HW + dx) * ROWB));
-                        const uint64_t bdesc = make_smem_desc_sw<ROWB>(smem_u32(smB + tap * TT_N * ROWB));
+            for (int r = 0; r < TR; ++r) {
+                float acc[2][8];
+                wg_fence();
 #pragma unroll
-                        for (int k = 0; k < C / 16; ++k)
-                            umma_f16(tmem_base + (uint32_t)(a * Cfg::ACC_COLS + r * TT_N), adesc + 2 * k, bdesc + 2 * k, idesc, (tap > 0 || k > 0) ? 1u : 0u);
+                for (int tap = 0; tap < 9; ++tap) {
+                    const int dy = tap / 3, dx = tap - 3 * dy;
+                    const uint32_t ap = smem_u32(hA + ((r + dy) * TT_HW + dx) * ROWB), bp = smem_u32(smB + tap * TT_N * ROWB);
+#pragma unroll
+                    for (int k = 0; k < C / 16; ++k) {
+                        const uint64_t bd = make_smem_desc_sw<ROWB>(bp + 32 * k);
+                        Wgmma<TT_N>::f16(acc[0], make_smem_desc_sw<ROWB>(ap + 32 * k), bd, (tap > 0 || k > 0) ? 1u : 0u);
+                        Wgmma<TT_N>::f16(acc[1], make_smem_desc_sw<ROWB>(ap + 64 * ROWB + 32 * k), bd, (tap > 0 || k > 0) ? 1u : 0u);
                     }
-                umma_commit(smem_u32(h_empty + s));          // the halo slot is free once these MMAs have read it
-                umma_commit(smem_u32(acc_full + a));
+                }
+                wg_commit();
+                wg_wait<0>();
+                wg_fence_acc(acc[0]); wg_fence_acc(acc[1]);
+                float* srow = slot + r * (TT_W * TT_N);
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int j = 0; j < 2; ++j)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int px = h * 64 + warp * 16 + (lane >> 2) + 8 * e, col = 8 * j + 2 * (lane & 3);
+                            *reinterpret_cast<float2*>(srow + tp_slot_off(px, col)) = make_float2(acc[h][4 * j + 2 * e], acc[h][4 * j + 2 * e + 1]);
+                        }
             }
+            mbar_arrive(smem_u32(h_empty + s));          // this thread's wgmma have read the halo slot
+            mbar_arrive(smem_u32(acc_full + a));         // and its part of the accumulator slot is written
         }
     } else {
-        // ===== worker warps (2 ..): BOTH remaining stages, on every warp =====
+        // ===== worker warps (5 ..): BOTH remaining stages, on every warp =====
         //   transform(i + 1): normalise + activate the landed halo of the NEXT tile in place, all WORKERS threads;
-        //   drain(i):         one thread per output pixel of the current tile (the first 4 * TR warps).
-        // The first version gave the transform four dedicated warps: one warp per scheduler, 0.2 IPC on dependent
-        // conversions / MUFU, 7 000 cycles per tile and the slowest stage of the pipeline while sixteen drain warps waited
-        // (ncu source page, profiles/r02_tail_persist_notes.txt).  A thread owns ONE 16-byte chunk column (8 channels) of the
-        // halo rows wt / NCH + k * (WORKERS / NCH): its 16 coefficients live in registers, XU rows are in flight at once.
+        //   drain(i):         one thread per output pixel of the current tile.
+        // A thread owns ONE 16-byte chunk column (8 channels) of the halo rows wt / NCH + k * (WORKERS / NCH): its 16
+        // coefficients live in registers, XU rows are in flight at once.
         constexpr int WORKERS = Cfg::WORKER_WARPS * 32;
         constexpr int RSTEP = WORKERS / NCH;
         constexpr int ITEMS = (Cfg::HROWS + RSTEP - 1) / RSTEP, ITERS = (ITEMS + 5) / 6, XU = (ITEMS + ITERS - 1) / ITERS;
-        const int wt = tid - 64, wid = warp - 2;
+        const int wt = tid - 160, wid = warp - 5;
         const int jc = wt % NCH, r_first = wt / NCH;
         const int cpg = p.groups == 0 ? 1 : C / p.groups;
         const bool silu = p.act == ACT_SILU || p.act == ACT_SILU_FAST;
         const bool relu = p.act == ACT_RELU;
-        const int q = warp & 3;                                                  // TMEM lane quadrant this warp may access
-        const int dr = wid >> 2;                                                 // drain: tile row (each quadrant appears once per row)
+        const int q = wid & 3;                                                   // drain: 32-pixel group of the tile row
+        const int dr = wid >> 2;                                                 // drain: tile row
         float av[8], bv[8];
         int cur_n = -1;
 
@@ -430,8 +425,8 @@ __global__ void __launch_bounds__(TailPCfg<C, TR>::THREADS, 1) tail_tc_persist_k
 
         // The drain of a tile is split around the transform of the next one: phase A reads the two grid_change outputs of the
         // pixel and REQUESTS the four corner pixels of its sampling tap; the transform runs while they travel; phase B reads
-        // the accumulator again (cheap: TMEM) and finishes.  Unsplit, every tile paid one exposed global round trip with all
-        // sixteen drain warps waiting on it together (ncu source page: 60 % long-scoreboard in the drain, ~1.6 us per tile).
+        // the accumulator again (cheap: shared memory) and finishes.  Unsplit, every tile paid one exposed global round trip with all
+        // sixteen drain warps waiting on it together.
         // Every drain warp polls acc_full itself: a common named barrier made fifteen warps wait for the slowest (23 % of all
         // samples); with the drain behind the transform the accumulator has usually been complete for a while.
         float4 pre[4];
@@ -443,17 +438,22 @@ __global__ void __launch_bounds__(TailPCfg<C, TR>::THREADS, 1) tail_tc_persist_k
             x = tx * TT_W + q * 32 + lane; y = ty * TR + dr;
         };
         auto load_acc = [&](int a, float (&o)[TAIL_CO_PAD]) {
-            uint32_t acc[16];
-            tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * Cfg::ACC_COLS + dr * TT_N), acc);
+            const float* srow = slots + a * Cfg::SLOT_FLOATS + dr * (TT_W * TT_N);
+            const int px = q * 32 + lane;
+            float acc[16];
 #pragma unroll
-            for (int j = 0; j < TAIL_CO_PAD; ++j) o[j] = fmaf(__uint_as_float(acc[j]), p.acc_scale, sbias[j]);
+            for (int j = 0; j < 4; ++j) {
+                const float4 v = *reinterpret_cast<const float4*>(srow + tp_slot_off(px, 4 * j));
+                acc[4 * j] = v.x; acc[4 * j + 1] = v.y; acc[4 * j + 2] = v.z; acc[4 * j + 3] = v.w;
+            }
+#pragma unroll
+            for (int j = 0; j < TAIL_CO_PAD; ++j) o[j] = fmaf(acc[j], p.acc_scale, sbias[j]);
         };
         auto drain_issue = [&](int i) {
             const int a = i & 1;
             int n, x, y;
             tile_xy(i, n, x, y);
             mbar_wait(smem_u32(acc_full + a), (i >> 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
             have_pre = false;
             if (KIND != TAIL_DECOMPOSER && p.g0 != nullptr) {           // warp-uniform
                 float o[TAIL_CO_PAD];
@@ -467,8 +467,7 @@ __global__ void __launch_bounds__(TailPCfg<C, TR>::THREADS, 1) tail_tc_persist_k
             tile_xy(i, n, x, y);
             float o[TAIL_CO_PAD];
             load_acc(a, o);
-            asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-            if (lane == 0) mbar_arrive(smem_u32(acc_empty + a));                 // the accumulator slot may be overwritten
+            mbar_arrive(smem_u32(acc_empty + a));                                // this thread is done with the accumulator slot
             if (x < p.S)
                 tail_epilogue<KIND>(o, n, y, x, p.S, p.img0, p.img1, sbase, p.o[0], p.o[1], p.o[2], p.o[3], p.o[4], p.o[5], p.o[6], p.o[7],
                                     p.g0, p.g0_ld, p.g1, p.g1_ld, have_pre ? &pre : nullptr);
@@ -476,7 +475,7 @@ __global__ void __launch_bounds__(TailPCfg<C, TR>::THREADS, 1) tail_tc_persist_k
 
         // The transform runs TWO tiles ahead of the drain (the halo ring is three deep): the MMAs of tile i + 1 then have the
         // whole of drain(i) and transform(i + 2) to complete in.  One tile ahead, with the drain split around the transform,
-        // they had only the second half of drain(i): 31 % of all samples were drain warps polling acc_full (ncu, v5).
+        // they had only the second half of drain(i): 31 % of all samples were drain warps polling acc_full.
         transform(0);
         if (nt > 1) transform(1);
         for (int i = 0; i < nt; ++i) {
@@ -485,9 +484,6 @@ __global__ void __launch_bounds__(TailPCfg<C, TR>::THREADS, 1) tail_tc_persist_k
             drain_finish(i);
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" :: "r"(tmem_base), "r"(Cfg::TMEM_COLS) : "memory");
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -584,13 +580,6 @@ void launch_tail_tc(const TailWeights& tw, const View& f, const NormSpecTail& ns
 
 bool g_tail_persist = true;       // option "tail_persist": the persistent pipelined kernel (default) / one tile per CTA
 
-int tail_num_sms() {
-    static int sms[THA4_MAX_DEVICES] = {};
-    const int d = current_device();
-    if (!sms[d]) THA4_CUDA_CHECK(cudaDeviceGetAttribute(&sms[d], cudaDevAttrMultiProcessorCount, d));
-    return sms[d];
-}
-
 template <int KIND, int C, int TR>
 void launch_tail_persist(const TailWeights& tw, const View& f, const NormSpecTail& ns, const ImgView& i0, const ImgView& i1, float* const* o, int nout,
                          cudaStream_t s, const View* g0, const View* g1) {
@@ -611,7 +600,7 @@ void launch_tail_persist(const TailWeights& tw, const View& f, const NormSpecTai
     THA4_REQUIRE(f.H <= Cfg::MAX_S, "tail_tc: image size");
     THA4_ENSURE_SMEM((tail_tc_persist_kernel<KIND, C, TR>), Cfg::SMEM);
     const long total = (long)ceil_div(f.W, TT_W) * (f.H / TR) * f.N;
-    dim3 grid((unsigned)std::min<long>(total, tail_num_sms()));
+    dim3 grid((unsigned)std::min<long>(total, num_sms()));
     ProfScope prof(PROF_TAIL, s);
     {   // compulsory traffic as SURVEY 8d defines it (fp32 element size): feature map + image(s) read once, every returned tensor written once
         const int out_ch[4] = {15, 18, 24, 24};
@@ -629,9 +618,9 @@ void launch_tail_tc_c(const TailWeights& tw, const View& f, const NormSpecTail& 
         // tile rows per step (32-channel sites): 4 when that still gives every SM two tiles or more, else 2 (more, smaller tiles:
         // the small sites at B = 1 are one latency chain per CTA)
         const long tiles4 = (long)ceil_div(f.W, TT_W) * (f.H / 4) * f.N;
-        const bool tr4 = tiles4 >= 2L * tail_num_sms();
+        const bool tr4 = tiles4 >= 2L * num_sms();
         if (tw.C == 32) { if (tr4) launch_tail_persist<KIND, 32, 4>(tw, f, ns, i0, i1, o, nout, s, g0, g1); else launch_tail_persist<KIND, 32, 2>(tw, f, ns, i0, i1, o, nout, s, g0, g1); }
-        else            launch_tail_persist<KIND, 64, 2>(tw, f, ns, i0, i1, o, nout, s, g0, g1);        // three halo slots of 66 KB
+        else            launch_tail_persist<KIND, 64, 2>(tw, f, ns, i0, i1, o, nout, s, g0, g1);        // two halo slots of 66 KB
         return;
     }
     if (tw.C == 32) launch_tail_tc<KIND, 32>(tw, f, ns, i0, i1, o, nout, s);
@@ -662,6 +651,7 @@ void tail_make_half(TailWeights& tw, cudaStream_t s) {
     THA4_LAUNCH_CHECK();
     tw.w16 = h; tw.w16_scale = scale;
 }
+
 
 void tail_tc_enable_persist(bool on) { g_tail_persist = on; }
 

@@ -6,7 +6,7 @@
     (shion/core/training/distrib/distributed_training_states.py:184-187)  ->  Adam step (optimizer_factories.py:9-17).
 
 One process per GPU; the only collective is ONE all-reduce per step on the flat fp32 gradient buffer (331 567
-elements = 1.33 MB), issued through torch.distributed (NCCL over NVLink on B200, gloo in CPU tests of the host logic)."""
+elements = 1.33 MB), issued through torch.distributed (NCCL on GPUs, gloo in CPU tests of the host logic)."""
 from typing import Dict, List, Optional, Sequence
 
 import torch

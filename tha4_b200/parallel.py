@@ -22,7 +22,7 @@ def shard_range(total: int, rank: int, world: int) -> Tuple[int, int]:
 
 class ShardedPoseSweep:
     """Runs a batch of poses of ONE character image through a poser, each rank handling its contiguous shard
-    (BASELINE config 4: "pose-sweep batch=512 full-poser forward sharded across 8xB200")."""
+    (a 512-pose sweep sharded across the GPUs of one box)."""
 
     def __init__(self, poser: Poser, rank: Optional[int] = None, world: Optional[int] = None, chunk: int = 16):
         self.poser = poser

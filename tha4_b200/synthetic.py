@@ -8,12 +8,12 @@ otherwise a random-init teacher outputs zero warps and nothing downstream is exe
 
 Conditioning (round 2).  A plain He-init teacher is *chaotic* as a function of its conv operands: its heads paint
 full-amplitude white noise, the next network warps that noise, and a 1e-3 change of a warp offset moves the result
-by O(0.1) (profiles/r01_cpu_10bit_sensitivity.txt: rounding the conv operands of the CPU oracle to 10 mantissa bits
+by O(0.1) (scripts/dev/cpu_10bit_sensitivity.py: rounding the conv operands of the CPU oracle to 10 mantissa bits
 moved the face-morpher outputs by 4.9e-2 mean).  Trained weights do not behave like that: residual branches are
 small corrections, colour changes are small, alphas mostly keep the input image.  `_condition` gives the seeded
 weights that character (key-name based scaling of the head / residual / zero-init tensors), which makes the fp32
 oracle a usable yardstick for the tensor-core precision mode: the same 10-bit-operand emulation now moves every
-mode_07 output by <= 3e-4 mean / 1.4e-2 max (profiles/r02_cpu_10bit_sensitivity.txt), so the default-mode parity
+mode_07 output by <= 3e-4 mean / 1.4e-2 max (scripts/dev/cpu_10bit_sensitivity.py, on the CPU), so the default-mode parity
 tests can assert mean <= 2e-3, max <= 5e-2.
 """
 import math
