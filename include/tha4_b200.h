@@ -209,6 +209,28 @@ int tha4_test_attention(tha4_ctx* ctx, const float* qkv, int N, int C, int heads
 /* y[n][o] = b[o] + sum_i f(x[n][i]) W[o][i] */
 int tha4_test_linear(tha4_ctx* ctx, const float* x, int N, int I, const float* W, const float* b, int O, int silu_in,
                      float* y, void* stream);
+/* One level of a SIREN student on path 1 (wgmma) or 0 (mma.sync).  mode 0..2: body levels 0..2 (R = 128, 256, 512),
+ * 3: face (R = 128).  The layers come as a state_dict (described as for tha4_load_net) with the keys
+ * "layer.<i>.weight" [N_i, Cin_i] / "layer.<i>.bias" [N_i] for i < n_layers, and "head.weight" / "head.bias" if has_head;
+ * they are packed as the networks pack theirs.  Layer 0 is the level's first layer: its inputs are the previous level's
+ * channels (modes 1 / 2), then x, y and the pose_dim pose entries.  npad[i]: the padded width of layer i (the next layer's
+ * padded K); nb: the wgmma slice width of every GEMM layer in order, the head included (path 1; path 0 runs the production
+ * shapes only).  pose [B, pose_ld]; prev: fp16 NHWC [B, R/2, R/2, prev_c] (modes 1 / 2); image [B,4,512,512] (level 2 with
+ * a head).  outputs: without a head one fp16 NHWC tensor [B, R, R, npad[n_layers-1]]; level 2 with a head the five planes
+ * blended(4) alpha(1) color(4) warped(4) grid_change(2), fp32 or (out_f16) fp16; the face with a head [B,4,128,128] fp32. */
+int tha4_test_siren_level(tha4_ctx* ctx, int path, int mode, int n_tensors, const char* const* keys, const void* const* dev_ptrs,
+                          const int64_t* shapes, const int* ndims, int n_layers, int has_head, int pose_dim, const int* npad,
+                          const int* nb, const float* pose, int pose_ld, int B, const void* prev, int prev_c, const float* image,
+                          int out_f16, void* const* outputs, void* stream);
+/* y[i] = sin(x[i]) as the student kernels evaluate it: which 1 = the wgmma kernels' polynomial, 0 = the mma.sync kernels'
+ * range reduction + __sinf */
+int tha4_test_sine(tha4_ctx* ctx, int which, const float* x, int64_t n, float* y, void* stream);
+/* Host only, launches nothing: checks a wgmma student plan (per layer: padded K, padded N, slice width, sine 1 / head 0,
+ * first-layer terms 0 / 1) for level `mode` with resolution R, elementwise first-layer width e_npad (modes 0 / 3), previous
+ * level channels prev_c (modes 1 / 2) and output channels out_c.  Returns 0 if the kernel can run it, else
+ * THA4_ERR_INVALID with the reason in msg (msg_len bytes, NUL-terminated). */
+int tha4_test_siren_plan_check(int mode, int n_layers, const int* kpad, const int* npad, const int* nb, const int* sine,
+                               const int* first, int R, int e_npad, int prev_c, int out_c, char* msg, int msg_len);
 
 #ifdef __cplusplus
 }

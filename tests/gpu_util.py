@@ -100,6 +100,64 @@ def linear(x, W, b, silu_in):
     return y.cpu()
 
 
+SIREN_R = {0: 128, 1: 256, 2: 512, 3: 128}
+
+
+def siren_level(path, mode, layers, pose, pose_dim, head=None, npad=None, nb=None, prev=None, image=None, out_f16=0):
+    """One student level (tha4_test_siren_level).  layers: [(W [N, Cin], b [N])] in the reference layout; pose [B, pose_ld]
+    of which the first pose_dim entries are the pose; prev: fp16 [B, R/2, R/2, prev_c].  npad defaults to N rounded up to
+    32, nb to 96 (or 64 / 16 where 96 does not fit).  Returns the activations [B, R, R, N] as fp16 (no head), the five
+    tail planes (level 2) or the face [B,4,R,R], on the CPU."""
+    from tha4_b200._lib import _ptr_array
+    c = ctx()
+    R = SIREN_R[mode]
+    B = pose.shape[0]
+    sd = {}
+    for i, (W, b) in enumerate(layers):
+        sd['layer.%d.weight' % i], sd['layer.%d.bias' % i] = dev(W.float()), dev(b.float())
+    if head is not None:
+        sd['head.weight'], sd['head.bias'] = dev(head[0].float()), dev(head[1].float())
+    keys = list(sd)
+    shapes = (ctypes.c_int64 * (4 * len(keys)))()
+    ndims = (ctypes.c_int * len(keys))()
+    for i, k in enumerate(keys):
+        ndims[i] = sd[k].dim()
+        for d in range(4):
+            shapes[4 * i + d] = sd[k].shape[d] if d < sd[k].dim() else 1
+    npad = list(npad) if npad is not None else [(W.shape[0] + 31) // 32 * 32 for W, _ in layers]
+    n_gemm = len(layers) - (1 if mode in (0, 3) else 0) + (1 if head is not None else 0)
+    if nb is None:
+        gemm_npad = npad[1:] if mode in (0, 3) else npad
+        nb = [next(w for w in (96, 64, 16) if n % w == 0 and not (mode == 3 and w == 96)) for n in gemm_npad] + ([16] if head is not None else [])
+    assert len(nb) == n_gemm, (nb, n_gemm)
+    pd, prevd = dev(pose.float()), (dev(prev.half()) if prev is not None else None)
+    imaged = dev(image.float()) if image is not None else None
+    if head is None:
+        outs = [torch.empty(B, R, R, npad[-1], dtype=torch.float16, device='cuda:0')]
+    elif mode == 3:
+        outs = [torch.empty(B, 4, R, R, device='cuda:0')]
+    else:
+        dt = torch.float16 if out_f16 else torch.float32
+        outs = [torch.empty(B, ch, R, R, dtype=dt, device='cuda:0') for ch in (4, 1, 4, 4, 2)]
+    c._call('tha4_test_siren_level', path, mode, len(keys), (ctypes.c_char_p * len(keys))(*[k.encode() for k in keys]),
+            _ptr_array([sd[k] for k in keys]), shapes, ndims, len(layers), int(head is not None), pose_dim,
+            (ctypes.c_int * len(npad))(*npad), (ctypes.c_int * len(nb))(*nb), _ptr(pd), pose.shape[1], B, _ptr(prevd),
+            prev.shape[3] if prev is not None else 0, _ptr(imaged), out_f16, _ptr_array(outs), c._stream())
+    torch.cuda.synchronize()
+    if head is None:
+        return outs[0][..., :layers[-1][0].shape[0]].cpu()
+    return outs[0].cpu() if mode == 3 else [o.cpu() for o in outs]
+
+
+def sine(which, x):
+    c = ctx()
+    xd = dev(x.float())
+    y = torch.empty_like(xd)
+    c._call('tha4_test_sine', which, _ptr(xd), ctypes.c_int64(xd.numel()), _ptr(y), c._stream())
+    torch.cuda.synchronize()
+    return y.cpu()
+
+
 def grid_sample(img, gc, want_taps=True):
     c = ctx()
     N, C, H, W = img.shape

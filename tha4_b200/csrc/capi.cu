@@ -816,4 +816,49 @@ int tha4_test_linear(tha4_ctx* ctx, const float* x, int N, int I, const float* W
     return guarded(ctx, [&] { linear_forward(x, I, N, I, W, b, O, silu_in, y, O, (cudaStream_t)stream); });
 }
 
+int tha4_test_siren_level(tha4_ctx* ctx, int path, int mode, int n_tensors, const char* const* keys, const void* const* dev_ptrs,
+                          const int64_t* shapes, const int* ndims, int n_layers, int has_head, int pose_dim, const int* npad,
+                          const int* nb, const float* pose, int pose_ld, int B, const void* prev, int prev_c, const float* image,
+                          int out_f16, void* const* outputs, void* stream) {
+    return guarded(ctx, [&] {
+        THA4_REQUIRE(path == 0 || path == 1, "siren level: path must be 0 (mma.sync) or 1 (wgmma)");
+        begin_pass(ctx, (cudaStream_t)stream);
+        Runtime rt = make_rt(ctx, stream);
+        const StateDict sd = make_sd(n_tensors, keys, dev_ptrs, shapes, ndims);
+        siren_test_level(rt, path == 1, mode, sd, n_layers, has_head != 0, pose_dim, npad, nb, pose, pose_ld, B,
+                         (const __half*)prev, prev_c, image, out_f16 != 0, outputs);
+    });
+}
+
+int tha4_test_sine(tha4_ctx* ctx, int which, const float* x, int64_t n, float* y, void* stream) {
+    return guarded(ctx, [&] {
+        THA4_REQUIRE(which == 0 || which == 1, "sine: which must be 0 (siren_sin) or 1 (st_sin)");
+        if (which == 1) siren_tc_sine(x, (long)n, y, (cudaStream_t)stream);
+        else siren_sine(x, (long)n, y, (cudaStream_t)stream);
+    });
+}
+
+int tha4_test_siren_plan_check(int mode, int n_layers, const int* kpad, const int* npad, const int* nb, const int* sine,
+                               const int* first, int R, int e_npad, int prev_c, int out_c, char* msg, int msg_len) {
+    std::string err;
+    if (n_layers < 0 || n_layers > 8 || (n_layers > 0 && (!kpad || !npad || !nb || !sine || !first))) {
+        err = "layer count " + std::to_string(n_layers) + " is not 1..8";
+    } else {
+        SirenTcPlan plan;
+        plan.nl = n_layers;
+        for (int l = 0; l < n_layers; ++l) {
+            plan.kpad[l] = kpad[l]; plan.npad[l] = npad[l]; plan.nb[l] = nb[l]; plan.sine[l] = sine[l]; plan.first[l] = first[l];
+            plan.rows[l] = npad[l]; plan.W[l] = nullptr; plan.bias[l] = nullptr;
+        }
+        SirenTcLevel lv;
+        lv.R = R; lv.e_npad = e_npad; lv.prev_c = prev_c; lv.out_c = out_c;
+        err = siren_tc_plan_error(mode, plan, lv);
+    }
+    if (msg && msg_len > 0) {
+        std::strncpy(msg, err.c_str(), (size_t)msg_len - 1);
+        msg[msg_len - 1] = '\0';
+    }
+    return err.empty() ? THA4_OK : THA4_ERR_INVALID;
+}
+
 }  // extern "C"

@@ -29,6 +29,10 @@ __device__ __forceinline__ float siren_sin(float x) {
     return __sinf(r);
 }
 
+__global__ void siren_sin_kernel(const float* __restrict__ x, long n, float* __restrict__ y) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) y[i] = siren_sin(x[i]);
+}
+
 __device__ __forceinline__ void cp_async16h(void* smem_dst, const void* gmem_src) {
     unsigned sa = (unsigned)__cvta_generic_to_shared(smem_dst);
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" :: "r"(sa), "l"(gmem_src));
@@ -475,6 +479,117 @@ template <typename K> static void set_smem(K kernel, size_t bytes) {
     THA4_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
 }
 
+void siren_sine(const float* x, long n, float* y, cudaStream_t s) {
+    siren_sin_kernel<<<(int)std::min<long>(ceil_div(n, 256), 1024), 256, 0, s>>>(x, n, y);
+    THA4_LAUNCH_CHECK();
+}
+
+// ------------------------------------------------------------------------------------------------ one level
+void siren_level(Runtime& rt, const SirenLevelArgs& a) {
+    THA4_REQUIRE(a.mode >= 0 && a.mode <= 3 && a.nl >= 1 && a.L != nullptr, "siren level: mode / layers");
+    const SirenLayer* L = a.L;
+    const bool elementwise = (a.mode == 0 || a.mode == 3);
+    if (a.tc) {       // TMA + wgmma path (siren_tc.cu): one persistent kernel per level
+        SirenTcPlan plan;
+        int j = 0;
+        for (int i = elementwise ? 1 : 0; i < a.nl; ++i, ++j) plan.add(L[i], a.nb[j], 1, (!elementwise && i == 0) ? 1 : 0);
+        if (a.head) plan.add(*a.head, a.nb[j], 0, 0);
+        SirenTcLevel lv;
+        lv.R = a.R; lv.B = a.B;
+        if (elementwise) { lv.e_npad = L[0].NPAD; lv.e_pb = a.pb; lv.e_pb_ld = L[0].NPAD; lv.e_wxy = L[0].wxy; }
+        else { lv.f_pb = a.pb; lv.f_pb_ld = L[0].NPAD; lv.f_wxy = L[0].wxy; lv.prev = a.prev; lv.prev_c = a.prev_c; }
+        lv.out = a.out; lv.out_c = L[a.nl - 1].NPAD;
+        lv.image = a.image;
+        if (a.outputs) for (int i = 0; i < 5; ++i) lv.o[i] = a.outputs[i];
+        lv.o_f16 = a.out_f16;
+        lv.face_out = a.face_out;
+        lv.head_bias = a.head ? a.head->bias : nullptr;
+        siren_tc_run(rt, a.mode, plan, lv);
+        return;
+    }
+    // mma.sync path: one kernel per level, compiled for the production layer shapes only
+    THA4_REQUIRE(!a.out_f16, "siren body: f16 outputs need the tensor-core path (option siren_tc)");
+    auto shape = [&](int i, int kpad, int npad) { return a.L[i].KPAD == kpad && a.L[i].NPAD == npad; };
+    static const int kR[4] = {128, 256, 512, 128};
+    THA4_REQUIRE(a.R == kR[a.mode], "siren level (mma.sync): resolution of mode " + std::to_string(a.mode));
+    const int B = a.B, R = a.R;
+    cudaStream_t s = rt.stream;
+    ProfScope prof(PROF_SIREN, s);
+    if (a.mode == 0) {
+        THA4_REQUIRE(a.nl == 3 && !a.head && L[0].NPAD == 384 && shape(1, 384, 384) && shape(2, 384, 192) && a.out,
+                     "siren level 0 (mma.sync): production shapes only");
+        using SM0 = Smem<384, 384, 2>;
+        THA4_ENSURE_SMEM(siren_body_l0_kernel, SM0::bytes);
+        siren_body_l0_kernel<<<B * R * (R / TP), NTHREADS, SM0::bytes, s>>>(lw(L[0], a.pb), lw(L[1]), lw(L[2]), L[0].NPAD,
+                                                                          base_grid_table(R), R, a.out);
+    } else if (a.mode == 1) {
+        THA4_REQUIRE(a.nl == 3 && !a.head && shape(0, 192, 192) && shape(1, 192, 192) && shape(2, 192, 96) && a.prev_c == 192 && a.out,
+                     "siren level 1 (mma.sync): production shapes only");
+        using SM1 = Smem<192, 192, 3>;
+        THA4_ENSURE_SMEM(siren_body_l1_kernel, SM1::bytes);
+        siren_body_l1_kernel<<<B * R * (R / TP), NTHREADS, SM1::bytes, s>>>(lw(L[0], a.pb), lw(L[1]), lw(L[2]), L[0].NPAD,
+                                                                          base_grid_table(R), R, a.prev, a.out);
+    } else if (a.mode == 2) {
+        THA4_REQUIRE(a.nl == 3 && a.head && a.head->KPAD == 96 && a.head->NPAD == 8 && shape(0, 96, 96) && shape(1, 96, 96) &&
+                     shape(2, 96, 96) && a.prev_c == 96 && a.outputs, "siren level 2 (mma.sync): production shapes only");
+        using SM2 = Smem<96, 96, 3>;
+        THA4_ENSURE_SMEM(siren_body_l2_kernel, SM2::bytes);
+        siren_body_l2_kernel<<<B * R * (R / TP), NTHREADS, SM2::bytes, s>>>(lw(L[0], a.pb), lw(L[1]), lw(L[2]), lw(*a.head), L[0].NPAD,
+                                                                          base_grid_table(R), R, a.prev, a.image, a.outputs[0],
+                                                                          a.outputs[1], a.outputs[2], a.outputs[3], a.outputs[4]);
+    } else {
+        bool ok = a.nl == 8 && a.head && a.head->KPAD == 128 && a.head->NPAD == 8 && L[0].NPAD == 128 && a.face_out;
+        for (int i = 1; ok && i < 8; ++i) ok = shape(i, 128, 128);
+        THA4_REQUIRE(ok, "siren face (mma.sync): production shapes only");
+        FaceLayers FL;
+        FL.l[0] = lw(L[0], a.pb);
+        for (int i = 1; i < 8; ++i) FL.l[i] = lw(L[i]);
+        FL.head = lw(*a.head);
+        using SM = Smem<128, 128, 3>;
+        THA4_ENSURE_SMEM(siren_face_kernel, SM::bytes);
+        siren_face_kernel<<<B * R * (R / TP), NTHREADS, SM::bytes, s>>>(FL, L[0].NPAD, base_grid_table(R), R, a.face_out);
+    }
+    THA4_LAUNCH_CHECK();
+}
+
+void siren_test_level(Runtime& rt, bool tc, int mode, const StateDict& sd, int n_layers, bool has_head, int pose_dim,
+                      const int* npad, const int* nb, const float* pose, int pose_ld, int B, const __half* prev, int prev_c,
+                      const float* image, bool out_f16, void* const* outputs) {
+    THA4_REQUIRE(mode >= 0 && mode <= 3, "siren level: mode must be 0..3");
+    THA4_REQUIRE(n_layers >= 1 && n_layers <= 8 && pose_dim >= 1 && pose_ld >= pose_dim && B >= 1, "siren level: arguments");
+    static const int kR[4] = {128, 256, 512, 128};
+    const bool elementwise = (mode == 0 || mode == 3);
+    THA4_REQUIRE(elementwise ? n_layers >= (has_head ? 1 : 2) : (prev != nullptr && prev_c > 0), "siren level: layers / previous level");
+    cudaStream_t s = rt.stream;
+    AllocSink sink;                        // frees the packed layers on return
+    SirenLayer L[8], head;
+    {
+        SinkScope own(&sink);
+        for (int i = 0; i < n_layers; ++i) {
+            const std::string key = "layer." + std::to_string(i);
+            const int cin = (int)get(sd, key + ".weight").shape[1];
+            if (i == 0) L[0].load(sd, key, cin - 2 - pose_dim, pose_dim, elementwise ? 16 : prev_c, npad[0], 30.0f, s);
+            else L[i].load(sd, key, cin, 0, npad[i - 1], npad[i], 30.0f, s);
+        }
+        if (has_head) head.load(sd, "head", (int)get(sd, "head.weight").shape[1], 0, npad[n_layers - 1], 8, 1.0f, s);
+    }
+    SirenLevelArgs a;
+    a.tc = tc; a.mode = mode; a.R = kR[mode]; a.B = B;
+    a.L = L; a.nl = n_layers; a.head = has_head ? &head : nullptr; a.nb = nb;
+    a.pb = pose_bias(rt, L[0], pose, pose_ld, B);
+    a.prev = prev; a.prev_c = prev_c;
+    if (!has_head) a.out = reinterpret_cast<__half*>(outputs[0]);
+    else if (mode == 3) a.face_out = reinterpret_cast<float*>(outputs[0]);
+    else {
+        THA4_REQUIRE(mode == 2 && image != nullptr, "siren level: a head needs level 2 (with the image) or the face");
+        a.image = make_img(image, B, 4, 512, 512);
+        a.outputs = reinterpret_cast<float* const*>(outputs);
+        a.out_f16 = out_f16;
+    }
+    siren_level(rt, a);
+    THA4_CUDA_CHECK(cudaStreamSynchronize(s));
+}
+
 // ------------------------------------------------------------------------------------------------ SirenFaceNet
 void SirenFaceNet::load(const StateDict& sd, cudaStream_t s) {
     SinkScope own(&owned_);
@@ -488,26 +603,13 @@ void SirenFaceNet::load(const StateDict& sd, cudaStream_t s) {
 void SirenFaceNet::forward(Runtime& rt, const float* pose, int pose_ld, int B, float* out) {
     THA4_REQUIRE(loaded_, "network weights not loaded");
     const int R = 128;
-    float* pb = pose_bias(rt, layers_[0], pose, pose_ld, B);
-    if (siren_tc_enabled()) {       // TMA + wgmma path (siren_tc.cu)
-        SirenTcPlan plan;
-        for (int i = 1; i < 8; ++i) plan.add(layers_[i], 64, 1, 0);
-        plan.add(head_, 16, 0, 0);
-        SirenTcLevel lv;
-        lv.R = R; lv.B = B; lv.e_npad = layers_[0].NPAD; lv.e_pb = pb; lv.e_pb_ld = layers_[0].NPAD; lv.e_wxy = layers_[0].wxy;
-        lv.face_out = out; lv.head_bias = head_.bias;
-        siren_tc_run(rt, 3, plan, lv);
-        return;
-    }
-    FaceLayers L;
-    L.l[0] = lw(layers_[0], pb);
-    for (int i = 1; i < 8; ++i) L.l[i] = lw(layers_[i]);
-    L.head = lw(head_);
-    using SM = Smem<128, 128, 3>;
-    THA4_ENSURE_SMEM(siren_face_kernel, SM::bytes);
-    ProfScope prof(PROF_SIREN, rt.stream);
-    siren_face_kernel<<<B * R * (R / TP), NTHREADS, SM::bytes, rt.stream>>>(L, layers_[0].NPAD, base_grid_table(R), R, out);
-    THA4_LAUNCH_CHECK();
+    static const int nb[8] = {64, 64, 64, 64, 64, 64, 64, 16};
+    SirenLevelArgs a;
+    a.tc = siren_tc_enabled(); a.mode = 3; a.R = R; a.B = B;
+    a.L = layers_; a.nl = 8; a.head = &head_; a.nb = nb;
+    a.pb = pose_bias(rt, layers_[0], pose, pose_ld, B);
+    a.face_out = out;
+    siren_level(rt, a);
 }
 
 // ------------------------------------------------------------------------------------------------ SirenBodyNet
@@ -532,59 +634,22 @@ void SirenBodyNet::forward(Runtime& rt, const ImgView& image, const float* pose,
     THA4_REQUIRE(loaded_, "network weights not loaded");
     THA4_REQUIRE(image.H == 512 && image.W == 512 && image.C == 4, "siren body: image size");
     const int B = image.N;
-    cudaStream_t s = rt.stream;
-    float* pb0 = pose_bias(rt, l_[0][0], pose, pose_ld, B);
-    float* pb1 = pose_bias(rt, l_[1][0], pose, pose_ld, B);
-    float* pb2 = pose_bias(rt, l_[2][0], pose, pose_ld, B);
+    const float* pb[3];
+    for (int i = 0; i < 3; ++i) pb[i] = pose_bias(rt, l_[i][0], pose, pose_ld, B);
     __half* f0 = reinterpret_cast<__half*>(rt.persist->alloc((size_t)B * 128 * 128 * 192 / 2));
     __half* f1 = reinterpret_cast<__half*>(rt.persist->alloc((size_t)B * 256 * 256 * 96 / 2));
-    if (siren_tc_enabled()) {       // TMA + wgmma path (siren_tc.cu): one persistent kernel per level
-        {
-            SirenTcPlan plan;
-            plan.add(l_[0][1], 96, 1, 0); plan.add(l_[0][2], 96, 1, 0);
-            SirenTcLevel lv;
-            lv.R = 128; lv.B = B; lv.e_npad = 384; lv.e_pb = pb0; lv.e_pb_ld = 384; lv.e_wxy = l_[0][0].wxy;
-            lv.out = f0; lv.out_c = 192;
-            siren_tc_run(rt, 0, plan, lv);
-        }
-        {
-            SirenTcPlan plan;
-            plan.add(l_[1][0], 96, 1, 1); plan.add(l_[1][1], 96, 1, 0); plan.add(l_[1][2], 96, 1, 0);
-            SirenTcLevel lv;
-            lv.R = 256; lv.B = B; lv.f_pb = pb1; lv.f_pb_ld = 192; lv.f_wxy = l_[1][0].wxy;
-            lv.prev = f0; lv.prev_c = 192; lv.out = f1; lv.out_c = 96;
-            siren_tc_run(rt, 1, plan, lv);
-        }
-        {
-            SirenTcPlan plan;
-            plan.add(l_[2][0], 96, 1, 1); plan.add(l_[2][1], 96, 1, 0); plan.add(l_[2][2], 96, 1, 0); plan.add(head_, 16, 0, 0);
-            SirenTcLevel lv;
-            lv.R = 512; lv.B = B; lv.f_pb = pb2; lv.f_pb_ld = 96; lv.f_wxy = l_[2][0].wxy;
-            lv.prev = f1; lv.prev_c = 96; lv.image = image; lv.head_bias = head_.bias;
-            for (int i = 0; i < 5; ++i) lv.o[i] = outputs[i];
-            lv.o_f16 = outputs_f16;
-            siren_tc_run(rt, 2, plan, lv);
-        }
-        return;
+    const bool tc = siren_tc_enabled();
+    THA4_REQUIRE(tc || !outputs_f16, "siren body: f16 outputs need the tensor-core path (option siren_tc)");
+    static const int nb[4] = {96, 96, 96, 16};      // wgmma slice widths of the GEMM layers (level 2: + the head)
+    for (int i = 0; i < 3; ++i) {
+        SirenLevelArgs a;
+        a.tc = tc; a.mode = i; a.R = 128 << i; a.B = B;
+        a.L = l_[i]; a.nl = 3; a.nb = nb; a.pb = pb[i];
+        if (i > 0) { a.prev = i == 1 ? f0 : f1; a.prev_c = i == 1 ? 192 : 96; }
+        if (i < 2) a.out = i == 0 ? f0 : f1;
+        else { a.head = &head_; a.image = image; a.outputs = outputs; a.out_f16 = outputs_f16; }
+        siren_level(rt, a);
     }
-    THA4_REQUIRE(!outputs_f16, "siren body: f16 outputs need the tensor-core path (option siren_tc)");
-    using SM0 = Smem<384, 384, 2>;
-    using SM1 = Smem<192, 192, 3>;
-    using SM2 = Smem<96, 96, 3>;
-    THA4_ENSURE_SMEM(siren_body_l0_kernel, SM0::bytes);
-    THA4_ENSURE_SMEM(siren_body_l1_kernel, SM1::bytes);
-    THA4_ENSURE_SMEM(siren_body_l2_kernel, SM2::bytes);
-    ProfScope prof(PROF_SIREN, s);
-    siren_body_l0_kernel<<<B * 128 * (128 / TP), NTHREADS, SM0::bytes, s>>>(lw(l_[0][0], pb0), lw(l_[0][1]), lw(l_[0][2]), 384,
-                                                                          base_grid_table(128), 128, f0);
-    THA4_LAUNCH_CHECK();
-    siren_body_l1_kernel<<<B * 256 * (256 / TP), NTHREADS, SM1::bytes, s>>>(lw(l_[1][0], pb1), lw(l_[1][1]), lw(l_[1][2]), 192,
-                                                                          base_grid_table(256), 256, f0, f1);
-    THA4_LAUNCH_CHECK();
-    siren_body_l2_kernel<<<B * 512 * (512 / TP), NTHREADS, SM2::bytes, s>>>(lw(l_[2][0], pb2), lw(l_[2][1]), lw(l_[2][2]), lw(head_), 96,
-                                                                          base_grid_table(512), 512, f1, image, outputs[0],
-                                                                          outputs[1], outputs[2], outputs[3], outputs[4]);
-    THA4_LAUNCH_CHECK();
 }
 
 }  // namespace tha4

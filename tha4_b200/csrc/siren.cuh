@@ -29,8 +29,36 @@ struct SirenTcLevel {
     float* face_out = nullptr; const float* head_bias = nullptr;
 };
 void siren_tc_run(Runtime& rt, int mode, const SirenTcPlan& plan, const SirenTcLevel& lv);   // mode 0..2: body levels, 3: face
+// Checks a plan against the kernel of `mode` (host only, launches nothing): "" if it fits, else what does not.  The
+// kernel has no bounds checks of its own: K, N and the level's channel counts must fit its two operand buffers, its
+// weight tiles and its first-layer staging area, or it reads and writes past them.  siren_tc_run calls it per launch.
+std::string siren_tc_plan_error(int mode, const SirenTcPlan& plan, const SirenTcLevel& lv);
 void siren_tc_enable(bool on);
 bool siren_tc_enabled();
+void siren_tc_sine(const float* x, long n, float* y, cudaStream_t s);     // y = st_sin(x) of the wgmma kernels
+void siren_sine(const float* x, long n, float* y, cudaStream_t s);        // y = siren_sin(x) of the mma.sync kernels
+
+// One level of a student network (mode 0..2: body levels 0..2, 3: face) on the wgmma path (tc) or the mma.sync path.
+// L[0] is the level's first layer: its xy + pose columns enter through pb, the per-sample bias [B][L[0].NPAD], and
+// L[0].wxy.  Modes 0 / 3 evaluate it elementwise; modes 1 / 2 run it as a GEMM on the bilinear x2 of `prev`.
+// nb: the wgmma slice width of every GEMM layer in order, the head included.  Output: `out` [B,R,R,L[nl-1].NPAD] fp16
+// NHWC without a head; the five tail planes (mode 2) or face_out [B,4,R,R] (mode 3) with one.
+struct SirenLevelArgs {
+    bool tc = true;
+    int mode = 0, R = 0, B = 0;
+    const SirenLayer* L = nullptr; int nl = 0; const SirenLayer* head = nullptr;
+    const int* nb = nullptr;
+    const float* pb = nullptr;
+    const __half* prev = nullptr; int prev_c = 0;
+    __half* out = nullptr;
+    ImgView image; float* const* outputs = nullptr; bool out_f16 = false;
+    float* face_out = nullptr;
+};
+void siren_level(Runtime& rt, const SirenLevelArgs& a);
+// Kernel-level test entry: loads the layers "layer.<i>" (and "head") of `sd` as the networks do and runs one level.
+void siren_test_level(Runtime& rt, bool tc, int mode, const StateDict& sd, int n_layers, bool has_head, int pose_dim,
+                      const int* npad, const int* nb, const float* pose, int pose_ld, int B, const __half* prev, int prev_c,
+                      const float* image, bool out_f16, void* const* outputs);
 
 class SirenFaceNet {
 public:

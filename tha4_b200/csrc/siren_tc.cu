@@ -389,7 +389,67 @@ void launch_siren_tc(const StMaps& maps, const StParams& p, int ctas_per_sm, cud
 
 bool g_siren_tc = true;
 
+// per mode: the operand buffers' 64-column chunks (ACH) and the widest weight tile (NBMAX) of the launches in siren_tc_run
+constexpr int kStAch[4] = {6, 3, 2, 2};
+constexpr int kStNbMax[4] = {96, 96, 96, 64};
+constexpr int ST_FIRST_MAX = 384;          // sfirst: per-sample bias + xy weights of up to 384 first-layer columns
+
+__global__ void st_sin_kernel(const float* __restrict__ x, long n, float* __restrict__ y) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) y[i] = st_sin(x[i]);
+}
+
 }  // namespace
+
+void siren_tc_sine(const float* x, long n, float* y, cudaStream_t s) {
+    st_sin_kernel<<<(int)std::min<long>(ceil_div(n, 256), 1024), 256, 0, s>>>(x, n, y);
+    THA4_LAUNCH_CHECK();
+}
+
+std::string siren_tc_plan_error(int mode, const SirenTcPlan& plan, const SirenTcLevel& lv) {
+    if (mode < 0 || mode > 3) return "mode " + std::to_string(mode) + " is not 0..3";
+    const int ach = kStAch[mode], nbmax = kStNbMax[mode], width = ach * 64;
+    const bool elementwise = (mode == SM_BODY0 || mode == SM_FACE);
+    const std::string at = " (mode " + std::to_string(mode) + ")";
+    if (plan.nl < 1 || plan.nl > ST_MAXL) return "layer count " + std::to_string(plan.nl) + " is not 1.." + std::to_string(ST_MAXL) + at;
+    if (lv.R <= 0 || lv.R % ST_TILE != 0) return "R = " + std::to_string(lv.R) + " is not a multiple of 128" + at;
+    int produced;                          // columns of the operand the current layer reads that its producer wrote
+    if (elementwise) {
+        if (lv.e_npad <= 0 || lv.e_npad % 8 != 0) return "first-layer width e_npad = " + std::to_string(lv.e_npad) + " is not a positive multiple of 8" + at;
+        if (lv.e_npad > ST_FIRST_MAX) return "first-layer width e_npad = " + std::to_string(lv.e_npad) + " > 384" + at;
+        if (lv.e_npad > width) return "first-layer width e_npad = " + std::to_string(lv.e_npad) + " > the operand buffer (" + std::to_string(width) + ")" + at;
+        produced = lv.e_npad;
+    } else {
+        if (lv.prev_c <= 0 || lv.prev_c % 8 != 0) return "prev_c = " + std::to_string(lv.prev_c) + " is not a positive multiple of 8" + at;
+        if (lv.prev_c > width) return "prev_c = " + std::to_string(lv.prev_c) + " > the operand buffer (" + std::to_string(width) + ")" + at;
+        if (plan.npad[0] > ST_FIRST_MAX) return "first-layer width npad = " + std::to_string(plan.npad[0]) + " > 384" + at;
+        produced = lv.prev_c;
+    }
+    for (int l = 0; l < plan.nl; ++l) {
+        const std::string ly = "layer " + std::to_string(l) + ": ";
+        const int k = plan.kpad[l], n = plan.npad[l], nb = plan.nb[l];
+        const bool last = l == plan.nl - 1;
+        if (k <= 0 || k % 16 != 0) return ly + "kpad = " + std::to_string(k) + " is not a positive multiple of 16" + at;
+        if (k > width) return ly + "kpad = " + std::to_string(k) + " > the operand buffer (" + std::to_string(width) + ")" + at;
+        if (k > produced) return ly + "kpad = " + std::to_string(k) + " > the " + std::to_string(produced) + " columns its producer wrote" + at;
+        if (nb != 16 && nb != 64 && nb != 96) return ly + "slice width nb = " + std::to_string(nb) + " is not 16, 64 or 96" + at;
+        if (nb > nbmax) return ly + "slice width nb = " + std::to_string(nb) + " > NBMAX = " + std::to_string(nbmax) + at;
+        if (n <= 0 || n % nb != 0) return ly + "npad = " + std::to_string(n) + " is not a multiple of nb = " + std::to_string(nb) + at;
+        const bool want_first = !elementwise && l == 0;
+        if ((plan.first[l] != 0) != want_first)
+            return ly + (want_first ? "the first GEMM layer of levels 1 / 2 must take the first-layer terms" : "first-layer terms on a layer that is not the first GEMM layer of level 1 / 2") + at;
+        if (plan.sine[l]) {
+            if (n > width) return ly + "sine layer npad = " + std::to_string(n) + " > the operand buffer (" + std::to_string(width) + ")" + at;
+        } else {
+            if (!last) return ly + "the head must be the last layer" + at;
+            if (mode != SM_BODY2 && mode != SM_FACE) return ly + "a head on a level without one (modes 2 / 3 only)" + at;
+            if (n != 16 || nb != 16) return ly + "head npad = " + std::to_string(n) + ", nb = " + std::to_string(nb) + ": both must be 16" + at;
+        }
+        produced = n;
+    }
+    if (plan.sine[plan.nl - 1] && lv.out_c != plan.npad[plan.nl - 1])
+        return "out_c = " + std::to_string(lv.out_c) + " is not the last layer's npad = " + std::to_string(plan.npad[plan.nl - 1]) + at;
+    return "";
+}
 
 void siren_tc_enable(bool on) { g_siren_tc = on; }
 bool siren_tc_enabled() { return g_siren_tc; }
@@ -403,6 +463,8 @@ void SirenTcPlan::add(const SirenLayer& l, int nb, int sine, int first) {
 }
 
 void siren_tc_run(Runtime& rt, int mode, const SirenTcPlan& plan, const SirenTcLevel& lv) {
+    const std::string plan_err = siren_tc_plan_error(mode, plan, lv);
+    THA4_REQUIRE(plan_err.empty(), "siren_tc plan: " + plan_err);
     StParams p{};
     StMaps maps;
     p.R = lv.R; p.B = lv.B; p.nl = plan.nl;
@@ -431,10 +493,10 @@ void siren_tc_run(Runtime& rt, int mode, const SirenTcPlan& plan, const SirenTcL
     cudaStream_t s = rt.stream;
     ProfScope prof(PROF_SIREN, s);
     //                         A chunks, widest weight tile, ring
-    if (mode == SM_BODY0) launch_siren_tc<6, 96, 2, SM_BODY0>(maps, p, 1, s);          // two 96 KB operand buffers
-    else if (mode == SM_BODY1) launch_siren_tc<3, 96, 4, SM_BODY1>(maps, p, 1, s);
-    else if (mode == SM_BODY2) launch_siren_tc<2, 96, 2, SM_BODY2>(maps, p, 2, s);
-    else launch_siren_tc<2, 64, 2, SM_FACE>(maps, p, 2, s);
+    if (mode == SM_BODY0) launch_siren_tc<kStAch[0], kStNbMax[0], 2, SM_BODY0>(maps, p, 1, s);          // two 96 KB operand buffers
+    else if (mode == SM_BODY1) launch_siren_tc<kStAch[1], kStNbMax[1], 4, SM_BODY1>(maps, p, 1, s);
+    else if (mode == SM_BODY2) launch_siren_tc<kStAch[2], kStNbMax[2], 2, SM_BODY2>(maps, p, 2, s);
+    else launch_siren_tc<kStAch[3], kStNbMax[3], 2, SM_FACE>(maps, p, 2, s);
 }
 
 }  // namespace tha4
