@@ -57,6 +57,7 @@ const char* tha4_last_error(const tha4_ctx* ctx);
  *          "tcgen05" (1: convs on the wgmma/TMA kernels; 0: everything on mma.sync; the name is historical),
  *          "half_operands" (1: f16 conv operands, normalisations fused into the consumer conv's operand path),
  *          "halo_conv" (1: 3x3 stride-1 convs on the halo-reuse kernel), "tma_store" (1: unsplit conv epilogue through TMA stores),
+ *          "halo_m256" (-1: automatic; 0 / 1: force 128- / 256-pixel tiles on the unsplit launches of the halo kernel),
  *          "cluster_splitk" (1: K-split convs reduce through a thread-block cluster / DSMEM; 0: workspace + reduce kernel),
  *          "pdl" (1: programmatic dependent launch), "tc_stride2" (1: 4x4 stride-2 convs on the wgmma kernel),
  *          "small_bn" (1: narrower N tiles for small unsplit launches), "siren_tc" (1: students on the wgmma kernels; 0: mma.sync kernels),
@@ -191,6 +192,14 @@ int tha4_test_conv_norm(tha4_ctx* ctx, int kind, const float* x, int N, int Cin,
                         const float* gamma, const float* beta, const float* film0, const float* film1, int act,
                         const float* w, const float* bias, const float* res, int res_mode, int Cout, int ksplit,
                         float* y, float* y_from_f16, void* stream);
+/* same, and: norm_C = 0 convolves the raw input (no fused normalisation); y_stats (optional, device, [N,Cout,2] doubles): the
+ * per-(n, c) sum and sum of squares of the fp32 output that the conv accumulates for its consumer's normalisation;
+ * reps > 0: the conv is then launched `reps` more times between two CUDA events and *us_per_launch receives the mean
+ * device time per launch (microseconds). */
+int tha4_test_conv_norm_ex(tha4_ctx* ctx, int kind, const float* x, int N, int Cin, int H, int W, int norm_C, int groups,
+                           const float* gamma, const float* beta, const float* film0, const float* film1, int act,
+                           const float* w, const float* bias, const float* res, int res_mode, int Cout, int ksplit,
+                           float* y, float* y_from_f16, double* y_stats, int reps, float* us_per_launch, void* stream);
 /* y = act(norm(x)) with groups == 0: InstanceNorm2d, else GroupNorm(groups); act 0 none / 1 relu / 2 silu; pool 0/1;
  * film0 [2C] / film1 [N,2C] optional FiLM scale-shifts (unet.py:90-97); out_f16 = 1 runs the default-mode variant
  * (f16 output tensor, fast-math SiLU) and returns its values widened to fp32 */

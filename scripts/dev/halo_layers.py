@@ -1,0 +1,187 @@
+"""Developer measurement of the 3x3 halo convolution in the teacher_b1 frame (not a pytest file).
+
+1. The card's name and power limit.
+2. One warm teacher_b1 frame (mode_07, batch 1, eyebrow cache hot) under torch.profiler with CUDA activities, once with
+   128-pixel halo tiles forced (option halo_m256 = 0) and once with the automatic choice: device time per kernel
+   instantiation, and the share of the unsplit halo launches.
+3. Every unsplit halo conv shape of that frame (read from the library's launch log, THA4_HALO_DEBUG=2, in a child
+   process) timed alone with CUDA events over --reps launches after warm-up, with 128- and with 256-pixel tiles:
+   microseconds, TFLOP/s, and the compulsory HBM bytes computed from the shape (f16 input, f16 weights, the fp32 and f16
+   outputs, the fp32 residual).  The conv runs through the kernel-level test hook with the frame's input-normalisation
+   kind and residual; the hook always writes both outputs.
+
+Usage: python scripts/dev/halo_layers.py [--reps 200] [--out DIR]
+"""
+import argparse
+import collections
+import os
+import re
+import subprocess
+import sys
+
+import torch
+
+_ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, _ROOT)
+sys.path.insert(0, os.path.join(_ROOT, 'tests'))
+
+LAUNCH_RE = re.compile(r'halo launch: N (\d+) (\d+)x(\d+) cin (\d+) cout (\d+) \| bn (\d+) cs (\d+) wg (\d+) chunks (\d+) grid (\d+) x (\d+) \| '
+                       r'xf (\d+) groups (\d+) act (\d+) res (\d+) out32 (\d+) out16 (\d+) st_tma (\d+)')
+
+
+def card():
+    name = torch.cuda.get_device_name(0)
+    try:
+        q = subprocess.run(['nvidia-smi', '--query-gpu=power.limit,clocks.max.sm', '--format=csv,noheader'],
+                           capture_output=True, text=True, timeout=60).stdout.strip()
+    except (OSError, subprocess.SubprocessError) as e:
+        q = 'nvidia-smi unavailable (%s)' % e
+    return '%s | power limit, max SM clock: %s' % (name, q)
+
+
+def make_teacher():
+    import bench
+    from tha4_b200 import synthetic
+    from tha4_b200.poser.modes import mode_07
+    device = torch.device('cuda:0')
+    tsds, _ = bench.load_state_dicts('mode_07')
+    poser = mode_07.create_poser(device, state_dicts=tsds)
+    poser.get_modules()
+    poser.protocol.trust_image_identity = True
+    image = bench.load_image().to(device).unsqueeze(0).contiguous()
+    poses = synthetic.random_poses(8, seed=1234).to(device)
+    return poser, image, poses
+
+
+def frame_shapes():
+    """Runs two frames in a child process with the launch log on; returns the halo launches of the second (eyebrow cache
+    hot) frame as dicts, in frame order."""
+    code = ('import sys; sys.path.insert(0, %r); sys.path.insert(0, %r); import torch\n'
+            'from halo_layers import make_teacher\n'
+            'p, img, poses = make_teacher()\n'
+            'with torch.no_grad():\n'
+            '    p.get_posing_outputs(img, poses[0:1]); torch.cuda.synchronize()\n'
+            '    sys.stderr.write("SECOND FRAME\\n"); sys.stderr.flush()\n'
+            '    p.get_posing_outputs(img, poses[1:2]); torch.cuda.synchronize()\n') % (_ROOT, os.path.dirname(os.path.abspath(__file__)))
+    env = dict(os.environ, THA4_HALO_DEBUG='2')
+    r = subprocess.run([sys.executable, '-c', code], capture_output=True, text=True, env=env, cwd=_ROOT)
+    if r.returncode != 0:
+        raise RuntimeError('launch-log run failed:\n' + r.stderr[-4000:])
+    keys = ('N', 'H', 'W', 'cin', 'cout', 'bn', 'cs', 'wg', 'chunks', 'grid_m', 'grid_n', 'xf', 'groups', 'act', 'res', 'out32', 'out16', 'st_tma')
+    log = r.stderr.split('SECOND FRAME', 1)[1]
+    return [dict(zip(keys, map(int, m.groups()))) for m in LAUNCH_RE.finditer(log)]
+
+
+def profile_frame(poser, image, poses, m256, out_dir):
+    from torch.profiler import ProfilerActivity, profile
+    ctx = poser.get_context()
+    ctx.set_option('halo_m256', m256)
+    ctx.set_option('cuda_graphs', 0)          # one kernel record per launch
+    with torch.no_grad():
+        for i in range(3):
+            poser.get_posing_outputs(image, poses[i:i + 1])
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            poser.get_posing_outputs(image, poses[3:4])
+            torch.cuda.synchronize()
+    ctx.set_option('cuda_graphs', 1)
+    ctx.set_option('halo_m256', -1)
+    if out_dir:
+        prof.export_chrome_trace(os.path.join(out_dir, 'halo_layers_m256_%d.pt.trace.json' % m256))
+    per = collections.OrderedDict()
+    for ev in prof.events():
+        if ev.device_type.name != 'CUDA':
+            continue
+        t, n = per.get(ev.name, (0.0, 0))
+        per[ev.name] = (t + ev.time_range.elapsed_us(), n + 1)
+    return per
+
+
+def short(name):
+    name = name.replace('(anonymous namespace)::', '').replace('void ', '').replace('tha4::', '')
+    return re.sub(r'\(.*$', '', name)
+
+
+def halo_split(name):
+    """conv_halo_kernel<BN, SA, SB, CS, OP, XF, WG>: returns (CS, WG) or None."""
+    m = re.search(r'conv_halo_kernel<(\d+), (\d+), (\d+), (\d+), (\d+), (\d+), (\d+)>', name)
+    return (int(m.group(4)), int(m.group(7))) if m else None
+
+
+def print_frame(label, per):
+    total = sum(t for t, _ in per.values())
+    unsplit = sum(t for k, (t, _) in per.items() if halo_split(k) and halo_split(k)[0] == 1)
+    halo = sum(t for k, (t, _) in per.items() if halo_split(k))
+    print('\n== one warm teacher_b1 frame, %s: kernel time %.1f us; unsplit halo %.1f us (%.1f %%), all halo %.1f us (%.1f %%)'
+          % (label, total, unsplit, 100 * unsplit / total, halo, 100 * halo / total))
+    for k, (t, n) in sorted(per.items(), key=lambda kv: -kv[1][0]):
+        if t < 0.002 * total:
+            continue
+        print('  %9.1f us %5.1f %% %4d x  %s' % (t, 100 * t / total, n, short(k)))
+    return total, unsplit
+
+
+def shape_ab(shapes, reps):
+    import test_gpu_halo_m256 as H
+    c = __import__('gpu_util').ctx()
+    seen, rows = set(), []
+    for s in shapes:
+        if s['cs'] != 1:
+            continue
+        key = (s['N'], s['H'], s['W'], s['cin'], s['cout'], s['xf'], s['groups'], s['act'], s['res'])
+        if key in seen:
+            continue
+        seen.add(key)
+        count = sum(1 for t in shapes if t['cs'] == 1 and (t['N'], t['H'], t['W'], t['cin'], t['cout'], t['xf'], t['groups'], t['act'], t['res']) == key)
+        norm = None if not s['xf'] else ('gn' if s['groups'] else 'in')
+        inp = H.make_inputs(7, s['N'], s['cin'], s['H'], s['W'], s['cout'], norm, 1 if s['res'] == 1 else 0)
+        inp['act'] = s['act'] if s['xf'] else 0
+        us = {}
+        outs = {}
+        try:
+            for m in (0, 1):
+                c.set_option('halo_m256', m)
+                H.conv_norm_ex(**inp, reps=20)                        # warm-up
+                y, y16, st, us[m] = H.conv_norm_ex(**inp, reps=reps)
+                outs[m] = (y, y16)
+        except Exception as e:          # a shape the test hook cannot describe (e.g. Cin not a multiple of 8)
+            print('  skipped %s: %s' % (key, e), flush=True)
+            continue
+        finally:
+            c.set_option('halo_m256', -1)
+        same = torch.equal(outs[0][0], outs[1][0]) and torch.equal(outs[0][1], outs[1][1])
+        flop = 2.0 * s['N'] * s['H'] * s['W'] * s['cin'] * s['cout'] * 9
+        px = s['N'] * s['H'] * s['W']
+        hbm = px * s['cin'] * 2 + 9 * s['cin'] * s['cout'] * 2 + px * s['cout'] * (4 + 2) + (px * s['cout'] * 4 if s['res'] == 1 else 0)
+        rows.append((s, count, us, flop, hbm, same))
+    print('\n== unsplit halo shapes of the frame, alone: %d launches each after warm-up (CUDA events)' % reps)
+    print('  %-26s %3s %4s %6s | %9s %7s %6s | %9s %7s %6s | %6s %s' % ('N HxW cin->cout', 'n', 'bn', 'tiles', 'M128 us', 'TFLOP/s', 'GB/s',
+                                                                  'M256 us', 'TFLOP/s', 'GB/s', 'ratio', 'bit-identical'))
+    for s, count, us, flop, hbm, same in rows:
+        tiles = s['grid_m'] * s['grid_n'] * (2 if s['wg'] == 2 else 1)
+        print('  %-26s %3d %4d %6d | %9.2f %7.1f %6.0f | %9.2f %7.1f %6.0f | %6.3f %s' % (
+            '%d %dx%d %d->%d xf%d' % (s['N'], s['H'], s['W'], s['cin'], s['cout'], s['xf']), count, s['bn'], tiles,
+            us[0], flop / us[0] / 1e6, hbm / us[0] / 1e3, us[1], flop / us[1] / 1e6, hbm / us[1] / 1e3, us[0] / us[1], same))
+    return rows
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--reps', type=int, default=200)
+    ap.add_argument('--out', default=None, help='directory for the profiler traces')
+    args = ap.parse_args()
+    assert torch.cuda.is_available(), 'halo_layers.py needs a CUDA device'
+    if args.out:
+        os.makedirs(args.out, exist_ok=True)
+    print('card:', card(), flush=True)
+    shapes = frame_shapes()
+    print('halo launches in the frame: %d (%d unsplit)' % (len(shapes), sum(1 for s in shapes if s['cs'] == 1)), flush=True)
+    poser, image, poses = make_teacher()
+    before = print_frame('128-pixel tiles (halo_m256 = 0)', profile_frame(poser, image, poses, 0, args.out))
+    after = print_frame('automatic tile choice (halo_m256 = -1)', profile_frame(poser, image, poses, -1, args.out))
+    print('kernel time per frame: %.1f -> %.1f us (%.3fx)' % (before[0], after[0], before[0] / after[0]), flush=True)
+    shape_ab(shapes, args.reps)
+
+
+if __name__ == '__main__':
+    main()

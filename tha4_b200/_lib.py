@@ -27,7 +27,7 @@ EXPORTED_SYMBOLS = [
     'tha4_teacher_forward', 'tha4_student_forward', 'tha4_student_forward_io', 'tha4_siren_morpher_param_count', 'tha4_siren_morpher_train_step',
     'tha4_siren_face_morpher_param_count', 'tha4_siren_face_morpher_train_step',
     'tha4_adam_step', 'tha4_images_differ', 'tha4_frame_to_srgb8', 'tha4_rgba8_to_poser_image', 'tha4_grid_sample', 'tha4_resize_bilinear',
-    'tha4_base_grid', 'tha4_test_conv', 'tha4_test_conv_norm', 'tha4_test_norm', 'tha4_test_tail', 'tha4_test_attention', 'tha4_test_linear',
+    'tha4_base_grid', 'tha4_test_conv', 'tha4_test_conv_norm', 'tha4_test_conv_norm_ex', 'tha4_test_norm', 'tha4_test_tail', 'tha4_test_attention', 'tha4_test_linear',
     'tha4_test_siren_level', 'tha4_test_sine', 'tha4_test_siren_plan_check',
 ]
 

@@ -256,6 +256,7 @@ int tha4_set_option(tha4_ctx* ctx, const char* name, int64_t value) {
         else if (!strcmp(name, "cluster_splitk")) conv_tc_enable_cluster(value != 0);
         else if (!strcmp(name, "halo_conv")) conv_halo_enable(value != 0);
         else if (!strcmp(name, "tma_store")) conv_halo_enable_tma_store(value != 0);
+        else if (!strcmp(name, "halo_m256")) { THA4_REQUIRE(value >= -1 && value <= 1, "halo_m256: -1, 0 or 1"); conv_halo_set_m256((int)value); }
         else if (!strcmp(name, "siren_tc")) siren_tc_enable(value != 0);
         else if (!strcmp(name, "tc_stride2")) conv_tc_enable_stride2(value != 0);
         else if (!strcmp(name, "small_bn")) conv_tc_enable_small_bn(value != 0);
@@ -661,10 +662,10 @@ int tha4_test_conv(tha4_ctx* ctx, int kind, const float* x, const float* w, cons
     });
 }
 
-int tha4_test_conv_norm(tha4_ctx* ctx, int kind, const float* x, int N, int Cin, int H, int W, int norm_C, int groups,
-                        const float* gamma, const float* beta, const float* film0, const float* film1, int act,
-                        const float* w, const float* bias, const float* res, int res_mode, int Cout, int ksplit,
-                        float* y, float* y_from_f16, void* stream) {
+static int test_conv_norm(tha4_ctx* ctx, int kind, const float* x, int N, int Cin, int H, int W, int norm_C, int groups,
+                          const float* gamma, const float* beta, const float* film0, const float* film1, int act,
+                          const float* w, const float* bias, const float* res, int res_mode, int Cout, int ksplit,
+                          float* y, float* y_from_f16, double* y_stats, int reps, float* us_per_launch, void* stream) {
     return guarded(ctx, [&] {
         cudaStream_t s = (cudaStream_t)stream;
         begin_pass(ctx, s);
@@ -696,10 +697,14 @@ int tha4_test_conv_norm(tha4_ctx* ctx, int kind, const float* x, int N, int Cin,
         const bool x2 = (kind == CONVT_4x4_S2 || kind == CONV_UP2_3x3);
         const int Ho = (kind == CONV_4x4_S2) ? H / 2 : (x2 ? H * 2 : H), Wo = (kind == CONV_4x4_S2) ? W / 2 : (x2 ? W * 2 : W);
         View yo = mk(N, Ho, Wo, Cout);
-        View y16 = yo; y16.f16 = 1; y16.p = P->alloc(((size_t)N * Ho * Wo * Cout + 1) / 2);
+        if (y_stats) {        // per-(n, c) sum / sum of squares of the output, one replica
+            yo.stats = rt.alloc_stats((size_t)N * Cout * 2); yo.stats_ld = Cout; yo.stats_rep = 1; yo.stats_rep_stride = (long)N * Cout * 2;
+            THA4_CUDA_CHECK(cudaMemsetAsync(yo.stats, 0, (size_t)N * Cout * 2 * sizeof(double), s));
+        }
+        View y16 = yo; y16.f16 = 1; y16.stats = nullptr; y16.p = P->alloc(((size_t)N * Ho * Wo * Cout + 1) / 2);
         ConvArgs a;
         a.in = x16; a.out = yo; a.out16 = y16; a.ksplit = ksplit;
-        a.nin.on = true; a.nin.C = norm_C; a.nin.groups = groups; a.nin.act = act == ACT_SILU ? ACT_SILU_FAST : act;
+        a.nin.on = norm_C > 0; a.nin.C = norm_C; a.nin.groups = groups; a.nin.act = act == ACT_SILU ? ACT_SILU_FAST : act;
         a.nin.gamma = gamma; a.nin.beta = beta; a.nin.film0 = film0; a.nin.film1 = film1; a.nin.film1_ld = 2 * norm_C;
         a.nin.stats = xin.stats; a.nin.stats_ld = xin.stats_ld; a.nin.stats_rep = xin.stats_rep; a.nin.stats_rep_stride = xin.stats_rep_stride;
         if (res) {
@@ -712,7 +717,20 @@ int tha4_test_conv_norm(tha4_ctx* ctx, int kind, const float* x, int N, int Cin,
         const size_t wsf = conv_workspace_floats(cw, a);
         if (wsf) { a.ws = ctx->scratch.alloc(wsf); a.ws_floats = wsf; }
         conv_forward(cw, a, s);
+        if (y_stats) THA4_CUDA_CHECK(cudaMemcpyAsync(y_stats, yo.stats, (size_t)N * Cout * 2 * sizeof(double), cudaMemcpyDeviceToDevice, s));
         if (getenv("THA4_HALO_DEBUG")) { conv_forward(cw, a, s); conv_halo_debug_dump(); }
+        if (reps > 0) {       // device time of the conv alone: `reps` back-to-back launches between two events
+            cudaEvent_t e0, e1;
+            THA4_CUDA_CHECK(cudaEventCreate(&e0)); THA4_CUDA_CHECK(cudaEventCreate(&e1));
+            THA4_CUDA_CHECK(cudaEventRecord(e0, s));
+            for (int i = 0; i < reps; ++i) conv_forward(cw, a, s);
+            THA4_CUDA_CHECK(cudaEventRecord(e1, s));
+            THA4_CUDA_CHECK(cudaEventSynchronize(e1));
+            float ms = 0.0f;
+            THA4_CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
+            cudaEventDestroy(e0); cudaEventDestroy(e1);
+            if (us_per_launch) *us_per_launch = 1000.0f * ms / reps;
+        }
         nhwc_to_nchw(yo, y, s);
         if (y_from_f16) {
             View back = mk(N, Ho, Wo, Cout);
@@ -721,6 +739,22 @@ int tha4_test_conv_norm(tha4_ctx* ctx, int kind, const float* x, int N, int Cin,
         }
         THA4_CUDA_CHECK(cudaStreamSynchronize(s));
     });
+}
+
+int tha4_test_conv_norm(tha4_ctx* ctx, int kind, const float* x, int N, int Cin, int H, int W, int norm_C, int groups,
+                        const float* gamma, const float* beta, const float* film0, const float* film1, int act,
+                        const float* w, const float* bias, const float* res, int res_mode, int Cout, int ksplit,
+                        float* y, float* y_from_f16, void* stream) {
+    return test_conv_norm(ctx, kind, x, N, Cin, H, W, norm_C, groups, gamma, beta, film0, film1, act, w, bias, res, res_mode, Cout,
+                          ksplit, y, y_from_f16, nullptr, 0, nullptr, stream);
+}
+
+int tha4_test_conv_norm_ex(tha4_ctx* ctx, int kind, const float* x, int N, int Cin, int H, int W, int norm_C, int groups,
+                           const float* gamma, const float* beta, const float* film0, const float* film1, int act,
+                           const float* w, const float* bias, const float* res, int res_mode, int Cout, int ksplit,
+                           float* y, float* y_from_f16, double* y_stats, int reps, float* us_per_launch, void* stream) {
+    return test_conv_norm(ctx, kind, x, N, Cin, H, W, norm_C, groups, gamma, beta, film0, film1, act, w, bias, res, res_mode, Cout,
+                          ksplit, y, y_from_f16, y_stats, reps, us_per_launch, stream);
 }
 
 int tha4_test_norm(tha4_ctx* ctx, const float* x, int N, int C, int H, int W, int groups, const float* gamma,

@@ -30,29 +30,44 @@ namespace {
 using namespace tc;
 using namespace tcdev;
 
-constexpr int HT_W = 8, HT_H = 16;                 // CTA tile: 8 x 16 = 128 output pixels
-constexpr int HALO_W = HT_W + 2, HALO_H = HT_H + 2, HALO_ROWS = HALO_W * HALO_H;     // 10 x 18 = 180 pixel rows
-
-__host__ __device__ constexpr int halo_a_bytes(int rowb) { return ((HALO_ROWS * rowb + 1023) / 1024) * 1024; }
+// CTA tile: 8 x 16 = 128 output pixels per consumer warpgroup; WG = 2 consumer warpgroups stack two of them vertically
+// (8 x 32 = 256 pixels) and share every weight tile: half the weight traffic L2 -> shared memory per FLOP, half the
+// CTA start-up cost (barriers, PDL wait, statistic fold of the normalisation table) per pixel.
+constexpr int HT_W = 8, HT_H = 16;
+constexpr int HALO_W = HT_W + 2;
+__host__ __device__ constexpr int halo_h(int wg) { return HT_H * wg + 2; }                  // 18 / 34
+__host__ __device__ constexpr int halo_rows(int wg) { return HALO_W * halo_h(wg); }         // 180 / 340 pixel rows
+__host__ __device__ constexpr int halo_a_bytes(int rowb, int wg) { return ((halo_rows(wg) * rowb + 1023) / 1024) * 1024; }
+__host__ __device__ constexpr int halo_threads(int wg) { return 128 * wg + 32; }           // + the TMA producer warp
+// warpgroup 1 reads the halo 16 pixel rows (160 halo rows) further on: a multiple of 1024 bytes at both row widths, so
+// its descriptors see the same swizzle phase as warpgroup 0's
+static_assert((HT_H * HALO_W * 64) % 1024 == 0, "second warpgroup's halo offset keeps the swizzle phase");
 
 // SA / SB: stages of the activation-halo ring / of the weight-tile ring.  OP: OP_F16 (64 channels per chunk, 128-byte rows)
 // or OP_F16N (32 channels, 64-byte rows).  p.ksplit = cluster size CS (split over channel chunks), p.cpt = chunks.
 // MINB: resident CTAs per SM the register allocation must allow (4 for the single-chunk unsplit variants, whose small
-// rings fit four times: the layers at 256x256 / 512x512 are chains of dependent latencies, more CTAs = more overlap)
-__host__ __device__ constexpr int halo_min_ctas(int bn, int sa, int cs, int op) {
-    return cs > 1 || bn >= 128 ? 1 : ((sa == (op == OP_F16N ? 2 : 1) && bn <= 32) ? 4 : 2);
+// rings fit four times: the layers at 256x256 / 512x512 are chains of dependent latencies, more CTAs = more overlap).
+// Two-warpgroup CTAs (BN <= 64): two with BN = 32, as many consumer warps per SM as four one-warpgroup CTAs; one with
+// BN = 64 (two would cap the 288 threads at 96 registers, which spills the 64-column accumulator's epilogue)
+__host__ __device__ constexpr int halo_min_ctas(int bn, int sa, int cs, int op, int wg) {
+    return wg > 1 ? (bn <= 32 ? 2 : 1) : cs > 1 || bn >= 128 ? 1 : ((sa == (op == OP_F16N ? 2 : 1) && bn <= 32) ? 4 : 2);
 }
-template <int BN, int SA, int SB, int CS, int OP, int XF>
-__global__ void __launch_bounds__(TC_THREADS, halo_min_ctas(BN, SA, CS, OP)) conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+// WG: consumer warpgroups (1: 128-pixel tiles, 160 threads; 2: 256-pixel tiles, 288 threads, unsplit only)
+template <int BN, int SA, int SB, int CS, int OP, int XF, int WG>
+__global__ void __launch_bounds__(halo_threads(WG), halo_min_ctas(BN, SA, CS, OP, WG)) conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                                                                 const __grid_constant__ CUtensorMap tmO32, const __grid_constant__ CUtensorMap tmO16,
                                                                 const __grid_constant__ CUtensorMap tmR, const TcParams p) {
     static_assert(OP != OP_TF32, "halo kernel: f16 operands");
     static_assert(BN <= 128, "the accumulator of one warpgroup: BN registers per thread");
+    static_assert(WG == 1 || (WG == 2 && CS == 1 && BN <= 64), "two consumer warpgroups: unsplit launches, two accumulators of at most 64 columns");
     constexpr int ROWB = op_row_bytes(OP);
     constexpr int KCE = op_kch(OP);
-    constexpr int A_BYTES = halo_a_bytes(ROWB);
+    constexpr int HALO_ROWS = halo_rows(WG);
+    constexpr int A_BYTES = halo_a_bytes(ROWB, WG);
     constexpr int B_BYTES = BN * ROWB;
-    constexpr int NSLOT = CS == 1 ? epi_nslot(BN, (size_t)SA * A_BYTES + (size_t)SB * B_BYTES) : 0;     // TMA-store staging slots of the unsplit epilogue
+    constexpr int PRODUCER_WARP = 4 * WG;
+    constexpr int EPI_BYTES = (int)(((size_t)SA * A_BYTES + (size_t)SB * B_BYTES) / WG) & ~1023;      // idle ring per warpgroup in the epilogue
+    constexpr int NSLOT = CS == 1 ? epi_nslot(BN, EPI_BYTES) : 0;     // TMA-store staging slots of the unsplit epilogue
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);      // pointer arithmetic (not an integer round trip) keeps the shared address space: LDS / STS, not generic LD / ST
     uint8_t* smA = smem;
@@ -60,8 +75,8 @@ __global__ void __launch_bounds__(TC_THREADS, halo_min_ctas(BN, SA, CS, OP)) con
     uint64_t* bars = reinterpret_cast<uint64_t*>(smB + SB * B_BYTES);
     uint64_t* a_full = bars, *a_empty = bars + SA;
     uint64_t* b_full = bars + 2 * SA, *b_empty = b_full + SB;
-    uint64_t* res_bars = b_empty + SB;                                   // [4]: residual tiles of the unsplit epilogue (epi_direct)
-    float* xf_A = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(res_bars + 4) + ((16u - (tc::smem_u32(res_bars + 4) & 15u)) & 15u));
+    uint64_t* res_bars = b_empty + SB;                                   // [4 per warpgroup]: residual tiles of the unsplit epilogue (epi_direct)
+    float* xf_A = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(res_bars + 4 * WG) + ((16u - (tc::smem_u32(res_bars + 4 * WG) & 15u)) & 15u));
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // developer timing: CTA `slot` of every 97 records clock64 at its phase boundaries (8 stamps per role: dbg[slot][role][8])
@@ -73,7 +88,7 @@ __global__ void __launch_bounds__(TC_THREADS, halo_min_ctas(BN, SA, CS, OP)) con
     const int tx = tile % p.tiles_x; tile /= p.tiles_x;
     const int ty = tile % p.tiles_y;
     const int n = tile / p.tiles_y;
-    const int x0 = tx * HT_W, y0 = ty * HT_H;
+    const int x0 = tx * HT_W, y0 = ty * (HT_H * WG);
     const int n0 = blockIdx.y * BN;
     const int split = blockIdx.z;                                        // rank in the cluster (CS == gridDim.z)
     const int c_per = (p.cpt + CS - 1) / CS;
@@ -83,9 +98,9 @@ __global__ void __launch_bounds__(TC_THREADS, halo_min_ctas(BN, SA, CS, OP)) con
 
     if (threadIdx.x == 0) {
         // the empty barriers take one arrival per consumer thread: every thread arrives once its own wgmma wait has returned
-        for (int s = 0; s < SA; ++s) { mbar_init(smem_u32(a_full + s), 1); mbar_init(smem_u32(a_empty + s), 128); }
-        for (int s = 0; s < SB; ++s) { mbar_init(smem_u32(b_full + s), 1); mbar_init(smem_u32(b_empty + s), 128); }
-        for (int s = 0; s < 4; ++s) mbar_init(smem_u32(res_bars + s), 1);
+        for (int s = 0; s < SA; ++s) { mbar_init(smem_u32(a_full + s), 1); mbar_init(smem_u32(a_empty + s), 128 * WG); }
+        for (int s = 0; s < SB; ++s) { mbar_init(smem_u32(b_full + s), 1); mbar_init(smem_u32(b_empty + s), 128 * WG); }
+        for (int s = 0; s < 4 * WG; ++s) mbar_init(smem_u32(res_bars + s), 1);
         asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
         asm volatile("prefetch.tensormap [%0];\n" :: "l"(&tmA) : "memory");
         asm volatile("prefetch.tensormap [%0];\n" :: "l"(&tmB) : "memory");
@@ -95,7 +110,7 @@ __global__ void __launch_bounds__(TC_THREADS, halo_min_ctas(BN, SA, CS, OP)) con
     pdl_trigger();
     // weight tiles of the first ring pass do not depend on the previous kernel: fetch them ahead of the dependency wait
     const int npre = p.pre_b ? min(nb, SB) : 0;
-    if (warp == TC_PRODUCER_WARP && lane == 0) {
+    if (warp == PRODUCER_WARP && lane == 0) {
         for (int i = 0; i < npre; ++i) {
             const uint32_t full = smem_u32(b_full + i);
             mbar_expect_tx(full, B_BYTES);
@@ -107,7 +122,7 @@ __global__ void __launch_bounds__(TC_THREADS, halo_min_ctas(BN, SA, CS, OP)) con
 
     Acc<BN> acc;
     if (nc > 0) {
-        if (warp == TC_PRODUCER_WARP) {
+        if (warp == PRODUCER_WARP) {
             if (lane == 0) {   // ===== TMA producer: one halo box per chunk, nine weight tiles per chunk =====
                 int bi = 0;
                 for (int ci = 0; ci < nc; ++ci) {
@@ -125,15 +140,18 @@ __global__ void __launch_bounds__(TC_THREADS, halo_min_ctas(BN, SA, CS, OP)) con
                 }
             }
         } else {
-            // ===== consumer warpgroup: normalise each chunk's halo ONCE, in place (XF); 9 taps = 9 row-shifted views of the
-            // halo through wgmma; then the epilogue =====
-            const int te = threadIdx.x;
+            // ===== consumer warpgroup(s): normalise each chunk's halo ONCE, in place (XF); 9 taps = 9 row-shifted views of
+            // the halo through wgmma; then the epilogue.  With WG = 2 both warpgroups consume every weight stage; warpgroup
+            // wg computes tile rows 16 wg .. 16 wg + 15 =====
+            const int te = threadIdx.x;                                          // 0 .. 128 WG - 1
+            const int wg = WG == 1 ? 0 : te >> 7;
+            constexpr int XBAR = WG == 1 ? 1 : 3;                                // named barrier of all consumer threads
             __half* hA = reinterpret_cast<__half*>(xf_A);
             __half* hB = hA + p.xf_C;
             const bool silu = p.xf_act == ACT_SILU || p.xf_act == ACT_SILU_FAST;
             if (XF) {
                 double2* chs = reinterpret_cast<double2*>(xf_A + 2 * p.xf_C);
-                xf_build_coef(p, n, te, hA, hB, chs, cb0 * KCE, (cb0 + nc) * KCE);
+                xf_build_coef<128 * WG, XBAR>(p, n, te, hA, hB, chs, cb0 * KCE, (cb0 + nc) * KCE);
                 if (te == 0) HSTAMP(2, 0);
             }
             int bi = 0;
@@ -143,9 +161,10 @@ __global__ void __launch_bounds__(TC_THREADS, halo_min_ctas(BN, SA, CS, OP)) con
                 if (te == 0 && ci == 0) HSTAMP(2, 1);
                 if (XF) {
                     const int c0 = (cb0 + ci) * KCE;
-                    // items = (halo row, half row): 360 items over 128 threads
+                    // items = (halo row, half row): 360 / 680 items over 128 / 256 threads; the rows both warpgroups read
+                    // are transformed once
                     constexpr int HC = ROWB / 32;                                             // chunks per half row
-                    for (int it = te; it < 2 * HALO_ROWS; it += 128) {
+                    for (int it = te; it < 2 * HALO_ROWS; it += 128 * WG) {
                         const int row = it >> 1, half = it & 1;
                         const int hy = row / HALO_W, hx = row - hy * HALO_W;
                         const int iy = y0 - 1 + hy, ix = x0 - 1 + hx;
@@ -154,10 +173,10 @@ __global__ void __launch_bounds__(TC_THREADS, halo_min_ctas(BN, SA, CS, OP)) con
                         xf_chunks<HC>(smA + sa * A_BYTES + row * ROWB, swz, half * HC, c0, p, hA, hB, silu);
                     }
                     asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");   // generic-proxy writes -> wgmma's async-proxy reads
-                    asm volatile("bar.sync 1, 128;\n" ::: "memory");
+                    asm volatile("bar.sync %0, %1;\n" :: "n"(XBAR), "n"(128 * WG) : "memory");
                     if (te == 0 && ci == nc - 1) HSTAMP(2, 2);
                 }
-                const uint32_t a_base = smem_u32(smA + sa * A_BYTES);
+                const uint32_t a_base = smem_u32(smA + sa * A_BYTES) + (uint32_t)(wg * HT_H * HALO_W * ROWB);
                 // unrolled: the wait depth and the arrivals below depend on the tap only, so no branch separates wgmma issue
                 // from its wait (a data-dependent one makes ptxas serialise the wgmma)
 #pragma unroll
@@ -190,7 +209,10 @@ __global__ void __launch_bounds__(TC_THREADS, halo_min_ctas(BN, SA, CS, OP)) con
             }
             wg_fence_acc(acc.d[0]); wg_fence_acc(acc.d[1]);
             if (te == 0) { HSTAMP(1, 1); HSTAMP(2, 3); }
-            if (CS == 1) epi_direct<BN, HT_W, NSLOT>(p, acc, smem, n, y0, x0, n0, 0, 0, warp, lane, &tmO32, &tmO16, &tmR, res_bars);
+            // the epilogue reuses the ring: with two warpgroups, the other one may still be reading its last stages
+            if constexpr (WG > 1) asm volatile("bar.sync 3, 256;\n" ::: "memory");
+            if (CS == 1) epi_direct<BN, HT_W, NSLOT, WG>(p, acc, smem + wg * EPI_BYTES, n, y0 + wg * HT_H, x0, n0, 0, 0, warp, lane,
+                                                         &tmO32, &tmO16, &tmR, res_bars + 4 * wg, wg, EPI_BYTES);
             if (te == 0) HSTAMP(2, 4);
         }
     }
@@ -199,12 +221,12 @@ __global__ void __launch_bounds__(TC_THREADS, halo_min_ctas(BN, SA, CS, OP)) con
         asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
         asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
         if (threadIdx.x == 0) HSTAMP(2, 5);
-        if (warp < TC_PRODUCER_WARP && nc > 0) epi_push_partial<BN, CS>(acc, smem, split, warp, lane);
+        if (warp < PRODUCER_WARP && nc > 0) epi_push_partial<BN, CS>(acc, smem, split, warp, lane);
         // barrier B: the pushed slices are visible to their owners; nobody touches a peer's memory afterwards
         asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
         asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
         if (threadIdx.x == 0) HSTAMP(2, 7);
-        if (warp < TC_PRODUCER_WARP) epi_cluster_reduce<BN, CS, HT_W>(p, smem, n, y0, x0, n0, 0, split, warp, dbg);
+        if (warp < PRODUCER_WARP) epi_cluster_reduce<BN, CS, HT_W>(p, smem, n, y0, x0, n0, 0, split, warp, dbg);
         if (threadIdx.x == 0) HSTAMP(2, 6);
     }
     __syncthreads();
@@ -232,15 +254,15 @@ using HKey = std::tuple<int, const void*, long, long, long, long, long, int>;
 std::map<HKey, CUtensorMap> g_halo_maps;
 std::mutex g_halo_mu;
 
-const CUtensorMap& halo_activation_map(const View& v, int op) {
-    HKey key{current_device(), v.p, v.N, v.H, v.W, v.C, v.ld, op};
+const CUtensorMap& halo_activation_map(const View& v, int op, int wg) {
+    HKey key{current_device(), v.p, v.N, v.H, v.W, v.C, v.ld, op + 16 * wg};
     std::lock_guard<std::mutex> lock(g_halo_mu);
     auto it = g_halo_maps.find(key);
     if (it != g_halo_maps.end()) return it->second;
     CUtensorMap m;
     cuuint64_t dims[4] = {(cuuint64_t)v.C, (cuuint64_t)v.W, (cuuint64_t)v.H, (cuuint64_t)v.N};
     cuuint64_t strides[3] = {(cuuint64_t)v.ld * 2, (cuuint64_t)v.W * v.ld * 2, (cuuint64_t)v.H * v.W * v.ld * 2};
-    cuuint32_t box[4] = {(cuuint32_t)op_kch(op), (cuuint32_t)HALO_W, (cuuint32_t)HALO_H, 1};
+    cuuint32_t box[4] = {(cuuint32_t)op_kch(op), (cuuint32_t)HALO_W, (cuuint32_t)halo_h(wg), 1};
     cuuint32_t es[4] = {1, 1, 1, 1};
     CUresult r = halo_encode()(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, v.p, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                op == OP_F16N ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
@@ -290,7 +312,10 @@ bool halo_store_map(const View& v, bool f16, const CUtensorMap** out) {
     return true;
 }
 
-struct HaloPlan { int bn, tiles_x, tiles_y, tiles_m, tiles_n, cs, chunks; };
+int g_halo_m256 = -1;         // option "halo_m256": -1 automatic, 0 / 1 force 128- / 256-pixel tiles on unsplit launches
+
+// wg: consumer warpgroups per CTA (1: 128-pixel tiles; 2: 256-pixel tiles, unsplit launches only)
+struct HaloPlan { int bn, tiles_x, tiles_y, tiles_m, tiles_n, cs, chunks, wg; };
 
 HaloPlan halo_plan(const ConvWeights& cw, const ConvArgs& a, int op) {
     HaloPlan pl;
@@ -302,9 +327,15 @@ HaloPlan halo_plan(const ConvWeights& cw, const ConvArgs& a, int op) {
     const int sms = num_sms();
     pl.cs = 1;
     long ctas = (long)pl.tiles_m * (cw.cout_pad / pl.bn);
+    // 256-pixel tiles (two consumer warpgroups, see below) for every launch of at least an eighth of a wave of 128-pixel
+    // tiles, unsplit even when the CTAs do not fill the GPU: measured alone on an H100, every such layer of the teacher
+    // frame ran faster than on 128-pixel tiles (1.03 - 1.36x at a 400 W power limit, down to 128 tiles), and the 64 x 64
+    // layers with 128 - 512 channels (32 tiles) faster than their cluster split-K launches (1.1 - 2.1x at 700 W).  With fewer tiles (32 x 32 and
+    // below) the split-K launches win.
+    const bool m256 = g_halo_m256 > 0 || (g_halo_m256 < 0 && a.ksplit <= 1 && 8L * pl.tiles_m >= sms);
     if (a.ksplit > 1) {
         while (pl.cs * 2 <= std::min(8, a.ksplit)) pl.cs *= 2;
-    } else if (a.ksplit <= 0 && ctas < sms * 13 / 16) {
+    } else if (a.ksplit <= 0 && ctas < sms * 13 / 16 && !m256) {
         // Too few tiles to fill the GPU.  Narrow the N tiles first (down to 64 columns: more CTAs and nothing to exchange),
         // then split the channel chunks over a cluster.  The DSMEM exchange moves 128 x bn x 4 x (cs-1)/cs bytes per CTA at
         // a few bytes per clock, so a wide split of a wide tile costs more than the MMA phase it parallelises.
@@ -316,32 +347,64 @@ HaloPlan halo_plan(const ConvWeights& cw, const ConvArgs& a, int op) {
     }
     while (pl.cs > 1 && (pl.cs > pl.chunks || ceil_div(pl.chunks, ceil_div(pl.chunks, pl.cs)) != pl.cs)) pl.cs /= 2;   // every rank owns chunks
     pl.tiles_n = cw.cout_pad / pl.bn;
+    // Unsplit launches with many tiles take 256-pixel tiles: each weight tile then feeds 256 rows instead of 128.  Two
+    // 128-column accumulators do not fit the registers of a 288-thread CTA, so 128-column tiles become 256 x 64 (per FLOP:
+    // half the weight bytes, twice the halo bytes -- a third less L2 -> shared-memory traffic in all).
+    pl.wg = 1;
+    if (pl.cs == 1 && m256) {
+        pl.wg = 2;
+        pl.tiles_y = ceil_div(a.out.H, 2 * HT_H);
+        pl.tiles_m = pl.tiles_x * pl.tiles_y * a.in.N;
+        pl.bn = std::min(pl.bn, 64);
+        pl.tiles_n = cw.cout_pad / pl.bn;
+    }
     return pl;
 }
 
-template <int OP, int BN, int SA, int SB, int CS, int XF>
+template <int OP, int BN, int SA, int SB, int CS, int XF, int WG = 1>
 void launch_halo(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo32, const CUtensorMap& mo16, const CUtensorMap& mr, const TcParams& p, dim3 grid, cudaStream_t s) {
     constexpr int ROWB = op_row_bytes(OP);
-    constexpr size_t ring = (size_t)SA * halo_a_bytes(ROWB) + (size_t)SB * BN * ROWB;
-    constexpr size_t smem0 = 1024 + ring + (2 * SA + 2 * SB + 4) * 8 + 16;
+    constexpr size_t ring = (size_t)SA * halo_a_bytes(ROWB, WG) + (size_t)SB * BN * ROWB;
+    constexpr size_t smem0 = 1024 + ring + (2 * SA + 2 * SB + 4 * WG) * 8 + 16;
     static_assert(smem0 <= 227 * 1024, "shared memory budget");
-    static_assert(ring >= (size_t)4 * 32 * 33 * 4 + 4 * BN * 8, "epilogue scratch must fit in the pipeline buffers");
+    static_assert(ring / WG >= (size_t)4 * 32 * 33 * 4 + 4 * BN * 8, "epilogue scratch must fit in the pipeline buffers");
+    static_assert(WG == 1 || epi_nslot(BN, (ring / WG) & ~(size_t)1023) > 0, "two warpgroups: a TMA-store staging slot each");
     static_assert(CS == 1 || ring >= (size_t)128 * BN * 4 + 128 * 8 * 4 + 128 * 4 * 4, "partial tile + statistics scratch must fit");
     const size_t smem = smem0 + (XF ? (size_t)24 * p.xf_C + 32 : 0);
     THA4_REQUIRE(smem <= 227 * 1024, "conv_halo: shared memory budget (fused input normalisation)");
-    THA4_ENSURE_SMEM((conv_halo_kernel<BN, SA, SB, CS, OP, XF>), smem);
-    launch_pdl(conv_halo_kernel<BN, SA, SB, CS, OP, XF>, grid, dim3(TC_THREADS), smem, s, CS, ma, mb, mo32, mo16, mr, p);
+    THA4_ENSURE_SMEM((conv_halo_kernel<BN, SA, SB, CS, OP, XF, WG>), smem);
+    launch_pdl(conv_halo_kernel<BN, SA, SB, CS, OP, XF, WG>, grid, dim3(halo_threads(WG)), smem, s, CS, ma, mb, mo32, mo16, mr, p);
     THA4_LAUNCH_CHECK();
 }
 
 // SBD: weight-ring depth of the cluster split-K launches (few CTAs per SM, the ring is what hides the DRAM latency of weights
 // that are fetched ahead of the dependency wait); SBS: depth of the unsplit launches (many tiles: a shallow ring keeps
 // the CTA small so that 2 - 4 of them share an SM and overlap each other's load -> transform -> MMA -> drain chains).
+// Weight stages of a two-warpgroup CTA: at least sb_min, and enough that each warpgroup's half of the idle ring holds the
+// epilogue scratch and one TMA-store staging slot.
+constexpr int halo_sb_wg2(int op, int bn, int sa, int sb_min) {
+    const size_t a = (size_t)sa * halo_a_bytes(op_row_bytes(op), 2), b = (size_t)bn * op_row_bytes(op);
+    int sb = sb_min;
+    while (a + sb * b < 2 * (size_t)(epi_slot0(bn) + EPI_SLOT_BYTES)) ++sb;
+    return sb;
+}
+
 template <int OP, int BN, int SA, int SBD, int SBS, int XF>
-void launch_halo_cs(int cs, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo32, const CUtensorMap& mo16, const CUtensorMap& mr, const TcParams& p, dim3 grid, cudaStream_t s) {
+void launch_halo_cs(int cs, int wg, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo32, const CUtensorMap& mo16, const CUtensorMap& mr, const TcParams& p, dim3 grid, cudaStream_t s) {
+    constexpr int SA1 = OP == OP_F16N ? 2 : 1;
+    THA4_REQUIRE(wg == 1 || (BN <= 64 && cs == 1), "conv_halo: 256-pixel tiles need an unsplit launch with N tiles of at most 64 columns");
     if constexpr (BN <= 64) {
-        if (cs == 1 && p.cpt == 1) {     // one chunk: one halo, ever -> a ring that fits four times per SM
-            launch_halo<OP, BN, (OP == OP_F16N ? 2 : 1), SBS, 1, XF>(ma, mb, mo32, mo16, mr, p, grid, s);
+        if (cs == 1 && p.cpt == 1) {     // one chunk: one halo, ever -> a ring that fits four times per SM (twice with two warpgroups)
+            if (wg == 2) launch_halo<OP, BN, SA1, halo_sb_wg2(OP, BN, SA1, BN == 64 ? SBD : SBS), 1, XF, 2>(ma, mb, mo32, mo16, mr, p, grid, s);
+            else launch_halo<OP, BN, SA1, SBS, 1, XF>(ma, mb, mo32, mo16, mr, p, grid, s);
+            return;
+        }
+    }
+    if constexpr (BN <= 64) {
+        if (wg == 2) {
+            // BN = 64: one CTA per SM, which takes the deep weight ring; BN = 32: two CTAs per SM
+            constexpr int M = OP == OP_F16N ? 2 : 1;
+            launch_halo<OP, BN, SA, halo_sb_wg2(OP, BN, SA, BN == 64 ? SBD : 2 * M), 1, XF, 2>(ma, mb, mo32, mo16, mr, p, grid, s);
             return;
         }
     }
@@ -356,11 +419,11 @@ void launch_halo_cs(int cs, const CUtensorMap& ma, const CUtensorMap& mb, const 
 }
 
 template <int OP, int XF>
-void launch_halo_bn(int bn, int cs, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo32, const CUtensorMap& mo16, const CUtensorMap& mr, const TcParams& p, dim3 grid, cudaStream_t s) {
+void launch_halo_bn(int bn, int cs, int wg, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo32, const CUtensorMap& mo16, const CUtensorMap& mr, const TcParams& p, dim3 grid, cudaStream_t s) {
     constexpr int M = OP == OP_F16N ? 2 : 1;        // 64-byte rows: twice the stages for the same bytes in flight
-    if (bn == 128) launch_halo_cs<OP, 128, 2 * M, 6 * M, 3 * M, XF>(cs, ma, mb, mo32, mo16, mr, p, grid, s);        // unsplit:  95 KB
-    else if (bn == 64) launch_halo_cs<OP, 64, 2 * M, 8 * M, 3 * M, XF>(cs, ma, mb, mo32, mo16, mr, p, grid, s);     // unsplit:  71 KB
-    else launch_halo_cs<OP, 32, 2 * M, 9 * M, 5 * M, XF>(cs, ma, mb, mo32, mo16, mr, p, grid, s);                    // unsplit:  67 KB
+    if (bn == 128) launch_halo_cs<OP, 128, 2 * M, 6 * M, 3 * M, XF>(cs, wg, ma, mb, mo32, mo16, mr, p, grid, s);        // unsplit:  95 KB
+    else if (bn == 64) launch_halo_cs<OP, 64, 2 * M, 8 * M, 3 * M, XF>(cs, wg, ma, mb, mo32, mo16, mr, p, grid, s);     // unsplit:  71 KB
+    else launch_halo_cs<OP, 32, 2 * M, 9 * M, 5 * M, XF>(cs, wg, ma, mb, mo32, mo16, mr, p, grid, s);                    // unsplit:  67 KB
 }
 
 bool g_use_halo = true;
@@ -370,6 +433,7 @@ bool g_tma_store = true;      // option "tma_store": unsplit epilogue through sh
 
 void conv_halo_enable(bool on) { g_use_halo = on; }
 void conv_halo_enable_tma_store(bool on) { g_tma_store = on; }
+void conv_halo_set_m256(int mode) { g_halo_m256 = mode; }
 
 bool conv_halo_supported(const ConvWeights& cw, const ConvArgs& a) {
     if (!g_use_halo || !conv_tc_supported(cw, a)) return false;
@@ -424,7 +488,7 @@ void conv_halo_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s)
     }
     ProfScope prof(PROF_CONV, s);
     prof_add_work(PROF_CONV, 2.0 * (double)p.N * p.MH * p.MW * cw.cout * cw.cin * 9, 0.0);
-    const CUtensorMap& ma = halo_activation_map(a.in, op);
+    const CUtensorMap& ma = halo_activation_map(a.in, op, pl.wg);
     const CUtensorMap& mb = halo_weight_map(cw, pl.bn, op);
     const CUtensorMap* mo32 = &ma;                   // placeholders when an output does not leave through TMA
     const CUtensorMap* mo16 = &ma;
@@ -441,16 +505,16 @@ void conv_halo_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s)
               (!a.res.p || ((reinterpret_cast<uintptr_t>(a.res.p) & 15) == 0 && a.res.ld % 4 == 0))) ? 1 : 0;
     dim3 grid(pl.tiles_m, pl.tiles_n, pl.cs);
     if (op == OP_F16) {
-        if (a.nin.on) launch_halo_bn<OP_F16, 1>(pl.bn, pl.cs, ma, mb, *mo32, *mo16, *mr, p, grid, s);
-        else launch_halo_bn<OP_F16, 0>(pl.bn, pl.cs, ma, mb, *mo32, *mo16, *mr, p, grid, s);
+        if (a.nin.on) launch_halo_bn<OP_F16, 1>(pl.bn, pl.cs, pl.wg, ma, mb, *mo32, *mo16, *mr, p, grid, s);
+        else launch_halo_bn<OP_F16, 0>(pl.bn, pl.cs, pl.wg, ma, mb, *mo32, *mo16, *mr, p, grid, s);
     } else {
-        if (a.nin.on) launch_halo_bn<OP_F16N, 1>(pl.bn, pl.cs, ma, mb, *mo32, *mo16, *mr, p, grid, s);
-        else launch_halo_bn<OP_F16N, 0>(pl.bn, pl.cs, ma, mb, *mo32, *mo16, *mr, p, grid, s);
+        if (a.nin.on) launch_halo_bn<OP_F16N, 1>(pl.bn, pl.cs, pl.wg, ma, mb, *mo32, *mo16, *mr, p, grid, s);
+        else launch_halo_bn<OP_F16N, 0>(pl.bn, pl.cs, pl.wg, ma, mb, *mo32, *mo16, *mr, p, grid, s);
     }
     static const bool dbg_all = dbg_env && !strcmp(getenv("THA4_HALO_DEBUG"), "2");
     if (dbg_all) {       // developer: stamps of every launch of a real forward (serialises the stream)
-        fprintf(stderr, "halo launch: N %d %dx%d cin %d cout %d | bn %d cs %d chunks %d grid %d x %d | xf %d groups %d act %d res %d out32 %d out16 %d st_tma %d\n",
-                p.N, p.MH, p.MW, cw.cin, cw.cout, pl.bn, pl.cs, pl.chunks, pl.tiles_m, pl.tiles_n, a.nin.on ? 1 : 0, p.xf_groups, p.xf_act,
+        fprintf(stderr, "halo launch: N %d %dx%d cin %d cout %d | bn %d cs %d wg %d chunks %d grid %d x %d | xf %d groups %d act %d res %d out32 %d out16 %d st_tma %d\n",
+                p.N, p.MH, p.MW, cw.cin, cw.cout, pl.bn, pl.cs, pl.wg, pl.chunks, pl.tiles_m, pl.tiles_n, a.nin.on ? 1 : 0, p.xf_groups, p.xf_act,
                 p.res_mode, p.out ? 1 : 0, p.out16 ? 1 : 0, p.st_tma);
         conv_halo_debug_dump();
     }

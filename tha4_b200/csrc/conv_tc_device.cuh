@@ -22,13 +22,22 @@ constexpr int TC_PRODUCER_WARP = 4;
 // The 128 x BN fp32 accumulator of a CTA tile, in the registers of the consumer warpgroup: two m64 halves (rows 0-63, 64-127).
 template <int BN> struct Acc { float d[2][BN / 2]; };
 
+// Named barrier of one consumer warpgroup.  WG: consumer warpgroups of the CTA; warpgroup wg synchronises on barrier 1 + wg
+// (barrier 3 spans all consumer threads of a two-warpgroup CTA).
+template <int WG>
+__device__ __forceinline__ void wg_bar(int wg) {
+    if (WG == 1 || wg == 0) asm volatile("bar.sync 1, 128;\n" ::: "memory");       // immediate ids: ptxas reserves
+    else asm volatile("bar.sync 2, 128;\n" ::: "memory");                         // all 16 barriers for a register id
+}
+
 // Columns [c0, c0 + 32) of the accumulator, transposed through `stage` ([128][33] floats) so that thread t receives the 32
-// values of tile row t (the row-per-thread layout the epilogues are written for).  Called by all 128 consumer threads with
-// the same c0 (a constant after unrolling: the accumulator stays in registers).
-template <int BN>
-__device__ __forceinline__ void acc_rows32(const Acc<BN>& acc, int c0, float* stage, uint32_t (&r)[32]) {
-    const int t = threadIdx.x, w = t >> 5, l = t & 31;
-    asm volatile("bar.sync 1, 128;\n" ::: "memory");            // earlier readers of the stage are done
+// values of tile row t (the row-per-thread layout the epilogues are written for).  Called by all 128 threads of consumer
+// warpgroup wg with the same c0 (a constant after unrolling: the accumulator stays in registers); t: the thread's index in
+// its warpgroup.
+template <int BN, int WG = 1>
+__device__ __forceinline__ void acc_rows32(const Acc<BN>& acc, int c0, float* stage, uint32_t (&r)[32], int t, int wg) {
+    const int w = t >> 5, l = t & 31;
+    wg_bar<WG>(wg);                                              // earlier readers of the stage are done
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -38,7 +47,7 @@ __device__ __forceinline__ void acc_rows32(const Acc<BN>& acc, int c0, float* st
             stage[row * 33 + col] = acc.d[h][4 * g];             stage[row * 33 + col + 1] = acc.d[h][4 * g + 1];
             stage[(row + 8) * 33 + col] = acc.d[h][4 * g + 2];   stage[(row + 8) * 33 + col + 1] = acc.d[h][4 * g + 3];
         }
-    asm volatile("bar.sync 1, 128;\n" ::: "memory");
+    wg_bar<WG>(wg);
 #pragma unroll
     for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(stage[t * 33 + j]);
 }
@@ -87,9 +96,11 @@ __host__ __device__ constexpr int op_stages(int op, int stages) { return op == O
 
 // ===== fused input normalisation (XF kernels) =====
 // Per-channel affine of sample n's pending normalisation, as packed halves (the operand is f16; HFMA2 / tanh.approx.f16x2
-// keep the in-place pass cheap).  Called by the 128 consumer threads (te = 0..127); chs: scratch [xf_C] double2.
+// keep the in-place pass cheap).  Called by the NT consumer threads (te = 0..NT-1), which synchronise on named barrier BAR;
+// chs: scratch [xf_C] double2.
 // [c_lo, c_hi): the channels this CTA will transform (its K chunks); widened to whole normalisation groups.  A cluster
 // split-K CTA builds 1 / CS of the table (the fold of the statistic replicas is the expensive part).
+template <int NT = 128, int BAR = 1>
 __device__ __forceinline__ void xf_build_coef(const TcParams& p, int n, int te, __half* hA, __half* hB, double2* chs, int c_lo, int c_hi) {
     const int cpg = p.xf_groups == 0 ? 1 : p.xf_C / p.xf_groups;
     c_lo = (c_lo / cpg) * cpg;
@@ -103,11 +114,11 @@ __device__ __forceinline__ void xf_build_coef(const TcParams& p, int n, int te, 
     const float g1 = h1 ? __ldg(p.xf_gamma + c1) : 0.0f, b1 = h1 ? __ldg(p.xf_beta + c1) : 0.0f;
     const float f0s = (h1 && p.xf_film0) ? __ldg(p.xf_film0 + c1) : 0.0f, f0h = (h1 && p.xf_film0) ? __ldg(p.xf_film0 + p.xf_C + c1) : 0.0f;
     const float f1s = (h1 && f1p) ? __ldg(f1p + c1) : 0.0f, f1h = (h1 && f1p) ? __ldg(f1p + p.xf_C + c1) : 0.0f;
-    for (int c = c_lo + te; c < c_hi; c += 128)
+    for (int c = c_lo + te; c < c_hi; c += NT)
         chs[c] = fold_stat_replicas16(p.in_stats + ((long)n * p.in_stats_ld + c) * 2, p.in_stats_rep_stride, p.in_stats_rep);
-    asm volatile("bar.sync 1, 128;\n" ::: "memory");
+    asm volatile("bar.sync %0, %1;\n" :: "n"(BAR), "n"(NT) : "memory");
     const bool silu = p.xf_act == ACT_SILU || p.xf_act == ACT_SILU_FAST;
-    for (int c = c_lo + te; c < c_hi; c += 128) {
+    for (int c = c_lo + te; c < c_hi; c += NT) {
         const int g0 = (c / cpg) * cpg;
         double su = 0.0, sq = 0.0;
         for (int j = 0; j < cpg; ++j) { const double2 v = chs[g0 + j]; su += v.x; sq += v.y; }
@@ -125,7 +136,7 @@ __device__ __forceinline__ void xf_build_coef(const TcParams& p, int n, int te, 
         if (silu) { A *= 0.5f; B *= 0.5f; }                      // silu(v) = h + h * tanh(h) with h = v / 2
         hA[c] = __float2half_rn(fminf(fmaxf(A, -65504.0f), 65504.0f)); hB[c] = __float2half_rn(fminf(fmaxf(B, -65504.0f), 65504.0f));
     }
-    asm volatile("bar.sync 1, 128;\n" ::: "memory");
+    asm volatile("bar.sync %0, %1;\n" :: "n"(BAR), "n"(NT) : "memory");
 }
 
 // NC consecutive 16-byte chunks (8 channels each, logical chunk index j0 .. j0 + NC) of one operand row normalised +
@@ -222,17 +233,25 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, uint32_t sr
                  :: "l"(map), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
 
-template <int BN, int TW, int NSLOT = 0>
+// WG == 2 (conv_halo.cu's 256-pixel tiles): each consumer warpgroup wg runs this on its own 128 rows, with its own named
+// barrier, its own shared-memory region `smem` (warpgroup 1's starts wg_bytes after warpgroup 0's) and its own residual
+// barriers; y0 is the first pixel row of the warpgroup's rows.  The two warpgroups' channel sums are folded in shared
+// memory before the fp64 atomics: one pair per (CTA, channel).
+template <int BN, int TW, int NSLOT = 0, int WG = 1>
 __device__ __forceinline__ void epi_direct(const TcParams& p, const Acc<BN>& acc, uint8_t* smem, int n, int y0, int x0,
                                            int n0, int phase, int split, int warp, int lane,
                                            const CUtensorMap* tm32 = nullptr, const CUtensorMap* tm16 = nullptr,
-                                           const CUtensorMap* tmR = nullptr, uint64_t* res_bars = nullptr) {
+                                           const CUtensorMap* tmR = nullptr, uint64_t* res_bars = nullptr,
+                                           int wg = 0, int wg_bytes = 0) {
+    static_assert(WG == 1 || WG == 2, "one or two consumer warpgroups");
     const int q = warp & 3;
+    const int t = WG == 1 ? (int)threadIdx.x : (int)threadIdx.x & 127;     // index in the warpgroup
+    const bool rows_in = WG == 1 || y0 < p.MH;                             // a second warpgroup's rows may all lie below the image
     // p.st_tma bit 2: the residual tile (same geometry as the fp32 output) ARRIVES by TMA as well, into the fp32 stage of
     // the slot it will leave from: 8 conflict-free LDS.128 per thread instead of 8 LDG.128 whose lanes hit 32 different lines
     const bool res_tma = NSLOT > 0 && (p.st_tma & 4) != 0;
     const int nsteps = min(BN / 32, (p.outC - n0 + 31) / 32);
-    if (res_tma && threadIdx.x == 0) {
+    if (res_tma && t == 0) {
         for (int s = 0; s < NSLOT && s < nsteps; ++s) {
             const uint32_t bar = smem_u32(res_bars + s);
             mbar_expect_tx(bar, 128 * 128);
@@ -252,7 +271,7 @@ __device__ __forceinline__ void epi_direct(const TcParams& p, const Acc<BN>& acc
 #pragma unroll
     for (int c0 = 0; c0 < BN; c0 += 32) {
         uint32_t r[32];
-        acc_rows32<BN>(acc, c0, reinterpret_cast<float*>(smem), r);    // the stage is the statistics scratch: row t at t * 33
+        acc_rows32<BN, WG>(acc, c0, reinterpret_cast<float*>(smem), r, t, wg);    // the stage is the statistics scratch: row t at t * 33
         const int cbase = n0 + c0;
         if (cbase >= p.outC) continue;                         // warp-uniform
         float v[32];
@@ -338,8 +357,8 @@ __device__ __forceinline__ void epi_direct(const TcParams& p, const Acc<BN>& acc
         if (NSLOT > 0 && st_tma) {
             // every row is staged (rows outside the image hold values of zero-padded inputs; the store clips them)
             if (step >= NSLOT && !res_tma) {
-                if (threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group.read %0;\n" :: "n"(NSLOT > 0 ? NSLOT - 1 : 0) : "memory");
-                asm volatile("bar.sync 1, 128;\n" ::: "memory");
+                if (t == 0) asm volatile("cp.async.bulk.wait_group.read %0;\n" :: "n"(NSLOT > 0 ? NSLOT - 1 : 0) : "memory");
+                wg_bar<WG>(wg);
             }
             uint8_t* slot = smem + epi_slot0(BN) + (NSLOT > 0 ? step % NSLOT : 0) * EPI_SLOT_BYTES;
             if (res_tma) {
@@ -370,10 +389,10 @@ __device__ __forceinline__ void epi_direct(const TcParams& p, const Acc<BN>& acc
                 }
             }
             asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
-            asm volatile("bar.sync 1, 128;\n" ::: "memory");
-            if (threadIdx.x == 0) {
-                if (st_tma & 1) tma_store_4d(tm32, smem_u32(slot), cbase, x0, y0, n);
-                if (st_tma & 2) tma_store_4d(tm16, smem_u32(slot + 128 * 128), cbase, x0, y0, n);
+            wg_bar<WG>(wg);
+            if (t == 0) {
+                if ((st_tma & 1) && rows_in) tma_store_4d(tm32, smem_u32(slot), cbase, x0, y0, n);
+                if ((st_tma & 2) && rows_in) tma_store_4d(tm16, smem_u32(slot + 128 * 128), cbase, x0, y0, n);
                 asm volatile("cp.async.bulk.commit_group;\n" ::: "memory");
                 if (res_tma && step + NSLOT < nsteps) {      // refill the slot with the residual of the step that will use it next
                     asm volatile("cp.async.bulk.wait_group.read 0;\n" ::: "memory");
@@ -399,18 +418,26 @@ __device__ __forceinline__ void epi_direct(const TcParams& p, const Acc<BN>& acc
         }
     }
     if (p.stats && p.ksplit == 1) {
-        // combine the four warps' partial sums: one double atomic pair per (tile, channel), spread over replicas
-        asm volatile("bar.sync 1, 128;\n" ::: "memory");
-        const float2* part = reinterpret_cast<const float2*>(reinterpret_cast<float*>(smem) + 4 * 32 * 33);
+        // combine the warps' partial sums: one double atomic pair per (tile, channel), spread over replicas
+        if constexpr (WG == 1) asm volatile("bar.sync 1, 128;\n" ::: "memory");
+        else asm volatile("bar.sync 3, 256;\n" ::: "memory");                   // both warpgroups' partials are written
+        const float2* part = reinterpret_cast<const float2*>(reinterpret_cast<float*>(smem - wg * wg_bytes) + 4 * 32 * 33);
         double* base = p.stats + (long)(blockIdx.x % p.stats_rep) * p.stats_rep_stride + ((long)n * p.stats_ld + n0) * 2;
-        for (int c = (int)threadIdx.x; c < BN; c += 128) {
+        for (int c = (int)threadIdx.x; c < BN; c += 128 * WG) {
             if (n0 + c >= p.outC) break;
             const float2 a = part[c], b = part[BN + c], cc = part[2 * BN + c], d = part[3 * BN + c];
-            atomicAdd(base + 2 * c, (double)a.x + (double)b.x + (double)cc.x + (double)d.x);
-            atomicAdd(base + 2 * c + 1, (double)a.y + (double)b.y + (double)cc.y + (double)d.y);
+            if constexpr (WG == 1) {
+                atomicAdd(base + 2 * c, (double)a.x + (double)b.x + (double)cc.x + (double)d.x);
+                atomicAdd(base + 2 * c + 1, (double)a.y + (double)b.y + (double)cc.y + (double)d.y);
+            } else {
+                const float2* part1 = part + wg_bytes / (int)sizeof(float2);
+                const float2 e = part1[c], f = part1[BN + c], g = part1[2 * BN + c], h = part1[3 * BN + c];
+                atomicAdd(base + 2 * c, (double)a.x + (double)b.x + (double)cc.x + (double)d.x + (double)e.x + (double)f.x + (double)g.x + (double)h.x);
+                atomicAdd(base + 2 * c + 1, (double)a.y + (double)b.y + (double)cc.y + (double)d.y + (double)e.y + (double)f.y + (double)g.y + (double)h.y);
+            }
         }
     }
-    if (NSLOT > 0 && st_tma && threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group.read 0;\n" ::: "memory");   // the staging slots have been read before the CTA retires (the writes themselves complete with the grid)
+    if (NSLOT > 0 && st_tma && t == 0) asm volatile("cp.async.bulk.wait_group.read 0;\n" ::: "memory");   // the staging slots have been read before the CTA retires (the writes themselves complete with the grid)
 }
 
 // ===== cluster split-K, step 2 (consumer warpgroup, after the cluster barrier that publishes the pushes): sum the CS slots of this
