@@ -4,13 +4,17 @@
 2. One warm teacher_b1 frame (mode_07, batch 1, eyebrow cache hot) under torch.profiler with CUDA activities, once with
    128-pixel halo tiles forced (option halo_m256 = 0) and once with the automatic choice: device time per kernel
    instantiation, and the share of the unsplit halo launches.
-3. Every unsplit halo conv shape of that frame (read from the library's launch log, THA4_HALO_DEBUG=2, in a child
+3. Every unsplit 3x3 halo conv shape of that frame (read from the library's launch log, THA4_HALO_DEBUG=2, in a child
    process) timed alone with CUDA events over --reps launches after warm-up, with 128- and with 256-pixel tiles:
    microseconds, TFLOP/s, and the compulsory HBM bytes computed from the shape (f16 input, f16 weights, the fp32 and f16
    outputs, the fp32 residual).  The conv runs through the kernel-level test hook with the frame's input-normalisation
    kind and residual; the hook always writes both outputs.
+4. Every four-phase shape of the teacher frame (nearest-x2 + 3x3 of the up-sampling ResBlocks, transposed 4x4 convs),
+   and two at batch 32, timed the same way on three paths: conv_tc.cu's automatic plan (halo_conv = 0), the four-phase
+   halo kernel (halo_conv = 1, an unsplit launch requested) and the automatic choice; TFLOP/s count the executed
+   products (4 phases x 4 taps per low-resolution pixel).
 
-Usage: python scripts/dev/halo_layers.py [--reps 200] [--out DIR]
+Usage: python scripts/dev/halo_layers.py [--reps 200] [--out DIR] [--phase-only]
 """
 import argparse
 import collections
@@ -26,7 +30,7 @@ sys.path.insert(0, _ROOT)
 sys.path.insert(0, os.path.join(_ROOT, 'tests'))
 
 LAUNCH_RE = re.compile(r'halo launch: N (\d+) (\d+)x(\d+) cin (\d+) cout (\d+) \| bn (\d+) cs (\d+) wg (\d+) chunks (\d+) grid (\d+) x (\d+) \| '
-                       r'xf (\d+) groups (\d+) act (\d+) res (\d+) out32 (\d+) out16 (\d+) st_tma (\d+)')
+                       r'xf (\d+) groups (\d+) act (\d+) res (\d+) out32 (\d+) out16 (\d+) st_tma (\d+) \| phases (\d+)')
 
 
 def card():
@@ -67,7 +71,8 @@ def frame_shapes():
     r = subprocess.run([sys.executable, '-c', code], capture_output=True, text=True, env=env, cwd=_ROOT)
     if r.returncode != 0:
         raise RuntimeError('launch-log run failed:\n' + r.stderr[-4000:])
-    keys = ('N', 'H', 'W', 'cin', 'cout', 'bn', 'cs', 'wg', 'chunks', 'grid_m', 'grid_n', 'xf', 'groups', 'act', 'res', 'out32', 'out16', 'st_tma')
+    keys = ('N', 'H', 'W', 'cin', 'cout', 'bn', 'cs', 'wg', 'chunks', 'grid_m', 'grid_n', 'xf', 'groups', 'act', 'res', 'out32', 'out16', 'st_tma',
+            'phases')
     log = r.stderr.split('SECOND FRAME', 1)[1]
     return [dict(zip(keys, map(int, m.groups()))) for m in LAUNCH_RE.finditer(log)]
 
@@ -103,8 +108,8 @@ def short(name):
 
 
 def halo_split(name):
-    """conv_halo_kernel<BN, SA, SB, CS, OP, XF, WG>: returns (CS, WG) or None."""
-    m = re.search(r'conv_halo_kernel<(\d+), (\d+), (\d+), (\d+), (\d+), (\d+), (\d+)>', name)
+    """conv_halo_kernel<BN, SA, SB, CS, OP, XF, WG, PH>: returns (CS, WG) or None."""
+    m = re.search(r'conv_halo_kernel<(\d+), (\d+), (\d+), (\d+), (\d+), (\d+), (\d+), (\d+)>', name)
     return (int(m.group(4)), int(m.group(7))) if m else None
 
 
@@ -126,13 +131,13 @@ def shape_ab(shapes, reps):
     c = __import__('gpu_util').ctx()
     seen, rows = set(), []
     for s in shapes:
-        if s['cs'] != 1:
+        if s['cs'] != 1 or s['phases'] != 1:
             continue
         key = (s['N'], s['H'], s['W'], s['cin'], s['cout'], s['xf'], s['groups'], s['act'], s['res'])
         if key in seen:
             continue
         seen.add(key)
-        count = sum(1 for t in shapes if t['cs'] == 1 and (t['N'], t['H'], t['W'], t['cin'], t['cout'], t['xf'], t['groups'], t['act'], t['res']) == key)
+        count = sum(1 for t in shapes if t['cs'] == 1 and t['phases'] == 1 and (t['N'], t['H'], t['W'], t['cin'], t['cout'], t['xf'], t['groups'], t['act'], t['res']) == key)
         norm = None if not s['xf'] else ('gn' if s['groups'] else 'in')
         inp = H.make_inputs(7, s['N'], s['cin'], s['H'], s['W'], s['cout'], norm, 1 if s['res'] == 1 else 0)
         inp['act'] = s['act'] if s['xf'] else 0
@@ -165,15 +170,45 @@ def shape_ab(shapes, reps):
     return rows
 
 
+def phase_ab(reps):
+    import test_gpu_halo_phase as P
+    c = __import__('gpu_util').ctx()
+    shapes = [s for s in P.CASES if s[1] == 32 or P.CASES.index(s) < 11]
+    paths = (('conv_tc', 0, 0), ('halo', 1, 1), ('auto', 1, 0))          # (label, halo_conv, ksplit)
+    print('\n== four-phase shapes, alone: %d launches each after warm-up (CUDA events); executed TFLOP/s' % reps)
+    print('  %-4s %-24s | %s' % ('kind', 'N HxW cin->cout norm', ' | '.join('%9s %7s' % (p[0] + ' us', 'TFLOP/s') for p in paths)) + ' | ratio')
+    rows = []
+    for s in shapes:
+        kind, N, Cin, H, W, Cout, norm = s
+        inp = P.make_inputs(7, kind, N, Cin, H, W, Cout, norm)
+        flop = 2.0 * N * H * W * 16 * Cin * Cout
+        us = {}
+        try:
+            for label, halo, ksplit in paths:
+                c.set_option('halo_conv', halo)
+                P.conv_phase(**inp, ksplit=ksplit, reps=20)                  # warm-up
+                us[label] = P.conv_phase(**inp, ksplit=ksplit, reps=reps)[3]
+        finally:
+            c.set_option('halo_conv', 1)
+        rows.append((s, us))
+        print('  %-4d %-24s | %s | %6.3f' % (kind, '%d %dx%d %d->%d %s' % (N, H, W, Cin, Cout, norm), ' | '.join(
+            '%9.2f %7.1f' % (us[p[0]], flop / us[p[0]] / 1e6) for p in paths), us['conv_tc'] / us['halo']), flush=True)
+    return rows
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--reps', type=int, default=200)
     ap.add_argument('--out', default=None, help='directory for the profiler traces')
+    ap.add_argument('--phase-only', action='store_true', help='only the four-phase A/B (step 4)')
     args = ap.parse_args()
     assert torch.cuda.is_available(), 'halo_layers.py needs a CUDA device'
     if args.out:
         os.makedirs(args.out, exist_ok=True)
     print('card:', card(), flush=True)
+    if args.phase_only:
+        phase_ab(args.reps)
+        return
     shapes = frame_shapes()
     print('halo launches in the frame: %d (%d unsplit)' % (len(shapes), sum(1 for s in shapes if s['cs'] == 1)), flush=True)
     poser, image, poses = make_teacher()
@@ -181,6 +216,7 @@ def main():
     after = print_frame('automatic tile choice (halo_m256 = -1)', profile_frame(poser, image, poses, -1, args.out))
     print('kernel time per frame: %.1f -> %.1f us (%.3fx)' % (before[0], after[0], before[0] / after[0]), flush=True)
     shape_ab(shapes, args.reps)
+    phase_ab(args.reps)
 
 
 if __name__ == '__main__':

@@ -13,6 +13,10 @@
 //   * weights stream per (chunk, tap) through their own TMA ring, pre-issued ahead of the programmatic-dependency wait;
 //   * K (channel chunks) can be split over a thread-block cluster, partials meeting in distributed shared memory
 //     (same epilogues as conv_tc.cu: conv_tc_device.cuh).
+// The four-phase layers (CONV_UP2_3x3, CONVT_4x4_S2: 4 output phases x 2x2 taps, tap offsets in {-1, 0, 1} on the
+// low-resolution input) run on the same halo: one 8 x 16 low-resolution tile per CTA, its 10 x 18 halo loaded and
+// normalised once per chunk instead of once per (phase, tap) -- 180 rows instead of 16 x 128.  Consumer warpgroup py holds
+// the accumulators of phases (py, 0) and (py, 1); the 16 weight tiles of a chunk alternate between the two warpgroups.
 #include "conv.cuh"
 #include "profiler.cuh"
 #include "conv_tc_device.cuh"
@@ -48,26 +52,39 @@ static_assert((HT_H * HALO_W * 64) % 1024 == 0, "second warpgroup's halo offset 
 // MINB: resident CTAs per SM the register allocation must allow (4 for the single-chunk unsplit variants, whose small
 // rings fit four times: the layers at 256x256 / 512x512 are chains of dependent latencies, more CTAs = more overlap).
 // Two-warpgroup CTAs (BN <= 64): two with BN = 32, as many consumer warps per SM as four one-warpgroup CTAs; one with
-// BN = 64 (two would cap the 288 threads at 96 registers, which spills the 64-column accumulator's epilogue)
-__host__ __device__ constexpr int halo_min_ctas(int bn, int sa, int cs, int op, int wg) {
-    return wg > 1 ? (bn <= 32 ? 2 : 1) : cs > 1 || bn >= 128 ? 1 : ((sa == (op == OP_F16N ? 2 : 1) && bn <= 32) ? 4 : 2);
+// BN = 64 (two would cap the 288 threads at 96 registers, which spills the 64-column accumulator's epilogue).  Four-phase
+// CTAs (two 32-column accumulators per warpgroup) count as BN = 64.
+__host__ __device__ constexpr int halo_min_ctas(int bn, int sa, int cs, int op, int wg, int ph = 1) {
+    return wg > 1 ? (bn * (ph == 4 ? 2 : 1) <= 32 ? 2 : 1) : cs > 1 || bn >= 128 ? 1 : ((sa == (op == OP_F16N ? 2 : 1) && bn <= 32) ? 4 : 2);
 }
+// Weight tile j of a channel chunk, as the third coordinate of the [phase * tap][cout][cin] weight map.  3x3: tap j.
+// Four phases: j = 2 (2 tap + px) + py, so the tiles of the two warpgroups (py) alternate in the ring.
+template <int PH>
+__host__ __device__ constexpr int halo_wtile(int j) { return PH == 1 ? j : ((j & 1) * 2 + ((j >> 1) & 1)) * 4 + (j >> 2); }
+
 // WG: consumer warpgroups (1: 128-pixel tiles, 160 threads; 2: 256-pixel tiles, 288 threads, unsplit only)
-template <int BN, int SA, int SB, int CS, int OP, int XF, int WG>
-__global__ void __launch_bounds__(halo_threads(WG), halo_min_ctas(BN, SA, CS, OP, WG)) conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+// PH: output phases (1: 3x3; 4: four-phase layers, two warpgroups on one 8 x 16 low-resolution tile, unsplit only)
+template <int BN, int SA, int SB, int CS, int OP, int XF, int WG, int PH = 1>
+__global__ void __launch_bounds__(halo_threads(WG), halo_min_ctas(BN, SA, CS, OP, WG, PH)) conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                                                                 const __grid_constant__ CUtensorMap tmO32, const __grid_constant__ CUtensorMap tmO16,
                                                                 const __grid_constant__ CUtensorMap tmR, const TcParams p) {
     static_assert(OP != OP_TF32, "halo kernel: f16 operands");
     static_assert(BN <= 128, "the accumulator of one warpgroup: BN registers per thread");
     static_assert(WG == 1 || (WG == 2 && CS == 1 && BN <= 64), "two consumer warpgroups: unsplit launches, two accumulators of at most 64 columns");
+    // four phases: two 128-row accumulators per warpgroup, no more registers than one 128 x 64 accumulator
+    static_assert(PH == 1 || (PH == 4 && WG == 2 && BN <= 32), "four-phase layers: two warpgroups, two 128 x 32 accumulators each");
+    constexpr int SLABS = PH == 1 ? WG : 1;                              // 16-row slabs of the tile (8 x 16 pixels each)
+    constexpr int NACC = PH == 1 ? 1 : 2;                                // accumulators per warpgroup
+    constexpr int TPC = PH == 1 ? 9 : 16;                                // weight tiles per channel chunk
     constexpr int ROWB = op_row_bytes(OP);
     constexpr int KCE = op_kch(OP);
-    constexpr int HALO_ROWS = halo_rows(WG);
-    constexpr int A_BYTES = halo_a_bytes(ROWB, WG);
+    constexpr int HALO_ROWS = halo_rows(SLABS);
+    constexpr int A_BYTES = halo_a_bytes(ROWB, SLABS);
     constexpr int B_BYTES = BN * ROWB;
     constexpr int PRODUCER_WARP = 4 * WG;
     constexpr int EPI_BYTES = (int)(((size_t)SA * A_BYTES + (size_t)SB * B_BYTES) / WG) & ~1023;      // idle ring per warpgroup in the epilogue
-    constexpr int NSLOT = CS == 1 ? epi_nslot(BN, EPI_BYTES) : 0;     // TMA-store staging slots of the unsplit epilogue
+    // TMA-store staging slots of the unsplit epilogue (none for the phase-strided outputs of the four-phase layers)
+    constexpr int NSLOT = CS == 1 && PH == 1 ? epi_nslot(BN, EPI_BYTES) : 0;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);      // pointer arithmetic (not an integer round trip) keeps the shared address space: LDS / STS, not generic LD / ST
     uint8_t* smA = smem;
@@ -88,18 +105,19 @@ __global__ void __launch_bounds__(halo_threads(WG), halo_min_ctas(BN, SA, CS, OP
     const int tx = tile % p.tiles_x; tile /= p.tiles_x;
     const int ty = tile % p.tiles_y;
     const int n = tile / p.tiles_y;
-    const int x0 = tx * HT_W, y0 = ty * (HT_H * WG);
+    const int x0 = tx * HT_W, y0 = ty * (HT_H * SLABS);
     const int n0 = blockIdx.y * BN;
     const int split = blockIdx.z;                                        // rank in the cluster (CS == gridDim.z)
     const int c_per = (p.cpt + CS - 1) / CS;
     const int cb0 = split * c_per;
     const int nc = max(0, min(p.cpt, cb0 + c_per) - cb0);                // channel chunks of this CTA
-    const int nb = nc * 9;                                               // weight tiles of this CTA
+    const int nb = nc * TPC;                                             // weight tiles of this CTA
 
     if (threadIdx.x == 0) {
         // the empty barriers take one arrival per consumer thread: every thread arrives once its own wgmma wait has returned
+        // (a four-phase weight tile is read by one warpgroup)
         for (int s = 0; s < SA; ++s) { mbar_init(smem_u32(a_full + s), 1); mbar_init(smem_u32(a_empty + s), 128 * WG); }
-        for (int s = 0; s < SB; ++s) { mbar_init(smem_u32(b_full + s), 1); mbar_init(smem_u32(b_empty + s), 128 * WG); }
+        for (int s = 0; s < SB; ++s) { mbar_init(smem_u32(b_full + s), 1); mbar_init(smem_u32(b_empty + s), PH == 1 ? 128 * WG : 128); }
         for (int s = 0; s < 4 * WG; ++s) mbar_init(smem_u32(res_bars + s), 1);
         asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
         asm volatile("prefetch.tensormap [%0];\n" :: "l"(&tmA) : "memory");
@@ -114,28 +132,28 @@ __global__ void __launch_bounds__(halo_threads(WG), halo_min_ctas(BN, SA, CS, OP
         for (int i = 0; i < npre; ++i) {
             const uint32_t full = smem_u32(b_full + i);
             mbar_expect_tx(full, B_BYTES);
-            tma_load_3d(smem_u32(smB + i * B_BYTES), &tmB, (cb0 + i / 9) * KCE, n0, i % 9, full);
+            tma_load_3d(smem_u32(smB + i * B_BYTES), &tmB, (cb0 + i / TPC) * KCE, n0, halo_wtile<PH>(i % TPC), full);
         }
     }
     pdl_wait();
     if (threadIdx.x == 0) HSTAMP(0, 2);
 
-    Acc<BN> acc;
+    Acc<BN> acc[NACC];
     if (nc > 0) {
         if (warp == PRODUCER_WARP) {
-            if (lane == 0) {   // ===== TMA producer: one halo box per chunk, nine weight tiles per chunk =====
+            if (lane == 0) {   // ===== TMA producer: one halo box per chunk, nine (four-phase: sixteen) weight tiles per chunk =====
                 int bi = 0;
                 for (int ci = 0; ci < nc; ++ci) {
                     const int sa = ci % SA;
                     mbar_wait(smem_u32(a_empty + sa), ((ci / SA) & 1) ^ 1);
                     mbar_expect_tx(smem_u32(a_full + sa), HALO_ROWS * ROWB);
                     tma_load_4d(smem_u32(smA + sa * A_BYTES), &tmA, (cb0 + ci) * KCE, x0 - 1, y0 - 1, n, smem_u32(a_full + sa));
-                    for (int tap = 0; tap < 9; ++tap, ++bi) {
+                    for (int tap = 0; tap < TPC; ++tap, ++bi) {
                         if (bi < npre) continue;
                         const int sb = bi % SB;
                         mbar_wait(smem_u32(b_empty + sb), ((bi / SB) & 1) ^ 1);
                         mbar_expect_tx(smem_u32(b_full + sb), B_BYTES);
-                        tma_load_3d(smem_u32(smB + sb * B_BYTES), &tmB, (cb0 + ci) * KCE, n0, tap, smem_u32(b_full + sb));
+                        tma_load_3d(smem_u32(smB + sb * B_BYTES), &tmB, (cb0 + ci) * KCE, n0, halo_wtile<PH>(tap), smem_u32(b_full + sb));
                     }
                 }
             }
@@ -176,43 +194,88 @@ __global__ void __launch_bounds__(halo_threads(WG), halo_min_ctas(BN, SA, CS, OP
                     asm volatile("bar.sync %0, %1;\n" :: "n"(XBAR), "n"(128 * WG) : "memory");
                     if (te == 0 && ci == nc - 1) HSTAMP(2, 2);
                 }
-                const uint32_t a_base = smem_u32(smA + sa * A_BYTES) + (uint32_t)(wg * HT_H * HALO_W * ROWB);
-                // unrolled: the wait depth and the arrivals below depend on the tap only, so no branch separates wgmma issue
-                // from its wait (a data-dependent one makes ptxas serialise the wgmma)
+                const uint32_t a_base = smem_u32(smA + sa * A_BYTES) + (uint32_t)(SLABS > 1 ? wg * HT_H * HALO_W * ROWB : 0);
+                if constexpr (PH == 4) {
+                    // warpgroup py: steps s = 2 tap + px into the accumulator of phase (py, px); its weight tile is tile
+                    // 2 s + py of the chunk.  K order per phase: chunk, then tap (conv_tc: tap, then chunk)
 #pragma unroll
-                for (int tap = 0; tap < 9; ++tap, ++bi) {
-                    const int sb = bi % SB;
-                    mbar_wait(smem_u32(b_full + sb), (bi / SB) & 1);
-                    const int shift = (p.dy[0][tap] + 1) * HALO_W + (p.dx[0][tap] + 1);
-                    // rows 0-63 of the tile are tile rows 0-7 (halo rows from `shift`), rows 64-127 tile rows 8-15 (8 halo pitches on)
-                    const uint32_t a0 = a_base + shift * ROWB, a1 = a0 + 8 * HALO_W * ROWB;
-                    const uint32_t b_addr = smem_u32(smB + sb * B_BYTES);
-                    wg_fence();
+                    for (int s = 0; s < 8; ++s) {
+                        const int tap = s >> 1, px = s & 1, phase = 2 * wg + px;
+                        const int bj = ci * 16 + 2 * s + wg;
+                        const int sb = bj % SB;
+                        mbar_wait(smem_u32(b_full + sb), (bj / SB) & 1);
+                        const int shift = (p.dy[phase][tap] + 1) * HALO_W + (p.dx[phase][tap] + 1);
+                        const uint32_t a0 = a_base + shift * ROWB, a1 = a0 + 8 * HALO_W * ROWB;
+                        const uint32_t b_addr = smem_u32(smB + sb * B_BYTES);
+                        wg_fence();
 #pragma unroll
-                    for (int k = 0; k < ROWB / 32; ++k) {
-                        const uint64_t bd = make_smem_desc_sw<ROWB>(b_addr + 32 * k);
-                        const uint32_t accum = (ci > 0 || tap > 0 || k > 0) ? 1u : 0u;
-                        Wgmma<BN>::f16(acc.d[0], make_desc_sbo<ROWB>(a0 + 32 * k, HALO_W * ROWB), bd, accum);
-                        Wgmma<BN>::f16(acc.d[1], make_desc_sbo<ROWB>(a1 + 32 * k, HALO_W * ROWB), bd, accum);
+                        for (int k = 0; k < ROWB / 32; ++k) {
+                            const uint64_t bd = make_smem_desc_sw<ROWB>(b_addr + 32 * k);
+                            const uint32_t accum = (ci > 0 || tap > 0 || k > 0) ? 1u : 0u;
+                            Wgmma<BN>::f16(acc[px].d[0], make_desc_sbo<ROWB>(a0 + 32 * k, HALO_W * ROWB), bd, accum);
+                            Wgmma<BN>::f16(acc[px].d[1], make_desc_sbo<ROWB>(a1 + 32 * k, HALO_W * ROWB), bd, accum);
+                        }
+                        wg_commit();
+                        if (s < 7) {
+                            wg_wait<1>();                                       // the previous step's weight tile has been read
+                            if (s > 0) mbar_arrive(smem_u32(b_empty + (bj - 2) % SB));
+                        } else {
+                            wg_wait<0>();                                       // the chunk's halo and this warpgroup's last two tiles are free
+                            mbar_arrive(smem_u32(b_empty + (bj - 2) % SB));
+                            mbar_arrive(smem_u32(b_empty + sb));
+                            mbar_arrive(smem_u32(a_empty + sa));
+                        }
                     }
-                    wg_commit();
-                    if (tap < 8) {
-                        wg_wait<1>();                                           // the previous tap's weight tile has been read
-                        if (tap > 0) mbar_arrive(smem_u32(b_empty + (bi - 1) % SB));
-                    } else {
-                        wg_wait<0>();                                           // the chunk's halo and its last two weight tiles are free
-                        mbar_arrive(smem_u32(b_empty + (bi - 1) % SB));
-                        mbar_arrive(smem_u32(b_empty + bi % SB));
-                        mbar_arrive(smem_u32(a_empty + sa));
+                } else {
+                    // unrolled: the wait depth and the arrivals below depend on the tap only, so no branch separates wgmma issue
+                    // from its wait (a data-dependent one makes ptxas serialise the wgmma)
+#pragma unroll
+                    for (int tap = 0; tap < 9; ++tap, ++bi) {
+                        const int sb = bi % SB;
+                        mbar_wait(smem_u32(b_full + sb), (bi / SB) & 1);
+                        const int shift = (p.dy[0][tap] + 1) * HALO_W + (p.dx[0][tap] + 1);
+                        // rows 0-63 of the tile are tile rows 0-7 (halo rows from `shift`), rows 64-127 tile rows 8-15 (8 halo pitches on)
+                        const uint32_t a0 = a_base + shift * ROWB, a1 = a0 + 8 * HALO_W * ROWB;
+                        const uint32_t b_addr = smem_u32(smB + sb * B_BYTES);
+                        wg_fence();
+#pragma unroll
+                        for (int k = 0; k < ROWB / 32; ++k) {
+                            const uint64_t bd = make_smem_desc_sw<ROWB>(b_addr + 32 * k);
+                            const uint32_t accum = (ci > 0 || tap > 0 || k > 0) ? 1u : 0u;
+                            Wgmma<BN>::f16(acc[0].d[0], make_desc_sbo<ROWB>(a0 + 32 * k, HALO_W * ROWB), bd, accum);
+                            Wgmma<BN>::f16(acc[0].d[1], make_desc_sbo<ROWB>(a1 + 32 * k, HALO_W * ROWB), bd, accum);
+                        }
+                        wg_commit();
+                        if (tap < 8) {
+                            wg_wait<1>();                                           // the previous tap's weight tile has been read
+                            if (tap > 0) mbar_arrive(smem_u32(b_empty + (bi - 1) % SB));
+                        } else {
+                            wg_wait<0>();                                           // the chunk's halo and its last two weight tiles are free
+                            mbar_arrive(smem_u32(b_empty + (bi - 1) % SB));
+                            mbar_arrive(smem_u32(b_empty + bi % SB));
+                            mbar_arrive(smem_u32(a_empty + sa));
+                        }
                     }
                 }
             }
-            wg_fence_acc(acc.d[0]); wg_fence_acc(acc.d[1]);
+#pragma unroll
+            for (int a = 0; a < NACC; ++a) { wg_fence_acc(acc[a].d[0]); wg_fence_acc(acc[a].d[1]); }
             if (te == 0) { HSTAMP(1, 1); HSTAMP(2, 3); }
             // the epilogue reuses the ring: with two warpgroups, the other one may still be reading its last stages
             if constexpr (WG > 1) asm volatile("bar.sync 3, 256;\n" ::: "memory");
-            if (CS == 1) epi_direct<BN, HT_W, NSLOT, WG>(p, acc, smem + wg * EPI_BYTES, n, y0 + wg * HT_H, x0, n0, 0, 0, warp, lane,
-                                                         &tmO32, &tmO16, &tmR, res_bars + 4 * wg, wg, EPI_BYTES);
+            if constexpr (PH == 4) {
+                // phase (wg, px) of the low-resolution tile: output pixels (2 y + wg, 2 x + px), plain stores
+#pragma unroll
+                for (int px = 0; px < 2; ++px) {
+                    // the statistics fold of the first call reads both warpgroups' partials before the second rewrites them
+                    if (px > 0) asm volatile("bar.sync 3, 256;\n" ::: "memory");
+                    epi_direct<BN, HT_W, 0, WG>(p, acc[px], smem + wg * EPI_BYTES, n, y0, x0, n0, 2 * wg + px, 0, warp, lane,
+                                                nullptr, nullptr, nullptr, nullptr, wg, EPI_BYTES);
+                }
+            } else if (CS == 1) {
+                epi_direct<BN, HT_W, NSLOT, WG>(p, acc[0], smem + wg * EPI_BYTES, n, y0 + wg * HT_H, x0, n0, 0, 0, warp, lane,
+                                                &tmO32, &tmO16, &tmR, res_bars + 4 * wg, wg, EPI_BYTES);
+            }
             if (te == 0) HSTAMP(2, 4);
         }
     }
@@ -221,7 +284,7 @@ __global__ void __launch_bounds__(halo_threads(WG), halo_min_ctas(BN, SA, CS, OP
         asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
         asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
         if (threadIdx.x == 0) HSTAMP(2, 5);
-        if (warp < PRODUCER_WARP && nc > 0) epi_push_partial<BN, CS>(acc, smem, split, warp, lane);
+        if (warp < PRODUCER_WARP && nc > 0) epi_push_partial<BN, CS>(acc[0], smem, split, warp, lane);
         // barrier B: the pushed slices are visible to their owners; nobody touches a peer's memory afterwards
         asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
         asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
@@ -272,12 +335,12 @@ const CUtensorMap& halo_activation_map(const View& v, int op, int wg) {
 }
 
 const CUtensorMap& halo_weight_map(const ConvWeights& cw, int bn, int op) {
-    HKey key{current_device(), cw.w16, cw.cin_pad, cw.cout_pad, cw.ntaps, bn, -1, op};
+    HKey key{current_device(), cw.w16, cw.cin_pad, cw.cout_pad, cw.ntaps * cw.nphase, bn, -1, op};
     std::lock_guard<std::mutex> lock(g_halo_mu);
     auto it = g_halo_maps.find(key);
     if (it != g_halo_maps.end()) return it->second;
     CUtensorMap m;
-    cuuint64_t dims[3] = {(cuuint64_t)cw.cin_pad, (cuuint64_t)cw.cout_pad, (cuuint64_t)cw.ntaps};
+    cuuint64_t dims[3] = {(cuuint64_t)cw.cin_pad, (cuuint64_t)cw.cout_pad, (cuuint64_t)cw.ntaps * cw.nphase};
     cuuint64_t strides[2] = {(cuuint64_t)cw.cin_pad * 2, (cuuint64_t)cw.cout_pad * cw.cin_pad * 2};
     cuuint32_t box[3] = {(cuuint32_t)op_kch(op), (cuuint32_t)bn, 1};
     cuuint32_t es[3] = {1, 1, 1};
@@ -319,9 +382,16 @@ struct HaloPlan { int bn, tiles_x, tiles_y, tiles_m, tiles_n, cs, chunks, wg; };
 
 HaloPlan halo_plan(const ConvWeights& cw, const ConvArgs& a, int op) {
     HaloPlan pl;
+    pl.chunks = cw.cin_pad / op_kch(op);
+    if (cw.nphase == 4) {
+        // one 8 x 16 low-resolution tile (4 x 128 output pixels) x 32 columns per CTA, unsplit
+        pl.tiles_x = ceil_div(a.in.W, HT_W); pl.tiles_y = ceil_div(a.in.H, HT_H);
+        pl.tiles_m = pl.tiles_x * pl.tiles_y * a.in.N;
+        pl.bn = 32; pl.tiles_n = cw.cout_pad / 32; pl.cs = 1; pl.wg = 2;
+        return pl;
+    }
     pl.tiles_x = ceil_div(a.out.W, HT_W); pl.tiles_y = ceil_div(a.out.H, HT_H);
     pl.tiles_m = pl.tiles_x * pl.tiles_y * a.in.N;
-    pl.chunks = cw.cin_pad / op_kch(op);
     // N tile: at most 128 columns, the accumulator of one consumer warpgroup (BN fp32 registers per thread)
     pl.bn = (cw.cout_pad % 128 == 0) ? 128 : (cw.cout_pad % 64 == 0 ? 64 : 32);
     const int sms = num_sms();
@@ -361,19 +431,19 @@ HaloPlan halo_plan(const ConvWeights& cw, const ConvArgs& a, int op) {
     return pl;
 }
 
-template <int OP, int BN, int SA, int SB, int CS, int XF, int WG = 1>
+template <int OP, int BN, int SA, int SB, int CS, int XF, int WG = 1, int PH = 1>
 void launch_halo(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo32, const CUtensorMap& mo16, const CUtensorMap& mr, const TcParams& p, dim3 grid, cudaStream_t s) {
     constexpr int ROWB = op_row_bytes(OP);
-    constexpr size_t ring = (size_t)SA * halo_a_bytes(ROWB, WG) + (size_t)SB * BN * ROWB;
+    constexpr size_t ring = (size_t)SA * halo_a_bytes(ROWB, PH == 1 ? WG : 1) + (size_t)SB * BN * ROWB;
     constexpr size_t smem0 = 1024 + ring + (2 * SA + 2 * SB + 4 * WG) * 8 + 16;
     static_assert(smem0 <= 227 * 1024, "shared memory budget");
     static_assert(ring / WG >= (size_t)4 * 32 * 33 * 4 + 4 * BN * 8, "epilogue scratch must fit in the pipeline buffers");
-    static_assert(WG == 1 || epi_nslot(BN, (ring / WG) & ~(size_t)1023) > 0, "two warpgroups: a TMA-store staging slot each");
+    static_assert(WG == 1 || PH == 4 || epi_nslot(BN, (ring / WG) & ~(size_t)1023) > 0, "two warpgroups: a TMA-store staging slot each");
     static_assert(CS == 1 || ring >= (size_t)128 * BN * 4 + 128 * 8 * 4 + 128 * 4 * 4, "partial tile + statistics scratch must fit");
     const size_t smem = smem0 + (XF ? (size_t)24 * p.xf_C + 32 : 0);
     THA4_REQUIRE(smem <= 227 * 1024, "conv_halo: shared memory budget (fused input normalisation)");
-    THA4_ENSURE_SMEM((conv_halo_kernel<BN, SA, SB, CS, OP, XF, WG>), smem);
-    launch_pdl(conv_halo_kernel<BN, SA, SB, CS, OP, XF, WG>, grid, dim3(halo_threads(WG)), smem, s, CS, ma, mb, mo32, mo16, mr, p);
+    THA4_ENSURE_SMEM((conv_halo_kernel<BN, SA, SB, CS, OP, XF, WG, PH>), smem);
+    launch_pdl(conv_halo_kernel<BN, SA, SB, CS, OP, XF, WG, PH>, grid, dim3(halo_threads(WG)), smem, s, CS, ma, mb, mo32, mo16, mr, p);
     THA4_LAUNCH_CHECK();
 }
 
@@ -437,10 +507,21 @@ void conv_halo_set_m256(int mode) { g_halo_m256 = mode; }
 
 bool conv_halo_supported(const ConvWeights& cw, const ConvArgs& a) {
     if (!g_use_halo || !conv_tc_supported(cw, a)) return false;
-    if (!a.in.f16 || cw.ntaps != 9 || cw.nphase != 1 || cw.stride != 1 || cw.out_mul != 1) return false;
-    for (int t = 0; t < 9; ++t)
-        if (cw.dy[0][t] < -1 || cw.dy[0][t] > 1 || cw.dx[0][t] < -1 || cw.dx[0][t] > 1) return false;
-    return a.in.H == a.out.H && a.in.W == a.out.W;
+    if (!a.in.f16 || cw.stride != 1) return false;
+    const bool four_phase = cw.nphase == 4 && cw.ntaps == 4 && cw.out_mul == 2;
+    if (!four_phase && (cw.ntaps != 9 || cw.nphase != 1 || cw.out_mul != 1)) return false;
+    for (int ph = 0; ph < cw.nphase; ++ph)
+        for (int t = 0; t < cw.ntaps; ++t)
+            if (cw.dy[ph][t] < -1 || cw.dy[ph][t] > 1 || cw.dx[ph][t] < -1 || cw.dx[ph][t] > 1) return false;
+    if (!four_phase) return a.in.H == a.out.H && a.in.W == a.out.W;
+    // four phases: 64-channel chunks only (the layers of the networks), unsplit.  An explicit split goes to conv_tc.cu
+    if (cw.cin_pad % 64 != 0 || a.ksplit > 1 || a.out.H != 2 * a.in.H || a.out.W != 2 * a.in.W) return false;
+    // The automatic plan takes the halo kernel from 64 CTAs (8 x 16 x 32 tiles) up.  Measured alone on an H100 SXM (132 SMs)
+    // it ran 1.1 - 2.5x faster than conv_tc.cu's launches on every such layer of the teacher frame and at batch 32; with
+    // 16 - 48 CTAs (the 16^2 - 32^2 low-resolution layers of 256 - 512 channels) conv_tc.cu's cluster split-K was as fast
+    // or faster (0.55 - 1.02x).
+    const HaloPlan pl = halo_plan(cw, a, OP_F16);
+    return a.ksplit == 1 || (long)pl.tiles_m * pl.tiles_n >= 64;
 }
 
 bool conv_halo_fuses_stats(const ConvWeights&, const ConvArgs&) { return true; }       // unsplit or cluster split: always final
@@ -467,15 +548,17 @@ void conv_halo_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s)
     p.bias = cw.bias;
     p.res = a.res.p; p.res_mode = a.res.p ? a.res_mode : RES_NONE;
     p.resH = a.res.H; p.resW = a.res.W; p.res_ld = a.res.ld;
-    p.N = a.in.N; p.out_mul = 1; p.in_mul = 1;
+    p.N = a.in.N; p.out_mul = cw.out_mul; p.in_mul = 1;
     const HaloPlan pl = halo_plan(cw, a, op);
-    p.MH = a.out.H; p.MW = a.out.W; p.tiles_x = pl.tiles_x; p.tiles_y = pl.tiles_y;
+    p.MH = a.out.H / cw.out_mul; p.MW = a.out.W / cw.out_mul; p.tiles_x = pl.tiles_x; p.tiles_y = pl.tiles_y;
     p.pre_b = cw.dynamic ? 0 : 1;
-    p.ntaps = 9; p.cpt = pl.chunks;
+    p.ntaps = cw.ntaps; p.cpt = pl.chunks;
     if (!cw.w16) { conv_make_half(cw, s); p.pre_b = 0; }
     p.acc_scale = 1.0f / cw.w16_scale;
-    for (int t = 0; t < 9; ++t) { p.dy[0][t] = cw.dy[0][t]; p.dx[0][t] = cw.dx[0][t]; }
-    p.ph_oy[0] = 0; p.ph_ox[0] = 0;
+    for (int ph = 0; ph < cw.nphase; ++ph) {
+        p.ph_oy[ph] = cw.ph_oy[ph]; p.ph_ox[ph] = cw.ph_ox[ph];
+        for (int t = 0; t < cw.ntaps; ++t) { p.dy[ph][t] = cw.dy[ph][t]; p.dx[ph][t] = cw.dx[ph][t]; }
+    }
     p.ksplit = 1;                                    // the epilogues' "split-K through a workspace / atomics" modes are not used here
     p.ws = nullptr;
     p.stats = a.out.stats; p.stats_ld = a.out.stats_ld;
@@ -487,14 +570,14 @@ void conv_halo_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s)
         p.dbg = g_dbg_buf;
     }
     ProfScope prof(PROF_CONV, s);
-    prof_add_work(PROF_CONV, 2.0 * (double)p.N * p.MH * p.MW * cw.cout * cw.cin * 9, 0.0);
-    const CUtensorMap& ma = halo_activation_map(a.in, op, pl.wg);
+    prof_add_work(PROF_CONV, 2.0 * (double)p.N * p.MH * p.MW * cw.cout * cw.cin * cw.ntaps * cw.nphase, 0.0);
+    const CUtensorMap& ma = halo_activation_map(a.in, op, cw.nphase == 1 ? pl.wg : 1);
     const CUtensorMap& mb = halo_weight_map(cw, pl.bn, op);
     const CUtensorMap* mo32 = &ma;                   // placeholders when an output does not leave through TMA
     const CUtensorMap* mo16 = &ma;
     const CUtensorMap* mr = &ma;
     p.st_tma = 0;
-    if (pl.cs == 1 && g_tma_store) {
+    if (pl.cs == 1 && g_tma_store && cw.nphase == 1) {
         if (a.out.p && halo_store_map(a.out, false, &mo32)) p.st_tma |= 1;
         if (a.out16.p && halo_store_map(a.out16, true, &mo16)) p.st_tma |= 2;
         // the residual of a ResBlock's second conv has the geometry of the fp32 output: it arrives through the same box
@@ -504,7 +587,11 @@ void conv_halo_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s)
     p.vec4 = ((!cw.bias || (reinterpret_cast<uintptr_t>(cw.bias) & 15) == 0) &&
               (!a.res.p || ((reinterpret_cast<uintptr_t>(a.res.p) & 15) == 0 && a.res.ld % 4 == 0))) ? 1 : 0;
     dim3 grid(pl.tiles_m, pl.tiles_n, pl.cs);
-    if (op == OP_F16) {
+    if (cw.nphase == 4) {
+        // OP_F16 (conv_halo_supported).  One CTA per SM: the ring takes two halo stages and a whole chunk of weight tiles
+        if (a.nin.on) launch_halo<OP_F16, 32, 2, 16, 1, 1, 2, 4>(ma, mb, *mo32, *mo16, *mr, p, grid, s);
+        else launch_halo<OP_F16, 32, 2, 16, 1, 0, 2, 4>(ma, mb, *mo32, *mo16, *mr, p, grid, s);
+    } else if (op == OP_F16) {
         if (a.nin.on) launch_halo_bn<OP_F16, 1>(pl.bn, pl.cs, pl.wg, ma, mb, *mo32, *mo16, *mr, p, grid, s);
         else launch_halo_bn<OP_F16, 0>(pl.bn, pl.cs, pl.wg, ma, mb, *mo32, *mo16, *mr, p, grid, s);
     } else {
@@ -513,9 +600,9 @@ void conv_halo_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s)
     }
     static const bool dbg_all = dbg_env && !strcmp(getenv("THA4_HALO_DEBUG"), "2");
     if (dbg_all) {       // developer: stamps of every launch of a real forward (serialises the stream)
-        fprintf(stderr, "halo launch: N %d %dx%d cin %d cout %d | bn %d cs %d wg %d chunks %d grid %d x %d | xf %d groups %d act %d res %d out32 %d out16 %d st_tma %d\n",
+        fprintf(stderr, "halo launch: N %d %dx%d cin %d cout %d | bn %d cs %d wg %d chunks %d grid %d x %d | xf %d groups %d act %d res %d out32 %d out16 %d st_tma %d | phases %d\n",
                 p.N, p.MH, p.MW, cw.cin, cw.cout, pl.bn, pl.cs, pl.wg, pl.chunks, pl.tiles_m, pl.tiles_n, a.nin.on ? 1 : 0, p.xf_groups, p.xf_act,
-                p.res_mode, p.out ? 1 : 0, p.out16 ? 1 : 0, p.st_tma);
+                p.res_mode, p.out ? 1 : 0, p.out16 ? 1 : 0, p.st_tma, cw.nphase);
         conv_halo_debug_dump();
     }
 }

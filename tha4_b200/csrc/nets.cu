@@ -182,6 +182,9 @@ Tens make_act(Pool* pool, Runtime& rt, int N, int H, int W, int C, bool want_f32
     if (want_f16) a.h = make_view16(pool, N, H, W, C);
     return a;
 }
+// `a` without its fp32 copy (geometry and statistics slot kept): a conv writing it stores the f16 copy and the statistics
+// only.  For tensors whose consumers read the data in f16 and the fp32 copy's statistics only.
+Tens f16_only(Tens a) { a.f.p = nullptr; return a; }
 Tens slice_act(const Tens& a, int c0, int c) {
     Tens r;
     if (a.f.p) r.f = a.f.slice(c0, c);
@@ -681,7 +684,11 @@ struct UNetFused {
     // ResBlock (unet.py:154-165).  mode: 0 same, 1 up (nearest x2), 2 down (AvgPool2d(2)).
     void res_block(const ResBlockW& w, const Tens& x, int mode, const Tens& out) {
         rt.scratch->reset();
-        THA4_REQUIRE(x.f.C == w.cin && out.f.C == w.cout && x.f.p && x.h.p, "res_block: stream tensors carry both precisions");
+        // x's fp32 data feeds the down-sampling norm pass or the residual (a block with a 1x1 skip adds skip(x) instead);
+        // its f16 copy feeds conv0 (mode 0, 1) and the skip conv
+        const bool reads_f32 = mode == 2 || !w.has_skip, reads_f16 = mode != 2 || w.has_skip;
+        THA4_REQUIRE(x.f.C == w.cin && out.f.C == w.cout && (x.f.p || !reads_f32) && (x.h.p || !reads_f16),
+                     "res_block: the input lacks a precision the block reads");
         const int B = x.f.N;
         const int act = ACT_SILU_FAST;
         Tens h0 = make_act(rt.scratch, rt, B, out.f.H, out.f.W, w.cout, false, true);
@@ -787,6 +794,7 @@ void UNetNet::forward_fused(Runtime& rt, const ImgView& image, const float* coar
         ch_h[j] = (j == 0) ? mc_ * mults_[L_ - 1] : ((j & 1) ? mc_ * mults_[lvl] : mc_ * mults_[lvl + 1]);
         const int cs = hs_ch[NH - 1 - j];
         THA4_REQUIRE(ch_h[j] + cs == up_res_[j].cin, "unet: concat plan does not match weights");
+        THA4_REQUIRE(up_res_[j].has_skip, "unet: an up ResBlock reads its concatenation through a 1x1 skip (no fp32 residual)");
         cat[j] = make_act(P, rt, B, sp, sp, ch_h[j] + cs, true, true);
         hs[NH - 1 - j] = slice_act(cat[j], ch_h[j], cs);
     }
@@ -805,14 +813,15 @@ void UNetNet::forward_fused(Runtime& rt, const ImgView& image, const float* coar
         }
         cur = hs[2 * i + 1];
         if (i < L_ - 1) {
-            F.res_block(down_ds_[i], cur, 2, hs[2 * i + 2]);
-            cur = hs[2 * i + 2];
+            // read by the next ResBlock and, through cat, by an up ResBlock: in fp32 only as the former's residual
+            cur = down_res_[i + 1].has_skip ? f16_only(hs[2 * i + 2]) : hs[2 * i + 2];
+            F.res_block(down_ds_[i], hs[2 * i + 1], 2, cur);
         }
     }
     // ---- middle: Res, Attn, Res, Attn, Res, Attn, Res (unet.py:481-498) ----
     for (int j = 0; j < 4; ++j) {
         const bool last = (j == 3);
-        Tens r = last ? slice_act(cat[0], 0, ch_h[0]) : make_act(P, rt, B, cur.f.H, cur.f.W, cur.f.C, true, true);
+        Tens r = last ? f16_only(slice_act(cat[0], 0, ch_h[0])) : make_act(P, rt, B, cur.f.H, cur.f.W, cur.f.C, true, true);
         F.res_block(mid_res_[j], cur, 0, r);
         cur = r;
         if (!last) {
@@ -822,14 +831,17 @@ void UNetNet::forward_fused(Runtime& rt, const ImgView& image, const float* coar
         }
     }
     // ---- up path (unet.py:540-544) ----
+    // The up half of cat[j] is read by up ResBlock j only, which has a 1x1 skip (cin = both halves): f16 and statistics.
+    // The second block of a level feeds the up-sampler (fp32 residual) or, at the top, the tail (f16 on the wgmma tail).
+    const bool tc_tail = tail_.w16 != nullptr;
     Tens feat;
     for (int j = 0; j < NH; ++j) {
         const int lvl = L_ - 1 - j / 2;
         const bool second = (j & 1);
         const int co = up_res_[j].cout;
         Tens dst;
-        if (!second) dst = slice_act(cat[j + 1], 0, ch_h[j + 1]);
-        else dst = make_act(P, rt, B, cat[j].f.H, cat[j].f.W, co, true, true);   // goes to the upsampler or is the final feature
+        if (!second) dst = f16_only(slice_act(cat[j + 1], 0, ch_h[j + 1]));
+        else dst = make_act(P, rt, B, cat[j].f.H, cat[j].f.W, co, lvl > 0 || !tc_tail, true);   // goes to the upsampler or is the final feature
         if (lvl == L_ - 1) {
             Tens tmp = make_act(P, rt, B, cat[j].f.H, cat[j].f.W, co, true, true);
             F.res_block(up_res_[j], cat[j], 0, tmp);
@@ -838,14 +850,14 @@ void UNetNet::forward_fused(Runtime& rt, const ImgView& image, const float* coar
             F.res_block(up_res_[j], cat[j], 0, dst);
         }
         if (second) {
-            if (lvl > 0) F.res_block(up_us_[L_ - 1 - lvl], dst, 1, slice_act(cat[j + 1], 0, ch_h[j + 1]));
+            if (lvl > 0) F.res_block(up_us_[L_ - 1 - lvl], dst, 1, f16_only(slice_act(cat[j + 1], 0, ch_h[j + 1])));
             else feat = dst;
         }
     }
     // ---- last: GroupNorm + SiLU pending, applied inside the fused tail (unet.py:526-529; morpher_00.py:53-58) ----
     rt.scratch->reset();
     ImgView none{};
-    if (tail_.w16 != nullptr && feat.h.ld == feat.h.C) {
+    if (tc_tail) {
         View fv = feat.h;
         fv.stats = feat.f.stats; fv.stats_ld = feat.f.stats_ld; fv.stats_rep = feat.f.stats_rep; fv.stats_rep_stride = feat.f.stats_rep_stride;
         NormSpecTail ns; ns.groups = 32; ns.act = ACT_SILU_FAST; ns.gamma = last_n_.gamma; ns.beta = last_n_.beta;
