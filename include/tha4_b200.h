@@ -150,6 +150,17 @@ int64_t tha4_siren_face_morpher_param_count(void);
 int tha4_siren_face_morpher_train_step(tha4_ctx* ctx, const float* pose, int pose_ld, const float* target, const float* mask,
                                        const float* loss_weights, const float* params, float* grads, double* host_loss_means,
                                        int B, void* stream);
+/* ---- parameter gradients of the students for arbitrary upstream gradients (backward of the modules under torch.autograd) ---- */
+/* dL/d params of SirenMorpher03 at (image [B,4,512,512], pose [B,45]) for upstream gradients grad_outputs[5] =
+ * d blended, d alpha, d color_change, d warped, d grid_change (NCHW fp32, contiguous; NULL = zero).
+ * params / grads: flat fp32 in state_dict order (331 567); grads is overwritten.  The forward is recomputed (TF32
+ * products, as in tha4_siren_morpher_train_step).  Any B >= 1 (micro-batches of <= 8). */
+int tha4_siren_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
+                                const float* const* grad_outputs, const float* params, float* grads, void* stream);
+/* same for SirenFaceMorpher00: pose [B, >= 39] rows pose_ld apart, grad_output [B,4,128,128] (121 476 params;
+ * micro-batches of <= 64) */
+int tha4_siren_face_morpher_backward(tha4_ctx* ctx, const float* pose, int pose_ld, int B, const float* grad_output,
+                                     const float* params, float* grads, void* stream);
 /* torch.optim.Adam step on flat buffers (shion/base/optimizer_factories.py:9-17); grads are scaled by grad_scale first
  * (1/world_size after a summing all-reduce = DDP's gradient averaging) */
 int tha4_adam_step(tha4_ctx* ctx, float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t n, float lr,

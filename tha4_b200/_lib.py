@@ -26,6 +26,7 @@ EXPORTED_SYMBOLS = [
     'tha4_morpher_forward', 'tha4_upscaler_forward', 'tha4_siren_face_morpher_forward', 'tha4_siren_morpher_forward',
     'tha4_teacher_forward', 'tha4_student_forward', 'tha4_student_forward_io', 'tha4_siren_morpher_param_count', 'tha4_siren_morpher_train_step',
     'tha4_siren_face_morpher_param_count', 'tha4_siren_face_morpher_train_step',
+    'tha4_siren_morpher_backward', 'tha4_siren_face_morpher_backward',
     'tha4_adam_step', 'tha4_images_differ', 'tha4_frame_to_srgb8', 'tha4_rgba8_to_poser_image', 'tha4_grid_sample', 'tha4_resize_bilinear',
     'tha4_base_grid', 'tha4_test_conv', 'tha4_test_conv_norm', 'tha4_test_conv_norm_ex', 'tha4_test_norm', 'tha4_test_tail', 'tha4_test_attention', 'tha4_test_linear',
     'tha4_test_siren_level', 'tha4_test_sine', 'tha4_test_siren_plan_check',
@@ -218,12 +219,20 @@ class Context:
         self._call('tha4_siren_face_morpher_forward', _ptr(pose), 39, B, _ptr(out), self._stream())
         return out
 
+    SIREN_MORPHER_SPECS = [(4, 512), (1, 512), (4, 512), (4, 512), (2, 512)]
+
     def siren_morpher(self, image: Tensor, pose: Tensor) -> List[Tensor]:
+        B = image.shape[0]
+        return self.siren_morpher_into(image, pose, self._empty(self.SIREN_MORPHER_SPECS, B))
+
+    def siren_morpher_into(self, image: Tensor, pose: Tensor, outs: List[Tensor]) -> List[Tensor]:
+        """SirenMorpher03 forward into caller-allocated contiguous outputs (shapes SIREN_MORPHER_SPECS)."""
         image = _check_input(image, self.device, 'image')
         pose = _check_input(pose, self.device, 'pose')
         B = image.shape[0]
         assert image.shape[1:] == (4, 512, 512) and pose.shape == (B, 45)
-        outs = self._empty([(4, 512), (1, 512), (4, 512), (4, 512), (2, 512)], B)
+        for o, (c, s) in zip(outs, self.SIREN_MORPHER_SPECS):
+            assert o.shape == (B, c, s, s) and o.is_contiguous() and o.dtype == torch.float32 and o.device == self.device
         self._call('tha4_siren_morpher_forward', _ptr(image), _ptr(pose), 45, B, _ptr_array(outs), self._stream())
         return outs
 
@@ -315,6 +324,36 @@ class Context:
         self._call('tha4_siren_face_morpher_train_step', _ptr(pose), int(pose.shape[1]), _ptr(target), _ptr(mask), w, _ptr(params),
                    _ptr(grads), losses if want_losses else None, B, self._stream())
         return list(losses) if want_losses else None
+
+    def siren_morpher_backward(self, image: Tensor, pose: Tensor, grad_outputs: Sequence[Optional[Tensor]], params: Tensor,
+                               grads: Tensor):
+        """grads <- dL/d params of SirenMorpher03 (flat, state_dict order) for the upstream gradients of its five outputs
+        (None = zero); the forward is recomputed with TF32 products as in the train step.  Any batch size."""
+        image = _check_input(image, self.device, 'image')
+        pose = _check_input(pose, self.device, 'pose')
+        B = image.shape[0]
+        assert image.shape[1:] == (4, 512, 512) and pose.shape == (B, 45) and len(grad_outputs) == 5
+        gs = []
+        for (c, s), g, name in zip(self.SIREN_MORPHER_SPECS, grad_outputs, ('blended', 'alpha', 'color_change', 'warped', 'grid_change')):
+            if g is not None:
+                g = _check_input(g, self.device, 'grad of ' + name)
+                assert g.shape == (B, c, s, s), (name, tuple(g.shape))
+            gs.append(g)
+        assert params.is_contiguous() and grads.is_contiguous() and params.dtype == torch.float32 and grads.dtype == torch.float32
+        assert params.numel() == grads.numel() == self.lib.tha4_siren_morpher_param_count()
+        self._call('tha4_siren_morpher_backward', _ptr(image), _ptr(pose), 45, B, _ptr_array(gs), _ptr(params), _ptr(grads),
+                   self._stream())
+
+    def siren_face_morpher_backward(self, pose: Tensor, grad_output: Tensor, params: Tensor, grads: Tensor):
+        """grads <- dL/d params of SirenFaceMorpher00 for the upstream gradient [B,4,128,128] of its output."""
+        pose = _check_input(pose, self.device, 'pose')
+        grad_output = _check_input(grad_output, self.device, 'grad_output')
+        B = pose.shape[0]
+        assert pose.shape[1] >= 39 and grad_output.shape == (B, 4, 128, 128)
+        assert params.is_contiguous() and grads.is_contiguous() and params.dtype == torch.float32 and grads.dtype == torch.float32
+        assert params.numel() == grads.numel() == self.lib.tha4_siren_face_morpher_param_count()
+        self._call('tha4_siren_face_morpher_backward', _ptr(pose), int(pose.shape[1]), B, _ptr(grad_output), _ptr(params), _ptr(grads),
+                   self._stream())
 
     def adam_step(self, params: Tensor, grads: Tensor, exp_avg: Tensor, exp_avg_sq: Tensor, lr: float, step: int,
                   betas=(0.9, 0.999), eps: float = 1e-8, grad_scale: float = 1.0):

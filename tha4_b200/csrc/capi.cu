@@ -581,6 +581,44 @@ int tha4_siren_face_morpher_train_step(tha4_ctx* ctx, const float* pose, int pos
     });
 }
 
+int tha4_siren_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
+                                const float* const* grad_outputs, const float* params, float* grads, void* stream) {
+    return guarded(ctx, [&] {
+        THA4_REQUIRE(B >= 1, "student backward: batch must be >= 1");
+        THA4_REQUIRE(pose_ld >= 45, "student backward: pose rows need at least 45 entries");
+        cudaStream_t s = (cudaStream_t)stream;
+        Runtime rt = make_rt(ctx, stream);
+        THA4_CUDA_CHECK(cudaMemsetAsync(grads, 0, siren_body_param_count() * sizeof(float), s));
+        const int ch[5] = {4, 1, 4, 4, 2};
+        for (int n0 = 0; n0 < B; n0 += SIREN_BODY_MAX_BATCH) {       // micro-batches share the workspace and accumulate
+            const int b = std::min(SIREN_BODY_MAX_BATCH, B - n0);
+            begin_pass(ctx, s);
+            const float* g[5];
+            for (int i = 0; i < 5; ++i)
+                g[i] = (grad_outputs && grad_outputs[i]) ? grad_outputs[i] + (size_t)n0 * ch[i] * 512 * 512 : nullptr;
+            siren_body_backward(rt, make_img(image + (size_t)n0 * 4 * 512 * 512, b, 4, 512, 512), pose + (size_t)n0 * pose_ld, pose_ld, g,
+                                params, grads);
+        }
+    });
+}
+
+int tha4_siren_face_morpher_backward(tha4_ctx* ctx, const float* pose, int pose_ld, int B, const float* grad_output,
+                                     const float* params, float* grads, void* stream) {
+    return guarded(ctx, [&] {
+        THA4_REQUIRE(B >= 1, "face student backward: batch must be >= 1");
+        THA4_REQUIRE(pose_ld >= 39, "face student backward: pose rows need at least 39 entries");
+        THA4_REQUIRE(grad_output != nullptr, "face student backward: grad_output is required");
+        cudaStream_t s = (cudaStream_t)stream;
+        Runtime rt = make_rt(ctx, stream);
+        THA4_CUDA_CHECK(cudaMemsetAsync(grads, 0, siren_face_param_count() * sizeof(float), s));
+        for (int n0 = 0; n0 < B; n0 += SIREN_FACE_MAX_BATCH) {
+            const int b = std::min(SIREN_FACE_MAX_BATCH, B - n0);
+            begin_pass(ctx, s);
+            siren_face_backward(rt, pose + (size_t)n0 * pose_ld, pose_ld, b, grad_output + (size_t)n0 * 4 * 128 * 128, params, grads);
+        }
+    });
+}
+
 int tha4_adam_step(tha4_ctx* ctx, float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t n, float lr,
                    float beta1, float beta2, float eps, int step, float grad_scale, void* stream) {
     return guarded(ctx, [&] { adam_step(params, grads, exp_avg, exp_avg_sq, (long)n, lr, beta1, beta2, eps, step, grad_scale, (cudaStream_t)stream); });

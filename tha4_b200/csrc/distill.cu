@@ -199,6 +199,47 @@ __global__ void pad_bias_kernel(const float* __restrict__ b, int nreal, int npad
     if (i < npad) dst[i] = i < nreal ? b[i] : 0.0f;
 }
 
+// Bilinear sample of one pixel at base + grid change (the arithmetic of gridsample.cuh), with what its backward needs.
+// mx / my: d(ix)/d(grid_x), d(iy)/d(grid_y) = R/2 inside the image, 0 where the border clamp is active (ATen
+// clip_coordinates_set_grad).  Out-of-range corners read as 0.
+struct SampleAt {
+    int x0, y0;
+    bool xin, yin;
+    float tx, ty, mx, my;
+};
+__device__ __forceinline__ SampleAt sample_locate(const float* __restrict__ base, int x, int y, float gcx, float gcy, int R) {
+    SampleAt s;
+    const float ixu = __fdiv_rn(__fsub_rn(__fmul_rn(__fadd_rn(__fadd_rn(base[x], gcx), 1.0f), (float)R), 1.0f), 2.0f);
+    const float iyu = __fdiv_rn(__fsub_rn(__fmul_rn(__fadd_rn(__fadd_rn(base[y], gcy), 1.0f), (float)R), 1.0f), 2.0f);
+    const float ix = fminf((float)(R - 1), fmaxf(ixu, 0.0f)), iy = fminf((float)(R - 1), fmaxf(iyu, 0.0f));
+    s.mx = (ixu <= 0.0f || ixu >= (float)(R - 1)) ? 0.0f : 0.5f * R;
+    s.my = (iyu <= 0.0f || iyu >= (float)(R - 1)) ? 0.0f : 0.5f * R;
+    const float fx = floorf(ix), fy = floorf(iy);
+    s.x0 = (int)fx; s.y0 = (int)fy;
+    s.xin = s.x0 + 1 < R; s.yin = s.y0 + 1 < R;
+    s.tx = ix - fx; s.ty = iy - fy;
+    return s;
+}
+// the four corners of one channel plane `im` (row stride sh), the sampled value and its derivatives w.r.t. ix and iy
+struct Corners { float v00, v01, v10, v11; };
+__device__ __forceinline__ Corners sample_corners(const float* im, long sh, const SampleAt& s) {
+    Corners v;
+    v.v00 = im[(long)s.y0 * sh + s.x0];
+    v.v01 = s.xin ? im[(long)s.y0 * sh + s.x0 + 1] : 0.0f;
+    v.v10 = s.yin ? im[(long)(s.y0 + 1) * sh + s.x0] : 0.0f;
+    v.v11 = (s.xin && s.yin) ? im[(long)(s.y0 + 1) * sh + s.x0 + 1] : 0.0f;
+    return v;
+}
+__device__ __forceinline__ float sample_value(const Corners& v, const SampleAt& s) {
+    return (v.v00 * (1.0f - s.tx) + v.v01 * s.tx) * (1.0f - s.ty) + (v.v10 * (1.0f - s.tx) + v.v11 * s.tx) * s.ty;
+}
+__device__ __forceinline__ float sample_dix(const Corners& v, const SampleAt& s) {
+    return (v.v01 - v.v00) * (1.0f - s.ty) + (v.v11 - v.v10) * s.ty;
+}
+__device__ __forceinline__ float sample_diy(const Corners& v, const SampleAt& s) {
+    return (v.v10 - v.v00) * (1.0f - s.tx) + (v.v11 - v.v01) * s.tx;
+}
+
 // Fused tail: forward of grid_sample + blend, the four L1 terms, and the gradient w.r.t. the head output.
 // out7: [P][8] = grid_change(0,1) alpha(2) colour(3..6) pad; image / targets NCHW.  d_out7: [P][8].
 // loss_acc: doubles [4] = sum|blended-T0|, sum|warped-T2|, sum|grid-T3|, sum|colour-T0|.
@@ -217,26 +258,13 @@ __global__ void __launch_bounds__(256) train_tail_kernel(const float* __restrict
         const float4 oa = *reinterpret_cast<const float4*>(out7 + i * 8), ob = *reinterpret_cast<const float4*>(out7 + i * 8 + 4);
         const float gcx = oa.x, gcy = oa.y, alpha = oa.z;
         const float col[4] = {oa.w, ob.x, ob.y, ob.z};
-        // forward sample (same arithmetic as gridsample.cuh) keeping the corner values for the backward pass
-        const float ixu = __fdiv_rn(__fsub_rn(__fmul_rn(__fadd_rn(__fadd_rn(base[x], gcx), 1.0f), (float)R), 1.0f), 2.0f);
-        const float iyu = __fdiv_rn(__fsub_rn(__fmul_rn(__fadd_rn(__fadd_rn(base[y], gcy), 1.0f), (float)R), 1.0f), 2.0f);
-        const float ix = fminf((float)(R - 1), fmaxf(ixu, 0.0f)), iy = fminf((float)(R - 1), fmaxf(iyu, 0.0f));
-        // d(ix)/d(grid_x) = R/2 inside the image, 0 where the border clamp is active (ATen clip_coordinates_set_grad)
-        const float mx = (ixu <= 0.0f || ixu >= (float)(R - 1)) ? 0.0f : 0.5f * R;
-        const float my = (iyu <= 0.0f || iyu >= (float)(R - 1)) ? 0.0f : 0.5f * R;
-        const float fx = floorf(ix), fy = floorf(iy);
-        const int x0 = (int)fx, y0 = (int)fy;
-        const bool xin = x0 + 1 < R, yin = y0 + 1 < R;
-        const float tx = ix - fx, ty = iy - fy;
+        const SampleAt sa = sample_locate(base, x, y, gcx, gcy, R);
+        const float mx = sa.mx, my = sa.my;
         float gix = 0.0f, giy = 0.0f, dalpha = 0.0f, dcol[4];
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
-            const float* im = image.p + n * image.sn + c * image.sc;
-            const float v00 = im[(long)y0 * image.sh + x0];
-            const float v01 = xin ? im[(long)y0 * image.sh + x0 + 1] : 0.0f;
-            const float v10 = yin ? im[(long)(y0 + 1) * image.sh + x0] : 0.0f;
-            const float v11 = (xin && yin) ? im[(long)(y0 + 1) * image.sh + x0 + 1] : 0.0f;
-            const float wp = (v00 * (1.0f - tx) + v01 * tx) * (1.0f - ty) + (v10 * (1.0f - tx) + v11 * tx) * ty;
+            const Corners v = sample_corners(image.p + n * image.sn + c * image.sc, image.sh, sa);
+            const float wp = sample_value(v, sa);
             const float bl = (1.0f - alpha) * wp + alpha * col[c];
             const long ti = ((long)n * 4 + c) * hw + pp;
             const float t0 = T0[ti], t2 = T2[ti];
@@ -245,8 +273,8 @@ __global__ void __launch_bounds__(256) train_tail_kernel(const float* __restrict
             const float dwp = dbl * (1.0f - alpha) + wn.y * sgn(wp - t2);
             dalpha += dbl * (col[c] - wp);
             dcol[c] = dbl * alpha + wn.w * sgn(col[c] - t0);
-            gix += dwp * ((v01 - v00) * (1.0f - ty) + (v11 - v10) * ty);
-            giy += dwp * ((v10 - v00) * (1.0f - tx) + (v11 - v01) * tx);
+            gix += dwp * sample_dix(v, sa);
+            giy += dwp * sample_diy(v, sa);
         }
         const float t3x = T3[((long)n * 2) * hw + pp], t3y = T3[((long)n * 2 + 1) * hw + pp];
         l[2] += fabsf(gcx - t3x) + fabsf(gcy - t3y);
@@ -302,6 +330,52 @@ __global__ void __launch_bounds__(256) face_tail_kernel(const float* __restrict_
     }
 }
 
+// Tail of the backward from arbitrary upstream gradients (module-level autograd): recomputes the sample of
+// train_tail_kernel and applies the chain rule of blended = (1 - alpha) warped + alpha colour (alpha and colour raw,
+// siren_morpher_03.py:127-131).  g_bl / g_wp / g_col [N,4,R,R], g_al [N,1,R,R], g_grid [N,2,R,R] (NCHW; NULL = zero).
+// d_out7: [P][8] in the layout of out7.
+__global__ void __launch_bounds__(256) grad_tail_kernel(const float* __restrict__ out7, ImgView image, const float* __restrict__ g_bl,
+                                                        const float* __restrict__ g_al, const float* __restrict__ g_col,
+                                                        const float* __restrict__ g_wp, const float* __restrict__ g_grid,
+                                                        const float* __restrict__ base, int R, float* __restrict__ d_out7) {
+    const long hw = (long)R * R, total = image.N * hw;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+        const int x = (int)(i % R), y = (int)((i / R) % R), n = (int)(i / hw);
+        const long pp = (long)y * R + x;
+        const float4 oa = *reinterpret_cast<const float4*>(out7 + i * 8), ob = *reinterpret_cast<const float4*>(out7 + i * 8 + 4);
+        const float gcx = oa.x, gcy = oa.y, alpha = oa.z;
+        const float col[4] = {oa.w, ob.x, ob.y, ob.z};
+        const SampleAt sa = sample_locate(base, x, y, gcx, gcy, R);
+        float gix = 0.0f, giy = 0.0f, dalpha = g_al ? g_al[(long)n * hw + pp] : 0.0f, dcol[4];
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            const long ti = ((long)n * 4 + c) * hw + pp;
+            const Corners v = sample_corners(image.p + n * image.sn + c * image.sc, image.sh, sa);
+            const float wp = sample_value(v, sa);
+            const float gbl = g_bl ? g_bl[ti] : 0.0f;
+            const float dwp = gbl * (1.0f - alpha) + (g_wp ? g_wp[ti] : 0.0f);
+            dalpha += gbl * (col[c] - wp);
+            dcol[c] = gbl * alpha + (g_col ? g_col[ti] : 0.0f);
+            gix += dwp * sample_dix(v, sa);
+            giy += dwp * sample_diy(v, sa);
+        }
+        float dgx = gix * sa.mx, dgy = giy * sa.my;
+        if (g_grid) { dgx += g_grid[((long)n * 2) * hw + pp]; dgy += g_grid[((long)n * 2 + 1) * hw + pp]; }
+        *reinterpret_cast<float4*>(d_out7 + i * 8) = make_float4(dgx, dgy, dalpha, dcol[0]);
+        *reinterpret_cast<float4*>(d_out7 + i * 8 + 4) = make_float4(dcol[1], dcol[2], dcol[3], 0.0f);
+    }
+}
+
+// d_out [P][4] (NHWC, what the face backward reads) from the upstream gradient g [N,4,R,R] (NCHW)
+__global__ void __launch_bounds__(256) face_grad_layout_kernel(const float* __restrict__ g, int R, int N, float* __restrict__ d_out) {
+    const long hw = (long)R * R, total = (long)N * hw;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+        const long pp = i % hw, n = i / hw;
+        const float* gi = g + n * 4 * hw + pp;
+        *reinterpret_cast<float4*>(d_out + i * 4) = make_float4(gi[0], gi[hw], gi[2 * hw], gi[3 * hw]);
+    }
+}
+
 // torch.optim.Adam (no weight decay, no amsgrad): optimizer_factories.py:9-17 (betas 0.9 / 0.999, eps 1e-8)
 __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, long n,
                             float lr, float b1, float b2, float eps, float bc1, float bc2, float gscale) {
@@ -346,6 +420,17 @@ void dense_gemm(Runtime& rt, const float* W, int nreal, int kreal, bool transpos
     conv_forward(cw, a, rt.stream);
 }
 
+// weight and bias gradients of layer d: dW += dz^T x, db += column sums of dz
+void dense_wgrad(cudaStream_t s, const View& dz, const View& x, const Dense& d, float* grads) {
+    const long Pn = (long)dz.N * dz.H * dz.W;
+    const int psplit = (int)std::max<long>(1, std::min<long>(64, Pn / 4096));
+    dim3 grid(ceil_div(dz.C, 64), ceil_div(x.C, 64), psplit);
+    wgrad_kernel<<<grid, 128, 0, s>>>(dz.p, dz.C, x.p, x.C, Pn, d.nreal, d.kreal, grads + d.w_off);
+    THA4_LAUNCH_CHECK();
+    colsum_kernel<<<std::min<long>(148, std::max<long>(1, Pn / 512)), 256, 0, s>>>(dz.p, Pn, dz.C, d.nreal, grads + d.b_off);
+    THA4_LAUNCH_CHECK();
+}
+
 }  // namespace
 
 // reference layer table of SirenMorpher03 (mode_14.py:108-131), in state_dict order
@@ -363,80 +448,68 @@ static void body_layers(Dense (&L)[10]) {
 
 long siren_body_param_count() { Dense L[10]; body_layers(L); return L[9].b_off + 7; }
 
-void siren_body_train_step(Runtime& rt, const ImgView& image, const float* pose, int pose_ld, const float* T0, const float* T2,
-                           const float* T3, const float loss_w[4], const float* params, float* grads, double* loss_acc) {
-    THA4_REQUIRE(image.H == 512 && image.W == 512 && image.C == 4, "distill: image size");
+namespace {
+
+constexpr int BODY_RS[3] = {128, 256, 512};
+constexpr int BODY_CPREV[3] = {0, 180, 90};     // real channels carried up from the previous level
+
+struct BodyActs {          // what the body backward reads: level inputs, pre-activations z, activations a, head output
+    View xin[3], z[3][3], a[3][3], out7;
+};
+
+// forward of N images with stored activations (TF32 products)
+void body_forward_store(Runtime& rt, const Dense (&L)[10], const float* pose, int pose_ld, int N, const float* params, BodyActs& A) {
     cudaStream_t s = rt.stream;
     Pool* P = rt.persist;
-    const int N = image.N;
-    Dense L[10];
-    body_layers(L);
-    const long nparams = L[9].b_off + 7;
-    THA4_CUDA_CHECK(cudaMemsetAsync(grads, 0, nparams * sizeof(float), s));
-    THA4_CUDA_CHECK(cudaMemsetAsync(loss_acc, 0, 4 * sizeof(double), s));
-    ProfScope prof(PROF_SIREN, s);
-
-    const int Rs[3] = {128, 256, 512};
-    const int Cprev[3] = {0, 180, 90};          // real channels carried up from the previous level
-    View xin[3], z[3][3], a[3][3];
     float* bias_pad[10];
     for (int i = 0; i < 10; ++i) {
         bias_pad[i] = P->alloc(L[i].npad);
         pad_bias_kernel<<<ceil_div(L[i].npad, 128), 128, 0, s>>>(params + L[i].b_off, L[i].nreal, L[i].npad, bias_pad[i]);
         THA4_LAUNCH_CHECK();
     }
-    // ------------------------------------------------------------------ forward, activations stored
     for (int l = 0; l < 3; ++l) {
-        const int R = Rs[l];
-        xin[l] = mk(P, N, R, L[3 * l].kpad);
-        const View* prev = l > 0 ? &a[l - 1][2] : nullptr;
-        level_input_kernel<<<grid_for((long)N * R * R * xin[l].C), 256, 0, s>>>(prev ? prev->p : nullptr, Cprev[l], prev ? prev->ld : 0, pose,
-                                                                              pose_ld, base_grid_table(R), R, N, xin[l].C, 45, xin[l].p);
+        const int R = BODY_RS[l];
+        A.xin[l] = mk(P, N, R, L[3 * l].kpad);
+        const View* prev = l > 0 ? &A.a[l - 1][2] : nullptr;
+        level_input_kernel<<<grid_for((long)N * R * R * A.xin[l].C), 256, 0, s>>>(prev ? prev->p : nullptr, BODY_CPREV[l], prev ? prev->ld : 0,
+                                                                                pose, pose_ld, base_grid_table(R), R, N, A.xin[l].C, 45,
+                                                                                A.xin[l].p);
         THA4_LAUNCH_CHECK();
         for (int j = 0; j < 3; ++j) {
             const Dense& d = L[3 * l + j];
             rt.scratch->reset();
-            z[l][j] = mk(P, N, R, d.npad);
-            a[l][j] = mk(P, N, R, d.npad);
-            dense_gemm(rt, params + d.w_off, d.nreal, d.kreal, false, bias_pad[3 * l + j], j == 0 ? xin[l] : a[l][j - 1], z[l][j]);
+            A.z[l][j] = mk(P, N, R, d.npad);
+            A.a[l][j] = mk(P, N, R, d.npad);
+            dense_gemm(rt, params + d.w_off, d.nreal, d.kreal, false, bias_pad[3 * l + j], j == 0 ? A.xin[l] : A.a[l][j - 1], A.z[l][j]);
             const long n4 = (long)N * R * R * d.npad / 4;
-            sine_forward_kernel<<<grid_for(n4), 256, 0, s>>>(z[l][j].p, a[l][j].p, n4);
+            sine_forward_kernel<<<grid_for(n4), 256, 0, s>>>(A.z[l][j].p, A.a[l][j].p, n4);
             THA4_LAUNCH_CHECK();
         }
     }
     rt.scratch->reset();
-    View out7 = mk(P, N, 512, 8);
-    dense_gemm(rt, params + L[9].w_off, 7, 90, false, bias_pad[9], a[2][2], out7);
-    // ------------------------------------------------------------------ losses + d(out7)
-    View d_out = mk(P, N, 512, 8);
-    const double nb = (double)N * 4 * 512 * 512, ng = (double)N * 2 * 512 * 512;
-    const float4 wn = make_float4((float)(loss_w[0] / nb), (float)(loss_w[1] / nb), (float)(loss_w[2] / ng), (float)(loss_w[3] / nb));
-    train_tail_kernel<<<grid_for((long)N * 512 * 512), 256, 0, s>>>(out7.p, image, T0, T2, T3, base_grid_table(512), 512, wn, d_out.p, loss_acc);
-    THA4_LAUNCH_CHECK();
-    // ------------------------------------------------------------------ backward
-    auto wgrad = [&](const View& dz, const View& x, const Dense& d) {
-        const long Pn = (long)dz.N * dz.H * dz.W;
-        const int psplit = (int)std::max<long>(1, std::min<long>(64, Pn / 4096));
-        dim3 grid(ceil_div(dz.C, 64), ceil_div(x.C, 64), psplit);
-        wgrad_kernel<<<grid, 128, 0, s>>>(dz.p, dz.C, x.p, x.C, Pn, d.nreal, d.kreal, grads + d.w_off);
-        THA4_LAUNCH_CHECK();
-        colsum_kernel<<<std::min<long>(148, std::max<long>(1, Pn / 512)), 256, 0, s>>>(dz.p, Pn, dz.C, d.nreal, grads + d.b_off);
-        THA4_LAUNCH_CHECK();
-    };
+    A.out7 = mk(P, N, 512, 8);
+    dense_gemm(rt, params + L[9].w_off, 7, 90, false, bias_pad[9], A.a[2][2], A.out7);
+}
+
+// backward from d(out7) [P][8]; accumulates into grads, which the caller zeroes
+void body_backward(Runtime& rt, const Dense (&L)[10], const BodyActs& A, const View& d_out, const float* params, float* grads) {
+    cudaStream_t s = rt.stream;
+    Pool* P = rt.persist;
+    const int N = d_out.N;
     // head: out7 = a22 W9^T + b9
-    wgrad(d_out, a[2][2], L[9]);
+    dense_wgrad(s, d_out, A.a[2][2], L[9], grads);
     View da = mk(P, N, 512, L[8].npad);
     rt.scratch->reset();
     dense_gemm(rt, params + L[9].w_off, 7, 90, true, nullptr, d_out, da);     // d a22 = d_out W9
     for (int l = 2; l >= 0; --l) {
-        const int R = Rs[l];
+        const int R = BODY_RS[l];
         for (int j = 2; j >= 0; --j) {
             const Dense& d = L[3 * l + j];
             const long n4 = (long)N * R * R * d.npad / 4;
-            sine_backward_kernel<<<grid_for(n4), 256, 0, s>>>(z[l][j].p, da.p, n4);       // da -> dz (in place)
+            sine_backward_kernel<<<grid_for(n4), 256, 0, s>>>(A.z[l][j].p, da.p, n4);       // da -> dz (in place)
             THA4_LAUNCH_CHECK();
-            const View& x = (j == 0) ? xin[l] : a[l][j - 1];
-            wgrad(da, x, d);
+            const View& x = (j == 0) ? A.xin[l] : A.a[l][j - 1];
+            dense_wgrad(s, da, x, d, grads);
             if (j == 0 && l == 0) break;
             View dx = mk(P, N, R, d.kpad);
             rt.scratch->reset();
@@ -445,11 +518,54 @@ void siren_body_train_step(Runtime& rt, const ImgView& image, const float* pose,
             // level boundary: the first Cprev channels of dx are the gradient of the upsampled previous level
             View dprev = mk(P, N, R / 2, L[3 * l - 1].npad);
             THA4_CUDA_CHECK(cudaMemsetAsync(dprev.p, 0, dprev.pixels() * dprev.C * sizeof(float), s));
-            upsample_backward_kernel<<<grid_for((long)N * (R / 2) * (R / 2) * Cprev[l]), 256, 0, s>>>(dx.p, dx.ld, Cprev[l], R, N, dprev.p, dprev.ld);
+            upsample_backward_kernel<<<grid_for((long)N * (R / 2) * (R / 2) * BODY_CPREV[l]), 256, 0, s>>>(dx.p, dx.ld, BODY_CPREV[l], R, N,
+                                                                                                        dprev.p, dprev.ld);
             THA4_LAUNCH_CHECK();
             da = dprev;
         }
     }
+}
+
+}  // namespace
+
+void siren_body_train_step(Runtime& rt, const ImgView& image, const float* pose, int pose_ld, const float* T0, const float* T2,
+                           const float* T3, const float loss_w[4], const float* params, float* grads, double* loss_acc) {
+    THA4_REQUIRE(image.H == 512 && image.W == 512 && image.C == 4, "distill: image size");
+    cudaStream_t s = rt.stream;
+    const int N = image.N;
+    Dense L[10];
+    body_layers(L);
+    const long nparams = L[9].b_off + 7;
+    THA4_CUDA_CHECK(cudaMemsetAsync(grads, 0, nparams * sizeof(float), s));
+    THA4_CUDA_CHECK(cudaMemsetAsync(loss_acc, 0, 4 * sizeof(double), s));
+    ProfScope prof(PROF_SIREN, s);
+    BodyActs A;
+    body_forward_store(rt, L, pose, pose_ld, N, params, A);
+    // losses + d(out7)
+    View d_out = mk(rt.persist, N, 512, 8);
+    const double nb = (double)N * 4 * 512 * 512, ng = (double)N * 2 * 512 * 512;
+    const float4 wn = make_float4((float)(loss_w[0] / nb), (float)(loss_w[1] / nb), (float)(loss_w[2] / ng), (float)(loss_w[3] / nb));
+    train_tail_kernel<<<grid_for((long)N * 512 * 512), 256, 0, s>>>(A.out7.p, image, T0, T2, T3, base_grid_table(512), 512, wn, d_out.p, loss_acc);
+    THA4_LAUNCH_CHECK();
+    body_backward(rt, L, A, d_out, params, grads);
+}
+
+void siren_body_backward(Runtime& rt, const ImgView& image, const float* pose, int pose_ld, const float* const g[5], const float* params,
+                         float* grads) {
+    THA4_REQUIRE(image.H == 512 && image.W == 512 && image.C == 4, "student backward: image size");
+    THA4_REQUIRE(image.N >= 1 && image.N <= SIREN_BODY_MAX_BATCH, "student backward: micro-batch must be 1..8");
+    cudaStream_t s = rt.stream;
+    const int N = image.N;
+    Dense L[10];
+    body_layers(L);
+    ProfScope prof(PROF_SIREN, s);
+    BodyActs A;
+    body_forward_store(rt, L, pose, pose_ld, N, params, A);
+    View d_out = mk(rt.persist, N, 512, 8);
+    grad_tail_kernel<<<grid_for((long)N * 512 * 512), 256, 0, s>>>(A.out7.p, image, g[0], g[1], g[2], g[3], g[4], base_grid_table(512), 512,
+                                                                   d_out.p);
+    THA4_LAUNCH_CHECK();
+    body_backward(rt, L, A, d_out, params, grads);
 }
 
 // reference layer table of SirenFaceMorpher00 (mode_14.py:93-105; vanilla/siren.py:60-91), in state_dict order
@@ -465,72 +581,102 @@ static void face_layers(Dense (&L)[9]) {
 
 long siren_face_param_count() { Dense L[9]; face_layers(L); return L[8].b_off + 4; }
 
-// Face-student distillation step (SURVEY.md section 8 a17): SirenFaceMorpher00 forward with stored activations, L1 +
-// eye/mouth-masked L1 against the teacher crop, full backward into a flat gradient buffer.
-// Reference: siren_face_morpher_protocols_00.py:48-105, siren_face_morpher_00_trainer.py:112-186.
-void siren_face_train_step(Runtime& rt, const float* pose, int pose_ld, int N, const float* target, const float* mask,
-                           const float loss_w[2], const float* params, float* grads, double* loss_acc) {
+namespace {
+
+constexpr int FACE_R = 128;
+
+struct FaceActs { View xin, z[8], a[8], out4; };
+
+void face_forward_store(Runtime& rt, const Dense (&L)[9], const float* pose, int pose_ld, int N, const float* params, FaceActs& A) {
     cudaStream_t s = rt.stream;
     Pool* P = rt.persist;
-    constexpr int R = 128;
-    Dense L[9];
-    face_layers(L);
-    const long nparams = L[8].b_off + 4;
-    THA4_CUDA_CHECK(cudaMemsetAsync(grads, 0, nparams * sizeof(float), s));
-    THA4_CUDA_CHECK(cudaMemsetAsync(loss_acc, 0, 4 * sizeof(double), s));
-    ProfScope prof(PROF_SIREN, s);
+    constexpr int R = FACE_R;
     float* bias_pad[9];
     for (int i = 0; i < 9; ++i) {
         bias_pad[i] = P->alloc(L[i].npad);
         pad_bias_kernel<<<1, 128, 0, s>>>(params + L[i].b_off, L[i].nreal, L[i].npad, bias_pad[i]);
         THA4_LAUNCH_CHECK();
     }
-    // ------------------------------------------------------------------ forward, activations stored
-    View xin = mk(P, N, R, L[0].kpad), z[8], a[8];
-    level_input_kernel<<<grid_for((long)N * R * R * xin.C), 256, 0, s>>>(nullptr, 0, 0, pose, pose_ld, base_grid_table(R), R, N, xin.C, 39, xin.p);
+    A.xin = mk(P, N, R, L[0].kpad);
+    level_input_kernel<<<grid_for((long)N * R * R * A.xin.C), 256, 0, s>>>(nullptr, 0, 0, pose, pose_ld, base_grid_table(R), R, N, A.xin.C, 39,
+                                                                          A.xin.p);
     THA4_LAUNCH_CHECK();
     const long n4 = (long)N * R * R * 128 / 4;
     for (int j = 0; j < 8; ++j) {
         rt.scratch->reset();
-        z[j] = mk(P, N, R, 128);
-        a[j] = mk(P, N, R, 128);
-        dense_gemm(rt, params + L[j].w_off, L[j].nreal, L[j].kreal, false, bias_pad[j], j == 0 ? xin : a[j - 1], z[j]);
-        sine_forward_kernel<<<grid_for(n4), 256, 0, s>>>(z[j].p, a[j].p, n4);
+        A.z[j] = mk(P, N, R, 128);
+        A.a[j] = mk(P, N, R, 128);
+        dense_gemm(rt, params + L[j].w_off, L[j].nreal, L[j].kreal, false, bias_pad[j], j == 0 ? A.xin : A.a[j - 1], A.z[j]);
+        sine_forward_kernel<<<grid_for(n4), 256, 0, s>>>(A.z[j].p, A.a[j].p, n4);
         THA4_LAUNCH_CHECK();
     }
     rt.scratch->reset();
-    View out4 = mk(P, N, R, 4);
-    dense_gemm(rt, params + L[8].w_off, 4, 128, false, bias_pad[8], a[7], out4);
-    // ------------------------------------------------------------------ losses + d(out4)
-    View d_out = mk(P, N, R, 4);
-    const double nel = (double)N * 4 * R * R;
-    face_tail_kernel<<<grid_for((long)N * R * R), 256, 0, s>>>(out4.p, target, mask, R, N,
-                                                              make_float2((float)(loss_w[0] / nel), (float)(loss_w[1] / nel)), d_out.p, loss_acc);
-    THA4_LAUNCH_CHECK();
-    // ------------------------------------------------------------------ backward
-    auto wgrad = [&](const View& dz, const View& x, const Dense& d) {
-        const long Pn = (long)dz.N * dz.H * dz.W;
-        const int psplit = (int)std::max<long>(1, std::min<long>(64, Pn / 4096));
-        dim3 grid(ceil_div(dz.C, 64), ceil_div(x.C, 64), psplit);
-        wgrad_kernel<<<grid, 128, 0, s>>>(dz.p, dz.C, x.p, x.C, Pn, d.nreal, d.kreal, grads + d.w_off);
-        THA4_LAUNCH_CHECK();
-        colsum_kernel<<<std::min<long>(148, std::max<long>(1, Pn / 512)), 256, 0, s>>>(dz.p, Pn, dz.C, d.nreal, grads + d.b_off);
-        THA4_LAUNCH_CHECK();
-    };
-    wgrad(d_out, a[7], L[8]);
+    A.out4 = mk(P, N, R, 4);
+    dense_gemm(rt, params + L[8].w_off, 4, 128, false, bias_pad[8], A.a[7], A.out4);
+}
+
+// backward from d(out4) [P][4]; accumulates into grads, which the caller zeroes
+void face_backward(Runtime& rt, const Dense (&L)[9], const FaceActs& A, const View& d_out, const float* params, float* grads) {
+    cudaStream_t s = rt.stream;
+    Pool* P = rt.persist;
+    constexpr int R = FACE_R;
+    const int N = d_out.N;
+    const long n4 = (long)N * R * R * 128 / 4;
+    dense_wgrad(s, d_out, A.a[7], L[8], grads);
     View da = mk(P, N, R, 128);
     rt.scratch->reset();
     dense_gemm(rt, params + L[8].w_off, 4, 128, true, nullptr, d_out, da);       // d a7 = d_out W8
     for (int j = 7; j >= 0; --j) {
-        sine_backward_kernel<<<grid_for(n4), 256, 0, s>>>(z[j].p, da.p, n4);       // da -> dz (in place)
+        sine_backward_kernel<<<grid_for(n4), 256, 0, s>>>(A.z[j].p, da.p, n4);       // da -> dz (in place)
         THA4_LAUNCH_CHECK();
-        wgrad(da, j == 0 ? xin : a[j - 1], L[j]);
+        dense_wgrad(s, da, j == 0 ? A.xin : A.a[j - 1], L[j], grads);
         if (j == 0) break;
         View dx = mk(P, N, R, 128);
         rt.scratch->reset();
         dense_gemm(rt, params + L[j].w_off, L[j].nreal, L[j].kreal, true, nullptr, da, dx);   // dx = dz W
         da = dx;
     }
+}
+
+}  // namespace
+
+// Face-student distillation step (SURVEY.md section 8 a17): SirenFaceMorpher00 forward with stored activations, L1 +
+// eye/mouth-masked L1 against the teacher crop, full backward into a flat gradient buffer.
+// Reference: siren_face_morpher_protocols_00.py:48-105, siren_face_morpher_00_trainer.py:112-186.
+void siren_face_train_step(Runtime& rt, const float* pose, int pose_ld, int N, const float* target, const float* mask,
+                           const float loss_w[2], const float* params, float* grads, double* loss_acc) {
+    cudaStream_t s = rt.stream;
+    constexpr int R = FACE_R;
+    Dense L[9];
+    face_layers(L);
+    const long nparams = L[8].b_off + 4;
+    THA4_CUDA_CHECK(cudaMemsetAsync(grads, 0, nparams * sizeof(float), s));
+    THA4_CUDA_CHECK(cudaMemsetAsync(loss_acc, 0, 4 * sizeof(double), s));
+    ProfScope prof(PROF_SIREN, s);
+    FaceActs A;
+    face_forward_store(rt, L, pose, pose_ld, N, params, A);
+    // losses + d(out4)
+    View d_out = mk(rt.persist, N, R, 4);
+    const double nel = (double)N * 4 * R * R;
+    face_tail_kernel<<<grid_for((long)N * R * R), 256, 0, s>>>(A.out4.p, target, mask, R, N,
+                                                              make_float2((float)(loss_w[0] / nel), (float)(loss_w[1] / nel)), d_out.p, loss_acc);
+    THA4_LAUNCH_CHECK();
+    face_backward(rt, L, A, d_out, params, grads);
+}
+
+void siren_face_backward(Runtime& rt, const float* pose, int pose_ld, int N, const float* grad_output, const float* params, float* grads) {
+    THA4_REQUIRE(N >= 1 && N <= SIREN_FACE_MAX_BATCH, "face student backward: micro-batch must be 1..64");
+    cudaStream_t s = rt.stream;
+    constexpr int R = FACE_R;
+    Dense L[9];
+    face_layers(L);
+    ProfScope prof(PROF_SIREN, s);
+    FaceActs A;
+    face_forward_store(rt, L, pose, pose_ld, N, params, A);
+    View d_out = mk(rt.persist, N, R, 4);
+    face_grad_layout_kernel<<<grid_for((long)N * R * R), 256, 0, s>>>(grad_output, R, N, d_out.p);
+    THA4_LAUNCH_CHECK();
+    face_backward(rt, L, A, d_out, params, grads);
 }
 
 void adam_step(float* params, const float* grads, float* m, float* v, long n, float lr, float beta1, float beta2, float eps,

@@ -5,6 +5,7 @@ from typing import Optional
 from torch import Tensor
 
 from tha4_b200.nn.common.native_module import NativeModule
+from tha4_b200.nn.siren import student_autograd
 from tha4_b200.nn.state_dict_spec import siren_face_morpher_spec
 
 
@@ -17,4 +18,6 @@ class SirenFaceMorpher00(NativeModule):
 
     def forward(self, pose: Tensor, position: Optional[Tensor] = None) -> Tensor:
         assert position is None, 'only the default affine_grid position image (siren_face_morpher_00.py:38-44) is supported'
+        if student_autograd.wants_autograd(self):       # loss.backward() reaches the parameters (student_autograd.py)
+            return student_autograd.siren_face_morpher(self, pose)
         return self.sync_weights().siren_face_morpher(pose)

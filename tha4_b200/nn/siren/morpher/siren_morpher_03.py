@@ -5,6 +5,7 @@ from typing import List
 from torch import Tensor
 
 from tha4_b200.nn.common.native_module import NativeModule
+from tha4_b200.nn.siren import student_autograd
 from tha4_b200.nn.state_dict_spec import siren_morpher_03_spec
 
 
@@ -16,6 +17,8 @@ class SirenMorpher03(NativeModule):
         self.args = args
 
     def forward(self, image: Tensor, pose: Tensor) -> List[Tensor]:
+        if student_autograd.wants_autograd(self):       # loss.backward() reaches the parameters (student_autograd.py)
+            return student_autograd.siren_morpher(self, image, pose)
         return self.sync_weights().siren_morpher(image, pose)
 
     INDEX_BLENDED_IMAGE = 0
