@@ -161,6 +161,22 @@ int tha4_siren_morpher_backward(tha4_ctx* ctx, const float* image, const float* 
  * micro-batches of <= 64) */
 int tha4_siren_face_morpher_backward(tha4_ctx* ctx, const float* pose, int pose_ld, int B, const float* grad_output,
                                      const float* params, float* grads, void* stream);
+/* ---- input gradients of the students (frozen students under torch.autograd: pose fitting, training through them) ---- */
+/* The backward of SirenMorpher03 with every output optional (NULL = not computed; at least one non-NULL; each is
+ * overwritten):
+ *   grads   [331 567]      dL/d params, as tha4_siren_morpher_backward;
+ *   d_image [B,4,512,512]  dL/d image: the exact adjoint of the warp the forward returned, computed from its returned
+ *                          grid_change [B,2,512,512] and alpha [B,1,512,512] and grad_outputs[0] / [3] (d blended,
+ *                          d warped) with no SIREN recompute.  Float atomics: not bit-reproducible run to run;
+ *   d_pose  [B,45]         dL/d pose of the TF32 recompute (as grads); fixed-order reduction, bit-reproducible.
+ * grid_change / alpha are needed only for d_image; image / pose / params only for grads / d_pose.  Any B >= 1
+ * (micro-batches of <= 8). */
+int tha4_siren_morpher_backward_ex(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
+                                   const float* const* grad_outputs, const float* grid_change, const float* alpha,
+                                   const float* params, float* grads, float* d_image, float* d_pose, void* stream);
+/* same for SirenFaceMorpher00: grads [121 476] and / or d_pose [B,39] (micro-batches of <= 64) */
+int tha4_siren_face_morpher_backward_ex(tha4_ctx* ctx, const float* pose, int pose_ld, int B, const float* grad_output,
+                                        const float* params, float* grads, float* d_pose, void* stream);
 /* torch.optim.Adam step on flat buffers (shion/base/optimizer_factories.py:9-17); grads are scaled by grad_scale first
  * (1/world_size after a summing all-reduce = DDP's gradient averaging) */
 int tha4_adam_step(tha4_ctx* ctx, float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t n, float lr,

@@ -597,7 +597,7 @@ int tha4_siren_morpher_backward(tha4_ctx* ctx, const float* image, const float* 
             for (int i = 0; i < 5; ++i)
                 g[i] = (grad_outputs && grad_outputs[i]) ? grad_outputs[i] + (size_t)n0 * ch[i] * 512 * 512 : nullptr;
             siren_body_backward(rt, make_img(image + (size_t)n0 * 4 * 512 * 512, b, 4, 512, 512), pose + (size_t)n0 * pose_ld, pose_ld, g,
-                                params, grads);
+                                params, grads, nullptr);
         }
     });
 }
@@ -614,7 +614,57 @@ int tha4_siren_face_morpher_backward(tha4_ctx* ctx, const float* pose, int pose_
         for (int n0 = 0; n0 < B; n0 += SIREN_FACE_MAX_BATCH) {
             const int b = std::min(SIREN_FACE_MAX_BATCH, B - n0);
             begin_pass(ctx, s);
-            siren_face_backward(rt, pose + (size_t)n0 * pose_ld, pose_ld, b, grad_output + (size_t)n0 * 4 * 128 * 128, params, grads);
+            siren_face_backward(rt, pose + (size_t)n0 * pose_ld, pose_ld, b, grad_output + (size_t)n0 * 4 * 128 * 128, params, grads,
+                                nullptr);
+        }
+    });
+}
+
+int tha4_siren_morpher_backward_ex(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
+                                   const float* const* grad_outputs, const float* grid_change, const float* alpha,
+                                   const float* params, float* grads, float* d_image, float* d_pose, void* stream) {
+    return guarded(ctx, [&] {
+        THA4_REQUIRE(B >= 1, "student backward: batch must be >= 1");
+        THA4_REQUIRE(grads || d_image || d_pose, "student backward: no output requested");
+        const bool siren = grads || d_pose;          // the parameter and pose gradients need the SIREN recompute; d_image does not
+        THA4_REQUIRE(!siren || (image && pose && params), "student backward: image, pose and params are required");
+        THA4_REQUIRE(!siren || pose_ld >= 45, "student backward: pose rows need at least 45 entries");
+        THA4_REQUIRE(!d_image || (grid_change && alpha), "student backward: d_image needs the forward's grid_change and alpha");
+        cudaStream_t s = (cudaStream_t)stream;
+        Runtime rt = make_rt(ctx, stream);
+        if (grads) THA4_CUDA_CHECK(cudaMemsetAsync(grads, 0, siren_body_param_count() * sizeof(float), s));
+        constexpr size_t hw = 512 * 512;
+        const int ch[5] = {4, 1, 4, 4, 2};
+        for (int n0 = 0; n0 < B; n0 += SIREN_BODY_MAX_BATCH) {       // micro-batches share the workspace
+            const int b = std::min(SIREN_BODY_MAX_BATCH, B - n0);
+            begin_pass(ctx, s);
+            const float* g[5];
+            for (int i = 0; i < 5; ++i) g[i] = (grad_outputs && grad_outputs[i]) ? grad_outputs[i] + (size_t)n0 * ch[i] * hw : nullptr;
+            if (siren)
+                siren_body_backward(rt, make_img(image + (size_t)n0 * 4 * hw, b, 4, 512, 512), pose + (size_t)n0 * pose_ld, pose_ld, g,
+                                    params, grads, d_pose ? d_pose + (size_t)n0 * 45 : nullptr);
+            if (d_image)
+                siren_body_image_grad(rt, grid_change + (size_t)n0 * 2 * hw, alpha + (size_t)n0 * hw, g[0], g[3], b,
+                                      d_image + (size_t)n0 * 4 * hw);
+        }
+    });
+}
+
+int tha4_siren_face_morpher_backward_ex(tha4_ctx* ctx, const float* pose, int pose_ld, int B, const float* grad_output,
+                                        const float* params, float* grads, float* d_pose, void* stream) {
+    return guarded(ctx, [&] {
+        THA4_REQUIRE(B >= 1, "face student backward: batch must be >= 1");
+        THA4_REQUIRE(grads || d_pose, "face student backward: no output requested");
+        THA4_REQUIRE(pose_ld >= 39, "face student backward: pose rows need at least 39 entries");
+        THA4_REQUIRE(grad_output != nullptr, "face student backward: grad_output is required");
+        cudaStream_t s = (cudaStream_t)stream;
+        Runtime rt = make_rt(ctx, stream);
+        if (grads) THA4_CUDA_CHECK(cudaMemsetAsync(grads, 0, siren_face_param_count() * sizeof(float), s));
+        for (int n0 = 0; n0 < B; n0 += SIREN_FACE_MAX_BATCH) {
+            const int b = std::min(SIREN_FACE_MAX_BATCH, B - n0);
+            begin_pass(ctx, s);
+            siren_face_backward(rt, pose + (size_t)n0 * pose_ld, pose_ld, b, grad_output + (size_t)n0 * 4 * 128 * 128, params, grads,
+                                d_pose ? d_pose + (size_t)n0 * 39 : nullptr);
         }
     });
 }

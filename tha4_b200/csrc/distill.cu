@@ -376,6 +376,122 @@ __global__ void __launch_bounds__(256) face_grad_layout_kernel(const float* __re
     }
 }
 
+// ---------------------------------------------------------------------------------------------- input gradients
+// d(image) of warped = grid_sample(image, base + grid_change) (bilinear, border, align_corners=False) through blended =
+// (1 - alpha) warped + alpha colour: each output pixel scatters its bilinear weights x (g_bl (1 - alpha) + g_wp) into the
+// corners it sampled.  grid_change [N,2,R,R] and alpha [N,1,R,R] are the values the forward returned, and the corners and
+// weights are located with the inference tail's arithmetic (gs_locate / gs_sample), so d(image) is the exact adjoint of the
+// returned warp.  Out-of-range corners are skipped, as the forward skips them.  g_bl / g_wp [N,4,R,R] NCHW, NULL = zero.
+// d_nhwc: [N][R][R][4], zeroed by the caller; one red.global.add.v4.f32 per corner.  The float atomics make the result
+// not bit-reproducible run to run (like torch's CUDA grid_sample backward).  Measured against 16 scalar reds per pixel
+// straight into NCHW (H100 80GB HBM3, 700 W; zeroing and layout pass included, one 512x512 sample): 20.5 vs 24.3 us for a
+// gently varying grid, 22.7 vs 51.9 us for a rough one; the scalar form is faster only on the identity grid (13.5 vs 16.6).
+__global__ void __launch_bounds__(256) image_grad_kernel(const float* __restrict__ grid_change, const float* __restrict__ alpha,
+                                                         const float* __restrict__ g_bl, const float* __restrict__ g_wp,
+                                                         const float* __restrict__ base, int R, int N, float* __restrict__ d_nhwc) {
+    const long hw = (long)R * R, total = (long)N * hw;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+        const int x = (int)(i % R), y = (int)((i / R) % R), n = (int)(i / hw);
+        const long pp = i - (long)n * hw;
+        const GsTap t = gs_locate(base[x], base[y], grid_change[(2L * n) * hw + pp], grid_change[(2L * n + 1) * hw + pp], R, R);
+        const float om = g_bl ? 1.0f - alpha[i] : 0.0f;
+        float dw[4];
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            const long ti = ((long)n * 4 + c) * hw + pp;
+            dw[c] = (g_bl ? g_bl[ti] * om : 0.0f) + (g_wp ? g_wp[ti] : 0.0f);
+        }
+        const float wx1 = __fsub_rn(t.ix, t.fx), wx0 = __fsub_rn(__fadd_rn(t.fx, 1.0f), t.ix);
+        const float wy1 = __fsub_rn(t.iy, t.fy), wy0 = __fsub_rn(__fadd_rn(t.fy, 1.0f), t.iy);
+        const float wnw = __fmul_rn(wx0, wy0), wne = __fmul_rn(wx1, wy0), wsw = __fmul_rn(wx0, wy1), wse = __fmul_rn(wx1, wy1);
+        const bool xin = (t.x0 + 1) < R, yin = (t.y0 + 1) < R;
+        float4* d = reinterpret_cast<float4*>(d_nhwc) + n * hw + (long)t.y0 * R + t.x0;
+        atomicAdd(d, make_float4(wnw * dw[0], wnw * dw[1], wnw * dw[2], wnw * dw[3]));
+        if (xin) atomicAdd(d + 1, make_float4(wne * dw[0], wne * dw[1], wne * dw[2], wne * dw[3]));
+        if (yin) atomicAdd(d + R, make_float4(wsw * dw[0], wsw * dw[1], wsw * dw[2], wsw * dw[3]));
+        if (xin && yin) atomicAdd(d + R + 1, make_float4(wse * dw[0], wse * dw[1], wse * dw[2], wse * dw[3]));
+    }
+}
+
+// [N][hw][4] (NHWC) -> [N][4][hw] (NCHW)
+__global__ void __launch_bounds__(256) nhwc4_to_nchw_kernel(const float* __restrict__ src, long hw, int N, float* __restrict__ dst) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < (long)N * hw; i += (long)gridDim.x * blockDim.x) {
+        const long n = i / hw, pp = i - n * hw;
+        const float4 v = reinterpret_cast<const float4*>(src)[i];
+        float* o = dst + n * 4 * hw + pp;
+        o[0] = v.x; o[hw] = v.y; o[2 * hw] = v.z; o[3 * hw] = v.w;
+    }
+}
+
+// d(pose), stage 1: the pose enters only as columns col0 .. col0 + npose - 1 of each level's first layer, so
+// d pose[n][k] = sum_levels sum_c S[n][c] W0[c][col0 + k] with S[n][c] = sum over sample n's pixels of the first layer's dz.
+// This stage sums dz [N][hw][C] over chunks of POSE_CHUNK pixels in a fixed order: part[n][chunk][C] (fp32).  Grid
+// (hw / POSE_CHUNK, N).  C % 4 == 0, C <= 1024.  No atomics: d(pose) is bit-reproducible and independent of the batch.
+constexpr int POSE_CHUNK = 256;
+__global__ void __launch_bounds__(256) pose_colsum_kernel(const float* __restrict__ dz, int C, long hw, float* __restrict__ part) {
+    __shared__ float4 red[256];
+    const int cq = C >> 2, PL = 256 / cq;
+    const int tid = threadIdx.x, pl = tid / cq, q = tid - pl * cq;
+    const long n = blockIdx.y, chunk = blockIdx.x;
+    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (pl < PL) {
+        const float* src = dz + (n * hw + chunk * POSE_CHUNK) * C + 4 * q;
+        for (int r = pl; r < POSE_CHUNK; r += PL) {
+            const float4 v = *reinterpret_cast<const float4*>(src + (long)r * C);
+            s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+        }
+    }
+    red[tid] = s;
+    __syncthreads();
+    if (pl == 0) {
+        float4 acc = red[q];
+        for (int j = 1; j < PL; ++j) {
+            const float4 v = red[j * cq + q];
+            acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+        }
+        *reinterpret_cast<float4*>(part + (n * gridDim.x + chunk) * C + 4 * q) = acc;
+    }
+}
+
+// d(pose), stage 2: one block per sample.  S[l][c] = the chunk partials of level l summed in fp64 (fixed order), then
+// d pose[n][k] = sum_l sum_c S[l][c] W_l[c][col0_l + k] in fp64 with the fp32 weights of the flat parameter buffer.
+struct PoseLevel {
+    const float* part;     // [N][nchunk][C] from pose_colsum_kernel
+    const float* W;        // first-layer weight [nreal][kreal]
+    int nchunk, C, nreal, kreal, col0;
+};
+struct PoseGrad {
+    PoseLevel lv[3];
+    int nl = 0, npose = 0;
+};
+constexpr int POSE_PROJECT_THREADS = 384;
+__global__ void __launch_bounds__(POSE_PROJECT_THREADS) pose_project_kernel(const PoseGrad p, float* __restrict__ dpose) {
+    __shared__ double S[3][POSE_PROJECT_THREADS];
+    const int n = blockIdx.x, tid = threadIdx.x;
+#pragma unroll
+    for (int l = 0; l < 3; ++l) {
+        if (l >= p.nl) break;
+        const PoseLevel& L = p.lv[l];
+        if (tid < L.nreal) {
+            const float* src = L.part + (long)n * L.nchunk * L.C + tid;
+            double s = 0.0;
+            for (int k = 0; k < L.nchunk; ++k) s += (double)src[(long)k * L.C];
+            S[l][tid] = s;
+        }
+    }
+    __syncthreads();
+    if (tid < p.npose) {
+        double acc = 0.0;
+#pragma unroll
+        for (int l = 0; l < 3; ++l) {
+            if (l >= p.nl) break;
+            const PoseLevel& L = p.lv[l];
+            for (int c = 0; c < L.nreal; ++c) acc += S[l][c] * (double)L.W[(long)c * L.kreal + L.col0 + tid];
+        }
+        dpose[(long)n * p.npose + tid] = (float)acc;
+    }
+}
+
 // torch.optim.Adam (no weight decay, no amsgrad): optimizer_factories.py:9-17 (betas 0.9 / 0.999, eps 1e-8)
 __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, long n,
                             float lr, float b1, float b2, float eps, float bc1, float bc2, float gscale) {
@@ -428,6 +544,25 @@ void dense_wgrad(cudaStream_t s, const View& dz, const View& x, const Dense& d, 
     wgrad_kernel<<<grid, 128, 0, s>>>(dz.p, dz.C, x.p, x.C, Pn, d.nreal, d.kreal, grads + d.w_off);
     THA4_LAUNCH_CHECK();
     colsum_kernel<<<std::min<long>(148, std::max<long>(1, Pn / 512)), 256, 0, s>>>(dz.p, Pn, dz.C, d.nreal, grads + d.b_off);
+    THA4_LAUNCH_CHECK();
+}
+
+// d(pose) stage 1 for one level: chunk sums of the first layer's dz (layer d; the pose columns start at col0)
+void pose_colsum(Runtime& rt, const View& dz, const Dense& d, const float* params, int col0, PoseGrad& pg) {
+    const long hw = (long)dz.H * dz.W;
+    THA4_REQUIRE(hw % POSE_CHUNK == 0 && dz.C % 4 == 0 && dz.C <= 1024 && d.nreal <= POSE_PROJECT_THREADS, "pose gradient: level shape");
+    PoseLevel& L = pg.lv[pg.nl++];
+    L.nchunk = (int)(hw / POSE_CHUNK); L.C = dz.C; L.nreal = d.nreal; L.kreal = d.kreal; L.col0 = col0;
+    L.W = params + d.w_off;
+    float* part = rt.persist->alloc((size_t)dz.N * L.nchunk * L.C);
+    L.part = part;
+    pose_colsum_kernel<<<dim3(L.nchunk, dz.N), 256, 0, rt.stream>>>(dz.p, dz.C, hw, part);
+    THA4_LAUNCH_CHECK();
+}
+
+// d(pose) stage 2: dpose [N][npose], overwritten
+void pose_project(cudaStream_t s, const PoseGrad& pg, int N, float* dpose) {
+    pose_project_kernel<<<N, POSE_PROJECT_THREADS, 0, s>>>(pg, dpose);
     THA4_LAUNCH_CHECK();
 }
 
@@ -491,13 +626,15 @@ void body_forward_store(Runtime& rt, const Dense (&L)[10], const float* pose, in
     dense_gemm(rt, params + L[9].w_off, 7, 90, false, bias_pad[9], A.a[2][2], A.out7);
 }
 
-// backward from d(out7) [P][8]; accumulates into grads, which the caller zeroes
-void body_backward(Runtime& rt, const Dense (&L)[10], const BodyActs& A, const View& d_out, const float* params, float* grads) {
+// backward from d(out7) [P][8]; accumulates into grads, which the caller zeroes.  grads == NULL: no weight gradients.
+// pose_grad != NULL: also the stage-1 chunk sums of d(pose) (the caller runs pose_project).
+void body_backward(Runtime& rt, const Dense (&L)[10], const BodyActs& A, const View& d_out, const float* params, float* grads,
+                   PoseGrad* pose_grad = nullptr) {
     cudaStream_t s = rt.stream;
     Pool* P = rt.persist;
     const int N = d_out.N;
     // head: out7 = a22 W9^T + b9
-    dense_wgrad(s, d_out, A.a[2][2], L[9], grads);
+    if (grads) dense_wgrad(s, d_out, A.a[2][2], L[9], grads);
     View da = mk(P, N, 512, L[8].npad);
     rt.scratch->reset();
     dense_gemm(rt, params + L[9].w_off, 7, 90, true, nullptr, d_out, da);     // d a22 = d_out W9
@@ -509,7 +646,8 @@ void body_backward(Runtime& rt, const Dense (&L)[10], const BodyActs& A, const V
             sine_backward_kernel<<<grid_for(n4), 256, 0, s>>>(A.z[l][j].p, da.p, n4);       // da -> dz (in place)
             THA4_LAUNCH_CHECK();
             const View& x = (j == 0) ? A.xin[l] : A.a[l][j - 1];
-            dense_wgrad(s, da, x, d, grads);
+            if (grads) dense_wgrad(s, da, x, d, grads);
+            if (j == 0 && pose_grad) pose_colsum(rt, da, d, params, BODY_CPREV[l] + 2, *pose_grad);
             if (j == 0 && l == 0) break;
             View dx = mk(P, N, R, d.kpad);
             rt.scratch->reset();
@@ -551,7 +689,7 @@ void siren_body_train_step(Runtime& rt, const ImgView& image, const float* pose,
 }
 
 void siren_body_backward(Runtime& rt, const ImgView& image, const float* pose, int pose_ld, const float* const g[5], const float* params,
-                         float* grads) {
+                         float* grads, float* d_pose) {
     THA4_REQUIRE(image.H == 512 && image.W == 512 && image.C == 4, "student backward: image size");
     THA4_REQUIRE(image.N >= 1 && image.N <= SIREN_BODY_MAX_BATCH, "student backward: micro-batch must be 1..8");
     cudaStream_t s = rt.stream;
@@ -565,7 +703,28 @@ void siren_body_backward(Runtime& rt, const ImgView& image, const float* pose, i
     grad_tail_kernel<<<grid_for((long)N * 512 * 512), 256, 0, s>>>(A.out7.p, image, g[0], g[1], g[2], g[3], g[4], base_grid_table(512), 512,
                                                                    d_out.p);
     THA4_LAUNCH_CHECK();
-    body_backward(rt, L, A, d_out, params, grads);
+    PoseGrad pg;
+    pg.npose = 45;
+    body_backward(rt, L, A, d_out, params, grads, d_pose ? &pg : nullptr);
+    if (d_pose) pose_project(s, pg, N, d_pose);
+}
+
+void siren_body_image_grad(Runtime& rt, const float* grid_change, const float* alpha, const float* g_bl, const float* g_wp, int N,
+                           float* d_image) {
+    THA4_REQUIRE(N >= 1 && N <= SIREN_BODY_MAX_BATCH, "student image gradient: micro-batch must be 1..8");
+    cudaStream_t s = rt.stream;
+    constexpr int R = 512;
+    const long hw = (long)R * R;
+    if (!g_bl && !g_wp) {               // warped reaches no output that has a gradient
+        THA4_CUDA_CHECK(cudaMemsetAsync(d_image, 0, (size_t)N * 4 * hw * sizeof(float), s));
+        return;
+    }
+    float* acc = rt.persist->alloc((size_t)N * hw * 4);
+    THA4_CUDA_CHECK(cudaMemsetAsync(acc, 0, (size_t)N * hw * 4 * sizeof(float), s));
+    image_grad_kernel<<<grid_for(N * hw), 256, 0, s>>>(grid_change, alpha, g_bl, g_wp, base_grid_table(R), R, N, acc);
+    THA4_LAUNCH_CHECK();
+    nhwc4_to_nchw_kernel<<<grid_for(N * hw), 256, 0, s>>>(acc, hw, N, d_image);
+    THA4_LAUNCH_CHECK();
 }
 
 // reference layer table of SirenFaceMorpher00 (mode_14.py:93-105; vanilla/siren.py:60-91), in state_dict order
@@ -615,21 +774,24 @@ void face_forward_store(Runtime& rt, const Dense (&L)[9], const float* pose, int
     dense_gemm(rt, params + L[8].w_off, 4, 128, false, bias_pad[8], A.a[7], A.out4);
 }
 
-// backward from d(out4) [P][4]; accumulates into grads, which the caller zeroes
-void face_backward(Runtime& rt, const Dense (&L)[9], const FaceActs& A, const View& d_out, const float* params, float* grads) {
+// backward from d(out4) [P][4]; accumulates into grads, which the caller zeroes.  grads == NULL: no weight gradients.
+// pose_grad != NULL: also the stage-1 chunk sums of d(pose) (the caller runs pose_project).
+void face_backward(Runtime& rt, const Dense (&L)[9], const FaceActs& A, const View& d_out, const float* params, float* grads,
+                   PoseGrad* pose_grad = nullptr) {
     cudaStream_t s = rt.stream;
     Pool* P = rt.persist;
     constexpr int R = FACE_R;
     const int N = d_out.N;
     const long n4 = (long)N * R * R * 128 / 4;
-    dense_wgrad(s, d_out, A.a[7], L[8], grads);
+    if (grads) dense_wgrad(s, d_out, A.a[7], L[8], grads);
     View da = mk(P, N, R, 128);
     rt.scratch->reset();
     dense_gemm(rt, params + L[8].w_off, 4, 128, true, nullptr, d_out, da);       // d a7 = d_out W8
     for (int j = 7; j >= 0; --j) {
         sine_backward_kernel<<<grid_for(n4), 256, 0, s>>>(A.z[j].p, da.p, n4);       // da -> dz (in place)
         THA4_LAUNCH_CHECK();
-        dense_wgrad(s, da, j == 0 ? A.xin : A.a[j - 1], L[j], grads);
+        if (grads) dense_wgrad(s, da, j == 0 ? A.xin : A.a[j - 1], L[j], grads);
+        if (j == 0 && pose_grad) pose_colsum(rt, da, L[0], params, 2, *pose_grad);
         if (j == 0) break;
         View dx = mk(P, N, R, 128);
         rt.scratch->reset();
@@ -664,7 +826,8 @@ void siren_face_train_step(Runtime& rt, const float* pose, int pose_ld, int N, c
     face_backward(rt, L, A, d_out, params, grads);
 }
 
-void siren_face_backward(Runtime& rt, const float* pose, int pose_ld, int N, const float* grad_output, const float* params, float* grads) {
+void siren_face_backward(Runtime& rt, const float* pose, int pose_ld, int N, const float* grad_output, const float* params, float* grads,
+                         float* d_pose) {
     THA4_REQUIRE(N >= 1 && N <= SIREN_FACE_MAX_BATCH, "face student backward: micro-batch must be 1..64");
     cudaStream_t s = rt.stream;
     constexpr int R = FACE_R;
@@ -676,7 +839,10 @@ void siren_face_backward(Runtime& rt, const float* pose, int pose_ld, int N, con
     View d_out = mk(rt.persist, N, R, 4);
     face_grad_layout_kernel<<<grid_for((long)N * R * R), 256, 0, s>>>(grad_output, R, N, d_out.p);
     THA4_LAUNCH_CHECK();
-    face_backward(rt, L, A, d_out, params, grads);
+    PoseGrad pg;
+    pg.npose = 39;
+    face_backward(rt, L, A, d_out, params, grads, d_pose ? &pg : nullptr);
+    if (d_pose) pose_project(s, pg, N, d_pose);
 }
 
 void adam_step(float* params, const float* grads, float* m, float* v, long n, float lr, float beta1, float beta2, float eps,

@@ -20,4 +20,6 @@ class SirenFaceMorpher00(NativeModule):
         assert position is None, 'only the default affine_grid position image (siren_face_morpher_00.py:38-44) is supported'
         if student_autograd.wants_autograd(self):       # loss.backward() reaches the parameters (student_autograd.py)
             return student_autograd.siren_face_morpher(self, pose)
+        if student_autograd.wants_input_grad(pose):             # frozen: loss.backward() reaches the pose
+            return student_autograd.siren_face_morpher_input_grad(self, pose)
         return self.sync_weights().siren_face_morpher(pose)

@@ -19,6 +19,8 @@ class SirenMorpher03(NativeModule):
     def forward(self, image: Tensor, pose: Tensor) -> List[Tensor]:
         if student_autograd.wants_autograd(self):       # loss.backward() reaches the parameters (student_autograd.py)
             return student_autograd.siren_morpher(self, image, pose)
+        if student_autograd.wants_input_grad(image, pose):      # frozen: loss.backward() reaches image / pose
+            return student_autograd.siren_morpher_input_grad(self, image, pose)
         return self.sync_weights().siren_morpher(image, pose)
 
     INDEX_BLENDED_IMAGE = 0
