@@ -92,6 +92,18 @@ int tha4_eyebrow_morphing_combiner_forward(tha4_ctx* ctx, const float* backgroun
 /* FaceMorpher08.forward (src/tha4/nn/face_morpher/face_morpher_08.py:158-193): image [B,4,192,192], pose [B,27] -> 8 */
 int tha4_face_morpher_forward(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
                               float* const* outputs, void* stream);
+/* Input gradients of the three encoder-decoder networks for upstream gradients of their outputs (grad_outputs: 6 / 8
+ * entries in the forward's output order, NCHW, an entry may be NULL = zero).  Every gradient output is optional (NULL = not
+ * computed), at least one must be non-NULL, and each is overwritten: d_image / d_background_layer / d_eyebrow_layer have the
+ * shape of the input, d_pose is [B,12] / [B,27] (contiguous).  The forward is recomputed in the context's precision mode
+ * (default: f16 operands; strict: 3xTF32) and differentiated with fp32 data gradients.  Any B >= 1 (micro-batched). */
+int tha4_eyebrow_decomposer_backward(tha4_ctx* ctx, const float* image, int B, const float* const* grad_outputs,
+                                     float* d_image, void* stream);
+int tha4_eyebrow_morphing_combiner_backward(tha4_ctx* ctx, const float* background_layer, const float* eyebrow_layer,
+                                            const float* pose, int pose_ld, int B, const float* const* grad_outputs,
+                                            float* d_background_layer, float* d_eyebrow_layer, float* d_pose, void* stream);
+int tha4_face_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
+                               const float* const* grad_outputs, float* d_image, float* d_pose, void* stream);
 /* Morpher00.forward (src/tha4/nn/morpher/morpher_00.py:42-66): image [B,4,256,256], pose [B,6] ->
  * merged(4) alpha(1) warped(4) grid_change(2) direct(4) */
 int tha4_morpher_forward(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
@@ -240,6 +252,20 @@ int tha4_test_norm(tha4_ctx* ctx, const float* x, int N, int C, int H, int W, in
 int tha4_test_tail(tha4_ctx* ctx, int kind, const float* feature, int N, int C, int S, const float* gamma, const float* beta,
                    int groups, int act, const float* head_w, const float* head_b, const int* head_cout, int n_heads,
                    const float* image0, const float* image1, float* const* outputs, int strict, void* stream);
+/* Data gradient of a conv on the conv kernels with adjoint-packed weights: kind 0 3x3 s1 p1 (w [Cout,Cin,3,3]), 1 4x4 s2 p1
+ * (w [Cout,Cin,4,4]), 2 4x4 s2 p1 transposed (w [Cin,Cout,4,4]); dy [N,Cout,Ho,Wo] -> dx [N,Cin,H,W].  Cout % 4 == 0.
+ * strict: 3xTF32, else TF32 (fp32 operands in both). */
+int tha4_test_conv_backward_data(tha4_ctx* ctx, int kind, const float* dy, const float* w, float* dx, int N, int Cin, int H, int W,
+                                 int Cout, int strict, void* stream);
+/* InstanceNorm2d(affine) (+ReLU when act == 1) backward: x, dy, dx [N,C,H,W] (statistics of x computed on the device) */
+int tha4_test_norm_backward(tha4_ctx* ctx, const float* x, int N, int C, int H, int W, const float* gamma, const float* beta,
+                            int act, const float* dy, float* dx, void* stream);
+/* Tail backward of one encoder-decoder kind (1 decomposer, 2 combiner, 3 face morpher) in isolation: outputs / grad_outputs as
+ * tha4_test_tail returns them (grad entries may be NULL), image0 / image1 as for tha4_test_tail.  d_head [N,12,S,S]: gradients
+ * of the head pre-activations in the channel order of tail.cu; d_image0 / d_image1 [N,4,S,S] (NULL = not computed). */
+int tha4_test_tail_backward(tha4_ctx* ctx, int kind, const float* const* outputs, int N, int S, const float* image0,
+                            const float* image1, const float* const* grad_outputs, float* d_head, float* d_image0,
+                            float* d_image1, void* stream);
 /* qkv_attention, "new order" (src/tha4/nn/common/unet.py:192-202): qkv [N,3C,16,16] -> out [N,C,16,16] */
 int tha4_test_attention(tha4_ctx* ctx, const float* qkv, int N, int C, int heads, float* out, void* stream);
 /* y[n][o] = b[o] + sum_i f(x[n][i]) W[o][i] */

@@ -29,6 +29,8 @@ EXPORTED_SYMBOLS = [
     'tha4_siren_morpher_backward', 'tha4_siren_face_morpher_backward',
     'tha4_siren_morpher_backward_ex', 'tha4_siren_face_morpher_backward_ex',
     'tha4_adam_step', 'tha4_images_differ', 'tha4_frame_to_srgb8', 'tha4_rgba8_to_poser_image', 'tha4_grid_sample', 'tha4_resize_bilinear',
+    'tha4_eyebrow_decomposer_backward', 'tha4_eyebrow_morphing_combiner_backward', 'tha4_face_morpher_backward',
+    'tha4_test_conv_backward_data', 'tha4_test_norm_backward', 'tha4_test_tail_backward',
     'tha4_base_grid', 'tha4_test_conv', 'tha4_test_conv_norm', 'tha4_test_conv_norm_ex', 'tha4_test_norm', 'tha4_test_tail', 'tha4_test_attention', 'tha4_test_linear',
     'tha4_test_siren_level', 'tha4_test_sine', 'tha4_test_siren_plan_check',
 ]
@@ -100,6 +102,7 @@ class Context:
         self.loaded: Dict[str, object] = {}
         self.epoch = 0                       # bumped whenever options or weights change: results cached by callers are stale
         self.modules = weakref.WeakSet()     # NativeModules whose weights live in this context
+        self.owners: Dict[str, object] = {}  # net name -> weakref to the module whose weights the library holds for it
 
     def __del__(self):
         try:
@@ -189,6 +192,62 @@ class Context:
         outs = self._empty([(4, 192), (1, 192), (4, 192), (4, 192), (1, 192), (4, 192), (4, 192), (2, 192)], B)
         self._call('tha4_face_morpher_forward', _ptr(image), _ptr(pose), 27, B, _ptr_array(outs), self._stream())
         return outs
+
+    DECOMPOSER_SPECS = [(4, 128), (1, 128), (4, 128), (4, 128), (1, 128), (4, 128)]
+    COMBINER_SPECS = [(4, 128), (1, 128), (4, 128), (4, 128), (1, 128), (4, 128), (4, 128), (2, 128)]
+    FACE_MORPHER_SPECS = [(4, 192), (1, 192), (4, 192), (4, 192), (1, 192), (4, 192), (4, 192), (2, 192)]
+
+    def _grads(self, specs, grad_outputs: Sequence[Optional[Tensor]], B: int) -> List[Optional[Tensor]]:
+        assert len(grad_outputs) == len(specs)
+        gs = []
+        for i, ((c, s), g) in enumerate(zip(specs, grad_outputs)):
+            if g is not None:
+                g = _check_input(g, self.device, 'gradient of output %d' % i)
+                assert g.shape == (B, c, s, s), (i, tuple(g.shape))
+            gs.append(g)
+        return gs
+
+    def eyebrow_decomposer_backward(self, image: Tensor, grad_outputs: Sequence[Optional[Tensor]], d_image: Tensor):
+        """d_image [B,4,128,128] <- the input gradient of EyebrowDecomposer00 for the upstream gradients of its six outputs
+        (None = zero); the forward is recomputed in the context's precision mode."""
+        image = _check_input(image, self.device, 'image')
+        B = image.shape[0]
+        assert image.shape[1:] == (4, 128, 128)
+        gs = self._grads(self.DECOMPOSER_SPECS, grad_outputs, B)
+        self._check_out(d_image, (B, 4, 128, 128), 'd_image')
+        self._call('tha4_eyebrow_decomposer_backward', _ptr(image), B, _ptr_array(gs), _ptr(d_image), self._stream())
+
+    def eyebrow_morphing_combiner_backward(self, background_layer: Tensor, eyebrow_layer: Tensor, pose: Tensor,
+                                           grad_outputs: Sequence[Optional[Tensor]], d_background_layer: Optional[Tensor] = None,
+                                           d_eyebrow_layer: Optional[Tensor] = None, d_pose: Optional[Tensor] = None):
+        """Input gradients of EyebrowMorphingCombiner00 into any of d_background_layer / d_eyebrow_layer [B,4,128,128] and
+        d_pose [B,12] (None = not computed)."""
+        assert d_background_layer is not None or d_eyebrow_layer is not None or d_pose is not None
+        background_layer = _check_input(background_layer, self.device, 'background_layer')
+        eyebrow_layer = _check_input(eyebrow_layer, self.device, 'eyebrow_layer')
+        pose = _check_input(pose, self.device, 'pose')
+        B = background_layer.shape[0]
+        assert background_layer.shape[1:] == (4, 128, 128) and eyebrow_layer.shape == background_layer.shape and pose.shape == (B, 12)
+        gs = self._grads(self.COMBINER_SPECS, grad_outputs, B)
+        self._check_out(d_background_layer, (B, 4, 128, 128), 'd_background_layer')
+        self._check_out(d_eyebrow_layer, (B, 4, 128, 128), 'd_eyebrow_layer')
+        self._check_out(d_pose, (B, 12), 'd_pose')
+        self._call('tha4_eyebrow_morphing_combiner_backward', _ptr(background_layer), _ptr(eyebrow_layer), _ptr(pose), 12, B,
+                   _ptr_array(gs), _ptr(d_background_layer), _ptr(d_eyebrow_layer), _ptr(d_pose), self._stream())
+
+    def face_morpher_backward(self, image: Tensor, pose: Tensor, grad_outputs: Sequence[Optional[Tensor]],
+                              d_image: Optional[Tensor] = None, d_pose: Optional[Tensor] = None):
+        """Input gradients of FaceMorpher08 into d_image [B,4,192,192] and / or d_pose [B,27] (None = not computed)."""
+        assert d_image is not None or d_pose is not None
+        image = _check_input(image, self.device, 'image')
+        pose = _check_input(pose, self.device, 'pose')
+        B = image.shape[0]
+        assert image.shape[1:] == (4, 192, 192) and pose.shape == (B, 27)
+        gs = self._grads(self.FACE_MORPHER_SPECS, grad_outputs, B)
+        self._check_out(d_image, (B, 4, 192, 192), 'd_image')
+        self._check_out(d_pose, (B, 27), 'd_pose')
+        self._call('tha4_face_morpher_backward', _ptr(image), _ptr(pose), 27, B, _ptr_array(gs), _ptr(d_image), _ptr(d_pose),
+                   self._stream())
 
     def morpher(self, image: Tensor, pose: Tensor) -> List[Tensor]:
         image = _check_input(image, self.device, 'image')

@@ -188,6 +188,12 @@ void offset_outputs(float* const* outputs, const OutSpec* spec, int n0, float** 
     for (int i = 0; i < NOUT; ++i) dst[i] = outputs[i] + (size_t)n0 * spec[i].c * spec[i].s * spec[i].s;
 }
 
+// the upstream gradients of one micro-batch (an entry may be null)
+template <int NOUT>
+void offset_grads(const float* const* grads, const OutSpec* spec, int n0, const float** dst) {
+    for (int i = 0; i < NOUT; ++i) dst[i] = (grads && grads[i]) ? grads[i] + (size_t)n0 * spec[i].c * spec[i].s * spec[i].s : nullptr;
+}
+
 
 }  // namespace
 
@@ -343,6 +349,56 @@ int tha4_face_morpher_forward(tha4_ctx* ctx, const float* image, const float* po
             float* o[8]; offset_outputs<8>(outputs, kFace, n0, o);
             ctx->face->forward(rt, make_img(image + (size_t)n0 * 4 * 192 * 192, b, 4, 192, 192), ImgView{},
                                pose + (size_t)n0 * pose_ld, pose_ld, o);
+        });
+    });
+}
+
+int tha4_eyebrow_decomposer_backward(tha4_ctx* ctx, const float* image, int B, const float* const* grad_outputs,
+                                     float* d_image, void* stream) {
+    return guarded(ctx, [&] {
+        THA4_REQUIRE(d_image != nullptr, "decomposer backward: no gradient requested");
+        Runtime rt = make_rt(ctx, stream);
+        for_chunks(ctx, B, rt.stream, [&](int n0, int b) {
+            const float* g[6]; offset_grads<6>(grad_outputs, kEncDecDecomposer, n0, g);
+            EncDecGrads eg; eg.grad_outputs = g; eg.d_image0 = d_image + (size_t)n0 * 4 * 128 * 128;
+            ctx->decomposer->backward(rt, make_img(image + (size_t)n0 * 4 * 128 * 128, b, 4, 128, 128), ImgView{}, nullptr, 0, eg);
+        });
+    });
+}
+
+int tha4_eyebrow_morphing_combiner_backward(tha4_ctx* ctx, const float* background_layer, const float* eyebrow_layer,
+                                            const float* pose, int pose_ld, int B, const float* const* grad_outputs,
+                                            float* d_background_layer, float* d_eyebrow_layer, float* d_pose, void* stream) {
+    return guarded(ctx, [&] {
+        THA4_REQUIRE(d_background_layer || d_eyebrow_layer || d_pose, "combiner backward: no gradient requested");
+        THA4_REQUIRE(pose_ld >= 12, "combiner backward: pose rows need at least 12 entries");
+        Runtime rt = make_rt(ctx, stream);
+        for_chunks(ctx, B, rt.stream, [&](int n0, int b) {
+            const float* g[8]; offset_grads<8>(grad_outputs, kCombiner, n0, g);
+            const size_t off = (size_t)n0 * 4 * 128 * 128;
+            EncDecGrads eg; eg.grad_outputs = g;
+            eg.d_image0 = d_eyebrow_layer ? d_eyebrow_layer + off : nullptr;
+            eg.d_image1 = d_background_layer ? d_background_layer + off : nullptr;
+            eg.d_pose = d_pose ? d_pose + (size_t)n0 * 12 : nullptr; eg.d_pose_ld = 12;
+            ctx->combiner->backward(rt, make_img(eyebrow_layer + off, b, 4, 128, 128), make_img(background_layer + off, b, 4, 128, 128),
+                                    pose + (size_t)n0 * pose_ld, pose_ld, eg);
+        });
+    });
+}
+
+int tha4_face_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
+                               const float* const* grad_outputs, float* d_image, float* d_pose, void* stream) {
+    return guarded(ctx, [&] {
+        THA4_REQUIRE(d_image || d_pose, "face morpher backward: no gradient requested");
+        THA4_REQUIRE(pose_ld >= 27, "face morpher backward: pose rows need at least 27 entries");
+        Runtime rt = make_rt(ctx, stream);
+        for_chunks(ctx, B, rt.stream, [&](int n0, int b) {
+            const float* g[8]; offset_grads<8>(grad_outputs, kFace, n0, g);
+            EncDecGrads eg; eg.grad_outputs = g;
+            eg.d_image0 = d_image ? d_image + (size_t)n0 * 4 * 192 * 192 : nullptr;
+            eg.d_pose = d_pose ? d_pose + (size_t)n0 * 27 : nullptr; eg.d_pose_ld = 27;
+            ctx->face->backward(rt, make_img(image + (size_t)n0 * 4 * 192 * 192, b, 4, 192, 192), ImgView{}, pose + (size_t)n0 * pose_ld,
+                                pose_ld, eg);
         });
     });
 }
@@ -917,6 +973,79 @@ int tha4_test_tail(tha4_ctx* ctx, int kind, const float* feature, int N, int C, 
             tail_forward((TailKind)kind, tw, f, coef, a, i0, i1, outputs, s, strict);
         }
         THA4_CUDA_CHECK(cudaStreamSynchronize(s));       // `sink` frees the head weights on return
+    });
+}
+
+int tha4_test_conv_backward_data(tha4_ctx* ctx, int kind, const float* dy, const float* w, float* dx, int N, int Cin, int H, int W,
+                                 int Cout, int strict, void* stream) {
+    return guarded(ctx, [&] {
+        cudaStream_t s = (cudaStream_t)stream;
+        begin_pass(ctx, s);
+        THA4_REQUIRE(kind >= 0 && kind <= 2 && Cout % 4 == 0 && (kind == 0 || Cin % 4 == 0),
+                     "test_conv_backward_data: kind 0..2, Cout % 4 == 0 (and Cin % 4 == 0 for the 4x4 kinds)");
+        Runtime rt = make_rt(ctx, stream);
+        rt.strict = strict;
+        Pool* P = &ctx->persist;
+        AllocSink sink;
+        ConvWeights cw;
+        {
+            SinkScope own(&sink);
+            conv_set_pack_rounding(!strict);
+            conv_pack_adjoint(cw, (ConvKind)kind, w, Cin, Cout, kind == CONV_3x3 ? round_up(Cin, 4) : 0, s);
+        }
+        const int cin_k = kind == CONV_3x3 ? round_up(Cin, 4) : Cin;
+        const int Ho = kind == 1 ? H / 2 : (kind == 2 ? 2 * H : H), Wo = kind == 1 ? W / 2 : (kind == 2 ? 2 * W : W);
+        auto mk = [&](int h, int ww, int c) { View v; v.N = N; v.H = h; v.W = ww; v.C = c; v.ld = c; v.p = P->alloc((size_t)N * h * ww * c); return v; };
+        View g = mk(Ho, Wo, Cout);
+        nchw_to_nhwc(make_img(dy, N, Cout, Ho, Wo), g, s);
+        View o = mk(H, W, cin_k);
+        ConvArgs a;
+        a.in = g; a.out = o; a.strict = strict;
+        const size_t wsf = conv_workspace_floats(cw, a);
+        if (wsf) { a.ws = ctx->scratch.alloc(wsf); a.ws_floats = wsf; }
+        conv_forward(cw, a, s);
+        nhwc_to_nchw(o.slice(0, Cin), dx, s);
+        THA4_CUDA_CHECK(cudaStreamSynchronize(s));       // `sink` frees the packed weights on return
+    });
+}
+
+int tha4_test_norm_backward(tha4_ctx* ctx, const float* x, int N, int C, int H, int W, const float* gamma, const float* beta,
+                            int act, const float* dy, float* dx, void* stream) {
+    return guarded(ctx, [&] {
+        cudaStream_t s = (cudaStream_t)stream;
+        begin_pass(ctx, s);
+        Runtime rt = make_rt(ctx, stream);
+        Pool* P = &ctx->persist;
+        auto mk = [&](int c) { View v; v.N = N; v.H = H; v.W = W; v.C = c; v.ld = c; v.p = P->alloc((size_t)N * H * W * c); return v; };
+        View xin = mk(C);
+        xin.stats_rep = 2; xin.stats_rep_stride = (long)N * C * 2;
+        xin.stats = rt.alloc_stats((size_t)2 * N * C * 2); xin.stats_ld = C;
+        nchw_to_nhwc(make_img(x, N, C, H, W), xin, s);
+        norm_stats(xin, s);
+        View g = mk(C), o = mk(C);
+        nchw_to_nhwc(make_img(dy, N, C, H, W), g, s);
+        norm_backward(xin, gamma, beta, act, g, o, rt.alloc_stats((size_t)N * C * 2), s);
+        nhwc_to_nchw(o, dx, s);
+    });
+}
+
+int tha4_test_tail_backward(tha4_ctx* ctx, int kind, const float* const* outputs, int N, int S, const float* image0,
+                            const float* image1, const float* const* grad_outputs, float* d_head, float* d_image0,
+                            float* d_image1, void* stream) {
+    return guarded(ctx, [&] {
+        cudaStream_t s = (cudaStream_t)stream;
+        THA4_REQUIRE(kind >= TAIL_DECOMPOSER && kind <= TAIL_FACE, "test_tail_backward: kind 1..3");
+        THA4_REQUIRE(!image1 == (kind != TAIL_COMBINER), "test_tail_backward: image1 is the combiner's background layer");
+        begin_pass(ctx, s);
+        Pool* P = &ctx->persist;
+        auto mk = [&](int c) { View v; v.N = N; v.H = S; v.W = S; v.C = c; v.ld = c; v.p = P->alloc((size_t)N * S * S * c); return v; };
+        View dh = mk(16), dimg = mk(8);
+        THA4_CUDA_CHECK(cudaMemsetAsync(dimg.p, 0, dimg.pixels() * 8 * sizeof(float), s));
+        tail_backward((TailKind)kind, outputs, grad_outputs, make_img(image0, N, 4, S, S), image1 ? make_img(image1, N, 4, S, S) : ImgView{},
+                      dh, d_image0 ? dimg.p : nullptr, d_image1 ? dimg.p + 4 : nullptr, 8, s);
+        nhwc_to_nchw(dh.slice(0, 12), d_head, s);
+        if (d_image0) nhwc_to_nchw(dimg.slice(0, 4), d_image0, s);
+        if (d_image1) nhwc_to_nchw(dimg.slice(4, 4), d_image1, s);
     });
 }
 

@@ -48,6 +48,11 @@ size_t conv_packed_floats(const ConvWeights& cw);
 void conv_pack(const ConvWeights& cw, ConvKind kind, const float* w_ref, int w_cin, int cin_offset, cudaStream_t s);
 void conv_set_pack_rounding(bool round_tf32);   // applies to subsequent conv_pack calls (set from the context's strict option)
 bool conv_pack_rounding();
+// Data gradient of a conv as a conv of the same family (encdec_backward.cu): packs the adjoint of the FORWARD conv `kind`
+// (w_ref [cout,cin,k,k], or [cin,cout,4,4] for CONVT_4x4_S2) into cw, a conv from cout to cin channels (cout_kernel > cin:
+// zero extra output channels).  3x3 s1 p1 -> 3x3 with W^T flipped; 4x4 s2 conv <-> 4x4 s2 transposed conv, same tensor.
+// Allocates cw.w with tracked_malloc; honours conv_pack_rounding().
+void conv_pack_adjoint(ConvWeights& cw, ConvKind kind, const float* w_ref, int cin, int cout, int cout_kernel, cudaStream_t s);
 
 // Pending normalisation of the conv's INPUT, applied by the wgmma kernel to its f16 operand tiles in shared memory
 // (conv_tc.cu, XF kernels): y = act(A_c x + B_c) with (A, B) built per CTA from the statistics the producing conv

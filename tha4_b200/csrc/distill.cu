@@ -199,47 +199,6 @@ __global__ void pad_bias_kernel(const float* __restrict__ b, int nreal, int npad
     if (i < npad) dst[i] = i < nreal ? b[i] : 0.0f;
 }
 
-// Bilinear sample of one pixel at base + grid change (the arithmetic of gridsample.cuh), with what its backward needs.
-// mx / my: d(ix)/d(grid_x), d(iy)/d(grid_y) = R/2 inside the image, 0 where the border clamp is active (ATen
-// clip_coordinates_set_grad).  Out-of-range corners read as 0.
-struct SampleAt {
-    int x0, y0;
-    bool xin, yin;
-    float tx, ty, mx, my;
-};
-__device__ __forceinline__ SampleAt sample_locate(const float* __restrict__ base, int x, int y, float gcx, float gcy, int R) {
-    SampleAt s;
-    const float ixu = __fdiv_rn(__fsub_rn(__fmul_rn(__fadd_rn(__fadd_rn(base[x], gcx), 1.0f), (float)R), 1.0f), 2.0f);
-    const float iyu = __fdiv_rn(__fsub_rn(__fmul_rn(__fadd_rn(__fadd_rn(base[y], gcy), 1.0f), (float)R), 1.0f), 2.0f);
-    const float ix = fminf((float)(R - 1), fmaxf(ixu, 0.0f)), iy = fminf((float)(R - 1), fmaxf(iyu, 0.0f));
-    s.mx = (ixu <= 0.0f || ixu >= (float)(R - 1)) ? 0.0f : 0.5f * R;
-    s.my = (iyu <= 0.0f || iyu >= (float)(R - 1)) ? 0.0f : 0.5f * R;
-    const float fx = floorf(ix), fy = floorf(iy);
-    s.x0 = (int)fx; s.y0 = (int)fy;
-    s.xin = s.x0 + 1 < R; s.yin = s.y0 + 1 < R;
-    s.tx = ix - fx; s.ty = iy - fy;
-    return s;
-}
-// the four corners of one channel plane `im` (row stride sh), the sampled value and its derivatives w.r.t. ix and iy
-struct Corners { float v00, v01, v10, v11; };
-__device__ __forceinline__ Corners sample_corners(const float* im, long sh, const SampleAt& s) {
-    Corners v;
-    v.v00 = im[(long)s.y0 * sh + s.x0];
-    v.v01 = s.xin ? im[(long)s.y0 * sh + s.x0 + 1] : 0.0f;
-    v.v10 = s.yin ? im[(long)(s.y0 + 1) * sh + s.x0] : 0.0f;
-    v.v11 = (s.xin && s.yin) ? im[(long)(s.y0 + 1) * sh + s.x0 + 1] : 0.0f;
-    return v;
-}
-__device__ __forceinline__ float sample_value(const Corners& v, const SampleAt& s) {
-    return (v.v00 * (1.0f - s.tx) + v.v01 * s.tx) * (1.0f - s.ty) + (v.v10 * (1.0f - s.tx) + v.v11 * s.tx) * s.ty;
-}
-__device__ __forceinline__ float sample_dix(const Corners& v, const SampleAt& s) {
-    return (v.v01 - v.v00) * (1.0f - s.ty) + (v.v11 - v.v10) * s.ty;
-}
-__device__ __forceinline__ float sample_diy(const Corners& v, const SampleAt& s) {
-    return (v.v10 - v.v00) * (1.0f - s.tx) + (v.v11 - v.v01) * s.tx;
-}
-
 // Fused tail: forward of grid_sample + blend, the four L1 terms, and the gradient w.r.t. the head output.
 // out7: [P][8] = grid_change(0,1) alpha(2) colour(3..6) pad; image / targets NCHW.  d_out7: [P][8].
 // loss_acc: doubles [4] = sum|blended-T0|, sum|warped-T2|, sum|grid-T3|, sum|colour-T0|.

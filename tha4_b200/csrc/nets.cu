@@ -193,6 +193,14 @@ Tens slice_act(const Tens& a, int c0, int c) {
     return r;
 }
 
+// the data (fp32 copy if there is one, else the f16 copy) and the statistics slot of a raw conv output
+View raw_view(const Tens& a) {
+    if (a.f.p) return a.f;
+    View v = a.h;
+    v.stats = a.f.stats; v.stats_ld = a.f.stats_ld; v.stats_rep = a.f.stats_rep; v.stats_rep_stride = a.f.stats_rep_stride;
+    return v;
+}
+
 // pending normalisation of `src` (its statistics) with the weights of the layer that follows it in the reference graph
 ConvNormIn norm_in(const View& src_stats, const NormW& nw, int groups, int act, const float* film0 = nullptr,
                    const float* film1 = nullptr, int film1_ld = 0, int C = 0) {
@@ -266,12 +274,13 @@ void EncDecNet::load(const StateDict& sd, cudaStream_t s) {
         tail_add_head(tail_, sd, "eye_alpha.0", true, s);
     }
     if (conv_pack_rounding()) tail_make_half(tail_, s);       // default mode: the wgmma tail's f16 head weights
+    load_adjoints(sd, p, s);
     THA4_CUDA_CHECK(cudaStreamSynchronize(s));
     loaded_ = true;
 }
 
 void EncDecNet::forward(Runtime& rt, const ImgView& image0, const ImgView& image1, const float* pose, int pose_ld,
-                        float* const* outputs) {
+                        float* const* outputs, EncDecTape* tape) {
     THA4_REQUIRE(loaded_, "network weights not loaded");
     THA4_REQUIRE(image0.H == S_ && image0.W == S_ && image0.C == 4, "encdec: image size");
     const int B = image0.N;
@@ -286,43 +295,54 @@ void EncDecNet::forward(Runtime& rt, const ImgView& image0, const ImgView& image
     } else {
         nchw_to_nhwc(image0, x0, s);
     }
-    if (rt.f16) { forward_fused(rt, x0, image0, image1, pose, pose_ld, outputs); return; }
+    if (tape) tape->x0 = x0;
+    if (rt.f16) { forward_fused(rt, x0, image0, image1, pose, pose_ld, outputs, tape); return; }
     // conv -> InstanceNorm -> ReLU; the activated tensor goes to `dst`, or to a fresh f16 tensor when its only consumer is
-    // a wgmma conv (to16), or back in place
+    // a wgmma conv (to16), or back in place (out of place when a backward keeps the raw output: `keep`)
     const bool h16 = false;
-    auto conv_in_relu = [&](const ConvWeights& cw, const NormW& nw, const View& in, int oh, const View* dst, bool to16) -> View {
+    auto conv_in_relu = [&](const ConvWeights& cw, const NormW& nw, const View& in, int oh, const View* dst, bool to16,
+                            View* keep = nullptr) -> View {
         View raw = make_view(P, B, oh, oh, cw.cout, &rt);
         run_conv(rt, cw, in, raw);
-        const View y = dst ? *dst : (to16 ? make_view16(P, B, oh, oh, cw.cout) : raw);
+        const View y = dst ? *dst : (to16 ? make_view16(P, B, oh, oh, cw.cout) : (keep ? make_view(P, B, oh, oh, cw.cout) : raw));
         run_norm(rt, raw, nw, 0, nullptr, nullptr, 0, ACT_RELU, 0, nullptr, y);
+        if (keep) *keep = raw;
         return y;
     };
-    View f = conv_in_relu(down_[0], down_n_[0], x0, S_, nullptr, false);       // the stride-2 convs read fp32
-    f = conv_in_relu(down_[1], down_n_[1], f, S_ / 2, nullptr, false);
-    f = conv_in_relu(down_[2], down_n_[2], f, S_ / 4, nullptr, false);
+    View f = conv_in_relu(down_[0], down_n_[0], x0, S_, nullptr, false, tape ? &tape->down[0] : nullptr);       // the stride-2 convs read fp32
+    f = conv_in_relu(down_[1], down_n_[1], f, S_ / 2, nullptr, false, tape ? &tape->down[1] : nullptr);
+    f = conv_in_relu(down_[2], down_n_[2], f, S_ / 4, nullptr, false, tape ? &tape->down[2] : nullptr);
     const int b = S_ / 8;
     View bin = h16 ? make_view16(P, B, b, b, 512 + pose_pad_) : make_view(P, B, b, b, 512 + pose_pad_);
     View bfeat = bin.slice(0, 512);
-    conv_in_relu(down_[3], down_n_[3], f, b, &bfeat, false);
+    conv_in_relu(down_[3], down_n_[3], f, b, &bfeat, false, tape ? &tape->down[3] : nullptr);
     if (pose_pad_ > 0) tile_vector(pose, pose_ld, pose_ch_, bin.slice(512, pose_pad_), s);   // poser_encoder_decoder_00.py:110-113
     // the bottleneck stream x is both a residual (fp32) and a conv operand (f16 copy x16)
     View x = make_view(P, B, b, b, bott0_.cout, &rt), x16;
     run_conv(rt, bott0_, bin, x);
     if (h16) x16 = make_view16(P, B, b, b, bott0_.cout);
-    run_norm(rt, x, bott0_n_, 0, nullptr, nullptr, 0, ACT_RELU, 0, nullptr, x, h16 ? &x16 : nullptr);
+    {
+        const View y = tape ? make_view(P, B, b, b, bott0_.cout) : x;
+        run_norm(rt, x, bott0_n_, 0, nullptr, nullptr, 0, ACT_RELU, 0, nullptr, y, h16 ? &x16 : nullptr);
+        if (tape) tape->bott0 = x;
+        x = y;
+    }
     for (int i = 0; i < 5; ++i) {   // ResnetBlock: x + IN(conv(relu(IN(conv(x)))))  (resnet_block.py:52-67)
-        View h = conv_in_relu(res_[i][0], res_n_[i][0], h16 ? x16 : x, b, nullptr, h16);
+        View h = conv_in_relu(res_[i][0], res_n_[i][0], h16 ? x16 : x, b, nullptr, h16, tape ? &tape->res[i][0] : nullptr);
         View raw = make_view(P, B, b, b, 512, &rt);
         run_conv(rt, res_[i][1], h, raw);
         View n16; if (h16) n16 = make_view16(P, B, b, b, 512);
-        run_norm(rt, raw, res_n_[i][1], 0, nullptr, nullptr, 0, ACT_NONE, 0, &x, raw, h16 ? &n16 : nullptr);
-        x = raw; x16 = n16;
+        const View y = tape ? make_view(P, B, b, b, 512) : raw;
+        run_norm(rt, raw, res_n_[i][1], 0, nullptr, nullptr, 0, ACT_NONE, 0, &x, y, h16 ? &n16 : nullptr);
+        if (tape) tape->res[i][1] = raw;
+        x = y; x16 = n16;
     }
-    x = conv_in_relu(up_[0], up_n_[0], h16 ? x16 : x, b * 2, nullptr, h16);
-    x = conv_in_relu(up_[1], up_n_[1], x, b * 4, nullptr, h16);
+    x = conv_in_relu(up_[0], up_n_[0], h16 ? x16 : x, b * 2, nullptr, h16, tape ? &tape->up[0] : nullptr);
+    x = conv_in_relu(up_[1], up_n_[1], x, b * 4, nullptr, h16, tape ? &tape->up[1] : nullptr);
     // last block: leave InstanceNorm + ReLU pending; the tail kernel applies them while staging its halo tile
     View raw = make_view(P, B, S_, S_, 64, &rt);
     run_conv(rt, up_[2], x, raw);
+    if (tape) tape->up[2] = raw;
     float* coef = tail_coef(rt, raw, up_n_[2], 0);
     tail_forward(kind_, tail_, raw, coef, ACT_RELU, image0, image1, outputs, s, rt.strict);
 }
@@ -332,17 +352,19 @@ void EncDecNet::forward(Runtime& rt, const ImgView& image0, const ImgView& image
 // a pass: the bottleneck entry (its result is both a residual stream and an operand) and the end of each ResnetBlock
 // (x + IN(conv(...)), resnet_block.py:64-67).
 void EncDecNet::forward_fused(Runtime& rt, const View& x0, const ImgView& image0, const ImgView& image1, const float* pose,
-                              int pose_ld, float* const* outputs) {
+                              int pose_ld, float* const* outputs, EncDecTape* tape) {
     const int B = x0.N;
     cudaStream_t s = rt.stream;
     Pool* P = rt.persist;
     Tens r0 = make_act(P, rt, B, S_, S_, 64, false, true);
     run_conv_tc(rt, down_[0], x0, nullptr, r0);                                  // fp32 image operand (kind::tf32)
+    if (tape) tape->down[0] = raw_view(r0);
     Tens prev = r0;
     for (int i = 1; i < 3; ++i) {
         Tens r = make_act(P, rt, B, S_ >> i, S_ >> i, down_[i].cout, false, true);
         const ConvNormIn ni = norm_in(prev.f, down_n_[i - 1], 0, ACT_RELU);
         run_conv_tc(rt, down_[i], prev.h, &ni, r);
+        if (tape) tape->down[i] = raw_view(r);
         prev = r;
     }
     const int b = S_ / 8;
@@ -352,6 +374,7 @@ void EncDecNet::forward_fused(Runtime& rt, const View& x0, const ImgView& image0
     {
         const ConvNormIn ni = norm_in(prev.f, down_n_[2], 0, ACT_RELU);
         run_conv_tc(rt, down_[3], prev.h, &ni, r3);
+        if (tape) tape->down[3] = raw_view(r3);
     }
     if (pose_pad_ > 0) tile_vector(pose, pose_ld, pose_ch_, bin16.slice(512, pose_pad_), s);   // poser_encoder_decoder_00.py:110-113
     // bottleneck entry: conv -> IN -> ReLU; the result x is a residual stream (fp32) and a conv operand (f16 copy)
@@ -361,7 +384,10 @@ void EncDecNet::forward_fused(Runtime& rt, const View& x0, const ImgView& image0
         Tens xr; xr.f = x;
         const ConvNormIn ni = norm_in(r3.f, down_n_[3], 0, ACT_RELU, nullptr, nullptr, 0, 512);
         run_conv_tc(rt, bott0_, bin16, &ni, xr);
-        run_norm(rt, x, bott0_n_, 0, nullptr, nullptr, 0, ACT_RELU, 0, nullptr, x, &x16);
+        const View y = tape ? make_view(P, B, b, b, bott0_.cout) : x;
+        run_norm(rt, x, bott0_n_, 0, nullptr, nullptr, 0, ACT_RELU, 0, nullptr, y, &x16);
+        if (tape) tape->bott0 = x;
+        x = y;
     }
     for (int i = 0; i < 5; ++i) {   // ResnetBlock: x + IN(conv(relu(IN(conv(x)))))  (resnet_block.py:52-67)
         Tens ha = make_act(P, rt, B, b, b, 512, false, true);
@@ -370,8 +396,10 @@ void EncDecNet::forward_fused(Runtime& rt, const View& x0, const ImgView& image0
         const ConvNormIn ni = norm_in(ha.f, res_n_[i][0], 0, ACT_RELU);
         run_conv_tc(rt, res_[i][1], ha.h, &ni, hb);
         View n16 = make_view16(P, B, b, b, 512);
-        run_norm(rt, hb.f, res_n_[i][1], 0, nullptr, nullptr, 0, ACT_NONE, 0, &x, hb.f, &n16);
-        x = hb.f; x16 = n16;
+        const View y = tape ? make_view(P, B, b, b, 512) : hb.f;
+        run_norm(rt, hb.f, res_n_[i][1], 0, nullptr, nullptr, 0, ACT_NONE, 0, &x, y, &n16);
+        if (tape) { tape->res[i][0] = raw_view(ha); tape->res[i][1] = hb.f; }
+        x = y; x16 = n16;
     }
     Tens u0 = make_act(P, rt, B, 2 * b, 2 * b, up_[0].cout, false, true);
     run_conv_tc(rt, up_[0], x16, nullptr, u0);
@@ -380,6 +408,7 @@ void EncDecNet::forward_fused(Runtime& rt, const View& x0, const ImgView& image0
         const ConvNormIn ni = norm_in(u0.f, up_n_[0], 0, ACT_RELU);
         run_conv_tc(rt, up_[1], u0.h, &ni, u1);
     }
+    if (tape) { tape->up[0] = raw_view(u0); tape->up[1] = raw_view(u1); }
     // last block: InstanceNorm + ReLU stay pending; the tail kernel applies them while staging its halo tile
     const bool tc_tail = tail_.w16 != nullptr;
     Tens feat = make_act(P, rt, B, S_, S_, 64, !tc_tail, tc_tail);
@@ -387,6 +416,7 @@ void EncDecNet::forward_fused(Runtime& rt, const View& x0, const ImgView& image0
         const ConvNormIn ni = norm_in(u1.f, up_n_[1], 0, ACT_RELU);
         run_conv_tc(rt, up_[2], u1.h, &ni, feat);
     }
+    if (tape) tape->up[2] = raw_view(feat);
     if (tc_tail) {
         View fv = feat.h;                                 // f16 data + the statistics slot of the tensor
         fv.stats = feat.f.stats; fv.stats_ld = feat.f.stats_ld; fv.stats_rep = feat.f.stats_rep; fv.stats_rep_stride = feat.f.stats_rep_stride;

@@ -51,6 +51,24 @@ struct Runtime {                      // per-call execution context
 };
 
 // ------------------------------------------------------------------ encoder-decoder networks
+// The activations a backward pass reads from the forward it recomputes: the NHWC network input and the RAW output of every
+// conv that is followed by an InstanceNorm (fp32 or f16 data, with the statistics the producing conv accumulated).
+struct EncDecTape {
+    View x0;
+    View down[4], bott0, res[5][2], up[3];
+};
+
+// What EncDecNet::backward computes.  grad_outputs: the upstream gradients of the network's outputs (NCHW, an entry may be
+// null = zero).  Every other pointer is an output, null = not computed: d_image0 / d_image1 follow forward()'s image0 /
+// image1, d_pose is [N][d_pose_ld] (its first pose_ch entries per row are written).
+struct EncDecGrads {
+    const float* const* grad_outputs = nullptr;
+    float* d_image0 = nullptr;
+    float* d_image1 = nullptr;
+    float* d_pose = nullptr;
+    int d_pose_ld = 0;
+};
+
 // EyebrowDecomposer00 / EyebrowMorphingCombiner00 / FaceMorpher08 (poser_encoder_decoder_00.py:43-121,
 // face_morpher_08.py:48-202): conv3 + 3 stride-2 convs, bottleneck conv (pose concat) + 5 ResnetBlocks, 3 transposed
 // convs, fused head tail.
@@ -61,13 +79,17 @@ public:
     // image0 / image1: see tail.cu (decomposer, face: image1 unused; combiner: image0 = eyebrow layer,
     // image1 = background layer, network input = cat(background, eyebrow)).
     void forward(Runtime& rt, const ImgView& image0, const ImgView& image1, const float* pose, int pose_ld,
-                 float* const* outputs);
+                 float* const* outputs, EncDecTape* tape = nullptr);
+    // Input gradients (encdec_backward.cu): recomputes the forward in the context's precision mode, keeping its activations,
+    // then runs the adjoint of every layer back to the inputs that were asked for.
+    void backward(Runtime& rt, const ImgView& image0, const ImgView& image1, const float* pose, int pose_ld, const EncDecGrads& g);
     int size() const { return S_; }
     int num_outputs() const { return kind_ == TAIL_DECOMPOSER ? 6 : 8; }
     bool loaded() const { return loaded_; }
 private:
     void forward_fused(Runtime& rt, const View& x0, const ImgView& image0, const ImgView& image1, const float* pose, int pose_ld,
-                       float* const* outputs);
+                       float* const* outputs, EncDecTape* tape);
+    void load_adjoints(const StateDict& sd, const std::string& prefix, cudaStream_t s);
     AllocSink owned_;          // every device allocation made by load()
     TailKind kind_;
     int S_, in_ch_, pose_ch_, pose_pad_;
@@ -75,6 +97,8 @@ private:
     ConvWeights down_[4], bott0_, res_[5][2], up_[3];
     NormW down_n_[4], bott0_n_, res_n_[5][2], up_n_[3];
     TailWeights tail_;
+    // adjoint-packed weights (data gradients on the same conv kernels): 3x3 -> 3x3 with W^T flipped, 4x4 s2 <-> transposed
+    ConvWeights adj_down_[4], adj_bott0_, adj_res_[5][2], adj_up_[3], adj_head_;
 };
 
 // ------------------------------------------------------------------ U-Net networks

@@ -100,4 +100,14 @@ void tail_tc_enable_persist(bool on);      // option "tail_persist": persistent 
 void tail_tc_forward(TailKind kind, const TailWeights& tw, const View& feature, const NormSpecTail& ns, const ImgView& image0,
                      const ImgView& image1, float* const* outputs, cudaStream_t s, const View* gather0 = nullptr, const View* gather1 = nullptr);
 
+// ---------------------------------------------------------------- backward of the encoder-decoder networks (encdec_backward.cu)
+// InstanceNorm2d(affine) (+ReLU) backward: dx = d/dx of y = act(gamma (x - mean) rstd + beta) for the upstream gradient dy.
+// x: the RAW input (fp32 or f16) with its statistics; dy / dx fp32.  sums: N*C*2 zeroed doubles of workspace.
+void norm_backward(const View& x, const float* gamma, const float* beta, int act, const View& dy, const View& dx, double* sums, cudaStream_t s);
+// Encoder-decoder tail backward (decomposer / combiner / face): from the forward's outputs and their upstream gradients
+// (grads[k] may be null) to dh [N,S,S,16] (head pre-activation gradients in the tail's channel order, rest zero) and the image
+// terms: d0 / d1 NHWC with `dld` floats per pixel (null = not wanted); d0 must be zero on entry for the warping kinds.
+void tail_backward(TailKind kind, const float* const* outputs, const float* const* grads, const ImgView& image0, const ImgView& image1,
+                   const View& dh, float* d0, float* d1, int dld, cudaStream_t s);
+
 }  // namespace tha4

@@ -1,6 +1,7 @@
 """Base class of the seven network modules: an `nn.Module` that owns parameters under the reference's state_dict
 keys and whose forward is one C-ABI call into libtha4_b200.so (no PyTorch-op fallback)."""
 import math
+import weakref
 from typing import Dict, Optional
 
 import torch
@@ -121,9 +122,12 @@ class NativeModule(Module):
             self._param_cache = None
         params = self._params()
         key = (id(params[0]), params[0].data_ptr(), [p._version for p in params])
-        if key != self._uploaded_key:
+        owner = ctx.owners.get(self.NET_NAME)
+        if key != self._uploaded_key or (owner is not None and owner() is not self):
+            # (re)upload: weights changed, or another module of this class loaded its own weights into the context since
             ctx.load_net(self.NET_NAME, self.state_dict())
             ctx.modules.add(self)
+            ctx.owners[self.NET_NAME] = weakref.ref(self)
             self._uploaded_key = key
         return ctx
 

@@ -82,30 +82,36 @@ class FiveStepPoserComputationProtocol(CachedComputationProtocol):
             for net in Network:
                 if net.name in state.modules:
                     state.modules[net.name].sync_weights()
-            # one image posed B times (image.expand(B, ...)) is compared through its single stored frame
-            key_image = image[:1] if (image.shape[0] > 1 and image.stride(0) == 0) else image
-            if (self.cached_batch_0 is None or image.shape[0] != self.cached_batch_size
-                    or key_image.shape != self.cached_batch_0.shape
-                    or self.cached_epoch != ctx.epoch):          # options / weights changed: cached outputs are stale
-                new_batch_0 = True
-            elif self.trust_image_identity and key_image is self.cached_batch_0 and key_image._version == self.cached_version:
-                new_batch_0 = False
-            else:
-                new_batch_0 = ctx.images_differ(key_image, self.cached_batch_0)
+            new_batch_0, key_image = self.eyebrow_cache_miss(ctx, image)
             cached = None if new_batch_0 else self.cached_eyebrow_decomposer_output
             output = ctx.teacher_forward(self.TEACHER_MODE, image, state.batch[1], self.eyebrow_morphed_image_index, cached)
             for key, sl in self.SLICES.items():
                 state.outputs[key] = output[sl]
             state.outputs[Branch.all_outputs.name] = output
             if new_batch_0:
-                self.cached_batch_0 = key_image
-                self.cached_batch_size = image.shape[0]
-                self.cached_version = key_image._version
-                self.cached_epoch = ctx.epoch
-                self.cached_eyebrow_decomposer_output = output[self.SLICES[Network.eyebrow_decomposer.outputs_key]]
+                self.eyebrow_cache_store(ctx, image, key_image, output[self.SLICES[Network.eyebrow_decomposer.outputs_key]])
             return output
 
         return func
+
+    def eyebrow_cache_miss(self, ctx, image: Tensor):
+        """(True iff the cached decomposer outputs cannot be used for `image`, the tensor the cache is keyed by)."""
+        # one image posed B times (image.expand(B, ...)) is compared through its single stored frame
+        key_image = image[:1] if (image.shape[0] > 1 and image.stride(0) == 0) else image
+        if (self.cached_batch_0 is None or image.shape[0] != self.cached_batch_size
+                or key_image.shape != self.cached_batch_0.shape
+                or self.cached_epoch != ctx.epoch):          # options / weights changed: cached outputs are stale
+            return True, key_image
+        if self.trust_image_identity and key_image is self.cached_batch_0 and key_image._version == self.cached_version:
+            return False, key_image
+        return ctx.images_differ(key_image, self.cached_batch_0), key_image
+
+    def eyebrow_cache_store(self, ctx, image: Tensor, key_image: Tensor, decomposer_outputs: List[Tensor]):
+        self.cached_batch_0 = key_image
+        self.cached_batch_size = image.shape[0]
+        self.cached_version = key_image._version
+        self.cached_epoch = ctx.epoch
+        self.cached_eyebrow_decomposer_output = decomposer_outputs
 
     def compute_output(self, key: str, state: ComputationState) -> List[Tensor]:
         if key in self.SLICES or key == Branch.all_outputs.name:
