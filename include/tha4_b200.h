@@ -162,33 +162,29 @@ int64_t tha4_siren_face_morpher_param_count(void);
 int tha4_siren_face_morpher_train_step(tha4_ctx* ctx, const float* pose, int pose_ld, const float* target, const float* mask,
                                        const float* loss_weights, const float* params, float* grads, double* host_loss_means,
                                        int B, void* stream);
-/* ---- parameter gradients of the students for arbitrary upstream gradients (backward of the modules under torch.autograd) ---- */
-/* dL/d params of SirenMorpher03 at (image [B,4,512,512], pose [B,45]) for upstream gradients grad_outputs[5] =
- * d blended, d alpha, d color_change, d warped, d grid_change (NCHW fp32, contiguous; NULL = zero).
- * params / grads: flat fp32 in state_dict order (331 567); grads is overwritten.  The forward is recomputed (TF32
- * products, as in tha4_siren_morpher_train_step).  Any B >= 1 (micro-batches of <= 8). */
-int tha4_siren_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
-                                const float* const* grad_outputs, const float* params, float* grads, void* stream);
-/* same for SirenFaceMorpher00: pose [B, >= 39] rows pose_ld apart, grad_output [B,4,128,128] (121 476 params;
- * micro-batches of <= 64) */
-int tha4_siren_face_morpher_backward(tha4_ctx* ctx, const float* pose, int pose_ld, int B, const float* grad_output,
-                                     const float* params, float* grads, void* stream);
-/* ---- input gradients of the students (frozen students under torch.autograd: pose fitting, training through them) ---- */
-/* The backward of SirenMorpher03 with every output optional (NULL = not computed; at least one non-NULL; each is
- * overwritten):
- *   grads   [331 567]      dL/d params, as tha4_siren_morpher_backward;
+/* ---- backward of the students under torch.autograd: parameter gradients, and input gradients of frozen students ---- */
+/* ABI note: these two names used to declare parameter-gradient-only entries without the grid_change / alpha / d_image /
+ * d_pose arguments.  A binding written against that signature must be updated; tha4_b200/_lib.py, the only one in this
+ * tree, ships with the library.
+ * The backward of SirenMorpher03 at (image [B,4,512,512], pose [B,45]) for upstream gradients grad_outputs[5] =
+ * d blended, d alpha, d color_change, d warped, d grid_change (NCHW fp32, contiguous; NULL = zero).  Every output is
+ * optional (NULL = not computed; at least one non-NULL; each is overwritten):
+ *   grads   [331 567]      dL/d params, flat fp32 in state_dict order (params: the same layout).  The forward is
+ *                          recomputed with TF32 products, as in tha4_siren_morpher_train_step;
  *   d_image [B,4,512,512]  dL/d image: the exact adjoint of the warp the forward returned, computed from its returned
  *                          grid_change [B,2,512,512] and alpha [B,1,512,512] and grad_outputs[0] / [3] (d blended,
  *                          d warped) with no SIREN recompute.  Float atomics: not bit-reproducible run to run;
  *   d_pose  [B,45]         dL/d pose of the TF32 recompute (as grads); fixed-order reduction, bit-reproducible.
  * grid_change / alpha are needed only for d_image; image / pose / params only for grads / d_pose.  Any B >= 1
  * (micro-batches of <= 8). */
-int tha4_siren_morpher_backward_ex(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
-                                   const float* const* grad_outputs, const float* grid_change, const float* alpha,
-                                   const float* params, float* grads, float* d_image, float* d_pose, void* stream);
-/* same for SirenFaceMorpher00: grads [121 476] and / or d_pose [B,39] (micro-batches of <= 64) */
-int tha4_siren_face_morpher_backward_ex(tha4_ctx* ctx, const float* pose, int pose_ld, int B, const float* grad_output,
-                                        const float* params, float* grads, float* d_pose, void* stream);
+int tha4_siren_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
+                                const float* const* grad_outputs, const float* grid_change, const float* alpha,
+                                const float* params, float* grads, float* d_image, float* d_pose, void* stream);
+/* The backward of SirenFaceMorpher00 at pose [B, >= 39] (rows pose_ld apart) for the upstream gradient grad_output
+ * [B,4,128,128] (required), into grads [121 476] (as above) and / or d_pose [B,39] (every output optional, at least one
+ * non-NULL, each overwritten).  Any B >= 1 (micro-batches of <= 64). */
+int tha4_siren_face_morpher_backward(tha4_ctx* ctx, const float* pose, int pose_ld, int B, const float* grad_output,
+                                     const float* params, float* grads, float* d_pose, void* stream);
 /* torch.optim.Adam step on flat buffers (shion/base/optimizer_factories.py:9-17); grads are scaled by grad_scale first
  * (1/world_size after a summing all-reduce = DDP's gradient averaging) */
 int tha4_adam_step(tha4_ctx* ctx, float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t n, float lr,

@@ -2,7 +2,7 @@
 
   fused     *Distiller.train_step: teacher forward, then forward + L1 terms + backward + Adam in the library on flat buffers
   autograd  teacher forward under no_grad, then the student module forward, the same L1 terms in PyTorch, loss.backward()
-            (tha4_siren_*_backward) and torch.optim.Adam over module.parameters()
+            (tha4_siren_*_backward with the parameter gradients requested) and torch.optim.Adam over module.parameters()
   teacher   the teacher forward alone (part of both iterations above)
 
 for the body student (mode_07 teacher) and the face student (mode_12 teacher) at B = 1 and 8.  Also prints the kernel launches

@@ -1,10 +1,11 @@
 """Developer timing of the frozen SIREN students' input gradients (not a pytest file), device time between CUDA events.
 
-One forward + backward of a frozen student module for an MSE loss on its outputs, with the gradient requested for
-  image   the body student's d(image) only (scatter from the returned warp, no SIREN recompute)
-  pose    d(pose) only (TF32 recompute + dgrad chain, no weight gradients)
+One forward + backward of a student module for an MSE loss on its outputs; the backward is one tha4_siren_*_backward
+call that computes only what is requested:
+  image   the frozen body student's d(image) (scatter from the returned warp, no SIREN recompute)
+  pose    the frozen student's d(pose) (TF32 recompute + dgrad chain, no weight gradients)
   both    d(image) and d(pose)
-  params  the parameter backward of the trainable module (tha4_siren_*_backward), for comparison
+  params  the parameter gradients of the trainable module, for comparison
 for the body student at B = 1 and 8 and the face student at B = 1 and 64, with the kernel launches of one backward.
 
 Then a pose-fitting loop: the frozen lambda_00 students composed as in mode_14 (face pasted into the image the body

@@ -242,9 +242,9 @@ def test_body_micro_batches_accumulate(student_sds):
     flat = torch.cat([v.reshape(-1) for v in sd.values()]).to(DEV)
     ctx = G.ctx()
     g10, g8, g2 = torch.empty_like(flat), torch.empty_like(flat), torch.empty_like(flat)
-    ctx.siren_morpher_backward(image, pose, ups, flat, g10)
-    ctx.siren_morpher_backward(image[:8], pose[:8], [u[:8] for u in ups], flat, g8)
-    ctx.siren_morpher_backward(image[8:], pose[8:], [u[8:] for u in ups], flat, g2)
+    ctx.siren_morpher_backward(image, pose, ups, params=flat, grads=g10)
+    ctx.siren_morpher_backward(image[:8], pose[:8], [u[:8] for u in ups], params=flat, grads=g8)
+    ctx.siren_morpher_backward(image[8:], pose[8:], [u[8:] for u in ups], params=flat, grads=g2)
     torch.cuda.synchronize()
     s = g8 + g2
     rel = ((g10 - s).norm() / s.norm()).item()
@@ -258,9 +258,9 @@ def test_face_micro_batches_accumulate(student_sds):
     flat = torch.cat([v.reshape(-1) for v in sd.values()]).to(DEV)
     ctx = G.ctx()
     g70, g64, g6 = torch.empty_like(flat), torch.empty_like(flat), torch.empty_like(flat)
-    ctx.siren_face_morpher_backward(pose, up, flat, g70)
-    ctx.siren_face_morpher_backward(pose[:64], up[:64], flat, g64)
-    ctx.siren_face_morpher_backward(pose[64:], up[64:], flat, g6)
+    ctx.siren_face_morpher_backward(pose, up, flat, grads=g70)
+    ctx.siren_face_morpher_backward(pose[:64], up[:64], flat, grads=g64)
+    ctx.siren_face_morpher_backward(pose[64:], up[64:], flat, grads=g6)
     torch.cuda.synchronize()
     s = g64 + g6
     assert ((g70 - s).norm() / s.norm()).item() <= 1e-5

@@ -256,10 +256,11 @@ def test_body_micro_batches(student_sds):
     for key, sl in (('all', slice(0, 10)), ('8', slice(0, 8)), ('2', slice(8, 10))):
         b = sl.stop - sl.start
         di, dp = torch.empty(b, 4, 512, 512, device=DEV), torch.empty(b, 45, device=DEV)
-        ctx.siren_morpher_backward_ex(image[sl], pose[sl], [u[sl] for u in ups], outs[4][sl], outs[1][sl], flat, d_image=di, d_pose=dp)
+        ctx.siren_morpher_backward(image[sl], pose[sl], [u[sl] for u in ups], grid_change=outs[4][sl], alpha=outs[1][sl], params=flat,
+                                   d_image=di, d_pose=dp)
         res[key] = (di, dp)
     again = torch.empty(10, 45, device=DEV)
-    ctx.siren_morpher_backward_ex(image, pose, ups, outs[4], outs[1], flat, d_pose=again)
+    ctx.siren_morpher_backward(image, pose, ups, params=flat, d_pose=again)
     torch.cuda.synchronize()
     sep_i, sep_p = torch.cat([res['8'][0], res['2'][0]]), torch.cat([res['8'][1], res['2'][1]])
     assert torch.equal(res['all'][1], sep_p)
@@ -274,15 +275,15 @@ def test_face_micro_batches(student_sds):
     up = torch.randn(70, 4, 128, 128, generator=torch.Generator().manual_seed(2)).to(DEV) * 1e-3
     flat = torch.cat([v.reshape(-1) for v in sd.values()]).to(DEV)
     d70, d64, d6 = torch.empty(70, 39, device=DEV), torch.empty(64, 39, device=DEV), torch.empty(6, 39, device=DEV)
-    ctx.siren_face_morpher_backward_ex(pose, up, flat, d_pose=d70)
-    ctx.siren_face_morpher_backward_ex(pose[:64], up[:64], flat, d_pose=d64)
-    ctx.siren_face_morpher_backward_ex(pose[64:], up[64:], flat, d_pose=d6)
+    ctx.siren_face_morpher_backward(pose, up, flat, d_pose=d70)
+    ctx.siren_face_morpher_backward(pose[:64], up[:64], flat, d_pose=d64)
+    ctx.siren_face_morpher_backward(pose[64:], up[64:], flat, d_pose=d6)
     torch.cuda.synchronize()
     assert torch.equal(d70, torch.cat([d64, d6]))
 
 
-def test_parameter_gradients_unchanged_by_the_extended_entry(student_sds):
-    """tha4_siren_morpher_backward_ex with grads (and d pose) gives the parameter gradient of tha4_siren_morpher_backward."""
+def test_parameter_gradients_unchanged_by_other_requested_outputs(student_sds):
+    """tha4_siren_morpher_backward with grads and d pose, or grads and d image, gives the parameter gradient of grads alone."""
     sd = student_sds['body_morpher']
     ctx = G.ctx()
     image, pose = synth.synthetic_image(15, 2).to(DEV), synth.random_poses(2, seed=16).to(DEV)
@@ -290,11 +291,14 @@ def test_parameter_gradients_unchanged_by_the_extended_entry(student_sds):
     with torch.no_grad():
         outs = _body(sd)(image, pose)
     flat = torch.cat([v.reshape(-1) for v in sd.values()]).to(DEV)
-    g_old, g_new, dp = torch.empty_like(flat), torch.empty_like(flat), torch.empty(2, 45, device=DEV)
-    ctx.siren_morpher_backward(image, pose, ups, flat, g_old)
-    ctx.siren_morpher_backward_ex(image, pose, ups, outs[4], outs[1], flat, grads=g_new, d_pose=dp)
+    g_alone, g_pose, g_image = torch.empty_like(flat), torch.empty_like(flat), torch.empty_like(flat)
+    dp, di = torch.empty(2, 45, device=DEV), torch.empty(2, 4, 512, 512, device=DEV)
+    ctx.siren_morpher_backward(image, pose, ups, params=flat, grads=g_alone)
+    ctx.siren_morpher_backward(image, pose, ups, params=flat, grads=g_pose, d_pose=dp)
+    ctx.siren_morpher_backward(image, pose, ups, grid_change=outs[4], alpha=outs[1], params=flat, grads=g_image, d_image=di)
     torch.cuda.synchronize()
-    assert ((g_new - g_old).norm() / g_old.norm()).item() <= 1e-5
+    for g in (g_pose, g_image):
+        assert ((g - g_alone).norm() / g_alone.norm()).item() <= 1e-5
 
 
 # ------------------------------------------------------------------------------------------ hygiene

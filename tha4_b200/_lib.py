@@ -27,7 +27,6 @@ EXPORTED_SYMBOLS = [
     'tha4_teacher_forward', 'tha4_student_forward', 'tha4_student_forward_io', 'tha4_siren_morpher_param_count', 'tha4_siren_morpher_train_step',
     'tha4_siren_face_morpher_param_count', 'tha4_siren_face_morpher_train_step',
     'tha4_siren_morpher_backward', 'tha4_siren_face_morpher_backward',
-    'tha4_siren_morpher_backward_ex', 'tha4_siren_face_morpher_backward_ex',
     'tha4_adam_step', 'tha4_images_differ', 'tha4_frame_to_srgb8', 'tha4_rgba8_to_poser_image', 'tha4_grid_sample', 'tha4_resize_bilinear',
     'tha4_eyebrow_decomposer_backward', 'tha4_eyebrow_morphing_combiner_backward', 'tha4_face_morpher_backward',
     'tha4_test_conv_backward_data', 'tha4_test_norm_backward', 'tha4_test_tail_backward',
@@ -385,83 +384,61 @@ class Context:
                    _ptr(grads), losses if want_losses else None, B, self._stream())
         return list(losses) if want_losses else None
 
-    def siren_morpher_backward(self, image: Tensor, pose: Tensor, grad_outputs: Sequence[Optional[Tensor]], params: Tensor,
-                               grads: Tensor):
-        """grads <- dL/d params of SirenMorpher03 (flat, state_dict order) for the upstream gradients of its five outputs
-        (None = zero); the forward is recomputed with TF32 products as in the train step.  Any batch size."""
-        image = _check_input(image, self.device, 'image')
-        pose = _check_input(pose, self.device, 'pose')
-        B = image.shape[0]
-        assert image.shape[1:] == (4, 512, 512) and pose.shape == (B, 45) and len(grad_outputs) == 5
-        gs = []
-        for (c, s), g, name in zip(self.SIREN_MORPHER_SPECS, grad_outputs, ('blended', 'alpha', 'color_change', 'warped', 'grid_change')):
-            if g is not None:
-                g = _check_input(g, self.device, 'grad of ' + name)
-                assert g.shape == (B, c, s, s), (name, tuple(g.shape))
-            gs.append(g)
-        assert params.is_contiguous() and grads.is_contiguous() and params.dtype == torch.float32 and grads.dtype == torch.float32
-        assert params.numel() == grads.numel() == self.lib.tha4_siren_morpher_param_count()
-        self._call('tha4_siren_morpher_backward', _ptr(image), _ptr(pose), 45, B, _ptr_array(gs), _ptr(params), _ptr(grads),
-                   self._stream())
-
-    def siren_face_morpher_backward(self, pose: Tensor, grad_output: Tensor, params: Tensor, grads: Tensor):
-        """grads <- dL/d params of SirenFaceMorpher00 for the upstream gradient [B,4,128,128] of its output."""
-        pose = _check_input(pose, self.device, 'pose')
-        grad_output = _check_input(grad_output, self.device, 'grad_output')
-        B = pose.shape[0]
-        assert pose.shape[1] >= 39 and grad_output.shape == (B, 4, 128, 128)
-        assert params.is_contiguous() and grads.is_contiguous() and params.dtype == torch.float32 and grads.dtype == torch.float32
-        assert params.numel() == grads.numel() == self.lib.tha4_siren_face_morpher_param_count()
-        self._call('tha4_siren_face_morpher_backward', _ptr(pose), int(pose.shape[1]), B, _ptr(grad_output), _ptr(params), _ptr(grads),
-                   self._stream())
-
     @staticmethod
     def _check_out(t: Optional[Tensor], shape, name: str):
         if t is not None:
             assert t.shape == shape and t.is_contiguous() and t.dtype == torch.float32, (name, tuple(t.shape))
 
-    def siren_morpher_backward_ex(self, image: Tensor, pose: Tensor, grad_outputs: Sequence[Optional[Tensor]], grid_change: Tensor,
-                                  alpha: Tensor, params: Optional[Tensor], grads: Optional[Tensor] = None,
-                                  d_image: Optional[Tensor] = None, d_pose: Optional[Tensor] = None):
-        """The backward of SirenMorpher03 into any of grads (flat, state_dict order), d_image [B,4,512,512] and d_pose [B,45]
-        (None = not computed; the others are overwritten).  d_image is the adjoint of the warp the forward returned, from its
-        grid_change / alpha outputs, with no SIREN recompute; grads and d_pose recompute the forward with TF32 products."""
+    @staticmethod
+    def _check_flat(t: Optional[Tensor], n: int, name: str):
+        """A flat fp32 buffer of a student's n parameters in state_dict order (params / grads)."""
+        assert t is not None and t.is_contiguous() and t.dtype == torch.float32 and t.numel() == n, (name, n)
+
+    def siren_morpher_backward(self, image: Tensor, pose: Tensor, grad_outputs: Sequence[Optional[Tensor]], *,
+                               grid_change: Optional[Tensor] = None, alpha: Optional[Tensor] = None,
+                               params: Optional[Tensor] = None, grads: Optional[Tensor] = None,
+                               d_image: Optional[Tensor] = None, d_pose: Optional[Tensor] = None):
+        """The backward of SirenMorpher03 for the upstream gradients of its five outputs (None = zero) into any of grads
+        (dL/d params, flat in state_dict order), d_image [B,4,512,512] and d_pose [B,45] (None = not computed; the others
+        are overwritten).  grads and d_pose recompute the forward with TF32 products, as the train step does, and need
+        params; d_image is the adjoint of the warp the forward returned, from its grid_change / alpha outputs, with no
+        SIREN recompute.  Any batch size."""
         assert grads is not None or d_image is not None or d_pose is not None
         image = _check_input(image, self.device, 'image')
         pose = _check_input(pose, self.device, 'pose')
         B = image.shape[0]
-        assert image.shape[1:] == (4, 512, 512) and pose.shape == (B, 45) and len(grad_outputs) == 5
-        gs = []
-        for (c, s), g, name in zip(self.SIREN_MORPHER_SPECS, grad_outputs, ('blended', 'alpha', 'color_change', 'warped', 'grid_change')):
-            if g is not None:
-                g = _check_input(g, self.device, 'grad of ' + name)
-                assert g.shape == (B, c, s, s), (name, tuple(g.shape))
-            gs.append(g)
-        grid_change = _check_input(grid_change, self.device, 'grid_change')
-        alpha = _check_input(alpha, self.device, 'alpha')
-        assert grid_change.shape == (B, 2, 512, 512) and alpha.shape == (B, 1, 512, 512)
+        assert image.shape[1:] == (4, 512, 512) and pose.shape == (B, 45)
+        gs = self._grads(self.SIREN_MORPHER_SPECS, grad_outputs, B)
+        if d_image is not None:
+            assert grid_change is not None and alpha is not None, 'd_image needs the forward\'s grid_change and alpha'
+            grid_change = _check_input(grid_change, self.device, 'grid_change')
+            alpha = _check_input(alpha, self.device, 'alpha')
+            assert grid_change.shape == (B, 2, 512, 512) and alpha.shape == (B, 1, 512, 512)
         n = self.lib.tha4_siren_morpher_param_count()
         if grads is not None or d_pose is not None:
-            assert params is not None and params.is_contiguous() and params.dtype == torch.float32 and params.numel() == n
-        self._check_out(grads, (n,), 'grads')
+            self._check_flat(params, n, 'params')
+        if grads is not None:
+            self._check_flat(grads, n, 'grads')
         self._check_out(d_image, (B, 4, 512, 512), 'd_image')
         self._check_out(d_pose, (B, 45), 'd_pose')
-        self._call('tha4_siren_morpher_backward_ex', _ptr(image), _ptr(pose), 45, B, _ptr_array(gs), _ptr(grid_change), _ptr(alpha),
+        self._call('tha4_siren_morpher_backward', _ptr(image), _ptr(pose), 45, B, _ptr_array(gs), _ptr(grid_change), _ptr(alpha),
                    _ptr(params), _ptr(grads), _ptr(d_image), _ptr(d_pose), self._stream())
 
-    def siren_face_morpher_backward_ex(self, pose: Tensor, grad_output: Tensor, params: Tensor, grads: Optional[Tensor] = None,
-                                       d_pose: Optional[Tensor] = None):
-        """The backward of SirenFaceMorpher00 into grads and / or d_pose [B,39] (None = not computed)."""
+    def siren_face_morpher_backward(self, pose: Tensor, grad_output: Tensor, params: Tensor, *, grads: Optional[Tensor] = None,
+                                    d_pose: Optional[Tensor] = None):
+        """The backward of SirenFaceMorpher00 for the upstream gradient [B,4,128,128] of its output into grads (dL/d params,
+        flat in state_dict order) and / or d_pose [B,39] (None = not computed; the others are overwritten).  pose [B, >= 39]."""
         assert grads is not None or d_pose is not None
         pose = _check_input(pose, self.device, 'pose')
         grad_output = _check_input(grad_output, self.device, 'grad_output')
         B = pose.shape[0]
         assert pose.shape[1] >= 39 and grad_output.shape == (B, 4, 128, 128)
         n = self.lib.tha4_siren_face_morpher_param_count()
-        assert params.is_contiguous() and params.dtype == torch.float32 and params.numel() == n
-        self._check_out(grads, (n,), 'grads')
+        self._check_flat(params, n, 'params')
+        if grads is not None:
+            self._check_flat(grads, n, 'grads')
         self._check_out(d_pose, (B, 39), 'd_pose')
-        self._call('tha4_siren_face_morpher_backward_ex', _ptr(pose), int(pose.shape[1]), B, _ptr(grad_output), _ptr(params),
+        self._call('tha4_siren_face_morpher_backward', _ptr(pose), int(pose.shape[1]), B, _ptr(grad_output), _ptr(params),
                    _ptr(grads), _ptr(d_pose), self._stream())
 
     def adam_step(self, params: Tensor, grads: Tensor, exp_avg: Tensor, exp_avg_sq: Tensor, lr: float, step: int,

@@ -149,6 +149,7 @@ struct OutSpec { int c, s; };
 const OutSpec kEncDecDecomposer[6] = {{4, 128}, {1, 128}, {4, 128}, {4, 128}, {1, 128}, {4, 128}};
 const OutSpec kCombiner[8] = {{4, 128}, {1, 128}, {4, 128}, {4, 128}, {1, 128}, {4, 128}, {4, 128}, {2, 128}};
 const OutSpec kFace[8] = {{4, 192}, {1, 192}, {4, 192}, {4, 192}, {1, 192}, {4, 192}, {4, 192}, {2, 192}};
+const OutSpec kSirenBody[5] = {{4, 512}, {1, 512}, {4, 512}, {4, 512}, {2, 512}};
 
 void fill_unet_spec(OutSpec* o, int S) { o[0] = {4, S}; o[1] = {1, S}; o[2] = {4, S}; o[3] = {2, S}; o[4] = {4, S}; }
 
@@ -163,7 +164,6 @@ StateDict make_sd(int n, const char* const* keys, const void* const* ptrs, const
     return sd;
 }
 
-// Runs `fn(chunk offset n0, chunk size b)` over micro-batches; resets the workspace per chunk.
 // Start of one pass over the workspace: every pool block becomes reusable and the part of the statistics arena the
 // previous pass dirtied is re-zeroed (the arena is all-zero at the start of every pass).
 void begin_pass(tha4_ctx* ctx, cudaStream_t stream) {
@@ -173,11 +173,12 @@ void begin_pass(tha4_ctx* ctx, cudaStream_t stream) {
     ctx->stats_off = 0;
 }
 
+// Runs `fn(chunk offset n0, chunk size b)` over micro-batches of at most `chunk` frames; resets the workspace per chunk.
 template <typename F>
-void for_chunks(tha4_ctx* ctx, int B, cudaStream_t stream, F&& fn) {
+void for_chunks(tha4_ctx* ctx, int B, int chunk, cudaStream_t stream, F&& fn) {
     THA4_REQUIRE(B >= 1, "batch must be >= 1");
-    for (int n0 = 0; n0 < B; n0 += ctx->microbatch) {
-        const int b = std::min(ctx->microbatch, B - n0);
+    for (int n0 = 0; n0 < B; n0 += chunk) {
+        const int b = std::min(chunk, B - n0);
         begin_pass(ctx, stream);
         fn(n0, b);
     }
@@ -321,7 +322,7 @@ int tha4_load_net(tha4_ctx* ctx, int net, int n_tensors, const char* const* keys
 int tha4_eyebrow_decomposer_forward(tha4_ctx* ctx, const float* image, int B, float* const* outputs, void* stream) {
     return guarded(ctx, [&] {
         Runtime rt = make_rt(ctx, stream);
-        for_chunks(ctx, B, rt.stream, [&](int n0, int b) {
+        for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
             float* o[6]; offset_outputs<6>(outputs, kEncDecDecomposer, n0, o);
             ctx->decomposer->forward(rt, make_img(image + (size_t)n0 * 4 * 128 * 128, b, 4, 128, 128), ImgView{}, nullptr, 0, o);
         });
@@ -332,7 +333,7 @@ int tha4_eyebrow_morphing_combiner_forward(tha4_ctx* ctx, const float* backgroun
                                            const float* pose, int pose_ld, int B, float* const* outputs, void* stream) {
     return guarded(ctx, [&] {
         Runtime rt = make_rt(ctx, stream);
-        for_chunks(ctx, B, rt.stream, [&](int n0, int b) {
+        for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
             float* o[8]; offset_outputs<8>(outputs, kCombiner, n0, o);
             const size_t off = (size_t)n0 * 4 * 128 * 128;
             ctx->combiner->forward(rt, make_img(eyebrow_layer + off, b, 4, 128, 128), make_img(background_layer + off, b, 4, 128, 128),
@@ -345,7 +346,7 @@ int tha4_face_morpher_forward(tha4_ctx* ctx, const float* image, const float* po
                               float* const* outputs, void* stream) {
     return guarded(ctx, [&] {
         Runtime rt = make_rt(ctx, stream);
-        for_chunks(ctx, B, rt.stream, [&](int n0, int b) {
+        for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
             float* o[8]; offset_outputs<8>(outputs, kFace, n0, o);
             ctx->face->forward(rt, make_img(image + (size_t)n0 * 4 * 192 * 192, b, 4, 192, 192), ImgView{},
                                pose + (size_t)n0 * pose_ld, pose_ld, o);
@@ -358,7 +359,7 @@ int tha4_eyebrow_decomposer_backward(tha4_ctx* ctx, const float* image, int B, c
     return guarded(ctx, [&] {
         THA4_REQUIRE(d_image != nullptr, "decomposer backward: no gradient requested");
         Runtime rt = make_rt(ctx, stream);
-        for_chunks(ctx, B, rt.stream, [&](int n0, int b) {
+        for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
             const float* g[6]; offset_grads<6>(grad_outputs, kEncDecDecomposer, n0, g);
             EncDecGrads eg; eg.grad_outputs = g; eg.d_image0 = d_image + (size_t)n0 * 4 * 128 * 128;
             ctx->decomposer->backward(rt, make_img(image + (size_t)n0 * 4 * 128 * 128, b, 4, 128, 128), ImgView{}, nullptr, 0, eg);
@@ -373,7 +374,7 @@ int tha4_eyebrow_morphing_combiner_backward(tha4_ctx* ctx, const float* backgrou
         THA4_REQUIRE(d_background_layer || d_eyebrow_layer || d_pose, "combiner backward: no gradient requested");
         THA4_REQUIRE(pose_ld >= 12, "combiner backward: pose rows need at least 12 entries");
         Runtime rt = make_rt(ctx, stream);
-        for_chunks(ctx, B, rt.stream, [&](int n0, int b) {
+        for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
             const float* g[8]; offset_grads<8>(grad_outputs, kCombiner, n0, g);
             const size_t off = (size_t)n0 * 4 * 128 * 128;
             EncDecGrads eg; eg.grad_outputs = g;
@@ -392,7 +393,7 @@ int tha4_face_morpher_backward(tha4_ctx* ctx, const float* image, const float* p
         THA4_REQUIRE(d_image || d_pose, "face morpher backward: no gradient requested");
         THA4_REQUIRE(pose_ld >= 27, "face morpher backward: pose rows need at least 27 entries");
         Runtime rt = make_rt(ctx, stream);
-        for_chunks(ctx, B, rt.stream, [&](int n0, int b) {
+        for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
             const float* g[8]; offset_grads<8>(grad_outputs, kFace, n0, g);
             EncDecGrads eg; eg.grad_outputs = g;
             eg.d_image0 = d_image ? d_image + (size_t)n0 * 4 * 192 * 192 : nullptr;
@@ -408,7 +409,7 @@ int tha4_morpher_forward(tha4_ctx* ctx, const float* image, const float* pose, i
     return guarded(ctx, [&] {
         Runtime rt = make_rt(ctx, stream);
         OutSpec spec[5]; fill_unet_spec(spec, 256);
-        for_chunks(ctx, B, rt.stream, [&](int n0, int b) {
+        for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
             float* o[5]; offset_outputs<5>(outputs, spec, n0, o);
             ctx->body->forward(rt, make_img(image + (size_t)n0 * 4 * 256 * 256, b, 4, 256, 256), nullptr, nullptr, 0,
                                pose + (size_t)n0 * pose_ld, pose_ld, o);
@@ -422,7 +423,7 @@ int tha4_upscaler_forward(tha4_ctx* ctx, const float* rest_image, const float* c
     return guarded(ctx, [&] {
         Runtime rt = make_rt(ctx, stream);
         OutSpec spec[5]; fill_unet_spec(spec, 512);
-        for_chunks(ctx, B, rt.stream, [&](int n0, int b) {
+        for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
             float* o[5]; offset_outputs<5>(outputs, spec, n0, o);
             ctx->upscaler->forward(rt, make_img(rest_image + (size_t)n0 * 4 * 512 * 512, b, 4, 512, 512),
                                    coarse_posed_image + (size_t)n0 * 4 * coarse_size * coarse_size,
@@ -468,7 +469,7 @@ int tha4_teacher_forward(tha4_ctx* ctx, int mode, const float* image, int64_t im
         for (int i = 0; i < 6; ++i) spec[n++] = kEncDecDecomposer[i];
         const int nout = n;
         auto run = [&](const float* img_p, const float* pose_p, float* const* outs, const float* const* cached_p) {
-            for_chunks(ctx, B, rt.stream, [&](int n0, int b) {
+            for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
                 float* o[33];
                 for (int i = 0; i < nout; ++i) o[i] = outs[i] ? outs[i] + (size_t)n0 * spec[i].c * spec[i].s * spec[i].s : nullptr;
                 const float* cd[6];
@@ -638,47 +639,8 @@ int tha4_siren_face_morpher_train_step(tha4_ctx* ctx, const float* pose, int pos
 }
 
 int tha4_siren_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
-                                const float* const* grad_outputs, const float* params, float* grads, void* stream) {
-    return guarded(ctx, [&] {
-        THA4_REQUIRE(B >= 1, "student backward: batch must be >= 1");
-        THA4_REQUIRE(pose_ld >= 45, "student backward: pose rows need at least 45 entries");
-        cudaStream_t s = (cudaStream_t)stream;
-        Runtime rt = make_rt(ctx, stream);
-        THA4_CUDA_CHECK(cudaMemsetAsync(grads, 0, siren_body_param_count() * sizeof(float), s));
-        const int ch[5] = {4, 1, 4, 4, 2};
-        for (int n0 = 0; n0 < B; n0 += SIREN_BODY_MAX_BATCH) {       // micro-batches share the workspace and accumulate
-            const int b = std::min(SIREN_BODY_MAX_BATCH, B - n0);
-            begin_pass(ctx, s);
-            const float* g[5];
-            for (int i = 0; i < 5; ++i)
-                g[i] = (grad_outputs && grad_outputs[i]) ? grad_outputs[i] + (size_t)n0 * ch[i] * 512 * 512 : nullptr;
-            siren_body_backward(rt, make_img(image + (size_t)n0 * 4 * 512 * 512, b, 4, 512, 512), pose + (size_t)n0 * pose_ld, pose_ld, g,
-                                params, grads, nullptr);
-        }
-    });
-}
-
-int tha4_siren_face_morpher_backward(tha4_ctx* ctx, const float* pose, int pose_ld, int B, const float* grad_output,
-                                     const float* params, float* grads, void* stream) {
-    return guarded(ctx, [&] {
-        THA4_REQUIRE(B >= 1, "face student backward: batch must be >= 1");
-        THA4_REQUIRE(pose_ld >= 39, "face student backward: pose rows need at least 39 entries");
-        THA4_REQUIRE(grad_output != nullptr, "face student backward: grad_output is required");
-        cudaStream_t s = (cudaStream_t)stream;
-        Runtime rt = make_rt(ctx, stream);
-        THA4_CUDA_CHECK(cudaMemsetAsync(grads, 0, siren_face_param_count() * sizeof(float), s));
-        for (int n0 = 0; n0 < B; n0 += SIREN_FACE_MAX_BATCH) {
-            const int b = std::min(SIREN_FACE_MAX_BATCH, B - n0);
-            begin_pass(ctx, s);
-            siren_face_backward(rt, pose + (size_t)n0 * pose_ld, pose_ld, b, grad_output + (size_t)n0 * 4 * 128 * 128, params, grads,
-                                nullptr);
-        }
-    });
-}
-
-int tha4_siren_morpher_backward_ex(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
-                                   const float* const* grad_outputs, const float* grid_change, const float* alpha,
-                                   const float* params, float* grads, float* d_image, float* d_pose, void* stream) {
+                                const float* const* grad_outputs, const float* grid_change, const float* alpha,
+                                const float* params, float* grads, float* d_image, float* d_pose, void* stream) {
     return guarded(ctx, [&] {
         THA4_REQUIRE(B >= 1, "student backward: batch must be >= 1");
         THA4_REQUIRE(grads || d_image || d_pose, "student backward: no output requested");
@@ -686,42 +648,34 @@ int tha4_siren_morpher_backward_ex(tha4_ctx* ctx, const float* image, const floa
         THA4_REQUIRE(!siren || (image && pose && params), "student backward: image, pose and params are required");
         THA4_REQUIRE(!siren || pose_ld >= 45, "student backward: pose rows need at least 45 entries");
         THA4_REQUIRE(!d_image || (grid_change && alpha), "student backward: d_image needs the forward's grid_change and alpha");
-        cudaStream_t s = (cudaStream_t)stream;
         Runtime rt = make_rt(ctx, stream);
-        if (grads) THA4_CUDA_CHECK(cudaMemsetAsync(grads, 0, siren_body_param_count() * sizeof(float), s));
+        if (grads) THA4_CUDA_CHECK(cudaMemsetAsync(grads, 0, siren_body_param_count() * sizeof(float), rt.stream));
         constexpr size_t hw = 512 * 512;
-        const int ch[5] = {4, 1, 4, 4, 2};
-        for (int n0 = 0; n0 < B; n0 += SIREN_BODY_MAX_BATCH) {       // micro-batches share the workspace
-            const int b = std::min(SIREN_BODY_MAX_BATCH, B - n0);
-            begin_pass(ctx, s);
-            const float* g[5];
-            for (int i = 0; i < 5; ++i) g[i] = (grad_outputs && grad_outputs[i]) ? grad_outputs[i] + (size_t)n0 * ch[i] * hw : nullptr;
+        for_chunks(ctx, B, SIREN_BODY_MAX_BATCH, rt.stream, [&](int n0, int b) {     // micro-batches accumulate into grads
+            const float* g[5]; offset_grads<5>(grad_outputs, kSirenBody, n0, g);
             if (siren)
                 siren_body_backward(rt, make_img(image + (size_t)n0 * 4 * hw, b, 4, 512, 512), pose + (size_t)n0 * pose_ld, pose_ld, g,
                                     params, grads, d_pose ? d_pose + (size_t)n0 * 45 : nullptr);
             if (d_image)
                 siren_body_image_grad(rt, grid_change + (size_t)n0 * 2 * hw, alpha + (size_t)n0 * hw, g[0], g[3], b,
                                       d_image + (size_t)n0 * 4 * hw);
-        }
+        });
     });
 }
 
-int tha4_siren_face_morpher_backward_ex(tha4_ctx* ctx, const float* pose, int pose_ld, int B, const float* grad_output,
-                                        const float* params, float* grads, float* d_pose, void* stream) {
+int tha4_siren_face_morpher_backward(tha4_ctx* ctx, const float* pose, int pose_ld, int B, const float* grad_output,
+                                     const float* params, float* grads, float* d_pose, void* stream) {
     return guarded(ctx, [&] {
         THA4_REQUIRE(B >= 1, "face student backward: batch must be >= 1");
         THA4_REQUIRE(grads || d_pose, "face student backward: no output requested");
         THA4_REQUIRE(pose_ld >= 39, "face student backward: pose rows need at least 39 entries");
         THA4_REQUIRE(grad_output != nullptr, "face student backward: grad_output is required");
-        cudaStream_t s = (cudaStream_t)stream;
         Runtime rt = make_rt(ctx, stream);
-        if (grads) THA4_CUDA_CHECK(cudaMemsetAsync(grads, 0, siren_face_param_count() * sizeof(float), s));
-        for (int n0 = 0; n0 < B; n0 += SIREN_FACE_MAX_BATCH) {
-            const int b = std::min(SIREN_FACE_MAX_BATCH, B - n0);
-            begin_pass(ctx, s);
+        if (grads) THA4_CUDA_CHECK(cudaMemsetAsync(grads, 0, siren_face_param_count() * sizeof(float), rt.stream));
+        for_chunks(ctx, B, SIREN_FACE_MAX_BATCH, rt.stream, [&](int n0, int b) {     // micro-batches accumulate into grads
             siren_face_backward(rt, pose + (size_t)n0 * pose_ld, pose_ld, b, grad_output + (size_t)n0 * 4 * 128 * 128, params, grads,
                                 d_pose ? d_pose + (size_t)n0 * 39 : nullptr);
-        }
+        });
     });
 }
 

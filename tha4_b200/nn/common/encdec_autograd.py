@@ -18,25 +18,12 @@ import torch
 from torch import Tensor
 from torch.autograd.function import once_differentiable
 
-from tha4_b200._lib import Tha4Error
-
-
-def wants_input_grad(*inputs: Tensor) -> bool:
-    return torch.is_grad_enabled() and any(t.requires_grad for t in inputs)
-
-
-def _refuse_double_backward(module_name: str):
-    if torch.is_grad_enabled():
-        raise Tha4Error('%s: double backward (create_graph=True) is not supported' % module_name)
+from tha4_b200.nn.common.native_module import contiguous_grads, refuse_double_backward
 
 
 def _own(outs: Sequence[Tensor]):
     # one allocation per output: autograd refuses in-place ops on outputs that are views created inside a Function
     return tuple(o.clone() for o in outs)
-
-
-def _grads(grad_outputs):
-    return [None if g is None else g.contiguous() for g in grad_outputs]
 
 
 def _empty_like(t: Tensor) -> Tensor:
@@ -54,7 +41,7 @@ class _DecomposerFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, *grad_outputs):
-        _refuse_double_backward('EyebrowDecomposer00')
+        refuse_double_backward('EyebrowDecomposer00')
         return _decomposer_backward(ctx, *grad_outputs)
 
 
@@ -65,7 +52,7 @@ def _decomposer_backward(ctx, *grad_outputs):
     if not ctx.needs_input_grad[1] or all(g is None for g in grad_outputs):
         return (None, None) + none
     d_image = _empty_like(image)
-    ctx.module.sync_weights().eyebrow_decomposer_backward(image, _grads(grad_outputs), d_image)
+    ctx.module.sync_weights().eyebrow_decomposer_backward(image, contiguous_grads(grad_outputs), d_image)
     return (None, d_image) + none
 
 
@@ -80,7 +67,7 @@ class _CombinerFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, *grad_outputs):
-        _refuse_double_backward('EyebrowMorphingCombiner00')
+        refuse_double_backward('EyebrowMorphingCombiner00')
         return _combiner_backward(ctx, *grad_outputs)
 
 
@@ -94,7 +81,7 @@ def _combiner_backward(ctx, *grad_outputs):
     d_bg = _empty_like(background_layer) if want[0] else None
     d_eb = _empty_like(eyebrow_layer) if want[1] else None
     d_pose = _empty_like(pose) if want[2] else None
-    ctx.module.sync_weights().eyebrow_morphing_combiner_backward(background_layer, eyebrow_layer, pose, _grads(grad_outputs),
+    ctx.module.sync_weights().eyebrow_morphing_combiner_backward(background_layer, eyebrow_layer, pose, contiguous_grads(grad_outputs),
                                                                 d_background_layer=d_bg, d_eyebrow_layer=d_eb, d_pose=d_pose)
     return (None, d_bg, d_eb, d_pose) + none
 
@@ -110,7 +97,7 @@ class _FaceMorpherFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, *grad_outputs):
-        _refuse_double_backward('FaceMorpher08')
+        refuse_double_backward('FaceMorpher08')
         return _face_morpher_backward(ctx, *grad_outputs)
 
 
@@ -123,7 +110,7 @@ def _face_morpher_backward(ctx, *grad_outputs):
         return (None, None, None) + none
     d_image = _empty_like(image) if want_image else None
     d_pose = _empty_like(pose) if want_pose else None
-    ctx.module.sync_weights().face_morpher_backward(image, pose, _grads(grad_outputs), d_image=d_image, d_pose=d_pose)
+    ctx.module.sync_weights().face_morpher_backward(image, pose, contiguous_grads(grad_outputs), d_image=d_image, d_pose=d_pose)
     return (None, d_image, d_pose) + none
 
 

@@ -2,13 +2,30 @@
 keys and whose forward is one C-ABI call into libtha4_b200.so (no PyTorch-op fallback)."""
 import math
 import weakref
-from typing import Dict, Optional
+from typing import Dict, List, Optional, Sequence
 
 import torch
 from torch import Tensor
 from torch.nn import Module, Parameter
 
 from tha4_b200._lib import Context, Tha4Error
+
+
+# ---------------------------------------------------------------------- shared by the modules' autograd.Functions
+def wants_autograd(*tensors: Tensor) -> bool:
+    """Dispatch rule of the differentiable modules: forward goes through the module's autograd.Function when grad mode is
+    on and any of `tensors` (its inputs; for the students, its parameters too) requires grad; otherwise it is the plain
+    inference call."""
+    return torch.is_grad_enabled() and any(t.requires_grad for t in tensors)
+
+
+def refuse_double_backward(module_name: str):
+    if torch.is_grad_enabled():
+        raise Tha4Error('%s: double backward (create_graph=True) is not supported' % module_name)
+
+
+def contiguous_grads(grad_outputs: Sequence[Optional[Tensor]]) -> List[Optional[Tensor]]:
+    return [None if g is None else g.contiguous() for g in grad_outputs]
 
 
 class _Node(Module):

@@ -5,7 +5,7 @@ from typing import List
 from torch import Tensor
 
 from tha4_b200.nn.common import encdec_autograd
-from tha4_b200.nn.common.native_module import NativeModule
+from tha4_b200.nn.common.native_module import NativeModule, wants_autograd
 from tha4_b200.nn.state_dict_spec import eyebrow_decomposer_spec
 
 
@@ -17,7 +17,7 @@ class EyebrowDecomposer00(NativeModule):
         self.args = args
 
     def forward(self, image: Tensor, *args) -> List[Tensor]:
-        if encdec_autograd.wants_input_grad(image):
+        if wants_autograd(image):
             return encdec_autograd.eyebrow_decomposer(self, image)
         return self.sync_weights().eyebrow_decomposer(image)
 

@@ -4,7 +4,7 @@ from typing import Optional
 
 from torch import Tensor
 
-from tha4_b200.nn.common.native_module import NativeModule
+from tha4_b200.nn.common.native_module import NativeModule, wants_autograd
 from tha4_b200.nn.siren import student_autograd
 from tha4_b200.nn.state_dict_spec import siren_face_morpher_spec
 
@@ -18,8 +18,6 @@ class SirenFaceMorpher00(NativeModule):
 
     def forward(self, pose: Tensor, position: Optional[Tensor] = None) -> Tensor:
         assert position is None, 'only the default affine_grid position image (siren_face_morpher_00.py:38-44) is supported'
-        if student_autograd.wants_autograd(self):       # loss.backward() reaches the parameters (student_autograd.py)
+        if wants_autograd(pose, *self._params()):            # loss.backward() reaches the parameters, or the pose
             return student_autograd.siren_face_morpher(self, pose)
-        if student_autograd.wants_input_grad(pose):             # frozen: loss.backward() reaches the pose
-            return student_autograd.siren_face_morpher_input_grad(self, pose)
         return self.sync_weights().siren_face_morpher(pose)

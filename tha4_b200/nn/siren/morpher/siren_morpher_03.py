@@ -4,7 +4,7 @@ from typing import List
 
 from torch import Tensor
 
-from tha4_b200.nn.common.native_module import NativeModule
+from tha4_b200.nn.common.native_module import NativeModule, wants_autograd
 from tha4_b200.nn.siren import student_autograd
 from tha4_b200.nn.state_dict_spec import siren_morpher_03_spec
 
@@ -17,10 +17,8 @@ class SirenMorpher03(NativeModule):
         self.args = args
 
     def forward(self, image: Tensor, pose: Tensor) -> List[Tensor]:
-        if student_autograd.wants_autograd(self):       # loss.backward() reaches the parameters (student_autograd.py)
+        if wants_autograd(image, pose, *self._params()):     # loss.backward() reaches the parameters, or image / pose
             return student_autograd.siren_morpher(self, image, pose)
-        if student_autograd.wants_input_grad(image, pose):      # frozen: loss.backward() reaches image / pose
-            return student_autograd.siren_morpher_input_grad(self, image, pose)
         return self.sync_weights().siren_morpher(image, pose)
 
     INDEX_BLENDED_IMAGE = 0
