@@ -108,6 +108,13 @@ int tha4_face_morpher_backward(tha4_ctx* ctx, const float* image, const float* p
  * merged(4) alpha(1) warped(4) grid_change(2) direct(4) */
 int tha4_morpher_forward(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
                          float* const* outputs, void* stream);
+/* Input gradients of Morpher00 for upstream gradients of its 5 outputs (grad_outputs in the forward's output order, NCHW,
+ * an entry may be NULL = zero), with the rules of the encoder-decoder entries above: d_image [B,4,256,256] and d_pose [B,6]
+ * (contiguous) are optional (NULL = not computed), at least one non-NULL, each overwritten.  The forward is recomputed in the
+ * context's precision mode and differentiated with fp32 data gradients.  Any B >= 1 (micro-batched).  The adjoint weights
+ * are packed by the first call. */
+int tha4_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
+                          const float* const* grad_outputs, float* d_image, float* d_pose, void* stream);
 /* Upscaler02.forward (src/tha4/nn/upscaler/upscaler_02.py:59-96): rest_image [B,4,512,512], coarse_posed_image
  * [B,4,S,S], coarse_grid_change [B,2,S,S], pose [B,6] -> merged alpha warped grid_change direct.
  * coarse_size S = 512: the reference signature.  S = 256: the half-resolution body-morpher outputs; the bilinear x2
@@ -249,19 +256,30 @@ int tha4_test_tail(tha4_ctx* ctx, int kind, const float* feature, int N, int C, 
                    int groups, int act, const float* head_w, const float* head_b, const int* head_cout, int n_heads,
                    const float* image0, const float* image1, float* const* outputs, int strict, void* stream);
 /* Data gradient of a conv on the conv kernels with adjoint-packed weights: kind 0 3x3 s1 p1 (w [Cout,Cin,3,3]), 1 4x4 s2 p1
- * (w [Cout,Cin,4,4]), 2 4x4 s2 p1 transposed (w [Cin,Cout,4,4]); dy [N,Cout,Ho,Wo] -> dx [N,Cin,H,W].  Cout % 4 == 0.
+ * (w [Cout,Cin,4,4]), 2 4x4 s2 p1 transposed (w [Cin,Cout,4,4]), 3 1x1 (w [Cout,Cin,1,1]), 4 nearest x2 upsample + 3x3 s1 p1
+ * (w [Cout,Cin,3,3]; Ho = 2H); dy [N,Cout,Ho,Wo] -> dx [N,Cin,H,W].  Cout % 4 == 0 (and Cin % 4 == 0 for kinds 1..4).
+ * Kinds 3 and 4 pack the forward conv first and derive the adjoint from the packed weights, as the U-Net backward does.
  * strict: 3xTF32, else TF32 (fp32 operands in both). */
 int tha4_test_conv_backward_data(tha4_ctx* ctx, int kind, const float* dy, const float* w, float* dx, int N, int Cin, int H, int W,
                                  int Cout, int strict, void* stream);
 /* InstanceNorm2d(affine) (+ReLU when act == 1) backward: x, dy, dx [N,C,H,W] (statistics of x computed on the device) */
 int tha4_test_norm_backward(tha4_ctx* ctx, const float* x, int N, int C, int H, int W, const float* gamma, const float* beta,
                             int act, const float* dy, float* dx, void* stream);
-/* Tail backward of one encoder-decoder kind (1 decomposer, 2 combiner, 3 face morpher) in isolation: outputs / grad_outputs as
+/* Tail backward of one kind (0 U-Net, 1 decomposer, 2 combiner, 3 face morpher) in isolation: outputs / grad_outputs as
  * tha4_test_tail returns them (grad entries may be NULL), image0 / image1 as for tha4_test_tail.  d_head [N,12,S,S]: gradients
  * of the head pre-activations in the channel order of tail.cu; d_image0 / d_image1 [N,4,S,S] (NULL = not computed). */
 int tha4_test_tail_backward(tha4_ctx* ctx, int kind, const float* const* outputs, int N, int S, const float* image0,
                             const float* image1, const float* const* grad_outputs, float* d_head, float* d_image0,
                             float* d_image1, void* stream);
+/* GroupNorm(groups) (+FiLM) (+SiLU) backward of the U-Net ResBlocks (src/tha4/nn/common/unet.py:154-165): y = act(h), h =
+ * (GN(x) * (1 + film0[c]) + film0[C+c]) * (1 + film1[n][c]) + film1[n][C+c] (film0 [2C], film1 [N,2C]; either may be NULL),
+ * act 0 none / 2 SiLU.  x, dy, dx [N,C,H,W] (statistics of x computed on the device); d_film [N,2C] (NULL = not computed; needs
+ * film1): d(scale) then d(shift) of film1.  C <= 512. */
+int tha4_test_group_norm_backward(tha4_ctx* ctx, const float* x, int N, int C, int H, int W, int groups, const float* gamma,
+                                  const float* beta, const float* film0, const float* film1, int act, const float* dy, float* dx,
+                                  float* d_film, void* stream);
+/* qkv_attention backward (fp32): qkv [N,3C,16,16], dout = d(attention output) [N,C,16,16] -> dqkv [N,3C,16,16] */
+int tha4_test_attention_backward(tha4_ctx* ctx, const float* qkv, const float* dout, int N, int C, int heads, float* dqkv, void* stream);
 /* qkv_attention, "new order" (src/tha4/nn/common/unet.py:192-202): qkv [N,3C,16,16] -> out [N,C,16,16] */
 int tha4_test_attention(tha4_ctx* ctx, const float* qkv, int N, int C, int heads, float* out, void* stream);
 /* y[n][o] = b[o] + sum_i f(x[n][i]) W[o][i] */

@@ -1,4 +1,4 @@
-"""Device time of the encoder-decoder teachers' input gradients (developer tool; H100).
+"""Device time of the teachers' input gradients: the encoder-decoder networks and the body morpher (developer tool; H100).
 
 For each network at B = 1 and 8: the forward alone (no grad) and forward + backward with every input requiring grad, in ms
 from CUDA events after a warm-up, and the kernel launches of the backward.  Then one mode_12 pose-fitting step at B = 1
@@ -14,6 +14,7 @@ from oracle import synth  # noqa: E402
 from tha4_b200.nn.eyebrow_decomposer.eyebrow_decomposer_00 import EyebrowDecomposer00  # noqa: E402
 from tha4_b200.nn.eyebrow_morphing_combiner.eyebrow_morphing_combiner_00 import EyebrowMorphingCombiner00  # noqa: E402
 from tha4_b200.nn.face_morpher.face_morpher_08 import FaceMorpher08  # noqa: E402
+from tha4_b200.nn.morpher.morpher_00 import Morpher00  # noqa: E402
 from tha4_b200.poser.modes import mode_12  # noqa: E402
 
 DEV = torch.device('cuda:0')
@@ -49,6 +50,8 @@ def inputs(name, B):
     if name == 'eyebrow_morphing_combiner':
         c = img[:, :, 64:192, 192:320].contiguous()
         return [c, c.flip(3).contiguous(), pose[:, :12].contiguous()]
+    if name == 'body_morpher':
+        return [img[:, :, ::2, ::2].contiguous(), pose[:, 39:45].contiguous()]
     return [img[:, :, 32:224, 160:352].contiguous(), pose[:, 12:39].contiguous()]
 
 
@@ -56,7 +59,7 @@ def main():
     sds = synth.teacher_state_dicts(0)
     print('card: %s' % card())
     for name, cls in (('eyebrow_decomposer', EyebrowDecomposer00), ('eyebrow_morphing_combiner', EyebrowMorphingCombiner00),
-                      ('face_morpher', FaceMorpher08)):
+                      ('face_morpher', FaceMorpher08), ('body_morpher', Morpher00)):
         m = cls()
         m.load_state_dict(sds[name])
         m.to(DEV)

@@ -29,7 +29,9 @@ EXPORTED_SYMBOLS = [
     'tha4_siren_morpher_backward', 'tha4_siren_face_morpher_backward',
     'tha4_adam_step', 'tha4_images_differ', 'tha4_frame_to_srgb8', 'tha4_rgba8_to_poser_image', 'tha4_grid_sample', 'tha4_resize_bilinear',
     'tha4_eyebrow_decomposer_backward', 'tha4_eyebrow_morphing_combiner_backward', 'tha4_face_morpher_backward',
+    'tha4_morpher_backward',
     'tha4_test_conv_backward_data', 'tha4_test_norm_backward', 'tha4_test_tail_backward',
+    'tha4_test_group_norm_backward', 'tha4_test_attention_backward',
     'tha4_base_grid', 'tha4_test_conv', 'tha4_test_conv_norm', 'tha4_test_conv_norm_ex', 'tha4_test_norm', 'tha4_test_tail', 'tha4_test_attention', 'tha4_test_linear',
     'tha4_test_siren_level', 'tha4_test_sine', 'tha4_test_siren_plan_check',
 ]
@@ -248,13 +250,30 @@ class Context:
         self._call('tha4_face_morpher_backward', _ptr(image), _ptr(pose), 27, B, _ptr_array(gs), _ptr(d_image), _ptr(d_pose),
                    self._stream())
 
+    MORPHER_SPECS = [(4, 256), (1, 256), (4, 256), (2, 256), (4, 256)]
+
     def morpher(self, image: Tensor, pose: Tensor) -> List[Tensor]:
         image = _check_input(image, self.device, 'image')
         pose = _check_input(pose, self.device, 'pose')
         B = image.shape[0]
-        outs = self._empty([(4, 256), (1, 256), (4, 256), (2, 256), (4, 256)], B)
+        outs = self._empty(self.MORPHER_SPECS, B)
         self._call('tha4_morpher_forward', _ptr(image), _ptr(pose), 6, B, _ptr_array(outs), self._stream())
         return outs
+
+    def morpher_backward(self, image: Tensor, pose: Tensor, grad_outputs: Sequence[Optional[Tensor]],
+                         d_image: Optional[Tensor] = None, d_pose: Optional[Tensor] = None):
+        """Input gradients of Morpher00 into d_image [B,4,256,256] and / or d_pose [B,6] (None = not computed) for the upstream
+        gradients of its five outputs (None = zero); the forward is recomputed in the context's precision mode."""
+        assert d_image is not None or d_pose is not None
+        image = _check_input(image, self.device, 'image')
+        pose = _check_input(pose, self.device, 'pose')
+        B = image.shape[0]
+        assert image.shape[1:] == (4, 256, 256) and pose.shape == (B, 6)
+        gs = self._grads(self.MORPHER_SPECS, grad_outputs, B)
+        self._check_out(d_image, (B, 4, 256, 256), 'd_image')
+        self._check_out(d_pose, (B, 6), 'd_pose')
+        self._call('tha4_morpher_backward', _ptr(image), _ptr(pose), 6, B, _ptr_array(gs), _ptr(d_image), _ptr(d_pose),
+                   self._stream())
 
     def upscaler(self, rest_image: Tensor, coarse_posed: Tensor, coarse_grid: Tensor, pose: Tensor) -> List[Tensor]:
         rest_image = _check_input(rest_image, self.device, 'rest_image')

@@ -417,6 +417,23 @@ int tha4_morpher_forward(tha4_ctx* ctx, const float* image, const float* pose, i
     });
 }
 
+int tha4_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
+                          const float* const* grad_outputs, float* d_image, float* d_pose, void* stream) {
+    return guarded(ctx, [&] {
+        THA4_REQUIRE(d_image || d_pose, "morpher backward: no gradient requested");
+        THA4_REQUIRE(pose_ld >= 6, "morpher backward: pose rows need at least 6 entries");
+        Runtime rt = make_rt(ctx, stream);
+        OutSpec spec[5]; fill_unet_spec(spec, 256);
+        for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
+            const float* g[5]; offset_grads<5>(grad_outputs, spec, n0, g);
+            UNetGrads ug; ug.grad_outputs = g;
+            ug.d_image = d_image ? d_image + (size_t)n0 * 4 * 256 * 256 : nullptr;
+            ug.d_pose = d_pose ? d_pose + (size_t)n0 * 6 : nullptr; ug.d_pose_ld = 6;
+            ctx->body->backward(rt, make_img(image + (size_t)n0 * 4 * 256 * 256, b, 4, 256, 256), pose + (size_t)n0 * pose_ld, pose_ld, ug);
+        });
+    });
+}
+
 int tha4_upscaler_forward(tha4_ctx* ctx, const float* rest_image, const float* coarse_posed_image,
                           const float* coarse_grid_change, int coarse_size, const float* pose, int pose_ld, int B,
                           float* const* outputs, void* stream) {
@@ -935,8 +952,8 @@ int tha4_test_conv_backward_data(tha4_ctx* ctx, int kind, const float* dy, const
     return guarded(ctx, [&] {
         cudaStream_t s = (cudaStream_t)stream;
         begin_pass(ctx, s);
-        THA4_REQUIRE(kind >= 0 && kind <= 2 && Cout % 4 == 0 && (kind == 0 || Cin % 4 == 0),
-                     "test_conv_backward_data: kind 0..2, Cout % 4 == 0 (and Cin % 4 == 0 for the 4x4 kinds)");
+        THA4_REQUIRE(kind >= 0 && kind <= 4 && Cout % 4 == 0 && (kind == 0 || Cin % 4 == 0),
+                     "test_conv_backward_data: kind 0..4, Cout % 4 == 0 (and Cin % 4 == 0 for kinds 1..4)");
         Runtime rt = make_rt(ctx, stream);
         rt.strict = strict;
         Pool* P = &ctx->persist;
@@ -945,10 +962,20 @@ int tha4_test_conv_backward_data(tha4_ctx* ctx, int kind, const float* dy, const
         {
             SinkScope own(&sink);
             conv_set_pack_rounding(!strict);
-            conv_pack_adjoint(cw, (ConvKind)kind, w, Cin, Cout, kind == CONV_3x3 ? round_up(Cin, 4) : 0, s);
+            if (kind <= 2) {
+                conv_pack_adjoint(cw, (ConvKind)kind, w, Cin, Cout, kind == CONV_3x3 ? round_up(Cin, 4) : 0, s);
+            } else {   // the U-Net's path: the forward conv packed as the network packs it, its adjoint made from the packed weights
+                ConvWeights fwd;
+                conv_describe(fwd, (ConvKind)kind, Cin, Cout);
+                fwd.w = reinterpret_cast<float*>(tracked_malloc(conv_packed_floats(fwd) * sizeof(float)));
+                THA4_CUDA_CHECK(cudaMemsetAsync(fwd.w, 0, conv_packed_floats(fwd) * sizeof(float), s));
+                conv_pack(fwd, (ConvKind)kind, w, Cin, 0, s);
+                fwd.tf32_rounded = !strict;
+                conv_adjoint_from_packed(cw, fwd, (ConvKind)kind, s);
+            }
         }
         const int cin_k = kind == CONV_3x3 ? round_up(Cin, 4) : Cin;
-        const int Ho = kind == 1 ? H / 2 : (kind == 2 ? 2 * H : H), Wo = kind == 1 ? W / 2 : (kind == 2 ? 2 * W : W);
+        const int Ho = kind == 1 ? H / 2 : ((kind == 2 || kind == 4) ? 2 * H : H), Wo = kind == 1 ? W / 2 : ((kind == 2 || kind == 4) ? 2 * W : W);
         auto mk = [&](int h, int ww, int c) { View v; v.N = N; v.H = h; v.W = ww; v.C = c; v.ld = c; v.p = P->alloc((size_t)N * h * ww * c); return v; };
         View g = mk(Ho, Wo, Cout);
         nchw_to_nhwc(make_img(dy, N, Cout, Ho, Wo), g, s);
@@ -988,7 +1015,7 @@ int tha4_test_tail_backward(tha4_ctx* ctx, int kind, const float* const* outputs
                             float* d_image1, void* stream) {
     return guarded(ctx, [&] {
         cudaStream_t s = (cudaStream_t)stream;
-        THA4_REQUIRE(kind >= TAIL_DECOMPOSER && kind <= TAIL_FACE, "test_tail_backward: kind 1..3");
+        THA4_REQUIRE(kind >= TAIL_UNET && kind <= TAIL_FACE, "test_tail_backward: kind 0..3");
         THA4_REQUIRE(!image1 == (kind != TAIL_COMBINER), "test_tail_backward: image1 is the combiner's background layer");
         begin_pass(ctx, s);
         Pool* P = &ctx->persist;
@@ -1000,6 +1027,44 @@ int tha4_test_tail_backward(tha4_ctx* ctx, int kind, const float* const* outputs
         nhwc_to_nchw(dh.slice(0, 12), d_head, s);
         if (d_image0) nhwc_to_nchw(dimg.slice(0, 4), d_image0, s);
         if (d_image1) nhwc_to_nchw(dimg.slice(4, 4), d_image1, s);
+    });
+}
+
+int tha4_test_group_norm_backward(tha4_ctx* ctx, const float* x, int N, int C, int H, int W, int groups, const float* gamma,
+                                  const float* beta, const float* film0, const float* film1, int act, const float* dy, float* dx,
+                                  float* d_film, void* stream) {
+    return guarded(ctx, [&] {
+        cudaStream_t s = (cudaStream_t)stream;
+        THA4_REQUIRE(act == ACT_NONE || act == ACT_SILU, "test_group_norm_backward: act 0 or 2");
+        THA4_REQUIRE(!d_film || film1, "test_group_norm_backward: d_film needs film1");
+        begin_pass(ctx, s);
+        Runtime rt = make_rt(ctx, stream);
+        Pool* P = &ctx->persist;
+        auto mk = [&](int c) { View v; v.N = N; v.H = H; v.W = W; v.C = c; v.ld = c; v.p = P->alloc((size_t)N * H * W * c); return v; };
+        View xin = mk(C);
+        xin.stats_rep = 2; xin.stats_rep_stride = (long)N * C * 2;
+        xin.stats = rt.alloc_stats((size_t)2 * N * C * 2); xin.stats_ld = C;
+        nchw_to_nhwc(make_img(x, N, C, H, W), xin, s);
+        norm_stats(xin, s);
+        View g = mk(C), o = mk(C);
+        nchw_to_nhwc(make_img(dy, N, C, H, W), g, s);
+        group_norm_backward(xin, groups, gamma, beta, film0, film1, 2 * C, act, g, 0, o, d_film, 2 * C, nullptr, RES_NONE, nullptr,
+                            rt.alloc_stats((size_t)N * C * 2), P->alloc((size_t)N * C * 8), s);
+        nhwc_to_nchw(o, dx, s);
+    });
+}
+
+int tha4_test_attention_backward(tha4_ctx* ctx, const float* qkv, const float* dout, int N, int C, int heads, float* dqkv, void* stream) {
+    return guarded(ctx, [&] {
+        cudaStream_t s = (cudaStream_t)stream;
+        begin_pass(ctx, s);
+        Pool* P = &ctx->persist;
+        auto mk = [&](int c) { View v; v.N = N; v.H = 16; v.W = 16; v.C = c; v.ld = c; v.p = P->alloc((size_t)N * 256 * c); return v; };
+        View q = mk(3 * C), g = mk(C), o = mk(3 * C);
+        nchw_to_nhwc(make_img(qkv, N, 3 * C, 16, 16), q, s);
+        nchw_to_nhwc(make_img(dout, N, C, 16, 16), g, s);
+        attention_backward(q, g, heads, o, P->alloc((size_t)N * heads * 256 * 4), s);
+        nhwc_to_nchw(o, dqkv, s);
     });
 }
 

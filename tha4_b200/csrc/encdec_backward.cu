@@ -247,6 +247,19 @@ __global__ void __launch_bounds__(256) tail_bwd_kernel(const TailBwdArgs a) {
                 dh[2] = dalpha * alpha * (1.0f - alpha);
                 dh[7] = dca * ca * (1.0f - ca);
                 if (a.d1) *reinterpret_cast<float4*>(a.d1 + i * a.dld) = make_float4(dbg[0], dbg[1], dbg[2], dbg[3]);
+            } else if (KIND == TAIL_UNET) {
+                // U-Net: outputs merged(4) alpha(1) warped(4) grid(2) direct(4); heads direct(0..3) grid(4,5) alpha logit(6)
+                const float alpha = a.out[1][at(1, 0, 1)];
+                float dalpha = gv(a.g[1], at(1, 0, 1));
+#pragma unroll
+                for (int c = 0; c < 4; ++c) {
+                    const float direct = a.out[4][at(4, c, 4)], warped = a.out[2][at(2, c, 4)];
+                    const float g0 = gv(a.g[0], at(0, c, 4));
+                    dh[c] = gv(a.g[4], at(4, c, 4)) + g0 * alpha;
+                    dalpha += g0 * (direct - warped);
+                    dwarp[c] = gv(a.g[2], at(2, c, 4)) + g0 * (1.0f - alpha);
+                }
+                dh[6] = dalpha * alpha * (1.0f - alpha);
             } else {
                 const float eya = a.out[1][at(1, 0, 1)], ima = a.out[4][at(4, 0, 1)];
                 float deya = gv(a.g[1], at(1, 0, 1)), dima = gv(a.g[4], at(4, 0, 1));
@@ -268,7 +281,8 @@ __global__ void __launch_bounds__(256) tail_bwd_kernel(const TailBwdArgs a) {
                 dh[11] = deya * eya * (1.0f - eya);
             }
             // grid_sample(img0, base + grid) w.r.t. the grid (zero where the border clamp is active) and w.r.t. img0
-            const float gcx = a.out[7][at(7, 0, 2)], gcy = a.out[7][at(7, 1, 2)];
+            constexpr int GO = KIND == TAIL_UNET ? 3 : 7, GH = KIND == TAIL_UNET ? 4 : 0;     // grid output, grid head channel
+            const float gcx = a.out[GO][at(GO, 0, 2)], gcy = a.out[GO][at(GO, 1, 2)];
             const SampleAt sa = sample_locate(a.base, x, y, gcx, gcy, S);
             float gix = 0.0f, giy = 0.0f;
 #pragma unroll
@@ -277,8 +291,8 @@ __global__ void __launch_bounds__(256) tail_bwd_kernel(const TailBwdArgs a) {
                 gix += dwarp[c] * sample_dix(v, sa);
                 giy += dwarp[c] * sample_diy(v, sa);
             }
-            dh[0] = gv(a.g[7], at(7, 0, 2)) + gix * sa.mx;
-            dh[1] = gv(a.g[7], at(7, 1, 2)) + giy * sa.my;
+            dh[GH] = gv(a.g[GO], at(GO, 0, 2)) + gix * sa.mx;
+            dh[GH + 1] = gv(a.g[GO], at(GO, 1, 2)) + giy * sa.my;
             if (a.d0) {      // corners and weights of the inference tail (gs_locate / gs_sample), as image_grad_kernel
                 const GsTap t = gs_locate(a.base[x], a.base[y], gcx, gcy, S, S);
                 const float wx1 = __fsub_rn(t.ix, t.fx), wx0 = __fsub_rn(__fadd_rn(t.fx, 1.0f), t.ix);
@@ -311,7 +325,10 @@ View fresh(Pool* P, int N, int H, int W, int C) {
     return v;
 }
 
-void run_dgrad(Runtime& rt, const ConvWeights& cw, const View& dy, const View& dx, const View* add = nullptr) {
+}  // namespace
+
+// ------------------------------------------------------------------------------------------------ shared entry points
+void run_dgrad(Runtime& rt, const ConvWeights& cw, const View& dy, const View& dx, const View* add) {
     ConvArgs a;
     a.in = dy; a.out = dx; a.strict = rt.strict;
     if (add) { a.res = *add; a.res_mode = RES_SAME; }
@@ -320,9 +337,15 @@ void run_dgrad(Runtime& rt, const ConvWeights& cw, const View& dy, const View& d
     conv_forward(cw, a, rt.stream);
 }
 
-}  // namespace
+void head_pack_adjoint(ConvWeights& cw, const TailWeights& tw, bool round_w, cudaStream_t s) {
+    conv_describe(cw, CONV_3x3, 16, tw.C);
+    cw.w = reinterpret_cast<float*>(tracked_malloc(conv_packed_floats(cw) * sizeof(float)));
+    THA4_CUDA_CHECK(cudaMemsetAsync(cw.w, 0, conv_packed_floats(cw) * sizeof(float), s));
+    cw.tf32_rounded = round_w;
+    head_adjoint_pack_kernel<<<grid_for(9L * tw.C * tw.CO), 256, 0, s>>>(cw.w, tw.w, tw.C, tw.CO, cw.cin_pad, cw.cout_pad, round_w ? 1 : 0);
+    THA4_LAUNCH_CHECK();
+}
 
-// ------------------------------------------------------------------------------------------------ shared entry points
 void conv_pack_adjoint(ConvWeights& cw, ConvKind kind, const float* w_ref, int cin, int cout, int cout_kernel, cudaStream_t s) {
     // kind / cin / cout describe the FORWARD conv (w_ref in its reference layout); cw becomes the conv from cout to cin channels
     // (cout_kernel >= cin output channels, the extra ones zero)
@@ -376,15 +399,15 @@ void norm_backward(const View& x, const float* gamma, const float* beta, int act
 
 void tail_backward(TailKind kind, const float* const* outputs, const float* const* grads, const ImgView& image0, const ImgView& image1,
                    const View& dh, float* d0, float* d1, int dld, cudaStream_t s) {
-    THA4_REQUIRE(kind != TAIL_UNET, "tail backward: encoder-decoder tails only");
     THA4_REQUIRE(dh.C == 16 && dh.ld == 16 && dh.H == image0.H && dh.W == image0.W && image0.H == image0.W, "tail backward: dims");
     TailBwdArgs a;
-    const int nout = kind == TAIL_DECOMPOSER ? 6 : 8;
+    const int nout = kind == TAIL_UNET ? 5 : (kind == TAIL_DECOMPOSER ? 6 : 8);
     for (int k = 0; k < 8; ++k) { a.out[k] = k < nout ? outputs[k] : nullptr; a.g[k] = (grads && k < nout) ? grads[k] : nullptr; }
     a.img0 = image0; a.img1 = image1; a.base = base_grid_table(image0.H);
     a.S = image0.H; a.N = dh.N; a.dh = dh.p; a.d0 = d0; a.d1 = d1; a.dld = dld;
     const long total = (long)a.N * a.S * a.S;
-    if (kind == TAIL_DECOMPOSER) tail_bwd_kernel<TAIL_DECOMPOSER><<<grid_for(total), 256, 0, s>>>(a);
+    if (kind == TAIL_UNET) tail_bwd_kernel<TAIL_UNET><<<grid_for(total), 256, 0, s>>>(a);
+    else if (kind == TAIL_DECOMPOSER) tail_bwd_kernel<TAIL_DECOMPOSER><<<grid_for(total), 256, 0, s>>>(a);
     else if (kind == TAIL_COMBINER) tail_bwd_kernel<TAIL_COMBINER><<<grid_for(total), 256, 0, s>>>(a);
     else tail_bwd_kernel<TAIL_FACE><<<grid_for(total), 256, 0, s>>>(a);
     THA4_LAUNCH_CHECK();
@@ -410,13 +433,7 @@ void EncDecNet::load_adjoints(const StateDict& sd, const std::string& p, cudaStr
     }
     for (int i = 0; i < 3; ++i) adj(adj_up_[i], p + "upsample_blocks." + std::to_string(i) + ".0", CONVT_4x4_S2);
     // the heads: one 3x3 conv from the 16-channel head-gradient tensor to the 64 feature channels
-    conv_describe(adj_head_, CONV_3x3, 16, tail_.C);
-    adj_head_.w = reinterpret_cast<float*>(tracked_malloc(conv_packed_floats(adj_head_) * sizeof(float)));
-    THA4_CUDA_CHECK(cudaMemsetAsync(adj_head_.w, 0, conv_packed_floats(adj_head_) * sizeof(float), s));
-    adj_head_.tf32_rounded = conv_pack_rounding();
-    head_adjoint_pack_kernel<<<grid_for(9L * tail_.C * tail_.CO), 256, 0, s>>>(adj_head_.w, tail_.w, tail_.C, tail_.CO, adj_head_.cin_pad,
-                                                                             adj_head_.cout_pad, conv_pack_rounding() ? 1 : 0);
-    THA4_LAUNCH_CHECK();
+    head_pack_adjoint(adj_head_, tail_, conv_pack_rounding(), s);
 }
 
 void EncDecNet::backward(Runtime& rt, const ImgView& image0, const ImgView& image1, const float* pose, int pose_ld, const EncDecGrads& g) {

@@ -558,7 +558,7 @@ void UNetNet::load(const StateDict& sd, cudaStream_t s) {
 }
 
 // ResBlock (unet.py:154-165).  mode: 0 same, 1 up (nearest x2), 2 down (AvgPool2d(2)).
-void UNetNet::res_block(Runtime& rt, const ResBlockW& w, const View& x, int mode, const float* film1, const View& out) {
+void UNetNet::res_block(Runtime& rt, const ResBlockW& w, const View& x, int mode, const float* film1, const View& out, UNetTape* tape) {
     cudaStream_t s = rt.stream;
     rt.scratch->reset();
     THA4_REQUIRE(x.C == w.cin && out.C == w.cout, "res_block: channels");
@@ -568,10 +568,11 @@ void UNetNet::res_block(Runtime& rt, const ResBlockW& w, const View& x, int mode
     const bool h16 = rt.f16 != 0;
     View t0 = h16 ? make_view16(rt.scratch, B, th, th, w.cin) : make_view(rt.scratch, B, th, th, w.cin);
     run_norm(rt, x, w.norm0, 32, nullptr, nullptr, 0, rt.strict ? ACT_SILU : ACT_SILU_FAST, mode == 2 ? 1 : 0, nullptr, t0);
-    View h = make_view(rt.scratch, B, out.H, out.W, w.cout, &rt);
+    View h = make_view(tape ? rt.persist : rt.scratch, B, out.H, out.W, w.cout, &rt);
     run_conv(rt, w.conv0, t0, h);      // mode 1: conv0 was packed as CONV_UP2_3x3 (upsample folded into 4 phases)
+    if (tape) tape->res[&w] = {x, h};
     // norm1 -> FiLM(time) -> FiLM(pose) -> SiLU, folded into one per-(n,c) affine
-    const View h2 = h16 ? make_view16(rt.scratch, B, out.H, out.W, w.cout) : h;
+    const View h2 = h16 ? make_view16(rt.scratch, B, out.H, out.W, w.cout) : (tape ? make_view(rt.scratch, B, out.H, out.W, w.cout) : h);
     run_norm(rt, h, w.norm1, 32, w.film0, film1 + w.film1_off, film1_total_, rt.strict ? ACT_SILU : ACT_SILU_FAST, 0, nullptr, h2);
     if (w.has_skip) {
         THA4_REQUIRE(mode == 0, "res_block: skip conv only on same-resolution blocks");
@@ -584,23 +585,24 @@ void UNetNet::res_block(Runtime& rt, const ResBlockW& w, const View& x, int mode
 }
 
 // AttentionBlock (unet.py:230-239)
-void UNetNet::attn_block(Runtime& rt, const AttnW& w, const View& x, const View& out) {
+void UNetNet::attn_block(Runtime& rt, const AttnW& w, const View& x, const View& out, UNetTape* tape) {
     cudaStream_t s = rt.stream;
     rt.scratch->reset();
     View t = rt.f16 ? make_view16(rt.scratch, x.N, x.H, x.W, x.C) : make_view(rt.scratch, x.N, x.H, x.W, x.C);
     run_norm(rt, x, w.norm, 32, nullptr, nullptr, 0, ACT_NONE, 0, nullptr, t);
-    View qkv = make_view(rt.scratch, x.N, x.H, x.W, 3 * x.C);
+    View qkv = make_view(tape ? rt.persist : rt.scratch, x.N, x.H, x.W, 3 * x.C);
     run_conv(rt, w.qkv, t, qkv);
+    if (tape) tape->attn[&w] = {x, qkv};
     View a = make_view(rt.scratch, x.N, x.H, x.W, x.C);
     attention_forward(qkv, 8, a, s, !rt.strict);
     run_conv(rt, w.proj, a, out, 0, &x, RES_SAME);
 }
 
 void UNetNet::forward(Runtime& rt, const ImgView& image, const float* coarse_posed, const float* coarse_grid, int coarse_size,
-                      const float* pose, int pose_ld, float* const* outputs) {
+                      const float* pose, int pose_ld, float* const* outputs, UNetTape* tape) {
     THA4_REQUIRE(loaded_, "network weights not loaded");
     THA4_REQUIRE(image.H == S_ && image.W == S_ && image.C == 4, "unet: image size");
-    if (rt.f16) { forward_fused(rt, image, coarse_posed, coarse_grid, coarse_size, pose, pose_ld, outputs); return; }
+    if (rt.f16) { forward_fused(rt, image, coarse_posed, coarse_grid, coarse_size, pose, pose_ld, outputs, tape); return; }
     const int B = image.N;
     cudaStream_t s = rt.stream;
     Pool* P = rt.persist;
@@ -613,6 +615,7 @@ void UNetNet::forward(Runtime& rt, const ImgView& image, const float* coarse_pos
     linear_forward(pose, pose_ld, B, 6, cond_w0_, cond_b0_, 256, 0, c1, 256, s);
     linear_forward(c1, 256, B, 256, cond_w2_, cond_b2_, 256, 1, c2, 256, s);
     linear_forward(c2, 256, B, 256, film1_w_, film1_b_, film1_total_, 1, film1, film1_total_, s);
+    if (tape) { tape->c1 = c1; tape->c2 = c2; tape->film1 = film1; }
 
     View x0;
     if (upscaler_) {
@@ -649,14 +652,14 @@ void UNetNet::forward(Runtime& rt, const ImgView& image, const float* coarse_pos
     for (int i = 0; i < L_; ++i) {
         if (i == L_ - 1) {
             View tmp = make_view(P, B, cur.H, cur.W, down_res_[i].cout, &rt);
-            res_block(rt, down_res_[i], cur, 0, film1, tmp);
-            attn_block(rt, down_attn_, tmp, hs[2 * i + 1]);
+            res_block(rt, down_res_[i], cur, 0, film1, tmp, tape);
+            attn_block(rt, down_attn_, tmp, hs[2 * i + 1], tape);
         } else {
-            res_block(rt, down_res_[i], cur, 0, film1, hs[2 * i + 1]);
+            res_block(rt, down_res_[i], cur, 0, film1, hs[2 * i + 1], tape);
         }
         cur = hs[2 * i + 1];
         if (i < L_ - 1) {
-            res_block(rt, down_ds_[i], cur, 2, film1, hs[2 * i + 2]);
+            res_block(rt, down_ds_[i], cur, 2, film1, hs[2 * i + 2], tape);
             cur = hs[2 * i + 2];
         }
     }
@@ -664,11 +667,11 @@ void UNetNet::forward(Runtime& rt, const ImgView& image, const float* coarse_pos
     for (int j = 0; j < 4; ++j) {
         const bool last = (j == 3);
         View r = last ? cat[0].slice(0, ch_h[0]) : make_view(P, B, cur.H, cur.W, cur.C, &rt);
-        res_block(rt, mid_res_[j], cur, 0, film1, r);
+        res_block(rt, mid_res_[j], cur, 0, film1, r, tape);
         cur = r;
         if (!last) {
             View a = make_view(P, B, cur.H, cur.W, cur.C, &rt);
-            attn_block(rt, mid_attn_[j], cur, a);
+            attn_block(rt, mid_attn_[j], cur, a, tape);
             cur = a;
         }
     }
@@ -683,18 +686,19 @@ void UNetNet::forward(Runtime& rt, const ImgView& image, const float* coarse_pos
         else dst = make_view(P, B, cat[j].H, cat[j].W, co, &rt);      // goes to the upsampler or is the final feature
         if (lvl == L_ - 1) {
             View tmp = make_view(P, B, cat[j].H, cat[j].W, co, &rt);
-            res_block(rt, up_res_[j], cat[j], 0, film1, tmp);
-            attn_block(rt, up_attn_[second ? 1 : 0], tmp, dst);
+            res_block(rt, up_res_[j], cat[j], 0, film1, tmp, tape);
+            attn_block(rt, up_attn_[second ? 1 : 0], tmp, dst, tape);
         } else {
-            res_block(rt, up_res_[j], cat[j], 0, film1, dst);
+            res_block(rt, up_res_[j], cat[j], 0, film1, dst, tape);
         }
         if (second) {
-            if (lvl > 0) res_block(rt, up_us_[L_ - 1 - lvl], dst, 1, film1, cat[j + 1].slice(0, ch_h[j + 1]));
+            if (lvl > 0) res_block(rt, up_us_[L_ - 1 - lvl], dst, 1, film1, cat[j + 1].slice(0, ch_h[j + 1]), tape);
             else feat = dst;
         }
     }
     // ---- last: GroupNorm + SiLU pending, applied inside the fused tail (unet.py:526-529; morpher_00.py:53-58) ----
     rt.scratch->reset();
+    if (tape) tape->feat = feat;
     float* coef = tail_coef(rt, feat, last_n_, 32);
     ImgView none{};
     tail_forward(TAIL_UNET, tail_, feat, coef, rt.strict ? ACT_SILU : ACT_SILU_FAST, image, none, outputs, s, rt.strict);
@@ -706,10 +710,19 @@ void UNetNet::forward(Runtime& rt, const ImgView& image, const float* coarse_pos
 // Only the down-sampling blocks keep a normalisation pass (SiLU must precede the 2x2 mean, unet.py:58,158).
 namespace {
 
+// a normalisation's input as the fused consumer conv reads it: the f16 operand copy when there is one, with the statistics
+View op_view(const Tens& a) {
+    if (!a.h.p) return a.f;
+    View v = a.h;
+    v.stats = a.f.stats; v.stats_ld = a.f.stats_ld; v.stats_rep = a.f.stats_rep; v.stats_rep_stride = a.f.stats_rep_stride;
+    return v;
+}
+
 struct UNetFused {
     Runtime& rt;
     const float* film1;
     int film1_total;
+    UNetTape* tape;
 
     // ResBlock (unet.py:154-165).  mode: 0 same, 1 up (nearest x2), 2 down (AvgPool2d(2)).
     void res_block(const ResBlockW& w, const Tens& x, int mode, const Tens& out) {
@@ -721,7 +734,8 @@ struct UNetFused {
                      "res_block: the input lacks a precision the block reads");
         const int B = x.f.N;
         const int act = ACT_SILU_FAST;
-        Tens h0 = make_act(rt.scratch, rt, B, out.f.H, out.f.W, w.cout, false, true);
+        Tens h0 = make_act(tape ? rt.persist : rt.scratch, rt, B, out.f.H, out.f.W, w.cout, false, true);
+        if (tape) tape->res[&w] = {mode == 2 ? x.f : op_view(x), raw_view(h0)};
         Tens sk;
         if (w.has_skip) {
             // skip(x) depends on x only: it runs on the side stream next to norm0 -> conv0 (a latency-bound chain,
@@ -764,9 +778,10 @@ struct UNetFused {
     // AttentionBlock (unet.py:230-239): GroupNorm fused into the qkv conv
     void attn_block(const AttnW& w, const Tens& x, const Tens& out) {
         rt.scratch->reset();
-        Tens qkv = make_act(rt.scratch, rt, x.f.N, x.f.H, x.f.W, 3 * x.f.C, true, false, false);
+        Tens qkv = make_act(tape ? rt.persist : rt.scratch, rt, x.f.N, x.f.H, x.f.W, 3 * x.f.C, true, false, false);
         const ConvNormIn n = norm_in(x.f, w.norm, 32, ACT_NONE);
         run_conv_tc(rt, w.qkv, x.h, &n, qkv);
+        if (tape) tape->attn[&w] = {op_view(x), qkv.f};
         View a = make_view(rt.scratch, x.f.N, x.f.H, x.f.W, x.f.C);
         attention_forward(qkv.f, 8, a, rt.stream, true);
         run_conv_tc(rt, w.proj, a, nullptr, out, &x.f, RES_SAME);
@@ -776,7 +791,7 @@ struct UNetFused {
 }  // namespace
 
 void UNetNet::forward_fused(Runtime& rt, const ImgView& image, const float* coarse_posed, const float* coarse_grid, int coarse_size,
-                            const float* pose, int pose_ld, float* const* outputs) {
+                            const float* pose, int pose_ld, float* const* outputs, UNetTape* tape) {
     const int B = image.N;
     cudaStream_t s = rt.stream;
     Pool* P = rt.persist;
@@ -797,7 +812,8 @@ void UNetNet::forward_fused(Runtime& rt, const ImgView& image, const float* coar
     linear_forward(c1, 256, B, 256, cond_w2_, cond_b2_, 256, 1, c2, 256, ls);
     linear_forward(c2, 256, B, 256, film1_w_, film1_b_, film1_total_, 1, film1, film1_total_, ls);
     if (rt.side) THA4_CUDA_CHECK(cudaEventRecord(rt.ev_join, rt.side));
-    UNetFused F{rt, film1, film1_total_};
+    if (tape) { tape->c1 = c1; tape->c2 = c2; tape->film1 = film1; }
+    UNetFused F{rt, film1, film1_total_, tape};
 
     View x0;
     if (upscaler_) {
@@ -891,9 +907,11 @@ void UNetNet::forward_fused(Runtime& rt, const ImgView& image, const float* coar
         View fv = feat.h;
         fv.stats = feat.f.stats; fv.stats_ld = feat.f.stats_ld; fv.stats_rep = feat.f.stats_rep; fv.stats_rep_stride = feat.f.stats_rep_stride;
         NormSpecTail ns; ns.groups = 32; ns.act = ACT_SILU_FAST; ns.gamma = last_n_.gamma; ns.beta = last_n_.beta;
+        if (tape) tape->feat = fv;
         const View g0 = x0.slice(0, 4);       // channels 0-3 of the network input are the image the tail warps (Upscaler02: the rest image)
         tail_tc_forward(TAIL_UNET, tail_, fv, ns, image, none, outputs, s, &g0);
     } else {
+        if (tape) tape->feat = feat.f;
         float* coef = tail_coef(rt, feat.f, last_n_, 32);
         tail_forward(TAIL_UNET, tail_, feat.f, coef, ACT_SILU_FAST, image, none, outputs, s, rt.strict);
     }

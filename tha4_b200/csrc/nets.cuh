@@ -112,6 +112,29 @@ struct ResBlockW {
 };
 struct AttnW { int C = 0; NormW norm; ConvWeights qkv, proj; };
 
+// The activations the U-Net backward reads from the forward it recomputes, keyed by the block's weights (each block runs
+// once per forward).  Normalised tensors are kept as the normalisation read them (fp32, or the f16 operand copy), with the
+// statistics their producer accumulated.
+struct UNetTape {
+    struct Res { View x, h0; };       // block input (norm0), raw conv0 output (norm1)
+    struct Attn { View x, qkv; };     // block input (norm), qkv projection (fp32)
+    std::map<const ResBlockW*, Res> res;
+    std::map<const AttnW*, Attn> attn;
+    const float* c1 = nullptr;        // pose MLP pre-activations [N][256] (unet.py:449-452): cond_embed.0 output
+    const float* c2 = nullptr;        //   cond_embed.2 output
+    const float* film1 = nullptr;     // the batched pose FiLM table [N][film1_total]
+    View feat;                        // last feature map (last.0's input)
+};
+
+// What UNetNet::backward computes: grad_outputs[5] (merged, alpha, warped, grid_change, direct; NCHW, null = zero);
+// d_image [N,4,S,S] and d_pose [N][d_pose_ld] (first 6 entries per row) are outputs, null = not computed.
+struct UNetGrads {
+    const float* const* grad_outputs = nullptr;
+    float* d_image = nullptr;
+    float* d_pose = nullptr;
+    int d_pose_ld = 0;
+};
+
 // Morpher00 (morpher_00.py:35-72) and Upscaler02 (upscaler_02.py:37-102) on Unet / UnetWithFirstConvAddition
 // (unet.py:438-546,549-658).
 class UNetNet {
@@ -119,16 +142,29 @@ public:
     UNetNet(bool upscaler, int size, int model_channels, std::vector<int> mults);
     void load(const StateDict& sd, cudaStream_t s);
     // morpher: image = [B,4,S,S]; upscaler: image = rest image, half_posed / half_grid at S/2 (mode_07.py:111-118).
+    // tape: keep what backward() reads (its tensors then live in rt.persist; normalisations write out of place).
     void forward(Runtime& rt, const ImgView& image, const float* coarse_posed, const float* coarse_grid, int coarse_size,
-                 const float* pose, int pose_ld, float* const* outputs);
+                 const float* pose, int pose_ld, float* const* outputs, UNetTape* tape = nullptr);
+    // Input gradients of the body morpher (unet_backward.cu): recomputes the forward in the context's precision mode with a
+    // tape, then runs the adjoint of every layer back to the inputs that were asked for.  Refused on the upscaler.
+    void backward(Runtime& rt, const ImgView& image, const float* pose, int pose_ld, const UNetGrads& g);
     int size() const { return S_; }
     bool loaded() const { return loaded_; }
 private:
     AllocSink owned_;          // every device allocation made by load()
     void forward_fused(Runtime& rt, const ImgView& image, const float* coarse_posed, const float* coarse_grid, int coarse_size,
-                       const float* pose, int pose_ld, float* const* outputs);
-    void res_block(Runtime& rt, const ResBlockW& w, const View& x, int mode, const float* film1, const View& out);
-    void attn_block(Runtime& rt, const AttnW& w, const View& x, const View& out);
+                       const float* pose, int pose_ld, float* const* outputs, UNetTape* tape);
+    void res_block(Runtime& rt, const ResBlockW& w, const View& x, int mode, const float* film1, const View& out, UNetTape* tape);
+    void attn_block(Runtime& rt, const AttnW& w, const View& x, const View& out, UNetTape* tape);
+    // adjoint-packed weights, made from the packed forward weights by the first backward() (inference-only contexts never
+    // hold them): per ResBlock conv0 / conv1 / skip, per attention block qkv / proj, the first conv and the last.2 head
+    struct ResAdj { ConvWeights conv0, conv1, skip; };
+    struct AttnAdj { ConvWeights qkv, proj; };
+    void pack_adjoints(Runtime& rt);
+    bool adj_ready_ = false;
+    std::map<const ResBlockW*, ResAdj> adj_res_;
+    std::map<const AttnW*, AttnAdj> adj_attn_;
+    ConvWeights adj_first_, adj_head_;
     bool upscaler_;
     int S_, mc_, L_;
     std::vector<int> mults_;
@@ -143,5 +179,15 @@ private:
     NormW last_n_;
     TailWeights tail_;
 };
+
+// ------------------------------------------------------------------ backward helpers shared by the networks
+// Data gradient of a conv on the conv kernels: dx = conv(dy) with adjoint-packed weights (+ add, same resolution).
+void run_dgrad(Runtime& rt, const ConvWeights& cw, const View& dy, const View& dx, const View* add = nullptr);
+// The fused tail's head conv (tw.w) as one packed 3x3 conv from its 16-channel head-gradient tensor to the tw.C features.
+void head_pack_adjoint(ConvWeights& cw, const TailWeights& tw, bool round_w, cudaStream_t s);
+// adjoint of a PACKED forward conv (fwd, of kind `kind`) as a conv from fwd.cout to fwd.cin channels: 3x3 -> 3x3 with W^T
+// flipped, 1x1 -> 1x1 with W^T, CONV_UP2_3x3 (nearest x2 + 3x3, pre-summed phases) -> 4x4 stride-2 conv with W^T.  Allocates
+// cw.w with tracked_malloc; the values are those of fwd (TF32-rounded iff fwd's are).
+void conv_adjoint_from_packed(ConvWeights& cw, const ConvWeights& fwd, ConvKind kind, cudaStream_t s);
 
 }  // namespace tha4

@@ -104,10 +104,28 @@ void tail_tc_forward(TailKind kind, const TailWeights& tw, const View& feature, 
 // InstanceNorm2d(affine) (+ReLU) backward: dx = d/dx of y = act(gamma (x - mean) rstd + beta) for the upstream gradient dy.
 // x: the RAW input (fp32 or f16) with its statistics; dy / dx fp32.  sums: N*C*2 zeroed doubles of workspace.
 void norm_backward(const View& x, const float* gamma, const float* beta, int act, const View& dy, const View& dx, double* sums, cudaStream_t s);
-// Encoder-decoder tail backward (decomposer / combiner / face): from the forward's outputs and their upstream gradients
-// (grads[k] may be null) to dh [N,S,S,16] (head pre-activation gradients in the tail's channel order, rest zero) and the image
-// terms: d0 / d1 NHWC with `dld` floats per pixel (null = not wanted); d0 must be zero on entry for the warping kinds.
+// Tail backward (any kind): from the forward's outputs and their upstream gradients (grads[k] may be null) to dh [N,S,S,16]
+// (head pre-activation gradients in the tail's channel order, rest zero) and the image terms: d0 / d1 NHWC with `dld` floats
+// per pixel (null = not wanted); d0 must be zero on entry for the warping kinds (U-Net, combiner, face).
 void tail_backward(TailKind kind, const float* const* outputs, const float* const* grads, const ImgView& image0, const ImgView& image1,
                    const View& dh, float* d0, float* d1, int dld, cudaStream_t s);
+
+// ---------------------------------------------------------------- backward of the U-Net (unet_backward.cu)
+// GroupNorm(groups) (+ FiLM scale-shifts film0 [2C] / film1 [N][film1_ld]) (+ SiLU when act == ACT_SILU) backward, exact SiLU'
+// at the recomputed pre-activation.  x: the RAW input (fp32 or f16) with its statistics; dy, dx fp32 at x's resolution, or dy at
+// half of it when dy_pool (the layer's output was 2x2-mean-pooled).  dx also gets + res (res_mode RES_SAME, RES_UP2: 2x2 sum of
+// a 2x tensor, RES_DOWN2: 1/4 of a half-resolution tensor; conv.cuh) + add (same resolution); either may be null.  dfilm
+// (optional, needs film1): d(scale) / d(shift) of film1 into [N][dfilm_ld] at c / C + c.  sums: N*C*2 zeroed doubles;
+// coef: N*C*8 floats of workspace.  C <= 512.
+void group_norm_backward(const View& x, int groups, const float* gamma, const float* beta, const float* film0, const float* film1,
+                         int film1_ld, int act, const View& dy, int dy_pool, const View& dx, float* dfilm, int dfilm_ld,
+                         const View* res, int res_mode, const View* add, double* sums, float* coef, cudaStream_t s);
+// qkv_attention backward (fp32, deterministic): qkv NHWC [N,256,3C] as attention_forward read it, dout [N,256,C] -> dqkv
+// [N,256,3C] (dq | dk | dv).  rowstat: N*heads*256*4 floats of workspace.
+void attention_backward(const View& qkv, const View& dout, int heads, const View& dqkv, float* rowstat, cudaStream_t s);
+// data gradient of linear_forward: dx[n][k] = SiLU'(pre[n][k]) sum_r dy[n][r] W[r][k] (pre null: no SiLU), W [R][K], fixed
+// order in fp64
+void linear_backward(const float* dy, int dy_ld, int N, int R, const float* W, int K, const float* pre, int pre_ld, float* dx, int dx_ld,
+                     cudaStream_t s);
 
 }  // namespace tha4

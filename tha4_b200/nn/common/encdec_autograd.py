@@ -1,8 +1,8 @@
 """torch.autograd for the three encoder-decoder teacher networks (EyebrowDecomposer00, EyebrowMorphingCombiner00,
-FaceMorpher08): their outputs are differentiable w.r.t. image, layers and pose, as the reference modules are
-(eyebrow_decomposer_00.py:46-64, eyebrow_morphing_combiner_00.py:47-72, face_morpher_08.py:158-193).  This is what pose
-fitting on an arbitrary character, or training an image -> expression regressor with the face teacher as a differentiable
-renderer, needs.
+FaceMorpher08) and the body morpher U-Net (Morpher00): their outputs are differentiable w.r.t. image, layers and pose, as the
+reference modules are (eyebrow_decomposer_00.py:46-64, eyebrow_morphing_combiner_00.py:47-72, face_morpher_08.py:158-193,
+morpher_00.py:42-66).  This is what pose fitting on an arbitrary character (expression and body parameters), or training an
+image -> pose regressor with a teacher as a differentiable renderer, needs.
 
 Dispatch: the autograd path runs when grad mode is on and an input (image, layer or pose) requires grad; in every other
 case the forward is the plain inference call.  Teacher parameters never receive gradients (there is no teacher training
@@ -114,6 +114,34 @@ def _face_morpher_backward(ctx, *grad_outputs):
     return (None, d_image, d_pose) + none
 
 
+class _MorpherFunction(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, module, image: Tensor, pose: Tensor, *params: Tensor):
+        outs = module.sync_weights().morpher(image, pose)
+        ctx.set_materialize_grads(False)
+        ctx.module = module
+        ctx.save_for_backward(image, pose, *params)
+        return _own(outs)
+
+    @staticmethod
+    def backward(ctx, *grad_outputs):
+        refuse_double_backward('Morpher00')
+        return _morpher_backward(ctx, *grad_outputs)
+
+
+@once_differentiable
+def _morpher_backward(ctx, *grad_outputs):
+    image, pose, *params = ctx.saved_tensors
+    none = (None,) * len(params)
+    want_image, want_pose = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
+    if not (want_image or want_pose) or all(g is None for g in grad_outputs):
+        return (None, None, None) + none
+    d_image = _empty_like(image) if want_image else None
+    d_pose = _empty_like(pose) if want_pose else None
+    ctx.module.sync_weights().morpher_backward(image, pose, contiguous_grads(grad_outputs), d_image=d_image, d_pose=d_pose)
+    return (None, d_image, d_pose) + none
+
+
 def eyebrow_decomposer(module, image: Tensor) -> List[Tensor]:
     return list(_DecomposerFunction.apply(module, image, *module._params()))
 
@@ -124,3 +152,7 @@ def eyebrow_morphing_combiner(module, background_layer: Tensor, eyebrow_layer: T
 
 def face_morpher(module, image: Tensor, pose: Tensor) -> List[Tensor]:
     return list(_FaceMorpherFunction.apply(module, image, pose, *module._params()))
+
+
+def morpher(module, image: Tensor, pose: Tensor) -> List[Tensor]:
+    return list(_MorpherFunction.apply(module, image, pose, *module._params()))
