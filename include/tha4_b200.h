@@ -122,6 +122,15 @@ int tha4_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, 
 int tha4_upscaler_forward(tha4_ctx* ctx, const float* rest_image, const float* coarse_posed_image,
                           const float* coarse_grid_change, int coarse_size, const float* pose, int pose_ld, int B,
                           float* const* outputs, void* stream);
+/* Input gradients of Upscaler02 at the inputs of tha4_upscaler_forward (coarse_size 256 or 512) for upstream gradients of its
+ * 5 outputs (grad_outputs in the forward's output order, NCHW, an entry may be NULL = zero), with the rules of
+ * tha4_morpher_backward: d_rest_image [B,4,512,512], d_coarse_posed_image [B,4,S,S], d_coarse_grid_change [B,2,S,S] (S =
+ * coarse_size; at 256 through the adjoint of the fused bilinear x2) and d_pose [B,6] (contiguous) are optional (NULL = not
+ * computed), at least one non-NULL, each overwritten.  Any B >= 1, in passes of at most min(microbatch, 6) frames (the
+ * backward's workspace is about 2.6 GiB per frame at 512x512).  The adjoint weights are packed by the first call. */
+int tha4_upscaler_backward(tha4_ctx* ctx, const float* rest_image, const float* coarse_posed_image, const float* coarse_grid_change,
+                           int coarse_size, const float* pose, int pose_ld, int B, const float* const* grad_outputs,
+                           float* d_rest_image, float* d_coarse_posed_image, float* d_coarse_grid_change, float* d_pose, void* stream);
 /* SirenFaceMorpher00.forward (src/tha4/nn/siren/face_morpher/siren_face_morpher_00.py:34-51): pose [B,39] -> [B,4,128,128] */
 int tha4_siren_face_morpher_forward(tha4_ctx* ctx, const float* pose, int pose_ld, int B, float* output, void* stream);
 /* SirenMorpher03.forward (src/tha4/nn/siren/morpher/siren_morpher_03.py:107-139): image [B,4,512,512], pose [B,45] ->
@@ -257,8 +266,9 @@ int tha4_test_tail(tha4_ctx* ctx, int kind, const float* feature, int N, int C, 
                    const float* image0, const float* image1, float* const* outputs, int strict, void* stream);
 /* Data gradient of a conv on the conv kernels with adjoint-packed weights: kind 0 3x3 s1 p1 (w [Cout,Cin,3,3]), 1 4x4 s2 p1
  * (w [Cout,Cin,4,4]), 2 4x4 s2 p1 transposed (w [Cin,Cout,4,4]), 3 1x1 (w [Cout,Cin,1,1]), 4 nearest x2 upsample + 3x3 s1 p1
- * (w [Cout,Cin,3,3]; Ho = 2H); dy [N,Cout,Ho,Wo] -> dx [N,Cin,H,W].  Cout % 4 == 0 (and Cin % 4 == 0 for kinds 1..4).
- * Kinds 3 and 4 pack the forward conv first and derive the adjoint from the packed weights, as the U-Net backward does.
+ * (w [Cout,Cin,3,3]; Ho = 2H), 5 3x3 s1 p1 as kind 0; dy [N,Cout,Ho,Wo] -> dx [N,Cin,H,W].  Cout % 4 == 0 (and Cin % 4 == 0
+ * for kinds 1..4).  Kinds 3, 4 and 5 pack the forward conv first (Cin zero-padded to a multiple of 4, as the upscaler's fused
+ * 16-channel first conv) and derive the adjoint from the packed weights, as the U-Net backward does.
  * strict: 3xTF32, else TF32 (fp32 operands in both). */
 int tha4_test_conv_backward_data(tha4_ctx* ctx, int kind, const float* dy, const float* w, float* dx, int N, int Cin, int H, int W,
                                  int Cout, int strict, void* stream);
@@ -271,6 +281,13 @@ int tha4_test_norm_backward(tha4_ctx* ctx, const float* x, int N, int C, int H, 
 int tha4_test_tail_backward(tha4_ctx* ctx, int kind, const float* const* outputs, int N, int S, const float* image0,
                             const float* image1, const float* const* grad_outputs, float* d_head, float* d_image0,
                             float* d_image1, void* stream);
+/* Adjoint of the Upscaler02 prologue (rest image, bilinear x2 of the coarse posed image and grid change, warp of the rest image
+ * by the coarse grid; see tha4_upscaler_forward): rest_image [N,4,512,512], coarse_grid_change [N,2,S,S] (S = coarse_size,
+ * 256 or 512), d_x0 [N,16,512,512] the gradient of the prologue's output channels rest(4) posed(4) warped(4) grid(2) pad(2)
+ * -> d_rest_image [N,4,512,512], d_coarse_posed_image [N,4,S,S], d_coarse_grid_change [N,2,S,S] (NULL = not computed). */
+int tha4_test_upscaler_prologue_backward(tha4_ctx* ctx, const float* rest_image, const float* coarse_grid_change, int coarse_size,
+                                         int N, const float* d_x0, float* d_rest_image, float* d_coarse_posed_image,
+                                         float* d_coarse_grid_change, void* stream);
 /* GroupNorm(groups) (+FiLM) (+SiLU) backward of the U-Net ResBlocks (src/tha4/nn/common/unet.py:154-165): y = act(h), h =
  * (GN(x) * (1 + film0[c]) + film0[C+c]) * (1 + film1[n][c]) + film1[n][C+c] (film0 [2C], film1 [N,2C]; either may be NULL),
  * act 0 none / 2 SiLU.  x, dy, dx [N,C,H,W] (statistics of x computed on the device); d_film [N,2C] (NULL = not computed; needs

@@ -29,8 +29,8 @@ EXPORTED_SYMBOLS = [
     'tha4_siren_morpher_backward', 'tha4_siren_face_morpher_backward',
     'tha4_adam_step', 'tha4_images_differ', 'tha4_frame_to_srgb8', 'tha4_rgba8_to_poser_image', 'tha4_grid_sample', 'tha4_resize_bilinear',
     'tha4_eyebrow_decomposer_backward', 'tha4_eyebrow_morphing_combiner_backward', 'tha4_face_morpher_backward',
-    'tha4_morpher_backward',
-    'tha4_test_conv_backward_data', 'tha4_test_norm_backward', 'tha4_test_tail_backward',
+    'tha4_morpher_backward', 'tha4_upscaler_backward',
+    'tha4_test_conv_backward_data', 'tha4_test_norm_backward', 'tha4_test_tail_backward', 'tha4_test_upscaler_prologue_backward',
     'tha4_test_group_norm_backward', 'tha4_test_attention_backward',
     'tha4_base_grid', 'tha4_test_conv', 'tha4_test_conv_norm', 'tha4_test_conv_norm_ex', 'tha4_test_norm', 'tha4_test_tail', 'tha4_test_attention', 'tha4_test_linear',
     'tha4_test_siren_level', 'tha4_test_sine', 'tha4_test_siren_plan_check',
@@ -275,7 +275,9 @@ class Context:
         self._call('tha4_morpher_backward', _ptr(image), _ptr(pose), 6, B, _ptr_array(gs), _ptr(d_image), _ptr(d_pose),
                    self._stream())
 
-    def upscaler(self, rest_image: Tensor, coarse_posed: Tensor, coarse_grid: Tensor, pose: Tensor) -> List[Tensor]:
+    UPSCALER_SPECS = [(4, 512), (1, 512), (4, 512), (2, 512), (4, 512)]
+
+    def _upscaler_inputs(self, rest_image: Tensor, coarse_posed: Tensor, coarse_grid: Tensor, pose: Tensor):
         rest_image = _check_input(rest_image, self.device, 'rest_image')
         coarse_posed = _check_input(coarse_posed, self.device, 'coarse_posed_image')
         coarse_grid = _check_input(coarse_grid, self.device, 'coarse_grid_change')
@@ -284,10 +286,31 @@ class Context:
         S = coarse_posed.shape[2]
         assert rest_image.shape[1:] == (4, 512, 512) and S in (256, 512)
         assert coarse_posed.shape == (B, 4, S, S) and coarse_grid.shape == (B, 2, S, S) and pose.shape == (B, 6)
-        outs = self._empty([(4, 512), (1, 512), (4, 512), (2, 512), (4, 512)], B)
+        return rest_image, coarse_posed, coarse_grid, pose, B, S
+
+    def upscaler(self, rest_image: Tensor, coarse_posed: Tensor, coarse_grid: Tensor, pose: Tensor) -> List[Tensor]:
+        rest_image, coarse_posed, coarse_grid, pose, B, S = self._upscaler_inputs(rest_image, coarse_posed, coarse_grid, pose)
+        outs = self._empty(self.UPSCALER_SPECS, B)
         self._call('tha4_upscaler_forward', _ptr(rest_image), _ptr(coarse_posed), _ptr(coarse_grid), S, _ptr(pose), 6, B,
                    _ptr_array(outs), self._stream())
         return outs
+
+    def upscaler_backward(self, rest_image: Tensor, coarse_posed: Tensor, coarse_grid: Tensor, pose: Tensor,
+                          grad_outputs: Sequence[Optional[Tensor]], d_rest_image: Optional[Tensor] = None,
+                          d_coarse_posed: Optional[Tensor] = None, d_coarse_grid: Optional[Tensor] = None,
+                          d_pose: Optional[Tensor] = None):
+        """Input gradients of Upscaler02 into any of d_rest_image [B,4,512,512], d_coarse_posed [B,4,S,S], d_coarse_grid
+        [B,2,S,S] (S = the coarse inputs' size, 256 or 512) and d_pose [B,6] (None = not computed) for the upstream gradients
+        of its five outputs (None = zero); the forward is recomputed in the context's precision mode."""
+        assert d_rest_image is not None or d_coarse_posed is not None or d_coarse_grid is not None or d_pose is not None
+        rest_image, coarse_posed, coarse_grid, pose, B, S = self._upscaler_inputs(rest_image, coarse_posed, coarse_grid, pose)
+        gs = self._grads(self.UPSCALER_SPECS, grad_outputs, B)
+        self._check_out(d_rest_image, (B, 4, 512, 512), 'd_rest_image')
+        self._check_out(d_coarse_posed, (B, 4, S, S), 'd_coarse_posed')
+        self._check_out(d_coarse_grid, (B, 2, S, S), 'd_coarse_grid')
+        self._check_out(d_pose, (B, 6), 'd_pose')
+        self._call('tha4_upscaler_backward', _ptr(rest_image), _ptr(coarse_posed), _ptr(coarse_grid), S, _ptr(pose), 6, B,
+                   _ptr_array(gs), _ptr(d_rest_image), _ptr(d_coarse_posed), _ptr(d_coarse_grid), _ptr(d_pose), self._stream())
 
     def siren_face_morpher(self, pose: Tensor) -> Tensor:
         pose = _check_input(pose, self.device, 'pose')

@@ -429,7 +429,31 @@ int tha4_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, 
             UNetGrads ug; ug.grad_outputs = g;
             ug.d_image = d_image ? d_image + (size_t)n0 * 4 * 256 * 256 : nullptr;
             ug.d_pose = d_pose ? d_pose + (size_t)n0 * 6 : nullptr; ug.d_pose_ld = 6;
-            ctx->body->backward(rt, make_img(image + (size_t)n0 * 4 * 256 * 256, b, 4, 256, 256), pose + (size_t)n0 * pose_ld, pose_ld, ug);
+            ctx->body->backward(rt, make_img(image + (size_t)n0 * 4 * 256 * 256, b, 4, 256, 256), nullptr, nullptr, 0,
+                                pose + (size_t)n0 * pose_ld, pose_ld, ug);
+        });
+    });
+}
+
+int tha4_upscaler_backward(tha4_ctx* ctx, const float* rest_image, const float* coarse_posed_image, const float* coarse_grid_change,
+                           int coarse_size, const float* pose, int pose_ld, int B, const float* const* grad_outputs,
+                           float* d_rest_image, float* d_coarse_posed_image, float* d_coarse_grid_change, float* d_pose, void* stream) {
+    return guarded(ctx, [&] {
+        THA4_REQUIRE(d_rest_image || d_coarse_posed_image || d_coarse_grid_change || d_pose, "upscaler backward: no gradient requested");
+        THA4_REQUIRE(coarse_size == 256 || coarse_size == 512, "upscaler backward: coarse_size must be 256 or 512");
+        THA4_REQUIRE(pose_ld >= 6, "upscaler backward: pose rows need at least 6 entries");
+        Runtime rt = make_rt(ctx, stream);
+        OutSpec spec[5]; fill_unet_spec(spec, 512);
+        const size_t hw = 512 * 512, chw = (size_t)coarse_size * coarse_size;
+        for_chunks(ctx, B, std::min(ctx->microbatch, UPSCALER_BWD_MAX_BATCH), rt.stream, [&](int n0, int b) {
+            const float* g[5]; offset_grads<5>(grad_outputs, spec, n0, g);
+            UNetGrads ug; ug.grad_outputs = g;
+            ug.d_image = d_rest_image ? d_rest_image + (size_t)n0 * 4 * hw : nullptr;
+            ug.d_coarse_posed = d_coarse_posed_image ? d_coarse_posed_image + (size_t)n0 * 4 * chw : nullptr;
+            ug.d_coarse_grid = d_coarse_grid_change ? d_coarse_grid_change + (size_t)n0 * 2 * chw : nullptr;
+            ug.d_pose = d_pose ? d_pose + (size_t)n0 * 6 : nullptr; ug.d_pose_ld = 6;
+            ctx->upscaler->backward(rt, make_img(rest_image + (size_t)n0 * 4 * hw, b, 4, 512, 512), coarse_posed_image + (size_t)n0 * 4 * chw,
+                                    coarse_grid_change + (size_t)n0 * 2 * chw, coarse_size, pose + (size_t)n0 * pose_ld, pose_ld, ug);
         });
     });
 }
@@ -952,8 +976,10 @@ int tha4_test_conv_backward_data(tha4_ctx* ctx, int kind, const float* dy, const
     return guarded(ctx, [&] {
         cudaStream_t s = (cudaStream_t)stream;
         begin_pass(ctx, s);
-        THA4_REQUIRE(kind >= 0 && kind <= 4 && Cout % 4 == 0 && (kind == 0 || Cin % 4 == 0),
-                     "test_conv_backward_data: kind 0..4, Cout % 4 == 0 (and Cin % 4 == 0 for kinds 1..4)");
+        THA4_REQUIRE(kind >= 0 && kind <= 5 && Cout % 4 == 0 && (kind == 0 || kind == 5 || Cin % 4 == 0),
+                     "test_conv_backward_data: kind 0..5, Cout % 4 == 0 (and Cin % 4 == 0 for kinds 1..4)");
+        const bool packed = kind >= 3;        // kind 5: a 3x3 conv through the packed forward weights (Cin zero-padded to 4)
+        if (kind == 5) kind = CONV_3x3;
         Runtime rt = make_rt(ctx, stream);
         rt.strict = strict;
         Pool* P = &ctx->persist;
@@ -962,11 +988,11 @@ int tha4_test_conv_backward_data(tha4_ctx* ctx, int kind, const float* dy, const
         {
             SinkScope own(&sink);
             conv_set_pack_rounding(!strict);
-            if (kind <= 2) {
+            if (!packed) {
                 conv_pack_adjoint(cw, (ConvKind)kind, w, Cin, Cout, kind == CONV_3x3 ? round_up(Cin, 4) : 0, s);
             } else {   // the U-Net's path: the forward conv packed as the network packs it, its adjoint made from the packed weights
                 ConvWeights fwd;
-                conv_describe(fwd, (ConvKind)kind, Cin, Cout);
+                conv_describe(fwd, (ConvKind)kind, round_up(Cin, 4), Cout);
                 fwd.w = reinterpret_cast<float*>(tracked_malloc(conv_packed_floats(fwd) * sizeof(float)));
                 THA4_CUDA_CHECK(cudaMemsetAsync(fwd.w, 0, conv_packed_floats(fwd) * sizeof(float), s));
                 conv_pack(fwd, (ConvKind)kind, w, Cin, 0, s);
@@ -1027,6 +1053,24 @@ int tha4_test_tail_backward(tha4_ctx* ctx, int kind, const float* const* outputs
         nhwc_to_nchw(dh.slice(0, 12), d_head, s);
         if (d_image0) nhwc_to_nchw(dimg.slice(0, 4), d_image0, s);
         if (d_image1) nhwc_to_nchw(dimg.slice(4, 4), d_image1, s);
+    });
+}
+
+int tha4_test_upscaler_prologue_backward(tha4_ctx* ctx, const float* rest_image, const float* coarse_grid_change, int coarse_size,
+                                         int N, const float* d_x0, float* d_rest_image, float* d_coarse_posed_image,
+                                         float* d_coarse_grid_change, void* stream) {
+    return guarded(ctx, [&] {
+        cudaStream_t s = (cudaStream_t)stream;
+        THA4_REQUIRE(coarse_size == 256 || coarse_size == 512, "test_upscaler_prologue_backward: coarse_size must be 256 or 512");
+        begin_pass(ctx, s);
+        Pool* P = &ctx->persist;
+        auto mk = [&](int c) { View v; v.N = N; v.H = 512; v.W = 512; v.C = c; v.ld = c; v.p = P->alloc((size_t)N * 512 * 512 * c); return v; };
+        View g = mk(16), dr = mk(4);
+        nchw_to_nhwc(make_img(d_x0, N, 16, 512, 512), g, s);
+        THA4_CUDA_CHECK(cudaMemsetAsync(dr.p, 0, dr.pixels() * 4 * sizeof(float), s));
+        upscaler_prologue_backward(make_img(rest_image, N, 4, 512, 512), coarse_grid_change, coarse_size, g,
+                                   d_rest_image ? dr.p : nullptr, d_coarse_posed_image, d_coarse_grid_change, s);
+        if (d_rest_image) nhwc_to_nchw(dr, d_rest_image, s);
     });
 }
 

@@ -293,21 +293,8 @@ __global__ void __launch_bounds__(256) tail_bwd_kernel(const TailBwdArgs a) {
             }
             dh[GH] = gv(a.g[GO], at(GO, 0, 2)) + gix * sa.mx;
             dh[GH + 1] = gv(a.g[GO], at(GO, 1, 2)) + giy * sa.my;
-            if (a.d0) {      // corners and weights of the inference tail (gs_locate / gs_sample), as image_grad_kernel
-                const GsTap t = gs_locate(a.base[x], a.base[y], gcx, gcy, S, S);
-                const float wx1 = __fsub_rn(t.ix, t.fx), wx0 = __fsub_rn(__fadd_rn(t.fx, 1.0f), t.ix);
-                const float wy1 = __fsub_rn(t.iy, t.fy), wy0 = __fsub_rn(__fadd_rn(t.fy, 1.0f), t.iy);
-                const float wnw = __fmul_rn(wx0, wy0), wne = __fmul_rn(wx1, wy0), wsw = __fmul_rn(wx0, wy1), wse = __fmul_rn(wx1, wy1);
-                const bool xin = (t.x0 + 1) < S, yin = (t.y0 + 1) < S;
-                const long p00 = (long)n * hw + (long)t.y0 * S + t.x0;
-                auto put = [&](long pix, float w) {
-                    atomicAdd(reinterpret_cast<float4*>(a.d0 + pix * a.dld), make_float4(w * dwarp[0], w * dwarp[1], w * dwarp[2], w * dwarp[3]));
-                };
-                put(p00, wnw);
-                if (xin) put(p00 + 1, wne);
-                if (yin) put(p00 + S, wsw);
-                if (xin && yin) put(p00 + S + 1, wse);
-            }
+            if (a.d0)        // corners and weights of the inference tail (gs_locate / gs_sample), as image_grad_kernel
+                gs_scatter4_nhwc(a.d0 + (long)n * hw * a.dld, a.dld, S, S, gs_locate(a.base[x], a.base[y], gcx, gcy, S, S), dwarp);
         }
         float4* d = reinterpret_cast<float4*>(a.dh + i * 16);
         d[0] = make_float4(dh[0], dh[1], dh[2], dh[3]);

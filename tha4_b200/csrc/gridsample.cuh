@@ -134,6 +134,24 @@ __device__ __forceinline__ float sample_diy(const Corners& v, const SampleAt& s)
     return (v.v10 - v.v00) * (1.0f - s.tx) + (v.v11 - v.v01) * s.tx;
 }
 
+// Adjoint of gs_sample w.r.t. the image: adds w * g (4 channels) to the corners of tap t in an NHWC accumulator (`ld` floats
+// per pixel, 16-byte aligned; d points at pixel (0, 0) of the sample), with the corner weights of the inference sampling
+// (red.global.add.v4.f32: not bit-reproducible run to run).
+__device__ __forceinline__ void gs_scatter4_nhwc(float* d, int ld, int W, int H, const GsTap& t, const float (&g)[4]) {
+    const float wx1 = __fsub_rn(t.ix, t.fx), wx0 = __fsub_rn(__fadd_rn(t.fx, 1.0f), t.ix);
+    const float wy1 = __fsub_rn(t.iy, t.fy), wy0 = __fsub_rn(__fadd_rn(t.fy, 1.0f), t.iy);
+    const float wnw = __fmul_rn(wx0, wy0), wne = __fmul_rn(wx1, wy0), wsw = __fmul_rn(wx0, wy1), wse = __fmul_rn(wx1, wy1);
+    const bool xin = (t.x0 + 1) < W, yin = (t.y0 + 1) < H;
+    const long p00 = (long)t.y0 * W + t.x0;
+    auto put = [&](long pix, float w) {
+        atomicAdd(reinterpret_cast<float4*>(d + pix * ld), make_float4(w * g[0], w * g[1], w * g[2], w * g[3]));
+    };
+    put(p00, wnw);
+    if (xin) put(p00 + 1, wne);
+    if (yin) put(p00 + W, wsw);
+    if (xin && yin) put(p00 + W + 1, wse);
+}
+
 // interpolate(bilinear, align_corners=False) source coordinate for one axis.
 struct LerpTap { int i0, i1; float l0, l1; };
 __device__ __forceinline__ LerpTap lerp_locate(int dst, float scale, int in_size) {
@@ -151,6 +169,11 @@ __device__ __forceinline__ float lerp2(const float* __restrict__ im, long sh, co
     const float c = __ldg(im + ty.i1 * sh + tx.i0), d = __ldg(im + ty.i1 * sh + tx.i1);
     return __fadd_rn(__fmul_rn(ty.l0, __fadd_rn(__fmul_rn(tx.l0, a), __fmul_rn(tx.l1, b))),
                      __fmul_rn(ty.l1, __fadd_rn(__fmul_rn(tx.l0, c), __fmul_rn(tx.l1, d))));
+}
+// weight of source index `src` in the interpolation of destination `dst` (0 when neither tap reads it)
+__device__ __forceinline__ float lerp_weight(int dst, float scale, int in_size, int src) {
+    const LerpTap t = lerp_locate(dst, scale, in_size);
+    return (t.i0 == src ? t.l0 : 0.0f) + (t.i1 == src ? t.l1 : 0.0f);
 }
 
 }  // namespace tha4

@@ -187,6 +187,89 @@ __global__ void __launch_bounds__(256) upscaler_prologue_kernel(ImgView rest, co
     }
 }
 
+// Adjoint of upscaler_prologue_kernel.  One thread per COARSE pixel (X, Y) of sample n, r = S / Sh fine pixels per axis.
+// dx0: NHWC [N,S,S,ld] gradient of the prologue's output [rest | posed | warped | grid | 0 0] (channels 14, 15 unread).
+//   drest (NHWC [N,S,S,4], null = not wanted): += channels 0-3 at the thread's own r x r fine pixels, and the grid_sample
+//     image adjoint of channels 8-11 scattered into the corners each of them sampled (atomics, as the tail backward);
+//   d_posed [N,4,Sh,Sh] / d_grid [N,2,Sh,Sh] (NCHW, null = not wanted): the bilinear x2 adjoint as a GATHER over the fine
+//     pixels whose taps read (X, Y) (fixed order, no atomics; the identity when r == 1) of channels 4-7, and of channels
+//     12-13 plus the grid_sample grid gradient of channels 8-11 (zero where the border clamp is active).
+__global__ void __launch_bounds__(256) upscaler_prologue_bwd_kernel(ImgView rest, const float* __restrict__ half_grid,
+                                                                    const float* __restrict__ base, const float* __restrict__ dx0,
+                                                                    int ld, float* __restrict__ drest, float* __restrict__ d_posed,
+                                                                    float* __restrict__ d_grid, int Sh) {
+    const int S = rest.W, r = S / Sh;
+    const float scale = (float)Sh / (float)S;
+    const long hw = (long)S * S, hwh = (long)Sh * Sh;
+    const long total = rest.N * hwh;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+        const int X = (int)(i % Sh);
+        const int Y = (int)((i / Sh) % Sh);
+        const int n = (int)(i / hwh);
+        const float* rn = rest.p + n * rest.sn;
+        const float* gn = half_grid + n * 2L * hwh;
+        const float* dn = dx0 + n * hw * ld;
+        // the fine grid at (x, y), as the forward interpolated it
+        auto fine_grid = [&](int x, int y, float& gx, float& gy) {
+            const LerpTap ty = lerp_locate(y, scale, Sh), tx = lerp_locate(x, scale, Sh);
+            gx = lerp2(gn, Sh, ty, tx);
+            gy = lerp2(gn + hwh, Sh, ty, tx);
+        };
+        if (drest) {
+            float* dr = drest + n * hw * 4;
+            for (int y = r * Y; y < r * Y + r; ++y)
+                for (int x = r * X; x < r * X + r; ++x) {
+                    const float* d = dn + ((long)y * S + x) * ld;
+                    const float4 di = *reinterpret_cast<const float4*>(d);
+                    atomicAdd(reinterpret_cast<float4*>(dr + ((long)y * S + x) * 4), di);
+                    const float4 dw = *reinterpret_cast<const float4*>(d + 8);
+                    const float g[4] = {dw.x, dw.y, dw.z, dw.w};
+                    float gx, gy;
+                    fine_grid(x, y, gx, gy);
+                    gs_scatter4_nhwc(dr, 4, S, S, gs_locate(base[x], base[y], gx, gy, S, S), g);
+                }
+        }
+        if (!d_posed && !d_grid) continue;
+        // fine rows / columns whose taps can read coarse row Y / column X: r Y - (r - 1) .. r Y + 2 (r - 1)
+        float ap[4] = {0.f, 0.f, 0.f, 0.f}, ag[2] = {0.f, 0.f};
+        for (int y = max(r * Y - (r - 1), 0); y <= min(r * Y + 2 * (r - 1), S - 1); ++y) {
+            const float wy = lerp_weight(y, scale, Sh, Y);
+            if (wy == 0.0f) continue;
+            for (int x = max(r * X - (r - 1), 0); x <= min(r * X + 2 * (r - 1), S - 1); ++x) {
+                const float wx = lerp_weight(x, scale, Sh, X);
+                if (wx == 0.0f) continue;
+                const float w = wy * wx;
+                const float* d = dn + ((long)y * S + x) * ld;
+                if (d_posed)
+#pragma unroll
+                    for (int c = 0; c < 4; ++c) ap[c] = fmaf(w, d[4 + c], ap[c]);
+                if (d_grid) {
+                    float gx, gy;
+                    fine_grid(x, y, gx, gy);
+                    const SampleAt sa = sample_locate(base, x, y, gx, gy, S);
+                    float gix = 0.0f, giy = 0.0f;
+#pragma unroll
+                    for (int c = 0; c < 4; ++c) {
+                        const Corners v = sample_corners(rn + c * rest.sc, rest.sh, sa);
+                        gix += d[8 + c] * sample_dix(v, sa);
+                        giy += d[8 + c] * sample_diy(v, sa);
+                    }
+                    ag[0] = fmaf(w, d[12] + gix * sa.mx, ag[0]);
+                    ag[1] = fmaf(w, d[13] + giy * sa.my, ag[1]);
+                }
+            }
+        }
+        const long o = (long)Y * Sh + X;
+        if (d_posed)
+#pragma unroll
+            for (int c = 0; c < 4; ++c) d_posed[(n * 4L + c) * hwh + o] = ap[c];
+        if (d_grid) {
+            d_grid[n * 2L * hwh + o] = ag[0];
+            d_grid[(n * 2L + 1) * hwh + o] = ag[1];
+        }
+    }
+}
+
 __global__ void images_differ_kernel(const float* __restrict__ a, const float* __restrict__ b, size_t n, int* flag) {
     bool d = false;
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
@@ -306,6 +389,16 @@ void upscaler_prologue(const ImgView& rest, const float* half_posed, const float
     THA4_REQUIRE(rest.C == 4 && rest.H == rest.W && dst.C == 16 && dst.H == rest.H && dst.ld % 4 == 0, "upscaler_prologue: dims");
     upscaler_prologue_kernel<<<grid_for((long)rest.N * rest.H * rest.W), 256, 0, s>>>(rest, half_posed, half_grid,
                                                                                       base_grid_table(rest.W), dst.p, dst.ld, coarse_size);
+    THA4_LAUNCH_CHECK();
+}
+
+void upscaler_prologue_backward(const ImgView& rest, const float* half_grid, int coarse_size, const View& dx0, float* drest,
+                                float* d_posed, float* d_grid, cudaStream_t s) {
+    THA4_REQUIRE(coarse_size == rest.H || coarse_size * 2 == rest.H, "upscaler_prologue_backward: coarse size");
+    THA4_REQUIRE(rest.C == 4 && rest.H == rest.W && dx0.C >= 14 && dx0.H == rest.H && dx0.W == rest.W && dx0.N == rest.N &&
+                 !dx0.f16 && dx0.ld % 4 == 0, "upscaler_prologue_backward: dims");
+    upscaler_prologue_bwd_kernel<<<grid_for((long)rest.N * coarse_size * coarse_size), 256, 0, s>>>(
+        rest, half_grid, base_grid_table(rest.W), dx0.p, dx0.ld, drest, d_posed, d_grid, coarse_size);
     THA4_LAUNCH_CHECK();
 }
 

@@ -127,13 +127,21 @@ struct UNetTape {
 };
 
 // What UNetNet::backward computes: grad_outputs[5] (merged, alpha, warped, grid_change, direct; NCHW, null = zero);
-// d_image [N,4,S,S] and d_pose [N][d_pose_ld] (first 6 entries per row) are outputs, null = not computed.
+// d_image [N,4,S,S] (the upscaler: its rest image), d_pose [N][d_pose_ld] (first 6 entries per row) and, on the upscaler only,
+// d_coarse_posed [N,4,c,c] / d_coarse_grid [N,2,c,c] (c = coarse_size) are outputs, null = not computed.
 struct UNetGrads {
     const float* const* grad_outputs = nullptr;
     float* d_image = nullptr;
     float* d_pose = nullptr;
     int d_pose_ld = 0;
+    float* d_coarse_posed = nullptr;
+    float* d_coarse_grid = nullptr;
 };
+
+// Frames per pass of the upscaler backward.  Its taped forward and gradient buffers at 512x512 take 2610 MiB of the context's
+// workspace pool per frame (measured on an H100 at B = 1 and 2, DESIGN.md section 4), and the pool keeps its peak: 6 frames
+// keep a pass under 16 GiB.
+constexpr int UPSCALER_BWD_MAX_BATCH = 6;
 
 // Morpher00 (morpher_00.py:35-72) and Upscaler02 (upscaler_02.py:37-102) on Unet / UnetWithFirstConvAddition
 // (unet.py:438-546,549-658).
@@ -145,9 +153,10 @@ public:
     // tape: keep what backward() reads (its tensors then live in rt.persist; normalisations write out of place).
     void forward(Runtime& rt, const ImgView& image, const float* coarse_posed, const float* coarse_grid, int coarse_size,
                  const float* pose, int pose_ld, float* const* outputs, UNetTape* tape = nullptr);
-    // Input gradients of the body morpher (unet_backward.cu): recomputes the forward in the context's precision mode with a
-    // tape, then runs the adjoint of every layer back to the inputs that were asked for.  Refused on the upscaler.
-    void backward(Runtime& rt, const ImgView& image, const float* pose, int pose_ld, const UNetGrads& g);
+    // Input gradients (unet_backward.cu): recomputes the forward (same inputs as forward()) in the context's precision mode
+    // with a tape, then runs the adjoint of every layer back to the inputs that were asked for.
+    void backward(Runtime& rt, const ImgView& image, const float* coarse_posed, const float* coarse_grid, int coarse_size,
+                  const float* pose, int pose_ld, const UNetGrads& g);
     int size() const { return S_; }
     bool loaded() const { return loaded_; }
 private:

@@ -60,6 +60,12 @@ void grid_sample(const ImgView& image, const float* grid_change, float* out, int
 // coarse_size: resolution of `posed` / `grid` (S/2 in the fused pipeline; S when the caller already upsampled).
 void upscaler_prologue(const ImgView& rest, const float* posed, const float* grid, int coarse_size, const View& dst,
                        cudaStream_t s);
+// Its adjoint for dx0, the gradient of dst (NHWC, >= 14 channels; 14, 15 unread): drest (NHWC [N,S,S,4], 4 floats per pixel,
+// accumulated into with atomics; null = not wanted) += the rest-image terms (identity + the warp's image adjoint); d_posed
+// [N,4,coarse,coarse] / d_grid [N,2,coarse,coarse] (NCHW, overwritten, null = not wanted): the posed / grid terms through the
+// bilinear x2 adjoint (a fixed-order gather; the grid gradient of the warp is zero where the border clamp is active).
+void upscaler_prologue_backward(const ImgView& rest, const float* grid, int coarse_size, const View& dx0, float* drest,
+                                float* d_posed, float* d_grid, cudaStream_t s);
 // Poser output [B,4,H,W] in [-1,1] -> [B,H,W,4] uint8 sRGB (+ optional opaque background), and PNG pixels [H,W,4] uint8 ->
 // poser input [4,H,W]; see image_ops.cu.
 void frame_to_srgb8(const float* frame, int B, int H, int W, int background, int round_mode, unsigned char* out, cudaStream_t s);

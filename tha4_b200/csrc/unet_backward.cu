@@ -1,5 +1,6 @@
-// Input gradients of the body morpher U-Net (Morpher00; morpher_00.py:42-66 on unet.py:531-546): d(image) and d(pose) for
-// upstream gradients of its five outputs.
+// Input gradients of the U-Nets -- the body morpher (Morpher00; morpher_00.py:42-66 on unet.py:531-546): d(image) and d(pose),
+// and the upscaler (Upscaler02; upscaler_02.py:59-96 on unet.py:645-658): d(rest image), d(coarse posed image), d(coarse grid
+// change) and d(pose) -- for upstream gradients of their five outputs.
 //
 // The forward is recomputed with the inference kernels of the context's precision mode, keeping a tape (UNetTape): every
 // ResBlock's input and raw conv0 output, every attention block's input and qkv, the pose MLP pre-activations and the FiLM
@@ -13,7 +14,9 @@
 //   resampling: AvgPool2d(2) -> 1/4 nearest-up read inside the norm backward; nearest x2 residual -> 2x2 sum;
 //   attention: P recomputed from the taped qkv, fp32, dK / dV owned by one thread per key (no atomics);
 //   skips:     the d(cat) half of a skip tensor is added in the epilogue of its down-path consumer's last adjoint;
-//   pose:      d(film1) through the FiLM projection, cond_embed.2 and cond_embed.0 (fixed-order fp64 GEMVs).
+//   pose:      d(film1) through the FiLM projection, cond_embed.2 and cond_embed.0 (fixed-order fp64 GEMVs);
+//   upscaler:  the fused 16-channel first conv's data gradient goes through the prologue's adjoint (image_ops.cu): identity
+//              and warp terms to the rest image (which the tail warps too), the posed / grid terms through the bilinear x2.
 #include "nets.cuh"
 
 namespace tha4 {
@@ -506,11 +509,14 @@ void UNetNet::pack_adjoints(Runtime& rt) {
     adj_ready_ = true;
 }
 
-void UNetNet::backward(Runtime& rt, const ImgView& image, const float* pose, int pose_ld, const UNetGrads& g) {
+void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_posed, const float* coarse_grid, int coarse_size,
+                       const float* pose, int pose_ld, const UNetGrads& g) {
     THA4_REQUIRE(loaded_, "network weights not loaded");
-    THA4_REQUIRE(!upscaler_, "unet backward: only the body morpher (Morpher00) is differentiable; Upscaler02 has no backward");
+    THA4_REQUIRE(upscaler_ || (!g.d_coarse_posed && !g.d_coarse_grid), "unet backward: only the upscaler has coarse inputs");
     const bool want_img = g.d_image != nullptr, want_pose = g.d_pose != nullptr;
-    THA4_REQUIRE(want_img || want_pose, "unet backward: no gradient requested");
+    const bool want_coarse = g.d_coarse_posed || g.d_coarse_grid;
+    const bool want_x0 = want_img || want_coarse;          // gradients that need the first conv's data gradient
+    THA4_REQUIRE(want_x0 || want_pose, "unet backward: no gradient requested");
     if (!adj_ready_) pack_adjoints(rt);
     const int B = image.N, S = S_, NH = 2 * L_;
     cudaStream_t s = rt.stream;
@@ -521,7 +527,7 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* pose, int
     float* outs[5];
     for (int k = 0; k < 5; ++k) outs[k] = P->alloc((size_t)B * kCh[k] * S * S);
     UNetTape tape;
-    forward(rt, image, nullptr, nullptr, 0, pose, pose_ld, outs, &tape);
+    forward(rt, image, coarse_posed, coarse_grid, coarse_size, pose, pose_ld, outs, &tape);
     float* dfilm = P->alloc((size_t)B * film1_total_);
 
     auto gn = [&](const View& x, const NormW& nw, const float* film0, const float* film1, int act, const View& dy, int dy_pool,
@@ -614,15 +620,21 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* pose, int
     for (int i = L_ - 1; i >= 0; --i) {
         const View d_blk = (i == L_ - 1) ? attn_bwd(down_attn_, gk) : gk;
         const View e_in = dhs(2 * i);
-        const View g_in = res_bwd(down_res_[i], 0, d_blk, &e_in, i > 0 || want_img);
+        const View g_in = res_bwd(down_res_[i], 0, d_blk, &e_in, i > 0 || want_x0);
         if (i == 0) { gk = g_in; break; }
         const View e_ds = dhs(2 * i - 1);
         gk = res_bwd(down_ds_[i - 1], 2, g_in, &e_ds, true);
     }
-    if (want_img) {     // first conv: its data gradient joins the warp's image term in the epilogue
+    if (want_x0 && !upscaler_) {     // first conv: its data gradient joins the warp's image term in the epilogue
         View dx0 = fresh(P, B, S, S, 4);
         run_dgrad(rt, adj_first_, gk, dx0, &dimg);
         nhwc_to_nchw(dx0, g.d_image, s);
+    } else if (want_x0) {            // the fused 16-channel first conv, then the prologue's adjoint (channels 14, 15 are padding)
+        View dx0 = fresh(P, B, S, S, 16);
+        run_dgrad(rt, adj_first_, gk, dx0);
+        upscaler_prologue_backward(image, coarse_grid, coarse_size, dx0, want_img ? dimg.p : nullptr, g.d_coarse_posed,
+                                   g.d_coarse_grid, s);
+        if (want_img) nhwc_to_nchw(dimg, g.d_image, s);
     }
     if (want_pose) {    // d(film1) -> FiLM projection (SiLU' at c2) -> cond_embed.2 (SiLU' at c1) -> cond_embed.0
         float* dc2 = P->alloc((size_t)B * 256);

@@ -1,7 +1,7 @@
 """torch.autograd for the three encoder-decoder teacher networks (EyebrowDecomposer00, EyebrowMorphingCombiner00,
-FaceMorpher08) and the body morpher U-Net (Morpher00): their outputs are differentiable w.r.t. image, layers and pose, as the
-reference modules are (eyebrow_decomposer_00.py:46-64, eyebrow_morphing_combiner_00.py:47-72, face_morpher_08.py:158-193,
-morpher_00.py:42-66).  This is what pose fitting on an arbitrary character (expression and body parameters), or training an
+FaceMorpher08) and the two U-Nets (Morpher00, Upscaler02): their outputs are differentiable w.r.t. images, layers and pose, as
+the reference modules are (eyebrow_decomposer_00.py:46-64, eyebrow_morphing_combiner_00.py:47-72, face_morpher_08.py:158-193,
+morpher_00.py:42-66, upscaler_02.py:59-96).  This is what pose fitting on an arbitrary character (expression and body parameters), or training an
 image -> pose regressor with a teacher as a differentiable renderer, needs.
 
 Dispatch: the autograd path runs when grad mode is on and an input (image, layer or pose) requires grad; in every other
@@ -142,6 +142,34 @@ def _morpher_backward(ctx, *grad_outputs):
     return (None, d_image, d_pose) + none
 
 
+class _UpscalerFunction(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, module, rest_image: Tensor, coarse_posed_image: Tensor, coarse_grid_change: Tensor, pose: Tensor, *params: Tensor):
+        outs = module.sync_weights().upscaler(rest_image, coarse_posed_image, coarse_grid_change, pose)
+        ctx.set_materialize_grads(False)
+        ctx.module = module
+        ctx.save_for_backward(rest_image, coarse_posed_image, coarse_grid_change, pose, *params)
+        return _own(outs)
+
+    @staticmethod
+    def backward(ctx, *grad_outputs):
+        refuse_double_backward('Upscaler02')
+        return _upscaler_backward(ctx, *grad_outputs)
+
+
+@once_differentiable
+def _upscaler_backward(ctx, *grad_outputs):
+    rest_image, coarse_posed_image, coarse_grid_change, pose, *params = ctx.saved_tensors
+    none = (None,) * len(params)
+    want = ctx.needs_input_grad[1:5]
+    if not any(want) or all(g is None for g in grad_outputs):
+        return (None, None, None, None, None) + none
+    d = [_empty_like(t) if w else None for t, w in zip((rest_image, coarse_posed_image, coarse_grid_change, pose), want)]
+    ctx.module.sync_weights().upscaler_backward(rest_image, coarse_posed_image, coarse_grid_change, pose, contiguous_grads(grad_outputs),
+                                                d_rest_image=d[0], d_coarse_posed=d[1], d_coarse_grid=d[2], d_pose=d[3])
+    return (None, *d) + none
+
+
 def eyebrow_decomposer(module, image: Tensor) -> List[Tensor]:
     return list(_DecomposerFunction.apply(module, image, *module._params()))
 
@@ -156,3 +184,7 @@ def face_morpher(module, image: Tensor, pose: Tensor) -> List[Tensor]:
 
 def morpher(module, image: Tensor, pose: Tensor) -> List[Tensor]:
     return list(_MorpherFunction.apply(module, image, pose, *module._params()))
+
+
+def upscaler(module, rest_image: Tensor, coarse_posed_image: Tensor, coarse_grid_change: Tensor, pose: Tensor) -> List[Tensor]:
+    return list(_UpscalerFunction.apply(module, rest_image, coarse_posed_image, coarse_grid_change, pose, *module._params()))

@@ -3,7 +3,8 @@
 
 The reference evaluates a memoised Python DAG that dispatches ~1 600 PyTorch ops per frame; here the whole DAG of
 mode_07.py:72-132 (crops, pastes, bilinear resizes and the five networks) is one C call,
-`tha4_teacher_forward(mode=7)`, which returns the same 33 tensors in the same order.
+`tha4_teacher_forward(mode=7)`, which returns the same 33 tensors in the same order.  When grad mode is on and the image or
+the pose requires grad, the five modules are composed instead, each differentiable (all 45 pose parameters can be fitted).
 """
 from enum import Enum
 from typing import Dict, List, Optional
@@ -74,25 +75,76 @@ class FiveStepPoserComputationProtocol(CachedComputationProtocol):
 
     def compute_func(self):
         def func(state: ComputationState) -> List[Tensor]:
-            ctx = state.context
-            image = state.batch[0]
-            # eyebrow cache (mode_07.py:56-68): recompute the decomposer iff there is no cache, the batch size changed
-            # or the image differs anywhere.  The comparison is skipped when the caller passes the very same, unmodified
-            # tensor object; otherwise it is one reduction kernel + the same host sync the reference pays for .item().
-            for net in Network:
-                if net.name in state.modules:
-                    state.modules[net.name].sync_weights()
-            new_batch_0, key_image = self.eyebrow_cache_miss(ctx, image)
-            cached = None if new_batch_0 else self.cached_eyebrow_decomposer_output
-            output = ctx.teacher_forward(self.TEACHER_MODE, image, state.batch[1], self.eyebrow_morphed_image_index, cached)
-            for key, sl in self.SLICES.items():
-                state.outputs[key] = output[sl]
-            state.outputs[Branch.all_outputs.name] = output
-            if new_batch_0:
-                self.eyebrow_cache_store(ctx, image, key_image, output[self.SLICES[Network.eyebrow_decomposer.outputs_key]])
-            return output
+            image, pose = state.batch[0], state.batch[1]
+            if torch.is_grad_enabled() and (image.requires_grad or pose.requires_grad):
+                return self._differentiable(state)
+            return self._single_call(state)
 
         return func
+
+    def _single_call(self, state: ComputationState) -> List[Tensor]:
+        ctx = state.context
+        image = state.batch[0]
+        # eyebrow cache (mode_07.py:56-68): recompute the decomposer iff there is no cache, the batch size changed
+        # or the image differs anywhere.  The comparison is skipped when the caller passes the very same, unmodified
+        # tensor object; otherwise it is one reduction kernel + the same host sync the reference pays for .item().
+        for net in Network:
+            if net.name in state.modules:
+                state.modules[net.name].sync_weights()
+        new_batch_0, key_image = self.eyebrow_cache_miss(ctx, image)
+        cached = None if new_batch_0 else self.cached_eyebrow_decomposer_output
+        output = ctx.teacher_forward(self.TEACHER_MODE, image, state.batch[1], self.eyebrow_morphed_image_index, cached)
+        self._store(state, output)
+        if new_batch_0:
+            self.eyebrow_cache_store(ctx, image, key_image, output[self.SLICES[Network.eyebrow_decomposer.outputs_key]])
+        return output
+
+    def _store(self, state: ComputationState, output: List[Tensor]):
+        for key, sl in self.SLICES.items():
+            state.outputs[key] = output[sl]
+        state.outputs[Branch.all_outputs.name] = output
+
+    def _differentiable(self, state: ComputationState) -> List[Tensor]:
+        """The modules composed as in the reference (mode_07.py:72-132; mode_12.py:66-94 for the face part), each through its
+        autograd.Function, when the image or the pose requires grad.  The eyebrow cache is used only when the image does not
+        require grad: its outputs are then constants."""
+        ctx = state.context
+        image, pose = state.batch[0], state.batch[1]
+        modules = state.modules
+        decomposer = modules[Network.eyebrow_decomposer.name]
+        if image.requires_grad:
+            dec = decomposer(image[:, :, 64:192, 192:320])
+        else:
+            decomposer.sync_weights()
+            miss, key_image = self.eyebrow_cache_miss(ctx, image)
+            if miss:
+                with torch.no_grad():
+                    dec = decomposer(image[:, :, 64:192, 192:320])
+                self.eyebrow_cache_store(ctx, image, key_image, dec)
+            else:
+                dec = self.cached_eyebrow_decomposer_output
+        comb = modules[Network.eyebrow_morphing_combiner.name](dec[3], dec[0], pose[:, :NUM_EYEBROW_PARAMS])
+        face_in = image[:, :, 32:224, 160:352].clone()
+        face_in[:, :, 32:160, 32:160] = comb[self.eyebrow_morphed_image_index]
+        n_face = NUM_EYEBROW_PARAMS + NUM_FACE_PARAMS
+        face = modules[Network.face_morpher.name](face_in, pose[:, NUM_EYEBROW_PARAMS:n_face])
+        output = self._body(state, face[0]) + list(face) + list(comb) + list(dec)
+        self._store(state, output)
+        return output
+
+    def _body(self, state: ComputationState, face_morphed: Tensor) -> List[Tensor]:
+        """upscaler(5) + face_morphed_full + body_morpher(5) of mode_07.py:93-124; the upscaler takes the body morpher's
+        256x256 outputs and upsamples them itself, as the single call does."""
+        image, pose = state.batch[0], state.batch[1]
+        full = image.clone()
+        full[:, :, 32:224, 160:352] = face_morphed
+        # interpolate(size=256, bilinear, align_corners=False) of a 512x512 image is the mean of each 2x2 block; summed in the
+        # order of the library's resize_bilinear, ((a + b) + (c + d)) / 4, it gives the single call's values exactly
+        half = ((full[:, :, 0::2, 0::2] + full[:, :, 0::2, 1::2]) + (full[:, :, 1::2, 0::2] + full[:, :, 1::2, 1::2])) * 0.25
+        rot = pose[:, NUM_EYEBROW_PARAMS + NUM_FACE_PARAMS:]
+        body = state.modules[Network.body_morpher.name](half, rot)
+        up = state.modules[Network.upscaler.name](full, body[Morpher00.INDEX_MERGED], body[Morpher00.INDEX_GRID_CHANGE], rot)
+        return list(up) + [full] + list(body)
 
     def eyebrow_cache_miss(self, ctx, image: Tensor):
         """(True iff the cached decomposer outputs cannot be used for `image`, the tensor the cache is keyed by)."""

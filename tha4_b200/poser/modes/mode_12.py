@@ -41,45 +41,8 @@ class FiveStepPoserComputationProtocol(mode_07.FiveStepPoserComputationProtocol)
         Network.eyebrow_decomposer.outputs_key: slice(16, 22),
     }
 
-    def compute_func(self):
-        single_call = super().compute_func()
-
-        def func(state: ComputationState) -> List[Tensor]:
-            image, pose = state.batch[0], state.batch[1]
-            if torch.is_grad_enabled() and (image.requires_grad or pose.requires_grad):
-                return self._differentiable(state)
-            return single_call(state)          # one tha4_teacher_forward call
-
-        return func
-
-    def _differentiable(self, state: ComputationState) -> List[Tensor]:
-        """The three modules composed as in the reference (mode_12.py:66-94), each through its autograd.Function.  The eyebrow
-        cache is used only when the image does not require grad: its outputs are then constants."""
-        ctx = state.context
-        image, pose = state.batch[0], state.batch[1]
-        modules = state.modules
-        decomposer = modules[Network.eyebrow_decomposer.name]
-        if image.requires_grad:
-            dec = decomposer(image[:, :, 64:192, 192:320])
-        else:
-            decomposer.sync_weights()
-            miss, key_image = self.eyebrow_cache_miss(ctx, image)
-            if miss:
-                with torch.no_grad():
-                    dec = decomposer(image[:, :, 64:192, 192:320])
-                self.eyebrow_cache_store(ctx, image, key_image, dec)
-            else:
-                dec = self.cached_eyebrow_decomposer_output
-        comb = modules[Network.eyebrow_morphing_combiner.name](dec[3], dec[0], pose[:, :mode_07.NUM_EYEBROW_PARAMS])
-        face_in = image[:, :, 32:224, 160:352].clone()
-        face_in[:, :, 32:160, 32:160] = comb[self.eyebrow_morphed_image_index]
-        n_face = mode_07.NUM_EYEBROW_PARAMS + mode_07.NUM_FACE_PARAMS
-        face = modules[Network.face_morpher.name](face_in, pose[:, mode_07.NUM_EYEBROW_PARAMS:n_face])
-        output = list(face) + list(comb) + list(dec)
-        for key, sl in self.SLICES.items():
-            state.outputs[key] = output[sl]
-        state.outputs[Branch.all_outputs.name] = output
-        return output
+    def _body(self, state: ComputationState, face_morphed: Tensor) -> List[Tensor]:
+        return []          # the face-only teacher stops after the face morpher (mode_12.py:88-94)
 
 
 _CLASSES = {
