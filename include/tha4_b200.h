@@ -318,6 +318,34 @@ int tha4_test_siren_level(tha4_ctx* ctx, int path, int mode, int n_tensors, cons
 /* y[i] = sin(x[i]) as the student kernels evaluate it: which 1 = the wgmma kernels' polynomial, 0 = the mma.sync kernels'
  * range reduction + __sinf */
 int tha4_test_sine(tha4_ctx* ctx, int which, const float* x, int64_t n, float* y, void* stream);
+/* ---- stages of the student training step (distill.cu), each through the host function the step calls ----
+ * Tensors are device fp32, row-major [pixels][channels] (NHWC) as the step holds them. */
+/* y [N*R*R][Cout] = x [N*R*R][Cin] W^T (+ bias_padded [Cout], may be NULL) on the wgmma 1x1 conv with W [nreal][kreal] packed
+ * (TF32-rounded) by the step's packing kernel; transpose = 1: y = x W (Cin >= nreal, Cout >= kreal).  Channels past the real
+ * ones are written as 0. */
+int tha4_test_dense_gemm(tha4_ctx* ctx, const float* W, int nreal, int kreal, int transpose, const float* bias_padded, const float* x,
+                         int Cin, float* y, int Cout, int N, int R, void* stream);
+/* ACCUMULATES dW [nreal][kreal] += dz^T x and db [nreal] += column sums of dz over P pixels: dz [P][Nc], x [P][Kc] */
+int tha4_test_dense_wgrad(tha4_ctx* ctx, const float* dz, int Nc, const float* x, int Kc, int64_t P, int nreal, int kreal, float* dW,
+                          float* db, void* stream);
+/* dir 0: the level input out [N][R][R][C] = [bilinear x2 of prev [N][R/2][R/2] (first Cprev of prev_ld channels) | x | y |
+ * pose (npose of pose_ld per sample) | 0].  dir 1: its adjoint for the upsampled channels, out = dprev [N][R/2][R/2] (pixel
+ * stride prev_ld; only channels 0..Cprev-1 are written) from up [N][R][R] (pixel stride up_ld). */
+int tha4_test_level_input(tha4_ctx* ctx, int dir, const float* prev, int Cprev, int prev_ld, const float* pose, int pose_ld, int npose,
+                          int R, int N, int C, const float* up, int up_ld, float* out, void* stream);
+/* dir 0: out = sin(30 z); dir 1: out = da * 30 cos(30 z) (da is not modified).  n % 4 == 0. */
+int tha4_test_distill_sine(tha4_ctx* ctx, int dir, const float* z, const float* da, int64_t n, float* out, void* stream);
+/* d(pose) [N][npose] (overwritten) from 1..3 levels: level l has the first layer's dz [N][hw[l]][C[l]] and weight W[l]
+ * [nreal[l]][kreal[l]] whose pose columns start at col0[l]. */
+int tha4_test_pose_grad(tha4_ctx* ctx, int n_levels, const float* const* dz, const int* C, const int* hw, const float* const* W,
+                        const int* nreal, const int* kreal, const int* col0, int N, int npose, float* dpose, void* stream);
+/* Loss / gradient tails.  kind 0 (body loss): out = out7 [N*512*512][8], image [N,4,512,512], t0 / t1 / t2 = T0 posed / T2
+ * warped [N,4,512,512], T3 grid change [N,2,512,512], loss_w[4]; loss_sums[4] (device doubles, overwritten) = the sums of |a-b|
+ * of the four terms.  kind 1 (body upstream gradients): grads[5] = d blended, d alpha, d colour, d warped, d grid_change (NCHW,
+ * entries or grads itself may be NULL = zero).  kind 2 (face loss): out = out4 [N*128*128][4], t0 = target, t1 = mask
+ * [N,4,128,128], loss_w[2], loss_sums[0..1] (overwritten).  d_out: the gradient in the layout of out. */
+int tha4_test_distill_tail(tha4_ctx* ctx, int kind, const float* out, const float* image, int N, const float* t0, const float* t1,
+                           const float* t2, const float* const* grads, const float* loss_w, float* d_out, double* loss_sums, void* stream);
 /* Host only, launches nothing: checks a wgmma student plan (per layer: padded K, padded N, slice width, sine 1 / head 0,
  * first-layer terms 0 / 1) for level `mode` with resolution R, elementwise first-layer width e_npad (modes 0 / 3), previous
  * level channels prev_c (modes 1 / 2) and output channels out_c.  Returns 0 if the kernel can run it, else

@@ -34,6 +34,8 @@ EXPORTED_SYMBOLS = [
     'tha4_test_group_norm_backward', 'tha4_test_attention_backward',
     'tha4_base_grid', 'tha4_test_conv', 'tha4_test_conv_norm', 'tha4_test_conv_norm_ex', 'tha4_test_norm', 'tha4_test_tail', 'tha4_test_attention', 'tha4_test_linear',
     'tha4_test_siren_level', 'tha4_test_sine', 'tha4_test_siren_plan_check',
+    'tha4_test_dense_gemm', 'tha4_test_dense_wgrad', 'tha4_test_level_input', 'tha4_test_distill_sine', 'tha4_test_pose_grad',
+    'tha4_test_distill_tail',
 ]
 
 _lib = None
@@ -64,6 +66,13 @@ def load_library() -> ctypes.CDLL:
                                    ctypes.c_void_p]
     lib.tha4_images_differ.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64,
                                        ctypes.POINTER(ctypes.c_int), ctypes.c_void_p]
+    P, I, I64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64
+    lib.tha4_test_dense_gemm.argtypes = [P, P, I, I, I, P, P, I, P, I, I, I, P]
+    lib.tha4_test_dense_wgrad.argtypes = [P, P, I, P, I, I64, I, I, P, P, P]
+    lib.tha4_test_level_input.argtypes = [P, I, P, I, I, P, I, I, I, I, I, P, I, P, P]
+    lib.tha4_test_distill_sine.argtypes = [P, I, P, P, I64, P, P]
+    lib.tha4_test_pose_grad.argtypes = [P, I, P, P, P, P, P, P, P, I, I, P, P]
+    lib.tha4_test_distill_tail.argtypes = [P, I, P, P, I, P, P, P, P, P, P, P, P]
     _lib = lib
     return lib
 

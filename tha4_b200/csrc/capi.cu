@@ -1152,6 +1152,53 @@ int tha4_test_sine(tha4_ctx* ctx, int which, const float* x, int64_t n, float* y
     });
 }
 
+int tha4_test_dense_gemm(tha4_ctx* ctx, const float* W, int nreal, int kreal, int transpose, const float* bias_padded, const float* x,
+                         int Cin, float* y, int Cout, int N, int R, void* stream) {
+    return guarded(ctx, [&] {
+        begin_pass(ctx, (cudaStream_t)stream);
+        Runtime rt = make_rt(ctx, stream);
+        distill_test_dense_gemm(rt, W, nreal, kreal, transpose != 0, bias_padded, x, Cin, y, Cout, N, R);
+    });
+}
+
+int tha4_test_dense_wgrad(tha4_ctx* ctx, const float* dz, int Nc, const float* x, int Kc, int64_t P, int nreal, int kreal, float* dW,
+                          float* db, void* stream) {
+    return guarded(ctx, [&] { distill_test_dense_wgrad((cudaStream_t)stream, dz, Nc, x, Kc, (long)P, nreal, kreal, dW, db); });
+}
+
+int tha4_test_level_input(tha4_ctx* ctx, int dir, const float* prev, int Cprev, int prev_ld, const float* pose, int pose_ld, int npose,
+                          int R, int N, int C, const float* up, int up_ld, float* out, void* stream) {
+    return guarded(ctx, [&] {
+        THA4_REQUIRE(dir == 0 || dir == 1, "test_level_input: dir 0 (level input) or 1 (upsample adjoint)");
+        distill_test_level_input((cudaStream_t)stream, dir, prev, Cprev, prev_ld, pose, pose_ld, npose, R, N, C, up, up_ld, out);
+    });
+}
+
+int tha4_test_distill_sine(tha4_ctx* ctx, int dir, const float* z, const float* da, int64_t n, float* out, void* stream) {
+    return guarded(ctx, [&] {
+        THA4_REQUIRE(dir == 0 || dir == 1, "test_distill_sine: dir 0 (forward) or 1 (backward)");
+        distill_test_sine((cudaStream_t)stream, dir, z, da, (long)n, out);
+    });
+}
+
+int tha4_test_pose_grad(tha4_ctx* ctx, int n_levels, const float* const* dz, const int* C, const int* hw, const float* const* W,
+                        const int* nreal, const int* kreal, const int* col0, int N, int npose, float* dpose, void* stream) {
+    return guarded(ctx, [&] {
+        begin_pass(ctx, (cudaStream_t)stream);
+        Runtime rt = make_rt(ctx, stream);
+        distill_test_pose_grad(rt, n_levels, dz, C, hw, W, nreal, kreal, col0, N, npose, dpose);
+    });
+}
+
+int tha4_test_distill_tail(tha4_ctx* ctx, int kind, const float* out, const float* image, int N, const float* t0, const float* t1,
+                           const float* t2, const float* const* grads, const float* loss_w, float* d_out, double* loss_sums, void* stream) {
+    return guarded(ctx, [&] {
+        const float* g[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+        if (grads) for (int i = 0; i < 5; ++i) g[i] = grads[i];
+        distill_test_tail((cudaStream_t)stream, kind, out, image, N, t0, t1, t2, g, loss_w, d_out, loss_sums);
+    });
+}
+
 int tha4_test_siren_plan_check(int mode, int n_layers, const int* kpad, const int* npad, const int* nb, const int* sine,
                                const int* first, int R, int e_npad, int prev_c, int out_c, char* msg, int msg_len) {
     std::string err;

@@ -37,7 +37,9 @@ __global__ void __launch_bounds__(256) level_input_kernel(const float* __restric
             const float* pp = prev + (long)n * Rh * Rh * prev_ld + c;
             const float a = pp[((long)ty.i0 * Rh + tx.i0) * prev_ld], b = pp[((long)ty.i0 * Rh + tx.i1) * prev_ld];
             const float cc = pp[((long)ty.i1 * Rh + tx.i0) * prev_ld], d = pp[((long)ty.i1 * Rh + tx.i1) * prev_ld];
-            v = ty.l0 * (tx.l0 * a + tx.l1 * b) + ty.l1 * (tx.l0 * cc + tx.l1 * d);
+            // explicit roundings (no FMA contraction): bit-identical to interpolate(bilinear) as oracle/gridsample_ref.c states it
+            v = __fadd_rn(__fmul_rn(ty.l0, __fadd_rn(__fmul_rn(tx.l0, a), __fmul_rn(tx.l1, b))),
+                          __fmul_rn(ty.l1, __fadd_rn(__fmul_rn(tx.l0, cc), __fmul_rn(tx.l1, d))));
         } else if (c == Cprev) v = base[x];
         else if (c == Cprev + 1) v = base[y];
         else if (c < Cprev + 2 + npose) v = pose[(long)n * pose_ld + (c - Cprev - 2)];
@@ -466,6 +468,49 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
 
 inline int grid_for(long total, int cap = 148 * 8) { return (int)std::max<long>(1, std::min<long>((total + 255) / 256, cap)); }
 
+// Host launchers of the small kernels: the training step and the kernel-level test entries both go through these, so the
+// tests run the production launch configuration.
+void level_input(cudaStream_t s, const float* prev, int Cprev, int prev_ld, const float* pose, int pose_ld, int npose, int R, int N,
+                 int C, float* out) {
+    level_input_kernel<<<grid_for((long)N * R * R * C), 256, 0, s>>>(prev, Cprev, prev_ld, pose, pose_ld, base_grid_table(R), R, N, C, npose,
+                                                                      out);
+    THA4_LAUNCH_CHECK();
+}
+// writes channels 0 .. Cprev-1 of dprev [N][R/2][R/2] (pixel stride prev_ld) and nothing else
+void upsample_backward(cudaStream_t s, const float* dup, int up_ld, int Cprev, int R, int N, float* dprev, int prev_ld) {
+    upsample_backward_kernel<<<grid_for((long)N * (R / 2) * (R / 2) * Cprev), 256, 0, s>>>(dup, up_ld, Cprev, R, N, dprev, prev_ld);
+    THA4_LAUNCH_CHECK();
+}
+void sine_forward(cudaStream_t s, const float* z, float* a, long n4) {
+    sine_forward_kernel<<<grid_for(n4), 256, 0, s>>>(z, a, n4);
+    THA4_LAUNCH_CHECK();
+}
+void sine_backward(cudaStream_t s, const float* z, float* da, long n4) {
+    sine_backward_kernel<<<grid_for(n4), 256, 0, s>>>(z, da, n4);
+    THA4_LAUNCH_CHECK();
+}
+// body loss tail at R = 512: loss_w are the weights of the four terms, normalised here by their element counts
+void body_loss_tail(cudaStream_t s, const float* out7, const ImgView& image, const float* T0, const float* T2, const float* T3,
+                    const float loss_w[4], float* d_out7, double* loss_acc) {
+    const int N = image.N;
+    const double nb = (double)N * 4 * 512 * 512, ng = (double)N * 2 * 512 * 512;
+    const float4 wn = make_float4((float)(loss_w[0] / nb), (float)(loss_w[1] / nb), (float)(loss_w[2] / ng), (float)(loss_w[3] / nb));
+    train_tail_kernel<<<grid_for((long)N * 512 * 512), 256, 0, s>>>(out7, image, T0, T2, T3, base_grid_table(512), 512, wn, d_out7, loss_acc);
+    THA4_LAUNCH_CHECK();
+}
+void body_grad_tail(cudaStream_t s, const float* out7, const ImgView& image, const float* const g[5], float* d_out7) {
+    grad_tail_kernel<<<grid_for((long)image.N * 512 * 512), 256, 0, s>>>(out7, image, g[0], g[1], g[2], g[3], g[4], base_grid_table(512), 512,
+                                                                         d_out7);
+    THA4_LAUNCH_CHECK();
+}
+void face_loss_tail(cudaStream_t s, const float* out4, const float* target, const float* mask, int R, int N, const float loss_w[2],
+                    float* d_out, double* loss_acc) {
+    const double nel = (double)N * 4 * R * R;
+    face_tail_kernel<<<grid_for((long)N * R * R), 256, 0, s>>>(out4, target, mask, R, N, make_float2((float)(loss_w[0] / nel), (float)(loss_w[1] / nel)),
+                                                              d_out, loss_acc);
+    THA4_LAUNCH_CHECK();
+}
+
 struct Dense {             // one 1x1 layer of the student in the flat parameter buffer
     long w_off, b_off;     // offsets (floats)
     int nreal, kreal;      // reference [Cout][Cin]
@@ -495,15 +540,18 @@ void dense_gemm(Runtime& rt, const float* W, int nreal, int kreal, bool transpos
     conv_forward(cw, a, rt.stream);
 }
 
-// weight and bias gradients of layer d: dW += dz^T x, db += column sums of dz
-void dense_wgrad(cudaStream_t s, const View& dz, const View& x, const Dense& d, float* grads) {
+// weight and bias gradients of a layer W [nreal][kreal]: dW += dz^T x, db += column sums of dz
+void dense_wgrad(cudaStream_t s, const View& dz, const View& x, int nreal, int kreal, float* dW, float* db) {
     const long Pn = (long)dz.N * dz.H * dz.W;
     const int psplit = (int)std::max<long>(1, std::min<long>(64, Pn / 4096));
     dim3 grid(ceil_div(dz.C, 64), ceil_div(x.C, 64), psplit);
-    wgrad_kernel<<<grid, 128, 0, s>>>(dz.p, dz.C, x.p, x.C, Pn, d.nreal, d.kreal, grads + d.w_off);
+    wgrad_kernel<<<grid, 128, 0, s>>>(dz.p, dz.C, x.p, x.C, Pn, nreal, kreal, dW);
     THA4_LAUNCH_CHECK();
-    colsum_kernel<<<std::min<long>(148, std::max<long>(1, Pn / 512)), 256, 0, s>>>(dz.p, Pn, dz.C, d.nreal, grads + d.b_off);
+    colsum_kernel<<<std::min<long>(148, std::max<long>(1, Pn / 512)), 256, 0, s>>>(dz.p, Pn, dz.C, nreal, db);
     THA4_LAUNCH_CHECK();
+}
+void dense_wgrad(cudaStream_t s, const View& dz, const View& x, const Dense& d, float* grads) {
+    dense_wgrad(s, dz, x, d.nreal, d.kreal, grads + d.w_off, grads + d.b_off);
 }
 
 // d(pose) stage 1 for one level: chunk sums of the first layer's dz (layer d; the pose columns start at col0)
@@ -565,19 +613,14 @@ void body_forward_store(Runtime& rt, const Dense (&L)[10], const float* pose, in
         const int R = BODY_RS[l];
         A.xin[l] = mk(P, N, R, L[3 * l].kpad);
         const View* prev = l > 0 ? &A.a[l - 1][2] : nullptr;
-        level_input_kernel<<<grid_for((long)N * R * R * A.xin[l].C), 256, 0, s>>>(prev ? prev->p : nullptr, BODY_CPREV[l], prev ? prev->ld : 0,
-                                                                                pose, pose_ld, base_grid_table(R), R, N, A.xin[l].C, 45,
-                                                                                A.xin[l].p);
-        THA4_LAUNCH_CHECK();
+        level_input(s, prev ? prev->p : nullptr, BODY_CPREV[l], prev ? prev->ld : 0, pose, pose_ld, 45, R, N, A.xin[l].C, A.xin[l].p);
         for (int j = 0; j < 3; ++j) {
             const Dense& d = L[3 * l + j];
             rt.scratch->reset();
             A.z[l][j] = mk(P, N, R, d.npad);
             A.a[l][j] = mk(P, N, R, d.npad);
             dense_gemm(rt, params + d.w_off, d.nreal, d.kreal, false, bias_pad[3 * l + j], j == 0 ? A.xin[l] : A.a[l][j - 1], A.z[l][j]);
-            const long n4 = (long)N * R * R * d.npad / 4;
-            sine_forward_kernel<<<grid_for(n4), 256, 0, s>>>(A.z[l][j].p, A.a[l][j].p, n4);
-            THA4_LAUNCH_CHECK();
+            sine_forward(s, A.z[l][j].p, A.a[l][j].p, (long)N * R * R * d.npad / 4);
         }
     }
     rt.scratch->reset();
@@ -601,9 +644,7 @@ void body_backward(Runtime& rt, const Dense (&L)[10], const BodyActs& A, const V
         const int R = BODY_RS[l];
         for (int j = 2; j >= 0; --j) {
             const Dense& d = L[3 * l + j];
-            const long n4 = (long)N * R * R * d.npad / 4;
-            sine_backward_kernel<<<grid_for(n4), 256, 0, s>>>(A.z[l][j].p, da.p, n4);       // da -> dz (in place)
-            THA4_LAUNCH_CHECK();
+            sine_backward(s, A.z[l][j].p, da.p, (long)N * R * R * d.npad / 4);       // da -> dz (in place)
             const View& x = (j == 0) ? A.xin[l] : A.a[l][j - 1];
             if (grads) dense_wgrad(s, da, x, d, grads);
             if (j == 0 && pose_grad) pose_colsum(rt, da, d, params, BODY_CPREV[l] + 2, *pose_grad);
@@ -615,9 +656,7 @@ void body_backward(Runtime& rt, const Dense (&L)[10], const BodyActs& A, const V
             // level boundary: the first Cprev channels of dx are the gradient of the upsampled previous level
             View dprev = mk(P, N, R / 2, L[3 * l - 1].npad);
             THA4_CUDA_CHECK(cudaMemsetAsync(dprev.p, 0, dprev.pixels() * dprev.C * sizeof(float), s));
-            upsample_backward_kernel<<<grid_for((long)N * (R / 2) * (R / 2) * BODY_CPREV[l]), 256, 0, s>>>(dx.p, dx.ld, BODY_CPREV[l], R, N,
-                                                                                                        dprev.p, dprev.ld);
-            THA4_LAUNCH_CHECK();
+            upsample_backward(s, dx.p, dx.ld, BODY_CPREV[l], R, N, dprev.p, dprev.ld);
             da = dprev;
         }
     }
@@ -640,10 +679,7 @@ void siren_body_train_step(Runtime& rt, const ImgView& image, const float* pose,
     body_forward_store(rt, L, pose, pose_ld, N, params, A);
     // losses + d(out7)
     View d_out = mk(rt.persist, N, 512, 8);
-    const double nb = (double)N * 4 * 512 * 512, ng = (double)N * 2 * 512 * 512;
-    const float4 wn = make_float4((float)(loss_w[0] / nb), (float)(loss_w[1] / nb), (float)(loss_w[2] / ng), (float)(loss_w[3] / nb));
-    train_tail_kernel<<<grid_for((long)N * 512 * 512), 256, 0, s>>>(A.out7.p, image, T0, T2, T3, base_grid_table(512), 512, wn, d_out.p, loss_acc);
-    THA4_LAUNCH_CHECK();
+    body_loss_tail(s, A.out7.p, image, T0, T2, T3, loss_w, d_out.p, loss_acc);
     body_backward(rt, L, A, d_out, params, grads);
 }
 
@@ -659,9 +695,7 @@ void siren_body_backward(Runtime& rt, const ImgView& image, const float* pose, i
     BodyActs A;
     body_forward_store(rt, L, pose, pose_ld, N, params, A);
     View d_out = mk(rt.persist, N, 512, 8);
-    grad_tail_kernel<<<grid_for((long)N * 512 * 512), 256, 0, s>>>(A.out7.p, image, g[0], g[1], g[2], g[3], g[4], base_grid_table(512), 512,
-                                                                   d_out.p);
-    THA4_LAUNCH_CHECK();
+    body_grad_tail(s, A.out7.p, image, g, d_out.p);
     PoseGrad pg;
     pg.npose = 45;
     body_backward(rt, L, A, d_out, params, grads, d_pose ? &pg : nullptr);
@@ -716,17 +750,14 @@ void face_forward_store(Runtime& rt, const Dense (&L)[9], const float* pose, int
         THA4_LAUNCH_CHECK();
     }
     A.xin = mk(P, N, R, L[0].kpad);
-    level_input_kernel<<<grid_for((long)N * R * R * A.xin.C), 256, 0, s>>>(nullptr, 0, 0, pose, pose_ld, base_grid_table(R), R, N, A.xin.C, 39,
-                                                                          A.xin.p);
-    THA4_LAUNCH_CHECK();
+    level_input(s, nullptr, 0, 0, pose, pose_ld, 39, R, N, A.xin.C, A.xin.p);
     const long n4 = (long)N * R * R * 128 / 4;
     for (int j = 0; j < 8; ++j) {
         rt.scratch->reset();
         A.z[j] = mk(P, N, R, 128);
         A.a[j] = mk(P, N, R, 128);
         dense_gemm(rt, params + L[j].w_off, L[j].nreal, L[j].kreal, false, bias_pad[j], j == 0 ? A.xin : A.a[j - 1], A.z[j]);
-        sine_forward_kernel<<<grid_for(n4), 256, 0, s>>>(A.z[j].p, A.a[j].p, n4);
-        THA4_LAUNCH_CHECK();
+        sine_forward(s, A.z[j].p, A.a[j].p, n4);
     }
     rt.scratch->reset();
     A.out4 = mk(P, N, R, 4);
@@ -747,8 +778,7 @@ void face_backward(Runtime& rt, const Dense (&L)[9], const FaceActs& A, const Vi
     rt.scratch->reset();
     dense_gemm(rt, params + L[8].w_off, 4, 128, true, nullptr, d_out, da);       // d a7 = d_out W8
     for (int j = 7; j >= 0; --j) {
-        sine_backward_kernel<<<grid_for(n4), 256, 0, s>>>(A.z[j].p, da.p, n4);       // da -> dz (in place)
-        THA4_LAUNCH_CHECK();
+        sine_backward(s, A.z[j].p, da.p, n4);       // da -> dz (in place)
         if (grads) dense_wgrad(s, da, j == 0 ? A.xin : A.a[j - 1], L[j], grads);
         if (j == 0 && pose_grad) pose_colsum(rt, da, L[0], params, 2, *pose_grad);
         if (j == 0) break;
@@ -778,10 +808,7 @@ void siren_face_train_step(Runtime& rt, const float* pose, int pose_ld, int N, c
     face_forward_store(rt, L, pose, pose_ld, N, params, A);
     // losses + d(out4)
     View d_out = mk(rt.persist, N, R, 4);
-    const double nel = (double)N * 4 * R * R;
-    face_tail_kernel<<<grid_for((long)N * R * R), 256, 0, s>>>(A.out4.p, target, mask, R, N,
-                                                              make_float2((float)(loss_w[0] / nel), (float)(loss_w[1] / nel)), d_out.p, loss_acc);
-    THA4_LAUNCH_CHECK();
+    face_loss_tail(s, A.out4.p, target, mask, R, N, loss_w, d_out.p, loss_acc);
     face_backward(rt, L, A, d_out, params, grads);
 }
 
@@ -802,6 +829,75 @@ void siren_face_backward(Runtime& rt, const float* pose, int pose_ld, int N, con
     pg.npose = 39;
     face_backward(rt, L, A, d_out, params, grads, d_pose ? &pg : nullptr);
     if (d_pose) pose_project(s, pg, N, d_pose);
+}
+
+// ---------------------------------------------------------------------------------------------- kernel-level test entries
+// Each runs one stage of the training step through the host function the step itself calls (same grids, psplit,
+// POSE_CHUNK and weight packing).  Tensors are fp32 row-major [pixels][channels] as the step holds them.
+static View flat_view(const float* p, int N, int H, int W, int C) {
+    View v; v.N = N; v.H = H; v.W = W; v.C = C; v.ld = C; v.p = const_cast<float*>(p);
+    return v;
+}
+
+void distill_test_dense_gemm(Runtime& rt, const float* W, int nreal, int kreal, bool transpose, const float* bias_padded, const float* x,
+                             int Cin, float* y, int Cout, int N, int R) {
+    THA4_REQUIRE(Cin % 4 == 0 && Cout % 4 == 0, "test_dense_gemm: channel counts must be multiples of 4");
+    THA4_REQUIRE(transpose ? (Cout >= kreal && Cin >= nreal) : (Cout >= nreal && Cin >= kreal), "test_dense_gemm: padded widths too small");
+    rt.scratch->reset();
+    dense_gemm(rt, W, nreal, kreal, transpose, bias_padded, flat_view(x, N, R, R, Cin), flat_view(y, N, R, R, Cout));
+}
+
+void distill_test_dense_wgrad(cudaStream_t s, const float* dz, int Nc, const float* x, int Kc, long P, int nreal, int kreal, float* dW,
+                              float* db) {
+    THA4_REQUIRE(Nc % 4 == 0 && Kc % 4 == 0 && Nc <= 1024 && nreal <= Nc && kreal <= Kc && P >= 1 && P <= (1L << 30),
+                 "test_dense_wgrad: shapes");
+    dense_wgrad(s, flat_view(dz, 1, 1, (int)P, Nc), flat_view(x, 1, 1, (int)P, Kc), nreal, kreal, dW, db);
+}
+
+void distill_test_level_input(cudaStream_t s, int dir, const float* prev, int Cprev, int prev_ld, const float* pose, int pose_ld, int npose,
+                              int R, int N, int C, const float* up, int up_ld, float* out) {
+    THA4_REQUIRE(R % 2 == 0 && Cprev >= 0 && (Cprev == 0 || prev_ld >= Cprev), "test_level_input: shapes");
+    if (dir == 0) {
+        THA4_REQUIRE(Cprev + 2 + npose <= C && pose_ld >= npose && (Cprev == 0 || prev), "test_level_input: channels");
+        level_input(s, prev, Cprev, prev_ld, pose, pose_ld, npose, R, N, C, out);
+    } else {
+        THA4_REQUIRE(up && up_ld >= Cprev, "test_level_input: upsampled gradient");
+        upsample_backward(s, up, up_ld, Cprev, R, N, out, prev_ld);
+    }
+}
+
+void distill_test_sine(cudaStream_t s, int dir, const float* z, const float* da, long n, float* out) {
+    THA4_REQUIRE(n % 4 == 0, "test_distill_sine: n must be a multiple of 4");
+    if (dir == 0) {
+        sine_forward(s, z, out, n / 4);
+    } else {                // in place, as the step runs it
+        THA4_CUDA_CHECK(cudaMemcpyAsync(out, da, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
+        sine_backward(s, z, out, n / 4);
+    }
+}
+
+void distill_test_pose_grad(Runtime& rt, int nl, const float* const* dz, const int* C, const int* hw, const float* const* W,
+                            const int* nreal, const int* kreal, const int* col0, int N, int npose, float* dpose) {
+    THA4_REQUIRE(nl >= 1 && nl <= 3 && npose >= 1 && npose <= POSE_PROJECT_THREADS, "test_pose_grad: 1..3 levels");
+    PoseGrad pg;
+    pg.npose = npose;
+    for (int l = 0; l < nl; ++l) {
+        THA4_REQUIRE(col0[l] + npose <= kreal[l] && nreal[l] <= C[l], "test_pose_grad: level columns");
+        Dense d;
+        d.w_off = 0; d.b_off = 0; d.nreal = nreal[l]; d.kreal = kreal[l]; d.npad = C[l]; d.kpad = 0;
+        pose_colsum(rt, flat_view(dz[l], N, 1, hw[l], C[l]), d, W[l], col0[l], pg);
+    }
+    pose_project(rt.stream, pg, N, dpose);
+}
+
+void distill_test_tail(cudaStream_t s, int kind, const float* out, const float* image, int N, const float* t0, const float* t1, const float* t2,
+                       const float* const g[5], const float* loss_w, float* d_out, double* loss_acc) {
+    THA4_REQUIRE(kind >= 0 && kind <= 2, "test_distill_tail: kind 0..2");
+    THA4_REQUIRE(kind == 1 || (loss_w && loss_acc), "test_distill_tail: loss weights and sums");
+    if (kind != 1) THA4_CUDA_CHECK(cudaMemsetAsync(loss_acc, 0, 4 * sizeof(double), s));
+    if (kind == 0) body_loss_tail(s, out, make_img(image, N, 4, 512, 512), t0, t1, t2, loss_w, d_out, loss_acc);
+    else if (kind == 1) body_grad_tail(s, out, make_img(image, N, 4, 512, 512), g, d_out);
+    else face_loss_tail(s, out, t0, t1, FACE_R, N, loss_w, d_out, loss_acc);
 }
 
 void adam_step(float* params, const float* grads, float* m, float* v, long n, float lr, float beta1, float beta2, float eps,

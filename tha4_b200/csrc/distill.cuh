@@ -47,4 +47,18 @@ void siren_body_image_grad(Runtime& rt, const float* grid_change, const float* a
 void adam_step(float* params, const float* grads, float* m, float* v, long n, float lr, float beta1, float beta2, float eps,
                int step, float grad_scale, cudaStream_t s);
 
+// Kernel-level test entries (tha4_test_dense_gemm ... tha4_test_distill_tail in include/tha4_b200.h): each runs one stage
+// of the training step through the host function the step calls.
+void distill_test_dense_gemm(Runtime& rt, const float* W, int nreal, int kreal, bool transpose, const float* bias_padded, const float* x,
+                             int Cin, float* y, int Cout, int N, int R);
+void distill_test_dense_wgrad(cudaStream_t s, const float* dz, int Nc, const float* x, int Kc, long P, int nreal, int kreal, float* dW,
+                              float* db);
+void distill_test_level_input(cudaStream_t s, int dir, const float* prev, int Cprev, int prev_ld, const float* pose, int pose_ld, int npose,
+                              int R, int N, int C, const float* up, int up_ld, float* out);
+void distill_test_sine(cudaStream_t s, int dir, const float* z, const float* da, long n, float* out);
+void distill_test_pose_grad(Runtime& rt, int nl, const float* const* dz, const int* C, const int* hw, const float* const* W,
+                            const int* nreal, const int* kreal, const int* col0, int N, int npose, float* dpose);
+void distill_test_tail(cudaStream_t s, int kind, const float* out, const float* image, int N, const float* t0, const float* t1, const float* t2,
+                       const float* const g[5], const float* loss_w, float* d_out, double* loss_acc);
+
 }  // namespace tha4
