@@ -155,6 +155,30 @@ int tha4_student_forward(tha4_ctx* ctx, const float* image, const float* pose, i
  * ("fp16 I/O + fp32 accumulate", BASELINE configs[2]: image [B,4,512,512] __half in, __half planes out; the pose stays
  * fp32).  The arithmetic is the same: fp16 operands, fp32 accumulation, results rounded once on the store. */
 int tha4_student_forward_io(tha4_ctx* ctx, const void* image, const float* pose, int B, void* const* outputs, int io_dtype, void* stream);
+/* ---- character bank: mode 14 for batches that mix characters ----
+ * The reference deploys a student as a character model: one image plus one pair of student weight files
+ * (src/tha4/charmodel/character_model.py:12-69), one poser per character.  A bank holds up to `capacity` character models
+ * in one context, packed as tha4_load_net packs the two students but with the character as the outermost dimension of
+ * every buffer, and tha4_bank_forward poses a batch in which every frame names its character: the wgmma student kernels
+ * take a tile's weights, biases and image from the slot of the tile's frame.  A context has at most one bank;
+ * tha4_bank_create replaces it, tha4_bank_destroy (and tha4_ctx_destroy) frees it. capacity: 1..4096; a character costs
+ * about 0.9 MB of packed weights and 4 MB of image. */
+int tha4_bank_create(tha4_ctx* ctx, int capacity);
+int tha4_bank_destroy(tha4_ctx* ctx);
+/* Fills (or replaces) slot 0 <= slot < capacity with one character: the state_dicts of SirenFaceMorpher00 and SirenMorpher03,
+ * each described as for tha4_load_net, and its image [4,512,512] fp32 on the device (copied).  Other slots are not
+ * touched.  Synchronises the device.  If the call fails the slot is left empty. */
+int tha4_bank_set_character(tha4_ctx* ctx, int slot, int n_face, const char* const* face_keys, const void* const* face_ptrs,
+                            const int64_t* face_shapes, const int* face_ndims, int n_body, const char* const* body_keys,
+                            const void* const* body_ptrs, const int64_t* body_shapes, const int* body_ndims, const float* image,
+                            void* stream);
+/* tha4_student_forward_io for B frames of possibly different characters: frame n is the character in slot char_ids[n] at
+ * pose[n] (pose [B,45] device fp32), its image is the slot's.  char_ids is a HOST array [B]: every id is checked
+ * (0 <= id < capacity, slot filled) before anything is launched, then the library copies the array to the device itself.
+ * outputs: the six of tha4_student_forward, fp32 (io_dtype 0) or fp16 (io_dtype 1; the slot's image is then rounded to
+ * fp16 first, as the fp16 image of tha4_student_forward_io is).  A frame's outputs are bit-identical to what a context
+ * holding that character alone returns for it.  wgmma kernels only: with option "siren_tc" = 0 the call is an error. */
+int tha4_bank_forward(tha4_ctx* ctx, const int* char_ids, const float* pose, int B, void* const* outputs, int io_dtype, void* stream);
 /* ---- distillation inner loop of the body student (replaces the autograd part of
  * SirenMorpherTrainingProtocol03.run_training_iteration, src/tha4/nn/siren/morpher/siren_morpher_protocols_03.py:178-214) ---- */
 /* number of fp32 parameters of SirenMorpher03 in state_dict order (331 567) */

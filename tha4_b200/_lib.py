@@ -24,7 +24,8 @@ EXPORTED_SYMBOLS = [
     'tha4_ctx_create', 'tha4_ctx_destroy', 'tha4_last_error', 'tha4_set_option', 'tha4_get_counter', 'tha4_load_net',
     'tha4_eyebrow_decomposer_forward', 'tha4_eyebrow_morphing_combiner_forward', 'tha4_face_morpher_forward',
     'tha4_morpher_forward', 'tha4_upscaler_forward', 'tha4_siren_face_morpher_forward', 'tha4_siren_morpher_forward',
-    'tha4_teacher_forward', 'tha4_student_forward', 'tha4_student_forward_io', 'tha4_siren_morpher_param_count', 'tha4_siren_morpher_train_step',
+    'tha4_teacher_forward', 'tha4_student_forward', 'tha4_student_forward_io',
+    'tha4_bank_create', 'tha4_bank_destroy', 'tha4_bank_set_character', 'tha4_bank_forward', 'tha4_siren_morpher_param_count', 'tha4_siren_morpher_train_step',
     'tha4_siren_face_morpher_param_count', 'tha4_siren_face_morpher_train_step',
     'tha4_siren_morpher_backward', 'tha4_siren_face_morpher_backward',
     'tha4_adam_step', 'tha4_images_differ', 'tha4_frame_to_srgb8', 'tha4_rgba8_to_poser_image', 'tha4_grid_sample', 'tha4_resize_bilinear',
@@ -141,8 +142,9 @@ class Context:
     def counter(self, name: str) -> int:
         return int(self.lib.tha4_get_counter(self.handle, name.encode()))
 
-    def load_net(self, net: str, state_dict: Dict[str, Tensor]):
-        """Hands a reference-format state_dict to the library (it packs its own copies)."""
+    def _describe(self, state_dict: Dict[str, Tensor]):
+        """(n, keys, dev_ptrs, shapes, ndims) of a reference-format state_dict as the C ABI takes it, and the device
+        tensors the pointers refer to (to be kept alive until the call has returned)."""
         keys, tensors = [], []
         for k, v in state_dict.items():
             keys.append(k.encode())
@@ -154,10 +156,15 @@ class Context:
             ndims[i] = t.dim()
             for d in range(4):
                 shapes[4 * i + d] = t.shape[d] if d < t.dim() else 1
+        return (n, (ctypes.c_char_p * n)(*keys), _ptr_array(tensors), shapes, ndims), tensors
+
+    def load_net(self, net: str, state_dict: Dict[str, Tensor]):
+        """Hands a reference-format state_dict to the library (it packs its own copies)."""
+        args, keep = self._describe(state_dict)
         with torch.cuda.device(self.device):
-            self._call('tha4_load_net', NET_IDS[net], n, (ctypes.c_char_p * n)(*keys), _ptr_array(tensors), shapes, ndims,
-                       self._stream())
+            self._call('tha4_load_net', NET_IDS[net], *args, self._stream())
             torch.cuda.current_stream(self.device).synchronize()
+        del keep
         self.loaded[net] = True
         self.epoch += 1
 
@@ -406,6 +413,43 @@ class Context:
             outs.append(flat[o:o + n].view(B, c, r, r))
             o += n
         self._call('tha4_student_forward_io', _ptr(image), _ptr(pose), B, _ptr_array(outs), 1, self._stream())
+        return outs
+
+    # ------------------------------------------------------------------ character bank
+    def bank_create(self, capacity: int):
+        """One bank of `capacity` character slots on this context (replaces an existing one)."""
+        self._call('tha4_bank_create', int(capacity))
+
+    def bank_destroy(self):
+        self._call('tha4_bank_destroy')
+
+    def bank_set_character(self, slot: int, face_state_dict: Dict[str, Tensor], body_state_dict: Dict[str, Tensor], image: Tensor):
+        """Packs one character (the two students' state_dicts and its [4,512,512] image) into `slot`."""
+        image = _check_input(image, self.device, 'image')
+        assert image.shape == (4, 512, 512)
+        face, keep_f = self._describe(face_state_dict)
+        body, keep_b = self._describe(body_state_dict)
+        with torch.cuda.device(self.device):
+            self._call('tha4_bank_set_character', int(slot), *face, *body, _ptr(image), self._stream())
+        del keep_f, keep_b
+
+    def bank_forward(self, char_ids: Sequence[int], pose: Tensor, half: bool = False) -> List[Tensor]:
+        """The six student outputs for frames of possibly different characters: frame n is the character in slot
+        char_ids[n] (host integers, checked by the library before it launches anything) at pose[n]."""
+        pose = _check_input(pose, self.device, 'pose')
+        B = len(char_ids)
+        assert B >= 1 and pose.shape == (B, 45)
+        specs = [(4, 512), (1, 512), (4, 512), (4, 512), (2, 512), (4, 128)]
+        if half:
+            flat = torch.empty(sum(B * c * r * r for c, r in specs), dtype=torch.float16, device=self.device)
+            outs, o = [], 0
+            for c, r in specs:
+                outs.append(flat[o:o + B * c * r * r].view(B, c, r, r))
+                o += B * c * r * r
+        else:
+            outs = self._empty(specs, B)
+        ids = (ctypes.c_int * B)(*[int(i) for i in char_ids])
+        self._call('tha4_bank_forward', ids, _ptr(pose), B, _ptr_array(outs), 1 if half else 0, self._stream())
         return outs
 
     # ------------------------------------------------------------------ distillation

@@ -69,6 +69,7 @@ struct tha4_ctx {
     std::unique_ptr<UNetNet> body, upscaler;
     std::unique_ptr<SirenFaceNet> sface;
     std::unique_ptr<SirenBodyNet> sbody;
+    std::unique_ptr<SirenBank> bank;       // tha4_bank_create: the students of many characters for mixed batches
 };
 
 namespace {
@@ -632,6 +633,51 @@ int tha4_student_forward_io(tha4_ctx* ctx, const void* image, const float* pose,
         copy_window(make_img(face32, B, 4, 128, 128), body_in + 80 * 512 + 192, 4L * 512 * 512, 512L * 512, 512, s);
         convert_flat_f16(face32, (__half*)outputs[5], face_n, s);
         ctx->sbody->forward(rt, make_img(body_in, B, 4, 512, 512), pose, 45, (float* const*)outputs, true);
+    });
+}
+
+int tha4_bank_create(tha4_ctx* ctx, int capacity) {
+    return guarded(ctx, [&] {
+        cudaDeviceSynchronize();              // a forward on another stream may still read the bank this one replaces
+        ctx->bank.reset();
+        ctx->bank.reset(new SirenBank(capacity));
+    });
+}
+
+int tha4_bank_destroy(tha4_ctx* ctx) {
+    return guarded(ctx, [&] {
+        cudaDeviceSynchronize();
+        ctx->bank.reset();
+    });
+}
+
+int tha4_bank_set_character(tha4_ctx* ctx, int slot, int n_face, const char* const* face_keys, const void* const* face_ptrs,
+                            const int64_t* face_shapes, const int* face_ndims, int n_body, const char* const* body_keys,
+                            const void* const* body_ptrs, const int64_t* body_shapes, const int* body_ndims, const float* image,
+                            void* stream) {
+    return guarded(ctx, [&] {
+        THA4_REQUIRE(ctx->bank != nullptr, "character bank: tha4_bank_create has not been called");
+        cudaDeviceSynchronize();              // a forward on another stream may still read the slot
+        ctx->bank->set_character(slot, make_sd(n_face, face_keys, face_ptrs, face_shapes, face_ndims),
+                                 make_sd(n_body, body_keys, body_ptrs, body_shapes, body_ndims), image, (cudaStream_t)stream);
+    });
+}
+
+int tha4_bank_forward(tha4_ctx* ctx, const int* char_ids, const float* pose, int B, void* const* outputs, int io_dtype, void* stream) {
+    return guarded(ctx, [&] {
+        THA4_REQUIRE(ctx->bank != nullptr, "character bank: tha4_bank_create has not been called");
+        THA4_REQUIRE(B >= 1 && char_ids && pose && outputs, "bank forward: batch must be >= 1 and every argument given");
+        THA4_REQUIRE(io_dtype == 0 || io_dtype == 1, "bank forward: io_dtype must be 0 (fp32) or 1 (fp16)");
+        // the ids become TMA coordinates and array offsets on the device: nothing is launched on a bad one
+        for (int n = 0; n < B; ++n) {
+            THA4_REQUIRE(char_ids[n] >= 0 && char_ids[n] < ctx->bank->capacity(), "bank forward: character id " + std::to_string(char_ids[n]) +
+                         " of frame " + std::to_string(n) + " is not 0.." + std::to_string(ctx->bank->capacity() - 1));
+            THA4_REQUIRE(ctx->bank->filled(char_ids[n]), "bank forward: slot " + std::to_string(char_ids[n]) + " (frame " + std::to_string(n) +
+                         ") holds no character");
+        }
+        Runtime rt = make_rt(ctx, stream);
+        begin_pass(ctx, (cudaStream_t)stream);
+        ctx->bank->forward(rt, char_ids, pose, B, outputs, io_dtype == 1);
     });
 }
 

@@ -433,7 +433,7 @@ const TensorRef& get(const StateDict& sd, const std::string& k) {
 }  // namespace
 
 // Packs one sine layer.  feat: number of leading "feature" input channels that go through the MMA (0: none).
-void SirenLayer::load(const StateDict& sd, const std::string& prefix, int feat, int pose, int kpad, int npad, float scale,
+void SirenLayer::pack(const StateDict& sd, const std::string& prefix, int feat, int pose, int kpad, int npad, float scale,
                       cudaStream_t s) {
     const TensorRef& w = get(sd, prefix + ".weight");
     const TensorRef& b = get(sd, prefix + ".bias");
@@ -443,21 +443,34 @@ void SirenLayer::load(const StateDict& sd, const std::string& prefix, int feat, 
     THA4_REQUIRE(nreal <= npad && feat <= kpad, "siren layer padding: " + prefix);
     N = nreal; NPAD = npad; KPAD = kpad; P = pose;
     if (feat > 0) {
-        W = dmalloc<__half>((size_t)npad * kpad);
         pack_w_kernel<<<64, 256, 0, s>>>(w.p, cin, 0, feat, nreal, kpad, npad, scale, reinterpret_cast<__half*>(W));
         THA4_LAUNCH_CHECK();
     }
-    bias = dmalloc<float>(npad);
     pack_vec_kernel<<<ceil_div(npad, 128), 128, 0, s>>>(b.p, nreal, npad, scale, bias);
     THA4_LAUNCH_CHECK();
     if (first) {
-        wxy = dmalloc<float>((size_t)npad * 2);
         pack_cols_kernel<<<16, 256, 0, s>>>(w.p, cin, feat, 2, nreal, npad, scale, wxy);
         THA4_LAUNCH_CHECK();
-        wpose = dmalloc<float>((size_t)npad * pose);
         pack_cols_kernel<<<64, 256, 0, s>>>(w.p, cin, feat + 2, pose, nreal, npad, scale, wpose);
         THA4_LAUNCH_CHECK();
     }
+}
+
+// allocates `count` layers' buffers back to back (count = 1: one network; the bank: one per character)
+static void alloc_layer(SirenLayer& l, int feat, int pose, int kpad, int npad, size_t count) {
+    if (feat > 0) l.W = dmalloc<__half>(count * npad * kpad);
+    l.bias = dmalloc<float>(count * npad);
+    if (pose > 0) {
+        l.wxy = dmalloc<float>(count * npad * 2);
+        l.wpose = dmalloc<float>(count * npad * pose);
+    }
+    l.NPAD = npad; l.KPAD = kpad; l.P = pose;
+}
+
+void SirenLayer::load(const StateDict& sd, const std::string& prefix, int feat, int pose, int kpad, int npad, float scale,
+                      cudaStream_t s) {
+    alloc_layer(*this, feat, pose, kpad, npad, 1);
+    pack(sd, prefix, feat, pose, kpad, npad, scale, s);
 }
 
 // per-sample bias of a first layer: pb[n][:] = scale*b + (scale*Wpose) . pose[n]
@@ -465,6 +478,47 @@ static float* pose_bias(Runtime& rt, const SirenLayer& l, const float* pose, int
     float* pb = rt.persist->alloc((size_t)B * l.NPAD);
     linear_forward(pose, pose_ld, B, l.P, l.wpose, l.bias, l.NPAD, 0, pb, l.NPAD, rt.stream);
     return pb;
+}
+
+// The same for a bank: pb[n][:] = bias[c] + wpose[c] . pose[n] with c = char_of[n].  One block per sample, one warp per
+// output at a time, in the summation order of linear_forward (lane-strided FMAs, xor-shuffle tree, bias last), so a
+// sample's pb is bit-identical to what its character's own network computes.
+__global__ void __launch_bounds__(256) pose_bias_bank_kernel(const float* __restrict__ pose, int pose_ld, int I,
+                                                             const float* __restrict__ wpose, const float* __restrict__ bias, int O,
+                                                             const int* __restrict__ char_of, float* __restrict__ pb) {
+    const int n = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int c = char_of[n];
+    const float* xr = pose + (long)n * pose_ld;
+    for (int o = warp; o < O; o += 8) {
+        const float* wr = wpose + ((long)c * O + o) * I;
+        float acc = 0.0f;
+        for (int i = lane; i < I; i += 32) acc = fmaf(xr[i], wr[i], acc);
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
+        if (lane == 0) pb[(long)n * O + o] = acc + bias[(long)c * O + o];
+    }
+}
+static float* pose_bias_bank(Runtime& rt, const SirenLayer& l, const float* pose, int pose_ld, int B, const int* char_of) {
+    float* pb = rt.persist->alloc((size_t)B * l.NPAD);
+    pose_bias_bank_kernel<<<B, 256, 0, rt.stream>>>(pose, pose_ld, l.P, l.wpose, l.bias, l.NPAD, char_of, pb);
+    THA4_LAUNCH_CHECK();
+    return pb;
+}
+
+// dst[n] = images[char_of[n]] ([4,512,512] fp32 each); round_f16: through fp16, as an fp16 input image would arrive
+__global__ void gather_images_kernel(const float4* __restrict__ images, const int* __restrict__ char_of, long per_image4,
+                                     int round_f16, float4* __restrict__ dst) {
+    const int n = blockIdx.y;
+    const float4* src = images + (long)char_of[n] * per_image4;
+    float4* d = dst + (long)n * per_image4;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < per_image4; i += (long)gridDim.x * blockDim.x) {
+        float4 v = __ldg(src + i);
+        if (round_f16) {
+            v.x = __half2float(__float2half_rn(v.x)); v.y = __half2float(__float2half_rn(v.y));
+            v.z = __half2float(__float2half_rn(v.z)); v.w = __half2float(__float2half_rn(v.w));
+        }
+        d[i] = v;
+    }
 }
 
 static LayerW lw(const SirenLayer& l, const float* bias_override = nullptr) {
@@ -504,9 +558,11 @@ void siren_level(Runtime& rt, const SirenLevelArgs& a) {
         lv.o_f16 = a.out_f16;
         lv.face_out = a.face_out;
         lv.head_bias = a.head ? a.head->bias : nullptr;
+        lv.char_of = a.char_of; lv.chars = a.chars; lv.head_cs = a.head ? a.head->NPAD : 0;
         siren_tc_run(rt, a.mode, plan, lv);
         return;
     }
+    THA4_REQUIRE(a.char_of == nullptr, "siren level: a character bank needs the wgmma kernels (option siren_tc = 1); the mma.sync kernels take one character's weights");
     // mma.sync path: one kernel per level, compiled for the production layer shapes only
     THA4_REQUIRE(!a.out_f16, "siren body: f16 outputs need the tensor-core path (option siren_tc)");
     auto shape = [&](int i, int kpad, int npad) { return a.L[i].KPAD == kpad && a.L[i].NPAD == npad; };
@@ -591,51 +647,65 @@ void siren_test_level(Runtime& rt, bool tc, int mode, const StateDict& sd, int n
 }
 
 // ------------------------------------------------------------------------------------------------ SirenFaceNet
+// The layers of the two students: state_dict prefix, feature / pose input channels, padded K and N, pre-scale.
+struct LayerSpec { std::string key; int feat, pose, kpad, npad; float scale; };
+static LayerSpec face_layer_spec(int i) {          // i = 8: the head
+    if (i == 8) return {"siren.last_linear", 128, 0, 128, 8, 1.0f};
+    return {"siren.sine_layers." + std::to_string(i) + ".linear", i == 0 ? 0 : 128, i == 0 ? 39 : 0, 128, 128, 30.0f};
+}
+static LayerSpec body_layer_spec(int level, int j) {   // level 3: the head
+    if (level == 3) return {"last_linear", 90, 0, 96, 8, 1.0f};
+    static const int feat[3][3] = {{0, 360, 360}, {180, 180, 180}, {90, 90, 90}};
+    static const int kpad[3][3] = {{32, 384, 384}, {192, 192, 192}, {96, 96, 96}};
+    static const int npad[3][3] = {{384, 384, 192}, {192, 192, 96}, {96, 96, 96}};
+    return {"siren_layers." + std::to_string(level) + "." + std::to_string(j) + ".linear", feat[level][j], j == 0 ? 45 : 0,
+            kpad[level][j], npad[level][j], 30.0f};
+}
+static void load_layer(SirenLayer& l, const StateDict& sd, const LayerSpec& sp, cudaStream_t s) {
+    l.load(sd, sp.key, sp.feat, sp.pose, sp.kpad, sp.npad, sp.scale, s);
+}
+
 void SirenFaceNet::load(const StateDict& sd, cudaStream_t s) {
     SinkScope own(&owned_);
-    for (int i = 0; i < 8; ++i)
-        layers_[i].load(sd, "siren.sine_layers." + std::to_string(i) + ".linear", i == 0 ? 0 : 128, i == 0 ? 39 : 0, 128, 128, 30.0f, s);
-    head_.load(sd, "siren.last_linear", 128, 0, 128, 8, 1.0f, s);
+    for (int i = 0; i < 8; ++i) load_layer(layers_[i], sd, face_layer_spec(i), s);
+    load_layer(head_, sd, face_layer_spec(8), s);
     THA4_CUDA_CHECK(cudaStreamSynchronize(s));
     loaded_ = true;
 }
 
-void SirenFaceNet::forward(Runtime& rt, const float* pose, int pose_ld, int B, float* out) {
-    THA4_REQUIRE(loaded_, "network weights not loaded");
-    const int R = 128;
+// the face network's one level on pb [B][128]; char_of / chars: see SirenLevelArgs (null / 0: one character)
+static void face_levels(Runtime& rt, const SirenLayer* layers, const SirenLayer& head, const float* pb, int B, float* out,
+                        const int* char_of, int chars) {
     static const int nb[8] = {64, 64, 64, 64, 64, 64, 64, 16};
     SirenLevelArgs a;
-    a.tc = siren_tc_enabled(); a.mode = 3; a.R = R; a.B = B;
-    a.L = layers_; a.nl = 8; a.head = &head_; a.nb = nb;
-    a.pb = pose_bias(rt, layers_[0], pose, pose_ld, B);
+    a.tc = siren_tc_enabled(); a.mode = 3; a.R = 128; a.B = B;
+    a.L = layers; a.nl = 8; a.head = &head; a.nb = nb;
+    a.pb = pb;
     a.face_out = out;
+    a.char_of = char_of; a.chars = chars;
     siren_level(rt, a);
+}
+
+void SirenFaceNet::forward(Runtime& rt, const float* pose, int pose_ld, int B, float* out) {
+    THA4_REQUIRE(loaded_, "network weights not loaded");
+    face_levels(rt, layers_, head_, pose_bias(rt, layers_[0], pose, pose_ld, B), B, out, nullptr, 0);
 }
 
 // ------------------------------------------------------------------------------------------------ SirenBodyNet
 void SirenBodyNet::load(const StateDict& sd, cudaStream_t s) {
     SinkScope own(&owned_);
-    auto key = [](int i, int j) { return "siren_layers." + std::to_string(i) + "." + std::to_string(j) + ".linear"; };
-    l_[0][0].load(sd, key(0, 0), 0, 45, 32, 384, 30.0f, s);
-    l_[0][1].load(sd, key(0, 1), 360, 0, 384, 384, 30.0f, s);
-    l_[0][2].load(sd, key(0, 2), 360, 0, 384, 192, 30.0f, s);
-    l_[1][0].load(sd, key(1, 0), 180, 45, 192, 192, 30.0f, s);
-    l_[1][1].load(sd, key(1, 1), 180, 0, 192, 192, 30.0f, s);
-    l_[1][2].load(sd, key(1, 2), 180, 0, 192, 96, 30.0f, s);
-    l_[2][0].load(sd, key(2, 0), 90, 45, 96, 96, 30.0f, s);
-    l_[2][1].load(sd, key(2, 1), 90, 0, 96, 96, 30.0f, s);
-    l_[2][2].load(sd, key(2, 2), 90, 0, 96, 96, 30.0f, s);
-    head_.load(sd, "last_linear", 90, 0, 96, 8, 1.0f, s);
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) load_layer(l_[i][j], sd, body_layer_spec(i, j), s);
+    load_layer(head_, sd, body_layer_spec(3, 0), s);
     THA4_CUDA_CHECK(cudaStreamSynchronize(s));
     loaded_ = true;
 }
 
-void SirenBodyNet::forward(Runtime& rt, const ImgView& image, const float* pose, int pose_ld, float* const* outputs, bool outputs_f16) {
-    THA4_REQUIRE(loaded_, "network weights not loaded");
+// the body network's three levels on the per-level pb; char_of / chars: see SirenLevelArgs (null / 0: one character)
+static void body_levels(Runtime& rt, const SirenLayer (*l)[3], const SirenLayer& head, const float* const* pb, const ImgView& image,
+                        float* const* outputs, bool outputs_f16, const int* char_of, int chars) {
     THA4_REQUIRE(image.H == 512 && image.W == 512 && image.C == 4, "siren body: image size");
     const int B = image.N;
-    const float* pb[3];
-    for (int i = 0; i < 3; ++i) pb[i] = pose_bias(rt, l_[i][0], pose, pose_ld, B);
     __half* f0 = reinterpret_cast<__half*>(rt.persist->alloc((size_t)B * 128 * 128 * 192 / 2));
     __half* f1 = reinterpret_cast<__half*>(rt.persist->alloc((size_t)B * 256 * 256 * 96 / 2));
     const bool tc = siren_tc_enabled();
@@ -644,12 +714,82 @@ void SirenBodyNet::forward(Runtime& rt, const ImgView& image, const float* pose,
     for (int i = 0; i < 3; ++i) {
         SirenLevelArgs a;
         a.tc = tc; a.mode = i; a.R = 128 << i; a.B = B;
-        a.L = l_[i]; a.nl = 3; a.nb = nb; a.pb = pb[i];
+        a.L = l[i]; a.nl = 3; a.nb = nb; a.pb = pb[i];
         if (i > 0) { a.prev = i == 1 ? f0 : f1; a.prev_c = i == 1 ? 192 : 96; }
         if (i < 2) a.out = i == 0 ? f0 : f1;
-        else { a.head = &head_; a.image = image; a.outputs = outputs; a.out_f16 = outputs_f16; }
+        else { a.head = &head; a.image = image; a.outputs = outputs; a.out_f16 = outputs_f16; }
+        a.char_of = char_of; a.chars = chars;
         siren_level(rt, a);
     }
+}
+
+void SirenBodyNet::forward(Runtime& rt, const ImgView& image, const float* pose, int pose_ld, float* const* outputs, bool outputs_f16) {
+    THA4_REQUIRE(loaded_, "network weights not loaded");
+    THA4_REQUIRE(image.H == 512 && image.W == 512 && image.C == 4, "siren body: image size");
+    const float* pb[3];
+    for (int i = 0; i < 3; ++i) pb[i] = pose_bias(rt, l_[i][0], pose, pose_ld, image.N);
+    body_levels(rt, l_, head_, pb, image, outputs, outputs_f16, nullptr, 0);
+}
+
+// ------------------------------------------------------------------------------------------------ SirenBank
+SirenBank::SirenBank(int capacity) : capacity_(capacity), filled_((size_t)std::max(capacity, 0), 0) {
+    THA4_REQUIRE(capacity >= 1 && capacity <= 4096, "character bank: capacity must be 1..4096");
+    SinkScope own(&owned_);
+    auto alloc = [&](SirenLayer& l, const LayerSpec& sp) { alloc_layer(l, sp.feat, sp.pose, sp.kpad, sp.npad, (size_t)capacity); };
+    for (int i = 0; i < 8; ++i) alloc(face_[i], face_layer_spec(i));
+    alloc(face_head_, face_layer_spec(8));
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) alloc(body_[i][j], body_layer_spec(i, j));
+    alloc(body_head_, body_layer_spec(3, 0));
+    images_ = dmalloc<float>((size_t)capacity * 4 * 512 * 512);
+}
+
+SirenLayer SirenBank::at(const SirenLayer& base, int slot) const {
+    SirenLayer l = base;
+    const size_t c = (size_t)slot;
+    if (base.W) l.W = reinterpret_cast<__half*>(base.W) + c * base.NPAD * base.KPAD;
+    l.bias = base.bias + c * base.NPAD;
+    if (base.wxy) { l.wxy = base.wxy + c * base.NPAD * 2; l.wpose = base.wpose + c * base.NPAD * base.P; }
+    return l;
+}
+
+void SirenBank::set_character(int slot, const StateDict& face, const StateDict& body, const float* image, cudaStream_t s) {
+    THA4_REQUIRE(slot >= 0 && slot < capacity_, "character bank: slot " + std::to_string(slot) + " is not 0.." + std::to_string(capacity_ - 1));
+    THA4_REQUIRE(image != nullptr, "character bank: the character's image is required");
+    filled_[slot] = 0;
+    auto pack = [&](const SirenLayer& base, const StateDict& sd, const LayerSpec& sp) {
+        at(base, slot).pack(sd, sp.key, sp.feat, sp.pose, sp.kpad, sp.npad, sp.scale, s);
+    };
+    for (int i = 0; i < 8; ++i) pack(face_[i], face, face_layer_spec(i));
+    pack(face_head_, face, face_layer_spec(8));
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) pack(body_[i][j], body, body_layer_spec(i, j));
+    pack(body_head_, body, body_layer_spec(3, 0));
+    const size_t img = (size_t)4 * 512 * 512;
+    THA4_CUDA_CHECK(cudaMemcpyAsync(images_ + (size_t)slot * img, image, img * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    THA4_CUDA_CHECK(cudaStreamSynchronize(s));
+    filled_[slot] = 1;
+}
+
+void SirenBank::forward(Runtime& rt, const int* char_of_host, const float* pose, int B, void* const* outputs, bool outputs_f16) {
+    THA4_REQUIRE(siren_tc_enabled(), "character bank: needs the wgmma student kernels (option siren_tc = 1); the mma.sync kernels take one character's weights");
+    cudaStream_t s = rt.stream;
+    int* char_of = reinterpret_cast<int*>(rt.persist->alloc((size_t)B));
+    THA4_CUDA_CHECK(cudaMemcpyAsync(char_of, char_of_host, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, s));
+    // face SIREN from pose[:, :39] (mode_14.py:64-71), pasted at rows 80:208, cols 192:320 of the character's image (:72-78)
+    const long face_n = (long)B * 4 * 128 * 128, per_image4 = 512L * 512;
+    float* face = outputs_f16 ? rt.persist->alloc((size_t)face_n) : reinterpret_cast<float*>(outputs[5]);
+    face_levels(rt, face_, face_head_, pose_bias_bank(rt, face_[0], pose, 45, B, char_of), B, face, char_of, capacity_);
+    float* body_in = rt.persist->alloc((size_t)B * 4 * 512 * 512);
+    gather_images_kernel<<<dim3(256, B), 256, 0, s>>>(reinterpret_cast<const float4*>(images_), char_of, per_image4, outputs_f16 ? 1 : 0,
+                                                      reinterpret_cast<float4*>(body_in));
+    THA4_LAUNCH_CHECK();
+    copy_window(make_img(face, B, 4, 128, 128), body_in + 80 * 512 + 192, 4L * 512 * 512, 512L * 512, 512, s);
+    if (outputs_f16) convert_flat_f16(face, reinterpret_cast<__half*>(outputs[5]), face_n, s);
+    const float* pb[3];
+    for (int i = 0; i < 3; ++i) pb[i] = pose_bias_bank(rt, body_[i][0], pose, 45, B, char_of);
+    body_levels(rt, body_, body_head_, pb, make_img(body_in, B, 4, 512, 512), reinterpret_cast<float* const*>(outputs), outputs_f16,
+                char_of, capacity_);
 }
 
 }  // namespace tha4

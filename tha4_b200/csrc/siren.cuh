@@ -11,6 +11,8 @@ struct SirenLayer {
     float* wpose = nullptr;   // [NPAD][P]   (first layers only)
     int N = 0, NPAD = 0, KPAD = 0, P = 0;
     void load(const StateDict& sd, const std::string& prefix, int feat, int pose, int kpad, int npad, float scale, cudaStream_t s);
+    // the packing of load() into buffers the caller owns (W / bias / wxy / wpose set, sized for kpad / npad / pose)
+    void pack(const StateDict& sd, const std::string& prefix, int feat, int pose, int kpad, int npad, float scale, cudaStream_t s);
 };
 
 // ---- wgmma path (siren_tc.cu): a level = a chain of GEMM layers on 128-pixel tiles, weights streamed by TMA ----
@@ -27,6 +29,9 @@ struct SirenTcLevel {
     const __half* prev = nullptr; int prev_c = 0; __half* out = nullptr; int out_c = 0;
     ImgView image; float* o[5] = {nullptr, nullptr, nullptr, nullptr, nullptr}; bool o_f16 = false;
     float* face_out = nullptr; const float* head_bias = nullptr;
+    // character bank: the plan's W / bias, e_wxy / f_wxy and head_bias point at character 0 of `chars` characters stored
+    // back to back, and sample n runs on the weights of character char_of[n] (device, [B], every entry in 0..chars-1)
+    const int* char_of = nullptr; int chars = 0; int head_cs = 0;     // head_cs: floats between two characters' head biases
 };
 void siren_tc_run(Runtime& rt, int mode, const SirenTcPlan& plan, const SirenTcLevel& lv);   // mode 0..2: body levels, 3: face
 // Checks a plan against the kernel of `mode` (host only, launches nothing): "" if it fits, else what does not.  The
@@ -53,6 +58,9 @@ struct SirenLevelArgs {
     __half* out = nullptr;
     ImgView image; float* const* outputs = nullptr; bool out_f16 = false;
     float* face_out = nullptr;
+    // character bank (wgmma path only): L / head are character 0 of `chars` characters whose buffers lie back to back
+    // (SirenBank); sample n runs on character char_of[n] (device, [B]) and pb holds its per-sample bias
+    const int* char_of = nullptr; int chars = 0;
 };
 void siren_level(Runtime& rt, const SirenLevelArgs& a);
 // Kernel-level test entry: loads the layers "layer.<i>" (and "head") of `sd` as the networks do and runs one level.
@@ -83,6 +91,30 @@ private:
     AllocSink owned_;
     SirenLayer l_[3][3], head_;
     bool loaded_ = false;
+};
+
+// C characters' students in one set of buffers, for batches that mix characters (tha4_bank_forward).  Every layer is
+// packed exactly as SirenFaceNet / SirenBodyNet pack it, into one allocation per layer with the character as the
+// outermost dimension: W [C][NPAD][KPAD] fp16, bias [C][NPAD], wxy [C][NPAD][2], wpose [C][NPAD][P], head bias [C][8].
+// The characters' images [C,4,512,512] fp32 live beside the weights, so a frame's image is addressed by its character.
+class SirenBank {
+public:
+    explicit SirenBank(int capacity);
+    int capacity() const { return capacity_; }
+    bool filled(int slot) const { return slot >= 0 && slot < capacity_ && filled_[slot]; }
+    // Packs one character into `slot` (other slots are not touched).  A slot whose packing fails is left empty.
+    void set_character(int slot, const StateDict& face, const StateDict& body, const float* image, cudaStream_t s);
+    // The mode_14 DAG for B frames: frame n is character char_of_host[n] (validated by the caller) at pose[n] ([B,45]).
+    // outputs: the six of tha4_student_forward, fp32 or (outputs_f16) fp16; fp16 also rounds the image to fp16 first,
+    // as the fp16 image of tha4_student_forward_io is.
+    void forward(Runtime& rt, const int* char_of_host, const float* pose, int B, void* const* outputs, bool outputs_f16);
+private:
+    SirenLayer at(const SirenLayer& base, int slot) const;
+    AllocSink owned_;
+    int capacity_;
+    std::vector<char> filled_;
+    SirenLayer face_[8], face_head_, body_[3][3], body_head_;          // character 0; character c lies c layer sizes further
+    float* images_ = nullptr;
 };
 
 }  // namespace tha4

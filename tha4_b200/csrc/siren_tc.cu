@@ -57,6 +57,10 @@ struct StParams {
     ImgView image; float* o[5]; int o_f16;          // level 2: tail (o_f16: the five outputs are __half planes, io_dtype = f16)
     float* face_out;                                // face: [B, 4, R, R]
     const float* head_bias;
+    // character bank (the BANK instantiations): sample n runs on character char_of[n].  The weight maps are 3-D with the
+    // character as the outermost coordinate; bias_table, e_wxy / f_wxy and head_bias point at character 0 and the
+    // *_cs members are the floats from one character to the next.
+    const int* char_of; int bias_cs, wxy_cs, head_cs;
 };
 
 // sin(x) WITHOUT the transcendental unit.  The mma.sync student kernels (siren.cu) and the first version of this file used
@@ -111,7 +115,10 @@ __device__ __forceinline__ void st_slice_mma(float (&d)[2][NBMAX / 2], int nb, u
     for (int h = 0; h < 2; ++h) wg_fence_acc(d[h]);
 }
 
-template <int ACH, int NBMAX, int SB, int MODE>
+// BANK: per-sample weights (see StParams::char_of).  A tile is one sample's, so its character selects the weight tiles the
+// producer fetches (third TMA coordinate), the biases staged in sbias (re-staged when the CTA's next tile is another
+// character's), the first layer's wxy and the head bias; everything else is the one-character kernel.
+template <int ACH, int NBMAX, int SB, int MODE, bool BANK>
 __global__ void __launch_bounds__(ST_THREADS) siren_tc_kernel(const __grid_constant__ StMaps maps, const StParams p) {
     constexpr int A_BYTES = ACH * ST_TILE * 128;
     constexpr int B_STAGE = NBMAX * 128;
@@ -134,13 +141,16 @@ __global__ void __launch_bounds__(ST_THREADS) siren_tc_kernel(const __grid_const
         asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
         for (int l = 0; l < p.nl; ++l) asm volatile("prefetch.tensormap [%0];\n" :: "l"(&maps.w[l]) : "memory");
     }
-    for (int i = threadIdx.x; i < p.bias_floats; i += ST_THREADS) sbias[i] = __ldg(p.bias_table + i);
+    if constexpr (!BANK)
+        for (int i = threadIdx.x; i < p.bias_floats; i += ST_THREADS) sbias[i] = __ldg(p.bias_table + i);
     __syncthreads();
 
     if (warp == 4) {
         if (lane == 0) {       // ===== TMA producer: the weight tiles of every layer of every tile, in order =====
             uint32_t it = 0;
-            for (long tile = blockIdx.x; tile < ntiles; tile += gridDim.x)
+            for (long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+                int ch = 0;
+                if constexpr (BANK) ch = __ldg(p.char_of + (int)(tile / ((long)p.R * tiles_per_row)));
                 for (int l = 0; l < p.nl; ++l) {
                     const StLayer& L = p.L[l];
                     const int nsl = L.npad / L.nb, nkc = (L.kpad + 63) >> 6;
@@ -149,27 +159,42 @@ __global__ void __launch_bounds__(ST_THREADS) siren_tc_kernel(const __grid_const
                             const int s = it % SB;
                             mbar_wait(smem_u32(b_empty + s), ((it / SB) & 1) ^ 1);
                             mbar_expect_tx(smem_u32(b_full + s), L.nb * 128);
-                            asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];\n"
-                                         :: "r"(smem_u32(smB + s * B_STAGE)), "l"(&maps.w[l]), "r"(smem_u32(b_full + s)), "r"(kc * 64), "r"(ns * L.nb) : "memory");
+                            if constexpr (BANK)
+                                asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];\n"
+                                             :: "r"(smem_u32(smB + s * B_STAGE)), "l"(&maps.w[l]), "r"(smem_u32(b_full + s)), "r"(kc * 64), "r"(ns * L.nb), "r"(ch) : "memory");
+                            else
+                                asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];\n"
+                                             :: "r"(smem_u32(smB + s * B_STAGE)), "l"(&maps.w[l]), "r"(smem_u32(b_full + s)), "r"(kc * 64), "r"(ns * L.nb) : "memory");
                         }
                 }
+            }
         }
     } else {                   // ===== consumer warpgroup: thread te = pixel (tile row) of the prologue / head; fragments for the MMAs =====
         const int te = threadIdx.x;                                        // 0..127
         const int fr = warp * 16 + (lane >> 2);                            // first accumulator row of this thread (+8, +64, +72)
         uint32_t it = 0;
         int cur = 0;                                                       // A buffer holding the current layer's operand
+        int staged = -1;                                                   // BANK: the character whose biases sbias holds
         for (long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
             const int n = (int)(tile / ((long)p.R * tiles_per_row));
             const int rem = (int)(tile - (long)n * p.R * tiles_per_row);
             const int y = rem / tiles_per_row, x0 = (rem - y * tiles_per_row) * ST_TILE;
             const float yv = __ldg(p.base + y);
             sx[te] = __ldg(p.base + x0 + te);
+            int ch = 0;
+            if constexpr (BANK) {
+                ch = __ldg(p.char_of + n);
+                if (ch != staged) {        // the previous tile's readers of sbias are past the barrier that ended it
+                    for (int i = te; i < p.bias_floats; i += 128) sbias[i] = __ldg(p.bias_table + (size_t)ch * p.bias_cs + i);
+                    staged = ch;
+                }
+            }
             {   // this tile's per-sample first-layer terms: bias (b + Wpose . pose[n]) and the xy weights
                 const bool elementwise = (MODE == SM_BODY0 || MODE == SM_FACE);
                 const int np = elementwise ? p.e_npad : p.L[0].npad;
                 const float* pb = elementwise ? p.e_pb + (size_t)n * p.e_pb_ld : p.f_pb + (size_t)n * p.f_pb_ld;
                 const float* wxy = elementwise ? p.e_wxy : p.f_wxy;
+                if constexpr (BANK) wxy += (size_t)ch * p.wxy_cs;
                 for (int i = te; i < np; i += 128) {
                     sfirst[i] = __ldg(pb + i);
                     sfirst[384 + 2 * i] = __ldg(wxy + 2 * i); sfirst[384 + 2 * i + 1] = __ldg(wxy + 2 * i + 1);
@@ -286,14 +311,16 @@ __global__ void __launch_bounds__(ST_THREADS) siren_tc_kernel(const __grid_const
                         asm volatile("bar.sync 1, 128;\n" ::: "memory");
                         const float* acc = stage + te * 17;
                         const int x = x0 + te;
+                        const float* head_bias = p.head_bias;
+                        if constexpr (BANK) head_bias += ch * p.head_cs;
                         if (MODE == SM_FACE) {
 #pragma unroll
                             for (int c = 0; c < 4; ++c)
-                                p.face_out[(((size_t)n * 4 + c) * p.R + y) * p.R + x] = acc[c] + __ldg(p.head_bias + c);
+                                p.face_out[(((size_t)n * 4 + c) * p.R + y) * p.R + x] = acc[c] + __ldg(head_bias + c);
                         } else {
                             float o[7];
 #pragma unroll
-                            for (int c = 0; c < 7; ++c) o[c] = acc[c] + __ldg(p.head_bias + c);   // grid_change(0,1) alpha(2) colour(3..6)
+                            for (int c = 0; c < 7; ++c) o[c] = acc[c] + __ldg(head_bias + c);   // grid_change(0,1) alpha(2) colour(3..6)
                             const GsTap t = gs_locate(sx[te], yv, o[0], o[1], p.R, p.R);
                             float w[4];
                             gs_sample<4>(p.image.p + n * p.image.sn, p.image.sc, p.image.sh, p.R, p.R, t, w);
@@ -360,31 +387,40 @@ EncodeTiledFn st_encode() {
     return fn;
 }
 
-// W: [rows][kpad] fp16 K-major; box {64 k, nb rows}; rows beyond `rows` and k beyond kpad are zero-filled by TMA
-CUtensorMap weight_tile_map(const void* W, int rows, int kpad, int nb) {
+// W: [rows][kpad] fp16 K-major; box {64 k, nb rows}; rows beyond `rows` and k beyond kpad are zero-filled by TMA.
+// chars > 0: W is [chars][rows][kpad] and the map is 3-D with the character outermost (box {64, nb, 1}), so a tile of one
+// character never reads another's rows: rows beyond `rows` are zero-filled per character as in the 2-D map.
+CUtensorMap weight_tile_map(const void* W, int rows, int kpad, int nb, int chars) {
     CUtensorMap m;
-    cuuint64_t dims[2] = {(cuuint64_t)kpad, (cuuint64_t)rows};
-    cuuint64_t strides[1] = {(cuuint64_t)kpad * 2};
-    cuuint32_t box[2] = {64, (cuuint32_t)nb};
-    cuuint32_t es[2] = {1, 1};
-    CUresult r = st_encode()(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(W), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    cuuint64_t dims[3] = {(cuuint64_t)kpad, (cuuint64_t)rows, (cuuint64_t)chars};
+    cuuint64_t strides[2] = {(cuuint64_t)kpad * 2, (cuuint64_t)rows * kpad * 2};
+    cuuint32_t box[3] = {64, (cuuint32_t)nb, 1};
+    cuuint32_t es[3] = {1, 1, 1};
+    CUresult r = st_encode()(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, chars > 0 ? 3 : 2, const_cast<void*>(W), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                              CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     THA4_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(siren weights) failed: " + std::to_string((int)r));
     return m;
 }
 
-template <int ACH, int NBMAX, int SB, int MODE>
-void launch_siren_tc(const StMaps& maps, const StParams& p, int ctas_per_sm, cudaStream_t s) {
+template <int ACH, int NBMAX, int SB, int MODE, bool BANK>
+void launch_siren_tc_kernel(const StMaps& maps, const StParams& p, int ctas_per_sm, cudaStream_t s) {
     const size_t smem = 1024 + 2 * (size_t)ACH * ST_TILE * 128 + (size_t)SB * NBMAX * 128 + 2 * SB * 8 +
                         ((size_t)((p.bias_floats + 3) & ~3) + 3 * 384 + 128) * sizeof(float);
     THA4_REQUIRE(smem <= 227 * 1024, "siren_tc: shared memory budget");
     for (int l = 0; l < p.nl; ++l)        // st_slice_mma issues the slice widths up to NBMAX only
         THA4_REQUIRE(p.L[l].nb <= NBMAX && p.L[l].npad % p.L[l].nb == 0, "siren_tc: N slice width of layer " + std::to_string(l));
-    THA4_ENSURE_SMEM((siren_tc_kernel<ACH, NBMAX, SB, MODE>), smem);
+    THA4_ENSURE_SMEM((siren_tc_kernel<ACH, NBMAX, SB, MODE, BANK>), smem);
     const long ntiles = (long)p.B * p.R * (p.R / ST_TILE);
     const int grid = (int)std::min<long>(ntiles, (long)num_sms() * ctas_per_sm);
-    siren_tc_kernel<ACH, NBMAX, SB, MODE><<<grid, ST_THREADS, smem, s>>>(maps, p);
+    siren_tc_kernel<ACH, NBMAX, SB, MODE, BANK><<<grid, ST_THREADS, smem, s>>>(maps, p);
     THA4_LAUNCH_CHECK();
+}
+
+// the bank instantiation for a call that carries per-sample characters, the one-character instantiation for every other
+template <int ACH, int NBMAX, int SB, int MODE>
+void launch_siren_tc(const StMaps& maps, const StParams& p, int ctas_per_sm, cudaStream_t s) {
+    if (p.char_of) launch_siren_tc_kernel<ACH, NBMAX, SB, MODE, true>(maps, p, ctas_per_sm, s);
+    else launch_siren_tc_kernel<ACH, NBMAX, SB, MODE, false>(maps, p, ctas_per_sm, s);
 }
 
 bool g_siren_tc = true;
@@ -465,23 +501,32 @@ void SirenTcPlan::add(const SirenLayer& l, int nb, int sine, int first) {
 void siren_tc_run(Runtime& rt, int mode, const SirenTcPlan& plan, const SirenTcLevel& lv) {
     const std::string plan_err = siren_tc_plan_error(mode, plan, lv);
     THA4_REQUIRE(plan_err.empty(), "siren_tc plan: " + plan_err);
+    const int chars = lv.char_of ? lv.chars : 0;
+    THA4_REQUIRE(!lv.char_of || chars >= 1, "siren_tc: a character bank without characters");
     StParams p{};
     StMaps maps;
     p.R = lv.R; p.B = lv.B; p.nl = plan.nl;
-    // bias table (device, rebuilt per call from the layers' bias vectors: tiny)
+    // bias table (device, rebuilt per call from the layers' bias vectors: tiny); a bank's is [chars][all layers' biases]
     int off = 0;
     for (int l = 0; l < plan.nl; ++l) {
         p.L[l].kpad = plan.kpad[l]; p.L[l].npad = plan.npad[l]; p.L[l].nb = plan.nb[l]; p.L[l].sine = plan.sine[l]; p.L[l].first = plan.first[l];
         p.L[l].bias_off = off;
         if (plan.sine[l]) off += plan.npad[l];
-        maps.w[l] = weight_tile_map(plan.W[l], plan.rows[l], plan.kpad[l], plan.nb[l]);
+        maps.w[l] = weight_tile_map(plan.W[l], plan.rows[l], plan.kpad[l], plan.nb[l], chars);
     }
     p.bias_floats = off;
-    float* table = rt.persist->alloc((size_t)std::max(off, 4));
+    float* table = rt.persist->alloc((size_t)std::max(off, 4) * std::max(chars, 1));
     for (int l = 0; l < plan.nl; ++l)
-        if (plan.sine[l])
-            THA4_CUDA_CHECK(cudaMemcpyAsync(table + p.L[l].bias_off, plan.bias[l], plan.npad[l] * sizeof(float), cudaMemcpyDeviceToDevice, rt.stream));
+        if (plan.sine[l]) {
+            if (chars)      // a sine layer's biases lie npad floats apart from character to character
+                THA4_CUDA_CHECK(cudaMemcpy2DAsync(table + p.L[l].bias_off, off * sizeof(float), plan.bias[l], plan.npad[l] * sizeof(float),
+                                                  plan.npad[l] * sizeof(float), chars, cudaMemcpyDeviceToDevice, rt.stream));
+            else
+                THA4_CUDA_CHECK(cudaMemcpyAsync(table + p.L[l].bias_off, plan.bias[l], plan.npad[l] * sizeof(float), cudaMemcpyDeviceToDevice, rt.stream));
+        }
     p.bias_table = table;
+    p.char_of = lv.char_of; p.bias_cs = off; p.head_cs = lv.head_cs;
+    p.wxy_cs = 2 * ((mode == SM_BODY0 || mode == SM_FACE) ? lv.e_npad : plan.npad[0]);
     p.e_npad = lv.e_npad; p.e_pb = lv.e_pb; p.e_pb_ld = lv.e_pb_ld; p.e_wxy = lv.e_wxy;
     p.f_pb = lv.f_pb; p.f_pb_ld = lv.f_pb_ld; p.f_wxy = lv.f_wxy;
     p.base = base_grid_table(lv.R);
