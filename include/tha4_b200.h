@@ -58,6 +58,8 @@ const char* tha4_last_error(const tha4_ctx* ctx);
  *          "half_operands" (1: f16 conv operands, normalisations fused into the consumer conv's operand path),
  *          "halo_conv" (1: 3x3 stride-1 convs on the halo-reuse kernel), "tma_store" (1: unsplit conv epilogue through TMA stores),
  *          "halo_m256" (-1: automatic; 0 / 1: force 128- / 256-pixel tiles on the unsplit launches of the halo kernel),
+ *          "halo_ctas" (-1: automatic; 1 / 2: force one 288-thread / two 256-thread CTAs per SM for the halo kernel's
+ *                       256 x 64 and four-phase tiles),
  *          "cluster_splitk" (1: K-split convs reduce through a thread-block cluster / DSMEM; 0: workspace + reduce kernel),
  *          "pdl" (1: programmatic dependent launch), "tc_stride2" (1: 4x4 stride-2 convs on the wgmma kernel),
  *          "small_bn" (1: narrower N tiles for small unsplit launches), "siren_tc" (1: students on the wgmma kernels; 0: mma.sync kernels),

@@ -1,18 +1,20 @@
 """Developer measurement of the 3x3 halo convolution in the teacher_b1 frame (not a pytest file).
 
 1. The card's name and power limit.
-2. One warm teacher_b1 frame (mode_07, batch 1, eyebrow cache hot) under torch.profiler with CUDA activities, once with
-   128-pixel halo tiles forced (option halo_m256 = 0) and once with the automatic choice: device time per kernel
-   instantiation, and the share of the unsplit halo launches.
+2. One warm teacher_b1 frame (mode_07, batch 1, eyebrow cache hot) under torch.profiler with CUDA activities, with
+   128-pixel halo tiles forced (option halo_m256 = 0), with one CTA per SM forced for the 256 x 64 and four-phase tiles
+   (halo_ctas = 1), and with the automatic choice: device time per kernel instantiation, and the share of the unsplit
+   halo launches.
 3. Every unsplit 3x3 halo conv shape of that frame (read from the library's launch log, THA4_HALO_DEBUG=2, in a child
    process) timed alone with CUDA events over --reps launches after warm-up, with 128- and with 256-pixel tiles:
    microseconds, TFLOP/s, and the compulsory HBM bytes computed from the shape (f16 input, f16 weights, the fp32 and f16
-   outputs, the fp32 residual).  The conv runs through the kernel-level test hook with the frame's input-normalisation
+   outputs, the fp32 residual).  The 256-pixel tiles run with one and with two CTAs per SM (halo_ctas = 1 / 2; the
+   same kernel where the tile is not 256 x 64).  The conv runs through the kernel-level test hook with the frame's input-normalisation
    kind and residual; the hook always writes both outputs.
 4. Every four-phase shape of the teacher frame (nearest-x2 + 3x3 of the up-sampling ResBlocks, transposed 4x4 convs),
    and two at batch 32, timed the same way on three paths: conv_tc.cu's automatic plan (halo_conv = 0), the four-phase
-   halo kernel (halo_conv = 1, an unsplit launch requested) and the automatic choice; TFLOP/s count the executed
-   products (4 phases x 4 taps per low-resolution pixel).
+   halo kernel (halo_conv = 1, an unsplit launch requested) with one and with two CTAs per SM (halo_ctas = 1 / 2), and
+   the automatic choice; TFLOP/s count the executed products (4 phases x 4 taps per low-resolution pixel).
 
 Usage: python scripts/dev/halo_layers.py [--reps 200] [--out DIR] [--phase-only]
 """
@@ -30,7 +32,7 @@ sys.path.insert(0, _ROOT)
 sys.path.insert(0, os.path.join(_ROOT, 'tests'))
 
 LAUNCH_RE = re.compile(r'halo launch: N (\d+) (\d+)x(\d+) cin (\d+) cout (\d+) \| bn (\d+) cs (\d+) wg (\d+) chunks (\d+) grid (\d+) x (\d+) \| '
-                       r'xf (\d+) groups (\d+) act (\d+) res (\d+) out32 (\d+) out16 (\d+) st_tma (\d+) \| phases (\d+)')
+                       r'xf (\d+) groups (\d+) act (\d+) res (\d+) out32 (\d+) out16 (\d+) st_tma (\d+) \| phases (\d+) ctas (\d+)')
 
 
 def card():
@@ -72,15 +74,17 @@ def frame_shapes():
     if r.returncode != 0:
         raise RuntimeError('launch-log run failed:\n' + r.stderr[-4000:])
     keys = ('N', 'H', 'W', 'cin', 'cout', 'bn', 'cs', 'wg', 'chunks', 'grid_m', 'grid_n', 'xf', 'groups', 'act', 'res', 'out32', 'out16', 'st_tma',
-            'phases')
+            'phases', 'ctas')
     log = r.stderr.split('SECOND FRAME', 1)[1]
     return [dict(zip(keys, map(int, m.groups()))) for m in LAUNCH_RE.finditer(log)]
 
 
-def profile_frame(poser, image, poses, m256, out_dir):
+def profile_frame(poser, image, poses, options, out_dir):
+    """options: {name: value} set for the frame and reset to -1 (automatic) afterwards."""
     from torch.profiler import ProfilerActivity, profile
     ctx = poser.get_context()
-    ctx.set_option('halo_m256', m256)
+    for k, v in options.items():
+        ctx.set_option(k, v)
     ctx.set_option('cuda_graphs', 0)          # one kernel record per launch
     with torch.no_grad():
         for i in range(3):
@@ -90,9 +94,11 @@ def profile_frame(poser, image, poses, m256, out_dir):
             poser.get_posing_outputs(image, poses[3:4])
             torch.cuda.synchronize()
     ctx.set_option('cuda_graphs', 1)
-    ctx.set_option('halo_m256', -1)
+    for k in options:
+        ctx.set_option(k, -1)
     if out_dir:
-        prof.export_chrome_trace(os.path.join(out_dir, 'halo_layers_m256_%d.pt.trace.json' % m256))
+        tag = '_'.join('%s_%d' % kv for kv in options.items()) or 'auto'
+        prof.export_chrome_trace(os.path.join(out_dir, 'halo_layers_%s.pt.trace.json' % tag))
     per = collections.OrderedDict()
     for ev in prof.events():
         if ev.device_type.name != 'CUDA':
@@ -108,8 +114,8 @@ def short(name):
 
 
 def halo_split(name):
-    """conv_halo_kernel<BN, SA, SB, CS, OP, XF, WG, PH>: returns (CS, WG) or None."""
-    m = re.search(r'conv_halo_kernel<(\d+), (\d+), (\d+), (\d+), (\d+), (\d+), (\d+), (\d+)>', name)
+    """conv_halo_kernel<BN, SA, SB, CS, OP, XF, WG, PH, CTAS>: returns (CS, WG) or None."""
+    m = re.search(r'conv_halo_kernel<(\d+), (\d+), (\d+), (\d+), (\d+), (\d+), (\d+), (\d+), (\d+)>', name)
     return (int(m.group(4)), int(m.group(7))) if m else None
 
 
@@ -144,8 +150,9 @@ def shape_ab(shapes, reps):
         us = {}
         outs = {}
         try:
-            for m in (0, 1):
-                c.set_option('halo_m256', m)
+            for m, (m256, ctas) in enumerate(((0, -1), (1, 1), (1, 2))):      # 128-pixel tiles; 256-pixel, 1 / 2 CTAs per SM
+                c.set_option('halo_m256', m256)
+                c.set_option('halo_ctas', ctas)
                 H.conv_norm_ex(**inp, reps=20)                        # warm-up
                 y, y16, st, us[m] = H.conv_norm_ex(**inp, reps=reps)
                 outs[m] = (y, y16)
@@ -154,19 +161,22 @@ def shape_ab(shapes, reps):
             continue
         finally:
             c.set_option('halo_m256', -1)
-        same = torch.equal(outs[0][0], outs[1][0]) and torch.equal(outs[0][1], outs[1][1])
+            c.set_option('halo_ctas', -1)
+        same = all(torch.equal(outs[0][i], outs[m][i]) for m in (1, 2) for i in (0, 1))
         flop = 2.0 * s['N'] * s['H'] * s['W'] * s['cin'] * s['cout'] * 9
         px = s['N'] * s['H'] * s['W']
         hbm = px * s['cin'] * 2 + 9 * s['cin'] * s['cout'] * 2 + px * s['cout'] * (4 + 2) + (px * s['cout'] * 4 if s['res'] == 1 else 0)
         rows.append((s, count, us, flop, hbm, same))
     print('\n== unsplit halo shapes of the frame, alone: %d launches each after warm-up (CUDA events)' % reps)
-    print('  %-26s %3s %4s %6s | %9s %7s %6s | %9s %7s %6s | %6s %s' % ('N HxW cin->cout', 'n', 'bn', 'tiles', 'M128 us', 'TFLOP/s', 'GB/s',
-                                                                  'M256 us', 'TFLOP/s', 'GB/s', 'ratio', 'bit-identical'))
+    print('  %-26s %3s %4s %6s | %9s %7s | %9s %7s %6s | %9s %7s %6s | %6s %s' % (
+        'N HxW cin->cout', 'n', 'bn', 'tiles', 'M128 us', 'TFLOP/s', 'M256x1 us', 'TFLOP/s', 'GB/s', 'M256x2 us', 'TFLOP/s', 'GB/s',
+        'x1/x2', 'bit-identical'))
     for s, count, us, flop, hbm, same in rows:
         tiles = s['grid_m'] * s['grid_n'] * (2 if s['wg'] == 2 else 1)
-        print('  %-26s %3d %4d %6d | %9.2f %7.1f %6.0f | %9.2f %7.1f %6.0f | %6.3f %s' % (
+        print('  %-26s %3d %4d %6d | %9.2f %7.1f | %9.2f %7.1f %6.0f | %9.2f %7.1f %6.0f | %6.3f %s' % (
             '%d %dx%d %d->%d xf%d' % (s['N'], s['H'], s['W'], s['cin'], s['cout'], s['xf']), count, s['bn'], tiles,
-            us[0], flop / us[0] / 1e6, hbm / us[0] / 1e3, us[1], flop / us[1] / 1e6, hbm / us[1] / 1e3, us[0] / us[1], same))
+            us[0], flop / us[0] / 1e6, us[1], flop / us[1] / 1e6, hbm / us[1] / 1e3, us[2], flop / us[2] / 1e6, hbm / us[2] / 1e3,
+            us[1] / us[2], same))
     return rows
 
 
@@ -174,9 +184,9 @@ def phase_ab(reps):
     import test_gpu_halo_phase as P
     c = __import__('gpu_util').ctx()
     shapes = [s for s in P.CASES if s[1] == 32 or P.CASES.index(s) < 11]
-    paths = (('conv_tc', 0, 0), ('halo', 1, 1), ('auto', 1, 0))          # (label, halo_conv, ksplit)
+    paths = (('conv_tc', 0, 0, -1), ('halo x1', 1, 1, 1), ('halo x2', 1, 1, 2), ('auto', 1, 0, -1))   # (label, halo_conv, ksplit, halo_ctas)
     print('\n== four-phase shapes, alone: %d launches each after warm-up (CUDA events); executed TFLOP/s' % reps)
-    print('  %-4s %-24s | %s' % ('kind', 'N HxW cin->cout norm', ' | '.join('%9s %7s' % (p[0] + ' us', 'TFLOP/s') for p in paths)) + ' | ratio')
+    print('  %-4s %-24s | %s' % ('kind', 'N HxW cin->cout norm', ' | '.join('%10s %7s' % (p[0] + ' us', 'TFLOP/s') for p in paths)) + ' | x1/x2')
     rows = []
     for s in shapes:
         kind, N, Cin, H, W, Cout, norm = s
@@ -184,15 +194,17 @@ def phase_ab(reps):
         flop = 2.0 * N * H * W * 16 * Cin * Cout
         us = {}
         try:
-            for label, halo, ksplit in paths:
+            for label, halo, ksplit, ctas in paths:
                 c.set_option('halo_conv', halo)
+                c.set_option('halo_ctas', ctas)
                 P.conv_phase(**inp, ksplit=ksplit, reps=20)                  # warm-up
                 us[label] = P.conv_phase(**inp, ksplit=ksplit, reps=reps)[3]
         finally:
             c.set_option('halo_conv', 1)
+            c.set_option('halo_ctas', -1)
         rows.append((s, us))
         print('  %-4d %-24s | %s | %6.3f' % (kind, '%d %dx%d %d->%d %s' % (N, H, W, Cin, Cout, norm), ' | '.join(
-            '%9.2f %7.1f' % (us[p[0]], flop / us[p[0]] / 1e6) for p in paths), us['conv_tc'] / us['halo']), flush=True)
+            '%10.2f %7.1f' % (us[p[0]], flop / us[p[0]] / 1e6) for p in paths), us['halo x1'] / us['halo x2']), flush=True)
     return rows
 
 
@@ -212,9 +224,11 @@ def main():
     shapes = frame_shapes()
     print('halo launches in the frame: %d (%d unsplit)' % (len(shapes), sum(1 for s in shapes if s['cs'] == 1)), flush=True)
     poser, image, poses = make_teacher()
-    before = print_frame('128-pixel tiles (halo_m256 = 0)', profile_frame(poser, image, poses, 0, args.out))
-    after = print_frame('automatic tile choice (halo_m256 = -1)', profile_frame(poser, image, poses, -1, args.out))
-    print('kernel time per frame: %.1f -> %.1f us (%.3fx)' % (before[0], after[0], before[0] / after[0]), flush=True)
+    m128 = print_frame('128-pixel tiles (halo_m256 = 0)', profile_frame(poser, image, poses, {'halo_m256': 0}, args.out))
+    one = print_frame('one CTA per SM (halo_ctas = 1)', profile_frame(poser, image, poses, {'halo_ctas': 1}, args.out))
+    auto = print_frame('automatic choice', profile_frame(poser, image, poses, {}, args.out))
+    print('kernel time per frame: 128-pixel tiles %.1f us, one CTA per SM %.1f us, automatic %.1f us (%.3fx over one CTA per SM)'
+          % (m128[0], one[0], auto[0], one[0] / auto[0]), flush=True)
     shape_ab(shapes, args.reps)
     phase_ab(args.reps)
 

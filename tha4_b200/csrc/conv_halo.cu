@@ -42,7 +42,8 @@ constexpr int HALO_W = HT_W + 2;
 __host__ __device__ constexpr int halo_h(int wg) { return HT_H * wg + 2; }                  // 18 / 34
 __host__ __device__ constexpr int halo_rows(int wg) { return HALO_W * halo_h(wg); }         // 180 / 340 pixel rows
 __host__ __device__ constexpr int halo_a_bytes(int rowb, int wg) { return ((halo_rows(wg) * rowb + 1023) / 1024) * 1024; }
-__host__ __device__ constexpr int halo_threads(int wg) { return 128 * wg + 32; }           // + the TMA producer warp
+// + the TMA producer warp, except in the two-warpgroup CTAs built to run two per SM (ctas = 2, see conv_halo_kernel)
+__host__ __device__ constexpr int halo_threads(int wg, int ctas = 1) { return 128 * wg + (ctas == 2 ? 0 : 32); }
 // warpgroup 1 reads the halo 16 pixel rows (160 halo rows) further on: a multiple of 1024 bytes at both row widths, so
 // its descriptors see the same swizzle phase as warpgroup 0's
 static_assert((HT_H * HALO_W * 64) % 1024 == 0, "second warpgroup's halo offset keeps the swizzle phase");
@@ -53,9 +54,10 @@ static_assert((HT_H * HALO_W * 64) % 1024 == 0, "second warpgroup's halo offset 
 // rings fit four times: the layers at 256x256 / 512x512 are chains of dependent latencies, more CTAs = more overlap).
 // Two-warpgroup CTAs (BN <= 64): two with BN = 32, as many consumer warps per SM as four one-warpgroup CTAs; one with
 // BN = 64 (two would cap the 288 threads at 96 registers, which spills the 64-column accumulator's epilogue).  Four-phase
-// CTAs (two 32-column accumulators per warpgroup) count as BN = 64.
-__host__ __device__ constexpr int halo_min_ctas(int bn, int sa, int cs, int op, int wg, int ph = 1) {
-    return wg > 1 ? (bn * (ph == 4 ? 2 : 1) <= 32 ? 2 : 1) : cs > 1 || bn >= 128 ? 1 : ((sa == (op == OP_F16N ? 2 : 1) && bn <= 32) ? 4 : 2);
+// CTAs (two 32-column accumulators per warpgroup) count as BN = 64.  ctas = 2: the 256-thread variant of those two, without
+// the producer warp: 2 x 8 warps put 4 warps on each SM sub-partition, and each thread keeps 128 registers.
+__host__ __device__ constexpr int halo_min_ctas(int bn, int sa, int cs, int op, int wg, int ph = 1, int ctas = 1) {
+    return ctas == 2 ? 2 : wg > 1 ? (bn * (ph == 4 ? 2 : 1) <= 32 ? 2 : 1) : cs > 1 || bn >= 128 ? 1 : ((sa == (op == OP_F16N ? 2 : 1) && bn <= 32) ? 4 : 2);
 }
 // Weight tile j of a channel chunk, as the third coordinate of the [phase * tap][cout][cin] weight map.  3x3: tap j.
 // Four phases: j = 2 (2 tap + px) + py, so the tiles of the two warpgroups (py) alternate in the ring.
@@ -64,8 +66,12 @@ __host__ __device__ constexpr int halo_wtile(int j) { return PH == 1 ? j : ((j &
 
 // WG: consumer warpgroups (1: 128-pixel tiles, 160 threads; 2: 256-pixel tiles, 288 threads, unsplit only)
 // PH: output phases (1: 3x3; 4: four-phase layers, two warpgroups on one 8 x 16 low-resolution tile, unsplit only)
-template <int BN, int SA, int SB, int CS, int OP, int XF, int WG, int PH = 1>
-__global__ void __launch_bounds__(halo_threads(WG), halo_min_ctas(BN, SA, CS, OP, WG, PH)) conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+// CTAS: resident CTAs per SM a two-warpgroup CTA is built for.  1: a TMA producer warp (288 threads, one CTA per SM for
+// 256 x 64 and four-phase tiles).  2: no producer warp (256 threads, two CTAs per SM with rings of at most ~113 KB): thread
+// 0 of the consumers issues the loads from inside the MMA loop, and while one CTA transforms a chunk, starts up or drains
+// its accumulator, the other one's MMAs keep the tensor pipe busy.
+template <int BN, int SA, int SB, int CS, int OP, int XF, int WG, int PH = 1, int CTAS = 1>
+__global__ void __launch_bounds__(halo_threads(WG, CTAS), halo_min_ctas(BN, SA, CS, OP, WG, PH, CTAS)) conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                                                                 const __grid_constant__ CUtensorMap tmO32, const __grid_constant__ CUtensorMap tmO16,
                                                                 const __grid_constant__ CUtensorMap tmR, const TcParams p) {
     static_assert(OP != OP_TF32, "halo kernel: f16 operands");
@@ -73,6 +79,11 @@ __global__ void __launch_bounds__(halo_threads(WG), halo_min_ctas(BN, SA, CS, OP
     static_assert(WG == 1 || (WG == 2 && CS == 1 && BN <= 64), "two consumer warpgroups: unsplit launches, two accumulators of at most 64 columns");
     // four phases: two 128-row accumulators per warpgroup, no more registers than one 128 x 64 accumulator
     static_assert(PH == 1 || (PH == 4 && WG == 2 && BN <= 32), "four-phase layers: two warpgroups, two 128 x 32 accumulators each");
+    constexpr bool SELF_LOAD = CTAS == 2;                                // consumer thread 0 issues the TMA loads
+    static_assert(CTAS == 1 || (CTAS == 2 && WG == 2), "two CTAs per SM: the two-warpgroup tiles");
+    // in-loop loads (below): at step i thread 0 issues the weight tiles up to i + SB - 2 (four phases: 2 i + SB - 3), and the
+    // tiles of step i + 1 must be out before thread 0 waits for them
+    static_assert(!SELF_LOAD || SB >= (PH == 1 ? 3 : 6), "weight ring too shallow for loads issued by a consumer");
     constexpr int SLABS = PH == 1 ? WG : 1;                              // 16-row slabs of the tile (8 x 16 pixels each)
     constexpr int NACC = PH == 1 ? 1 : 2;                                // accumulators per warpgroup
     constexpr int TPC = PH == 1 ? 9 : 16;                                // weight tiles per channel chunk
@@ -97,9 +108,15 @@ __global__ void __launch_bounds__(halo_threads(WG), halo_min_ctas(BN, SA, CS, OP
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // developer timing: CTA `slot` of every 97 records clock64 at its phase boundaries (8 stamps per role: dbg[slot][role][8])
-    const bool dbg_on = p.dbg != nullptr && (blockIdx.x % 97) == 0 && blockIdx.y == 0 && (blockIdx.x / 97) * CS + blockIdx.z < 32;
-    long long* dbg = dbg_on ? p.dbg + ((blockIdx.x / 97) * CS + blockIdx.z) * 32 : nullptr;
-#define HSTAMP(role, i) do { if (dbg) dbg[(role) * 8 + (i)] = clock64(); } while (0)
+    auto dbg_slot = [&]() -> long long* {
+        const bool dbg_on = p.dbg != nullptr && (blockIdx.x % 97) == 0 && blockIdx.y == 0 && (blockIdx.x / 97) * CS + blockIdx.z < 32;
+        return dbg_on ? p.dbg + ((blockIdx.x / 97) * CS + blockIdx.z) * 32 : nullptr;
+    };
+    // the two-CTA variant recomputes the slot at each stamp and has none from the MMA loop on: with 128 registers, a
+    // pointer held through the loop and the epilogue costs it a spill
+    long long* dbg = SELF_LOAD ? nullptr : dbg_slot();
+#define HSTAMP(role, i) do { long long* d_ = SELF_LOAD ? dbg_slot() : dbg; if (d_) d_[(role) * 8 + (i)] = clock64(); } while (0)
+#define HSTAMP_END(role, i) do { if (!SELF_LOAD) HSTAMP(role, i); } while (0)
     if (threadIdx.x == 0) HSTAMP(0, 0);
     int tile = blockIdx.x;
     const int tx = tile % p.tiles_x; tile /= p.tiles_x;
@@ -128,7 +145,7 @@ __global__ void __launch_bounds__(halo_threads(WG), halo_min_ctas(BN, SA, CS, OP
     pdl_trigger();
     // weight tiles of the first ring pass do not depend on the previous kernel: fetch them ahead of the dependency wait
     const int npre = p.pre_b ? min(nb, SB) : 0;
-    if (warp == PRODUCER_WARP && lane == 0) {
+    if (SELF_LOAD ? threadIdx.x == 0 : (warp == PRODUCER_WARP && lane == 0)) {
         for (int i = 0; i < npre; ++i) {
             const uint32_t full = smem_u32(b_full + i);
             mbar_expect_tx(full, B_BYTES);
@@ -140,7 +157,7 @@ __global__ void __launch_bounds__(halo_threads(WG), halo_min_ctas(BN, SA, CS, OP
 
     Acc<BN> acc[NACC];
     if (nc > 0) {
-        if (warp == PRODUCER_WARP) {
+        if (!SELF_LOAD && warp == PRODUCER_WARP) {
             if (lane == 0) {   // ===== TMA producer: one halo box per chunk, nine (four-phase: sixteen) weight tiles per chunk =====
                 int bi = 0;
                 for (int ci = 0; ci < nc; ++ci) {
@@ -167,16 +184,46 @@ __global__ void __launch_bounds__(halo_threads(WG), halo_min_ctas(BN, SA, CS, OP
             __half* hA = reinterpret_cast<__half*>(xf_A);
             __half* hB = hA + p.xf_C;
             const bool silu = p.xf_act == ACT_SILU || p.xf_act == ACT_SILU_FAST;
+            // SELF_LOAD: thread 0 (warpgroup 0) issues every TMA load, in consumption order.  Weight tile j + SB goes out
+            // once stage j % SB has been released by both warpgroups, the halo of chunk ci + SA once both have finished
+            // chunk ci.  Why no wait can be circular: at MMA step i (its own tile of step i committed), thread 0 waits only
+            // for releases the other warpgroup makes at its steps < i -- the tiles of step i - 2 -- and, after the last step
+            // of a chunk, for the other warpgroup's end of that same chunk.  For that, the other warpgroup needs the weight
+            // tiles of its steps <= i and the chunk's halo.  The tiles of step i + 1 go out at thread 0's step i, before
+            // either wait (3x3: tiles up to i + SB - 2, SB >= 3; four phases, two tiles per step: up to 2 i + SB - 3,
+            // SB >= 6); the halo at the end of an earlier chunk or before the loop.  The other warpgroup's only other wait
+            // is the transform barrier of a chunk, which thread 0 has passed.
+            auto load_b = [&](int j) {                           // weight tile j (those of the first ring pass go out before the loop)
+                if (j < SB || j >= nb) return;
+                const int sb = j % SB;
+                mbar_wait(smem_u32(b_empty + sb), ((j / SB) & 1) ^ 1);
+                mbar_expect_tx(smem_u32(b_full + sb), B_BYTES);
+                tma_load_3d(smem_u32(smB + sb * B_BYTES), &tmB, (cb0 + j / TPC) * KCE, n0, halo_wtile<PH>(j % TPC), smem_u32(b_full + sb));
+            };
+            auto load_a = [&](int ci) {                          // the halo of chunk ci
+                if (ci >= nc) return;
+                const int sa = ci % SA;
+                mbar_wait(smem_u32(a_empty + sa), ((ci / SA) & 1) ^ 1);
+                mbar_expect_tx(smem_u32(a_full + sa), HALO_ROWS * ROWB);
+                tma_load_4d(smem_u32(smA + sa * A_BYTES), &tmA, (cb0 + ci) * KCE, x0 - 1, y0 - 1, n, smem_u32(a_full + sa));
+            };
+            if (SELF_LOAD && te == 0) {                          // the first ring pass: nothing to wait for
+                for (int ci = 0; ci < SA; ++ci) load_a(ci);
+                for (int j = npre; j < min(nb, SB); ++j) {
+                    mbar_expect_tx(smem_u32(b_full + j), B_BYTES);
+                    tma_load_3d(smem_u32(smB + j * B_BYTES), &tmB, (cb0 + j / TPC) * KCE, n0, halo_wtile<PH>(j % TPC), smem_u32(b_full + j));
+                }
+            }
             if (XF) {
                 double2* chs = reinterpret_cast<double2*>(xf_A + 2 * p.xf_C);
                 xf_build_coef<128 * WG, XBAR>(p, n, te, hA, hB, chs, cb0 * KCE, (cb0 + nc) * KCE);
-                if (te == 0) HSTAMP(2, 0);
+                if (te == 0) HSTAMP_END(2, 0);
             }
             int bi = 0;
             for (int ci = 0; ci < nc; ++ci) {
                 const int sa = ci % SA;
                 mbar_wait(smem_u32(a_full + sa), (ci / SA) & 1);
-                if (te == 0 && ci == 0) HSTAMP(2, 1);
+                if (te == 0 && ci == 0) HSTAMP_END(2, 1);
                 if (XF) {
                     const int c0 = (cb0 + ci) * KCE;
                     // items = (halo row, half row): 360 / 680 items over 128 / 256 threads; the rows both warpgroups read
@@ -192,7 +239,7 @@ __global__ void __launch_bounds__(halo_threads(WG), halo_min_ctas(BN, SA, CS, OP
                     }
                     asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");   // generic-proxy writes -> wgmma's async-proxy reads
                     asm volatile("bar.sync %0, %1;\n" :: "n"(XBAR), "n"(128 * WG) : "memory");
-                    if (te == 0 && ci == nc - 1) HSTAMP(2, 2);
+                    if (te == 0 && ci == nc - 1) HSTAMP_END(2, 2);
                 }
                 const uint32_t a_base = smem_u32(smA + sa * A_BYTES) + (uint32_t)(SLABS > 1 ? wg * HT_H * HALO_W * ROWB : 0);
                 if constexpr (PH == 4) {
@@ -225,6 +272,11 @@ __global__ void __launch_bounds__(halo_threads(WG), halo_min_ctas(BN, SA, CS, OP
                             mbar_arrive(smem_u32(b_empty + sb));
                             mbar_arrive(smem_u32(a_empty + sa));
                         }
+                        if (SELF_LOAD && te == 0) {             // tiles up to bj - 3 (warpgroup 1's, step s - 2) are released
+                            load_b(bj + SB - 4);
+                            load_b(bj + SB - 3);
+                            if (s == 7) load_a(ci + SA);
+                        }
                     }
                 } else {
                     // unrolled: the wait depth and the arrivals below depend on the tap only, so no branch separates wgmma issue
@@ -255,12 +307,16 @@ __global__ void __launch_bounds__(halo_threads(WG), halo_min_ctas(BN, SA, CS, OP
                             mbar_arrive(smem_u32(b_empty + bi % SB));
                             mbar_arrive(smem_u32(a_empty + sa));
                         }
+                        if (SELF_LOAD && te == 0) {             // tiles up to bi - 2 are released
+                            load_b(bi + SB - 2);
+                            if (tap == 8) load_a(ci + SA);
+                        }
                     }
                 }
             }
 #pragma unroll
             for (int a = 0; a < NACC; ++a) { wg_fence_acc(acc[a].d[0]); wg_fence_acc(acc[a].d[1]); }
-            if (te == 0) { HSTAMP(1, 1); HSTAMP(2, 3); }
+            if (te == 0) { HSTAMP_END(1, 1); HSTAMP_END(2, 3); }
             // the epilogue reuses the ring: with two warpgroups, the other one may still be reading its last stages
             if constexpr (WG > 1) asm volatile("bar.sync 3, 256;\n" ::: "memory");
             if constexpr (PH == 4) {
@@ -276,7 +332,7 @@ __global__ void __launch_bounds__(halo_threads(WG), halo_min_ctas(BN, SA, CS, OP
                 epi_direct<BN, HT_W, NSLOT, WG>(p, acc[0], smem + wg * EPI_BYTES, n, y0 + wg * HT_H, x0, n0, 0, 0, warp, lane,
                                                 &tmO32, &tmO16, &tmR, res_bars + 4 * wg, wg, EPI_BYTES);
             }
-            if (te == 0) HSTAMP(2, 4);
+            if (te == 0) HSTAMP_END(2, 4);
         }
     }
     if (CS > 1) {
@@ -293,7 +349,8 @@ __global__ void __launch_bounds__(halo_threads(WG), halo_min_ctas(BN, SA, CS, OP
         if (threadIdx.x == 0) HSTAMP(2, 6);
     }
     __syncthreads();
-    if (threadIdx.x == 0) HSTAMP(0, 3);
+    if (threadIdx.x == 0) HSTAMP_END(0, 3);
+#undef HSTAMP_END
 #undef HSTAMP
 }
 
@@ -376,9 +433,45 @@ bool halo_store_map(const View& v, bool f16, const CUtensorMap** out) {
 }
 
 int g_halo_m256 = -1;         // option "halo_m256": -1 automatic, 0 / 1 force 128- / 256-pixel tiles on unsplit launches
+int g_halo_ctas = -1;         // option "halo_ctas": -1 automatic, 1 / 2 force the 288- / 256-thread two-warpgroup CTAs
+
+// Shared memory of a CTA: the rings, the barriers, the alignment slack (the XF table comes on top)
+constexpr size_t halo_ring(int op, int bn, int sa, int sb, int wg, int ph) {
+    return (size_t)sa * halo_a_bytes(op_row_bytes(op), ph == 1 ? wg : 1) + (size_t)sb * bn * op_row_bytes(op);
+}
+constexpr size_t halo_smem0(int op, int bn, int sa, int sb, int wg, int ph) {
+    return 1024 + halo_ring(op, bn, sa, sb, wg, ph) + (2 * sa + 2 * sb + 4 * wg) * 8 + 16;
+}
 
 // wg: consumer warpgroups per CTA (1: 128-pixel tiles; 2: 256-pixel tiles, unsplit launches only)
-struct HaloPlan { int bn, tiles_x, tiles_y, tiles_m, tiles_n, cs, chunks, wg; };
+// ctas: resident CTAs per SM of a two-warpgroup launch with 256 x 64 or four-phase tiles (conv_halo_kernel's CTAS)
+struct HaloPlan { int bn, tiles_x, tiles_y, tiles_m, tiles_n, cs, chunks, wg, ctas; };
+
+// Weight stages of a two-warpgroup CTA: at least sb_min, and enough that each warpgroup's half of the idle ring holds the
+// epilogue scratch and one TMA-store staging slot.
+constexpr int halo_sb_wg2(int op, int bn, int sa, int sb_min) {
+    const size_t a = (size_t)sa * halo_a_bytes(op_row_bytes(op), 2), b = (size_t)bn * op_row_bytes(op);
+    int sb = sb_min;
+    while (a + sb * b < 2 * (size_t)(epi_slot0(bn) + EPI_SLOT_BYTES)) ++sb;
+    return sb;
+}
+// Rings of the 256-thread CTAs, two per SM (<= ~113 KB each with the XF table of up to 512 channels).  256 x 64 tiles: one
+// halo stage of 64-channel chunks and six weight stages (two halo stages of 32-channel chunks, and the weight stages the
+// epilogue needs); four phases: two halo stages and twelve 32-column weight tiles, three quarters of a chunk.
+constexpr int halo2_sa(int op, int ph) { return ph == 4 || op == OP_F16N ? 2 : 1; }
+constexpr int halo2_sb(int op, int ph) { return ph == 4 ? 12 : halo_sb_wg2(op, 64, halo2_sa(op, ph), op == OP_F16N ? 12 : 6); }
+
+// Two-warpgroup launches with 256 x 64 or four-phase tiles run two 256-thread CTAs per SM when there are more CTAs than
+// SMs and two fit in shared memory (228 KB per SM on sm_90, 1 KB of it reserved per CTA).  With one CTA per SM, each SM
+// runs a CTA's start-up, its chunks' operand transforms and its epilogue with the tensor pipe idle; a second CTA's MMAs
+// fill those gaps.  Measured alone on an H100 SXM (700 W), every such layer of the teacher frame with 144 - 1024 CTAs ran
+// 1.04 - 1.18x faster on two CTAs per SM; with at most one CTA per SM (32 - 128 CTAs) nothing overlaps, and the
+// shallower rings made the same layers 1.2 - 1.8x slower.
+int halo_plan_ctas(int op, int bn, int ph, long ctas, const ConvArgs& a) {
+    if (g_halo_ctas > 0) return g_halo_ctas;
+    const size_t smem = halo_smem0(op, bn, halo2_sa(op, ph), halo2_sb(op, ph), 2, ph) + (a.nin.on ? (size_t)24 * a.nin.C + 32 : 0);
+    return ctas > num_sms() && 2 * (smem + 1024) <= (size_t)228 * 1024 ? 2 : 1;
+}
 
 HaloPlan halo_plan(const ConvWeights& cw, const ConvArgs& a, int op) {
     HaloPlan pl;
@@ -388,6 +481,7 @@ HaloPlan halo_plan(const ConvWeights& cw, const ConvArgs& a, int op) {
         pl.tiles_x = ceil_div(a.in.W, HT_W); pl.tiles_y = ceil_div(a.in.H, HT_H);
         pl.tiles_m = pl.tiles_x * pl.tiles_y * a.in.N;
         pl.bn = 32; pl.tiles_n = cw.cout_pad / 32; pl.cs = 1; pl.wg = 2;
+        pl.ctas = halo_plan_ctas(op, 32, 4, (long)pl.tiles_m * pl.tiles_n, a);
         return pl;
     }
     pl.tiles_x = ceil_div(a.out.W, HT_W); pl.tiles_y = ceil_div(a.out.H, HT_H);
@@ -428,41 +522,40 @@ HaloPlan halo_plan(const ConvWeights& cw, const ConvArgs& a, int op) {
         pl.bn = std::min(pl.bn, 64);
         pl.tiles_n = cw.cout_pad / pl.bn;
     }
+    pl.ctas = pl.wg == 2 && pl.bn == 64 ? halo_plan_ctas(op, 64, 1, (long)pl.tiles_m * pl.tiles_n, a) : 1;
     return pl;
 }
 
-template <int OP, int BN, int SA, int SB, int CS, int XF, int WG = 1, int PH = 1>
+template <int OP, int BN, int SA, int SB, int CS, int XF, int WG = 1, int PH = 1, int CTAS = 1>
 void launch_halo(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo32, const CUtensorMap& mo16, const CUtensorMap& mr, const TcParams& p, dim3 grid, cudaStream_t s) {
-    constexpr int ROWB = op_row_bytes(OP);
-    constexpr size_t ring = (size_t)SA * halo_a_bytes(ROWB, PH == 1 ? WG : 1) + (size_t)SB * BN * ROWB;
-    constexpr size_t smem0 = 1024 + ring + (2 * SA + 2 * SB + 4 * WG) * 8 + 16;
+    constexpr size_t ring = halo_ring(OP, BN, SA, SB, WG, PH);
+    constexpr size_t smem0 = halo_smem0(OP, BN, SA, SB, WG, PH);
     static_assert(smem0 <= 227 * 1024, "shared memory budget");
     static_assert(ring / WG >= (size_t)4 * 32 * 33 * 4 + 4 * BN * 8, "epilogue scratch must fit in the pipeline buffers");
     static_assert(WG == 1 || PH == 4 || epi_nslot(BN, (ring / WG) & ~(size_t)1023) > 0, "two warpgroups: a TMA-store staging slot each");
     static_assert(CS == 1 || ring >= (size_t)128 * BN * 4 + 128 * 8 * 4 + 128 * 4 * 4, "partial tile + statistics scratch must fit");
+    static_assert(CTAS == 1 || 2 * (smem0 + 1024) <= 228 * 1024, "two CTAs per SM");
     const size_t smem = smem0 + (XF ? (size_t)24 * p.xf_C + 32 : 0);
     THA4_REQUIRE(smem <= 227 * 1024, "conv_halo: shared memory budget (fused input normalisation)");
-    THA4_ENSURE_SMEM((conv_halo_kernel<BN, SA, SB, CS, OP, XF, WG, PH>), smem);
-    launch_pdl(conv_halo_kernel<BN, SA, SB, CS, OP, XF, WG, PH>, grid, dim3(halo_threads(WG)), smem, s, CS, ma, mb, mo32, mo16, mr, p);
+    THA4_ENSURE_SMEM((conv_halo_kernel<BN, SA, SB, CS, OP, XF, WG, PH, CTAS>), smem);
+    launch_pdl(conv_halo_kernel<BN, SA, SB, CS, OP, XF, WG, PH, CTAS>, grid, dim3(halo_threads(WG, CTAS)), smem, s, CS, ma, mb, mo32, mo16, mr, p);
     THA4_LAUNCH_CHECK();
 }
 
 // SBD: weight-ring depth of the cluster split-K launches (few CTAs per SM, the ring is what hides the DRAM latency of weights
 // that are fetched ahead of the dependency wait); SBS: depth of the unsplit launches (many tiles: a shallow ring keeps
 // the CTA small so that 2 - 4 of them share an SM and overlap each other's load -> transform -> MMA -> drain chains).
-// Weight stages of a two-warpgroup CTA: at least sb_min, and enough that each warpgroup's half of the idle ring holds the
-// epilogue scratch and one TMA-store staging slot.
-constexpr int halo_sb_wg2(int op, int bn, int sa, int sb_min) {
-    const size_t a = (size_t)sa * halo_a_bytes(op_row_bytes(op), 2), b = (size_t)bn * op_row_bytes(op);
-    int sb = sb_min;
-    while (a + sb * b < 2 * (size_t)(epi_slot0(bn) + EPI_SLOT_BYTES)) ++sb;
-    return sb;
-}
-
 template <int OP, int BN, int SA, int SBD, int SBS, int XF>
-void launch_halo_cs(int cs, int wg, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo32, const CUtensorMap& mo16, const CUtensorMap& mr, const TcParams& p, dim3 grid, cudaStream_t s) {
+void launch_halo_cs(int cs, int wg, int ctas, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo32, const CUtensorMap& mo16, const CUtensorMap& mr, const TcParams& p, dim3 grid, cudaStream_t s) {
     constexpr int SA1 = OP == OP_F16N ? 2 : 1;
     THA4_REQUIRE(wg == 1 || (BN <= 64 && cs == 1), "conv_halo: 256-pixel tiles need an unsplit launch with N tiles of at most 64 columns");
+    THA4_REQUIRE(ctas == 1 || (wg == 2 && BN == 64), "conv_halo: two CTAs per SM are built for 256 x 64 tiles");
+    if constexpr (BN == 64) {
+        if (ctas == 2) {     // one chunk or several: the same rings
+            launch_halo<OP, 64, halo2_sa(OP, 1), halo2_sb(OP, 1), 1, XF, 2, 1, 2>(ma, mb, mo32, mo16, mr, p, grid, s);
+            return;
+        }
+    }
     if constexpr (BN <= 64) {
         if (cs == 1 && p.cpt == 1) {     // one chunk: one halo, ever -> a ring that fits four times per SM (twice with two warpgroups)
             if (wg == 2) launch_halo<OP, BN, SA1, halo_sb_wg2(OP, BN, SA1, BN == 64 ? SBD : SBS), 1, XF, 2>(ma, mb, mo32, mo16, mr, p, grid, s);
@@ -489,11 +582,11 @@ void launch_halo_cs(int cs, int wg, const CUtensorMap& ma, const CUtensorMap& mb
 }
 
 template <int OP, int XF>
-void launch_halo_bn(int bn, int cs, int wg, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo32, const CUtensorMap& mo16, const CUtensorMap& mr, const TcParams& p, dim3 grid, cudaStream_t s) {
+void launch_halo_bn(int bn, int cs, int wg, int ctas, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo32, const CUtensorMap& mo16, const CUtensorMap& mr, const TcParams& p, dim3 grid, cudaStream_t s) {
     constexpr int M = OP == OP_F16N ? 2 : 1;        // 64-byte rows: twice the stages for the same bytes in flight
-    if (bn == 128) launch_halo_cs<OP, 128, 2 * M, 6 * M, 3 * M, XF>(cs, wg, ma, mb, mo32, mo16, mr, p, grid, s);        // unsplit:  95 KB
-    else if (bn == 64) launch_halo_cs<OP, 64, 2 * M, 8 * M, 3 * M, XF>(cs, wg, ma, mb, mo32, mo16, mr, p, grid, s);     // unsplit:  71 KB
-    else launch_halo_cs<OP, 32, 2 * M, 9 * M, 5 * M, XF>(cs, wg, ma, mb, mo32, mo16, mr, p, grid, s);                    // unsplit:  67 KB
+    if (bn == 128) launch_halo_cs<OP, 128, 2 * M, 6 * M, 3 * M, XF>(cs, wg, ctas, ma, mb, mo32, mo16, mr, p, grid, s);        // unsplit:  95 KB
+    else if (bn == 64) launch_halo_cs<OP, 64, 2 * M, 8 * M, 3 * M, XF>(cs, wg, ctas, ma, mb, mo32, mo16, mr, p, grid, s);     // unsplit:  71 KB
+    else launch_halo_cs<OP, 32, 2 * M, 9 * M, 5 * M, XF>(cs, wg, ctas, ma, mb, mo32, mo16, mr, p, grid, s);                    // unsplit:  67 KB
 }
 
 bool g_use_halo = true;
@@ -504,6 +597,7 @@ bool g_tma_store = true;      // option "tma_store": unsplit epilogue through sh
 void conv_halo_enable(bool on) { g_use_halo = on; }
 void conv_halo_enable_tma_store(bool on) { g_tma_store = on; }
 void conv_halo_set_m256(int mode) { g_halo_m256 = mode; }
+void conv_halo_set_ctas(int mode) { g_halo_ctas = mode; }
 
 bool conv_halo_supported(const ConvWeights& cw, const ConvArgs& a) {
     if (!g_use_halo || !conv_tc_supported(cw, a)) return false;
@@ -588,21 +682,26 @@ void conv_halo_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s)
               (!a.res.p || ((reinterpret_cast<uintptr_t>(a.res.p) & 15) == 0 && a.res.ld % 4 == 0))) ? 1 : 0;
     dim3 grid(pl.tiles_m, pl.tiles_n, pl.cs);
     if (cw.nphase == 4) {
-        // OP_F16 (conv_halo_supported).  One CTA per SM: the ring takes two halo stages and a whole chunk of weight tiles
-        if (a.nin.on) launch_halo<OP_F16, 32, 2, 16, 1, 1, 2, 4>(ma, mb, *mo32, *mo16, *mr, p, grid, s);
+        // OP_F16 (conv_halo_supported).  One CTA per SM: the ring takes two halo stages and a whole chunk of weight tiles;
+        // two: see halo2_sb
+        constexpr int SA2 = halo2_sa(OP_F16, 4), SB2 = halo2_sb(OP_F16, 4);
+        if (pl.ctas == 2) {
+            if (a.nin.on) launch_halo<OP_F16, 32, SA2, SB2, 1, 1, 2, 4, 2>(ma, mb, *mo32, *mo16, *mr, p, grid, s);
+            else launch_halo<OP_F16, 32, SA2, SB2, 1, 0, 2, 4, 2>(ma, mb, *mo32, *mo16, *mr, p, grid, s);
+        } else if (a.nin.on) launch_halo<OP_F16, 32, 2, 16, 1, 1, 2, 4>(ma, mb, *mo32, *mo16, *mr, p, grid, s);
         else launch_halo<OP_F16, 32, 2, 16, 1, 0, 2, 4>(ma, mb, *mo32, *mo16, *mr, p, grid, s);
     } else if (op == OP_F16) {
-        if (a.nin.on) launch_halo_bn<OP_F16, 1>(pl.bn, pl.cs, pl.wg, ma, mb, *mo32, *mo16, *mr, p, grid, s);
-        else launch_halo_bn<OP_F16, 0>(pl.bn, pl.cs, pl.wg, ma, mb, *mo32, *mo16, *mr, p, grid, s);
+        if (a.nin.on) launch_halo_bn<OP_F16, 1>(pl.bn, pl.cs, pl.wg, pl.ctas, ma, mb, *mo32, *mo16, *mr, p, grid, s);
+        else launch_halo_bn<OP_F16, 0>(pl.bn, pl.cs, pl.wg, pl.ctas, ma, mb, *mo32, *mo16, *mr, p, grid, s);
     } else {
-        if (a.nin.on) launch_halo_bn<OP_F16N, 1>(pl.bn, pl.cs, pl.wg, ma, mb, *mo32, *mo16, *mr, p, grid, s);
-        else launch_halo_bn<OP_F16N, 0>(pl.bn, pl.cs, pl.wg, ma, mb, *mo32, *mo16, *mr, p, grid, s);
+        if (a.nin.on) launch_halo_bn<OP_F16N, 1>(pl.bn, pl.cs, pl.wg, pl.ctas, ma, mb, *mo32, *mo16, *mr, p, grid, s);
+        else launch_halo_bn<OP_F16N, 0>(pl.bn, pl.cs, pl.wg, pl.ctas, ma, mb, *mo32, *mo16, *mr, p, grid, s);
     }
     static const bool dbg_all = dbg_env && !strcmp(getenv("THA4_HALO_DEBUG"), "2");
     if (dbg_all) {       // developer: stamps of every launch of a real forward (serialises the stream)
-        fprintf(stderr, "halo launch: N %d %dx%d cin %d cout %d | bn %d cs %d wg %d chunks %d grid %d x %d | xf %d groups %d act %d res %d out32 %d out16 %d st_tma %d | phases %d\n",
+        fprintf(stderr, "halo launch: N %d %dx%d cin %d cout %d | bn %d cs %d wg %d chunks %d grid %d x %d | xf %d groups %d act %d res %d out32 %d out16 %d st_tma %d | phases %d ctas %d\n",
                 p.N, p.MH, p.MW, cw.cin, cw.cout, pl.bn, pl.cs, pl.wg, pl.chunks, pl.tiles_m, pl.tiles_n, a.nin.on ? 1 : 0, p.xf_groups, p.xf_act,
-                p.res_mode, p.out ? 1 : 0, p.out16 ? 1 : 0, p.st_tma, cw.nphase);
+                p.res_mode, p.out ? 1 : 0, p.out16 ? 1 : 0, p.st_tma, cw.nphase, pl.ctas);
         conv_halo_debug_dump();
     }
 }
