@@ -60,6 +60,9 @@ const char* tha4_last_error(const tha4_ctx* ctx);
  *          "halo_m256" (-1: automatic; 0 / 1: force 128- / 256-pixel tiles on the unsplit launches of the halo kernel),
  *          "halo_ctas" (-1: automatic; 1 / 2: force one 288-thread / two 256-thread CTAs per SM for the halo kernel's
  *                       256 x 64 and four-phase tiles),
+ *          "halo_cs" (-1: automatic; 1: never / 2: wherever legal split a one-CTA-per-SM launch of the halo kernel's 256 x 64 or
+ *                     four-phase tiles over a cluster pair, each rank taking half of the channel chunks and finishing one
+ *                     warpgroup's rows),
  *          "cluster_splitk" (1: K-split convs reduce through a thread-block cluster / DSMEM; 0: workspace + reduce kernel),
  *          "pdl" (1: programmatic dependent launch), "tc_stride2" (1: 4x4 stride-2 convs on the wgmma kernel),
  *          "small_bn" (1: narrower N tiles for small unsplit launches), "siren_tc" (1: students on the wgmma kernels; 0: mma.sync kernels),

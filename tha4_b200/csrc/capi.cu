@@ -266,6 +266,7 @@ int tha4_set_option(tha4_ctx* ctx, const char* name, int64_t value) {
         else if (!strcmp(name, "tma_store")) conv_halo_enable_tma_store(value != 0);
         else if (!strcmp(name, "halo_m256")) { THA4_REQUIRE(value >= -1 && value <= 1, "halo_m256: -1, 0 or 1"); conv_halo_set_m256((int)value); }
         else if (!strcmp(name, "halo_ctas")) { THA4_REQUIRE(value == -1 || value == 1 || value == 2, "halo_ctas: -1, 1 or 2"); conv_halo_set_ctas((int)value); }
+        else if (!strcmp(name, "halo_cs")) { THA4_REQUIRE(value == -1 || value == 1 || value == 2, "halo_cs: -1, 1 or 2"); conv_halo_set_cs((int)value); }
         else if (!strcmp(name, "siren_tc")) siren_tc_enable(value != 0);
         else if (!strcmp(name, "tc_stride2")) conv_tc_enable_stride2(value != 0);
         else if (!strcmp(name, "small_bn")) conv_tc_enable_small_bn(value != 0);

@@ -101,6 +101,7 @@ void conv_halo_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s)
 void conv_halo_enable(bool on);
 void conv_halo_enable_tma_store(bool on);
 void conv_halo_set_ctas(int mode);        // option "halo_ctas": -1 automatic (default), 1 / 2 CTAs per SM for the 256 x 64 and four-phase halo tiles
+void conv_halo_set_cs(int mode);          // option "halo_cs": -1 automatic (default), 1 never / 2 always (where legal) split a two-warpgroup halo launch over a row-owning cluster pair
 void conv_halo_set_m256(int mode);        // option "halo_m256": -1 automatic (default), 0 / 1 force 128- / 256-pixel tiles on unsplit launches
 void conv_halo_debug_dump();   // developer: THA4_HALO_DEBUG=1 phase stamps of the last halo launch
 void conv_enable_tc(bool on);

@@ -64,8 +64,46 @@ __host__ __device__ constexpr int halo_min_ctas(int bn, int sa, int cs, int op, 
 template <int PH>
 __host__ __device__ constexpr int halo_wtile(int j) { return PH == 1 ? j : ((j & 1) * 2 + ((j >> 1) & 1)) * 4 + (j >> 2); }
 
-// WG: consumer warpgroups (1: 128-pixel tiles, 160 threads; 2: 256-pixel tiles, 288 threads, unsplit only)
-// PH: output phases (1: 3x3; 4: four-phase layers, two warpgroups on one 8 x 16 low-resolution tile, unsplit only)
+// every thread of every CTA of the cluster arrives; release / acquire order the shared-memory writes around it
+__device__ __forceinline__ void cluster_sync_all() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
+    asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
+}
+
+// Row-owning cluster pair (WG = 2, CS = 2): the accumulators of one warpgroup as 16-byte chunks [k][128 threads], chunk k of
+// thread t at (k * 128 + t) * 16 bytes.  Sender and receiver thread t hold the same fragment, so the receiver adds chunk k
+// to registers without a transpose, and a warp's 32 chunks fill 512 consecutive bytes (no bank conflicts either side).
+template <int BN, int NACC>
+__device__ __forceinline__ void halo_push_rows(const Acc<BN> (&acc)[NACC], uint32_t remote, int t) {
+#pragma unroll
+    for (int a = 0; a < NACC; ++a)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int j = 0; j < BN / 2; j += 4) {
+                const uint32_t addr = remote + (uint32_t)((((a * 2 + h) * (BN / 8) + j / 4) * 128 + t) * 16);
+                asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};\n" :: "r"(addr), "f"(acc[a].d[h][j]),
+                             "f"(acc[a].d[h][j + 1]), "f"(acc[a].d[h][j + 2]), "f"(acc[a].d[h][j + 3]) : "memory");
+            }
+}
+template <int BN, int NACC>
+__device__ __forceinline__ void halo_add_rows(Acc<BN> (&acc)[NACC], const uint8_t* recv, int t) {
+#pragma unroll
+    for (int a = 0; a < NACC; ++a)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int j = 0; j < BN / 2; j += 4) {
+                const float4 v = *reinterpret_cast<const float4*>(recv + (((a * 2 + h) * (BN / 8) + j / 4) * 128 + t) * 16);
+                acc[a].d[h][j] += v.x; acc[a].d[h][j + 1] += v.y; acc[a].d[h][j + 2] += v.z; acc[a].d[h][j + 3] += v.w;
+            }
+}
+
+// WG: consumer warpgroups (1: 128-pixel tiles, 160 threads; 2: 256-pixel tiles, 288 threads)
+// PH: output phases (1: 3x3; 4: four-phase layers, two warpgroups on one 8 x 16 low-resolution tile)
+// WG = 2 with CS = 2 (one CTA per SM only): a cluster pair splits the channel chunks, and rank r finishes the rows of
+// warpgroup r (3x3: tile rows 16 r .. 16 r + 15; four phases: phases (r, 0) and (r, 1)).  After the MMAs warpgroup 1 - r
+// pushes its accumulators into the peer's idle half of the ring; warpgroup r adds them and runs the unsplit epilogue.
 // CTAS: resident CTAs per SM a two-warpgroup CTA is built for.  1: a TMA producer warp (288 threads, one CTA per SM for
 // 256 x 64 and four-phase tiles).  2: no producer warp (256 threads, two CTAs per SM with rings of at most ~113 KB): thread
 // 0 of the consumers issues the loads from inside the MMA loop, and while one CTA transforms a chunk, starts up or drains
@@ -76,7 +114,9 @@ __global__ void __launch_bounds__(halo_threads(WG, CTAS), halo_min_ctas(BN, SA, 
                                                                 const __grid_constant__ CUtensorMap tmR, const TcParams p) {
     static_assert(OP != OP_TF32, "halo kernel: f16 operands");
     static_assert(BN <= 128, "the accumulator of one warpgroup: BN registers per thread");
-    static_assert(WG == 1 || (WG == 2 && CS == 1 && BN <= 64), "two consumer warpgroups: unsplit launches, two accumulators of at most 64 columns");
+    static_assert(WG == 1 || (WG == 2 && (CS == 1 || (CS == 2 && CTAS == 1)) && BN <= 64),
+                  "two consumer warpgroups: unsplit launches or a row-owning pair, two accumulators of at most 64 columns");
+    constexpr bool ROW_SPLIT = WG == 2 && CS == 2;
     // four phases: two 128-row accumulators per warpgroup, no more registers than one 128 x 64 accumulator
     static_assert(PH == 1 || (PH == 4 && WG == 2 && BN <= 32), "four-phase layers: two warpgroups, two 128 x 32 accumulators each");
     constexpr bool SELF_LOAD = CTAS == 2;                                // consumer thread 0 issues the TMA loads
@@ -95,7 +135,10 @@ __global__ void __launch_bounds__(halo_threads(WG, CTAS), halo_min_ctas(BN, SA, 
     constexpr int PRODUCER_WARP = 4 * WG;
     constexpr int EPI_BYTES = (int)(((size_t)SA * A_BYTES + (size_t)SB * B_BYTES) / WG) & ~1023;      // idle ring per warpgroup in the epilogue
     // TMA-store staging slots of the unsplit epilogue (none for the phase-strided outputs of the four-phase layers)
-    constexpr int NSLOT = CS == 1 && PH == 1 ? epi_nslot(BN, EPI_BYTES) : 0;
+    constexpr int NSLOT = (CS == 1 || ROW_SPLIT) && PH == 1 ? epi_nslot(BN, EPI_BYTES) : 0;
+    // ROW_SPLIT: the peer's partial lands in the other warpgroup's half of the ring, the owner's staging slots lie in its own
+    constexpr int RECV_BYTES = NACC * 128 * BN * 4;
+    static_assert(!ROW_SPLIT || (RECV_BYTES <= EPI_BYTES && (PH == 4 || NSLOT > 0)), "row-owning pair: receive slot and staging slot in the idle ring");
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);      // pointer arithmetic (not an integer round trip) keeps the shared address space: LDS / STS, not generic LD / ST
     uint8_t* smA = smem;
@@ -173,6 +216,11 @@ __global__ void __launch_bounds__(halo_threads(WG, CTAS), halo_min_ctas(BN, SA, 
                         tma_load_3d(smem_u32(smB + sb * B_BYTES), &tmB, (cb0 + ci) * KCE, n0, halo_wtile<PH>(tap), smem_u32(b_full + sb));
                     }
                 }
+            }
+            if constexpr (ROW_SPLIT) {      // the consumers' cluster barriers A and B (every thread of the cluster arrives)
+                __syncwarp();
+                cluster_sync_all();
+                cluster_sync_all();
             }
         } else {
             // ===== consumer warpgroup(s): normalise each chunk's halo ONCE, in place (XF); 9 taps = 9 row-shifted views of
@@ -317,25 +365,41 @@ __global__ void __launch_bounds__(halo_threads(WG, CTAS), halo_min_ctas(BN, SA, 
 #pragma unroll
             for (int a = 0; a < NACC; ++a) { wg_fence_acc(acc[a].d[0]); wg_fence_acc(acc[a].d[1]); }
             if (te == 0) { HSTAMP_END(1, 1); HSTAMP_END(2, 3); }
-            // the epilogue reuses the ring: with two warpgroups, the other one may still be reading its last stages
-            if constexpr (WG > 1) asm volatile("bar.sync 3, 256;\n" ::: "memory");
-            if constexpr (PH == 4) {
-                // phase (wg, px) of the low-resolution tile: output pixels (2 y + wg, 2 x + px), plain stores
-#pragma unroll
-                for (int px = 0; px < 2; ++px) {
-                    // the statistics fold of the first call reads both warpgroups' partials before the second rewrites them
-                    if (px > 0) asm volatile("bar.sync 3, 256;\n" ::: "memory");
-                    epi_direct<BN, HT_W, 0, WG>(p, acc[px], smem + wg * EPI_BYTES, n, y0, x0, n0, 2 * wg + px, 0, warp, lane,
-                                                nullptr, nullptr, nullptr, nullptr, wg, EPI_BYTES);
+            if constexpr (ROW_SPLIT) {
+                // barrier A: both CTAs' MMAs have retired, their rings are idle.  Warpgroup wg = 1 - split pushes its rows to
+                // their owner, rank wg, into the half of the ring the owner's epilogue (warpgroup wg there) leaves alone: half
+                // 1 - wg.  Barrier B: the pushes are visible; nobody touches a peer's memory afterwards.
+                cluster_sync_all();
+                if (wg != split) {
+                    uint32_t remote;
+                    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;\n" : "=r"(remote) : "r"(smem_u32(smem + (1 - wg) * EPI_BYTES)), "r"(wg));
+                    halo_push_rows<BN, NACC>(acc, remote, te & 127);
                 }
-            } else if (CS == 1) {
-                epi_direct<BN, HT_W, NSLOT, WG>(p, acc[0], smem + wg * EPI_BYTES, n, y0 + wg * HT_H, x0, n0, 0, 0, warp, lane,
-                                                &tmO32, &tmO16, &tmR, res_bars + 4 * wg, wg, EPI_BYTES);
+                cluster_sync_all();
+                if (wg == split) halo_add_rows<BN, NACC>(acc, smem + (1 - wg) * EPI_BYTES, te & 127);
+            } else if constexpr (WG > 1) {
+                // the epilogue reuses the ring: with two warpgroups, the other one may still be reading its last stages
+                asm volatile("bar.sync 3, 256;\n" ::: "memory");
+            }
+            if (!ROW_SPLIT || wg == split) {
+                if constexpr (PH == 4) {
+                    // phase (wg, px) of the low-resolution tile: output pixels (2 y + wg, 2 x + px), plain stores
+#pragma unroll
+                    for (int px = 0; px < 2; ++px) {
+                        // the statistics fold of the first call reads both warpgroups' partials before the second rewrites them
+                        if (px > 0 && !ROW_SPLIT) asm volatile("bar.sync 3, 256;\n" ::: "memory");
+                        epi_direct<BN, HT_W, 0, WG, !ROW_SPLIT>(p, acc[px], smem + wg * EPI_BYTES, n, y0, x0, n0, 2 * wg + px, 0, warp, lane,
+                                                                nullptr, nullptr, nullptr, nullptr, wg, EPI_BYTES);
+                    }
+                } else if (CS == 1 || ROW_SPLIT) {
+                    epi_direct<BN, HT_W, NSLOT, WG, !ROW_SPLIT>(p, acc[0], smem + wg * EPI_BYTES, n, y0 + wg * HT_H, x0, n0, 0, 0, warp, lane,
+                                                                &tmO32, &tmO16, &tmR, res_bars + 4 * wg, wg, EPI_BYTES);
+                }
             }
             if (te == 0) HSTAMP_END(2, 4);
         }
     }
-    if (CS > 1) {
+    if constexpr (CS > 1 && !ROW_SPLIT) {
         // barrier A: every CTA of the cluster has its accumulator and idle pipeline buffers -> peers may write into them
         asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
         asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
@@ -434,6 +498,7 @@ bool halo_store_map(const View& v, bool f16, const CUtensorMap** out) {
 
 int g_halo_m256 = -1;         // option "halo_m256": -1 automatic, 0 / 1 force 128- / 256-pixel tiles on unsplit launches
 int g_halo_ctas = -1;         // option "halo_ctas": -1 automatic, 1 / 2 force the 288- / 256-thread two-warpgroup CTAs
+int g_halo_cs = -1;           // option "halo_cs": -1 automatic, 1 never / 2 always (where legal) split a two-warpgroup launch over a cluster pair
 
 // Shared memory of a CTA: the rings, the barriers, the alignment slack (the XF table comes on top)
 constexpr size_t halo_ring(int op, int bn, int sa, int sb, int wg, int ph) {
@@ -473,6 +538,16 @@ int halo_plan_ctas(int op, int bn, int ph, long ctas, const ConvArgs& a) {
     return ctas > num_sms() && 2 * (smem + 1024) <= (size_t)228 * 1024 ? 2 : 1;
 }
 
+// A two-warpgroup launch of one CTA per SM becomes a row-owning cluster pair (cs = 2, conv_halo_kernel's ROW_SPLIT) when
+// twice its CTAs still fit one wave and every rank gets channel chunks: the idle SMs take half of each tile's K.  Measured
+// alone on an H100 SXM (700 W), the teacher frame's 64^2 3x3 layers (32 - 64 CTAs, 2 - 8 chunks) ran 1.20 - 1.66x faster
+// as pairs (64^2 256 -> 256: 29.0 -> 20.0 us), the four-phase layers from 32^2 and 64^2 (64 CTAs) 1.47x and 1.28x; with
+// 72 - 256 CTAs (a second wave) the pairs were 0.60 - 0.87x as fast, and those layers stay unsplit.
+int halo_plan_cs(long ctas, int chunks, const ConvArgs& a) {
+    if (g_halo_cs == 1 || chunks < 2) return 1;
+    return g_halo_cs == 2 || (a.ksplit <= 0 && 2 * ctas <= num_sms()) ? 2 : 1;
+}
+
 HaloPlan halo_plan(const ConvWeights& cw, const ConvArgs& a, int op) {
     HaloPlan pl;
     pl.chunks = cw.cin_pad / op_kch(op);
@@ -482,6 +557,7 @@ HaloPlan halo_plan(const ConvWeights& cw, const ConvArgs& a, int op) {
         pl.tiles_m = pl.tiles_x * pl.tiles_y * a.in.N;
         pl.bn = 32; pl.tiles_n = cw.cout_pad / 32; pl.cs = 1; pl.wg = 2;
         pl.ctas = halo_plan_ctas(op, 32, 4, (long)pl.tiles_m * pl.tiles_n, a);
+        if (pl.ctas == 1) pl.cs = halo_plan_cs((long)pl.tiles_m * pl.tiles_n, pl.chunks, a);
         return pl;
     }
     pl.tiles_x = ceil_div(a.out.W, HT_W); pl.tiles_y = ceil_div(a.out.H, HT_H);
@@ -523,6 +599,7 @@ HaloPlan halo_plan(const ConvWeights& cw, const ConvArgs& a, int op) {
         pl.tiles_n = cw.cout_pad / pl.bn;
     }
     pl.ctas = pl.wg == 2 && pl.bn == 64 ? halo_plan_ctas(op, 64, 1, (long)pl.tiles_m * pl.tiles_n, a) : 1;
+    if (pl.wg == 2 && pl.ctas == 1) pl.cs = halo_plan_cs((long)pl.tiles_m * pl.tiles_n, pl.chunks, a);
     return pl;
 }
 
@@ -548,8 +625,9 @@ void launch_halo(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap
 template <int OP, int BN, int SA, int SBD, int SBS, int XF>
 void launch_halo_cs(int cs, int wg, int ctas, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo32, const CUtensorMap& mo16, const CUtensorMap& mr, const TcParams& p, dim3 grid, cudaStream_t s) {
     constexpr int SA1 = OP == OP_F16N ? 2 : 1;
-    THA4_REQUIRE(wg == 1 || (BN <= 64 && cs == 1), "conv_halo: 256-pixel tiles need an unsplit launch with N tiles of at most 64 columns");
-    THA4_REQUIRE(ctas == 1 || (wg == 2 && BN == 64), "conv_halo: two CTAs per SM are built for 256 x 64 tiles");
+    THA4_REQUIRE(wg == 1 || (BN <= 64 && (cs == 1 || (cs == 2 && ctas == 1 && p.cpt >= 2))),
+                 "conv_halo: 256-pixel tiles need N tiles of at most 64 columns, unsplit or a pair of one-CTA-per-SM ranks with chunks each");
+    THA4_REQUIRE(ctas == 1 || (wg == 2 && BN == 64 && cs == 1), "conv_halo: two CTAs per SM are built for unsplit 256 x 64 tiles");
     if constexpr (BN == 64) {
         if (ctas == 2) {     // one chunk or several: the same rings
             launch_halo<OP, 64, halo2_sa(OP, 1), halo2_sb(OP, 1), 1, XF, 2, 1, 2>(ma, mb, mo32, mo16, mr, p, grid, s);
@@ -565,9 +643,11 @@ void launch_halo_cs(int cs, int wg, int ctas, const CUtensorMap& ma, const CUten
     }
     if constexpr (BN <= 64) {
         if (wg == 2) {
-            // BN = 64: one CTA per SM, which takes the deep weight ring; BN = 32: two CTAs per SM
+            // BN = 64: one CTA per SM, which takes the deep weight ring; BN = 32: two CTAs per SM.  A row-owning pair keeps the rings
             constexpr int M = OP == OP_F16N ? 2 : 1;
-            launch_halo<OP, BN, SA, halo_sb_wg2(OP, BN, SA, BN == 64 ? SBD : 2 * M), 1, XF, 2>(ma, mb, mo32, mo16, mr, p, grid, s);
+            constexpr int SB2 = halo_sb_wg2(OP, BN, SA, BN == 64 ? SBD : 2 * M);
+            if (cs == 2) launch_halo<OP, BN, SA, SB2, 2, XF, 2>(ma, mb, mo32, mo16, mr, p, grid, s);
+            else launch_halo<OP, BN, SA, SB2, 1, XF, 2>(ma, mb, mo32, mo16, mr, p, grid, s);
             return;
         }
     }
@@ -598,6 +678,7 @@ void conv_halo_enable(bool on) { g_use_halo = on; }
 void conv_halo_enable_tma_store(bool on) { g_tma_store = on; }
 void conv_halo_set_m256(int mode) { g_halo_m256 = mode; }
 void conv_halo_set_ctas(int mode) { g_halo_ctas = mode; }
+void conv_halo_set_cs(int mode) { g_halo_cs = mode; }
 
 bool conv_halo_supported(const ConvWeights& cw, const ConvArgs& a) {
     if (!g_use_halo || !conv_tc_supported(cw, a)) return false;
@@ -671,7 +752,7 @@ void conv_halo_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s)
     const CUtensorMap* mo16 = &ma;
     const CUtensorMap* mr = &ma;
     p.st_tma = 0;
-    if (pl.cs == 1 && g_tma_store && cw.nphase == 1) {
+    if ((pl.cs == 1 || pl.wg == 2) && g_tma_store && cw.nphase == 1) {
         if (a.out.p && halo_store_map(a.out, false, &mo32)) p.st_tma |= 1;
         if (a.out16.p && halo_store_map(a.out16, true, &mo16)) p.st_tma |= 2;
         // the residual of a ResBlock's second conv has the geometry of the fp32 output: it arrives through the same box
@@ -688,6 +769,10 @@ void conv_halo_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s)
         if (pl.ctas == 2) {
             if (a.nin.on) launch_halo<OP_F16, 32, SA2, SB2, 1, 1, 2, 4, 2>(ma, mb, *mo32, *mo16, *mr, p, grid, s);
             else launch_halo<OP_F16, 32, SA2, SB2, 1, 0, 2, 4, 2>(ma, mb, *mo32, *mo16, *mr, p, grid, s);
+        } else if (pl.cs == 2) {         // a row-owning pair: the one-CTA-per-SM rings
+            THA4_REQUIRE(pl.chunks >= 2, "conv_halo: a row-owning pair needs a channel chunk per rank");
+            if (a.nin.on) launch_halo<OP_F16, 32, 2, 16, 2, 1, 2, 4>(ma, mb, *mo32, *mo16, *mr, p, grid, s);
+            else launch_halo<OP_F16, 32, 2, 16, 2, 0, 2, 4>(ma, mb, *mo32, *mo16, *mr, p, grid, s);
         } else if (a.nin.on) launch_halo<OP_F16, 32, 2, 16, 1, 1, 2, 4>(ma, mb, *mo32, *mo16, *mr, p, grid, s);
         else launch_halo<OP_F16, 32, 2, 16, 1, 0, 2, 4>(ma, mb, *mo32, *mo16, *mr, p, grid, s);
     } else if (op == OP_F16) {

@@ -235,9 +235,10 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, uint32_t sr
 
 // WG == 2 (conv_halo.cu's 256-pixel tiles): each consumer warpgroup wg runs this on its own 128 rows, with its own named
 // barrier, its own shared-memory region `smem` (warpgroup 1's starts wg_bytes after warpgroup 0's) and its own residual
-// barriers; y0 is the first pixel row of the warpgroup's rows.  The two warpgroups' channel sums are folded in shared
-// memory before the fp64 atomics: one pair per (CTA, channel).
-template <int BN, int TW, int NSLOT = 0, int WG = 1>
+// barriers; y0 is the first pixel row of the warpgroup's rows.  FOLD: the two warpgroups' channel sums are folded in shared
+// memory before the fp64 atomics, one pair per (CTA, channel); without it (a CTA in which only one warpgroup runs the
+// epilogue) each warpgroup commits the sums of its own rows.
+template <int BN, int TW, int NSLOT = 0, int WG = 1, bool FOLD = true>
 __device__ __forceinline__ void epi_direct(const TcParams& p, const Acc<BN>& acc, uint8_t* smem, int n, int y0, int x0,
                                            int n0, int phase, int split, int warp, int lane,
                                            const CUtensorMap* tm32 = nullptr, const CUtensorMap* tm16 = nullptr,
@@ -419,14 +420,16 @@ __device__ __forceinline__ void epi_direct(const TcParams& p, const Acc<BN>& acc
     }
     if (p.stats && p.ksplit == 1) {
         // combine the warps' partial sums: one double atomic pair per (tile, channel), spread over replicas
+        constexpr bool FOLD2 = WG == 2 && FOLD;
         if constexpr (WG == 1) asm volatile("bar.sync 1, 128;\n" ::: "memory");
-        else asm volatile("bar.sync 3, 256;\n" ::: "memory");                   // both warpgroups' partials are written
-        const float2* part = reinterpret_cast<const float2*>(reinterpret_cast<float*>(smem - wg * wg_bytes) + 4 * 32 * 33);
+        else if constexpr (FOLD2) asm volatile("bar.sync 3, 256;\n" ::: "memory");   // both warpgroups' partials are written
+        else wg_bar<WG>(wg);
+        const float2* part = reinterpret_cast<const float2*>(reinterpret_cast<float*>(smem - (FOLD2 ? wg * wg_bytes : 0)) + 4 * 32 * 33);
         double* base = p.stats + (long)(blockIdx.x % p.stats_rep) * p.stats_rep_stride + ((long)n * p.stats_ld + n0) * 2;
-        for (int c = (int)threadIdx.x; c < BN; c += 128 * WG) {
+        for (int c = FOLD2 ? (int)threadIdx.x : t; c < BN; c += FOLD2 ? 128 * WG : 128) {
             if (n0 + c >= p.outC) break;
             const float2 a = part[c], b = part[BN + c], cc = part[2 * BN + c], d = part[3 * BN + c];
-            if constexpr (WG == 1) {
+            if constexpr (!FOLD2) {
                 atomicAdd(base + 2 * c, (double)a.x + (double)b.x + (double)cc.x + (double)d.x);
                 atomicAdd(base + 2 * c + 1, (double)a.y + (double)b.y + (double)cc.y + (double)d.y);
             } else {
