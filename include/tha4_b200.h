@@ -326,6 +326,37 @@ int tha4_test_group_norm_backward(tha4_ctx* ctx, const float* x, int N, int C, i
                                   float* d_film, void* stream);
 /* qkv_attention backward (fp32): qkv [N,3C,16,16], dout = d(attention output) [N,C,16,16] -> dqkv [N,3C,16,16] */
 int tha4_test_attention_backward(tha4_ctx* ctx, const float* qkv, const float* dout, int N, int C, int heads, float* dqkv, void* stream);
+/* The backward kernels in the layouts the network backwards run them.  Every tensor is an NHWC device tensor given by a
+ * pointer to its channel 0 and a pixel stride (`*_ld`, in elements), so that it can be a channel slice of a wider buffer.
+ * x (the raw input of the normalisation) is fp32, or f16 when x_f16; `stats` (device) holds its per-(n, c) sum and sum of
+ * squares as stats_rep replicas [rep][N][stats_ld][2] (doubles), which the kernels add up.
+ *
+ * GroupNorm(groups) (+FiLM) (+SiLU) backward, group_norm_backward: film1 / d_film [N][film1_ld] / [N][d_film_ld] with this
+ * layer's 2C columns at film1_off (d_film: d(scale) then d(shift); only those columns are written); dy [N,H,W,C], or
+ * [N,H/2,W/2,C] when dy_pool (the output was 2x2-mean-pooled); res_mode 0 none, 1 same resolution, 2 the 2x2 sum of a
+ * [N,2H,2W,C] res, 3 1/4 of a [N,H/2,W/2,C] res; add [N,H,W,C] or NULL.  C <= 512. */
+int tha4_test_group_norm_backward_ex(tha4_ctx* ctx, const void* x, int x_f16, int x_ld, int N, int C, int H, int W, int groups,
+                                     const double* stats, int stats_rep, int stats_ld, const float* gamma, const float* beta,
+                                     const float* film0, const float* film1, int film1_ld, int film1_off, int act, const float* dy,
+                                     int dy_ld, int dy_pool, const float* res, int res_ld, int res_mode, const float* add, int add_ld,
+                                     float* dx, int dx_ld, float* d_film, int d_film_ld, void* stream);
+/* InstanceNorm2d(affine) (+ReLU when act == 1) backward, norm_backward: x as above, dy / dx [N,H,W,C]. */
+int tha4_test_norm_backward_ex(tha4_ctx* ctx, const void* x, int x_f16, int x_ld, int N, int C, int H, int W, const double* stats,
+                               int stats_rep, int stats_ld, const float* gamma, const float* beta, int act, const float* dy, int dy_ld,
+                               float* dx, int dx_ld, void* stream);
+/* Conv data gradient through run_dgrad: kinds 0..5 and weights as tha4_test_conv_backward_data; kind 6 is the adjoint of the
+ * fused tail's head conv from the 16-channel head gradient to Cin feature channels (Cout = 16; head_w / head_b / head_cout /
+ * n_heads as for tha4_test_tail, packed with tail_init / tail_add and adjoint-packed by head_pack_adjoint).  dy
+ * [N,Ho,Wo,Cout], dx [N,H,W,Cin rounded up to 4] (+ add of the same shape, or NULL).  workspace 0 runs the same conv without
+ * the split-K workspace, so that a split launch that is not a cluster split accumulates atomically.  split_plan (host, may be
+ * NULL) receives how the tensor-core kernel split K: 0 not split or not that kernel (strict mode), 1 cluster, 2 workspace,
+ * 3 atomic. */
+int tha4_test_conv_backward_data_ex(tha4_ctx* ctx, int kind, const float* w, const float* head_b, const int* head_cout, int n_heads,
+                                    const float* dy, int dy_ld, const float* add, int add_ld, float* dx, int dx_ld, int N, int Cin,
+                                    int H, int W, int Cout, int strict, int workspace, int* split_plan, void* stream);
+/* linear_backward: dx[n][k] = SiLU'(pre[n][k]) sum_r dy[n][r] W[r][k] (pre NULL: no SiLU'), W [R][K] */
+int tha4_test_linear_backward(tha4_ctx* ctx, const float* dy, int dy_ld, int N, int R, const float* W, int K, const float* pre, int pre_ld,
+                              float* dx, int dx_ld, void* stream);
 /* qkv_attention, "new order" (src/tha4/nn/common/unet.py:192-202): qkv [N,3C,16,16] -> out [N,C,16,16] */
 int tha4_test_attention(tha4_ctx* ctx, const float* qkv, int N, int C, int heads, float* out, void* stream);
 /* y[n][o] = b[o] + sum_i f(x[n][i]) W[o][i] */

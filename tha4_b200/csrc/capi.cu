@@ -1160,6 +1160,120 @@ int tha4_test_attention_backward(tha4_ctx* ctx, const float* qkv, const float* d
     });
 }
 
+// ------------------------------------------------------------------------------------------------ backward hooks on strided operands
+// The layouts the network backwards hand these kernels: NHWC device tensors addressed by a pointer to their channel 0 and a
+// pixel stride `ld` (a slice of a wider buffer), f16 or fp32 raw inputs, and the caller's own statistics replicas.
+static View nhwc_view(const void* p, int N, int H, int W, int C, int ld, int f16 = 0) {
+    View v; v.p = const_cast<float*>(static_cast<const float*>(p)); v.N = N; v.H = H; v.W = W; v.C = C; v.ld = ld; v.f16 = f16;
+    return v;
+}
+
+static View stats_input(const void* x, int x_f16, int x_ld, int N, int C, int H, int W, const double* stats, int stats_rep, int stats_ld) {
+    THA4_REQUIRE(stats != nullptr && stats_rep >= 1 && stats_ld >= C, "backward hook: statistics [rep][N][stats_ld][2]");
+    View v = nhwc_view(x, N, H, W, C, x_ld, x_f16 ? 1 : 0);
+    v.stats = const_cast<double*>(stats); v.stats_ld = stats_ld; v.stats_rep = stats_rep; v.stats_rep_stride = (long)N * stats_ld * 2;
+    return v;
+}
+
+int tha4_test_group_norm_backward_ex(tha4_ctx* ctx, const void* x, int x_f16, int x_ld, int N, int C, int H, int W, int groups,
+                                     const double* stats, int stats_rep, int stats_ld, const float* gamma, const float* beta,
+                                     const float* film0, const float* film1, int film1_ld, int film1_off, int act, const float* dy,
+                                     int dy_ld, int dy_pool, const float* res, int res_ld, int res_mode, const float* add, int add_ld,
+                                     float* dx, int dx_ld, float* d_film, int d_film_ld, void* stream) {
+    return guarded(ctx, [&] {
+        cudaStream_t s = (cudaStream_t)stream;
+        THA4_REQUIRE(act == ACT_NONE || act == ACT_SILU, "test_group_norm_backward_ex: act 0 or 2");
+        THA4_REQUIRE(res_mode >= RES_NONE && res_mode <= RES_DOWN2 && (res != nullptr) == (res_mode != RES_NONE),
+                     "test_group_norm_backward_ex: res with res_mode 1..3, or neither");
+        begin_pass(ctx, s);
+        Runtime rt = make_rt(ctx, stream);
+        const View xin = stats_input(x, x_f16, x_ld, N, C, H, W, stats, stats_rep, stats_ld);
+        const View g = dy_pool ? nhwc_view(dy, N, H / 2, W / 2, C, dy_ld) : nhwc_view(dy, N, H, W, C, dy_ld);
+        const int rs = res_mode == RES_UP2 ? 2 : 1, rd = res_mode == RES_DOWN2 ? 2 : 1;
+        const View r = nhwc_view(res, N, H * rs / rd, W * rs / rd, C, res_ld);
+        const View a = nhwc_view(add, N, H, W, C, add_ld);
+        group_norm_backward(xin, groups, gamma, beta, film0, film1 ? film1 + film1_off : nullptr, film1_ld, act, g, dy_pool,
+                            nhwc_view(dx, N, H, W, C, dx_ld), d_film ? d_film + film1_off : nullptr, d_film_ld,
+                            res ? &r : nullptr, res_mode, add ? &a : nullptr, rt.alloc_stats((size_t)N * C * 2),
+                            ctx->persist.alloc((size_t)N * C * 8), s);
+    });
+}
+
+int tha4_test_norm_backward_ex(tha4_ctx* ctx, const void* x, int x_f16, int x_ld, int N, int C, int H, int W, const double* stats,
+                               int stats_rep, int stats_ld, const float* gamma, const float* beta, int act, const float* dy, int dy_ld,
+                               float* dx, int dx_ld, void* stream) {
+    return guarded(ctx, [&] {
+        cudaStream_t s = (cudaStream_t)stream;
+        THA4_REQUIRE(act == ACT_NONE || act == ACT_RELU, "test_norm_backward_ex: act 0 or 1");
+        begin_pass(ctx, s);
+        Runtime rt = make_rt(ctx, stream);
+        norm_backward(stats_input(x, x_f16, x_ld, N, C, H, W, stats, stats_rep, stats_ld), gamma, beta, act, nhwc_view(dy, N, H, W, C, dy_ld),
+                      nhwc_view(dx, N, H, W, C, dx_ld), rt.alloc_stats((size_t)N * C * 2), s);
+    });
+}
+
+int tha4_test_conv_backward_data_ex(tha4_ctx* ctx, int kind, const float* w, const float* head_b, const int* head_cout, int n_heads,
+                                    const float* dy, int dy_ld, const float* add, int add_ld, float* dx, int dx_ld, int N, int Cin,
+                                    int H, int W, int Cout, int strict, int workspace, int* split_plan, void* stream) {
+    return guarded(ctx, [&] {
+        cudaStream_t s = (cudaStream_t)stream;
+        begin_pass(ctx, s);
+        THA4_REQUIRE(kind >= 0 && kind <= 6 && Cout % 4 == 0 && (kind == 0 || kind == 5 || Cin % 4 == 0),
+                     "test_conv_backward_data_ex: kind 0..6, Cout % 4 == 0 (and Cin % 4 == 0 for kinds 1..4 and 6)");
+        THA4_REQUIRE(kind != 6 || (Cout == 16 && head_cout != nullptr && n_heads > 0), "test_conv_backward_data_ex: kind 6 maps 16 head channels");
+        const bool packed = kind >= 3 && kind <= 5;
+        const bool head = kind == 6;
+        if (kind == 5 || kind == 6) kind = CONV_3x3;
+        Runtime rt = make_rt(ctx, stream);
+        rt.strict = strict;
+        AllocSink sink;
+        ConvWeights cw;
+        {
+            SinkScope own(&sink);
+            conv_set_pack_rounding(!strict);
+            if (head) {         // the fused tail's head weights, adjoint-packed as the networks do
+                TailWeights tw;
+                tail_init(tw, Cin, s);
+                size_t woff = 0, boff = 0;
+                for (int i = 0; i < n_heads; ++i) {
+                    tail_add(tw, w + woff, head_b ? head_b + boff : nullptr, head_cout[i], s);
+                    woff += (size_t)head_cout[i] * Cin * 9; boff += head_cout[i];
+                }
+                head_pack_adjoint(cw, tw, !strict, s);
+            } else if (!packed) {
+                conv_pack_adjoint(cw, (ConvKind)kind, w, Cin, Cout, kind == CONV_3x3 ? round_up(Cin, 4) : 0, s);
+            } else {
+                ConvWeights fwd;
+                conv_describe(fwd, (ConvKind)kind, round_up(Cin, 4), Cout);
+                fwd.w = reinterpret_cast<float*>(tracked_malloc(conv_packed_floats(fwd) * sizeof(float)));
+                THA4_CUDA_CHECK(cudaMemsetAsync(fwd.w, 0, conv_packed_floats(fwd) * sizeof(float), s));
+                conv_pack(fwd, (ConvKind)kind, w, Cin, 0, s);
+                fwd.tf32_rounded = !strict;
+                conv_adjoint_from_packed(cw, fwd, (ConvKind)kind, s);
+            }
+        }
+        const int Ho = kind == 1 ? H / 2 : ((kind == 2 || kind == 4) ? 2 * H : H), Wo = kind == 1 ? W / 2 : ((kind == 2 || kind == 4) ? 2 * W : W);
+        THA4_REQUIRE(dy_ld >= Cout && dx_ld >= cw.cout && (!add || add_ld >= cw.cout), "test_conv_backward_data_ex: strides");
+        const View g = nhwc_view(dy, N, Ho, Wo, Cout, dy_ld), o = nhwc_view(dx, N, H, W, cw.cout, dx_ld), r = nhwc_view(add, N, H, W, cw.cout, add_ld);
+        ConvArgs a;         // run_dgrad's conv; without the workspace a split launch accumulates with atomics
+        a.in = g; a.out = o; a.strict = strict;
+        if (add) { a.res = r; a.res_mode = RES_SAME; }
+        if (workspace) {
+            const size_t ws = conv_workspace_floats(cw, a);
+            if (ws) { a.ws = ctx->scratch.alloc(ws); a.ws_floats = ws; }     // as run_dgrad allocates it
+        }
+        if (split_plan) *split_plan = conv_tc_split_plan(cw, a);
+        if (workspace) run_dgrad(rt, cw, g, o, add ? &r : nullptr);
+        else conv_forward(cw, a, s);
+        THA4_CUDA_CHECK(cudaStreamSynchronize(s));       // `sink` frees the packed weights on return
+    });
+}
+
+int tha4_test_linear_backward(tha4_ctx* ctx, const float* dy, int dy_ld, int N, int R, const float* W, int K, const float* pre, int pre_ld,
+                              float* dx, int dx_ld, void* stream) {
+    return guarded(ctx, [&] { linear_backward(dy, dy_ld, N, R, W, K, pre, pre_ld, dx, dx_ld, (cudaStream_t)stream); });
+}
+
 int tha4_test_attention(tha4_ctx* ctx, const float* qkv, int N, int C, int heads, float* out, void* stream) {
     return guarded(ctx, [&] {
         cudaStream_t s = (cudaStream_t)stream;

@@ -94,6 +94,9 @@ void conv_tc_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s); 
 // the caller runs norm_stats on the output.
 bool conv_fuses_stats(const ConvWeights& cw, const ConvArgs& a);
 bool conv_tc_fuses_stats(const ConvWeights& cw, const ConvArgs& a);
+// How the wgmma kernel would split K for this call: 0 not split (or not the wgmma kernel), 1 over a cluster, 2 through the
+// workspace, 3 with atomics into the output (no workspace given)
+int conv_tc_split_plan(const ConvWeights& cw, const ConvArgs& a);
 // conv_halo.cu: 3x3 stride-1 convs on f16 operands with halo reuse (one activation box per channel chunk, taps as
 // row-shifted UMMA descriptors); preferred over conv_tc_forward when it supports the configuration
 bool conv_halo_supported(const ConvWeights& cw, const ConvArgs& a);

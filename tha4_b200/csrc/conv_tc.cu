@@ -423,6 +423,14 @@ size_t conv_workspace_floats(const ConvWeights& cw, const ConvArgs& a) {
     return (size_t)cw.nphase * pl.ksplit * pl.tiles_m * 128 * cw.cout_pad;
 }
 
+int conv_tc_split_plan(const ConvWeights& cw, const ConvArgs& a) {
+    if (!conv_tc_enabled() || !conv_tc_supported(cw, a) || conv_halo_supported(cw, a)) return 0;
+    const TcPlan pl = tc_plan(cw, a);
+    if (pl.ksplit <= 1) return 0;
+    if (pl.cluster) return 1;
+    return a.ws && a.ws_floats >= (size_t)cw.nphase * pl.ksplit * pl.tiles_m * 128 * cw.cout_pad ? 2 : 3;
+}
+
 void conv_make_half(const ConvWeights& cw, cudaStream_t s) {
     if (cw.w16 || !cw.w) return;
     const long nw = (long)conv_packed_floats(cw);
