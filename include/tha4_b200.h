@@ -63,6 +63,8 @@ const char* tha4_last_error(const tha4_ctx* ctx);
  *          "halo_cs" (-1: automatic; 1: never / 2: wherever legal split a one-CTA-per-SM launch of the halo kernel's 256 x 64 or
  *                     four-phase tiles over a cluster pair, each rank taking half of the channel chunks and finishing one
  *                     warpgroup's rows),
+ *          "skip_fold" (1: the 1x1 skip of a U-Net ResBlock runs inside the K loop of the block's second conv, one halo launch;
+ *                       0: its own launch on the side stream, added as conv1's residual),
  *          "cluster_splitk" (1: K-split convs reduce through a thread-block cluster / DSMEM; 0: workspace + reduce kernel),
  *          "pdl" (1: programmatic dependent launch), "tc_stride2" (1: 4x4 stride-2 convs on the wgmma kernel),
  *          "small_bn" (1: narrower N tiles for small unsplit launches), "siren_tc" (1: students on the wgmma kernels; 0: mma.sync kernels),
@@ -283,6 +285,15 @@ int tha4_test_conv_norm_ex(tha4_ctx* ctx, int kind, const float* x, int N, int C
 /* y = act(norm(x)) with groups == 0: InstanceNorm2d, else GroupNorm(groups); act 0 none / 1 relu / 2 silu; pool 0/1;
  * film0 [2C] / film1 [N,2C] optional FiLM scale-shifts (unet.py:90-97); out_f16 = 1 runs the default-mode variant
  * (f16 output tensor, fast-math SiLU) and returns its values widened to fp32 */
+/* The second conv of a U-Net ResBlock with a 1x1 skip: y = conv3x3(act(norm(x))) + bias + conv1x1(x2) + b_skip, x [N,Cmid,H,W]
+ * the raw conv0 output (GroupNorm(groups) / InstanceNorm (groups 0) + film0 / film1 + act as in tha4_test_conv_norm_ex,
+ * norm_C = Cmid), x2 [N,Cin2,H,W] the block input, w [Cout,Cmid,3,3], w_skip [Cout,Cin2,1,1].  With option "skip_fold" on,
+ * one halo launch runs both (*folded = 1); with it off, the skip conv and conv1 with the skip as its residual (*folded = 0).  ksplit, y_stats, reps and us_per_launch as in tha4_test_conv_norm_ex (the
+ * time is that of the one launch or of the pair). */
+int tha4_test_conv_skip_fold(tha4_ctx* ctx, const float* x, int N, int Cmid, int H, int W, int groups, const float* gamma,
+                             const float* beta, const float* film0, const float* film1, int act, const float* w, const float* bias,
+                             const float* x2, int Cin2, const float* w_skip, const float* b_skip, int Cout, int ksplit,
+                             float* y, double* y_stats, int* folded, int reps, float* us_per_launch, void* stream);
 int tha4_test_norm(tha4_ctx* ctx, const float* x, int N, int C, int H, int W, int groups, const float* gamma,
                    const float* beta, const float* film0, const float* film1, int act, int pool, int out_f16, float* y, void* stream);
 /* One fused decoder tail (SURVEY 8 a-T) in isolation: feature [N,C,S,S] is the raw last feature map; the kernel applies

@@ -267,6 +267,7 @@ int tha4_set_option(tha4_ctx* ctx, const char* name, int64_t value) {
         else if (!strcmp(name, "halo_m256")) { THA4_REQUIRE(value >= -1 && value <= 1, "halo_m256: -1, 0 or 1"); conv_halo_set_m256((int)value); }
         else if (!strcmp(name, "halo_ctas")) { THA4_REQUIRE(value == -1 || value == 1 || value == 2, "halo_ctas: -1, 1 or 2"); conv_halo_set_ctas((int)value); }
         else if (!strcmp(name, "halo_cs")) { THA4_REQUIRE(value == -1 || value == 1 || value == 2, "halo_cs: -1, 1 or 2"); conv_halo_set_cs((int)value); }
+        else if (!strcmp(name, "skip_fold")) unet_set_skip_fold(value != 0);
         else if (!strcmp(name, "siren_tc")) siren_tc_enable(value != 0);
         else if (!strcmp(name, "tc_stride2")) conv_tc_enable_stride2(value != 0);
         else if (!strcmp(name, "small_bn")) conv_tc_enable_small_bn(value != 0);
@@ -942,6 +943,96 @@ int tha4_test_conv_norm_ex(tha4_ctx* ctx, int kind, const float* x, int N, int C
                            float* y, float* y_from_f16, double* y_stats, int reps, float* us_per_launch, void* stream) {
     return test_conv_norm(ctx, kind, x, N, Cin, H, W, norm_C, groups, gamma, beta, film0, film1, act, w, bias, res, res_mode, Cout,
                           ksplit, y, y_from_f16, y_stats, reps, us_per_launch, stream);
+}
+
+int tha4_test_conv_skip_fold(tha4_ctx* ctx, const float* x, int N, int Cmid, int H, int W, int groups, const float* gamma,
+                             const float* beta, const float* film0, const float* film1, int act, const float* w, const float* bias,
+                             const float* x2, int Cin2, const float* w_skip, const float* b_skip, int Cout, int ksplit,
+                             float* y, double* y_stats, int* folded, int reps, float* us_per_launch, void* stream) {
+    return guarded(ctx, [&] {
+        cudaStream_t s = (cudaStream_t)stream;
+        begin_pass(ctx, s);
+        Runtime rt = make_rt(ctx, stream);
+        Pool* P = &ctx->persist;
+        THA4_REQUIRE(Cmid % 8 == 0 && Cin2 % 8 == 0, "test_conv_skip_fold: channel counts must be multiples of 8");
+        AllocSink sink;
+        ConvWeights cw, sw, fw;
+        auto mk = [&](int n, int h, int ww, int c) { View v; v.N = n; v.H = h; v.W = ww; v.C = c; v.ld = c; v.p = P->alloc((size_t)n * h * ww * c); return v; };
+        {
+            SinkScope own(&sink);
+            conv_set_pack_rounding(true);
+            for (int k = 0; k < 2; ++k) {
+                ConvWeights& c = k ? sw : cw;
+                conv_describe(c, k ? CONV_1x1 : CONV_3x3, k ? Cin2 : Cmid, Cout);
+                c.tf32_rounded = true;
+                c.w = reinterpret_cast<float*>(tracked_malloc(conv_packed_floats(c) * sizeof(float)));
+                THA4_CUDA_CHECK(cudaMemsetAsync(c.w, 0, conv_packed_floats(c) * sizeof(float), s));
+                conv_pack(c, k ? CONV_1x1 : CONV_3x3, k ? w_skip : w, k ? Cin2 : Cmid, 0, s);
+                conv_make_half(c, s);
+            }
+        }
+        cw.bias = const_cast<float*>(bias); sw.bias = const_cast<float*>(b_skip);
+        // the raw conv0 output h0 (fp32 for its statistics, f16 operand) and the block input x (f16 operand)
+        View hin = mk(N, H, W, Cmid);
+        hin.stats_rep = 2; hin.stats_rep_stride = (long)N * Cmid * 2;
+        hin.stats = rt.alloc_stats((size_t)2 * N * Cmid * 2); hin.stats_ld = Cmid;
+        nchw_to_nhwc(make_img(x, N, Cmid, H, W), hin, s);
+        norm_stats(hin, s);
+        View h16 = hin; h16.f16 = 1; h16.stats = nullptr; h16.p = P->alloc(((size_t)N * H * W * Cmid + 1) / 2);
+        convert_f16(hin, h16, s);
+        View xin = mk(N, H, W, Cin2);
+        nchw_to_nhwc(make_img(x2, N, Cin2, H, W), xin, s);
+        View x16 = xin; x16.f16 = 1; x16.p = P->alloc(((size_t)N * H * W * Cin2 + 1) / 2);
+        convert_f16(xin, x16, s);
+        View yo = mk(N, H, W, Cout);
+        if (y_stats) {
+            yo.stats = rt.alloc_stats((size_t)N * Cout * 2); yo.stats_ld = Cout; yo.stats_rep = 1; yo.stats_rep_stride = (long)N * Cout * 2;
+            THA4_CUDA_CHECK(cudaMemsetAsync(yo.stats, 0, (size_t)N * Cout * 2 * sizeof(double), s));
+        }
+        View y16 = yo; y16.f16 = 1; y16.stats = nullptr; y16.p = P->alloc(((size_t)N * H * W * Cout + 1) / 2);
+        ConvArgs a;                               // conv1 of the block, on the normalised h0
+        a.in = h16; a.out = yo; a.out16 = y16; a.ksplit = ksplit;
+        a.nin.on = true; a.nin.C = Cmid; a.nin.groups = groups; a.nin.act = act == ACT_SILU ? ACT_SILU_FAST : act;
+        a.nin.gamma = gamma; a.nin.beta = beta; a.nin.film0 = film0; a.nin.film1 = film1; a.nin.film1_ld = 2 * Cmid;
+        a.nin.stats = hin.stats; a.nin.stats_ld = hin.stats_ld; a.nin.stats_rep = hin.stats_rep; a.nin.stats_rep_stride = hin.stats_rep_stride;
+        ConvArgs fa = a;
+        fa.in2 = x16;
+        {
+            SinkScope own(&sink);
+            conv_make_fold(fw, cw, sw, s);
+        }
+        const bool fold = unet_skip_fold() && conv_halo_supported(fw, fa);     // as UNetNet's default mode decides (res_block)
+        // the unfused pair: skip(x) in fp32, then conv1 adds it as its residual
+        View sk = mk(N, H, W, Cout);
+        ConvArgs sa; sa.in = x16; sa.out = sk;
+        a.res = sk; a.res_mode = RES_SAME;
+        const size_t wsf = std::max(conv_workspace_floats(sw, sa), conv_workspace_floats(cw, a));
+        float* ws = wsf ? ctx->scratch.alloc(wsf) : nullptr;
+        for (ConvArgs* c : {&sa, &a}) { c->ws = ws; c->ws_floats = wsf; }
+        auto run = [&] {
+            if (fold) { conv_forward(fw, fa, s); return; }
+            if (y_stats) THA4_CUDA_CHECK(cudaMemsetAsync(yo.stats, 0, (size_t)N * Cout * 2 * sizeof(double), s));
+            conv_forward(sw, sa, s);
+            conv_forward(cw, a, s);
+        };
+        run();
+        if (y_stats) THA4_CUDA_CHECK(cudaMemcpyAsync(y_stats, yo.stats, (size_t)N * Cout * 2 * sizeof(double), cudaMemcpyDeviceToDevice, s));
+        if (folded) *folded = fold ? 1 : 0;
+        if (reps > 0) {       // device time of the fused launch / of the pair: `reps` back-to-back runs between two events
+            cudaEvent_t e0, e1;
+            THA4_CUDA_CHECK(cudaEventCreate(&e0)); THA4_CUDA_CHECK(cudaEventCreate(&e1));
+            THA4_CUDA_CHECK(cudaEventRecord(e0, s));
+            for (int i = 0; i < reps; ++i) run();
+            THA4_CUDA_CHECK(cudaEventRecord(e1, s));
+            THA4_CUDA_CHECK(cudaEventSynchronize(e1));
+            float ms = 0.0f;
+            THA4_CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
+            cudaEventDestroy(e0); cudaEventDestroy(e1);
+            if (us_per_launch) *us_per_launch = 1000.0f * ms / reps;
+        }
+        nhwc_to_nchw(yo, y, s);
+        THA4_CUDA_CHECK(cudaStreamSynchronize(s));
+    });
 }
 
 int tha4_test_norm(tha4_ctx* ctx, const float* x, int N, int C, int H, int W, int groups, const float* gamma,

@@ -379,6 +379,7 @@ bool conv_fuses_stats(const ConvWeights& cw, const ConvArgs& a) {
 void conv_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s) {
     if (a.nin.on || a.out16.p || !a.out.p)
         THA4_REQUIRE(g_use_tc && conv_tc_supported(cw, a), "conv: fused input normalisation / f16 outputs exist on the wgmma kernel only");
+    THA4_REQUIRE(cw.cin2 == 0 || (g_use_tc && conv_halo_supported(cw, a)), "conv: a folded 1x1 conv runs on the halo kernel only");
     if (g_use_tc && conv_halo_supported(cw, a)) conv_halo_forward(cw, a, s);
     else if (g_use_tc && conv_tc_supported(cw, a)) conv_tc_forward(cw, a, s);
     else conv_mma_forward(cw, a, s);

@@ -31,6 +31,11 @@ struct ConvWeights {
     signed char dy[CONV_MAX_PHASES][CONV_MAX_TAPS];
     signed char dx[CONV_MAX_PHASES][CONV_MAX_TAPS];
     signed char ph_oy[CONV_MAX_PHASES], ph_ox[CONV_MAX_PHASES];
+    // A 1x1 convolution folded into this 3x3 one (conv_make_fold): a second K segment, the f16 weights w16b [cout_pad][cin2_pad]
+    // at their own scale w16b_scale, read against ConvArgs::in2; bias is the sum of both biases.  cin2 = 0: none.
+    int cin2 = 0, cin2_pad = 0;
+    __half* w16b = nullptr;
+    float w16b_scale = 1.0f;
 };
 
 // CONV_UP2_3x3: nearest-neighbour x2 upsample followed by a 3x3 conv (the up-sampling ResBlock, unet.py:46,119-123),
@@ -73,6 +78,7 @@ struct ConvArgs {
     View out;                   // geometry + statistics slot of the output; out.p may be null when only the f16 copy is wanted
     View out16;                 // optional f16 copy of the output (out16.p == nullptr: none)
     ConvNormIn nin;             // fused normalisation of the input (wgmma kernel, f16 input only)
+    View in2;                   // f16 input of a folded 1x1 conv (cw.cin2 > 0), at the output's resolution
     View res;                   // residual added in the epilogue (res.p == nullptr: none)
     int res_mode = RES_NONE;    // RES_UP2: res stored at half resolution; RES_DOWN2: res at double resolution (2x2 mean)
     int strict = 0;             // 1: 3xTF32 error-compensated products (fp32-equivalent); 0: single TF32
@@ -110,6 +116,9 @@ void conv_halo_debug_dump();   // developer: THA4_HALO_DEBUG=1 phase stamps of t
 void conv_enable_tc(bool on);
 bool conv_tc_enabled();
 void conv_make_half(const ConvWeights& cw, cudaStream_t s);   // f16 copy of the packed weights (cw.w16), recorded in the active AllocSink
+// conv3 (3x3) followed by conv1x1 (same Cout) as one K (ConvWeights::cin2): the two f16 copies as they are (not owned by
+// `fold`), and the summed bias, recorded in the active AllocSink
+void conv_make_fold(ConvWeights& fold, const ConvWeights& conv3, const ConvWeights& conv1x1, cudaStream_t s);
 void conv_tc_enable_cluster(bool on);
 void conv_tc_enable_small_bn(bool on);  // narrower N tiles for tiny unsplit GEMMs
 void conv_tc_enable_stride2(bool on);   // stride-2 4x4 convs on the wgmma kernel (element-strided TMA) instead of mma.sync

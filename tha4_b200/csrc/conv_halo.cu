@@ -17,6 +17,14 @@
 // low-resolution input) run on the same halo: one 8 x 16 low-resolution tile per CTA, its 10 x 18 halo loaded and
 // normalised once per chunk instead of once per (phase, tap) -- 180 rows instead of 16 x 128.  Consumer warpgroup py holds
 // the accumulators of phases (py, 0) and (py, 1); the 16 weight tiles of a chunk alternate between the two warpgroups.
+// Folded 1x1 skip (SK, the second conv of a U-Net ResBlock whose input and output widths differ): conv1(n1(h0)) + skip(x)
+// is one GEMM over a longer K.  The chunk list is the cpt chunks of h0 (halo through tmA, XF transform, nine weight tiles
+// from tmB) followed by the cpt2 chunks of x (halo through tmA2, no transform, the centre-tap view and one weight tile from
+// tmB2).  Each weight segment keeps the power-of-two scale of its f16 copy: after its last 3x3 chunk a CTA multiplies the
+// accumulator by acc_rescale (exact), so the products and their sums are those of the separate convs, in the skip weights'
+// units.  Summation order: within a CTA, chunk by chunk in list order (tap by tap inside a 3x3 chunk); a cluster split
+// gives rank r the contiguous chunks [halo_fold_c0(r), halo_fold_c0(r + 1)), balanced by weight tiles, and its partials
+// meet in the reduction of the unsplit kernel (rank order, conv_tc_device.cuh).
 #include "conv.cuh"
 #include "profiler.cuh"
 #include "conv_tc_device.cuh"
@@ -63,6 +71,12 @@ __host__ __device__ constexpr int halo_min_ctas(int bn, int sa, int cs, int op, 
 // Four phases: j = 2 (2 tap + px) + py, so the tiles of the two warpgroups (py) alternate in the ring.
 template <int PH>
 __host__ __device__ constexpr int halo_wtile(int j) { return PH == 1 ? j : ((j & 1) * 2 + ((j >> 1) & 1)) * 4 + (j >> 2); }
+// First chunk of rank r of a cluster split of a folded-skip chunk list (cpt 3x3 chunks of nine weight tiles, then cpt2
+// skip chunks of one): the chunk boundary nearest to r / cs of the weight tiles.  Rank cs ends the list.
+__host__ __device__ constexpr int halo_fold_c0(int r, int cs, int cpt, int cpt2) {
+    const int target = (r * (9 * cpt + cpt2) + cs / 2) / cs;
+    return target <= 9 * cpt ? (target + 4) / 9 : cpt + target - 9 * cpt;
+}
 
 // every thread of every CTA of the cluster arrives; release / acquire order the shared-memory writes around it
 __device__ __forceinline__ void cluster_sync_all() {
@@ -108,10 +122,12 @@ __device__ __forceinline__ void halo_add_rows(Acc<BN> (&acc)[NACC], const uint8_
 // 256 x 64 and four-phase tiles).  2: no producer warp (256 threads, two CTAs per SM with rings of at most ~113 KB): thread
 // 0 of the consumers issues the loads from inside the MMA loop, and while one CTA transforms a chunk, starts up or drains
 // its accumulator, the other one's MMAs keep the tensor pipe busy.
-template <int BN, int SA, int SB, int CS, int OP, int XF, int WG, int PH = 1, int CTAS = 1>
+// SK: a folded 1x1 skip (see the header): tmA2 / tmB2 are the skip input's halo map and the skip weights (else unused)
+template <int BN, int SA, int SB, int CS, int OP, int XF, int WG, int PH = 1, int CTAS = 1, int SK = 0>
 __global__ void __launch_bounds__(halo_threads(WG, CTAS), halo_min_ctas(BN, SA, CS, OP, WG, PH, CTAS)) conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                                                                 const __grid_constant__ CUtensorMap tmO32, const __grid_constant__ CUtensorMap tmO16,
-                                                                const __grid_constant__ CUtensorMap tmR, const TcParams p) {
+                                                                const __grid_constant__ CUtensorMap tmR, const TcParams p,
+                                                                const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2) {
     static_assert(OP != OP_TF32, "halo kernel: f16 operands");
     static_assert(BN <= 128, "the accumulator of one warpgroup: BN registers per thread");
     static_assert(WG == 1 || (WG == 2 && (CS == 1 || (CS == 2 && CTAS == 1)) && BN <= 64),
@@ -124,6 +140,7 @@ __global__ void __launch_bounds__(halo_threads(WG, CTAS), halo_min_ctas(BN, SA, 
     // in-loop loads (below): at step i thread 0 issues the weight tiles up to i + SB - 2 (four phases: 2 i + SB - 3), and the
     // tiles of step i + 1 must be out before thread 0 waits for them
     static_assert(!SELF_LOAD || SB >= (PH == 1 ? 3 : 6), "weight ring too shallow for loads issued by a consumer");
+    static_assert(!SK || (PH == 1 && XF), "folded skip: the second conv of a ResBlock (3x3, normalised input)");
     constexpr int SLABS = PH == 1 ? WG : 1;                              // 16-row slabs of the tile (8 x 16 pixels each)
     constexpr int NACC = PH == 1 ? 1 : 2;                                // accumulators per warpgroup
     constexpr int TPC = PH == 1 ? 9 : 16;                                // weight tiles per channel chunk
@@ -169,9 +186,20 @@ __global__ void __launch_bounds__(halo_threads(WG, CTAS), halo_min_ctas(BN, SA, 
     const int n0 = blockIdx.y * BN;
     const int split = blockIdx.z;                                        // rank in the cluster (CS == gridDim.z)
     const int c_per = (p.cpt + CS - 1) / CS;
-    const int cb0 = split * c_per;
-    const int nc = max(0, min(p.cpt, cb0 + c_per) - cb0);                // channel chunks of this CTA
-    const int nb = nc * TPC;                                             // weight tiles of this CTA
+    const int cb0 = SK ? halo_fold_c0(split, CS, p.cpt, p.cpt2) : split * c_per;
+    const int nc = SK ? halo_fold_c0(split + 1, CS, p.cpt, p.cpt2) - cb0 : max(0, min(p.cpt, cb0 + c_per) - cb0);   // channel chunks of this CTA
+    const int nconv = SK ? max(0, min(nc, p.cpt - cb0)) : nc;            // of them 3x3 chunks (the rest: skip chunks)
+    const int nb = SK ? nconv * TPC + nc - nconv : nc * TPC;             // weight tiles of this CTA
+    // weight tile j of this CTA: tap j % TPC of chunk j / TPC, then (SK) the one tile of each skip chunk
+    auto load_wtile = [&](int j, uint32_t dst, uint32_t full) {
+        if (SK && j >= nconv * TPC) tma_load_3d(dst, &tmB2, (cb0 + j - nconv * (TPC - 1) - p.cpt) * KCE, n0, 0, full);
+        else tma_load_3d(dst, &tmB, (cb0 + j / TPC) * KCE, n0, halo_wtile<PH>(j % TPC), full);
+    };
+    // the halo of chunk ci of this CTA
+    auto load_halo = [&](int ci, uint32_t dst, uint32_t full) {
+        if (SK && cb0 + ci >= p.cpt) tma_load_4d(dst, &tmA2, (cb0 + ci - p.cpt) * KCE, x0 - 1, y0 - 1, n, full);
+        else tma_load_4d(dst, &tmA, (cb0 + ci) * KCE, x0 - 1, y0 - 1, n, full);
+    };
 
     if (threadIdx.x == 0) {
         // the empty barriers take one arrival per consumer thread: every thread arrives once its own wgmma wait has returned
@@ -192,7 +220,8 @@ __global__ void __launch_bounds__(halo_threads(WG, CTAS), halo_min_ctas(BN, SA, 
         for (int i = 0; i < npre; ++i) {
             const uint32_t full = smem_u32(b_full + i);
             mbar_expect_tx(full, B_BYTES);
-            tma_load_3d(smem_u32(smB + i * B_BYTES), &tmB, (cb0 + i / TPC) * KCE, n0, halo_wtile<PH>(i % TPC), full);
+            if constexpr (SK) load_wtile(i, smem_u32(smB + i * B_BYTES), full);
+            else tma_load_3d(smem_u32(smB + i * B_BYTES), &tmB, (cb0 + i / TPC) * KCE, n0, halo_wtile<PH>(i % TPC), full);
         }
     }
     pdl_wait();
@@ -207,13 +236,16 @@ __global__ void __launch_bounds__(halo_threads(WG, CTAS), halo_min_ctas(BN, SA, 
                     const int sa = ci % SA;
                     mbar_wait(smem_u32(a_empty + sa), ((ci / SA) & 1) ^ 1);
                     mbar_expect_tx(smem_u32(a_full + sa), HALO_ROWS * ROWB);
-                    tma_load_4d(smem_u32(smA + sa * A_BYTES), &tmA, (cb0 + ci) * KCE, x0 - 1, y0 - 1, n, smem_u32(a_full + sa));
-                    for (int tap = 0; tap < TPC; ++tap, ++bi) {
+                    if constexpr (SK) load_halo(ci, smem_u32(smA + sa * A_BYTES), smem_u32(a_full + sa));
+                    else tma_load_4d(smem_u32(smA + sa * A_BYTES), &tmA, (cb0 + ci) * KCE, x0 - 1, y0 - 1, n, smem_u32(a_full + sa));
+                    const int ntile = SK && ci >= nconv ? 1 : TPC;
+                    for (int tap = 0; tap < ntile; ++tap, ++bi) {
                         if (bi < npre) continue;
                         const int sb = bi % SB;
                         mbar_wait(smem_u32(b_empty + sb), ((bi / SB) & 1) ^ 1);
                         mbar_expect_tx(smem_u32(b_full + sb), B_BYTES);
-                        tma_load_3d(smem_u32(smB + sb * B_BYTES), &tmB, (cb0 + ci) * KCE, n0, halo_wtile<PH>(tap), smem_u32(b_full + sb));
+                        if constexpr (SK) load_wtile(bi, smem_u32(smB + sb * B_BYTES), smem_u32(b_full + sb));
+                        else tma_load_3d(smem_u32(smB + sb * B_BYTES), &tmB, (cb0 + ci) * KCE, n0, halo_wtile<PH>(tap), smem_u32(b_full + sb));
                     }
                 }
             }
@@ -246,25 +278,29 @@ __global__ void __launch_bounds__(halo_threads(WG, CTAS), halo_min_ctas(BN, SA, 
                 const int sb = j % SB;
                 mbar_wait(smem_u32(b_empty + sb), ((j / SB) & 1) ^ 1);
                 mbar_expect_tx(smem_u32(b_full + sb), B_BYTES);
-                tma_load_3d(smem_u32(smB + sb * B_BYTES), &tmB, (cb0 + j / TPC) * KCE, n0, halo_wtile<PH>(j % TPC), smem_u32(b_full + sb));
+                if constexpr (SK) load_wtile(j, smem_u32(smB + sb * B_BYTES), smem_u32(b_full + sb));
+                else tma_load_3d(smem_u32(smB + sb * B_BYTES), &tmB, (cb0 + j / TPC) * KCE, n0, halo_wtile<PH>(j % TPC), smem_u32(b_full + sb));
             };
             auto load_a = [&](int ci) {                          // the halo of chunk ci
                 if (ci >= nc) return;
                 const int sa = ci % SA;
                 mbar_wait(smem_u32(a_empty + sa), ((ci / SA) & 1) ^ 1);
                 mbar_expect_tx(smem_u32(a_full + sa), HALO_ROWS * ROWB);
-                tma_load_4d(smem_u32(smA + sa * A_BYTES), &tmA, (cb0 + ci) * KCE, x0 - 1, y0 - 1, n, smem_u32(a_full + sa));
+                if constexpr (SK) load_halo(ci, smem_u32(smA + sa * A_BYTES), smem_u32(a_full + sa));
+                else tma_load_4d(smem_u32(smA + sa * A_BYTES), &tmA, (cb0 + ci) * KCE, x0 - 1, y0 - 1, n, smem_u32(a_full + sa));
             };
             if (SELF_LOAD && te == 0) {                          // the first ring pass: nothing to wait for
                 for (int ci = 0; ci < SA; ++ci) load_a(ci);
                 for (int j = npre; j < min(nb, SB); ++j) {
                     mbar_expect_tx(smem_u32(b_full + j), B_BYTES);
-                    tma_load_3d(smem_u32(smB + j * B_BYTES), &tmB, (cb0 + j / TPC) * KCE, n0, halo_wtile<PH>(j % TPC), smem_u32(b_full + j));
+                    if constexpr (SK) load_wtile(j, smem_u32(smB + j * B_BYTES), smem_u32(b_full + j));
+                    else tma_load_3d(smem_u32(smB + j * B_BYTES), &tmB, (cb0 + j / TPC) * KCE, n0, halo_wtile<PH>(j % TPC), smem_u32(b_full + j));
                 }
             }
             if (XF) {
                 double2* chs = reinterpret_cast<double2*>(xf_A + 2 * p.xf_C);
-                xf_build_coef<128 * WG, XBAR>(p, n, te, hA, hB, chs, cb0 * KCE, (cb0 + nc) * KCE);
+                // SK: the table covers the 3x3 chunks (the skip input is read raw)
+                xf_build_coef<128 * WG, XBAR>(p, n, te, hA, hB, chs, (SK ? min(cb0, p.cpt) : cb0) * KCE, (cb0 + nconv) * KCE);
                 if (te == 0) HSTAMP_END(2, 0);
             }
             int bi = 0;
@@ -272,7 +308,8 @@ __global__ void __launch_bounds__(halo_threads(WG, CTAS), halo_min_ctas(BN, SA, 
                 const int sa = ci % SA;
                 mbar_wait(smem_u32(a_full + sa), (ci / SA) & 1);
                 if (te == 0 && ci == 0) HSTAMP_END(2, 1);
-                if (XF) {
+                const bool skip_chunk = SK && ci >= nconv;
+                if (XF && !skip_chunk) {
                     const int c0 = (cb0 + ci) * KCE;
                     // items = (halo row, half row): 360 / 680 items over 128 / 256 threads; the rows both warpgroups read
                     // are transformed once
@@ -326,6 +363,29 @@ __global__ void __launch_bounds__(halo_threads(WG, CTAS), halo_min_ctas(BN, SA, 
                             if (s == 7) load_a(ci + SA);
                         }
                     }
+                } else if (skip_chunk) {
+                    // a chunk of the folded skip: the centre-tap view of the raw input's halo, one weight tile
+                    const int sb = bi % SB;
+                    mbar_wait(smem_u32(b_full + sb), (bi / SB) & 1);
+                    const uint32_t a0 = a_base + (HALO_W + 1) * ROWB, a1 = a0 + 8 * HALO_W * ROWB;
+                    const uint32_t b_addr = smem_u32(smB + sb * B_BYTES);
+                    wg_fence();
+#pragma unroll
+                    for (int k = 0; k < ROWB / 32; ++k) {
+                        const uint64_t bd = make_smem_desc_sw<ROWB>(b_addr + 32 * k);
+                        const uint32_t accum = (ci > 0 || k > 0) ? 1u : 0u;
+                        Wgmma<BN>::f16(acc[0].d[0], make_desc_sbo<ROWB>(a0 + 32 * k, HALO_W * ROWB), bd, accum);
+                        Wgmma<BN>::f16(acc[0].d[1], make_desc_sbo<ROWB>(a1 + 32 * k, HALO_W * ROWB), bd, accum);
+                    }
+                    wg_commit();
+                    wg_wait<0>();                                               // the chunk's halo and its weight tile are free
+                    mbar_arrive(smem_u32(b_empty + sb));
+                    mbar_arrive(smem_u32(a_empty + sa));
+                    if (SELF_LOAD && te == 0) {                 // tiles up to bi - 1 are released
+                        load_b(bi + SB - 2);
+                        load_a(ci + SA);
+                    }
+                    ++bi;
                 } else {
                     // unrolled: the wait depth and the arrivals below depend on the tap only, so no branch separates wgmma issue
                     // from its wait (a data-dependent one makes ptxas serialise the wgmma)
@@ -359,6 +419,12 @@ __global__ void __launch_bounds__(halo_threads(WG, CTAS), halo_min_ctas(BN, SA, 
                             load_b(bi + SB - 2);
                             if (tap == 8) load_a(ci + SA);
                         }
+                    }
+                    if (SK && ci == nconv - 1) {                // the 3x3 sum in the skip weights' units (a power of two: exact)
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+#pragma unroll
+                            for (int j = 0; j < BN / 2; ++j) acc[0].d[h][j] *= p.acc_rescale;
                     }
                 }
             }
@@ -548,9 +614,19 @@ int halo_plan_cs(long ctas, int chunks, const ConvArgs& a) {
     return g_halo_cs == 2 || (a.ksplit <= 0 && 2 * ctas <= num_sms()) ? 2 : 1;
 }
 
+// Every rank of a cs-way cluster split owns channel chunks (a folded skip's list: halo_fold_c0)
+bool halo_ranks_own_chunks(const ConvWeights& cw, int op, int cs) {
+    const int cpt = cw.cin_pad / op_kch(op), chunks = cpt + cw.cin2_pad / op_kch(op);
+    if (cs > chunks) return false;
+    if (cw.cin2 == 0) return ceil_div(chunks, ceil_div(chunks, cs)) == cs;
+    for (int r = 0; r < cs; ++r)
+        if (halo_fold_c0(r + 1, cs, cpt, chunks - cpt) <= halo_fold_c0(r, cs, cpt, chunks - cpt)) return false;
+    return true;
+}
+
 HaloPlan halo_plan(const ConvWeights& cw, const ConvArgs& a, int op) {
     HaloPlan pl;
-    pl.chunks = cw.cin_pad / op_kch(op);
+    pl.chunks = (cw.cin_pad + cw.cin2_pad) / op_kch(op);      // a folded skip's chunks included
     if (cw.nphase == 4) {
         // one 8 x 16 low-resolution tile (4 x 128 output pixels) x 32 columns per CTA, unsplit
         pl.tiles_x = ceil_div(a.in.W, HT_W); pl.tiles_y = ceil_div(a.in.H, HT_H);
@@ -585,7 +661,7 @@ HaloPlan halo_plan(const ConvWeights& cw, const ConvArgs& a, int op) {
         while (pl.cs < 8 && pl.cs * 2 <= want && pl.cs * 2 <= pl.chunks) pl.cs *= 2;
         while (pl.bn > 32 && (long)pl.tiles_m * (cw.cout_pad / pl.bn) * pl.cs < 96 && cw.cout_pad % (pl.bn / 2) == 0) pl.bn /= 2;
     }
-    while (pl.cs > 1 && (pl.cs > pl.chunks || ceil_div(pl.chunks, ceil_div(pl.chunks, pl.cs)) != pl.cs)) pl.cs /= 2;   // every rank owns chunks
+    while (pl.cs > 1 && !halo_ranks_own_chunks(cw, op, pl.cs)) pl.cs /= 2;
     pl.tiles_n = cw.cout_pad / pl.bn;
     // Unsplit launches with many tiles take 256-pixel tiles: each weight tile then feeds 256 rows instead of 128.  Two
     // 128-column accumulators do not fit the registers of a 288-thread CTA, so 128-column tiles become 256 x 64 (per FLOP:
@@ -603,8 +679,12 @@ HaloPlan halo_plan(const ConvWeights& cw, const ConvArgs& a, int op) {
     return pl;
 }
 
-template <int OP, int BN, int SA, int SB, int CS, int XF, int WG = 1, int PH = 1, int CTAS = 1>
-void launch_halo(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo32, const CUtensorMap& mo16, const CUtensorMap& mr, const TcParams& p, dim3 grid, cudaStream_t s) {
+// The tensor maps of a launch: activation halo, weights, fp32 / f16 output and residual tiles, and a folded skip's input
+// halo and weights (placeholders where a launch does not read them)
+struct HaloMaps { const CUtensorMap *a, *b, *o32, *o16, *r, *a2, *b2; };
+
+template <int OP, int BN, int SA, int SB, int CS, int XF, int WG = 1, int PH = 1, int CTAS = 1, int SK = 0>
+void launch_halo(const HaloMaps& m, const TcParams& p, dim3 grid, cudaStream_t s) {
     constexpr size_t ring = halo_ring(OP, BN, SA, SB, WG, PH);
     constexpr size_t smem0 = halo_smem0(OP, BN, SA, SB, WG, PH);
     static_assert(smem0 <= 227 * 1024, "shared memory budget");
@@ -614,30 +694,32 @@ void launch_halo(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap
     static_assert(CTAS == 1 || 2 * (smem0 + 1024) <= 228 * 1024, "two CTAs per SM");
     const size_t smem = smem0 + (XF ? (size_t)24 * p.xf_C + 32 : 0);
     THA4_REQUIRE(smem <= 227 * 1024, "conv_halo: shared memory budget (fused input normalisation)");
-    THA4_ENSURE_SMEM((conv_halo_kernel<BN, SA, SB, CS, OP, XF, WG, PH, CTAS>), smem);
-    launch_pdl(conv_halo_kernel<BN, SA, SB, CS, OP, XF, WG, PH, CTAS>, grid, dim3(halo_threads(WG, CTAS)), smem, s, CS, ma, mb, mo32, mo16, mr, p);
+    THA4_ENSURE_SMEM((conv_halo_kernel<BN, SA, SB, CS, OP, XF, WG, PH, CTAS, SK>), smem);
+    launch_pdl(conv_halo_kernel<BN, SA, SB, CS, OP, XF, WG, PH, CTAS, SK>, grid, dim3(halo_threads(WG, CTAS)), smem, s, CS,
+               *m.a, *m.b, *m.o32, *m.o16, *m.r, p, *m.a2, *m.b2);
     THA4_LAUNCH_CHECK();
 }
 
 // SBD: weight-ring depth of the cluster split-K launches (few CTAs per SM, the ring is what hides the DRAM latency of weights
 // that are fetched ahead of the dependency wait); SBS: depth of the unsplit launches (many tiles: a shallow ring keeps
 // the CTA small so that 2 - 4 of them share an SM and overlap each other's load -> transform -> MMA -> drain chains).
-template <int OP, int BN, int SA, int SBD, int SBS, int XF>
-void launch_halo_cs(int cs, int wg, int ctas, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo32, const CUtensorMap& mo16, const CUtensorMap& mr, const TcParams& p, dim3 grid, cudaStream_t s) {
+template <int OP, int BN, int SA, int SBD, int SBS, int XF, int SK>
+void launch_halo_cs(int cs, int wg, int ctas, const HaloMaps& m, const TcParams& p, dim3 grid, cudaStream_t s) {
     constexpr int SA1 = OP == OP_F16N ? 2 : 1;
-    THA4_REQUIRE(wg == 1 || (BN <= 64 && (cs == 1 || (cs == 2 && ctas == 1 && p.cpt >= 2))),
+    const int chunks = p.cpt + p.cpt2;
+    THA4_REQUIRE(wg == 1 || (BN <= 64 && (cs == 1 || (cs == 2 && ctas == 1 && chunks >= 2))),
                  "conv_halo: 256-pixel tiles need N tiles of at most 64 columns, unsplit or a pair of one-CTA-per-SM ranks with chunks each");
     THA4_REQUIRE(ctas == 1 || (wg == 2 && BN == 64 && cs == 1), "conv_halo: two CTAs per SM are built for unsplit 256 x 64 tiles");
     if constexpr (BN == 64) {
         if (ctas == 2) {     // one chunk or several: the same rings
-            launch_halo<OP, 64, halo2_sa(OP, 1), halo2_sb(OP, 1), 1, XF, 2, 1, 2>(ma, mb, mo32, mo16, mr, p, grid, s);
+            launch_halo<OP, 64, halo2_sa(OP, 1), halo2_sb(OP, 1), 1, XF, 2, 1, 2, SK>(m, p, grid, s);
             return;
         }
     }
     if constexpr (BN <= 64) {
-        if (cs == 1 && p.cpt == 1) {     // one chunk: one halo, ever -> a ring that fits four times per SM (twice with two warpgroups)
-            if (wg == 2) launch_halo<OP, BN, SA1, halo_sb_wg2(OP, BN, SA1, BN == 64 ? SBD : SBS), 1, XF, 2>(ma, mb, mo32, mo16, mr, p, grid, s);
-            else launch_halo<OP, BN, SA1, SBS, 1, XF>(ma, mb, mo32, mo16, mr, p, grid, s);
+        if (!SK && cs == 1 && chunks == 1) {     // one chunk: one halo, ever -> a ring that fits four times per SM (twice with two warpgroups)
+            if (wg == 2) launch_halo<OP, BN, SA1, halo_sb_wg2(OP, BN, SA1, BN == 64 ? SBD : SBS), 1, XF, 2>(m, p, grid, s);
+            else launch_halo<OP, BN, SA1, SBS, 1, XF>(m, p, grid, s);
             return;
         }
     }
@@ -646,27 +728,27 @@ void launch_halo_cs(int cs, int wg, int ctas, const CUtensorMap& ma, const CUten
             // BN = 64: one CTA per SM, which takes the deep weight ring; BN = 32: two CTAs per SM.  A row-owning pair keeps the rings
             constexpr int M = OP == OP_F16N ? 2 : 1;
             constexpr int SB2 = halo_sb_wg2(OP, BN, SA, BN == 64 ? SBD : 2 * M);
-            if (cs == 2) launch_halo<OP, BN, SA, SB2, 2, XF, 2>(ma, mb, mo32, mo16, mr, p, grid, s);
-            else launch_halo<OP, BN, SA, SB2, 1, XF, 2>(ma, mb, mo32, mo16, mr, p, grid, s);
+            if (cs == 2) launch_halo<OP, BN, SA, SB2, 2, XF, 2, 1, 1, SK>(m, p, grid, s);
+            else launch_halo<OP, BN, SA, SB2, 1, XF, 2, 1, 1, SK>(m, p, grid, s);
             return;
         }
     }
-    if (cs == 8) launch_halo<OP, BN, SA, SBD, 8, XF>(ma, mb, mo32, mo16, mr, p, grid, s);
-    else if (cs == 4) launch_halo<OP, BN, SA, SBD, 4, XF>(ma, mb, mo32, mo16, mr, p, grid, s);
-    else if (cs == 2) launch_halo<OP, BN, SA, SBD, 2, XF>(ma, mb, mo32, mo16, mr, p, grid, s);
+    if (cs == 8) launch_halo<OP, BN, SA, SBD, 8, XF, 1, 1, 1, SK>(m, p, grid, s);
+    else if (cs == 4) launch_halo<OP, BN, SA, SBD, 4, XF, 1, 1, 1, SK>(m, p, grid, s);
+    else if (cs == 2) launch_halo<OP, BN, SA, SBD, 2, XF, 1, 1, 1, SK>(m, p, grid, s);
     else if ((long)grid.x * grid.y * grid.z <= num_sms())
         // unsplit and at most one CTA per SM (e.g. 256 -> 256 channels at 128 x 128: 128 tiles): nothing shares the SM, so the
         // CTA takes the deep weight ring: with a two-stage ring the MMAs wait on weight tiles streaming from L2
-        launch_halo<OP, BN, SA, SBD, 1, XF>(ma, mb, mo32, mo16, mr, p, grid, s);
-    else launch_halo<OP, BN, SA, SBS, 1, XF>(ma, mb, mo32, mo16, mr, p, grid, s);
+        launch_halo<OP, BN, SA, SBD, 1, XF, 1, 1, 1, SK>(m, p, grid, s);
+    else launch_halo<OP, BN, SA, SBS, 1, XF, 1, 1, 1, SK>(m, p, grid, s);
 }
 
-template <int OP, int XF>
-void launch_halo_bn(int bn, int cs, int wg, int ctas, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo32, const CUtensorMap& mo16, const CUtensorMap& mr, const TcParams& p, dim3 grid, cudaStream_t s) {
+template <int OP, int XF, int SK = 0>
+void launch_halo_bn(int bn, int cs, int wg, int ctas, const HaloMaps& m, const TcParams& p, dim3 grid, cudaStream_t s) {
     constexpr int M = OP == OP_F16N ? 2 : 1;        // 64-byte rows: twice the stages for the same bytes in flight
-    if (bn == 128) launch_halo_cs<OP, 128, 2 * M, 6 * M, 3 * M, XF>(cs, wg, ctas, ma, mb, mo32, mo16, mr, p, grid, s);        // unsplit:  95 KB
-    else if (bn == 64) launch_halo_cs<OP, 64, 2 * M, 8 * M, 3 * M, XF>(cs, wg, ctas, ma, mb, mo32, mo16, mr, p, grid, s);     // unsplit:  71 KB
-    else launch_halo_cs<OP, 32, 2 * M, 9 * M, 5 * M, XF>(cs, wg, ctas, ma, mb, mo32, mo16, mr, p, grid, s);                    // unsplit:  67 KB
+    if (bn == 128) launch_halo_cs<OP, 128, 2 * M, 6 * M, 3 * M, XF, SK>(cs, wg, ctas, m, p, grid, s);        // unsplit:  95 KB
+    else if (bn == 64) launch_halo_cs<OP, 64, 2 * M, 8 * M, 3 * M, XF, SK>(cs, wg, ctas, m, p, grid, s);     // unsplit:  71 KB
+    else launch_halo_cs<OP, 32, 2 * M, 9 * M, 5 * M, XF, SK>(cs, wg, ctas, m, p, grid, s);                    // unsplit:  67 KB
 }
 
 bool g_use_halo = true;
@@ -680,9 +762,16 @@ void conv_halo_set_m256(int mode) { g_halo_m256 = mode; }
 void conv_halo_set_ctas(int mode) { g_halo_ctas = mode; }
 void conv_halo_set_cs(int mode) { g_halo_cs = mode; }
 
+// One operand format for both sources of a folded skip: 64-channel chunks only when both widths allow them
+static int halo_op(const ConvWeights& cw) { return cw.cin_pad % 64 == 0 && cw.cin2_pad % 64 == 0 ? OP_F16 : OP_F16N; }
+
 bool conv_halo_supported(const ConvWeights& cw, const ConvArgs& a) {
     if (!g_use_halo || !conv_tc_supported(cw, a)) return false;
     if (!a.in.f16 || cw.stride != 1) return false;
+    // a folded 1x1 conv: its f16 input at the output's resolution, TMA-able, on the 3x3 normalised-input kernels
+    if (cw.cin2 > 0 && (!cw.w16b || cw.ntaps != 9 || cw.nphase != 1 || !a.nin.on || a.res.p || !a.in2.f16 || !a.in2.p || a.in2.C != cw.cin2 ||
+                        a.in2.N != a.out.N || a.in2.H != a.out.H || a.in2.W != a.out.W || a.in2.ld % 8 != 0 || (((uintptr_t)a.in2.p) & 15) != 0))
+        return false;
     const bool four_phase = cw.nphase == 4 && cw.ntaps == 4 && cw.out_mul == 2;
     if (!four_phase && (cw.ntaps != 9 || cw.nphase != 1 || cw.out_mul != 1)) return false;
     for (int ph = 0; ph < cw.nphase; ++ph)
@@ -704,7 +793,7 @@ bool conv_halo_fuses_stats(const ConvWeights&, const ConvArgs&) { return true; }
 void conv_halo_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s) {
     THA4_REQUIRE(conv_halo_supported(cw, a), "conv_halo: unsupported configuration");
     THA4_REQUIRE(a.in.C == cw.cin && a.out.C == cw.cout && a.in.N == a.out.N, "conv_halo: shapes");
-    const int op = cw.cin_pad % 64 == 0 ? OP_F16 : OP_F16N;
+    const int op = halo_op(cw);
     TcParams p{};
     p.out = a.out.p; p.outH = a.out.H; p.outW = a.out.W; p.outC = a.out.C; p.out_ld = a.out.ld;
     p.out16 = a.out16.p ? a.out16.hp() : nullptr; p.out16_ld = a.out16.ld;
@@ -727,7 +816,7 @@ void conv_halo_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s)
     const HaloPlan pl = halo_plan(cw, a, op);
     p.MH = a.out.H / cw.out_mul; p.MW = a.out.W / cw.out_mul; p.tiles_x = pl.tiles_x; p.tiles_y = pl.tiles_y;
     p.pre_b = cw.dynamic ? 0 : 1;
-    p.ntaps = cw.ntaps; p.cpt = pl.chunks;
+    p.ntaps = cw.ntaps; p.cpt = cw.cin_pad / op_kch(op); p.cpt2 = cw.cin2_pad / op_kch(op);
     if (!cw.w16) { conv_make_half(cw, s); p.pre_b = 0; }
     p.acc_scale = 1.0f / cw.w16_scale;
     for (int ph = 0; ph < cw.nphase; ++ph) {
@@ -745,12 +834,22 @@ void conv_halo_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s)
         p.dbg = g_dbg_buf;
     }
     ProfScope prof(PROF_CONV, s);
-    prof_add_work(PROF_CONV, 2.0 * (double)p.N * p.MH * p.MW * cw.cout * cw.cin * cw.ntaps * cw.nphase, 0.0);
+    prof_add_work(PROF_CONV, 2.0 * (double)p.N * p.MH * p.MW * cw.cout * (cw.cin * cw.ntaps * cw.nphase + cw.cin2), 0.0);
     const CUtensorMap& ma = halo_activation_map(a.in, op, cw.nphase == 1 ? pl.wg : 1);
     const CUtensorMap& mb = halo_weight_map(cw, pl.bn, op);
     const CUtensorMap* mo32 = &ma;                   // placeholders when an output does not leave through TMA
     const CUtensorMap* mo16 = &ma;
     const CUtensorMap* mr = &ma;
+    const CUtensorMap* ma2 = &ma;
+    const CUtensorMap* mb2 = &mb;
+    if (cw.cin2 > 0) {                               // the folded skip: its input's halo and the weight segment after the taps
+        ConvWeights seg = cw;
+        seg.w16 = cw.w16b; seg.cin_pad = cw.cin2_pad; seg.ntaps = 1;
+        ma2 = &halo_activation_map(a.in2, op, pl.wg);
+        mb2 = &halo_weight_map(seg, pl.bn, op);
+        p.acc_scale = 1.0f / cw.w16b_scale;
+        p.acc_rescale = cw.w16b_scale / cw.w16_scale;
+    }
     p.st_tma = 0;
     if ((pl.cs == 1 || pl.wg == 2) && g_tma_store && cw.nphase == 1) {
         if (a.out.p && halo_store_map(a.out, false, &mo32)) p.st_tma |= 1;
@@ -762,31 +861,35 @@ void conv_halo_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s)
     p.vec4 = ((!cw.bias || (reinterpret_cast<uintptr_t>(cw.bias) & 15) == 0) &&
               (!a.res.p || ((reinterpret_cast<uintptr_t>(a.res.p) & 15) == 0 && a.res.ld % 4 == 0))) ? 1 : 0;
     dim3 grid(pl.tiles_m, pl.tiles_n, pl.cs);
-    if (cw.nphase == 4) {
+    const HaloMaps m{&ma, &mb, mo32, mo16, mr, ma2, mb2};
+    if (cw.cin2 > 0) {
+        if (op == OP_F16) launch_halo_bn<OP_F16, 1, 1>(pl.bn, pl.cs, pl.wg, pl.ctas, m, p, grid, s);
+        else launch_halo_bn<OP_F16N, 1, 1>(pl.bn, pl.cs, pl.wg, pl.ctas, m, p, grid, s);
+    } else if (cw.nphase == 4) {
         // OP_F16 (conv_halo_supported).  One CTA per SM: the ring takes two halo stages and a whole chunk of weight tiles;
         // two: see halo2_sb
         constexpr int SA2 = halo2_sa(OP_F16, 4), SB2 = halo2_sb(OP_F16, 4);
         if (pl.ctas == 2) {
-            if (a.nin.on) launch_halo<OP_F16, 32, SA2, SB2, 1, 1, 2, 4, 2>(ma, mb, *mo32, *mo16, *mr, p, grid, s);
-            else launch_halo<OP_F16, 32, SA2, SB2, 1, 0, 2, 4, 2>(ma, mb, *mo32, *mo16, *mr, p, grid, s);
+            if (a.nin.on) launch_halo<OP_F16, 32, SA2, SB2, 1, 1, 2, 4, 2>(m, p, grid, s);
+            else launch_halo<OP_F16, 32, SA2, SB2, 1, 0, 2, 4, 2>(m, p, grid, s);
         } else if (pl.cs == 2) {         // a row-owning pair: the one-CTA-per-SM rings
             THA4_REQUIRE(pl.chunks >= 2, "conv_halo: a row-owning pair needs a channel chunk per rank");
-            if (a.nin.on) launch_halo<OP_F16, 32, 2, 16, 2, 1, 2, 4>(ma, mb, *mo32, *mo16, *mr, p, grid, s);
-            else launch_halo<OP_F16, 32, 2, 16, 2, 0, 2, 4>(ma, mb, *mo32, *mo16, *mr, p, grid, s);
-        } else if (a.nin.on) launch_halo<OP_F16, 32, 2, 16, 1, 1, 2, 4>(ma, mb, *mo32, *mo16, *mr, p, grid, s);
-        else launch_halo<OP_F16, 32, 2, 16, 1, 0, 2, 4>(ma, mb, *mo32, *mo16, *mr, p, grid, s);
+            if (a.nin.on) launch_halo<OP_F16, 32, 2, 16, 2, 1, 2, 4>(m, p, grid, s);
+            else launch_halo<OP_F16, 32, 2, 16, 2, 0, 2, 4>(m, p, grid, s);
+        } else if (a.nin.on) launch_halo<OP_F16, 32, 2, 16, 1, 1, 2, 4>(m, p, grid, s);
+        else launch_halo<OP_F16, 32, 2, 16, 1, 0, 2, 4>(m, p, grid, s);
     } else if (op == OP_F16) {
-        if (a.nin.on) launch_halo_bn<OP_F16, 1>(pl.bn, pl.cs, pl.wg, pl.ctas, ma, mb, *mo32, *mo16, *mr, p, grid, s);
-        else launch_halo_bn<OP_F16, 0>(pl.bn, pl.cs, pl.wg, pl.ctas, ma, mb, *mo32, *mo16, *mr, p, grid, s);
+        if (a.nin.on) launch_halo_bn<OP_F16, 1>(pl.bn, pl.cs, pl.wg, pl.ctas, m, p, grid, s);
+        else launch_halo_bn<OP_F16, 0>(pl.bn, pl.cs, pl.wg, pl.ctas, m, p, grid, s);
     } else {
-        if (a.nin.on) launch_halo_bn<OP_F16N, 1>(pl.bn, pl.cs, pl.wg, pl.ctas, ma, mb, *mo32, *mo16, *mr, p, grid, s);
-        else launch_halo_bn<OP_F16N, 0>(pl.bn, pl.cs, pl.wg, pl.ctas, ma, mb, *mo32, *mo16, *mr, p, grid, s);
+        if (a.nin.on) launch_halo_bn<OP_F16N, 1>(pl.bn, pl.cs, pl.wg, pl.ctas, m, p, grid, s);
+        else launch_halo_bn<OP_F16N, 0>(pl.bn, pl.cs, pl.wg, pl.ctas, m, p, grid, s);
     }
     static const bool dbg_all = dbg_env && !strcmp(getenv("THA4_HALO_DEBUG"), "2");
     if (dbg_all) {       // developer: stamps of every launch of a real forward (serialises the stream)
-        fprintf(stderr, "halo launch: N %d %dx%d cin %d cout %d | bn %d cs %d wg %d chunks %d grid %d x %d | xf %d groups %d act %d res %d out32 %d out16 %d st_tma %d | phases %d ctas %d\n",
+        fprintf(stderr, "halo launch: N %d %dx%d cin %d cout %d | bn %d cs %d wg %d chunks %d grid %d x %d | xf %d groups %d act %d res %d out32 %d out16 %d st_tma %d | phases %d ctas %d | cin2 %d\n",
                 p.N, p.MH, p.MW, cw.cin, cw.cout, pl.bn, pl.cs, pl.wg, pl.chunks, pl.tiles_m, pl.tiles_n, a.nin.on ? 1 : 0, p.xf_groups, p.xf_act,
-                p.res_mode, p.out ? 1 : 0, p.out16 ? 1 : 0, p.st_tma, cw.nphase, pl.ctas);
+                p.res_mode, p.out ? 1 : 0, p.out16 ? 1 : 0, p.st_tma, cw.nphase, pl.ctas, cw.cin2);
         conv_halo_debug_dump();
     }
 }

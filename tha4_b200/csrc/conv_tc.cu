@@ -455,6 +455,24 @@ void conv_make_half(const ConvWeights& cw, cudaStream_t s) {
     cw.w16 = h; cw.w16_scale = scale;
 }
 
+__global__ void bias_sum_kernel(float* __restrict__ dst, const float* __restrict__ a, const float* __restrict__ b, int n) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) dst[i] = (a ? a[i] : 0.0f) + (b ? b[i] : 0.0f);
+}
+
+void conv_make_fold(ConvWeights& fold, const ConvWeights& conv3, const ConvWeights& conv1x1, cudaStream_t s) {
+    THA4_REQUIRE(conv3.ntaps == 9 && conv3.nphase == 1 && conv1x1.ntaps == 1 && conv1x1.nphase == 1 && conv3.cout_pad == conv1x1.cout_pad &&
+                 conv3.w16 && conv1x1.w16, "conv_make_fold: a 3x3 and a 1x1 conv of the same width, with f16 copies");
+    float* bias = reinterpret_cast<float*>(tracked_malloc(conv3.cout * sizeof(float)));
+    bias_sum_kernel<<<ceil_div(conv3.cout, 128), 128, 0, s>>>(bias, conv3.bias, conv1x1.bias, conv3.cout);
+    THA4_LAUNCH_CHECK();
+    fold = conv3;
+    fold.w = nullptr;                                                          // f16 only: the halo kernel's operands
+    fold.bias = bias;
+    fold.cin2 = conv1x1.cin; fold.cin2_pad = conv1x1.cin_pad;
+    fold.w16b = conv1x1.w16; fold.w16b_scale = conv1x1.w16_scale;
+}
+
 void conv_tc_enable_cluster(bool on) { g_use_cluster = on; }
 void conv_tc_enable_stride2(bool on) { g_use_s2 = on; }
 void conv_tc_enable_small_bn(bool on) { g_small_bn = on; }

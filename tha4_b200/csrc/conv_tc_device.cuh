@@ -77,6 +77,8 @@ struct TcParams {
     signed char dy[CONV_MAX_PHASES][CONV_MAX_TAPS];
     signed char dx[CONV_MAX_PHASES][CONV_MAX_TAPS];
     signed char ph_oy[CONV_MAX_PHASES], ph_ox[CONV_MAX_PHASES];
+    int cpt2;                                      // conv_halo.cu: channel chunks of a folded 1x1 skip's input (after the cpt 3x3 chunks)
+    float acc_rescale;                             // conv_halo.cu, folded skip: power of two that takes the 3x3 chunks' sum to the skip weights' scale
 };
 
 // CS > 1: the K dimension is split over a thread-block cluster of CS CTAs (cluster dims {1,1,CS} along blockIdx.z); the

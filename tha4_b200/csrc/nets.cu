@@ -215,10 +215,12 @@ ConvNormIn norm_in(const View& src_stats, const NormW& nw, int groups, int act, 
 
 // conv on the wgmma kernel: `in` is an f16 operand view (or fp32 for the first layer of a network), `nin` its pending
 // normalisation (nullptr: none), `out` receives the fp32 and / or f16 copies it has storage for, plus statistics
+// (in2: the f16 input of a folded 1x1 conv, cw.cin2 > 0)
 void run_conv_tc(Runtime& rt, const ConvWeights& cw, const View& in, const ConvNormIn* nin, const Tens& out,
-                 const View* res = nullptr, int res_mode = RES_NONE) {
+                 const View* res = nullptr, int res_mode = RES_NONE, const View* in2 = nullptr) {
     ConvArgs a;
     a.in = in; a.out = out.f; a.out16 = out.h; a.strict = 0;
+    if (in2) a.in2 = *in2;
     if (nin) a.nin = *nin;
     if (res) { a.res = *res; a.res_mode = res_mode; }
     const size_t ws = conv_workspace_floats(cw, a);
@@ -437,6 +439,8 @@ UNetNet::UNetNet(bool upscaler, int size, int model_channels, std::vector<int> m
 
 namespace {
 
+bool g_skip_fold = true;
+
 ResBlockW load_res_block(const StateDict& sd, const std::string& p, cudaStream_t s, bool upsampling = false) {
     ResBlockW w;
     w.norm0 = load_norm(sd, p + ".norm0", s);
@@ -446,6 +450,9 @@ ResBlockW load_res_block(const StateDict& sd, const std::string& p, cudaStream_t
     w.cin = w.conv0.cin; w.cout = w.conv0.cout;
     w.has_skip = sd.count(p + ".skip.weight") > 0;
     if (w.has_skip) w.skip = load_conv(sd, p + ".skip", CONV_1x1, true, s);
+    // default mode (f16 copies): conv1 and the skip as one K, with bias b1 + b_skip (the separate convs stay: strict mode
+    // and the backward's adjoints)
+    if (w.has_skip && w.conv1.w16 && w.skip.w16) conv_make_fold(w.fold, w.conv1, w.skip, s);
     return w;
 }
 
@@ -736,8 +743,12 @@ struct UNetFused {
         const int act = ACT_SILU_FAST;
         Tens h0 = make_act(tape ? rt.persist : rt.scratch, rt, B, out.f.H, out.f.W, w.cout, false, true);
         if (tape) tape->res[&w] = {mode == 2 ? x.f : op_view(x), raw_view(h0)};
+        // conv1 with the skip folded into its K loop: one launch, no skip(x) tensor, no fork / join around it
+        ConvArgs fa;
+        fa.in = h0.h; fa.out = out.f; fa.out16 = out.h; fa.in2 = x.h; fa.nin.on = true;
+        const bool fold = mode == 0 && w.fold.cin2 > 0 && g_skip_fold && conv_halo_supported(w.fold, fa);
         Tens sk;
-        if (w.has_skip) {
+        if (w.has_skip && !fold) {
             // skip(x) depends on x only: it runs on the side stream next to norm0 -> conv0 (a latency-bound chain,
             // ~30 times per frame) and is joined in front of conv1, which adds it as the residual
             sk = make_act(rt.scratch, rt, B, x.f.H, x.f.W, w.cout, true, false, false);
@@ -765,7 +776,9 @@ struct UNetFused {
         }
         // norm1 -> FiLM(time) -> FiLM(pose) -> SiLU, folded into one per-(n,c) affine inside conv1
         const ConvNormIn n1 = norm_in(h0.f, w.norm1, 32, act, w.film0, film1 + w.film1_off, film1_total);
-        if (w.has_skip) {
+        if (fold) {
+            run_conv_tc(rt, w.fold, h0.h, &n1, out, nullptr, RES_NONE, &x.h);
+        } else if (w.has_skip) {
             THA4_REQUIRE(mode == 0, "res_block: skip conv only on same-resolution blocks");
             if (rt.side) THA4_CUDA_CHECK(cudaStreamWaitEvent(rt.stream, rt.ev_join, 0));
             run_conv_tc(rt, w.conv1, h0.h, &n1, out, &sk.f, RES_SAME);
@@ -916,5 +929,8 @@ void UNetNet::forward_fused(Runtime& rt, const ImgView& image, const float* coar
         tail_forward(TAIL_UNET, tail_, feat.f, coef, ACT_SILU_FAST, image, none, outputs, s, rt.strict);
     }
 }
+
+void unet_set_skip_fold(bool on) { g_skip_fold = on; }
+bool unet_skip_fold() { return g_skip_fold; }
 
 }  // namespace tha4

@@ -106,6 +106,7 @@ struct ResBlockW {
     int cin = 0, cout = 0;
     NormW norm0, norm1;
     ConvWeights conv0, conv1, skip;
+    ConvWeights fold;           // default mode: conv1 with the skip folded into its K (fold.cin2 > 0; conv_make_fold), else empty
     bool has_skip = false;
     float* film0 = nullptr;     // [2*cout], constant (t = 0 time embedding, unet.py:365-376)
     int film1_off = 0;          // offset of this block's 2*cout FiLM vector in the batched pose projection
@@ -198,5 +199,9 @@ void head_pack_adjoint(ConvWeights& cw, const TailWeights& tw, bool round_w, cud
 // flipped, 1x1 -> 1x1 with W^T, CONV_UP2_3x3 (nearest x2 + 3x3, pre-summed phases) -> 4x4 stride-2 conv with W^T.  Allocates
 // cw.w with tracked_malloc; the values are those of fwd (TF32-rounded iff fwd's are).
 void conv_adjoint_from_packed(ConvWeights& cw, const ConvWeights& fwd, ConvKind kind, cudaStream_t s);
+
+// Option "skip_fold" (default on): the default mode runs a U-Net ResBlock's 1x1 skip inside conv1's K loop (ResBlockW::fold)
+void unet_set_skip_fold(bool on);
+bool unet_skip_fold();
 
 }  // namespace tha4
