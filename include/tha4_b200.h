@@ -368,6 +368,36 @@ int tha4_test_conv_backward_data_ex(tha4_ctx* ctx, int kind, const float* w, con
 /* linear_backward: dx[n][k] = SiLU'(pre[n][k]) sum_r dy[n][r] W[r][k] (pre NULL: no SiLU'), W [R][K] */
 int tha4_test_linear_backward(tha4_ctx* ctx, const float* dy, int dy_ld, int N, int R, const float* W, int K, const float* pre, int pre_ld,
                               float* dx, int dx_ld, void* stream);
+/* The default-mode forward kernels in the layouts the networks run them, on caller-owned device buffers so that a test can
+ * chain launches into one concatenation buffer.  Tensors are NHWC, given by a pointer to their channel 0 and a pixel stride;
+ * statistics slots by a pointer to their first column, a per-sample column stride stats_ld, `rep` replicas and the replica
+ * stride in doubles ([rep][N][stats_ld][2] when the stride is N * stats_ld * 2).
+ *
+ * One conv through conv_forward: kind and weights (w [Cout,Cin,k,k], or [Cin,Cout,4,4] for kind 2; TF32-rounded and f16-packed
+ * as the networks pack them) as tha4_test_conv; in [N,H,W,Cin] f16.  w_skip [Cout,Cin2,1,1] / b_skip / in2 [N,Ho,Wo,Cin2] f16:
+ * a 1x1 skip folded into the 3x3 conv (conv_make_fold), or NULL.  out (fp32) and out16 (f16) are optional (at least one);
+ * out_stats (or NULL) accumulates the output's per-(n, c) sums.  res fp32 with res_mode as tha4_test_conv (or NULL).  norm_C > 0:
+ * the pending GroupNorm(groups) / InstanceNorm (groups 0) of the first norm_C input channels from in_stats, with gamma / beta,
+ * film0 [2 norm_C] and film1 rows of film1_ld floats (or NULL), act 0 / 1 ReLU / 2 SiLU (run as the default mode's fast SiLU).
+ * plan (host, 10 ints, may be NULL): [0] the kernel that ran (1 halo, 2 tensor-core, 3 mma.sync); for the halo kernel [1] N tile
+ * [2] cluster size [3] consumer warpgroups [4] CTAs per SM [5] phases [6] TMA-store bits (1 fp32 out, 2 f16 out, 4 residual box)
+ * [7] channel chunks [8] 1 when the skip was folded; [9] the tensor-core split plan (as tha4_test_conv_backward_data_ex). */
+int tha4_test_conv_forward_ex(tha4_ctx* ctx, int kind, const float* w, const float* bias, int Cin, int Cout, const float* w_skip,
+                              const float* b_skip, int Cin2, const void* in, int in_ld, int N, int H, int W, const void* in2, int in2_ld,
+                              float* out, int out_ld, void* out16, int out16_ld, double* out_stats, int out_stats_ld, int out_stats_rep,
+                              int64_t out_stats_rep_stride, const float* res, int res_ld, int res_mode, const double* in_stats,
+                              int in_stats_ld, int in_stats_rep, int64_t in_stats_rep_stride, int norm_C, int groups, int act,
+                              const float* gamma, const float* beta, const float* film0, const float* film1, int film1_ld, int ksplit,
+                              int* plan, void* stream);
+/* The default mode's fused tail (tail_tc_forward) on a raw f16 feature map [N,S,S,C] and its statistics replicas; heads,
+ * gamma / beta / groups / act and outputs as tha4_test_tail.  image0 / image1 NCHW [.,4,S,S] with batch strides image*_sn
+ * (0: one image for every sample); g0 / g1: their interleaved NHWC copies with pixel stride g*_ld (a slice of the network
+ * input), or NULL (the kernel then reads the NCHW images). */
+int tha4_test_tail_ex(tha4_ctx* ctx, int kind, const void* feature, int N, int C, int S, const double* stats, int stats_ld, int stats_rep,
+                      int64_t stats_rep_stride, const float* gamma, const float* beta, int groups, int act, const float* head_w,
+                      const float* head_b, const int* head_cout, int n_heads, const float* image0, int64_t image0_sn,
+                      const float* image1, int64_t image1_sn, const float* g0, int g0_ld, const float* g1, int g1_ld,
+                      float* const* outputs, void* stream);
 /* qkv_attention, "new order" (src/tha4/nn/common/unet.py:192-202): qkv [N,3C,16,16] -> out [N,C,16,16] */
 int tha4_test_attention(tha4_ctx* ctx, const float* qkv, int N, int C, int heads, float* out, void* stream);
 /* y[n][o] = b[o] + sum_i f(x[n][i]) W[o][i] */

@@ -1365,6 +1365,117 @@ int tha4_test_linear_backward(tha4_ctx* ctx, const float* dy, int dy_ld, int N, 
     return guarded(ctx, [&] { linear_backward(dy, dy_ld, N, R, W, K, pre, pre_ld, dx, dx_ld, (cudaStream_t)stream); });
 }
 
+// One default-mode conv through conv_forward as run_conv_tc issues it, on the caller's own device buffers (views addressed by
+// a pointer to their channel 0, a pixel stride and, for statistics, a column stride and replicas).  Weights are packed as
+// the networks pack them: TF32-rounded, an f16 copy, and conv_make_fold when a 1x1 skip is given.
+int tha4_test_conv_forward_ex(tha4_ctx* ctx, int kind, const float* w, const float* bias, int Cin, int Cout, const float* w_skip,
+                              const float* b_skip, int Cin2, const void* in, int in_ld, int N, int H, int W, const void* in2, int in2_ld,
+                              float* out, int out_ld, void* out16, int out16_ld, double* out_stats, int out_stats_ld, int out_stats_rep,
+                              int64_t out_stats_rep_stride, const float* res, int res_ld, int res_mode, const double* in_stats,
+                              int in_stats_ld, int in_stats_rep, int64_t in_stats_rep_stride, int norm_C, int groups, int act,
+                              const float* gamma, const float* beta, const float* film0, const float* film1, int film1_ld, int ksplit,
+                              int* plan, void* stream) {
+    return guarded(ctx, [&] {
+        cudaStream_t s = (cudaStream_t)stream;
+        THA4_REQUIRE(kind >= CONV_3x3 && kind <= CONV_UP2_3x3 && Cin % 8 == 0 && (out || out16), "test_conv_forward_ex: kind 0..4, Cin % 8 == 0, an output");
+        THA4_REQUIRE((w_skip != nullptr) == (in2 != nullptr) && (!w_skip || (kind == CONV_3x3 && Cin2 % 8 == 0)),
+                     "test_conv_forward_ex: a folded skip needs its weights, its input and a 3x3 conv");
+        THA4_REQUIRE(res_mode >= RES_NONE && res_mode <= RES_DOWN2 && (res != nullptr) == (res_mode != RES_NONE),
+                     "test_conv_forward_ex: res with res_mode 1..3, or neither");
+        begin_pass(ctx, s);
+        AllocSink sink;
+        ConvWeights cw, sw, fw;
+        {
+            SinkScope own(&sink);
+            conv_set_pack_rounding(true);
+            for (int k = 0; k < (w_skip ? 2 : 1); ++k) {
+                ConvWeights& c = k ? sw : cw;
+                const ConvKind ck = k ? CONV_1x1 : (ConvKind)kind;
+                conv_describe(c, ck, k ? Cin2 : Cin, Cout);
+                c.tf32_rounded = true;
+                c.w = reinterpret_cast<float*>(tracked_malloc(conv_packed_floats(c) * sizeof(float)));
+                THA4_CUDA_CHECK(cudaMemsetAsync(c.w, 0, conv_packed_floats(c) * sizeof(float), s));
+                conv_pack(c, ck, k ? w_skip : w, k ? Cin2 : Cin, 0, s);
+                conv_make_half(c, s);
+            }
+            cw.bias = const_cast<float*>(bias); sw.bias = const_cast<float*>(b_skip);
+            if (w_skip) conv_make_fold(fw, cw, sw, s);
+        }
+        const bool x2 = (kind == CONVT_4x4_S2 || kind == CONV_UP2_3x3);
+        const int Ho = (kind == CONV_4x4_S2) ? H / 2 : (x2 ? H * 2 : H), Wo = (kind == CONV_4x4_S2) ? W / 2 : (x2 ? W * 2 : W);
+        ConvArgs a;
+        a.in = nhwc_view(in, N, H, W, Cin, in_ld, 1);
+        a.out = nhwc_view(out, N, Ho, Wo, Cout, out ? out_ld : out16_ld);
+        if (out_stats) {
+            a.out.stats = out_stats; a.out.stats_ld = out_stats_ld; a.out.stats_rep = out_stats_rep; a.out.stats_rep_stride = (long)out_stats_rep_stride;
+        }
+        if (out16) a.out16 = nhwc_view(out16, N, Ho, Wo, Cout, out16_ld, 1);
+        if (in2) a.in2 = nhwc_view(in2, N, Ho, Wo, Cin2, in2_ld, 1);
+        if (res) {
+            const int rs = res_mode == RES_UP2 ? 2 : 1, rd = res_mode == RES_DOWN2 ? 2 : 1;
+            a.res = nhwc_view(res, N, Ho * rd / rs, Wo * rd / rs, Cout, res_ld);
+            a.res_mode = res_mode;
+        }
+        if (norm_C > 0) {
+            ConvNormIn& n = a.nin;
+            n.on = true; n.C = norm_C; n.groups = groups; n.act = act == ACT_SILU ? ACT_SILU_FAST : act;
+            n.gamma = gamma; n.beta = beta; n.film0 = film0; n.film1 = film1; n.film1_ld = film1_ld;
+            n.stats = in_stats; n.stats_ld = in_stats_ld; n.stats_rep = in_stats_rep; n.stats_rep_stride = (long)in_stats_rep_stride;
+        }
+        a.ksplit = ksplit;
+        const ConvWeights& c = w_skip ? fw : cw;
+        const size_t wsf = conv_workspace_floats(c, a);
+        if (wsf) { a.ws = ctx->scratch.alloc(wsf); a.ws_floats = wsf; }
+        THA4_REQUIRE(!a.out.stats || conv_fuses_stats(c, a), "test_conv_forward_ex: statistics must be fused on the tensor-core path");
+        if (plan) {      // [0] 1 halo / 2 tensor-core / 3 mma.sync; halo: [1] bn [2] cs [3] wg [4] ctas [5] phases [6] st_tma [7] chunks;
+                         // [8] folded skip; [9] conv_tc_split_plan
+            for (int i = 0; i < 10; ++i) plan[i] = 0;
+            const bool halo = conv_tc_enabled() && conv_halo_plan_info(c, a, plan + 1);
+            plan[0] = halo ? 1 : (conv_tc_enabled() && conv_tc_supported(c, a) ? 2 : 3);
+            plan[8] = halo && c.cin2 > 0 ? 1 : 0;
+            plan[9] = conv_tc_split_plan(c, a);
+        }
+        conv_forward(c, a, s);
+        THA4_CUDA_CHECK(cudaStreamSynchronize(s));       // `sink` frees the weights on return
+    });
+}
+
+// tail_tc_forward on the caller's raw f16 feature map [N][S][S][C] and statistics replicas.  image0 / image1: NCHW with a batch
+// stride (0: one image for every sample) for the ImgView reads; g0 / g1: optional NHWC fp32 copies (pixel stride g_ld, e.g. a
+// slice of the network input), else the kernel reads the ImgViews.
+int tha4_test_tail_ex(tha4_ctx* ctx, int kind, const void* feature, int N, int C, int S, const double* stats, int stats_ld, int stats_rep,
+                      int64_t stats_rep_stride, const float* gamma, const float* beta, int groups, int act, const float* head_w,
+                      const float* head_b, const int* head_cout, int n_heads, const float* image0, int64_t image0_sn,
+                      const float* image1, int64_t image1_sn, const float* g0, int g0_ld, const float* g1, int g1_ld,
+                      float* const* outputs, void* stream) {
+    return guarded(ctx, [&] {
+        cudaStream_t s = (cudaStream_t)stream;
+        begin_pass(ctx, s);
+        View f = nhwc_view(feature, N, S, S, C, C, 1);
+        f.stats = const_cast<double*>(stats); f.stats_ld = stats_ld; f.stats_rep = stats_rep; f.stats_rep_stride = (long)stats_rep_stride;
+        AllocSink sink;
+        TailWeights tw;
+        {
+            SinkScope own(&sink);
+            tail_init(tw, C, s);
+            size_t woff = 0, boff = 0;
+            for (int i = 0; i < n_heads; ++i) {
+                const bool has_b = head_b != nullptr && !((kind == TAIL_COMBINER || kind == TAIL_FACE) && i == 0);   // grid_change heads have no bias
+                tail_add(tw, head_w + woff, has_b ? head_b + boff : nullptr, head_cout[i], s);
+                woff += (size_t)head_cout[i] * C * 9; boff += head_cout[i];
+            }
+            tail_make_half(tw, s);
+        }
+        NormSpecTail ns; ns.groups = groups; ns.act = act == ACT_SILU ? ACT_SILU_FAST : act; ns.gamma = gamma; ns.beta = beta;
+        ImgView i0 = make_img(image0, N, 4, S, S), i1 = image1 ? make_img(image1, N, 4, S, S) : ImgView{};
+        i0.sn = (long)image0_sn;
+        if (image1) i1.sn = (long)image1_sn;
+        const View gv0 = nhwc_view(g0, N, S, S, 4, g0_ld), gv1 = nhwc_view(g1, N, S, S, 4, g1_ld);
+        tail_tc_forward((TailKind)kind, tw, f, ns, i0, i1, outputs, s, g0 ? &gv0 : nullptr, g1 ? &gv1 : nullptr);
+        THA4_CUDA_CHECK(cudaStreamSynchronize(s));       // `sink` frees the head weights on return
+    });
+}
+
 int tha4_test_attention(tha4_ctx* ctx, const float* qkv, int N, int C, int heads, float* out, void* stream) {
     return guarded(ctx, [&] {
         cudaStream_t s = (cudaStream_t)stream;

@@ -107,6 +107,10 @@ int conv_tc_split_plan(const ConvWeights& cw, const ConvArgs& a);
 // row-shifted UMMA descriptors); preferred over conv_tc_forward when it supports the configuration
 bool conv_halo_supported(const ConvWeights& cw, const ConvArgs& a);
 void conv_halo_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s);
+// The halo launch conv_halo_forward(cw, a) would make, from the same plan (false: not the halo kernel).  info[0..6]: N tile
+// width, cluster size, consumer warpgroups, resident CTAs per SM, phases, TMA-store bits (1 fp32 out, 2 f16 out, 4 residual
+// box), channel chunks
+bool conv_halo_plan_info(const ConvWeights& cw, const ConvArgs& a, int* info);
 void conv_halo_enable(bool on);
 void conv_halo_enable_tma_store(bool on);
 void conv_halo_set_ctas(int mode);        // option "halo_ctas": -1 automatic (default), 1 / 2 CTAs per SM for the 256 x 64 and four-phase halo tiles

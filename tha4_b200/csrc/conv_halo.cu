@@ -790,6 +790,30 @@ bool conv_halo_supported(const ConvWeights& cw, const ConvArgs& a) {
 
 bool conv_halo_fuses_stats(const ConvWeights&, const ConvArgs&) { return true; }       // unsplit or cluster split: always final
 
+// Which outputs of a launch with plan `pl` leave through TMA stores (bit 0 fp32, bit 1 f16) and whether the residual arrives
+// through the same box (bit 2); the maps of those that do
+static int halo_st_tma(const ConvWeights& cw, const ConvArgs& a, const HaloPlan& pl, const CUtensorMap** mo32, const CUtensorMap** mo16,
+                       const CUtensorMap** mr) {
+    int st = 0;
+    if ((pl.cs == 1 || pl.wg == 2) && g_tma_store && cw.nphase == 1) {
+        if (a.out.p && halo_store_map(a.out, false, mo32)) st |= 1;
+        if (a.out16.p && halo_store_map(a.out16, true, mo16)) st |= 2;
+        // the residual of a ResBlock's second conv has the geometry of the fp32 output: it arrives through the same box
+        if ((st & 1) && a.res.p && a.res_mode == RES_SAME && !a.res.f16 && a.res.N == a.out.N && a.res.H == a.out.H &&
+            a.res.W == a.out.W && a.res.C >= a.out.C && halo_store_map(a.res, false, mr)) st |= 4;
+    }
+    return st;
+}
+
+bool conv_halo_plan_info(const ConvWeights& cw, const ConvArgs& a, int* info) {
+    if (!conv_halo_supported(cw, a)) return false;
+    const HaloPlan pl = halo_plan(cw, a, halo_op(cw));
+    const CUtensorMap *m32 = nullptr, *m16 = nullptr, *mr = nullptr;
+    info[0] = pl.bn; info[1] = pl.cs; info[2] = pl.wg; info[3] = pl.ctas; info[4] = cw.nphase;
+    info[5] = halo_st_tma(cw, a, pl, &m32, &m16, &mr); info[6] = pl.chunks;
+    return true;
+}
+
 void conv_halo_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s) {
     THA4_REQUIRE(conv_halo_supported(cw, a), "conv_halo: unsupported configuration");
     THA4_REQUIRE(a.in.C == cw.cin && a.out.C == cw.cout && a.in.N == a.out.N, "conv_halo: shapes");
@@ -850,14 +874,7 @@ void conv_halo_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s)
         p.acc_scale = 1.0f / cw.w16b_scale;
         p.acc_rescale = cw.w16b_scale / cw.w16_scale;
     }
-    p.st_tma = 0;
-    if ((pl.cs == 1 || pl.wg == 2) && g_tma_store && cw.nphase == 1) {
-        if (a.out.p && halo_store_map(a.out, false, &mo32)) p.st_tma |= 1;
-        if (a.out16.p && halo_store_map(a.out16, true, &mo16)) p.st_tma |= 2;
-        // the residual of a ResBlock's second conv has the geometry of the fp32 output: it arrives through the same box
-        if ((p.st_tma & 1) && a.res.p && p.res_mode == RES_SAME && !a.res.f16 && a.res.N == a.out.N && a.res.H == a.out.H &&
-            a.res.W == a.out.W && a.res.C >= a.out.C && halo_store_map(a.res, false, &mr)) p.st_tma |= 4;
-    }
+    p.st_tma = halo_st_tma(cw, a, pl, &mo32, &mo16, &mr);
     p.vec4 = ((!cw.bias || (reinterpret_cast<uintptr_t>(cw.bias) & 15) == 0) &&
               (!a.res.p || ((reinterpret_cast<uintptr_t>(a.res.p) & 15) == 0 && a.res.ld % 4 == 0))) ? 1 : 0;
     dim3 grid(pl.tiles_m, pl.tiles_n, pl.cs);
