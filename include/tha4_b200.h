@@ -66,14 +66,13 @@ const char* tha4_last_error(const tha4_ctx* ctx);
  *          "skip_fold" (1: the 1x1 skip of a U-Net ResBlock runs inside the K loop of the block's second conv, one halo launch;
  *                       0: its own launch on the side stream, added as conv1's residual),
  *          "cluster_splitk" (1: K-split convs reduce through a thread-block cluster / DSMEM; 0: workspace + reduce kernel),
- *          "pdl" (1: programmatic dependent launch), "tc_stride2" (1: 4x4 stride-2 convs on the wgmma kernel),
- *          "small_bn" (1: narrower N tiles for small unsplit launches), "siren_tc" (1: students on the wgmma kernels; 0: mma.sync kernels),
- *          "attn_split16", "attn_mma" (1: default-mode attention on mma.sync with f16 operands; 0: the fp32 kernel everywhere),
+ *          "siren_tc" (1: students on the wgmma kernels; 0: mma.sync kernels, one character only),
+ *          "tail_persist" (1: persistent pipelined decoder tail; 0: one tile per CTA),
  *          "profile" (1: time every kernel class with CUDA events on the launching stream, 2: same + reset, 0: off).
- * "strict", "microbatch", "cuda_graphs" and "half_operands" belong to the context.  The other developer switches select
- * kernels PROCESS-WIDE (they are statics of the kernel translation units): changing one on any context changes it for all
- * contexts of the process, and every change drops the captured graphs / cached outputs of the context it was made on.
- * A context is used by one thread at a time; the tensor-map caches shared between contexts are mutex-protected. */
+ * Every option belongs to the context it is set on, except "profile": the profiler's accumulators, like the
+ * "kernel_launches" counter, belong to the process, so profiling is on or off for all contexts.  Every change drops the
+ * context's captured graphs.  A context is used by one thread at a time; the tensor-map caches shared between contexts
+ * are mutex-protected. */
 int tha4_set_option(tha4_ctx* ctx, const char* name, int64_t value);
 /* counters: "kernel_launches" (kernels this library has launched so far, replayed graph nodes included), "workspace_bytes",
  *           "graph_replays" / "graph_captures" / "graph_failures",

@@ -5,7 +5,9 @@ sys.path.insert(0, _ROOT)
 sys.path.insert(0, os.path.join(_ROOT, 'tests'))
 from tha4_b200 import synthetic
 from tha4_b200.poser.modes import mode_07
-opt = sys.argv[1] if len(sys.argv) > 1 else 'small_bn'
+if len(sys.argv) != 2:
+    sys.exit('usage: debug_ab.py OPTION   (an on/off option of tha4_set_option, e.g. skip_fold)')
+opt = sys.argv[1]
 dev = torch.device('cuda:0')
 poser = mode_07.create_poser(dev, state_dicts=synthetic.teacher_state_dicts(0))
 ctx = poser.get_context()

@@ -12,13 +12,12 @@ constexpr int L = 256, D = 32;
 
 // grid = N * heads * (L / QPB), block = 256 threads = QPB queries x KSPLIT key splits.  Each thread runs an online softmax
 // over its L / KSPLIT keys; the KSPLIT partial (max, sum, acc) triples of a query are merged with warp shuffles.
-//   <64, 4, 36>: 4 CTAs per (sample, head) -- the measured default;  row pitch 36: the 4 key-split lanes hit 4 banks.
-//   <16, 16, 33>: 16 CTAs per (sample, head) for B=1 latency (128 CTAs instead of 32); row pitch 33: the 16 key-split
-//                 lanes read 16 consecutive rows = 16 different banks.  Opt-in (option "attn_split16"), not yet measured.
+// Launched as <64, 4, 36>: 4 CTAs per (sample, head); row pitch 36 (16-byte aligned rows): the 4 key-split lanes hit 4 banks.
 template <int QPB, int KSPLIT, int DP>
 __global__ void __launch_bounds__(QPB * KSPLIT) attention_kernel(const float* __restrict__ qkv, int qkv_ld, int C, int heads,
                                                                  float* __restrict__ out, int out_ld) {
     static_assert(QPB * KSPLIT == L, "one thread per token while staging K / V");
+    static_assert(DP % 4 == 0, "K / V rows are staged as float4");
     extern __shared__ __align__(16) float sm[];
     float* Ks = sm;            // [L][DP]
     float* Vs = sm + L * DP;   // [L][DP]
@@ -33,14 +32,8 @@ __global__ void __launch_bounds__(QPB * KSPLIT) attention_kernel(const float* __
 #pragma unroll
         for (int j = 0; j < D / 4; ++j) {
             const float4 kv = kp[j], vv = vp[j];
-            if (DP % 4 == 0) {
-                reinterpret_cast<float4*>(Ks + tid * DP)[j] = kv;
-                reinterpret_cast<float4*>(Vs + tid * DP)[j] = vv;
-            } else {        // odd pitch: rows are not 16-byte aligned
-                float* kd = Ks + tid * DP + 4 * j; float* vd = Vs + tid * DP + 4 * j;
-                kd[0] = kv.x; kd[1] = kv.y; kd[2] = kv.z; kd[3] = kv.w;
-                vd[0] = vv.x; vd[1] = vv.y; vd[2] = vv.z; vd[3] = vv.w;
-            }
+            reinterpret_cast<float4*>(Ks + tid * DP)[j] = kv;
+            reinterpret_cast<float4*>(Vs + tid * DP)[j] = vv;
         }
     }
     const int t = qq * QPB + tid / KSPLIT;      // query token
@@ -232,34 +225,22 @@ __global__ void __launch_bounds__(AT_WARPS * 32) attention_mma_kernel(const floa
     }
 }
 
-bool g_attn_split16 = false;
-bool g_attn_mma = true;           // option "attn_mma": the tensor-core kernel serves the default mode
-
-template <int QPB, int KSPLIT, int DP>
-void launch_attention(const View& qkv, int heads, const View& out, cudaStream_t s) {
-    const size_t smem = 2 * L * DP * sizeof(float);
-    THA4_ENSURE_SMEM((attention_kernel<QPB, KSPLIT, DP>), smem);
-    attention_kernel<QPB, KSPLIT, DP><<<qkv.N * heads * (L / QPB), QPB * KSPLIT, smem, s>>>(qkv.p, qkv.ld, out.C, heads, out.p, out.ld);
-    THA4_LAUNCH_CHECK();
-}
-
 }  // namespace
-
-void attention_enable_split16(bool on) { g_attn_split16 = on; }
-
-void attention_enable_mma(bool on) { g_attn_mma = on; }
 
 void attention_forward(const View& qkv, int heads, const View& out, cudaStream_t s, bool fast) {
     THA4_REQUIRE(qkv.H * qkv.W == L && out.C * 3 == qkv.C && out.C / heads == D, "attention: shape (L=256, head dim 32)");
     THA4_REQUIRE(qkv.ld % 4 == 0 && out.ld % 4 == 0, "attention: alignment");
     ProfScope prof(PROF_ATTN, s);
-    if (fast && g_attn_mma) {
+    if (fast) {
         attention_mma_kernel<<<qkv.N * heads * (L / (AT_WARPS * 16)), AT_WARPS * 32, 0, s>>>(qkv.p, qkv.ld, out.C, heads, out.p, out.ld);
         THA4_LAUNCH_CHECK();
         return;
     }
-    if (g_attn_split16) launch_attention<16, 16, 33>(qkv, heads, out, s);
-    else launch_attention<64, 4, 36>(qkv, heads, out, s);
+    constexpr int QPB = 64, KSPLIT = 4, DP = 36;
+    constexpr size_t smem = 2 * L * DP * sizeof(float);
+    THA4_ENSURE_SMEM((attention_kernel<QPB, KSPLIT, DP>), smem);
+    attention_kernel<QPB, KSPLIT, DP><<<qkv.N * heads * (L / QPB), QPB * KSPLIT, smem, s>>>(qkv.p, qkv.ld, out.C, heads, out.p, out.ld);
+    THA4_LAUNCH_CHECK();
 }
 
 }  // namespace tha4

@@ -12,7 +12,7 @@
 
 namespace tha4 {
 std::atomic<long> g_kernel_launches{0};
-bool g_use_pdl = true;
+thread_local const Options* g_options = nullptr;
 thread_local AllocSink* g_alloc_sink = nullptr;
 void* tracked_malloc(size_t bytes) {
     void* p = nullptr;
@@ -39,12 +39,11 @@ constexpr int GRAPH_CACHE = 8;
 
 struct tha4_ctx {
     int device = 0;
-    int use_graphs = 1;        // option "cuda_graphs" (default on): single-chunk teacher forwards replay as one graph launch
+    Options opt;
     std::map<std::vector<uintptr_t>, TeacherGraph> graphs;
     std::map<std::vector<uintptr_t>, int> graph_seen;      // how often a key was seen before it was captured
     long graph_clock = 0, graph_misses = 0, graph_pause = 0, graph_replays = 0, graph_captures = 0, graph_failures = 0;
-    int side_streams = 1;        // option "side_stream": independent DAG branches (ResBlock skip convs) on a second stream
-    cudaStream_t side = nullptr;
+    cudaStream_t side = nullptr;   // independent DAG branches (ResBlock skip convs) run on a second stream
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     cudaStream_t capture_stream = nullptr;   // the legacy default stream cannot be captured: its graphs are recorded here and launched there
     float* pose_stage = nullptr;   // [1024][45]: graphs read the pose from here, so the caller's pose address is not part of the key
@@ -57,9 +56,6 @@ struct tha4_ctx {
         graph_pause = 0;
     }
     std::string err;
-    int strict = 0;
-    int microbatch = 32;                   // frames per internal pass
-    int half_operands = 1;                 // f16 conv operands between normalisation and wgmma conv (non-strict mode)
     Pool persist, scratch;
     int* flag = nullptr;
     double* loss_acc = nullptr;            // 4 doubles: L1 sums of the distillation step
@@ -81,6 +77,7 @@ int guarded(tha4_ctx* ctx, F&& f) {
     if (!ctx) return THA4_ERR_INVALID;
     try {
         THA4_CUDA_CHECK(cudaSetDevice(ctx->device));
+        OptionsScope bind(&ctx->opt);      // per call, not per thread: autograd runs the backward entries on its own thread
         f();
         return THA4_OK;
     } catch (const CudaError& e) {
@@ -94,10 +91,10 @@ int guarded(tha4_ctx* ctx, F&& f) {
 
 Runtime make_rt(tha4_ctx* ctx, void* stream) {
     Runtime rt;
-    rt.persist = &ctx->persist; rt.scratch = &ctx->scratch; rt.stream = (cudaStream_t)stream; rt.strict = ctx->strict;
-    rt.f16 = ctx->half_operands && !ctx->strict && conv_tc_enabled();
+    rt.persist = &ctx->persist; rt.scratch = &ctx->scratch; rt.stream = (cudaStream_t)stream; rt.strict = ctx->opt.strict;
+    rt.f16 = ctx->opt.half_operands && !ctx->opt.strict && ctx->opt.tcgen05;
     rt.stats_base = ctx->stats_base; rt.stats_cap = ctx->stats_cap; rt.stats_off = &ctx->stats_off;
-    if (ctx->side_streams && !prof_enabled()) {
+    if (!prof_enabled()) {
         if (!ctx->side) {
             THA4_CUDA_CHECK(cudaStreamCreateWithFlags(&ctx->side, cudaStreamNonBlocking));
             THA4_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming));
@@ -257,27 +254,24 @@ int tha4_set_option(tha4_ctx* ctx, const char* name, int64_t value) {
     return guarded(ctx, [&] {
         cudaDeviceSynchronize();
         ctx->drop_graphs();                   // every option can change the launch sequence
-        if (!strcmp(name, "strict")) { ctx->strict = value ? 1 : 0; }
-        else if (!strcmp(name, "cuda_graphs")) ctx->use_graphs = value ? 1 : 0;
-        else if (!strcmp(name, "side_stream")) ctx->side_streams = value ? 1 : 0;
-        else if (!strcmp(name, "tcgen05")) conv_enable_tc(value != 0);
-        else if (!strcmp(name, "cluster_splitk")) conv_tc_enable_cluster(value != 0);
-        else if (!strcmp(name, "halo_conv")) conv_halo_enable(value != 0);
-        else if (!strcmp(name, "tma_store")) conv_halo_enable_tma_store(value != 0);
-        else if (!strcmp(name, "halo_m256")) { THA4_REQUIRE(value >= -1 && value <= 1, "halo_m256: -1, 0 or 1"); conv_halo_set_m256((int)value); }
-        else if (!strcmp(name, "halo_ctas")) { THA4_REQUIRE(value == -1 || value == 1 || value == 2, "halo_ctas: -1, 1 or 2"); conv_halo_set_ctas((int)value); }
-        else if (!strcmp(name, "halo_cs")) { THA4_REQUIRE(value == -1 || value == 1 || value == 2, "halo_cs: -1, 1 or 2"); conv_halo_set_cs((int)value); }
-        else if (!strcmp(name, "skip_fold")) unet_set_skip_fold(value != 0);
-        else if (!strcmp(name, "siren_tc")) siren_tc_enable(value != 0);
-        else if (!strcmp(name, "tc_stride2")) conv_tc_enable_stride2(value != 0);
-        else if (!strcmp(name, "small_bn")) conv_tc_enable_small_bn(value != 0);
-        else if (!strcmp(name, "attn_split16")) attention_enable_split16(value != 0);
-        else if (!strcmp(name, "tail_persist")) tail_tc_enable_persist(value != 0);
-        else if (!strcmp(name, "attn_mma")) attention_enable_mma(value != 0);
-        else if (!strcmp(name, "half_operands")) ctx->half_operands = value ? 1 : 0;
-        else if (!strcmp(name, "pdl")) g_use_pdl = value != 0;
-        else if (!strcmp(name, "profile")) { prof_enable(value != 0); if (value == 2) prof_reset(); }
-        else if (!strcmp(name, "microbatch")) { THA4_REQUIRE(value >= 1 && value <= 1024, "microbatch range"); ctx->microbatch = (int)value; }
+        Options& o = ctx->opt;
+        const bool on = value != 0;
+        if (!strcmp(name, "strict")) o.strict = on;
+        else if (!strcmp(name, "cuda_graphs")) o.cuda_graphs = on;
+        else if (!strcmp(name, "tcgen05")) o.tcgen05 = on;
+        else if (!strcmp(name, "cluster_splitk")) o.cluster_splitk = on;
+        else if (!strcmp(name, "halo_conv")) o.halo_conv = on;
+        else if (!strcmp(name, "tma_store")) o.tma_store = on;
+        else if (!strcmp(name, "halo_m256")) { THA4_REQUIRE(value >= -1 && value <= 1, "halo_m256: -1, 0 or 1"); o.halo_m256 = (int)value; }
+        else if (!strcmp(name, "halo_ctas")) { THA4_REQUIRE(value == -1 || value == 1 || value == 2, "halo_ctas: -1, 1 or 2"); o.halo_ctas = (int)value; }
+        else if (!strcmp(name, "halo_cs")) { THA4_REQUIRE(value == -1 || value == 1 || value == 2, "halo_cs: -1, 1 or 2"); o.halo_cs = (int)value; }
+        else if (!strcmp(name, "skip_fold")) o.skip_fold = on;
+        else if (!strcmp(name, "siren_tc")) o.siren_tc = on;
+        else if (!strcmp(name, "tail_persist")) o.tail_persist = on;
+        else if (!strcmp(name, "half_operands")) o.half_operands = on;
+        // the one process-wide option: the profiler's accumulators belong to the process, like the kernel_launches counter
+        else if (!strcmp(name, "profile")) { prof_enable(on); if (value == 2) prof_reset(); }
+        else if (!strcmp(name, "microbatch")) { THA4_REQUIRE(value >= 1 && value <= 1024, "microbatch range"); o.microbatch = (int)value; }
         else throw std::runtime_error(std::string("tha4: unknown option ") + name);
     });
 }
@@ -308,7 +302,7 @@ int tha4_load_net(tha4_ctx* ctx, int net, int n_tensors, const char* const* keys
         cudaStream_t s = (cudaStream_t)stream;
         cudaDeviceSynchronize();
         ctx->drop_graphs();                   // graphs hold pointers to the previous weights
-        conv_set_pack_rounding(!ctx->strict);     // non-strict: weights are rounded to TF32 once, at pack time
+        conv_set_pack_rounding(!ctx->opt.strict);     // non-strict: weights are rounded to TF32 once, at pack time
         switch (net) {
             case THA4_NET_EYEBROW_DECOMPOSER: ctx->decomposer.reset(new EncDecNet(TAIL_DECOMPOSER, 128, 4, 0)); ctx->decomposer->load(sd, s); break;
             case THA4_NET_EYEBROW_MORPHING_COMBINER: ctx->combiner.reset(new EncDecNet(TAIL_COMBINER, 128, 8, 12)); ctx->combiner->load(sd, s); break;
@@ -326,7 +320,7 @@ int tha4_load_net(tha4_ctx* ctx, int net, int n_tensors, const char* const* keys
 int tha4_eyebrow_decomposer_forward(tha4_ctx* ctx, const float* image, int B, float* const* outputs, void* stream) {
     return guarded(ctx, [&] {
         Runtime rt = make_rt(ctx, stream);
-        for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
+        for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             float* o[6]; offset_outputs<6>(outputs, kEncDecDecomposer, n0, o);
             ctx->decomposer->forward(rt, make_img(image + (size_t)n0 * 4 * 128 * 128, b, 4, 128, 128), ImgView{}, nullptr, 0, o);
         });
@@ -337,7 +331,7 @@ int tha4_eyebrow_morphing_combiner_forward(tha4_ctx* ctx, const float* backgroun
                                            const float* pose, int pose_ld, int B, float* const* outputs, void* stream) {
     return guarded(ctx, [&] {
         Runtime rt = make_rt(ctx, stream);
-        for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
+        for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             float* o[8]; offset_outputs<8>(outputs, kCombiner, n0, o);
             const size_t off = (size_t)n0 * 4 * 128 * 128;
             ctx->combiner->forward(rt, make_img(eyebrow_layer + off, b, 4, 128, 128), make_img(background_layer + off, b, 4, 128, 128),
@@ -350,7 +344,7 @@ int tha4_face_morpher_forward(tha4_ctx* ctx, const float* image, const float* po
                               float* const* outputs, void* stream) {
     return guarded(ctx, [&] {
         Runtime rt = make_rt(ctx, stream);
-        for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
+        for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             float* o[8]; offset_outputs<8>(outputs, kFace, n0, o);
             ctx->face->forward(rt, make_img(image + (size_t)n0 * 4 * 192 * 192, b, 4, 192, 192), ImgView{},
                                pose + (size_t)n0 * pose_ld, pose_ld, o);
@@ -363,7 +357,7 @@ int tha4_eyebrow_decomposer_backward(tha4_ctx* ctx, const float* image, int B, c
     return guarded(ctx, [&] {
         THA4_REQUIRE(d_image != nullptr, "decomposer backward: no gradient requested");
         Runtime rt = make_rt(ctx, stream);
-        for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
+        for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             const float* g[6]; offset_grads<6>(grad_outputs, kEncDecDecomposer, n0, g);
             EncDecGrads eg; eg.grad_outputs = g; eg.d_image0 = d_image + (size_t)n0 * 4 * 128 * 128;
             ctx->decomposer->backward(rt, make_img(image + (size_t)n0 * 4 * 128 * 128, b, 4, 128, 128), ImgView{}, nullptr, 0, eg);
@@ -378,7 +372,7 @@ int tha4_eyebrow_morphing_combiner_backward(tha4_ctx* ctx, const float* backgrou
         THA4_REQUIRE(d_background_layer || d_eyebrow_layer || d_pose, "combiner backward: no gradient requested");
         THA4_REQUIRE(pose_ld >= 12, "combiner backward: pose rows need at least 12 entries");
         Runtime rt = make_rt(ctx, stream);
-        for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
+        for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             const float* g[8]; offset_grads<8>(grad_outputs, kCombiner, n0, g);
             const size_t off = (size_t)n0 * 4 * 128 * 128;
             EncDecGrads eg; eg.grad_outputs = g;
@@ -397,7 +391,7 @@ int tha4_face_morpher_backward(tha4_ctx* ctx, const float* image, const float* p
         THA4_REQUIRE(d_image || d_pose, "face morpher backward: no gradient requested");
         THA4_REQUIRE(pose_ld >= 27, "face morpher backward: pose rows need at least 27 entries");
         Runtime rt = make_rt(ctx, stream);
-        for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
+        for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             const float* g[8]; offset_grads<8>(grad_outputs, kFace, n0, g);
             EncDecGrads eg; eg.grad_outputs = g;
             eg.d_image0 = d_image ? d_image + (size_t)n0 * 4 * 192 * 192 : nullptr;
@@ -413,7 +407,7 @@ int tha4_morpher_forward(tha4_ctx* ctx, const float* image, const float* pose, i
     return guarded(ctx, [&] {
         Runtime rt = make_rt(ctx, stream);
         OutSpec spec[5]; fill_unet_spec(spec, 256);
-        for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
+        for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             float* o[5]; offset_outputs<5>(outputs, spec, n0, o);
             ctx->body->forward(rt, make_img(image + (size_t)n0 * 4 * 256 * 256, b, 4, 256, 256), nullptr, nullptr, 0,
                                pose + (size_t)n0 * pose_ld, pose_ld, o);
@@ -428,7 +422,7 @@ int tha4_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, 
         THA4_REQUIRE(pose_ld >= 6, "morpher backward: pose rows need at least 6 entries");
         Runtime rt = make_rt(ctx, stream);
         OutSpec spec[5]; fill_unet_spec(spec, 256);
-        for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
+        for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             const float* g[5]; offset_grads<5>(grad_outputs, spec, n0, g);
             UNetGrads ug; ug.grad_outputs = g;
             ug.d_image = d_image ? d_image + (size_t)n0 * 4 * 256 * 256 : nullptr;
@@ -449,7 +443,7 @@ int tha4_upscaler_backward(tha4_ctx* ctx, const float* rest_image, const float* 
         Runtime rt = make_rt(ctx, stream);
         OutSpec spec[5]; fill_unet_spec(spec, 512);
         const size_t hw = 512 * 512, chw = (size_t)coarse_size * coarse_size;
-        for_chunks(ctx, B, std::min(ctx->microbatch, UPSCALER_BWD_MAX_BATCH), rt.stream, [&](int n0, int b) {
+        for_chunks(ctx, B, std::min(ctx->opt.microbatch, UPSCALER_BWD_MAX_BATCH), rt.stream, [&](int n0, int b) {
             const float* g[5]; offset_grads<5>(grad_outputs, spec, n0, g);
             UNetGrads ug; ug.grad_outputs = g;
             ug.d_image = d_rest_image ? d_rest_image + (size_t)n0 * 4 * hw : nullptr;
@@ -468,7 +462,7 @@ int tha4_upscaler_forward(tha4_ctx* ctx, const float* rest_image, const float* c
     return guarded(ctx, [&] {
         Runtime rt = make_rt(ctx, stream);
         OutSpec spec[5]; fill_unet_spec(spec, 512);
-        for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
+        for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             float* o[5]; offset_outputs<5>(outputs, spec, n0, o);
             ctx->upscaler->forward(rt, make_img(rest_image + (size_t)n0 * 4 * 512 * 512, b, 4, 512, 512),
                                    coarse_posed_image + (size_t)n0 * 4 * coarse_size * coarse_size,
@@ -514,7 +508,7 @@ int tha4_teacher_forward(tha4_ctx* ctx, int mode, const float* image, int64_t im
         for (int i = 0; i < 6; ++i) spec[n++] = kEncDecDecomposer[i];
         const int nout = n;
         auto run = [&](const float* img_p, const float* pose_p, float* const* outs, const float* const* cached_p) {
-            for_chunks(ctx, B, ctx->microbatch, rt.stream, [&](int n0, int b) {
+            for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
                 float* o[33];
                 for (int i = 0; i < nout; ++i) o[i] = outs[i] ? outs[i] + (size_t)n0 * spec[i].c * spec[i].s * spec[i].s : nullptr;
                 const float* cd[6];
@@ -527,7 +521,7 @@ int tha4_teacher_forward(tha4_ctx* ctx, int mode, const float* image, int64_t im
         // ---- CUDA-graph path: single-chunk calls whose buffer addresses repeat ----
         cudaStream_t s = rt.stream;
         if (ctx->graph_pause > 0) --ctx->graph_pause;
-        if (ctx->use_graphs && B <= ctx->microbatch && B <= 1024 && !prof_enabled() && ctx->graph_pause == 0) {
+        if (ctx->opt.cuda_graphs && B <= ctx->opt.microbatch && B <= 1024 && !prof_enabled() && ctx->graph_pause == 0) {
             if (!ctx->pose_stage) THA4_CUDA_CHECK(cudaMalloc(&ctx->pose_stage, 1024 * 45 * sizeof(float)));
             std::vector<uintptr_t> key;
             key.reserve(nout + 12);
@@ -829,7 +823,7 @@ int tha4_test_conv(tha4_ctx* ctx, int kind, const float* x, const float* w, cons
         View yo = mk(Ho, Wo, Cout);
         ConvArgs a;
         a.in = xin; a.in_up = in_up; a.out = yo; a.strict = strict; a.ksplit = ksplit;
-        if (ctx->half_operands && !strict && conv_tc_enabled() && cin_k % 8 == 0 && conv_tc_supported(cw, a)) {
+        if (ctx->opt.half_operands && !strict && ctx->opt.tcgen05 && cin_k % 8 == 0 && conv_tc_supported(cw, a)) {
             // exercise the f16-operand variant the networks use between a normalisation layer and a conv
             View x16 = xin; x16.f16 = 1; x16.p = P->alloc((xin.pixels() * cin_k + 1) / 2);
             convert_f16(xin, x16, s);
@@ -1001,7 +995,7 @@ int tha4_test_conv_skip_fold(tha4_ctx* ctx, const float* x, int N, int Cmid, int
             SinkScope own(&sink);
             conv_make_fold(fw, cw, sw, s);
         }
-        const bool fold = unet_skip_fold() && conv_halo_supported(fw, fa);     // as UNetNet's default mode decides (res_block)
+        const bool fold = ctx->opt.skip_fold && conv_halo_supported(fw, fa);     // as UNetNet's default mode decides (res_block)
         // the unfused pair: skip(x) in fp32, then conv1 adds it as its residual
         View sk = mk(N, H, W, Cout);
         ConvArgs sa; sa.in = x16; sa.out = sk;
@@ -1430,8 +1424,8 @@ int tha4_test_conv_forward_ex(tha4_ctx* ctx, int kind, const float* w, const flo
         if (plan) {      // [0] 1 halo / 2 tensor-core / 3 mma.sync; halo: [1] bn [2] cs [3] wg [4] ctas [5] phases [6] st_tma [7] chunks;
                          // [8] folded skip; [9] conv_tc_split_plan
             for (int i = 0; i < 10; ++i) plan[i] = 0;
-            const bool halo = conv_tc_enabled() && conv_halo_plan_info(c, a, plan + 1);
-            plan[0] = halo ? 1 : (conv_tc_enabled() && conv_tc_supported(c, a) ? 2 : 3);
+            const bool halo = ctx->opt.tcgen05 && conv_halo_plan_info(c, a, plan + 1);
+            plan[0] = halo ? 1 : (ctx->opt.tcgen05 && conv_tc_supported(c, a) ? 2 : 3);
             plan[8] = halo && c.cin2 > 0 ? 1 : 0;
             plan[9] = conv_tc_split_plan(c, a);
         }
@@ -1484,7 +1478,7 @@ int tha4_test_attention(tha4_ctx* ctx, const float* qkv, int N, int C, int heads
         View q; q.N = N; q.H = 16; q.W = 16; q.C = 3 * C; q.ld = 3 * C; q.p = P->alloc((size_t)N * 256 * 3 * C);
         nchw_to_nhwc(make_img(qkv, N, 3 * C, 16, 16), q, s);
         View o; o.N = N; o.H = 16; o.W = 16; o.C = C; o.ld = C; o.p = P->alloc((size_t)N * 256 * C);
-        attention_forward(q, heads, o, s, !ctx->strict);
+        attention_forward(q, heads, o, s, !ctx->opt.strict);
         nhwc_to_nchw(o, out, s);
     });
 }

@@ -13,7 +13,36 @@
 namespace tha4 {
 
 extern std::atomic<long> g_kernel_launches;   // every kernel this library launches is counted (bench "gpu_launches")
-extern bool g_use_pdl;                        // programmatic dependent launch on the kernels that support it (option "pdl")
+
+// The options of one context (tha4_set_option): its precision mode and which kernel and plan each launch takes.  Every API
+// call binds its context's options to the calling thread for the duration of the call (OptionsScope), so the dispatchers
+// read those of the context that is running; outside a call, opts() returns the defaults.
+struct Options {
+    bool strict = false;        // 3xTF32 error-compensated products (fp32-equivalent teacher convs) instead of TF32 / f16 operands
+    int microbatch = 32;        // frames per internal pass of the teacher pipeline, 1..1024
+    bool cuda_graphs = true;    // single-chunk teacher forwards on a repeating buffer set replay as one captured graph
+    bool half_operands = true;  // f16 conv operands between a normalisation and the wgmma conv that reads it (non-strict mode)
+    bool tcgen05 = true;        // convs on the wgmma / TMA kernels; off: every conv on mma.sync (the name is historical)
+    bool cluster_splitk = true; // K-split wgmma convs reduce through a thread-block cluster; off: through a workspace or atomics
+    bool halo_conv = true;      // 3x3 stride-1 and four-phase convs on the halo-reuse kernel; off: on conv_tc.cu
+    bool tma_store = true;      // unsplit halo epilogues through shared-memory staging and TMA stores; off: plain stores
+    int halo_m256 = -1;         // -1 automatic; 0 / 1 force 128- / 256-pixel tiles on unsplit halo launches
+    int halo_ctas = -1;         // -1 automatic; 1 / 2 force one 288-thread / two 256-thread CTAs per SM (256 x 64 and four-phase tiles)
+    int halo_cs = -1;           // -1 automatic; 1 never / 2 always (where legal) split a two-warpgroup halo launch over a cluster pair
+    bool skip_fold = true;      // a U-Net ResBlock's 1x1 skip runs inside conv1's K loop (halo kernel); off: its own launch
+    bool siren_tc = true;       // SIREN students on the wgmma kernels; off: on the mma.sync kernels (one character only)
+    bool tail_persist = true;   // persistent pipelined wgmma decoder tail; off: one tile per CTA
+};
+extern thread_local const Options* g_options;
+inline const Options& opts() {
+    static const Options defaults;
+    return g_options ? *g_options : defaults;
+}
+struct OptionsScope {
+    const Options* prev;
+    explicit OptionsScope(const Options* o) : prev(g_options) { g_options = o; }
+    ~OptionsScope() { g_options = prev; }
+};
 
 // NHWC fp32 activation view.  `ld` is the pixel stride in floats (>= C) so that a tensor can live in a channel
 // slice of a wider buffer (U-Net skip concatenation is free: producers write into their slice).
@@ -111,12 +140,9 @@ inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = s;
     cudaLaunchAttribute attr[2];
-    int na = 0;
-    if (g_use_pdl) {
-        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[na].val.programmaticStreamSerializationAllowed = 1;
-        ++na;
-    }
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    int na = 1;
     if (cluster_z > 1) {
         attr[na].id = cudaLaunchAttributeClusterDimension;
         attr[na].val.clusterDim.x = 1; attr[na].val.clusterDim.y = 1; attr[na].val.clusterDim.z = (unsigned)cluster_z;

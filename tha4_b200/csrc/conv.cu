@@ -366,22 +366,19 @@ void conv_pack(const ConvWeights& cw, ConvKind kind, const float* w_ref, int w_c
     THA4_LAUNCH_CHECK();
 }
 
-static bool g_use_tc = true;
-void conv_enable_tc(bool on) { g_use_tc = on; }
-bool conv_tc_enabled() { return g_use_tc; }
-
 bool conv_fuses_stats(const ConvWeights& cw, const ConvArgs& a) {
-    if (a.out.stats == nullptr || !g_use_tc) return false;
+    if (a.out.stats == nullptr || !opts().tcgen05) return false;
     if (conv_halo_supported(cw, a)) return true;
     return conv_tc_supported(cw, a) && conv_tc_fuses_stats(cw, a);
 }
 
 void conv_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s) {
+    const bool tc = opts().tcgen05;
     if (a.nin.on || a.out16.p || !a.out.p)
-        THA4_REQUIRE(g_use_tc && conv_tc_supported(cw, a), "conv: fused input normalisation / f16 outputs exist on the wgmma kernel only");
-    THA4_REQUIRE(cw.cin2 == 0 || (g_use_tc && conv_halo_supported(cw, a)), "conv: a folded 1x1 conv runs on the halo kernel only");
-    if (g_use_tc && conv_halo_supported(cw, a)) conv_halo_forward(cw, a, s);
-    else if (g_use_tc && conv_tc_supported(cw, a)) conv_tc_forward(cw, a, s);
+        THA4_REQUIRE(tc && conv_tc_supported(cw, a), "conv: fused input normalisation / f16 outputs exist on the wgmma kernel only");
+    THA4_REQUIRE(cw.cin2 == 0 || (tc && conv_halo_supported(cw, a)), "conv: a folded 1x1 conv runs on the halo kernel only");
+    if (tc && conv_halo_supported(cw, a)) conv_halo_forward(cw, a, s);
+    else if (tc && conv_tc_supported(cw, a)) conv_tc_forward(cw, a, s);
     else conv_mma_forward(cw, a, s);
 }
 

@@ -111,20 +111,10 @@ void conv_halo_forward(const ConvWeights& cw, const ConvArgs& a, cudaStream_t s)
 // width, cluster size, consumer warpgroups, resident CTAs per SM, phases, TMA-store bits (1 fp32 out, 2 f16 out, 4 residual
 // box), channel chunks
 bool conv_halo_plan_info(const ConvWeights& cw, const ConvArgs& a, int* info);
-void conv_halo_enable(bool on);
-void conv_halo_enable_tma_store(bool on);
-void conv_halo_set_ctas(int mode);        // option "halo_ctas": -1 automatic (default), 1 / 2 CTAs per SM for the 256 x 64 and four-phase halo tiles
-void conv_halo_set_cs(int mode);          // option "halo_cs": -1 automatic (default), 1 never / 2 always (where legal) split a two-warpgroup halo launch over a row-owning cluster pair
-void conv_halo_set_m256(int mode);        // option "halo_m256": -1 automatic (default), 0 / 1 force 128- / 256-pixel tiles on unsplit launches
 void conv_halo_debug_dump();   // developer: THA4_HALO_DEBUG=1 phase stamps of the last halo launch
-void conv_enable_tc(bool on);
-bool conv_tc_enabled();
 void conv_make_half(const ConvWeights& cw, cudaStream_t s);   // f16 copy of the packed weights (cw.w16), recorded in the active AllocSink
 // conv3 (3x3) followed by conv1x1 (same Cout) as one K (ConvWeights::cin2): the two f16 copies as they are (not owned by
 // `fold`), and the summed bias, recorded in the active AllocSink
 void conv_make_fold(ConvWeights& fold, const ConvWeights& conv3, const ConvWeights& conv1x1, cudaStream_t s);
-void conv_tc_enable_cluster(bool on);
-void conv_tc_enable_small_bn(bool on);  // narrower N tiles for tiny unsplit GEMMs
-void conv_tc_enable_stride2(bool on);   // stride-2 4x4 convs on the wgmma kernel (element-strided TMA) instead of mma.sync
 
 }  // namespace tha4

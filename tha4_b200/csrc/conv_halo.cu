@@ -562,10 +562,6 @@ bool halo_store_map(const View& v, bool f16, const CUtensorMap** out) {
     return true;
 }
 
-int g_halo_m256 = -1;         // option "halo_m256": -1 automatic, 0 / 1 force 128- / 256-pixel tiles on unsplit launches
-int g_halo_ctas = -1;         // option "halo_ctas": -1 automatic, 1 / 2 force the 288- / 256-thread two-warpgroup CTAs
-int g_halo_cs = -1;           // option "halo_cs": -1 automatic, 1 never / 2 always (where legal) split a two-warpgroup launch over a cluster pair
-
 // Shared memory of a CTA: the rings, the barriers, the alignment slack (the XF table comes on top)
 constexpr size_t halo_ring(int op, int bn, int sa, int sb, int wg, int ph) {
     return (size_t)sa * halo_a_bytes(op_row_bytes(op), ph == 1 ? wg : 1) + (size_t)sb * bn * op_row_bytes(op);
@@ -599,7 +595,7 @@ constexpr int halo2_sb(int op, int ph) { return ph == 4 ? 12 : halo_sb_wg2(op, 6
 // 1.04 - 1.18x faster on two CTAs per SM; with at most one CTA per SM (32 - 128 CTAs) nothing overlaps, and the
 // shallower rings made the same layers 1.2 - 1.8x slower.
 int halo_plan_ctas(int op, int bn, int ph, long ctas, const ConvArgs& a) {
-    if (g_halo_ctas > 0) return g_halo_ctas;
+    if (opts().halo_ctas > 0) return opts().halo_ctas;
     const size_t smem = halo_smem0(op, bn, halo2_sa(op, ph), halo2_sb(op, ph), 2, ph) + (a.nin.on ? (size_t)24 * a.nin.C + 32 : 0);
     return ctas > num_sms() && 2 * (smem + 1024) <= (size_t)228 * 1024 ? 2 : 1;
 }
@@ -610,8 +606,9 @@ int halo_plan_ctas(int op, int bn, int ph, long ctas, const ConvArgs& a) {
 // as pairs (64^2 256 -> 256: 29.0 -> 20.0 us), the four-phase layers from 32^2 and 64^2 (64 CTAs) 1.47x and 1.28x; with
 // 72 - 256 CTAs (a second wave) the pairs were 0.60 - 0.87x as fast, and those layers stay unsplit.
 int halo_plan_cs(long ctas, int chunks, const ConvArgs& a) {
-    if (g_halo_cs == 1 || chunks < 2) return 1;
-    return g_halo_cs == 2 || (a.ksplit <= 0 && 2 * ctas <= num_sms()) ? 2 : 1;
+    const int mode = opts().halo_cs;
+    if (mode == 1 || chunks < 2) return 1;
+    return mode == 2 || (a.ksplit <= 0 && 2 * ctas <= num_sms()) ? 2 : 1;
 }
 
 // Every rank of a cs-way cluster split owns channel chunks (a folded skip's list: halo_fold_c0)
@@ -648,7 +645,8 @@ HaloPlan halo_plan(const ConvWeights& cw, const ConvArgs& a, int op) {
     // frame ran faster than on 128-pixel tiles (1.03 - 1.36x at a 400 W power limit, down to 128 tiles), and the 64 x 64
     // layers with 128 - 512 channels (32 tiles) faster than their cluster split-K launches (1.1 - 2.1x at 700 W).  With fewer tiles (32 x 32 and
     // below) the split-K launches win.
-    const bool m256 = g_halo_m256 > 0 || (g_halo_m256 < 0 && a.ksplit <= 1 && 8L * pl.tiles_m >= sms);
+    const int m256_mode = opts().halo_m256;
+    const bool m256 = m256_mode > 0 || (m256_mode < 0 && a.ksplit <= 1 && 8L * pl.tiles_m >= sms);
     if (a.ksplit > 1) {
         while (pl.cs * 2 <= std::min(8, a.ksplit)) pl.cs *= 2;
     } else if (a.ksplit <= 0 && ctas < sms * 13 / 16 && !m256) {
@@ -751,22 +749,13 @@ void launch_halo_bn(int bn, int cs, int wg, int ctas, const HaloMaps& m, const T
     else launch_halo_cs<OP, 32, 2 * M, 9 * M, 5 * M, XF, SK>(cs, wg, ctas, m, p, grid, s);                    // unsplit:  67 KB
 }
 
-bool g_use_halo = true;
-bool g_tma_store = true;      // option "tma_store": unsplit epilogue through shared-memory staging + TMA stores
-
 }  // namespace
-
-void conv_halo_enable(bool on) { g_use_halo = on; }
-void conv_halo_enable_tma_store(bool on) { g_tma_store = on; }
-void conv_halo_set_m256(int mode) { g_halo_m256 = mode; }
-void conv_halo_set_ctas(int mode) { g_halo_ctas = mode; }
-void conv_halo_set_cs(int mode) { g_halo_cs = mode; }
 
 // One operand format for both sources of a folded skip: 64-channel chunks only when both widths allow them
 static int halo_op(const ConvWeights& cw) { return cw.cin_pad % 64 == 0 && cw.cin2_pad % 64 == 0 ? OP_F16 : OP_F16N; }
 
 bool conv_halo_supported(const ConvWeights& cw, const ConvArgs& a) {
-    if (!g_use_halo || !conv_tc_supported(cw, a)) return false;
+    if (!opts().halo_conv || !conv_tc_supported(cw, a)) return false;
     if (!a.in.f16 || cw.stride != 1) return false;
     // a folded 1x1 conv: its f16 input at the output's resolution, TMA-able, on the 3x3 normalised-input kernels
     if (cw.cin2 > 0 && (!cw.w16b || cw.ntaps != 9 || cw.nphase != 1 || !a.nin.on || a.res.p || !a.in2.f16 || !a.in2.p || a.in2.C != cw.cin2 ||
@@ -795,7 +784,7 @@ bool conv_halo_fuses_stats(const ConvWeights&, const ConvArgs&) { return true; }
 static int halo_st_tma(const ConvWeights& cw, const ConvArgs& a, const HaloPlan& pl, const CUtensorMap** mo32, const CUtensorMap** mo16,
                        const CUtensorMap** mr) {
     int st = 0;
-    if ((pl.cs == 1 || pl.wg == 2) && g_tma_store && cw.nphase == 1) {
+    if ((pl.cs == 1 || pl.wg == 2) && opts().tma_store && cw.nphase == 1) {
         if (a.out.p && halo_store_map(a.out, false, mo32)) st |= 1;
         if (a.out16.p && halo_store_map(a.out16, true, mo16)) st |= 2;
         // the residual of a ResBlock's second conv has the geometry of the fp32 output: it arrives through the same box

@@ -363,9 +363,6 @@ int op_for(const ConvWeights& cw, const ConvArgs& a) {
 
 namespace {
 struct TcPlan { int bn, tiles_x, tiles_y, tiles_m, tiles_n, ksplit, MH, MW; bool cluster; };
-bool g_use_cluster = true;
-bool g_small_bn = true;    // narrower N tiles for unsplit launches with < 64 CTAs (option "small_bn")
-bool g_use_s2 = true;      // 4x4 stride-2 convs through element-strided TMA boxes (option "tc_stride2")
 TcPlan tc_plan(const ConvWeights& cw, const ConvArgs& a) {
     TcPlan pl;
     pl.MH = a.out.H / cw.out_mul; pl.MW = a.out.W / cw.out_mul;
@@ -393,14 +390,14 @@ TcPlan tc_plan(const ConvWeights& cw, const ConvArgs& a) {
     ksplit = std::max(1, std::min(ksplit, KT));
     const int k_per = (KT + ksplit - 1) / ksplit;
     pl.ksplit = (KT + k_per - 1) / k_per;          // every split owns at least one k-block
-    if (g_small_bn && a.ksplit <= 0 && pl.ksplit == 1) {
+    if (a.ksplit <= 0 && pl.ksplit == 1) {
         // tiny GEMMs whose K is too short to split (the 1x1 qkv / proj convs at 16^2: 12 CTAs with BN = 128): narrower N
         // tiles put more SMs to work and shorten each CTA's weight fetch and epilogue
         while (pl.bn > 32 && (long)pl.tiles_m * (cw.cout_pad / pl.bn) * cw.nphase < 64 && cw.cout_pad % (pl.bn / 2) == 0) pl.bn /= 2;
         pl.tiles_n = cw.cout_pad / pl.bn;
     }
     pl.cluster = false;
-    if (g_use_cluster && pl.ksplit > 1 && KT >= 2) {
+    if (opts().cluster_splitk && pl.ksplit > 1 && KT >= 2) {
         // Split K over a thread-block cluster instead (partials meet in distributed shared memory, no workspace, no
         // second kernel).  Cluster size 2/4/8; narrower N tiles buy back the CTA count the smaller split gives up.
         int cs = 2;
@@ -424,7 +421,7 @@ size_t conv_workspace_floats(const ConvWeights& cw, const ConvArgs& a) {
 }
 
 int conv_tc_split_plan(const ConvWeights& cw, const ConvArgs& a) {
-    if (!conv_tc_enabled() || !conv_tc_supported(cw, a) || conv_halo_supported(cw, a)) return 0;
+    if (!opts().tcgen05 || !conv_tc_supported(cw, a) || conv_halo_supported(cw, a)) return 0;
     const TcPlan pl = tc_plan(cw, a);
     if (pl.ksplit <= 1) return 0;
     if (pl.cluster) return 1;
@@ -473,10 +470,6 @@ void conv_make_fold(ConvWeights& fold, const ConvWeights& conv3, const ConvWeigh
     fold.w16b = conv1x1.w16; fold.w16b_scale = conv1x1.w16_scale;
 }
 
-void conv_tc_enable_cluster(bool on) { g_use_cluster = on; }
-void conv_tc_enable_stride2(bool on) { g_use_s2 = on; }
-void conv_tc_enable_small_bn(bool on) { g_small_bn = on; }
-
 bool conv_tc_fuses_stats(const ConvWeights& cw, const ConvArgs& a) {
     const TcPlan pl = tc_plan(cw, a);
     if (pl.ksplit == 1 || pl.cluster) return true;
@@ -485,7 +478,8 @@ bool conv_tc_fuses_stats(const ConvWeights& cw, const ConvArgs& a) {
 
 bool conv_tc_supported(const ConvWeights& cw, const ConvArgs& a) {
     if (a.in_up || a.strict) return false;
-    if (cw.stride != 1 && !(g_use_s2 && cw.stride == 2 && cw.nphase == 1 && a.in.H % 2 == 0 && a.in.W % 2 == 0)) return false;
+    // 4x4 stride-2 convs read their taps through element-strided TMA boxes
+    if (cw.stride != 1 && !(cw.stride == 2 && cw.nphase == 1 && a.in.H % 2 == 0 && a.in.W % 2 == 0)) return false;
     if (a.in.ld % (a.in.f16 ? 8 : 4) != 0 || (((uintptr_t)a.in.p) & 15) != 0) return false;
     if (a.out.p && (a.out.ld % 4 != 0 || (((uintptr_t)a.out.p) & 15) != 0)) return false;
     if (a.out16.p && (a.out16.ld % 8 != 0 || (((uintptr_t)a.out16.p) & 15) != 0)) return false;

@@ -439,8 +439,6 @@ UNetNet::UNetNet(bool upscaler, int size, int model_channels, std::vector<int> m
 
 namespace {
 
-bool g_skip_fold = true;
-
 ResBlockW load_res_block(const StateDict& sd, const std::string& p, cudaStream_t s, bool upsampling = false) {
     ResBlockW w;
     w.norm0 = load_norm(sd, p + ".norm0", s);
@@ -746,7 +744,7 @@ struct UNetFused {
         // conv1 with the skip folded into its K loop: one launch, no skip(x) tensor, no fork / join around it
         ConvArgs fa;
         fa.in = h0.h; fa.out = out.f; fa.out16 = out.h; fa.in2 = x.h; fa.nin.on = true;
-        const bool fold = mode == 0 && w.fold.cin2 > 0 && g_skip_fold && conv_halo_supported(w.fold, fa);
+        const bool fold = mode == 0 && w.fold.cin2 > 0 && opts().skip_fold && conv_halo_supported(w.fold, fa);
         Tens sk;
         if (w.has_skip && !fold) {
             // skip(x) depends on x only: it runs on the side stream next to norm0 -> conv0 (a latency-bound chain,
@@ -929,8 +927,5 @@ void UNetNet::forward_fused(Runtime& rt, const ImgView& image, const float* coar
         tail_forward(TAIL_UNET, tail_, feat.f, coef, ACT_SILU_FAST, image, none, outputs, s, rt.strict);
     }
 }
-
-void unet_set_skip_fold(bool on) { g_skip_fold = on; }
-bool unet_skip_fold() { return g_skip_fold; }
 
 }  // namespace tha4

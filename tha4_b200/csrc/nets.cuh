@@ -200,8 +200,4 @@ void head_pack_adjoint(ConvWeights& cw, const TailWeights& tw, bool round_w, cud
 // cw.w with tracked_malloc; the values are those of fwd (TF32-rounded iff fwd's are).
 void conv_adjoint_from_packed(ConvWeights& cw, const ConvWeights& fwd, ConvKind kind, cudaStream_t s);
 
-// Option "skip_fold" (default on): the default mode runs a U-Net ResBlock's 1x1 skip inside conv1's K loop (ResBlockW::fold)
-void unet_set_skip_fold(bool on);
-bool unet_skip_fold();
-
 }  // namespace tha4

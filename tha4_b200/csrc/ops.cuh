@@ -39,8 +39,6 @@ void linear_forward(const float* x, int x_ld, int N, int I, const float* W, cons
 // out: NHWC [N,L,C].  L must be 256, head dim 32.
 // fast: the default precision mode may use the tensor-core kernel (f16 operands); strict callers pass false.
 void attention_forward(const View& qkv, int heads, const View& out, cudaStream_t s, bool fast = false);
-void attention_enable_mma(bool on);       // option "attn_mma" (default on)
-void attention_enable_split16(bool on);   // 16 CTAs per (sample, head) instead of 4 (B=1 latency; opt-in)
 
 // ---------------------------------------------------------------- image glue (image_ops.cu)
 void nchw_to_nhwc(const ImgView& src, const View& dst, cudaStream_t s);                 // dst.C == src.C
@@ -100,7 +98,6 @@ void tail_forward(TailKind kind, const TailWeights& tw, const View& feature, con
 // wgmma variant (tail_tc.cu): `feature` is the RAW f16 feature map with the statistics its producer accumulated
 void tail_make_half(TailWeights& tw, cudaStream_t s);     // f16 B-operand copy of the head weights (recorded in the active AllocSink)
 bool tail_tc_supported(const TailWeights& tw, const View& feature);
-void tail_tc_enable_persist(bool on);      // option "tail_persist": persistent pipelined tensor-core tail (default on)
 // gather0 / gather1: optional fp32 NHWC copies of image0 / image1 (4-channel slices, 16-byte aligned pixels), e.g. the
 // network's own input tensor: the persistent kernel then reads a pixel's RGBA with one 16-byte load (same values, same results)
 void tail_tc_forward(TailKind kind, const TailWeights& tw, const View& feature, const NormSpecTail& ns, const ImgView& image0,

@@ -678,7 +678,7 @@ static void face_levels(Runtime& rt, const SirenLayer* layers, const SirenLayer&
                         const int* char_of, int chars) {
     static const int nb[8] = {64, 64, 64, 64, 64, 64, 64, 16};
     SirenLevelArgs a;
-    a.tc = siren_tc_enabled(); a.mode = 3; a.R = 128; a.B = B;
+    a.tc = opts().siren_tc; a.mode = 3; a.R = 128; a.B = B;
     a.L = layers; a.nl = 8; a.head = &head; a.nb = nb;
     a.pb = pb;
     a.face_out = out;
@@ -708,7 +708,7 @@ static void body_levels(Runtime& rt, const SirenLayer (*l)[3], const SirenLayer&
     const int B = image.N;
     __half* f0 = reinterpret_cast<__half*>(rt.persist->alloc((size_t)B * 128 * 128 * 192 / 2));
     __half* f1 = reinterpret_cast<__half*>(rt.persist->alloc((size_t)B * 256 * 256 * 96 / 2));
-    const bool tc = siren_tc_enabled();
+    const bool tc = opts().siren_tc;
     THA4_REQUIRE(tc || !outputs_f16, "siren body: f16 outputs need the tensor-core path (option siren_tc)");
     static const int nb[4] = {96, 96, 96, 16};      // wgmma slice widths of the GEMM layers (level 2: + the head)
     for (int i = 0; i < 3; ++i) {
@@ -772,7 +772,7 @@ void SirenBank::set_character(int slot, const StateDict& face, const StateDict& 
 }
 
 void SirenBank::forward(Runtime& rt, const int* char_of_host, const float* pose, int B, void* const* outputs, bool outputs_f16) {
-    THA4_REQUIRE(siren_tc_enabled(), "character bank: needs the wgmma student kernels (option siren_tc = 1); the mma.sync kernels take one character's weights");
+    THA4_REQUIRE(opts().siren_tc, "character bank: needs the wgmma student kernels (option siren_tc = 1); the mma.sync kernels take one character's weights");
     cudaStream_t s = rt.stream;
     int* char_of = reinterpret_cast<int*>(rt.persist->alloc((size_t)B));
     THA4_CUDA_CHECK(cudaMemcpyAsync(char_of, char_of_host, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, s));

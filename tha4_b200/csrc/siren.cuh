@@ -38,8 +38,6 @@ void siren_tc_run(Runtime& rt, int mode, const SirenTcPlan& plan, const SirenTcL
 // kernel has no bounds checks of its own: K, N and the level's channel counts must fit its two operand buffers, its
 // weight tiles and its first-layer staging area, or it reads and writes past them.  siren_tc_run calls it per launch.
 std::string siren_tc_plan_error(int mode, const SirenTcPlan& plan, const SirenTcLevel& lv);
-void siren_tc_enable(bool on);
-bool siren_tc_enabled();
 void siren_tc_sine(const float* x, long n, float* y, cudaStream_t s);     // y = st_sin(x) of the wgmma kernels
 void siren_sine(const float* x, long n, float* y, cudaStream_t s);        // y = siren_sin(x) of the mma.sync kernels
 

@@ -423,8 +423,6 @@ void launch_siren_tc(const StMaps& maps, const StParams& p, int ctas_per_sm, cud
     else launch_siren_tc_kernel<ACH, NBMAX, SB, MODE, false>(maps, p, ctas_per_sm, s);
 }
 
-bool g_siren_tc = true;
-
 // per mode: the operand buffers' 64-column chunks (ACH) and the widest weight tile (NBMAX) of the launches in siren_tc_run
 constexpr int kStAch[4] = {6, 3, 2, 2};
 constexpr int kStNbMax[4] = {96, 96, 96, 64};
@@ -486,9 +484,6 @@ std::string siren_tc_plan_error(int mode, const SirenTcPlan& plan, const SirenTc
         return "out_c = " + std::to_string(lv.out_c) + " is not the last layer's npad = " + std::to_string(plan.npad[plan.nl - 1]) + at;
     return "";
 }
-
-void siren_tc_enable(bool on) { g_siren_tc = on; }
-bool siren_tc_enabled() { return g_siren_tc; }
 
 void SirenTcPlan::add(const SirenLayer& l, int nb, int sine, int first) {
     THA4_REQUIRE(nl < 8, "siren_tc: too many layers");

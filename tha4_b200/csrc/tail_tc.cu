@@ -578,8 +578,6 @@ void launch_tail_tc(const TailWeights& tw, const View& f, const NormSpecTail& ns
     THA4_LAUNCH_CHECK();
 }
 
-bool g_tail_persist = true;       // option "tail_persist": the persistent pipelined kernel (default) / one tile per CTA
-
 template <int KIND, int C, int TR>
 void launch_tail_persist(const TailWeights& tw, const View& f, const NormSpecTail& ns, const ImgView& i0, const ImgView& i1, float* const* o, int nout,
                          cudaStream_t s, const View* g0, const View* g1) {
@@ -614,7 +612,7 @@ void launch_tail_persist(const TailWeights& tw, const View& f, const NormSpecTai
 template <int KIND>
 void launch_tail_tc_c(const TailWeights& tw, const View& f, const NormSpecTail& ns, const ImgView& i0, const ImgView& i1, float* const* o, int nout,
                       cudaStream_t s, const View* g0, const View* g1) {
-    if (g_tail_persist) {
+    if (opts().tail_persist) {
         // tile rows per step (32-channel sites): 4 when that still gives every SM two tiles or more, else 2 (more, smaller tiles:
         // the small sites at B = 1 are one latency chain per CTA)
         const long tiles4 = (long)ceil_div(f.W, TT_W) * (f.H / 4) * f.N;
@@ -651,9 +649,6 @@ void tail_make_half(TailWeights& tw, cudaStream_t s) {
     THA4_LAUNCH_CHECK();
     tw.w16 = h; tw.w16_scale = scale;
 }
-
-
-void tail_tc_enable_persist(bool on) { g_tail_persist = on; }
 
 bool tail_tc_supported(const TailWeights& tw, const View& feature) {
     return feature.f16 && feature.stats != nullptr && (tw.C == 32 || tw.C == 64) && feature.C == tw.C && feature.ld == tw.C &&
