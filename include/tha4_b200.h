@@ -102,14 +102,21 @@ int tha4_face_morpher_forward(tha4_ctx* ctx, const float* image, const float* po
  * entries in the forward's output order, NCHW, an entry may be NULL = zero).  Every gradient output is optional (NULL = not
  * computed), at least one must be non-NULL, and each is overwritten: d_image / d_background_layer / d_eyebrow_layer have the
  * shape of the input, d_pose is [B,12] / [B,27] (contiguous).  The forward is recomputed in the context's precision mode
- * (default: f16 operands; strict: 3xTF32) and differentiated with fp32 data gradients.  Any B >= 1 (micro-batched). */
+ * (default: f16 operands; strict: 3xTF32) and differentiated with fp32 data gradients.  Any B >= 1 (micro-batched).
+ * d_params: the parameter gradients summed over the batch, a flat fp32 buffer of tha4_net_param_count(net) floats holding
+ * every state_dict tensor of the network in state_dict order (the order of the reference module's state_dict()), overwritten;
+ * NULL = not computed.  It counts as an output, and one call computes it together with the input gradients. */
 int tha4_eyebrow_decomposer_backward(tha4_ctx* ctx, const float* image, int B, const float* const* grad_outputs,
-                                     float* d_image, void* stream);
+                                     float* d_image, float* d_params, void* stream);
 int tha4_eyebrow_morphing_combiner_backward(tha4_ctx* ctx, const float* background_layer, const float* eyebrow_layer,
                                             const float* pose, int pose_ld, int B, const float* const* grad_outputs,
-                                            float* d_background_layer, float* d_eyebrow_layer, float* d_pose, void* stream);
+                                            float* d_background_layer, float* d_eyebrow_layer, float* d_pose, float* d_params,
+                                            void* stream);
 int tha4_face_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
-                               const float* const* grad_outputs, float* d_image, float* d_pose, void* stream);
+                               const float* const* grad_outputs, float* d_image, float* d_pose, float* d_params, void* stream);
+/* Floats of the parameters of THA4_NET_EYEBROW_DECOMPOSER / _EYEBROW_MORPHING_COMBINER / _FACE_MORPHER (the length of
+ * d_params above); -1 for any other network. */
+int64_t tha4_net_param_count(int net);
 /* Morpher00.forward (src/tha4/nn/morpher/morpher_00.py:42-66): image [B,4,256,256], pose [B,6] ->
  * merged(4) alpha(1) warped(4) grid_change(2) direct(4) */
 int tha4_morpher_forward(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
@@ -350,6 +357,17 @@ int tha4_test_group_norm_backward_ex(tha4_ctx* ctx, const void* x, int x_f16, in
                                      const float* film0, const float* film1, int film1_ld, int film1_off, int act, const float* dy,
                                      int dy_ld, int dy_pool, const float* res, int res_ld, int res_mode, const float* add, int add_ld,
                                      float* dx, int dx_ld, float* d_film, int d_film_ld, void* stream);
+/* The encoder-decoders' weight-gradient convolution (conv_wgrad.cu) through the launcher the network backward uses.  kind:
+ * 0 3x3 s1 p1, 1 4x4 s2 p1, 2 transposed 4x4 s2 p1, 3 the heads' 3x3 with output channel d written at d * c_real * 9 (the
+ * row map).  x: the forward conv's NHWC operand [N,H,W,x_ld] (f16 if x_f16), Cx channels; xf: 0 as stored, 1 the default
+ * mode's fused InstanceNorm + ReLU (f16 coefficients from the statistics), 2 / 3 the tail's (fp32 affine; 3 rounds to f16)
+ * on its first norm_C channels, statistics [stats_rep][N][norm_C][2].  dz: [N,Ho,Wo,dz_ld] fp32, Cout channels.  dW: the
+ * reference layout ([Cout][c_real][k][k], transposed conv [Cx][Cout][4][4]; c_real 0 = every channel), written.
+ * coef_out (optional): the [N][norm_C] (A, B) pairs the transform used.  plan[4]: N tile, M tiles, N tiles, pixel splits
+ * (ksplit > 0 forces the split). */
+int tha4_test_conv_wgrad(tha4_ctx* ctx, int kind, int strict, int ksplit, const void* x, int x_f16, int x_ld, int N, int H, int W,
+                         int Cx, int xf, const double* stats, int stats_rep, const float* gamma, const float* beta, int norm_C,
+                         const float* dz, int dz_ld, int Cout, int c_real, float* dW, float* coef_out, int* plan, void* stream);
 /* InstanceNorm2d(affine) (+ReLU when act == 1) backward, norm_backward: x as above, dy / dx [N,H,W,C]. */
 int tha4_test_norm_backward_ex(tha4_ctx* ctx, const void* x, int x_f16, int x_ld, int N, int C, int H, int W, const double* stats,
                                int stats_rep, int stats_ld, const float* gamma, const float* beta, int act, const float* dy, int dy_ld,

@@ -30,10 +30,10 @@ EXPORTED_SYMBOLS = [
     'tha4_siren_morpher_backward', 'tha4_siren_face_morpher_backward',
     'tha4_adam_step', 'tha4_images_differ', 'tha4_frame_to_srgb8', 'tha4_rgba8_to_poser_image', 'tha4_grid_sample', 'tha4_resize_bilinear',
     'tha4_eyebrow_decomposer_backward', 'tha4_eyebrow_morphing_combiner_backward', 'tha4_face_morpher_backward',
-    'tha4_morpher_backward', 'tha4_upscaler_backward',
+    'tha4_morpher_backward', 'tha4_upscaler_backward', 'tha4_net_param_count',
     'tha4_test_conv_backward_data', 'tha4_test_norm_backward', 'tha4_test_tail_backward', 'tha4_test_upscaler_prologue_backward',
     'tha4_test_group_norm_backward', 'tha4_test_attention_backward',
-    'tha4_test_group_norm_backward_ex', 'tha4_test_norm_backward_ex', 'tha4_test_conv_backward_data_ex', 'tha4_test_linear_backward',
+    'tha4_test_group_norm_backward_ex', 'tha4_test_norm_backward_ex', 'tha4_test_conv_backward_data_ex', 'tha4_test_conv_wgrad', 'tha4_test_linear_backward',
     'tha4_test_conv_forward_ex', 'tha4_test_tail_ex',
     'tha4_base_grid', 'tha4_test_conv', 'tha4_test_conv_norm', 'tha4_test_conv_norm_ex', 'tha4_test_conv_skip_fold', 'tha4_test_norm', 'tha4_test_tail', 'tha4_test_attention', 'tha4_test_linear',
     'tha4_test_siren_level', 'tha4_test_sine', 'tha4_test_siren_plan_check',
@@ -64,6 +64,8 @@ def load_library() -> ctypes.CDLL:
     lib.tha4_set_option.argtypes = [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_int64]
     lib.tha4_siren_morpher_param_count.restype = ctypes.c_int64
     lib.tha4_siren_face_morpher_param_count.restype = ctypes.c_int64
+    lib.tha4_net_param_count.restype = ctypes.c_int64
+    lib.tha4_net_param_count.argtypes = [ctypes.c_int]
     lib.tha4_adam_step.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64,
                                    ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_int, ctypes.c_float,
                                    ctypes.c_void_p]
@@ -226,22 +228,34 @@ class Context:
             gs.append(g)
         return gs
 
-    def eyebrow_decomposer_backward(self, image: Tensor, grad_outputs: Sequence[Optional[Tensor]], d_image: Tensor):
+    def param_count(self, net: str) -> int:
+        """Floats of an encoder-decoder network's parameters: the length of the flat d_params buffer of its backward."""
+        n = int(self.lib.tha4_net_param_count(NET_IDS[net]))
+        if n < 0:
+            raise Tha4Error('%s has no parameter gradients' % net)
+        return n
+
+    def eyebrow_decomposer_backward(self, image: Tensor, grad_outputs: Sequence[Optional[Tensor]], d_image: Optional[Tensor] = None,
+                                    d_params: Optional[Tensor] = None):
         """d_image [B,4,128,128] <- the input gradient of EyebrowDecomposer00 for the upstream gradients of its six outputs
-        (None = zero); the forward is recomputed in the context's precision mode."""
+        (None = zero); d_params [param_count] <- the parameter gradients, flat in state_dict order (None = not computed).
+        The forward is recomputed in the context's precision mode."""
+        assert d_image is not None or d_params is not None
         image = _check_input(image, self.device, 'image')
         B = image.shape[0]
         assert image.shape[1:] == (4, 128, 128)
         gs = self._grads(self.DECOMPOSER_SPECS, grad_outputs, B)
         self._check_out(d_image, (B, 4, 128, 128), 'd_image')
-        self._call('tha4_eyebrow_decomposer_backward', _ptr(image), B, _ptr_array(gs), _ptr(d_image), self._stream())
+        self._check_out(d_params, (self.param_count('eyebrow_decomposer'),), 'd_params')
+        self._call('tha4_eyebrow_decomposer_backward', _ptr(image), B, _ptr_array(gs), _ptr(d_image), _ptr(d_params), self._stream())
 
     def eyebrow_morphing_combiner_backward(self, background_layer: Tensor, eyebrow_layer: Tensor, pose: Tensor,
                                            grad_outputs: Sequence[Optional[Tensor]], d_background_layer: Optional[Tensor] = None,
-                                           d_eyebrow_layer: Optional[Tensor] = None, d_pose: Optional[Tensor] = None):
+                                           d_eyebrow_layer: Optional[Tensor] = None, d_pose: Optional[Tensor] = None,
+                                           d_params: Optional[Tensor] = None):
         """Input gradients of EyebrowMorphingCombiner00 into any of d_background_layer / d_eyebrow_layer [B,4,128,128] and
-        d_pose [B,12] (None = not computed)."""
-        assert d_background_layer is not None or d_eyebrow_layer is not None or d_pose is not None
+        d_pose [B,12], parameter gradients into d_params (flat, state_dict order) (None = not computed)."""
+        assert d_background_layer is not None or d_eyebrow_layer is not None or d_pose is not None or d_params is not None
         background_layer = _check_input(background_layer, self.device, 'background_layer')
         eyebrow_layer = _check_input(eyebrow_layer, self.device, 'eyebrow_layer')
         pose = _check_input(pose, self.device, 'pose')
@@ -251,13 +265,15 @@ class Context:
         self._check_out(d_background_layer, (B, 4, 128, 128), 'd_background_layer')
         self._check_out(d_eyebrow_layer, (B, 4, 128, 128), 'd_eyebrow_layer')
         self._check_out(d_pose, (B, 12), 'd_pose')
+        self._check_out(d_params, (self.param_count('eyebrow_morphing_combiner'),), 'd_params')
         self._call('tha4_eyebrow_morphing_combiner_backward', _ptr(background_layer), _ptr(eyebrow_layer), _ptr(pose), 12, B,
-                   _ptr_array(gs), _ptr(d_background_layer), _ptr(d_eyebrow_layer), _ptr(d_pose), self._stream())
+                   _ptr_array(gs), _ptr(d_background_layer), _ptr(d_eyebrow_layer), _ptr(d_pose), _ptr(d_params), self._stream())
 
     def face_morpher_backward(self, image: Tensor, pose: Tensor, grad_outputs: Sequence[Optional[Tensor]],
-                              d_image: Optional[Tensor] = None, d_pose: Optional[Tensor] = None):
-        """Input gradients of FaceMorpher08 into d_image [B,4,192,192] and / or d_pose [B,27] (None = not computed)."""
-        assert d_image is not None or d_pose is not None
+                              d_image: Optional[Tensor] = None, d_pose: Optional[Tensor] = None, d_params: Optional[Tensor] = None):
+        """Input gradients of FaceMorpher08 into d_image [B,4,192,192] and / or d_pose [B,27], parameter gradients into d_params
+        (flat, state_dict order) (None = not computed)."""
+        assert d_image is not None or d_pose is not None or d_params is not None
         image = _check_input(image, self.device, 'image')
         pose = _check_input(pose, self.device, 'pose')
         B = image.shape[0]
@@ -265,8 +281,9 @@ class Context:
         gs = self._grads(self.FACE_MORPHER_SPECS, grad_outputs, B)
         self._check_out(d_image, (B, 4, 192, 192), 'd_image')
         self._check_out(d_pose, (B, 27), 'd_pose')
+        self._check_out(d_params, (self.param_count('face_morpher'),), 'd_params')
         self._call('tha4_face_morpher_backward', _ptr(image), _ptr(pose), 27, B, _ptr_array(gs), _ptr(d_image), _ptr(d_pose),
-                   self._stream())
+                   _ptr(d_params), self._stream())
 
     MORPHER_SPECS = [(4, 256), (1, 256), (4, 256), (2, 256), (4, 256)]
 

@@ -1,6 +1,7 @@
 // extern "C" boundary of libtha4_b200.so (see include/tha4_b200.h) and the poser-level pipelines.
 #include "../../include/tha4_b200.h"
 #include "nets.cuh"
+#include "conv_wgrad.cuh"
 #include "siren.cuh"
 #include "profiler.cuh"
 #include "distill.cuh"
@@ -352,14 +353,33 @@ int tha4_face_morpher_forward(tha4_ctx* ctx, const float* image, const float* po
     });
 }
 
+int64_t tha4_net_param_count(int net) {
+    // floats of the reference state_dicts (src/tha4/nn/eyebrow_decomposer/eyebrow_decomposer_00.py and siblings)
+    switch (net) {
+        case THA4_NET_EYEBROW_DECOMPOSER: return 31479434;
+        case THA4_NET_EYEBROW_MORPHING_COMBINER: return 31535878;
+        case THA4_NET_FACE_MORPHER: return 31605002;
+        default: return -1;
+    }
+}
+
+namespace {
+// checks the network's flat parameter layout against the ABI's count before a backward writes d_params
+void check_param_layout(const EncDecNet& net, int id, const float* d_params) {
+    if (d_params) THA4_REQUIRE(net.param_count() == tha4_net_param_count(id), "backward: the loaded state_dict does not have the network's parameters");
+}
+}  // namespace
+
 int tha4_eyebrow_decomposer_backward(tha4_ctx* ctx, const float* image, int B, const float* const* grad_outputs,
-                                     float* d_image, void* stream) {
+                                     float* d_image, float* d_params, void* stream) {
     return guarded(ctx, [&] {
-        THA4_REQUIRE(d_image != nullptr, "decomposer backward: no gradient requested");
+        THA4_REQUIRE(d_image || d_params, "decomposer backward: no gradient requested");
+        check_param_layout(*ctx->decomposer, THA4_NET_EYEBROW_DECOMPOSER, d_params);
         Runtime rt = make_rt(ctx, stream);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             const float* g[6]; offset_grads<6>(grad_outputs, kEncDecDecomposer, n0, g);
-            EncDecGrads eg; eg.grad_outputs = g; eg.d_image0 = d_image + (size_t)n0 * 4 * 128 * 128;
+            EncDecGrads eg; eg.grad_outputs = g; eg.d_image0 = d_image ? d_image + (size_t)n0 * 4 * 128 * 128 : nullptr;
+            eg.d_params = d_params; eg.accumulate_params = n0 > 0;
             ctx->decomposer->backward(rt, make_img(image + (size_t)n0 * 4 * 128 * 128, b, 4, 128, 128), ImgView{}, nullptr, 0, eg);
         });
     });
@@ -367,9 +387,10 @@ int tha4_eyebrow_decomposer_backward(tha4_ctx* ctx, const float* image, int B, c
 
 int tha4_eyebrow_morphing_combiner_backward(tha4_ctx* ctx, const float* background_layer, const float* eyebrow_layer,
                                             const float* pose, int pose_ld, int B, const float* const* grad_outputs,
-                                            float* d_background_layer, float* d_eyebrow_layer, float* d_pose, void* stream) {
+                                            float* d_background_layer, float* d_eyebrow_layer, float* d_pose, float* d_params, void* stream) {
     return guarded(ctx, [&] {
-        THA4_REQUIRE(d_background_layer || d_eyebrow_layer || d_pose, "combiner backward: no gradient requested");
+        THA4_REQUIRE(d_background_layer || d_eyebrow_layer || d_pose || d_params, "combiner backward: no gradient requested");
+        check_param_layout(*ctx->combiner, THA4_NET_EYEBROW_MORPHING_COMBINER, d_params);
         THA4_REQUIRE(pose_ld >= 12, "combiner backward: pose rows need at least 12 entries");
         Runtime rt = make_rt(ctx, stream);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
@@ -379,6 +400,7 @@ int tha4_eyebrow_morphing_combiner_backward(tha4_ctx* ctx, const float* backgrou
             eg.d_image0 = d_eyebrow_layer ? d_eyebrow_layer + off : nullptr;
             eg.d_image1 = d_background_layer ? d_background_layer + off : nullptr;
             eg.d_pose = d_pose ? d_pose + (size_t)n0 * 12 : nullptr; eg.d_pose_ld = 12;
+            eg.d_params = d_params; eg.accumulate_params = n0 > 0;
             ctx->combiner->backward(rt, make_img(eyebrow_layer + off, b, 4, 128, 128), make_img(background_layer + off, b, 4, 128, 128),
                                     pose + (size_t)n0 * pose_ld, pose_ld, eg);
         });
@@ -386,9 +408,10 @@ int tha4_eyebrow_morphing_combiner_backward(tha4_ctx* ctx, const float* backgrou
 }
 
 int tha4_face_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
-                               const float* const* grad_outputs, float* d_image, float* d_pose, void* stream) {
+                               const float* const* grad_outputs, float* d_image, float* d_pose, float* d_params, void* stream) {
     return guarded(ctx, [&] {
-        THA4_REQUIRE(d_image || d_pose, "face morpher backward: no gradient requested");
+        THA4_REQUIRE(d_image || d_pose || d_params, "face morpher backward: no gradient requested");
+        check_param_layout(*ctx->face, THA4_NET_FACE_MORPHER, d_params);
         THA4_REQUIRE(pose_ld >= 27, "face morpher backward: pose rows need at least 27 entries");
         Runtime rt = make_rt(ctx, stream);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
@@ -396,6 +419,7 @@ int tha4_face_morpher_backward(tha4_ctx* ctx, const float* image, const float* p
             EncDecGrads eg; eg.grad_outputs = g;
             eg.d_image0 = d_image ? d_image + (size_t)n0 * 4 * 192 * 192 : nullptr;
             eg.d_pose = d_pose ? d_pose + (size_t)n0 * 27 : nullptr; eg.d_pose_ld = 27;
+            eg.d_params = d_params; eg.accumulate_params = n0 > 0;
             ctx->face->backward(rt, make_img(image + (size_t)n0 * 4 * 192 * 192, b, 4, 192, 192), ImgView{}, pose + (size_t)n0 * pose_ld,
                                 pose_ld, eg);
         });
@@ -1294,6 +1318,41 @@ int tha4_test_norm_backward_ex(tha4_ctx* ctx, const void* x, int x_f16, int x_ld
         Runtime rt = make_rt(ctx, stream);
         norm_backward(stats_input(x, x_f16, x_ld, N, C, H, W, stats, stats_rep, stats_ld), gamma, beta, act, nhwc_view(dy, N, H, W, C, dy_ld),
                       nhwc_view(dx, N, H, W, C, dx_ld), rt.alloc_stats((size_t)N * C * 2), s);
+    });
+}
+
+int tha4_test_conv_wgrad(tha4_ctx* ctx, int kind, int strict, int ksplit, const void* x, int x_f16, int x_ld, int N, int H, int W,
+                         int Cx, int xf, const double* stats, int stats_rep, const float* gamma, const float* beta, int norm_C,
+                         const float* dz, int dz_ld, int Cout, int c_real, float* dW, float* coef_out, int* plan, void* stream) {
+    return guarded(ctx, [&] {
+        cudaStream_t s = (cudaStream_t)stream;
+        THA4_REQUIRE(kind >= 0 && kind <= 3, "test_conv_wgrad: kind 0..3");
+        THA4_REQUIRE(xf >= WG_XF_NONE && xf <= WG_XF_FLOAT16 && (xf == WG_XF_NONE || (stats && norm_C > 0 && norm_C <= Cx)),
+                     "test_conv_wgrad: transform");
+        begin_pass(ctx, s);
+        WgradOperand xo;
+        xo.p = x; xo.f16 = x_f16 ? 1 : 0; xo.ld = x_ld; xo.N = N; xo.H = H; xo.W = W; xo.C = Cx;
+        if (xf != WG_XF_NONE) {
+            const View st = stats_input(x, x_f16, x_ld, N, norm_C, H, W, stats, stats_rep, norm_C);
+            float2* coef = reinterpret_cast<float2*>(ctx->persist.alloc((size_t)N * norm_C * 2));
+            if (xf == WG_XF_HALF) wgrad_xf_coef(st, gamma, beta, norm_C, ACT_RELU, coef, s);
+            else norm_finalize(st, 0, gamma, beta, nullptr, nullptr, 0, reinterpret_cast<float*>(coef), s);
+            if (coef_out) THA4_CUDA_CHECK(cudaMemcpyAsync(coef_out, coef, (size_t)N * norm_C * sizeof(float2), cudaMemcpyDeviceToDevice, s));
+            xo.xf = xf; xo.relu = 1; xo.coef = coef; xo.coef_C = norm_C;
+        }
+        const int oh = kind == 1 ? H / 2 : (kind == 2 ? 2 * H : H);
+        WgradOperand d;
+        d.p = dz; d.ld = dz_ld; d.N = N; d.H = oh; d.W = kind == 1 ? W / 2 : (kind == 2 ? 2 * W : W); d.C = Cout;
+        WgradArgs a;
+        a.c_real = c_real; a.out = dW;
+        if (kind == 3) {          // the heads' row map: output channel d at d * c_real * 9
+            THA4_REQUIRE(Cout <= 16, "test_conv_wgrad: at most 16 head channels");
+            a.n_map = Cout;
+            for (int k = 0; k < Cout; ++k) a.out_row[k] = (long)k * (c_real ? c_real : Cx) * 9;
+        }
+        const ConvKind ck = kind == 1 ? CONV_4x4_S2 : (kind == 2 ? CONVT_4x4_S2 : CONV_3x3);
+        const WgradPlan pl = conv_wgrad_layer(ck, xo, d, a, strict, ksplit, [&](size_t n) { return ctx->scratch.alloc(n); }, s);
+        if (plan) { plan[0] = pl.nt; plan[1] = pl.mtiles; plan[2] = pl.ntiles; plan[3] = pl.splits; }
     });
 }
 

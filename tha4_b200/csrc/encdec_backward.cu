@@ -9,8 +9,12 @@
 //   convs: data gradients on the same conv kernels with adjoint-packed weights (3x3 -> 3x3 with W^T flipped, 4x4 s2 conv <->
 //         4x4 s2 transposed conv), fp32 operands (TF32, or 3xTF32 in strict mode), never through f16 storage;
 //   InstanceNorm (+ReLU): dz = dy [A x + B > 0];  dx = gamma rstd (dz - mean(dz) - xhat mean(dz xhat)), sums in fp64;
-//   pose: spatial sum of the pose channels of the bottleneck entry's data gradient, in a fixed order (no atomics).
+//   pose: spatial sum of the pose channels of the bottleneck entry's data gradient, in a fixed order (no atomics);
+//   parameters (EncDecGrads::d_params): every conv's weight gradient on the wgmma weight-gradient kernel (conv_wgrad.cu) from
+//         the dz above and the operand the forward conv multiplied (EncDecTape::op_*), the InstanceNorm affine gradients
+//         folded over the batch from the per-(n, c) sums of the norm backward, the head biases as pixel sums of dh.
 #include "nets.cuh"
+#include "conv_wgrad.cuh"
 #include "gridsample.cuh"
 
 namespace tha4 {
@@ -162,6 +166,34 @@ __global__ void pose_sum_kernel(const float* __restrict__ dbin, int ld, long hw,
     double acc = 0.0;
     for (long p = 0; p < hw; ++p) acc += (double)src[p * ld];
     dpose[(long)n * dpose_ld + k] = (float)acc;
+}
+
+// d gamma[c] = sum_n sum dz xhat, d beta[c] = sum_n sum dz, from norm_bwd_reduce_kernel's per-(n, c) sums, folded in n order
+__global__ void norm_param_fold_kernel(const double* __restrict__ sums, int N, int C, float* __restrict__ dgamma, float* __restrict__ dbeta,
+                                       int accumulate) {
+    for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < C; c += gridDim.x * blockDim.x) {
+        double g = 0.0, b = 0.0;
+        for (int n = 0; n < N; ++n) { b += sums[((long)n * C + c) * 2]; g += sums[((long)n * C + c) * 2 + 1]; }
+        dgamma[c] = accumulate ? dgamma[c] + (float)g : (float)g;
+        dbeta[c] = accumulate ? dbeta[c] + (float)b : (float)b;
+    }
+}
+
+// bias gradient of head channel blockIdx.x: the sum of dh over every pixel of the batch (fp64, fixed order: strided per
+// thread, then a tree over the block)
+struct HeadBiasArgs { const float* dh; long pixels; float* out; long off[16]; int accumulate; };
+__global__ void __launch_bounds__(256) head_bias_kernel(const HeadBiasArgs a) {
+    __shared__ double red[256];
+    const int d = blockIdx.x;
+    double acc = 0.0;
+    for (long p = threadIdx.x; p < a.pixels; p += 256) acc += (double)a.dh[p * 16 + d];
+    red[threadIdx.x] = acc;
+    __syncthreads();
+    for (int w = 128; w > 0; w >>= 1) {
+        if (threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0 && a.off[d] >= 0) a.out[a.off[d]] = a.accumulate ? a.out[a.off[d]] + (float)red[0] : (float)red[0];
 }
 
 __device__ __forceinline__ float gv(const float* g, long off) { return g ? g[off] : 0.0f; }
@@ -423,10 +455,16 @@ void EncDecNet::load_adjoints(const StateDict& sd, const std::string& p, cudaStr
     head_pack_adjoint(adj_head_, tail_, conv_pack_rounding(), s);
 }
 
+long EncDecNet::param_offset(const std::string& key) const {
+    auto it = param_off_.find(key);
+    THA4_REQUIRE(it != param_off_.end(), "parameter gradients: no tensor " + key);
+    return it->second;
+}
+
 void EncDecNet::backward(Runtime& rt, const ImgView& image0, const ImgView& image1, const float* pose, int pose_ld, const EncDecGrads& g) {
     THA4_REQUIRE(loaded_, "network weights not loaded");
-    const bool want_img = g.d_image0 || g.d_image1, want_pose = g.d_pose != nullptr;
-    THA4_REQUIRE(want_img || want_pose, "encdec backward: no gradient requested");
+    const bool want_img = g.d_image0 || g.d_image1, want_pose = g.d_pose != nullptr, want_par = g.d_params != nullptr;
+    THA4_REQUIRE(want_img || want_pose || want_par, "encdec backward: no gradient requested");
     THA4_REQUIRE(!want_pose || pose_ch_ > 0, "encdec backward: this network has no pose input");
     THA4_REQUIRE(!g.d_image1 || kind_ == TAIL_COMBINER, "encdec backward: only the combiner has a second image");
     const int B = image0.N, S = S_, b = S_ / 8;
@@ -441,12 +479,40 @@ void EncDecNet::backward(Runtime& rt, const ImgView& image0, const ImgView& imag
     EncDecTape tape;
     forward(rt, image0, image1, pose, pose_ld, outs, &tape);
 
-    auto nbwd = [&](const View& x, const NormW& nw, int act, const View& dy) {
+    auto nbwd = [&](const View& x, const NormW& nw, int act, const View& dy, const std::string& key) {
         THA4_REQUIRE(nw.C == x.C, "norm backward: channel mismatch");
         View dx = fresh(P, x.N, x.H, x.W, x.C);
-        norm_backward(x, nw.gamma, nw.beta, act, dy, dx, rt.alloc_stats((size_t)x.N * x.C * 2), s);
+        double* sums = rt.alloc_stats((size_t)x.N * x.C * 2);
+        norm_backward(x, nw.gamma, nw.beta, act, dy, dx, sums, s);
+        if (want_par) {
+            norm_param_fold_kernel<<<ceil_div(x.C, 256), 256, 0, s>>>(sums, x.N, x.C, g.d_params + param_offset(key + ".weight"),
+                                                                      g.d_params + param_offset(key + ".bias"), g.accumulate_params);
+            THA4_LAUNCH_CHECK();
+        }
         return dx;
     };
+    // ---- weight gradients.  An operand as the forward conv multiplied it: the stored tensor, or (default mode) an f16 raw
+    // conv output with the pending InstanceNorm + ReLU its consumer applied, rebuilt from `stats`' statistics
+    auto operand = [&](const View& v, const NormW* nw = nullptr, const View* stats = nullptr) {
+        WgradOperand o;
+        o.p = v.p; o.f16 = v.f16; o.ld = v.ld; o.N = v.N; o.H = v.H; o.W = v.W; o.C = v.C;
+        if (nw && rt.f16) {
+            float2* coef = reinterpret_cast<float2*>(P->alloc((size_t)v.N * nw->C * 2));
+            wgrad_xf_coef(*stats, nw->gamma, nw->beta, nw->C, ACT_RELU, coef, s);
+            o.xf = WG_XF_HALF; o.relu = 1; o.coef = coef; o.coef_C = nw->C;
+        }
+        return o;
+    };
+    const auto ws_alloc = [&](size_t n) { return rt.scratch->alloc(n); };
+    auto wgrad = [&](const std::string& key, ConvKind kind, const WgradOperand& x, const View& dz, int c_real = 0) {
+        if (!want_par) return;
+        WgradArgs a;
+        a.c_real = c_real; a.accumulate = g.accumulate_params;
+        a.out = g.d_params + param_offset(key + ".weight");
+        conv_wgrad_layer(kind, x, operand(dz), a, rt.strict, 0, ws_alloc, s);
+    };
+    const std::string& p = prefix_;
+    auto blk = [&](const char* what, int i, const char* sub) { return p + what + std::to_string(i) + sub; };
     // tail: head pre-activation gradients + the image terms (in the layout of the network input x0)
     View dh = fresh(P, B, S, S, 16);
     View dimg;
@@ -460,41 +526,79 @@ void EncDecNet::backward(Runtime& rt, const ImgView& image0, const ImgView& imag
     tail_backward(kind_, outs, g.grad_outputs, image0, image1, dh, d0, d1, in_ch_, s);
     View df = fresh(P, B, S, S, tail_.C);
     run_dgrad(rt, adj_head_, dh, df);
+    if (want_par) {
+        // heads: one weight-gradient launch over the tail's 16-channel dh (head channels in N), operand relu(IN(up[2])) as
+        // the tail normalised it; biases as pixel sums of dh
+        const View& f = tape.up[2];
+        float2* coef = reinterpret_cast<float2*>(P->alloc((size_t)B * f.C * 2));
+        norm_finalize(f, 0, up_n_[2].gamma, up_n_[2].beta, nullptr, nullptr, 0, reinterpret_cast<float*>(coef), s);
+        WgradOperand x = operand(f);
+        x.xf = f.f16 ? WG_XF_FLOAT16 : WG_XF_FLOAT; x.relu = 1; x.coef = coef; x.coef_C = f.C;
+        WgradArgs a;
+        WgradOperand d = operand(dh);
+        HeadBiasArgs hb; hb.dh = dh.p; hb.pixels = (long)B * S * S; hb.out = g.d_params; hb.accumulate = g.accumulate_params;
+        int ch = 0;
+        for (size_t h = 0; h < head_key_.size(); ++h) {
+            const long wo = param_offset(head_key_[h] + ".weight");
+            auto bi = param_off_.find(head_key_[h] + ".bias");
+            for (int co = 0; co < head_cout_[h]; ++co, ++ch) {
+                a.out_row[ch] = wo + (long)co * f.C * 9;
+                hb.off[ch] = bi == param_off_.end() ? -1 : bi->second + co;
+            }
+        }
+        a.n_map = ch; d.C = ch;
+        a.out = g.d_params; a.accumulate = g.accumulate_params;
+        conv_wgrad_layer(CONV_3x3, x, d, a, rt.strict, 0, ws_alloc, s);
+        head_bias_kernel<<<ch, 256, 0, s>>>(hb);
+        THA4_LAUNCH_CHECK();
+    }
     // decoder
-    View d = nbwd(tape.up[2], up_n_[2], ACT_RELU, df);
+    View d = nbwd(tape.up[2], up_n_[2], ACT_RELU, df, blk("upsample_blocks.", 2, ".1"));
     for (int i = 2; i >= 1; --i) {
         View da = fresh(P, B, b << i, b << i, adj_up_[i].cout);
         run_dgrad(rt, adj_up_[i], d, da);
-        d = nbwd(tape.up[i - 1], up_n_[i - 1], ACT_RELU, da);
+        wgrad(blk("upsample_blocks.", i, ".0"), CONVT_4x4_S2, operand(tape.op_up[i], &up_n_[i - 1], &tape.up[i - 1]), d);
+        d = nbwd(tape.up[i - 1], up_n_[i - 1], ACT_RELU, da, blk("upsample_blocks.", i - 1, ".1"));
     }
     View gx = fresh(P, B, b, b, 512);
     run_dgrad(rt, adj_up_[0], d, gx);
+    wgrad(blk("upsample_blocks.", 0, ".0"), CONVT_4x4_S2, operand(tape.op_up[0]), d);
     // ResnetBlocks: x + IN(conv(relu(IN(conv(x))))): the residual gradient joins in the epilogue of the first conv's adjoint
     for (int i = 4; i >= 0; --i) {
-        View d1n = nbwd(tape.res[i][1], res_n_[i][1], ACT_NONE, gx);
+        const std::string rp = blk("bottleneck_blocks.", i + 1, ".resnet_path.");
+        View d1n = nbwd(tape.res[i][1], res_n_[i][1], ACT_NONE, gx, rp + "4");
         View dh1 = fresh(P, B, b, b, 512);
         run_dgrad(rt, adj_res_[i][1], d1n, dh1);
-        View d0n = nbwd(tape.res[i][0], res_n_[i][0], ACT_RELU, dh1);
+        wgrad(rp + "3", CONV_3x3, operand(tape.op_res[i][1], &res_n_[i][0], &tape.res[i][0]), d1n);
+        View d0n = nbwd(tape.res[i][0], res_n_[i][0], ACT_RELU, dh1, rp + "1");
         View gn = fresh(P, B, b, b, 512);
         run_dgrad(rt, adj_res_[i][0], d0n, gn, &gx);
+        wgrad(rp + "0", CONV_3x3, operand(tape.op_res[i][0]), d0n);
         gx = gn;
     }
     // bottleneck entry: conv over cat(feature, tiled pose)
-    View db = nbwd(tape.bott0, bott0_n_, ACT_RELU, gx);
+    View db = nbwd(tape.bott0, bott0_n_, ACT_RELU, gx, blk("bottleneck_blocks.", 0, ".1"));
     View dbin = fresh(P, B, b, b, 512 + pose_pad_);
     run_dgrad(rt, adj_bott0_, db, dbin);
+    {
+        WgradOperand x = operand(tape.op_bott0, &down_n_[3], &tape.down[3]);     // pose planes pass through the transform
+        wgrad(blk("bottleneck_blocks.", 0, ".0"), CONV_3x3, x, db, 512 + pose_ch_);
+    }
     if (want_pose) {
         pose_sum_kernel<<<B, round_up(pose_ch_, 32), 0, s>>>(dbin.p, dbin.ld, (long)b * b, 512, pose_ch_, g.d_pose, g.d_pose_ld);
         THA4_LAUNCH_CHECK();
     }
-    if (!want_img) return;
-    // encoder
-    d = nbwd(tape.down[3], down_n_[3], ACT_RELU, dbin.slice(0, 512));
+    if (!want_img && !want_par) return;
+    // encoder (walked for its parameters also when no image gradient is wanted)
+    d = nbwd(tape.down[3], down_n_[3], ACT_RELU, dbin.slice(0, 512), blk("downsample_blocks.", 3, ".1"));
     for (int i = 3; i >= 1; --i) {
         View da = fresh(P, B, S >> (i - 1), S >> (i - 1), adj_down_[i].cout);
         run_dgrad(rt, adj_down_[i], d, da);
-        d = nbwd(tape.down[i - 1], down_n_[i - 1], ACT_RELU, da);
+        wgrad(blk("downsample_blocks.", i, ".0"), CONV_4x4_S2, operand(tape.op_down[i], &down_n_[i - 1], &tape.down[i - 1]), d);
+        d = nbwd(tape.down[i - 1], down_n_[i - 1], ACT_RELU, da, blk("downsample_blocks.", i - 1, ".1"));
     }
+    wgrad(blk("downsample_blocks.", 0, ".0"), CONV_3x3, operand(tape.op_down[0]), d);
+    if (!want_img) return;
     View dx0 = fresh(P, B, S, S, in_ch_);
     run_dgrad(rt, adj_down_[0], d, dx0, &dimg);
     if (kind_ == TAIL_COMBINER) {

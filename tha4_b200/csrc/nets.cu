@@ -238,6 +238,7 @@ EncDecNet::EncDecNet(TailKind kind, int size, int in_ch, int pose_ch)
 void EncDecNet::load(const StateDict& sd, cudaStream_t s) {
     SinkScope own(&owned_);
     const std::string p = (kind_ == TAIL_FACE) ? "" : "body.";
+    prefix_ = p;
     down_[0] = load_conv(sd, p + "downsample_blocks.0.0", CONV_3x3, false, s);
     down_n_[0] = load_norm(sd, p + "downsample_blocks.0.1", s);
     for (int i = 1; i < 4; ++i) {
@@ -276,6 +277,28 @@ void EncDecNet::load(const StateDict& sd, cudaStream_t s) {
         tail_add_head(tail_, sd, "eye_alpha.0", true, s);
     }
     if (conv_pack_rounding()) tail_make_half(tail_, s);       // default mode: the wgmma tail's f16 head weights
+    // the flat parameter-gradient layout: the reference's state_dict order (registration order of the modules: per block its
+    // conv weight, then the InstanceNorm's weight and bias; then the heads in the tail's packing order, weight then bias)
+    head_key_.clear(); head_cout_.clear();
+    if (kind_ == TAIL_DECOMPOSER) head_key_ = {"background_layer_alpha.0", "background_layer_color_change.0", "eyebrow_layer_alpha.0", "eyebrow_layer_color_change.0"};
+    else if (kind_ == TAIL_COMBINER) head_key_ = {"morphed_eyebrow_layer_grid_change", "morphed_eyebrow_layer_alpha.0", "morphed_eyebrow_layer_color_change.0", "combine_alpha.0"};
+    else head_key_ = {"iris_mouth_grid_change", "iris_mouth_color_change.0", "iris_mouth_alpha.0", "eye_color_change.0", "eye_alpha.0"};
+    param_off_.clear(); param_total_ = 0;
+    auto reg = [&](const std::string& key) { param_off_[key] = param_total_; param_total_ += sd_get(sd, key).numel(); };
+    auto reg_block = [&](const std::string& conv, const std::string& norm) { reg(conv + ".weight"); reg(norm + ".weight"); reg(norm + ".bias"); };
+    for (int i = 0; i < 4; ++i) reg_block(p + "downsample_blocks." + std::to_string(i) + ".0", p + "downsample_blocks." + std::to_string(i) + ".1");
+    reg_block(p + "bottleneck_blocks.0.0", p + "bottleneck_blocks.0.1");
+    for (int i = 0; i < 5; ++i) {
+        const std::string rp = p + "bottleneck_blocks." + std::to_string(i + 1) + ".resnet_path.";
+        reg_block(rp + "0", rp + "1");
+        reg_block(rp + "3", rp + "4");
+    }
+    for (int i = 0; i < 3; ++i) reg_block(p + "upsample_blocks." + std::to_string(i) + ".0", p + "upsample_blocks." + std::to_string(i) + ".1");
+    for (const std::string& h : head_key_) {
+        reg(h + ".weight");
+        head_cout_.push_back((int)sd_get(sd, h + ".weight").shape[0]);
+        if (sd.count(h + ".bias")) reg(h + ".bias");
+    }
     load_adjoints(sd, p, s);
     THA4_CUDA_CHECK(cudaStreamSynchronize(s));
     loaded_ = true;
@@ -312,8 +335,11 @@ void EncDecNet::forward(Runtime& rt, const ImgView& image0, const ImgView& image
         return y;
     };
     View f = conv_in_relu(down_[0], down_n_[0], x0, S_, nullptr, false, tape ? &tape->down[0] : nullptr);       // the stride-2 convs read fp32
+    if (tape) { tape->op_down[0] = x0; tape->op_down[1] = f; }
     f = conv_in_relu(down_[1], down_n_[1], f, S_ / 2, nullptr, false, tape ? &tape->down[1] : nullptr);
+    if (tape) tape->op_down[2] = f;
     f = conv_in_relu(down_[2], down_n_[2], f, S_ / 4, nullptr, false, tape ? &tape->down[2] : nullptr);
+    if (tape) tape->op_down[3] = f;
     const int b = S_ / 8;
     View bin = h16 ? make_view16(P, B, b, b, 512 + pose_pad_) : make_view(P, B, b, b, 512 + pose_pad_);
     View bfeat = bin.slice(0, 512);
@@ -322,6 +348,7 @@ void EncDecNet::forward(Runtime& rt, const ImgView& image0, const ImgView& image
     // the bottleneck stream x is both a residual (fp32) and a conv operand (f16 copy x16)
     View x = make_view(P, B, b, b, bott0_.cout, &rt), x16;
     run_conv(rt, bott0_, bin, x);
+    if (tape) tape->op_bott0 = bin;
     if (h16) x16 = make_view16(P, B, b, b, bott0_.cout);
     {
         const View y = tape ? make_view(P, B, b, b, bott0_.cout) : x;
@@ -331,6 +358,7 @@ void EncDecNet::forward(Runtime& rt, const ImgView& image0, const ImgView& image
     }
     for (int i = 0; i < 5; ++i) {   // ResnetBlock: x + IN(conv(relu(IN(conv(x)))))  (resnet_block.py:52-67)
         View h = conv_in_relu(res_[i][0], res_n_[i][0], h16 ? x16 : x, b, nullptr, h16, tape ? &tape->res[i][0] : nullptr);
+        if (tape) { tape->op_res[i][0] = x; tape->op_res[i][1] = h; }
         View raw = make_view(P, B, b, b, 512, &rt);
         run_conv(rt, res_[i][1], h, raw);
         View n16; if (h16) n16 = make_view16(P, B, b, b, 512);
@@ -339,8 +367,11 @@ void EncDecNet::forward(Runtime& rt, const ImgView& image0, const ImgView& image
         if (tape) tape->res[i][1] = raw;
         x = y; x16 = n16;
     }
+    if (tape) tape->op_up[0] = x;
     x = conv_in_relu(up_[0], up_n_[0], h16 ? x16 : x, b * 2, nullptr, h16, tape ? &tape->up[0] : nullptr);
+    if (tape) tape->op_up[1] = x;
     x = conv_in_relu(up_[1], up_n_[1], x, b * 4, nullptr, h16, tape ? &tape->up[1] : nullptr);
+    if (tape) tape->op_up[2] = x;
     // last block: leave InstanceNorm + ReLU pending; the tail kernel applies them while staging its halo tile
     View raw = make_view(P, B, S_, S_, 64, &rt);
     run_conv(rt, up_[2], x, raw);
@@ -360,13 +391,13 @@ void EncDecNet::forward_fused(Runtime& rt, const View& x0, const ImgView& image0
     Pool* P = rt.persist;
     Tens r0 = make_act(P, rt, B, S_, S_, 64, false, true);
     run_conv_tc(rt, down_[0], x0, nullptr, r0);                                  // fp32 image operand (kind::tf32)
-    if (tape) tape->down[0] = raw_view(r0);
+    if (tape) { tape->down[0] = raw_view(r0); tape->op_down[0] = x0; }
     Tens prev = r0;
     for (int i = 1; i < 3; ++i) {
         Tens r = make_act(P, rt, B, S_ >> i, S_ >> i, down_[i].cout, false, true);
         const ConvNormIn ni = norm_in(prev.f, down_n_[i - 1], 0, ACT_RELU);
         run_conv_tc(rt, down_[i], prev.h, &ni, r);
-        if (tape) tape->down[i] = raw_view(r);
+        if (tape) { tape->down[i] = raw_view(r); tape->op_down[i] = prev.h; }
         prev = r;
     }
     const int b = S_ / 8;
@@ -376,7 +407,7 @@ void EncDecNet::forward_fused(Runtime& rt, const View& x0, const ImgView& image0
     {
         const ConvNormIn ni = norm_in(prev.f, down_n_[2], 0, ACT_RELU);
         run_conv_tc(rt, down_[3], prev.h, &ni, r3);
-        if (tape) tape->down[3] = raw_view(r3);
+        if (tape) { tape->down[3] = raw_view(r3); tape->op_down[3] = prev.h; }
     }
     if (pose_pad_ > 0) tile_vector(pose, pose_ld, pose_ch_, bin16.slice(512, pose_pad_), s);   // poser_encoder_decoder_00.py:110-113
     // bottleneck entry: conv -> IN -> ReLU; the result x is a residual stream (fp32) and a conv operand (f16 copy)
@@ -386,6 +417,7 @@ void EncDecNet::forward_fused(Runtime& rt, const View& x0, const ImgView& image0
         Tens xr; xr.f = x;
         const ConvNormIn ni = norm_in(r3.f, down_n_[3], 0, ACT_RELU, nullptr, nullptr, 0, 512);
         run_conv_tc(rt, bott0_, bin16, &ni, xr);
+        if (tape) tape->op_bott0 = bin16;
         const View y = tape ? make_view(P, B, b, b, bott0_.cout) : x;
         run_norm(rt, x, bott0_n_, 0, nullptr, nullptr, 0, ACT_RELU, 0, nullptr, y, &x16);
         if (tape) tape->bott0 = x;
@@ -400,7 +432,7 @@ void EncDecNet::forward_fused(Runtime& rt, const View& x0, const ImgView& image0
         View n16 = make_view16(P, B, b, b, 512);
         const View y = tape ? make_view(P, B, b, b, 512) : hb.f;
         run_norm(rt, hb.f, res_n_[i][1], 0, nullptr, nullptr, 0, ACT_NONE, 0, &x, y, &n16);
-        if (tape) { tape->res[i][0] = raw_view(ha); tape->res[i][1] = hb.f; }
+        if (tape) { tape->res[i][0] = raw_view(ha); tape->res[i][1] = hb.f; tape->op_res[i][0] = x16; tape->op_res[i][1] = ha.h; }
         x = y; x16 = n16;
     }
     Tens u0 = make_act(P, rt, B, 2 * b, 2 * b, up_[0].cout, false, true);
@@ -410,7 +442,7 @@ void EncDecNet::forward_fused(Runtime& rt, const View& x0, const ImgView& image0
         const ConvNormIn ni = norm_in(u0.f, up_n_[0], 0, ACT_RELU);
         run_conv_tc(rt, up_[1], u0.h, &ni, u1);
     }
-    if (tape) { tape->up[0] = raw_view(u0); tape->up[1] = raw_view(u1); }
+    if (tape) { tape->up[0] = raw_view(u0); tape->up[1] = raw_view(u1); tape->op_up[0] = x16; tape->op_up[1] = u0.h; tape->op_up[2] = u1.h; }
     // last block: InstanceNorm + ReLU stay pending; the tail kernel applies them while staging its halo tile
     const bool tc_tail = tail_.w16 != nullptr;
     Tens feat = make_act(P, rt, B, S_, S_, 64, !tc_tail, tc_tail);

@@ -53,9 +53,14 @@ struct Runtime {                      // per-call execution context
 // ------------------------------------------------------------------ encoder-decoder networks
 // The activations a backward pass reads from the forward it recomputes: the NHWC network input and the RAW output of every
 // conv that is followed by an InstanceNorm (fp32 or f16 data, with the statistics the producing conv accumulated).
+// op_*: the operand each trunk conv multiplied, for its weight gradient -- strict mode: the fp32 tensor it read (normalised,
+// the residual stream, the bottleneck input); default mode: the f16 tensor it read, whose pending normalisation (if any) the
+// conv applied on the fly (the producer's raw output, the bottleneck input bin16, the residual stream's f16 copy), or the
+// fp32 network input (op_down[0]).  Views of tensors the forward allocates anyway.
 struct EncDecTape {
     View x0;
     View down[4], bott0, res[5][2], up[3];
+    View op_down[4], op_bott0, op_res[5][2], op_up[3];
 };
 
 // What EncDecNet::backward computes.  grad_outputs: the upstream gradients of the network's outputs (NCHW, an entry may be
@@ -67,6 +72,10 @@ struct EncDecGrads {
     float* d_image1 = nullptr;
     float* d_pose = nullptr;
     int d_pose_ld = 0;
+    // parameter gradients: a flat fp32 buffer of param_count() floats in state_dict order (EncDecNet::param_offset);
+    // accumulate_params: add to what it holds (the second and later micro-batch chunks) instead of overwriting it
+    float* d_params = nullptr;
+    int accumulate_params = 0;
 };
 
 // EyebrowDecomposer00 / EyebrowMorphingCombiner00 / FaceMorpher08 (poser_encoder_decoder_00.py:43-121,
@@ -85,6 +94,9 @@ public:
     void backward(Runtime& rt, const ImgView& image0, const ImgView& image1, const float* pose, int pose_ld, const EncDecGrads& g);
     int size() const { return S_; }
     int num_outputs() const { return kind_ == TAIL_DECOMPOSER ? 6 : 8; }
+    // floats of the network's parameters, and the offset of a state_dict key's tensor in the flat state_dict-order buffer
+    long param_count() const { return param_total_; }
+    long param_offset(const std::string& key) const;
     bool loaded() const { return loaded_; }
 private:
     void forward_fused(Runtime& rt, const View& x0, const ImgView& image0, const ImgView& image1, const float* pose, int pose_ld,
@@ -94,6 +106,11 @@ private:
     TailKind kind_;
     int S_, in_ch_, pose_ch_, pose_pad_;
     bool loaded_ = false;
+    std::string prefix_;
+    std::map<std::string, long> param_off_;     // state_dict key -> offset in the flat parameter buffer
+    long param_total_ = 0;
+    std::vector<int> head_cout_;                // output channels of each head, in the tail's packing order
+    std::vector<std::string> head_key_;         //   and its state_dict prefix
     ConvWeights down_[4], bott0_, res_[5][2], up_[3];
     NormW down_n_[4], bott0_n_, res_n_[5][2], up_n_[3];
     TailWeights tail_;

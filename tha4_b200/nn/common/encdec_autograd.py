@@ -4,9 +4,13 @@ the reference modules are (eyebrow_decomposer_00.py:46-64, eyebrow_morphing_comb
 morpher_00.py:42-66, upscaler_02.py:59-96).  This is what pose fitting on an arbitrary character (expression and body parameters), or training an
 image -> pose regressor with a teacher as a differentiable renderer, needs.
 
-Dispatch: the autograd path runs when grad mode is on and an input (image, layer or pose) requires grad; in every other
-case the forward is the plain inference call.  Teacher parameters never receive gradients (there is no teacher training
-here), and unlike the SIREN students the module does not have to be frozen first.
+Dispatch: the autograd path runs when grad mode is on and an input (image, layer or pose) requires grad, or -- for the three
+encoder-decoder networks -- when the module was made trainable (`module.trainable_(True)`) and any of its parameters requires
+grad; in every other case the forward is the plain inference call.  Trainability is an explicit opt-in, not the students'
+"any parameter requires grad" rule, because a freshly built teacher's parameters require grad (as every nn.Module's do) and
+its inference calls must stay plain calls without a graph.  A trainable encoder-decoder module's backward returns the
+gradients of the parameters that require grad (flat d_params from the same library call as the input gradients); the
+U-Nets' parameters never receive gradients.
 
 Forward: the inference call; the outputs are bit-identical to the no-grad path (each in its own allocation, so in-place ops
 on them work).  Inputs and parameters are saved, so an in-place write to either between forward and backward raises torch's
@@ -19,6 +23,46 @@ from torch import Tensor
 from torch.autograd.function import once_differentiable
 
 from tha4_b200.nn.common.native_module import contiguous_grads, refuse_double_backward
+
+
+class Trainable:
+    """Opt-in parameter gradients of the encoder-decoder teacher modules (mixed into EyebrowDecomposer00,
+    EyebrowMorphingCombiner00, FaceMorpher08)."""
+    _trainable = False
+
+    def trainable_(self, mode: bool = True):
+        """Makes loss.backward() fill the .grad of this module's parameters that require grad; returns the module."""
+        self._trainable = bool(mode)
+        return self
+
+    def is_trainable(self) -> bool:
+        return self._trainable
+
+    def wants_autograd(self, *inputs: Tensor) -> bool:
+        if not torch.is_grad_enabled():
+            return False
+        return any(t.requires_grad for t in inputs) or (self._trainable and any(p.requires_grad for p in self._params()))
+
+
+def _param_grads(ctx, first: int, device):
+    """(flat d_params buffer or None, per-parameter gradient views or None) for the parameter slots that start at
+    needs_input_grad[first]: the views are in _params() order, which is state_dict order."""
+    need = ctx.needs_input_grad[first:]
+    module = ctx.module
+    if not (module.is_trainable() and any(need)):      # a module that is not trainable keeps its parameters' .grad untouched
+        return None, (None,) * len(need)
+    params = module._params()
+    if not getattr(module, '_param_order_checked', False):
+        assert [k for k, _ in module.named_parameters()] == list(module.state_dict().keys()), 'parameters are not in state_dict order'
+        module._param_order_checked = True
+    flat = torch.empty((ctx.lib.param_count(module.NET_NAME),), dtype=torch.float32, device=device)
+    views, off = [], 0
+    for p, w in zip(params, need):
+        n = p.numel()
+        views.append(flat[off:off + n].view_as(p) if w else None)
+        off += n
+    assert off == flat.numel(), (off, flat.numel())
+    return flat, tuple(views)
 
 
 def _own(outs: Sequence[Tensor]):
@@ -49,11 +93,15 @@ class _DecomposerFunction(torch.autograd.Function):
 def _decomposer_backward(ctx, *grad_outputs):
     image, *params = ctx.saved_tensors
     none = (None,) * len(params)
-    if not ctx.needs_input_grad[1] or all(g is None for g in grad_outputs):
+    if not any(ctx.needs_input_grad[1:]) or all(g is None for g in grad_outputs):
         return (None, None) + none
-    d_image = _empty_like(image)
-    ctx.module.sync_weights().eyebrow_decomposer_backward(image, contiguous_grads(grad_outputs), d_image)
-    return (None, d_image) + none
+    ctx.lib = ctx.module.sync_weights()
+    flat, dp = _param_grads(ctx, 2, image.device)
+    if flat is None and not ctx.needs_input_grad[1]:
+        return (None, None) + none
+    d_image = _empty_like(image) if ctx.needs_input_grad[1] else None
+    ctx.lib.eyebrow_decomposer_backward(image, contiguous_grads(grad_outputs), d_image, d_params=flat)
+    return (None, d_image) + dp
 
 
 class _CombinerFunction(torch.autograd.Function):
@@ -76,14 +124,18 @@ def _combiner_backward(ctx, *grad_outputs):
     background_layer, eyebrow_layer, pose, *params = ctx.saved_tensors
     none = (None,) * len(params)
     want = ctx.needs_input_grad[1:4]
-    if not any(want) or all(g is None for g in grad_outputs):
+    if not any(ctx.needs_input_grad[1:]) or all(g is None for g in grad_outputs):
+        return (None, None, None, None) + none
+    ctx.lib = ctx.module.sync_weights()
+    flat, dp = _param_grads(ctx, 4, background_layer.device)
+    if flat is None and not any(want):
         return (None, None, None, None) + none
     d_bg = _empty_like(background_layer) if want[0] else None
     d_eb = _empty_like(eyebrow_layer) if want[1] else None
     d_pose = _empty_like(pose) if want[2] else None
-    ctx.module.sync_weights().eyebrow_morphing_combiner_backward(background_layer, eyebrow_layer, pose, contiguous_grads(grad_outputs),
-                                                                d_background_layer=d_bg, d_eyebrow_layer=d_eb, d_pose=d_pose)
-    return (None, d_bg, d_eb, d_pose) + none
+    ctx.lib.eyebrow_morphing_combiner_backward(background_layer, eyebrow_layer, pose, contiguous_grads(grad_outputs),
+                                               d_background_layer=d_bg, d_eyebrow_layer=d_eb, d_pose=d_pose, d_params=flat)
+    return (None, d_bg, d_eb, d_pose) + dp
 
 
 class _FaceMorpherFunction(torch.autograd.Function):
@@ -106,12 +158,16 @@ def _face_morpher_backward(ctx, *grad_outputs):
     image, pose, *params = ctx.saved_tensors
     none = (None,) * len(params)
     want_image, want_pose = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
-    if not (want_image or want_pose) or all(g is None for g in grad_outputs):
+    if not any(ctx.needs_input_grad[1:]) or all(g is None for g in grad_outputs):
+        return (None, None, None) + none
+    ctx.lib = ctx.module.sync_weights()
+    flat, dp = _param_grads(ctx, 3, image.device)
+    if flat is None and not (want_image or want_pose):
         return (None, None, None) + none
     d_image = _empty_like(image) if want_image else None
     d_pose = _empty_like(pose) if want_pose else None
-    ctx.module.sync_weights().face_morpher_backward(image, pose, contiguous_grads(grad_outputs), d_image=d_image, d_pose=d_pose)
-    return (None, d_image, d_pose) + none
+    ctx.lib.face_morpher_backward(image, pose, contiguous_grads(grad_outputs), d_image=d_image, d_pose=d_pose, d_params=flat)
+    return (None, d_image, d_pose) + dp
 
 
 class _MorpherFunction(torch.autograd.Function):

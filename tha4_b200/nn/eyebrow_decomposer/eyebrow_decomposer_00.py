@@ -5,11 +5,11 @@ from typing import List
 from torch import Tensor
 
 from tha4_b200.nn.common import encdec_autograd
-from tha4_b200.nn.common.native_module import NativeModule, wants_autograd
+from tha4_b200.nn.common.native_module import NativeModule
 from tha4_b200.nn.state_dict_spec import eyebrow_decomposer_spec
 
 
-class EyebrowDecomposer00(NativeModule):
+class EyebrowDecomposer00(encdec_autograd.Trainable, NativeModule):
     NET_NAME = 'eyebrow_decomposer'
 
     def __init__(self, args=None):
@@ -17,7 +17,7 @@ class EyebrowDecomposer00(NativeModule):
         self.args = args
 
     def forward(self, image: Tensor, *args) -> List[Tensor]:
-        if wants_autograd(image):
+        if self.wants_autograd(image):
             return encdec_autograd.eyebrow_decomposer(self, image)
         return self.sync_weights().eyebrow_decomposer(image)
 

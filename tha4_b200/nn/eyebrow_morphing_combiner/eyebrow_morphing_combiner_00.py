@@ -5,11 +5,11 @@ from typing import List
 from torch import Tensor
 
 from tha4_b200.nn.common import encdec_autograd
-from tha4_b200.nn.common.native_module import NativeModule, wants_autograd
+from tha4_b200.nn.common.native_module import NativeModule
 from tha4_b200.nn.state_dict_spec import eyebrow_morphing_combiner_spec
 
 
-class EyebrowMorphingCombiner00(NativeModule):
+class EyebrowMorphingCombiner00(encdec_autograd.Trainable, NativeModule):
     NET_NAME = 'eyebrow_morphing_combiner'
 
     def __init__(self, args=None):
@@ -17,7 +17,7 @@ class EyebrowMorphingCombiner00(NativeModule):
         self.args = args
 
     def forward(self, background_layer: Tensor, eyebrow_layer: Tensor, pose: Tensor, *args) -> List[Tensor]:
-        if wants_autograd(background_layer, eyebrow_layer, pose):
+        if self.wants_autograd(background_layer, eyebrow_layer, pose):
             return encdec_autograd.eyebrow_morphing_combiner(self, background_layer, eyebrow_layer, pose)
         return self.sync_weights().eyebrow_morphing_combiner(background_layer, eyebrow_layer, pose)
 

@@ -5,11 +5,11 @@ from typing import List
 from torch import Tensor
 
 from tha4_b200.nn.common import encdec_autograd
-from tha4_b200.nn.common.native_module import NativeModule, wants_autograd
+from tha4_b200.nn.common.native_module import NativeModule
 from tha4_b200.nn.state_dict_spec import face_morpher_spec
 
 
-class FaceMorpher08(NativeModule):
+class FaceMorpher08(encdec_autograd.Trainable, NativeModule):
     NET_NAME = 'face_morpher'
 
     def __init__(self, args=None):
@@ -17,7 +17,7 @@ class FaceMorpher08(NativeModule):
         self.args = args
 
     def forward(self, image: Tensor, pose: Tensor, *args) -> List[Tensor]:
-        if wants_autograd(image, pose):
+        if self.wants_autograd(image, pose):
             return encdec_autograd.face_morpher(self, image, pose)
         return self.sync_weights().face_morpher(image, pose)
 

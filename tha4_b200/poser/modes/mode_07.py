@@ -76,7 +76,7 @@ class FiveStepPoserComputationProtocol(CachedComputationProtocol):
     def compute_func(self):
         def func(state: ComputationState) -> List[Tensor]:
             image, pose = state.batch[0], state.batch[1]
-            if torch.is_grad_enabled() and (image.requires_grad or pose.requires_grad):
+            if torch.is_grad_enabled() and (image.requires_grad or pose.requires_grad or self._trains_teacher(state)):
                 return self._differentiable(state)
             return self._single_call(state)
 
@@ -104,6 +104,13 @@ class FiveStepPoserComputationProtocol(CachedComputationProtocol):
             state.outputs[key] = output[sl]
         state.outputs[Branch.all_outputs.name] = output
 
+    @staticmethod
+    def _trains_teacher(state: ComputationState) -> bool:
+        """An encoder-decoder module of the poser was made trainable (trainable_(True)) and has parameters that require grad."""
+        return any(state.modules[net.name].wants_autograd()
+                   for net in (Network.eyebrow_decomposer, Network.eyebrow_morphing_combiner, Network.face_morpher)
+                   if net.name in state.modules)
+
     def _differentiable(self, state: ComputationState) -> List[Tensor]:
         """The modules composed as in the reference (mode_07.py:72-132; mode_12.py:66-94 for the face part), each through its
         autograd.Function, when the image or the pose requires grad.  The eyebrow cache is used only when the image does not
@@ -112,7 +119,7 @@ class FiveStepPoserComputationProtocol(CachedComputationProtocol):
         image, pose = state.batch[0], state.batch[1]
         modules = state.modules
         decomposer = modules[Network.eyebrow_decomposer.name]
-        if image.requires_grad:
+        if image.requires_grad or decomposer.wants_autograd():       # a trainable decomposer never reads the cache
             dec = decomposer(image[:, :, 64:192, 192:320])
         else:
             decomposer.sync_weights()
