@@ -114,8 +114,8 @@ int tha4_eyebrow_morphing_combiner_backward(tha4_ctx* ctx, const float* backgrou
                                             void* stream);
 int tha4_face_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
                                const float* const* grad_outputs, float* d_image, float* d_pose, float* d_params, void* stream);
-/* Floats of the parameters of THA4_NET_EYEBROW_DECOMPOSER / _EYEBROW_MORPHING_COMBINER / _FACE_MORPHER (the length of
- * d_params above); -1 for any other network. */
+/* Floats of the parameters of THA4_NET_EYEBROW_DECOMPOSER / _EYEBROW_MORPHING_COMBINER / _FACE_MORPHER / _BODY_MORPHER (the
+ * length of the d_params of their backward entries); -1 for any other network. */
 int64_t tha4_net_param_count(int net);
 /* Morpher00.forward (src/tha4/nn/morpher/morpher_00.py:42-66): image [B,4,256,256], pose [B,6] ->
  * merged(4) alpha(1) warped(4) grid_change(2) direct(4) */
@@ -125,9 +125,10 @@ int tha4_morpher_forward(tha4_ctx* ctx, const float* image, const float* pose, i
  * an entry may be NULL = zero), with the rules of the encoder-decoder entries above: d_image [B,4,256,256] and d_pose [B,6]
  * (contiguous) are optional (NULL = not computed), at least one non-NULL, each overwritten.  The forward is recomputed in the
  * context's precision mode and differentiated with fp32 data gradients.  Any B >= 1 (micro-batched).  The adjoint weights
- * are packed by the first call. */
+ * are packed by the first call.  d_params: the parameter gradients, as for the encoder-decoder entries (34 682 119 floats,
+ * state_dict order; the t = 0 time embedding and its FiLM projections included); NULL = not computed, counts as an output. */
 int tha4_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
-                          const float* const* grad_outputs, float* d_image, float* d_pose, void* stream);
+                          const float* const* grad_outputs, float* d_image, float* d_pose, float* d_params, void* stream);
 /* Upscaler02.forward (src/tha4/nn/upscaler/upscaler_02.py:59-96): rest_image [B,4,512,512], coarse_posed_image
  * [B,4,S,S], coarse_grid_change [B,2,S,S], pose [B,6] -> merged alpha warped grid_change direct.
  * coarse_size S = 512: the reference signature.  S = 256: the half-resolution body-morpher outputs; the bilinear x2
@@ -368,6 +369,18 @@ int tha4_test_group_norm_backward_ex(tha4_ctx* ctx, const void* x, int x_f16, in
 int tha4_test_conv_wgrad(tha4_ctx* ctx, int kind, int strict, int ksplit, const void* x, int x_f16, int x_ld, int N, int H, int W,
                          int Cx, int xf, const double* stats, int stats_rep, const float* gamma, const float* beta, int norm_C,
                          const float* dz, int dz_ld, int Cout, int c_real, float* dW, float* coef_out, int* plan, void* stream);
+/* The weight-gradient convolution's U-Net variants (Morpher00) through the same launcher.  kind: 0 3x3 s1 p1, 1 1x1, 2 nearest
+ * x2 + 3x3 (x at half dz's resolution), 3 the last.2 head (3x3, Cout <= 16 channels in the N dimension).  x: [N,H,W,x_ld]
+ * (f16 if x_f16), Cx channels; xf: 0 as stored, 1 the default mode's fused GroupNorm(groups) (+ FiLM0 [2 Cx] + FiLM1 row n
+ * at film1 + film1_off, ld film1_ld) (+act) with f16 coefficients from the forward's builder, 2 / 3 the tail's (fp32 affine
+ * from the statistics, 3 rounds to f16; no FiLM); act: 0 none, 1 ReLU, 2 SiLU, 3 the fast SiLU (tanh.approx) of the wgmma
+ * kernels.  Statistics [stats_rep][N][Cx][2].  dz: [N,Ho,Wo,dz_ld] fp32, Cout channels.  dW: [Cout][Cx][k][k], written.
+ * coef_out (optional): the [N][Cx] (A, B) pairs the transform used (f16 transform with SiLU: A / 2, B / 2).  plan[4]: as
+ * tha4_test_conv_wgrad. */
+int tha4_test_unet_wgrad(tha4_ctx* ctx, int kind, int strict, int ksplit, const void* x, int x_f16, int x_ld, int N, int H, int W,
+                         int Cx, int xf, int act, const double* stats, int stats_rep, int groups, const float* gamma, const float* beta,
+                         const float* film0, const float* film1, int film1_ld, int film1_off, const float* dz, int dz_ld, int Cout,
+                         float* dW, float* coef_out, int* plan, void* stream);
 /* InstanceNorm2d(affine) (+ReLU when act == 1) backward, norm_backward: x as above, dy / dx [N,H,W,C]. */
 int tha4_test_norm_backward_ex(tha4_ctx* ctx, const void* x, int x_f16, int x_ld, int N, int C, int H, int W, const double* stats,
                                int stats_rep, int stats_ld, const float* gamma, const float* beta, int act, const float* dy, int dy_ld,

@@ -33,7 +33,7 @@ EXPORTED_SYMBOLS = [
     'tha4_morpher_backward', 'tha4_upscaler_backward', 'tha4_net_param_count',
     'tha4_test_conv_backward_data', 'tha4_test_norm_backward', 'tha4_test_tail_backward', 'tha4_test_upscaler_prologue_backward',
     'tha4_test_group_norm_backward', 'tha4_test_attention_backward',
-    'tha4_test_group_norm_backward_ex', 'tha4_test_norm_backward_ex', 'tha4_test_conv_backward_data_ex', 'tha4_test_conv_wgrad', 'tha4_test_linear_backward',
+    'tha4_test_group_norm_backward_ex', 'tha4_test_norm_backward_ex', 'tha4_test_conv_backward_data_ex', 'tha4_test_conv_wgrad', 'tha4_test_unet_wgrad', 'tha4_test_linear_backward',
     'tha4_test_conv_forward_ex', 'tha4_test_tail_ex',
     'tha4_base_grid', 'tha4_test_conv', 'tha4_test_conv_norm', 'tha4_test_conv_norm_ex', 'tha4_test_conv_skip_fold', 'tha4_test_norm', 'tha4_test_tail', 'tha4_test_attention', 'tha4_test_linear',
     'tha4_test_siren_level', 'tha4_test_sine', 'tha4_test_siren_plan_check',
@@ -229,7 +229,8 @@ class Context:
         return gs
 
     def param_count(self, net: str) -> int:
-        """Floats of an encoder-decoder network's parameters: the length of the flat d_params buffer of its backward."""
+        """Floats of an encoder-decoder network's or the body morpher's parameters: the length of the flat d_params buffer of
+        its backward."""
         n = int(self.lib.tha4_net_param_count(NET_IDS[net]))
         if n < 0:
             raise Tha4Error('%s has no parameter gradients' % net)
@@ -296,10 +297,11 @@ class Context:
         return outs
 
     def morpher_backward(self, image: Tensor, pose: Tensor, grad_outputs: Sequence[Optional[Tensor]],
-                         d_image: Optional[Tensor] = None, d_pose: Optional[Tensor] = None):
-        """Input gradients of Morpher00 into d_image [B,4,256,256] and / or d_pose [B,6] (None = not computed) for the upstream
-        gradients of its five outputs (None = zero); the forward is recomputed in the context's precision mode."""
-        assert d_image is not None or d_pose is not None
+                         d_image: Optional[Tensor] = None, d_pose: Optional[Tensor] = None, d_params: Optional[Tensor] = None):
+        """Input gradients of Morpher00 into d_image [B,4,256,256] and / or d_pose [B,6], parameter gradients into d_params
+        (flat, state_dict order) (None = not computed) for the upstream gradients of its five outputs (None = zero); the
+        forward is recomputed in the context's precision mode."""
+        assert d_image is not None or d_pose is not None or d_params is not None
         image = _check_input(image, self.device, 'image')
         pose = _check_input(pose, self.device, 'pose')
         B = image.shape[0]
@@ -307,8 +309,9 @@ class Context:
         gs = self._grads(self.MORPHER_SPECS, grad_outputs, B)
         self._check_out(d_image, (B, 4, 256, 256), 'd_image')
         self._check_out(d_pose, (B, 6), 'd_pose')
+        self._check_out(d_params, (self.param_count('body_morpher'),), 'd_params')
         self._call('tha4_morpher_backward', _ptr(image), _ptr(pose), 6, B, _ptr_array(gs), _ptr(d_image), _ptr(d_pose),
-                   self._stream())
+                   _ptr(d_params), self._stream())
 
     UPSCALER_SPECS = [(4, 512), (1, 512), (4, 512), (2, 512), (4, 512)]
 

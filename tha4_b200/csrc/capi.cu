@@ -359,14 +359,15 @@ int64_t tha4_net_param_count(int net) {
         case THA4_NET_EYEBROW_DECOMPOSER: return 31479434;
         case THA4_NET_EYEBROW_MORPHING_COMBINER: return 31535878;
         case THA4_NET_FACE_MORPHER: return 31605002;
+        case THA4_NET_BODY_MORPHER: return 34682119;
         default: return -1;
     }
 }
 
 namespace {
 // checks the network's flat parameter layout against the ABI's count before a backward writes d_params
-void check_param_layout(const EncDecNet& net, int id, const float* d_params) {
-    if (d_params) THA4_REQUIRE(net.param_count() == tha4_net_param_count(id), "backward: the loaded state_dict does not have the network's parameters");
+void check_param_layout(long count, int id, const float* d_params) {
+    if (d_params) THA4_REQUIRE(count == tha4_net_param_count(id), "backward: the loaded state_dict does not have the network's parameters");
 }
 }  // namespace
 
@@ -374,7 +375,7 @@ int tha4_eyebrow_decomposer_backward(tha4_ctx* ctx, const float* image, int B, c
                                      float* d_image, float* d_params, void* stream) {
     return guarded(ctx, [&] {
         THA4_REQUIRE(d_image || d_params, "decomposer backward: no gradient requested");
-        check_param_layout(*ctx->decomposer, THA4_NET_EYEBROW_DECOMPOSER, d_params);
+        check_param_layout(d_params ? ctx->decomposer->param_count() : 0, THA4_NET_EYEBROW_DECOMPOSER, d_params);
         Runtime rt = make_rt(ctx, stream);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             const float* g[6]; offset_grads<6>(grad_outputs, kEncDecDecomposer, n0, g);
@@ -390,7 +391,7 @@ int tha4_eyebrow_morphing_combiner_backward(tha4_ctx* ctx, const float* backgrou
                                             float* d_background_layer, float* d_eyebrow_layer, float* d_pose, float* d_params, void* stream) {
     return guarded(ctx, [&] {
         THA4_REQUIRE(d_background_layer || d_eyebrow_layer || d_pose || d_params, "combiner backward: no gradient requested");
-        check_param_layout(*ctx->combiner, THA4_NET_EYEBROW_MORPHING_COMBINER, d_params);
+        check_param_layout(d_params ? ctx->combiner->param_count() : 0, THA4_NET_EYEBROW_MORPHING_COMBINER, d_params);
         THA4_REQUIRE(pose_ld >= 12, "combiner backward: pose rows need at least 12 entries");
         Runtime rt = make_rt(ctx, stream);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
@@ -411,7 +412,7 @@ int tha4_face_morpher_backward(tha4_ctx* ctx, const float* image, const float* p
                                const float* const* grad_outputs, float* d_image, float* d_pose, float* d_params, void* stream) {
     return guarded(ctx, [&] {
         THA4_REQUIRE(d_image || d_pose || d_params, "face morpher backward: no gradient requested");
-        check_param_layout(*ctx->face, THA4_NET_FACE_MORPHER, d_params);
+        check_param_layout(d_params ? ctx->face->param_count() : 0, THA4_NET_FACE_MORPHER, d_params);
         THA4_REQUIRE(pose_ld >= 27, "face morpher backward: pose rows need at least 27 entries");
         Runtime rt = make_rt(ctx, stream);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
@@ -440,9 +441,10 @@ int tha4_morpher_forward(tha4_ctx* ctx, const float* image, const float* pose, i
 }
 
 int tha4_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
-                          const float* const* grad_outputs, float* d_image, float* d_pose, void* stream) {
+                          const float* const* grad_outputs, float* d_image, float* d_pose, float* d_params, void* stream) {
     return guarded(ctx, [&] {
-        THA4_REQUIRE(d_image || d_pose, "morpher backward: no gradient requested");
+        THA4_REQUIRE(d_image || d_pose || d_params, "morpher backward: no gradient requested");
+        check_param_layout(d_params ? ctx->body->param_count() : 0, THA4_NET_BODY_MORPHER, d_params);
         THA4_REQUIRE(pose_ld >= 6, "morpher backward: pose rows need at least 6 entries");
         Runtime rt = make_rt(ctx, stream);
         OutSpec spec[5]; fill_unet_spec(spec, 256);
@@ -451,6 +453,7 @@ int tha4_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, 
             UNetGrads ug; ug.grad_outputs = g;
             ug.d_image = d_image ? d_image + (size_t)n0 * 4 * 256 * 256 : nullptr;
             ug.d_pose = d_pose ? d_pose + (size_t)n0 * 6 : nullptr; ug.d_pose_ld = 6;
+            ug.d_params = d_params; ug.accumulate_params = n0 > 0;
             ctx->body->backward(rt, make_img(image + (size_t)n0 * 4 * 256 * 256, b, 4, 256, 256), nullptr, nullptr, 0,
                                 pose + (size_t)n0 * pose_ld, pose_ld, ug);
         });
@@ -1338,7 +1341,7 @@ int tha4_test_conv_wgrad(tha4_ctx* ctx, int kind, int strict, int ksplit, const 
             if (xf == WG_XF_HALF) wgrad_xf_coef(st, gamma, beta, norm_C, ACT_RELU, coef, s);
             else norm_finalize(st, 0, gamma, beta, nullptr, nullptr, 0, reinterpret_cast<float*>(coef), s);
             if (coef_out) THA4_CUDA_CHECK(cudaMemcpyAsync(coef_out, coef, (size_t)N * norm_C * sizeof(float2), cudaMemcpyDeviceToDevice, s));
-            xo.xf = xf; xo.relu = 1; xo.coef = coef; xo.coef_C = norm_C;
+            xo.xf = xf; xo.act = ACT_RELU; xo.coef = coef; xo.coef_C = norm_C;
         }
         const int oh = kind == 1 ? H / 2 : (kind == 2 ? 2 * H : H);
         WgradOperand d;
@@ -1351,6 +1354,38 @@ int tha4_test_conv_wgrad(tha4_ctx* ctx, int kind, int strict, int ksplit, const 
             for (int k = 0; k < Cout; ++k) a.out_row[k] = (long)k * (c_real ? c_real : Cx) * 9;
         }
         const ConvKind ck = kind == 1 ? CONV_4x4_S2 : (kind == 2 ? CONVT_4x4_S2 : CONV_3x3);
+        const WgradPlan pl = conv_wgrad_layer(ck, xo, d, a, strict, ksplit, [&](size_t n) { return ctx->scratch.alloc(n); }, s);
+        if (plan) { plan[0] = pl.nt; plan[1] = pl.mtiles; plan[2] = pl.ntiles; plan[3] = pl.splits; }
+    });
+}
+
+int tha4_test_unet_wgrad(tha4_ctx* ctx, int kind, int strict, int ksplit, const void* x, int x_f16, int x_ld, int N, int H, int W,
+                         int Cx, int xf, int act, const double* stats, int stats_rep, int groups, const float* gamma, const float* beta,
+                         const float* film0, const float* film1, int film1_ld, int film1_off, const float* dz, int dz_ld, int Cout,
+                         float* dW, float* coef_out, int* plan, void* stream) {
+    return guarded(ctx, [&] {
+        cudaStream_t s = (cudaStream_t)stream;
+        THA4_REQUIRE(kind >= 0 && kind <= 3, "test_unet_wgrad: kind 0..3");
+        THA4_REQUIRE(act >= ACT_NONE && act <= ACT_SILU_FAST, "test_unet_wgrad: act 0..3");
+        THA4_REQUIRE(xf >= WG_XF_NONE && xf <= WG_XF_FLOAT16 && (xf == WG_XF_NONE || stats), "test_unet_wgrad: transform");
+        THA4_REQUIRE(xf == WG_XF_HALF || (!film0 && !film1), "test_unet_wgrad: FiLM on the f16 transform only");
+        begin_pass(ctx, s);
+        WgradOperand xo;
+        xo.p = x; xo.f16 = x_f16 ? 1 : 0; xo.ld = x_ld; xo.N = N; xo.H = H; xo.W = W; xo.C = Cx;
+        if (xf != WG_XF_NONE) {
+            const View st = stats_input(x, x_f16, x_ld, N, Cx, H, W, stats, stats_rep, Cx);
+            float2* coef = reinterpret_cast<float2*>(ctx->persist.alloc((size_t)N * Cx * 2));
+            if (xf == WG_XF_HALF) wgrad_xf_coef(st, gamma, beta, Cx, act, coef, s, groups, film0, film1 ? film1 + film1_off : nullptr, film1_ld);
+            else norm_finalize(st, groups, gamma, beta, nullptr, nullptr, 0, reinterpret_cast<float*>(coef), s);
+            if (coef_out) THA4_CUDA_CHECK(cudaMemcpyAsync(coef_out, coef, (size_t)N * Cx * sizeof(float2), cudaMemcpyDeviceToDevice, s));
+            xo.coef = coef; xo.coef_C = Cx;
+        }
+        xo.xf = xf; xo.act = act;
+        WgradOperand d;
+        d.p = dz; d.ld = dz_ld; d.N = N; d.H = kind == 2 ? 2 * H : H; d.W = kind == 2 ? 2 * W : W; d.C = Cout;
+        WgradArgs a;
+        a.out = dW;
+        const ConvKind ck = kind == 1 ? CONV_1x1 : (kind == 2 ? CONV_UP2_3x3 : CONV_3x3);
         const WgradPlan pl = conv_wgrad_layer(ck, xo, d, a, strict, ksplit, [&](size_t n) { return ctx->scratch.alloc(n); }, s);
         if (plan) { plan[0] = pl.nt; plan[1] = pl.mtiles; plan[2] = pl.ntiles; plan[3] = pl.splits; }
     });

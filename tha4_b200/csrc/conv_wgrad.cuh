@@ -1,4 +1,4 @@
-// Weight-gradient convolution of the encoder-decoder teachers (conv_wgrad.cu) -- declarations.
+// Weight-gradient convolution of the teacher networks (conv_wgrad.cu) -- declarations.
 #pragma once
 #include "common.cuh"
 #include "conv.cuh"
@@ -14,13 +14,18 @@ enum WgradXf {
     WG_XF_FLOAT16 = 3,     // fp32 FMA rounded to f16 (the default-mode tail's operand)
 };
 
-// An NHWC operand: `C` channels are read (ld elements per pixel), f16 or fp32; channels < coef_C get y = A x + B (+ReLU)
-// with coef[n][c] = (A, B); the rest pass through (pose planes).
+// An NHWC operand: `C` channels are read (ld elements per pixel), f16 or fp32; channels < coef_C get y = act(A x + B) with
+// coef[n][c] = (A, B); the rest pass through (pose planes).  act (Act):
+//   ACT_RELU       max(y, 0) in the transform's precision;
+//   ACT_SILU       fp32 y / (1 + expf(-y)) (WG_XF_FLOAT: the strict tail);
+//   ACT_SILU_FAST  h + h tanh(h) with h = y / 2 -- WG_XF_HALF: in f16 with tanh.approx.f16x2 on coefficients that hold A / 2,
+//                  B / 2 already (the wgmma convs' operand transform, conv_tc_device.cuh); WG_XF_FLOAT / WG_XF_FLOAT16: fp32
+//                  with tanh.approx.f32, the halving done here (the wgmma tail, tail_tc.cu).
 struct WgradOperand {
     const void* p = nullptr;
     int f16 = 0, ld = 0;
     int N = 0, H = 0, W = 0, C = 0;
-    int xf = WG_XF_NONE, relu = 0;
+    int xf = WG_XF_NONE, act = ACT_NONE;
     const float2* coef = nullptr;
     int coef_C = 0;
 };
@@ -40,6 +45,8 @@ struct WgradArgs {
     // filled by conv_wgrad from the plan
     int kblocks = 0, kb_per_split = 0, splits = 1;
     float* ws = nullptr; int ws_rows = 0, ws_cols = 0;
+    int up2 = 0;                       // G is read through a nearest x2 up-sampling: tap (y + ky - 1, x + kx - 1) is checked at D's
+                                       // resolution, then halved (CONV_UP2_3x3)
 };
 
 // How a launch is cut: nt output columns per CTA (16 / 64 / 128), 64-row tiles, pixel blocks of 32 split over `splits`
@@ -49,14 +56,16 @@ struct WgradPlan { int nt = 0, mtiles = 0, ntiles = 0, kblocks = 0, kb_per_split
 WgradPlan conv_wgrad_plan(const WgradArgs& a, int ksplit = 0);
 size_t conv_wgrad_workspace_floats(const WgradPlan& pl);
 void conv_wgrad(WgradArgs a, const WgradPlan& pl, int strict, float* ws, cudaStream_t s);
-// The weight gradient of one conv of `kind` (CONV_3x3, CONV_4x4_S2, CONVT_4x4_S2) from the operand x^ the forward multiplied
-// and the gradient dz at its raw output, as the network backward runs it: Conv2d G = x^, D = dz; ConvTranspose2d G = dz,
-// D = x^.  `a` carries the destination (out, out_row / n_map, c_real (0: every channel of G), accumulate); ksplit > 0 forces
+// The weight gradient of one conv of `kind` (CONV_3x3, CONV_1x1, CONV_UP2_3x3, CONV_4x4_S2, CONVT_4x4_S2) from the operand
+// x^ the forward multiplied and the gradient dz at its raw output, as the network backward runs it: Conv2d G = x^, D = dz;
+// ConvTranspose2d G = dz, D = x^; nearest x2 + 3x3: x^ at half D's resolution.  `a` carries the destination (out, out_row / n_map, c_real (0: every channel of G), accumulate); ksplit > 0 forces
 // the pixel split; ws_alloc hands out the split workspace.  Returns the plan that ran.
 WgradPlan conv_wgrad_layer(ConvKind kind, const WgradOperand& x, const WgradOperand& dz, WgradArgs a, int strict, int ksplit,
                            const std::function<float*(size_t)>& ws_alloc, cudaStream_t s);
-// coef[n][c] = the (A, B) of the pending InstanceNorm (+act) of `raw` (its statistics) as the forward's fused normalisation
-// rounds them to f16; C channels, coef holds raw.N * C float2
-float2* wgrad_xf_coef(const View& raw, const float* gamma, const float* beta, int C, int act, float2* coef, cudaStream_t s);
+// coef[n][c] = the (A, B) of the pending InstanceNorm (groups == 0) or GroupNorm (+ FiLM0 [2C] + FiLM1 row n of film1, ld
+// film1_ld) (+act) of `raw` (its statistics), built by the forward's fused-normalisation code (xf_build_coef) and rounded to
+// f16 as it rounds them (SiLU: A / 2, B / 2); C channels, coef holds raw.N * C float2
+float2* wgrad_xf_coef(const View& raw, const float* gamma, const float* beta, int C, int act, float2* coef, cudaStream_t s,
+                      int groups = 0, const float* film0 = nullptr, const float* film1 = nullptr, int film1_ld = 0);
 
 }  // namespace tha4

@@ -499,7 +499,7 @@ void EncDecNet::backward(Runtime& rt, const ImgView& image0, const ImgView& imag
         if (nw && rt.f16) {
             float2* coef = reinterpret_cast<float2*>(P->alloc((size_t)v.N * nw->C * 2));
             wgrad_xf_coef(*stats, nw->gamma, nw->beta, nw->C, ACT_RELU, coef, s);
-            o.xf = WG_XF_HALF; o.relu = 1; o.coef = coef; o.coef_C = nw->C;
+            o.xf = WG_XF_HALF; o.act = ACT_RELU; o.coef = coef; o.coef_C = nw->C;
         }
         return o;
     };
@@ -533,7 +533,7 @@ void EncDecNet::backward(Runtime& rt, const ImgView& image0, const ImgView& imag
         float2* coef = reinterpret_cast<float2*>(P->alloc((size_t)B * f.C * 2));
         norm_finalize(f, 0, up_n_[2].gamma, up_n_[2].beta, nullptr, nullptr, 0, reinterpret_cast<float*>(coef), s);
         WgradOperand x = operand(f);
-        x.xf = f.f16 ? WG_XF_FLOAT16 : WG_XF_FLOAT; x.relu = 1; x.coef = coef; x.coef_C = f.C;
+        x.xf = f.f16 ? WG_XF_FLOAT16 : WG_XF_FLOAT; x.act = ACT_RELU; x.coef = coef; x.coef_C = f.C;
         WgradArgs a;
         WgradOperand d = operand(dh);
         HeadBiasArgs hb; hb.dh = dh.p; hb.pixels = (long)B * S * S; hb.out = g.d_params; hb.accumulate = g.accumulate_params;

@@ -473,6 +473,7 @@ namespace {
 
 ResBlockW load_res_block(const StateDict& sd, const std::string& p, cudaStream_t s, bool upsampling = false) {
     ResBlockW w;
+    w.key = p;
     w.norm0 = load_norm(sd, p + ".norm0", s);
     w.conv0 = load_conv(sd, p + ".conv0", upsampling ? CONV_UP2_3x3 : CONV_3x3, true, s);
     w.norm1 = load_norm(sd, p + ".norm1", s);
@@ -488,6 +489,7 @@ ResBlockW load_res_block(const StateDict& sd, const std::string& p, cudaStream_t
 
 AttnW load_attn(const StateDict& sd, const std::string& p, cudaStream_t s) {
     AttnW a;
+    a.key = p;
     a.norm = load_norm(sd, p + ".norm", s);
     a.qkv = load_conv(sd, p + ".qkv", CONV_1x1, true, s);
     a.proj = load_conv(sd, p + ".conv", CONV_1x1, true, s);
@@ -564,10 +566,11 @@ void UNetNet::load(const StateDict& sd, cudaStream_t s) {
     // time embedding at t = 0 is a constant: cat(cos(0)..., sin(0)...) -> Linear -> SiLU -> Linear  (unet.py:365-376,443-447)
     std::vector<float> t0(mc_, 0.0f);
     for (int i = 0; i < mc_ / 2; ++i) t0[i] = 1.0f;
-    float* d_t0 = dev_alloc_tmp(mc_);
+    // the body morpher keeps them (and time_embed.3's weight) for its parameter gradients
+    float* d_t0 = upscaler_ ? dev_alloc_tmp(mc_) : dev_alloc(mc_);
     THA4_CUDA_CHECK(cudaMemcpyAsync(d_t0, t0.data(), mc_ * sizeof(float), cudaMemcpyHostToDevice, s));
-    float* d_t1 = dev_alloc_tmp(256);
-    float* d_t2 = dev_alloc_tmp(256);
+    float* d_t1 = upscaler_ ? dev_alloc_tmp(256) : dev_alloc(256);
+    float* d_t2 = upscaler_ ? dev_alloc_tmp(256) : dev_alloc(256);
     linear_forward(d_t0, mc_, 1, mc_, sd_get(sd, p + "time_embed.1.weight").p, sd_get(sd, p + "time_embed.1.bias").p, 256, 0, d_t1, 256, s);
     linear_forward(d_t1, 256, 1, 256, sd_get(sd, p + "time_embed.3.weight").p, sd_get(sd, p + "time_embed.3.bias").p, 256, 1, d_t2, 256, s);
 
@@ -576,12 +579,14 @@ void UNetNet::load(const StateDict& sd, cudaStream_t s) {
     for (auto& e : all_blocks) { e.first->film1_off = film1_total_; film1_total_ += 2 * e.first->cout; }
     film1_w_ = dev_alloc((size_t)film1_total_ * 256);
     film1_b_ = dev_alloc(film1_total_);
+    if (!upscaler_) film0_w_ = dev_alloc((size_t)film1_total_ * 256);
     for (auto& e : all_blocks) {
         ResBlockW* w = e.first;
         const TensorRef& c0w = sd_get(sd, e.second + ".cond0_layers.1.weight");
         THA4_REQUIRE(c0w.shape[0] == 2 * w->cout && c0w.shape[1] == 256, "cond0 shape: " + e.second);
         w->film0 = dev_alloc(2 * w->cout);
         linear_forward(d_t2, 256, 1, 256, c0w.p, sd_get(sd, e.second + ".cond0_layers.1.bias").p, 2 * w->cout, 1, w->film0, 2 * w->cout, s);
+        if (film0_w_) THA4_CUDA_CHECK(cudaMemcpyAsync(film0_w_ + (size_t)w->film1_off * 256, c0w.p, c0w.numel() * sizeof(float), cudaMemcpyDeviceToDevice, s));
         const TensorRef& c1w = sd_get(sd, e.second + ".cond1_layers.1.weight");
         THA4_REQUIRE(c1w.shape[0] == 2 * w->cout && c1w.shape[1] == 256, "cond1 shape: " + e.second);
         THA4_CUDA_CHECK(cudaMemcpyAsync(film1_w_ + (size_t)w->film1_off * 256, c1w.p, c1w.numel() * sizeof(float), cudaMemcpyDeviceToDevice, s));
@@ -589,9 +594,49 @@ void UNetNet::load(const StateDict& sd, cudaStream_t s) {
                                         2 * w->cout * sizeof(float), cudaMemcpyDeviceToDevice, s));
     }
     if (conv_pack_rounding()) tail_make_half(tail_, s);       // default mode: the wgmma tail's f16 head weights
+    param_off_.clear(); param_total_ = 0;
+    if (!upscaler_) {
+        time_t0_ = d_t0; time_t1_ = d_t1; time_t2_ = d_t2;
+        time_w3_ = dev_clone(sd_get(sd, p + "time_embed.3.weight"), s);
+        // the flat parameter-gradient layout: the reference's state_dict order (unet.py:438-529, registration order of the
+        // modules; per up level its ResBlocks, then its attention blocks, then the up-sampler)
+        auto reg = [&](const std::string& key) { param_off_[key] = param_total_; param_total_ += sd_get(sd, key).numel(); };
+        auto reg_res = [&](const ResBlockW& w) {
+            for (const char* k : {".norm0.weight", ".norm0.bias", ".conv0.weight", ".conv0.bias", ".cond0_layers.1.weight",
+                                  ".cond0_layers.1.bias", ".norm1.weight", ".norm1.bias", ".conv1.weight", ".conv1.bias",
+                                  ".cond1_layers.1.weight", ".cond1_layers.1.bias"})
+                reg(w.key + k);
+            if (w.has_skip) { reg(w.key + ".skip.weight"); reg(w.key + ".skip.bias"); }
+        };
+        auto reg_attn = [&](const AttnW& a) {
+            for (const char* k : {".norm.weight", ".norm.bias", ".qkv.weight", ".qkv.bias", ".conv.weight", ".conv.bias"}) reg(a.key + k);
+        };
+        for (const char* k : {"time_embed.1.weight", "time_embed.1.bias", "time_embed.3.weight", "time_embed.3.bias", "cond_embed.0.weight",
+                              "cond_embed.0.bias", "cond_embed.2.weight", "cond_embed.2.bias", "first_conv.weight", "first_conv.bias"})
+            reg(p + k);
+        for (int i = 0; i < L_; ++i) {
+            reg_res(down_res_[i]);
+            if (i == L_ - 1) reg_attn(down_attn_);
+            if (i < L_ - 1) reg_res(down_ds_[i]);
+        }
+        for (int j = 0; j < 7; ++j) { if (j % 2 == 0) reg_res(mid_res_[j / 2]); else reg_attn(mid_attn_[j / 2]); }
+        for (int bi = 0; bi < L_; ++bi) {
+            reg_res(up_res_[2 * bi]); reg_res(up_res_[2 * bi + 1]);
+            if (bi == 0) { reg_attn(up_attn_[0]); reg_attn(up_attn_[1]); }
+            if (bi < L_ - 1) reg_res(up_us_[bi]);
+        }
+        for (const char* k : {"last.0.weight", "last.0.bias", "last.2.weight", "last.2.bias"}) reg(p + k);
+        THA4_REQUIRE((long)param_off_.size() == (long)sd.size(), "unet: the state_dict has tensors outside the parameter layout");
+    }
     THA4_CUDA_CHECK(cudaStreamSynchronize(s));
-    cudaFree(d_t0); cudaFree(d_t1); cudaFree(d_t2);
+    if (upscaler_) { cudaFree(d_t0); cudaFree(d_t1); cudaFree(d_t2); }
     loaded_ = true;
+}
+
+long UNetNet::param_offset(const std::string& key) const {
+    auto it = param_off_.find(key);
+    THA4_REQUIRE(it != param_off_.end(), "parameter gradients: no tensor " + key);
+    return it->second;
 }
 
 // ResBlock (unet.py:154-165).  mode: 0 same, 1 up (nearest x2), 2 down (AvgPool2d(2)).
@@ -603,13 +648,15 @@ void UNetNet::res_block(Runtime& rt, const ResBlockW& w, const View& x, int mode
     // norm0 -> SiLU -> (avg-pool) ; the nearest-upsample is folded into conv0's gather
     const int th = (mode == 2) ? x.H / 2 : x.H;
     const bool h16 = rt.f16 != 0;
-    View t0 = h16 ? make_view16(rt.scratch, B, th, th, w.cin) : make_view(rt.scratch, B, th, th, w.cin);
+    const bool ops = tape && tape->ops;          // the normalised operands stay for the weight gradients
+    Pool* op_pool = ops ? rt.persist : rt.scratch;
+    View t0 = h16 ? make_view16(op_pool, B, th, th, w.cin) : make_view(op_pool, B, th, th, w.cin);
     run_norm(rt, x, w.norm0, 32, nullptr, nullptr, 0, rt.strict ? ACT_SILU : ACT_SILU_FAST, mode == 2 ? 1 : 0, nullptr, t0);
     View h = make_view(tape ? rt.persist : rt.scratch, B, out.H, out.W, w.cout, &rt);
     run_conv(rt, w.conv0, t0, h);      // mode 1: conv0 was packed as CONV_UP2_3x3 (upsample folded into 4 phases)
-    if (tape) tape->res[&w] = {x, h};
     // norm1 -> FiLM(time) -> FiLM(pose) -> SiLU, folded into one per-(n,c) affine
-    const View h2 = h16 ? make_view16(rt.scratch, B, out.H, out.W, w.cout) : (tape ? make_view(rt.scratch, B, out.H, out.W, w.cout) : h);
+    const View h2 = h16 ? make_view16(op_pool, B, out.H, out.W, w.cout) : (tape ? make_view(op_pool, B, out.H, out.W, w.cout) : h);
+    if (tape) tape->res[&w] = {x, h, ops ? t0 : View{}, ops ? h2 : View{}};
     run_norm(rt, h, w.norm1, 32, w.film0, film1 + w.film1_off, film1_total_, rt.strict ? ACT_SILU : ACT_SILU_FAST, 0, nullptr, h2);
     if (w.has_skip) {
         THA4_REQUIRE(mode == 0, "res_block: skip conv only on same-resolution blocks");
@@ -625,12 +672,14 @@ void UNetNet::res_block(Runtime& rt, const ResBlockW& w, const View& x, int mode
 void UNetNet::attn_block(Runtime& rt, const AttnW& w, const View& x, const View& out, UNetTape* tape) {
     cudaStream_t s = rt.stream;
     rt.scratch->reset();
-    View t = rt.f16 ? make_view16(rt.scratch, x.N, x.H, x.W, x.C) : make_view(rt.scratch, x.N, x.H, x.W, x.C);
+    const bool ops = tape && tape->ops;
+    Pool* op_pool = ops ? rt.persist : rt.scratch;
+    View t = rt.f16 ? make_view16(op_pool, x.N, x.H, x.W, x.C) : make_view(op_pool, x.N, x.H, x.W, x.C);
     run_norm(rt, x, w.norm, 32, nullptr, nullptr, 0, ACT_NONE, 0, nullptr, t);
     View qkv = make_view(tape ? rt.persist : rt.scratch, x.N, x.H, x.W, 3 * x.C);
     run_conv(rt, w.qkv, t, qkv);
-    if (tape) tape->attn[&w] = {x, qkv};
-    View a = make_view(rt.scratch, x.N, x.H, x.W, x.C);
+    View a = make_view(op_pool, x.N, x.H, x.W, x.C);
+    if (tape) tape->attn[&w] = {x, qkv, ops ? t : View{}, ops ? a : View{}};
     attention_forward(qkv, 8, a, s, !rt.strict);
     run_conv(rt, w.proj, a, out, 0, &x, RES_SAME);
 }
@@ -662,6 +711,7 @@ void UNetNet::forward(Runtime& rt, const ImgView& image, const float* coarse_pos
         x0 = make_view(P, B, S_, S_, 4);
         nchw_to_nhwc(image, x0, s);
     }
+    if (tape) tape->x0 = x0;
 
     // ---- plan the skip concatenations: up res-block j reads cat(h_j, hs[2L-1-j]) from one buffer ----
     const int NH = 2 * L_;
@@ -796,7 +846,8 @@ struct UNetFused {
         }
         View xpool;
         if (mode == 2) {          // norm0 -> SiLU -> 2x2 mean as a pass (f16 result), then a plain conv
-            View t0 = make_view16(rt.scratch, B, x.f.H / 2, x.f.W / 2, w.cin);
+            View t0 = make_view16(tape && tape->ops ? rt.persist : rt.scratch, B, x.f.H / 2, x.f.W / 2, w.cin);
+            if (tape && tape->ops) tape->res[&w].t0 = t0;
             xpool = make_view(rt.scratch, B, x.f.H / 2, x.f.W / 2, w.cin);       // AvgPool2d(2) of the skip path, written by the same pass
             run_norm(rt, x.f, w.norm0, 32, nullptr, nullptr, 0, act, 1, nullptr, t0, nullptr, &xpool);
             run_conv_tc(rt, w.conv0, t0, nullptr, h0);
@@ -824,8 +875,8 @@ struct UNetFused {
         Tens qkv = make_act(tape ? rt.persist : rt.scratch, rt, x.f.N, x.f.H, x.f.W, 3 * x.f.C, true, false, false);
         const ConvNormIn n = norm_in(x.f, w.norm, 32, ACT_NONE);
         run_conv_tc(rt, w.qkv, x.h, &n, qkv);
-        if (tape) tape->attn[&w] = {op_view(x), qkv.f};
-        View a = make_view(rt.scratch, x.f.N, x.f.H, x.f.W, x.f.C);
+        View a = make_view(tape && tape->ops ? rt.persist : rt.scratch, x.f.N, x.f.H, x.f.W, x.f.C);
+        if (tape) tape->attn[&w] = {op_view(x), qkv.f, View{}, tape->ops ? a : View{}};
         attention_forward(qkv.f, 8, a, rt.stream, true);
         run_conv_tc(rt, w.proj, a, nullptr, out, &x.f, RES_SAME);
     }
@@ -866,6 +917,7 @@ void UNetNet::forward_fused(Runtime& rt, const ImgView& image, const float* coar
         x0 = make_view(P, B, S_, S_, 4);
         nchw_to_nhwc(image, x0, s);
     }
+    if (tape) tape->x0 = x0;
 
     // ---- plan the skip concatenations: up res-block j reads cat(h_j, hs[2L-1-j]) from one buffer (both precisions) ----
     const int NH = 2 * L_;

@@ -126,16 +126,24 @@ struct ResBlockW {
     ConvWeights fold;           // default mode: conv1 with the skip folded into its K (fold.cin2 > 0; conv_make_fold), else empty
     bool has_skip = false;
     float* film0 = nullptr;     // [2*cout], constant (t = 0 time embedding, unet.py:365-376)
-    int film1_off = 0;          // offset of this block's 2*cout FiLM vector in the batched pose projection
+    int film1_off = 0;          // offset of this block's 2*cout FiLM vector in the batched pose projection (and of its
+                                // cond0 rows in the stacked time projection)
+    std::string key;            // state_dict prefix
 };
-struct AttnW { int C = 0; NormW norm; ConvWeights qkv, proj; };
+struct AttnW { int C = 0; NormW norm; ConvWeights qkv, proj; std::string key; };
 
 // The activations the U-Net backward reads from the forward it recomputes, keyed by the block's weights (each block runs
 // once per forward).  Normalised tensors are kept as the normalisation read them (fp32, or the f16 operand copy), with the
 // statistics their producer accumulated.
+// ops (set by the caller): also keep every conv's operand that is not one of those, for the weight gradients -- the
+// normalised conv0 / conv1 / qkv operands the separate normalisation passes write (strict mode; default mode: the pooled
+// conv0 operand of a down-sampling block only, the others are applied inside the consumer conv), the attention output
+// (the proj operand) and the network input.
 struct UNetTape {
-    struct Res { View x, h0; };       // block input (norm0), raw conv0 output (norm1)
-    struct Attn { View x, qkv; };     // block input (norm), qkv projection (fp32)
+    struct Res { View x, h0, t0, h2; };   // block input (norm0), raw conv0 output (norm1); ops: conv0's / conv1's operand
+    struct Attn { View x, qkv, t, a; };   // block input (norm), qkv projection (fp32); ops: qkv's operand, attention output
+    bool ops = false;
+    View x0;                          // ops: the first conv's input (NHWC)
     std::map<const ResBlockW*, Res> res;
     std::map<const AttnW*, Attn> attn;
     const float* c1 = nullptr;        // pose MLP pre-activations [N][256] (unet.py:449-452): cond_embed.0 output
@@ -154,6 +162,10 @@ struct UNetGrads {
     int d_pose_ld = 0;
     float* d_coarse_posed = nullptr;
     float* d_coarse_grid = nullptr;
+    // parameter gradients (the body morpher): a flat fp32 buffer of param_count() floats in state_dict order
+    // (UNetNet::param_offset); accumulate_params: add to what it holds (the second and later micro-batch chunks)
+    float* d_params = nullptr;
+    int accumulate_params = 0;
 };
 
 // Frames per pass of the upscaler backward.  Its taped forward and gradient buffers at 512x512 take 2610 MiB of the context's
@@ -177,8 +189,14 @@ public:
                   const float* pose, int pose_ld, const UNetGrads& g);
     int size() const { return S_; }
     bool loaded() const { return loaded_; }
+    // floats of the network's parameters (the body morpher's state_dict; 0 for the upscaler, which has no parameter
+    // gradients), and the offset of a state_dict key's tensor in the flat state_dict-order buffer
+    long param_count() const { return param_total_; }
+    long param_offset(const std::string& key) const;
 private:
     AllocSink owned_;          // every device allocation made by load()
+    std::map<std::string, long> param_off_;     // state_dict key -> offset in the flat parameter buffer
+    long param_total_ = 0;
     void forward_fused(Runtime& rt, const ImgView& image, const float* coarse_posed, const float* coarse_grid, int coarse_size,
                        const float* pose, int pose_ld, float* const* outputs, UNetTape* tape);
     void res_block(Runtime& rt, const ResBlockW& w, const View& x, int mode, const float* film1, const View& out, UNetTape* tape);
@@ -203,6 +221,9 @@ private:
     float *cond_w0_ = nullptr, *cond_b0_ = nullptr, *cond_w2_ = nullptr, *cond_b2_ = nullptr;
     float *film1_w_ = nullptr, *film1_b_ = nullptr;
     int film1_total_ = 0;
+    // the t = 0 time embedding's intermediates and weights its parameter gradients need (the body morpher): t0 [mc], t1 =
+    // time_embed.1(t0), t2 = time_embed.3(SiLU(t1)) [256], time_embed.3's weight, the cond0 projections stacked like film1_w_
+    float *time_t0_ = nullptr, *time_t1_ = nullptr, *time_t2_ = nullptr, *time_w3_ = nullptr, *film0_w_ = nullptr;
     NormW last_n_;
     TailWeights tail_;
 };

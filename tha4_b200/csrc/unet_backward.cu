@@ -17,7 +17,15 @@
 //   pose:      d(film1) through the FiLM projection, cond_embed.2 and cond_embed.0 (fixed-order fp64 GEMVs);
 //   upscaler:  the fused 16-channel first conv's data gradient goes through the prologue's adjoint (image_ops.cu): identity
 //              and warp terms to the rest image (which the tail warps too), the posed / grid terms through the bilinear x2.
+// Parameter gradients (the body morpher), into a flat state_dict-order buffer:
+//   conv weights: the weight-gradient convolution (conv_wgrad.cu) of each conv's taped operand, rebuilt as the forward
+//              multiplied it, against the dz its data gradient already reads; the default mode's folded conv1 + skip is two
+//              convs (conv1 on the normalised h0, skip on the raw x);
+//   conv biases: fixed-order fp64 pixel sums of the same dz;
+//   GroupNorm weights / biases and the time FiLM: from the norm backward's per-(n, c) sums (gn_param_fold_kernel);
+//   pose and time MLPs: d(film1) / d(film0) against the layer inputs (linear_wgrad_kernel), then back through the MLPs.
 #include "nets.cuh"
+#include "conv_wgrad.cuh"
 
 namespace tha4 {
 
@@ -390,6 +398,83 @@ __global__ void __launch_bounds__(256) linear_bwd_kernel(const float* __restrict
     }
 }
 
+// ------------------------------------------------------------------------------------------------ parameter gradients
+// dW[r][k] (+)= sum_n dy[n][r] u(x[n][k]), db[r] (+)= sum_n dy[n][r], n in order (fp64), u = SiLU (as linear_kernel applies
+// it to the layer's input) or the identity.  One thread per weight; the bias by the threads of column k = 0.
+__global__ void __launch_bounds__(256) linear_wgrad_kernel(const float* __restrict__ dy, int dy_ld, int N, int R, const float* __restrict__ x,
+                                                           int x_ld, int K, int silu_x, float* __restrict__ dW, float* __restrict__ db,
+                                                           int accumulate) {
+    const long total = (long)R * K;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+        const int r = (int)(i / K), k = (int)(i - (long)r * K);
+        double w = 0.0, b = 0.0;
+        for (int n = 0; n < N; ++n) {
+            const double g = dy[(long)n * dy_ld + r];
+            float v = x[(long)n * x_ld + k];
+            if (silu_x) v = v / (1.0f + expf(-v));
+            w += g * (double)v;
+            b += g;
+        }
+        dW[i] = accumulate ? dW[i] + (float)w : (float)w;
+        if (k == 0) db[r] = accumulate ? db[r] + (float)b : (float)b;
+    }
+}
+
+// GroupNorm (+FiLM) parameters from the backward reduction's per-(n, c) sums S1 = sum dz, S2 = sum dz xhat (dz: the
+// gradient at the affine's output, before the activation), with the forward's y = ((gamma xhat + beta)(1 + s0) + b0)(1 + s1)
+// + b1 and M = (1 + s0)(1 + s1), as gn_bwd_finalize_kernel forms d(s1), d(b1):
+//   d gamma = sum_n M S2,  d beta = sum_n M S1,  d s0 = sum_n (1 + s1)(gamma S2 + beta S1),  d b0 = sum_n (1 + s1) S1
+// (n in order, fp64).  d(film0) goes to dfilm0[c] / dfilm0[C + c] (written, not accumulated: one per backward pass).
+__global__ void gn_param_fold_kernel(const double* __restrict__ sums, int N, int C, const float* __restrict__ gamma,
+                                     const float* __restrict__ beta, const float* __restrict__ film0, const float* __restrict__ film1,
+                                     int film1_ld, float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ dfilm0,
+                                     int accumulate) {
+    for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < C; c += gridDim.x * blockDim.x) {
+        const double s0 = film0 ? 1.0 + (double)film0[c] : 1.0;
+        double g = 0.0, b = 0.0, ds0 = 0.0, db0 = 0.0;
+        for (int n = 0; n < N; ++n) {
+            const double S1 = sums[((long)n * C + c) * 2], S2 = sums[((long)n * C + c) * 2 + 1];
+            const double s1 = film1 ? 1.0 + (double)film1[(long)n * film1_ld + c] : 1.0;
+            g += s0 * s1 * S2;
+            b += s0 * s1 * S1;
+            ds0 += s1 * ((double)gamma[c] * S2 + (double)beta[c] * S1);
+            db0 += s1 * S1;
+        }
+        dgamma[c] = accumulate ? dgamma[c] + (float)g : (float)g;
+        dbeta[c] = accumulate ? dbeta[c] + (float)b : (float)b;
+        if (dfilm0) { dfilm0[c] = (float)ds0; dfilm0[C + c] = (float)db0; }
+    }
+}
+
+// per-channel sums of an NHWC tensor over its pixels (conv bias gradients), fixed order: stage 1 sums pixel chunk
+// blockIdx.y of 32 channels (8 pixel slices of 32 lanes, fp64, the slices added in order), stage 2 adds the chunks in order
+constexpr int CS_CHUNK = 4096;
+__global__ void __launch_bounds__(256) channel_sum_partial_kernel(const float* __restrict__ x, int ld, long pixels, int C,
+                                                                  double* __restrict__ part) {
+    __shared__ double red[8][32];
+    const int lane = threadIdx.x & 31, sl = threadIdx.x >> 5, c = blockIdx.x * 32 + lane;
+    const long p0 = (long)blockIdx.y * CS_CHUNK, p1 = min(pixels, p0 + CS_CHUNK);
+    double acc = 0.0;
+    if (c < C)
+        for (long p = p0 + sl; p < p1; p += 8) acc += (double)x[p * ld + c];
+    red[sl][lane] = acc;
+    __syncthreads();
+    if (sl == 0 && c < C) {
+        double t = 0.0;
+        for (int j = 0; j < 8; ++j) t += red[j][lane];
+        part[(long)blockIdx.y * C + c] = t;
+    }
+}
+__global__ void channel_sum_finish_kernel(const double* __restrict__ part, int chunks, int C, float* __restrict__ out,
+                                          float* __restrict__ out2, int accumulate) {
+    for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < C; c += gridDim.x * blockDim.x) {
+        double t = 0.0;
+        for (int z = 0; z < chunks; ++z) t += part[(long)z * C + c];
+        out[c] = accumulate ? out[c] + (float)t : (float)t;
+        if (out2) out2[c] = accumulate ? out2[c] + (float)t : (float)t;
+    }
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------ entry points
@@ -516,7 +601,9 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
     const bool want_img = g.d_image != nullptr, want_pose = g.d_pose != nullptr;
     const bool want_coarse = g.d_coarse_posed || g.d_coarse_grid;
     const bool want_x0 = want_img || want_coarse;          // gradients that need the first conv's data gradient
-    THA4_REQUIRE(want_x0 || want_pose, "unet backward: no gradient requested");
+    const bool want_par = g.d_params != nullptr;
+    THA4_REQUIRE(want_x0 || want_pose || want_par, "unet backward: no gradient requested");
+    THA4_REQUIRE(!want_par || (!upscaler_ && param_total_ > 0), "unet backward: parameter gradients are the body morpher's");
     if (!adj_ready_) pack_adjoints(rt);
     const int B = image.N, S = S_, NH = 2 * L_;
     cudaStream_t s = rt.stream;
@@ -527,25 +614,85 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
     float* outs[5];
     for (int k = 0; k < 5; ++k) outs[k] = P->alloc((size_t)B * kCh[k] * S * S);
     UNetTape tape;
+    tape.ops = want_par;
     forward(rt, image, coarse_posed, coarse_grid, coarse_size, pose, pose_ld, outs, &tape);
     float* dfilm = P->alloc((size_t)B * film1_total_);
+    float* dfilm0 = want_par ? P->alloc((size_t)film1_total_) : nullptr;     // sum over the batch of d(film0), film1's layout
+    const int acc = g.accumulate_params;
+    auto par = [&](const std::string& key) { return g.d_params + param_offset(key); };
 
+    // key: the state_dict prefix of the normalisation (parameter gradients), or empty
     auto gn = [&](const View& x, const NormW& nw, const float* film0, const float* film1, int act, const View& dy, int dy_pool,
-                  const View& dx, const View* res, int res_mode, const View* add) {
+                  const View& dx, const View* res, int res_mode, const View* add, const std::string& key) {
         THA4_REQUIRE(nw.C == x.C, "norm backward: channel mismatch");
+        double* sums = rt.alloc_stats((size_t)B * x.C * 2);
         group_norm_backward(x, 32, nw.gamma, nw.beta, film0, film1, film1_total_, act, dy, dy_pool, dx,
                             film1 ? dfilm + (film1 - tape.film1) : nullptr, film1_total_, res, res_mode, add,
-                            rt.alloc_stats((size_t)B * x.C * 2), rt.scratch->alloc((size_t)B * x.C * 8), s);
+                            sums, rt.scratch->alloc((size_t)B * x.C * 8), s);
+        if (want_par) {
+            gn_param_fold_kernel<<<ceil_div(x.C, 256), 256, 0, s>>>(sums, B, x.C, nw.gamma, nw.beta, film0, film1, film1_total_,
+                                                                    par(key + ".weight"), par(key + ".bias"),
+                                                                    film0 ? dfilm0 + (film1 - tape.film1) : nullptr, acc);
+            THA4_LAUNCH_CHECK();
+        }
+    };
+    // ---- parameter-gradient helpers ----
+    const auto ws_alloc = [&](size_t n) { return rt.scratch->alloc(n); };
+    auto operand = [&](const View& v) {
+        WgradOperand o;
+        o.p = v.p; o.f16 = v.f16; o.ld = v.ld; o.N = v.N; o.H = v.H; o.W = v.W; o.C = v.C;
+        return o;
+    };
+    // an f16 raw tensor with the pending GroupNorm (+FiLM) + act its consumer conv applied, coefficients from the forward's builder
+    auto pending = [&](const View& raw, const NormW& nw, int act, const float* film0, const float* film1) {
+        WgradOperand o = operand(raw);
+        float2* coef = reinterpret_cast<float2*>(P->alloc((size_t)B * nw.C * 2));
+        wgrad_xf_coef(raw, nw.gamma, nw.beta, nw.C, act, coef, s, 32, film0, film1, film1_total_);
+        o.xf = WG_XF_HALF; o.act = act; o.coef = coef; o.coef_C = nw.C;
+        return o;
+    };
+    auto wgrad = [&](const std::string& key, ConvKind kind, const WgradOperand& x, const View& dz) {
+        WgradArgs a;
+        a.accumulate = acc; a.out = par(key + ".weight");
+        conv_wgrad_layer(kind, x, operand(dz), a, rt.strict, 0, ws_alloc, s);
+    };
+    auto bias = [&](const View& dz, const std::string& key, const std::string& key2 = std::string()) {
+        const long pixels = (long)dz.N * dz.H * dz.W;
+        const int chunks = ceil_div(pixels, CS_CHUNK);
+        double* part = reinterpret_cast<double*>(rt.scratch->alloc((size_t)chunks * dz.C * 2));
+        channel_sum_partial_kernel<<<dim3(ceil_div(dz.C, 32), chunks), 256, 0, s>>>(dz.p, dz.ld, pixels, dz.C, part);
+        THA4_LAUNCH_CHECK();
+        channel_sum_finish_kernel<<<ceil_div(dz.C, 256), 256, 0, s>>>(part, chunks, dz.C, par(key + ".bias"),
+                                                                      key2.empty() ? nullptr : par(key2 + ".bias"), acc);
+        THA4_LAUNCH_CHECK();
+    };
+    auto linear_wgrad = [&](const float* dy, int dy_ld, int N, int R, const float* x, int x_ld, int K, int silu_x, const std::string& key) {
+        linear_wgrad_kernel<<<grid_for((long)R * K), 256, 0, s>>>(dy, dy_ld, N, R, x, x_ld, K, silu_x, par(key + ".weight"),
+                                                                  par(key + ".bias"), acc);
+        THA4_LAUNCH_CHECK();
     };
     // ResBlock: out = conv1(SiLU(FiLM(GN(h0)))) + skip(resample(x)),  h0 = conv0(resample(SiLU(GN(x)))).  Returns the gradient of x
     // (+ extra); with input_grad false it stops once the block's d(film1) is written.
     auto res_bwd = [&](const ResBlockW& w, int mode, const View& dout, const View* extra, bool input_grad) -> View {
         const UNetTape::Res& t = tape.res.at(&w);
         const ResAdj& A = adj_res_.at(&w);
+        const float* f1 = tape.film1 + w.film1_off;
         View du = fresh(P, B, dout.H, dout.W, w.cout);
         run_dgrad(rt, A.conv1, dout, du);
         View dh0 = fresh(P, B, t.h0.H, t.h0.W, w.cout);
-        gn(t.h0, w.norm1, w.film0, tape.film1 + w.film1_off, ACT_SILU, du, 0, dh0, nullptr, RES_NONE, nullptr);
+        gn(t.h0, w.norm1, w.film0, f1, ACT_SILU, du, 0, dh0, nullptr, RES_NONE, nullptr, w.key + ".norm1");
+        if (want_par) {
+            // conv1 (and the skip, which the default mode folds into conv1's launch) against dout; conv0 against dh0.  The
+            // operands: strict mode the normalised tensors the passes wrote; default mode the raw f16 tensors with the
+            // normalisation the consumer conv applied (a down-sampling block's pooled operand comes from a pass)
+            const WgradOperand x1 = rt.f16 ? pending(t.h0, w.norm1, ACT_SILU_FAST, w.film0, f1) : operand(t.h2);
+            wgrad(w.key + ".conv1", CONV_3x3, x1, dout);
+            if (w.has_skip) wgrad(w.key + ".skip", CONV_1x1, operand(t.x), dout);
+            bias(dout, w.key + ".conv1", w.has_skip ? w.key + ".skip" : std::string());
+            const WgradOperand x0 = (rt.f16 && mode != 2) ? pending(t.x, w.norm0, ACT_SILU_FAST, nullptr, nullptr) : operand(t.t0);
+            wgrad(w.key + ".conv0", mode == 1 ? CONV_UP2_3x3 : CONV_3x3, x0, dh0);
+            bias(dh0, w.key + ".conv0");
+        }
         if (!input_grad) return View{};
         const int th = mode == 2 ? t.x.H / 2 : t.x.H;
         View dt = fresh(P, B, th, th, w.cin);
@@ -554,9 +701,10 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
         if (w.has_skip) {
             View dsk = fresh(P, B, t.x.H, t.x.W, w.cin);
             run_dgrad(rt, A.skip, dout, dsk, extra);
-            gn(t.x, w.norm0, nullptr, nullptr, ACT_SILU, dt, 0, dx, &dsk, RES_SAME, nullptr);
+            gn(t.x, w.norm0, nullptr, nullptr, ACT_SILU, dt, 0, dx, &dsk, RES_SAME, nullptr, w.key + ".norm0");
         } else {
-            gn(t.x, w.norm0, nullptr, nullptr, ACT_SILU, dt, mode == 2, dx, &dout, mode == 0 ? RES_SAME : (mode == 1 ? RES_UP2 : RES_DOWN2), extra);
+            gn(t.x, w.norm0, nullptr, nullptr, ACT_SILU, dt, mode == 2, dx, &dout, mode == 0 ? RES_SAME : (mode == 1 ? RES_UP2 : RES_DOWN2), extra,
+               w.key + ".norm0");
         }
         return dx;
     };
@@ -568,10 +716,16 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
         run_dgrad(rt, A.proj, dout, da);
         View dqkv = fresh(P, B, dout.H, dout.W, 3 * w.C);
         attention_backward(t.qkv, da, 8, dqkv, rt.scratch->alloc((size_t)B * 8 * 256 * 4), s);
+        if (want_par) {
+            wgrad(w.key + ".conv", CONV_1x1, operand(t.a), dout);
+            bias(dout, w.key + ".conv");
+            wgrad(w.key + ".qkv", CONV_1x1, rt.f16 ? pending(t.x, w.norm, ACT_NONE, nullptr, nullptr) : operand(t.t), dqkv);
+            bias(dqkv, w.key + ".qkv");
+        }
         View dn = fresh(P, B, dout.H, dout.W, w.C);
         run_dgrad(rt, A.qkv, dqkv, dn);
         View dx = fresh(P, B, dout.H, dout.W, w.C);
-        gn(t.x, w.norm, nullptr, nullptr, ACT_NONE, dn, 0, dx, &dout, RES_SAME, nullptr);
+        gn(t.x, w.norm, nullptr, nullptr, ACT_NONE, dn, 0, dx, &dout, RES_SAME, nullptr, w.key + ".norm");
         return dx;
     };
 
@@ -585,8 +739,22 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
     tail_backward(TAIL_UNET, outs, g.grad_outputs, image, ImgView{}, dh, want_img ? dimg.p : nullptr, nullptr, 4, s);
     View df = fresh(P, B, S, S, mc_);
     run_dgrad(rt, adj_head_, dh, df);
+    const std::string p = "body.";
+    if (want_par) {
+        // last.2: the 7 head channels of dh in N; its operand SiLU(GroupNorm(feat)) as the tail applied it -- the wgmma tail
+        // (default mode): fp32 affine, tanh.approx.f32 SiLU, rounded to f16; the strict tail: fp32 affine, SiLU
+        const View& f = tape.feat;
+        float* coef = P->alloc((size_t)B * f.C * 2);
+        norm_finalize(f, 32, last_n_.gamma, last_n_.beta, nullptr, nullptr, 0, coef, s);
+        WgradOperand x = operand(f);
+        x.xf = f.f16 ? WG_XF_FLOAT16 : WG_XF_FLOAT; x.act = f.f16 ? ACT_SILU_FAST : ACT_SILU;
+        x.coef = reinterpret_cast<const float2*>(coef); x.coef_C = f.C;
+        View dh7 = dh; dh7.C = 7;
+        wgrad(p + "last.2", CONV_3x3, x, dh7);
+        bias(dh7, p + "last.2");
+    }
     View dfeat = fresh(P, B, S, S, mc_);
-    gn(tape.feat, last_n_, nullptr, nullptr, ACT_SILU, df, 0, dfeat, nullptr, RES_NONE, nullptr);
+    gn(tape.feat, last_n_, nullptr, nullptr, ACT_SILU, df, 0, dfeat, nullptr, RES_NONE, nullptr, p + "last.0");
 
     // ---- up path in reverse: dcat[j] = gradient of up ResBlock j's input cat(h_j, hs[NH-1-j]) ----
     std::vector<int> ch_h(NH);
@@ -620,10 +788,14 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
     for (int i = L_ - 1; i >= 0; --i) {
         const View d_blk = (i == L_ - 1) ? attn_bwd(down_attn_, gk) : gk;
         const View e_in = dhs(2 * i);
-        const View g_in = res_bwd(down_res_[i], 0, d_blk, &e_in, i > 0 || want_x0);
+        const View g_in = res_bwd(down_res_[i], 0, d_blk, &e_in, i > 0 || want_x0 || want_par);
         if (i == 0) { gk = g_in; break; }
         const View e_ds = dhs(2 * i - 1);
         gk = res_bwd(down_ds_[i - 1], 2, g_in, &e_ds, true);
+    }
+    if (want_par) {                  // first conv (the body morpher's: 4 input channels)
+        wgrad(p + "first_conv", CONV_3x3, operand(tape.x0), gk);
+        bias(gk, p + "first_conv");
     }
     if (want_x0 && !upscaler_) {     // first conv: its data gradient joins the warp's image term in the epilogue
         View dx0 = fresh(P, B, S, S, 4);
@@ -636,12 +808,30 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
                                    g.d_coarse_grid, s);
         if (want_img) nhwc_to_nchw(dimg, g.d_image, s);
     }
-    if (want_pose) {    // d(film1) -> FiLM projection (SiLU' at c2) -> cond_embed.2 (SiLU' at c1) -> cond_embed.0
+    if (want_pose || want_par) {    // d(film1) -> FiLM projection (SiLU' at c2) -> cond_embed.2 (SiLU' at c1) -> cond_embed.0
         float* dc2 = P->alloc((size_t)B * 256);
         float* dc1 = P->alloc((size_t)B * 256);
         linear_backward(dfilm, film1_total_, B, film1_total_, film1_w_, 256, tape.c2, 256, dc2, 256, s);
         linear_backward(dc2, 256, B, 256, cond_w2_, 256, tape.c1, 256, dc1, 256, s);
-        linear_backward(dc1, 256, B, 256, cond_w0_, 6, nullptr, 0, g.d_pose, g.d_pose_ld, s);
+        if (want_pose) linear_backward(dc1, 256, B, 256, cond_w0_, 6, nullptr, 0, g.d_pose, g.d_pose_ld, s);
+        if (want_par) {
+            for (const auto* blocks : {&down_res_, &down_ds_, &mid_res_, &up_res_, &up_us_})
+                for (const ResBlockW& w : *blocks)
+                    linear_wgrad(dfilm + w.film1_off, film1_total_, B, 2 * w.cout, tape.c2, 256, 256, 1, w.key + ".cond1_layers.1");
+            linear_wgrad(dc2, 256, B, 256, tape.c1, 256, 256, 1, p + "cond_embed.2");
+            linear_wgrad(dc1, 256, B, 256, pose, pose_ld, 6, 0, p + "cond_embed.0");
+        }
+    }
+    if (want_par) {     // the time FiLM at t = 0: sum_n d(film0) -> cond0 projections (SiLU' at t2) -> time_embed.3 (SiLU' at t1) -> time_embed.1
+        float* dt2 = P->alloc(256);
+        float* dt1 = P->alloc(256);
+        for (const auto* blocks : {&down_res_, &down_ds_, &mid_res_, &up_res_, &up_us_})
+            for (const ResBlockW& w : *blocks)
+                linear_wgrad(dfilm0 + w.film1_off, film1_total_, 1, 2 * w.cout, time_t2_, 256, 256, 1, w.key + ".cond0_layers.1");
+        linear_backward(dfilm0, film1_total_, 1, film1_total_, film0_w_, 256, time_t2_, 256, dt2, 256, s);
+        linear_wgrad(dt2, 256, 1, 256, time_t1_, 256, 256, 1, p + "time_embed.3");
+        linear_backward(dt2, 256, 1, 256, time_w3_, 256, time_t1_, 256, dt1, 256, s);
+        linear_wgrad(dt1, 256, 1, 256, time_t0_, mc_, mc_, 0, p + "time_embed.1");
     }
 }
 

@@ -5,12 +5,12 @@ morpher_00.py:42-66, upscaler_02.py:59-96).  This is what pose fitting on an arb
 image -> pose regressor with a teacher as a differentiable renderer, needs.
 
 Dispatch: the autograd path runs when grad mode is on and an input (image, layer or pose) requires grad, or -- for the three
-encoder-decoder networks -- when the module was made trainable (`module.trainable_(True)`) and any of its parameters requires
-grad; in every other case the forward is the plain inference call.  Trainability is an explicit opt-in, not the students'
+encoder-decoder networks and the body morpher -- when the module was made trainable (`module.trainable_(True)`) and any of its
+parameters requires grad; in every other case the forward is the plain inference call.  Trainability is an explicit opt-in, not the students'
 "any parameter requires grad" rule, because a freshly built teacher's parameters require grad (as every nn.Module's do) and
-its inference calls must stay plain calls without a graph.  A trainable encoder-decoder module's backward returns the
-gradients of the parameters that require grad (flat d_params from the same library call as the input gradients); the
-U-Nets' parameters never receive gradients.
+its inference calls must stay plain calls without a graph.  A trainable module's backward returns the gradients of the
+parameters that require grad (flat d_params from the same library call as the input gradients); only the upscaler's
+parameters never receive gradients.
 
 Forward: the inference call; the outputs are bit-identical to the no-grad path (each in its own allocation, so in-place ops
 on them work).  Inputs and parameters are saved, so an in-place write to either between forward and backward raises torch's
@@ -26,8 +26,8 @@ from tha4_b200.nn.common.native_module import contiguous_grads, refuse_double_ba
 
 
 class Trainable:
-    """Opt-in parameter gradients of the encoder-decoder teacher modules (mixed into EyebrowDecomposer00,
-    EyebrowMorphingCombiner00, FaceMorpher08)."""
+    """Opt-in parameter gradients of the teacher modules (mixed into EyebrowDecomposer00, EyebrowMorphingCombiner00,
+    FaceMorpher08, Morpher00)."""
     _trainable = False
 
     def trainable_(self, mode: bool = True):
@@ -190,12 +190,18 @@ def _morpher_backward(ctx, *grad_outputs):
     image, pose, *params = ctx.saved_tensors
     none = (None,) * len(params)
     want_image, want_pose = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
-    if not (want_image or want_pose) or all(g is None for g in grad_outputs):
+    if not any(ctx.needs_input_grad[1:]) or all(g is None for g in grad_outputs):
+        return (None, None, None) + none
+    ctx.lib = ctx.module.sync_weights()
+    flat, dp = _param_grads(ctx, 3, image.device)
+    if flat is None and not (want_image or want_pose):
         return (None, None, None) + none
     d_image = _empty_like(image) if want_image else None
     d_pose = _empty_like(pose) if want_pose else None
-    ctx.module.sync_weights().morpher_backward(image, pose, contiguous_grads(grad_outputs), d_image=d_image, d_pose=d_pose)
-    return (None, d_image, d_pose) + none
+    # d_params only from a trainable module: the plain one keeps the input-gradient call it always made
+    extra = {'d_params': flat} if ctx.module.is_trainable() else {}
+    ctx.lib.morpher_backward(image, pose, contiguous_grads(grad_outputs), d_image=d_image, d_pose=d_pose, **extra)
+    return (None, d_image, d_pose) + dp
 
 
 class _UpscalerFunction(torch.autograd.Function):

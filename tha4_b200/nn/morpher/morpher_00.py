@@ -6,11 +6,11 @@ import torch
 from torch import Tensor
 
 from tha4_b200.nn.common import encdec_autograd
-from tha4_b200.nn.common.native_module import NativeModule, wants_autograd
+from tha4_b200.nn.common.native_module import NativeModule
 from tha4_b200.nn.state_dict_spec import body_morpher_spec
 
 
-class Morpher00(NativeModule):
+class Morpher00(encdec_autograd.Trainable, NativeModule):
     NET_NAME = 'body_morpher'
 
     def __init__(self, args=None):
@@ -20,7 +20,7 @@ class Morpher00(NativeModule):
     def forward(self, image: torch.Tensor, pose: torch.Tensor) -> List[Tensor]:
         assert len(image.shape) == 4 and image.shape[1:] == (4, 256, 256)     # morpher_00.py:43-49
         assert len(pose.shape) == 2 and image.shape[0] == pose.shape[0] and pose.shape[1] == 6
-        if wants_autograd(image, pose):
+        if self.wants_autograd(image, pose):
             return encdec_autograd.morpher(self, image, pose)
         return self.sync_weights().morpher(image, pose)
 

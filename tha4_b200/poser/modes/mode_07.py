@@ -12,6 +12,7 @@ from typing import Dict, List, Optional
 import torch
 from torch import Tensor
 
+from tha4_b200.nn.common.encdec_autograd import Trainable
 from tha4_b200.nn.eyebrow_decomposer.eyebrow_decomposer_00 import EyebrowDecomposer00
 from tha4_b200.nn.eyebrow_morphing_combiner.eyebrow_morphing_combiner_00 import EyebrowMorphingCombiner00
 from tha4_b200.nn.face_morpher.face_morpher_08 import FaceMorpher08
@@ -106,10 +107,12 @@ class FiveStepPoserComputationProtocol(CachedComputationProtocol):
 
     @staticmethod
     def _trains_teacher(state: ComputationState) -> bool:
-        """An encoder-decoder module of the poser was made trainable (trainable_(True)) and has parameters that require grad."""
+        """A teacher module of the poser (an encoder-decoder or the body morpher) was made trainable (trainable_(True)) and has
+        parameters that require grad."""
         return any(state.modules[net.name].wants_autograd()
-                   for net in (Network.eyebrow_decomposer, Network.eyebrow_morphing_combiner, Network.face_morpher)
-                   if net.name in state.modules)
+                   for net in (Network.eyebrow_decomposer, Network.eyebrow_morphing_combiner, Network.face_morpher,
+                               Network.body_morpher)
+                   if isinstance(state.modules.get(net.name), Trainable))
 
     def _differentiable(self, state: ComputationState) -> List[Tensor]:
         """The modules composed as in the reference (mode_07.py:72-132; mode_12.py:66-94 for the face part), each through its
