@@ -114,8 +114,8 @@ int tha4_eyebrow_morphing_combiner_backward(tha4_ctx* ctx, const float* backgrou
                                             void* stream);
 int tha4_face_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, int pose_ld, int B,
                                const float* const* grad_outputs, float* d_image, float* d_pose, float* d_params, void* stream);
-/* Floats of the parameters of THA4_NET_EYEBROW_DECOMPOSER / _EYEBROW_MORPHING_COMBINER / _FACE_MORPHER / _BODY_MORPHER (the
- * length of the d_params of their backward entries); -1 for any other network. */
+/* Floats of the parameters of THA4_NET_EYEBROW_DECOMPOSER / _EYEBROW_MORPHING_COMBINER / _FACE_MORPHER / _BODY_MORPHER /
+ * _UPSCALER (the length of the d_params of their backward entries); -1 for any other network. */
 int64_t tha4_net_param_count(int net);
 /* Morpher00.forward (src/tha4/nn/morpher/morpher_00.py:42-66): image [B,4,256,256], pose [B,6] ->
  * merged(4) alpha(1) warped(4) grid_change(2) direct(4) */
@@ -140,11 +140,16 @@ int tha4_upscaler_forward(tha4_ctx* ctx, const float* rest_image, const float* c
  * 5 outputs (grad_outputs in the forward's output order, NCHW, an entry may be NULL = zero), with the rules of
  * tha4_morpher_backward: d_rest_image [B,4,512,512], d_coarse_posed_image [B,4,S,S], d_coarse_grid_change [B,2,S,S] (S =
  * coarse_size; at 256 through the adjoint of the fused bilinear x2) and d_pose [B,6] (contiguous) are optional (NULL = not
- * computed), at least one non-NULL, each overwritten.  Any B >= 1, in passes of at most min(microbatch, 6) frames (the
- * backward's workspace is about 2.6 GiB per frame at 512x512).  The adjoint weights are packed by the first call. */
+ * computed), at least one non-NULL, each overwritten.  d_params: the parameter gradients, as for the encoder-decoder entries
+ * (35 015 655 floats, state_dict order: the U-Net's tensors, then coarse_image_conv's; the t = 0 time embedding and its FiLM
+ * projections included); NULL = not computed, counts as an output.  Any B >= 1, in passes of at most min(microbatch, 6)
+ * frames (the backward's workspace is about 2.6 GiB per frame at 512x512), with d_params of at most min(microbatch, 4)
+ * (the backward then also keeps every conv's operand: about 3.3 GiB per frame in strict mode).  The adjoint weights are
+ * packed by the first call. */
 int tha4_upscaler_backward(tha4_ctx* ctx, const float* rest_image, const float* coarse_posed_image, const float* coarse_grid_change,
                            int coarse_size, const float* pose, int pose_ld, int B, const float* const* grad_outputs,
-                           float* d_rest_image, float* d_coarse_posed_image, float* d_coarse_grid_change, float* d_pose, void* stream);
+                           float* d_rest_image, float* d_coarse_posed_image, float* d_coarse_grid_change, float* d_pose,
+                           float* d_params, void* stream);
 /* SirenFaceMorpher00.forward (src/tha4/nn/siren/face_morpher/siren_face_morpher_00.py:34-51): pose [B,39] -> [B,4,128,128] */
 int tha4_siren_face_morpher_forward(tha4_ctx* ctx, const float* pose, int pose_ld, int B, float* output, void* stream);
 /* SirenMorpher03.forward (src/tha4/nn/siren/morpher/siren_morpher_03.py:107-139): image [B,4,512,512], pose [B,45] ->

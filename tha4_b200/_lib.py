@@ -229,8 +229,8 @@ class Context:
         return gs
 
     def param_count(self, net: str) -> int:
-        """Floats of an encoder-decoder network's or the body morpher's parameters: the length of the flat d_params buffer of
-        its backward."""
+        """Floats of a teacher network's parameters (the three encoder-decoders, the body morpher, the upscaler): the length of
+        the flat d_params buffer of its backward."""
         n = int(self.lib.tha4_net_param_count(NET_IDS[net]))
         if n < 0:
             raise Tha4Error('%s has no parameter gradients' % net)
@@ -336,19 +336,22 @@ class Context:
     def upscaler_backward(self, rest_image: Tensor, coarse_posed: Tensor, coarse_grid: Tensor, pose: Tensor,
                           grad_outputs: Sequence[Optional[Tensor]], d_rest_image: Optional[Tensor] = None,
                           d_coarse_posed: Optional[Tensor] = None, d_coarse_grid: Optional[Tensor] = None,
-                          d_pose: Optional[Tensor] = None):
+                          d_pose: Optional[Tensor] = None, d_params: Optional[Tensor] = None):
         """Input gradients of Upscaler02 into any of d_rest_image [B,4,512,512], d_coarse_posed [B,4,S,S], d_coarse_grid
-        [B,2,S,S] (S = the coarse inputs' size, 256 or 512) and d_pose [B,6] (None = not computed) for the upstream gradients
-        of its five outputs (None = zero); the forward is recomputed in the context's precision mode."""
-        assert d_rest_image is not None or d_coarse_posed is not None or d_coarse_grid is not None or d_pose is not None
+        [B,2,S,S] (S = the coarse inputs' size, 256 or 512) and d_pose [B,6], parameter gradients into d_params (flat,
+        state_dict order) (None = not computed) for the upstream gradients of its five outputs (None = zero); the forward is
+        recomputed in the context's precision mode."""
+        assert any(t is not None for t in (d_rest_image, d_coarse_posed, d_coarse_grid, d_pose, d_params))
         rest_image, coarse_posed, coarse_grid, pose, B, S = self._upscaler_inputs(rest_image, coarse_posed, coarse_grid, pose)
         gs = self._grads(self.UPSCALER_SPECS, grad_outputs, B)
         self._check_out(d_rest_image, (B, 4, 512, 512), 'd_rest_image')
         self._check_out(d_coarse_posed, (B, 4, S, S), 'd_coarse_posed')
         self._check_out(d_coarse_grid, (B, 2, S, S), 'd_coarse_grid')
         self._check_out(d_pose, (B, 6), 'd_pose')
+        self._check_out(d_params, (self.param_count('upscaler'),), 'd_params')
         self._call('tha4_upscaler_backward', _ptr(rest_image), _ptr(coarse_posed), _ptr(coarse_grid), S, _ptr(pose), 6, B,
-                   _ptr_array(gs), _ptr(d_rest_image), _ptr(d_coarse_posed), _ptr(d_coarse_grid), _ptr(d_pose), self._stream())
+                   _ptr_array(gs), _ptr(d_rest_image), _ptr(d_coarse_posed), _ptr(d_coarse_grid), _ptr(d_pose), _ptr(d_params),
+                   self._stream())
 
     def siren_face_morpher(self, pose: Tensor) -> Tensor:
         pose = _check_input(pose, self.device, 'pose')

@@ -360,6 +360,7 @@ int64_t tha4_net_param_count(int net) {
         case THA4_NET_EYEBROW_MORPHING_COMBINER: return 31535878;
         case THA4_NET_FACE_MORPHER: return 31605002;
         case THA4_NET_BODY_MORPHER: return 34682119;
+        case THA4_NET_UPSCALER: return 35015655;
         default: return -1;
     }
 }
@@ -462,21 +463,26 @@ int tha4_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, 
 
 int tha4_upscaler_backward(tha4_ctx* ctx, const float* rest_image, const float* coarse_posed_image, const float* coarse_grid_change,
                            int coarse_size, const float* pose, int pose_ld, int B, const float* const* grad_outputs,
-                           float* d_rest_image, float* d_coarse_posed_image, float* d_coarse_grid_change, float* d_pose, void* stream) {
+                           float* d_rest_image, float* d_coarse_posed_image, float* d_coarse_grid_change, float* d_pose, float* d_params,
+                           void* stream) {
     return guarded(ctx, [&] {
-        THA4_REQUIRE(d_rest_image || d_coarse_posed_image || d_coarse_grid_change || d_pose, "upscaler backward: no gradient requested");
+        THA4_REQUIRE(d_rest_image || d_coarse_posed_image || d_coarse_grid_change || d_pose || d_params,
+                     "upscaler backward: no gradient requested");
+        check_param_layout(d_params ? ctx->upscaler->param_count() : 0, THA4_NET_UPSCALER, d_params);
         THA4_REQUIRE(coarse_size == 256 || coarse_size == 512, "upscaler backward: coarse_size must be 256 or 512");
         THA4_REQUIRE(pose_ld >= 6, "upscaler backward: pose rows need at least 6 entries");
         Runtime rt = make_rt(ctx, stream);
         OutSpec spec[5]; fill_unet_spec(spec, 512);
         const size_t hw = 512 * 512, chw = (size_t)coarse_size * coarse_size;
-        for_chunks(ctx, B, std::min(ctx->opt.microbatch, UPSCALER_BWD_MAX_BATCH), rt.stream, [&](int n0, int b) {
+        const int max_batch = d_params ? UPSCALER_PARAM_BWD_MAX_BATCH : UPSCALER_BWD_MAX_BATCH;
+        for_chunks(ctx, B, std::min(ctx->opt.microbatch, max_batch), rt.stream, [&](int n0, int b) {
             const float* g[5]; offset_grads<5>(grad_outputs, spec, n0, g);
             UNetGrads ug; ug.grad_outputs = g;
             ug.d_image = d_rest_image ? d_rest_image + (size_t)n0 * 4 * hw : nullptr;
             ug.d_coarse_posed = d_coarse_posed_image ? d_coarse_posed_image + (size_t)n0 * 4 * chw : nullptr;
             ug.d_coarse_grid = d_coarse_grid_change ? d_coarse_grid_change + (size_t)n0 * 2 * chw : nullptr;
             ug.d_pose = d_pose ? d_pose + (size_t)n0 * 6 : nullptr; ug.d_pose_ld = 6;
+            ug.d_params = d_params; ug.accumulate_params = n0 > 0;
             ctx->upscaler->backward(rt, make_img(rest_image + (size_t)n0 * 4 * hw, b, 4, 512, 512), coarse_posed_image + (size_t)n0 * 4 * chw,
                                     coarse_grid_change + (size_t)n0 * 2 * chw, coarse_size, pose + (size_t)n0 * pose_ld, pose_ld, ug);
         });

@@ -45,11 +45,6 @@ const TensorRef& sd_get(const StateDict& sd, const std::string& key) {
 }
 
 float* dev_alloc(size_t n) { return reinterpret_cast<float*>(tracked_malloc(std::max<size_t>(n, 1) * sizeof(float))); }   // owned by the loading net
-float* dev_alloc_tmp(size_t n) {       // freed by the caller
-    float* p = nullptr;
-    THA4_CUDA_CHECK(cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(float)));
-    return p;
-}
 
 float* dev_clone(const TensorRef& t, cudaStream_t s) {
     float* p = dev_alloc(t.numel());
@@ -566,11 +561,11 @@ void UNetNet::load(const StateDict& sd, cudaStream_t s) {
     // time embedding at t = 0 is a constant: cat(cos(0)..., sin(0)...) -> Linear -> SiLU -> Linear  (unet.py:365-376,443-447)
     std::vector<float> t0(mc_, 0.0f);
     for (int i = 0; i < mc_ / 2; ++i) t0[i] = 1.0f;
-    // the body morpher keeps them (and time_embed.3's weight) for its parameter gradients
-    float* d_t0 = upscaler_ ? dev_alloc_tmp(mc_) : dev_alloc(mc_);
+    // kept (with time_embed.3's weight) for the parameter gradients
+    float* d_t0 = dev_alloc(mc_);
     THA4_CUDA_CHECK(cudaMemcpyAsync(d_t0, t0.data(), mc_ * sizeof(float), cudaMemcpyHostToDevice, s));
-    float* d_t1 = upscaler_ ? dev_alloc_tmp(256) : dev_alloc(256);
-    float* d_t2 = upscaler_ ? dev_alloc_tmp(256) : dev_alloc(256);
+    float* d_t1 = dev_alloc(256);
+    float* d_t2 = dev_alloc(256);
     linear_forward(d_t0, mc_, 1, mc_, sd_get(sd, p + "time_embed.1.weight").p, sd_get(sd, p + "time_embed.1.bias").p, 256, 0, d_t1, 256, s);
     linear_forward(d_t1, 256, 1, 256, sd_get(sd, p + "time_embed.3.weight").p, sd_get(sd, p + "time_embed.3.bias").p, 256, 1, d_t2, 256, s);
 
@@ -579,14 +574,14 @@ void UNetNet::load(const StateDict& sd, cudaStream_t s) {
     for (auto& e : all_blocks) { e.first->film1_off = film1_total_; film1_total_ += 2 * e.first->cout; }
     film1_w_ = dev_alloc((size_t)film1_total_ * 256);
     film1_b_ = dev_alloc(film1_total_);
-    if (!upscaler_) film0_w_ = dev_alloc((size_t)film1_total_ * 256);
+    film0_w_ = dev_alloc((size_t)film1_total_ * 256);
     for (auto& e : all_blocks) {
         ResBlockW* w = e.first;
         const TensorRef& c0w = sd_get(sd, e.second + ".cond0_layers.1.weight");
         THA4_REQUIRE(c0w.shape[0] == 2 * w->cout && c0w.shape[1] == 256, "cond0 shape: " + e.second);
         w->film0 = dev_alloc(2 * w->cout);
         linear_forward(d_t2, 256, 1, 256, c0w.p, sd_get(sd, e.second + ".cond0_layers.1.bias").p, 2 * w->cout, 1, w->film0, 2 * w->cout, s);
-        if (film0_w_) THA4_CUDA_CHECK(cudaMemcpyAsync(film0_w_ + (size_t)w->film1_off * 256, c0w.p, c0w.numel() * sizeof(float), cudaMemcpyDeviceToDevice, s));
+        THA4_CUDA_CHECK(cudaMemcpyAsync(film0_w_ + (size_t)w->film1_off * 256, c0w.p, c0w.numel() * sizeof(float), cudaMemcpyDeviceToDevice, s));
         const TensorRef& c1w = sd_get(sd, e.second + ".cond1_layers.1.weight");
         THA4_REQUIRE(c1w.shape[0] == 2 * w->cout && c1w.shape[1] == 256, "cond1 shape: " + e.second);
         THA4_CUDA_CHECK(cudaMemcpyAsync(film1_w_ + (size_t)w->film1_off * 256, c1w.p, c1w.numel() * sizeof(float), cudaMemcpyDeviceToDevice, s));
@@ -595,41 +590,39 @@ void UNetNet::load(const StateDict& sd, cudaStream_t s) {
     }
     if (conv_pack_rounding()) tail_make_half(tail_, s);       // default mode: the wgmma tail's f16 head weights
     param_off_.clear(); param_total_ = 0;
-    if (!upscaler_) {
-        time_t0_ = d_t0; time_t1_ = d_t1; time_t2_ = d_t2;
-        time_w3_ = dev_clone(sd_get(sd, p + "time_embed.3.weight"), s);
-        // the flat parameter-gradient layout: the reference's state_dict order (unet.py:438-529, registration order of the
-        // modules; per up level its ResBlocks, then its attention blocks, then the up-sampler)
-        auto reg = [&](const std::string& key) { param_off_[key] = param_total_; param_total_ += sd_get(sd, key).numel(); };
-        auto reg_res = [&](const ResBlockW& w) {
-            for (const char* k : {".norm0.weight", ".norm0.bias", ".conv0.weight", ".conv0.bias", ".cond0_layers.1.weight",
-                                  ".cond0_layers.1.bias", ".norm1.weight", ".norm1.bias", ".conv1.weight", ".conv1.bias",
-                                  ".cond1_layers.1.weight", ".cond1_layers.1.bias"})
-                reg(w.key + k);
-            if (w.has_skip) { reg(w.key + ".skip.weight"); reg(w.key + ".skip.bias"); }
-        };
-        auto reg_attn = [&](const AttnW& a) {
-            for (const char* k : {".norm.weight", ".norm.bias", ".qkv.weight", ".qkv.bias", ".conv.weight", ".conv.bias"}) reg(a.key + k);
-        };
-        for (const char* k : {"time_embed.1.weight", "time_embed.1.bias", "time_embed.3.weight", "time_embed.3.bias", "cond_embed.0.weight",
-                              "cond_embed.0.bias", "cond_embed.2.weight", "cond_embed.2.bias", "first_conv.weight", "first_conv.bias"})
-            reg(p + k);
-        for (int i = 0; i < L_; ++i) {
-            reg_res(down_res_[i]);
-            if (i == L_ - 1) reg_attn(down_attn_);
-            if (i < L_ - 1) reg_res(down_ds_[i]);
-        }
-        for (int j = 0; j < 7; ++j) { if (j % 2 == 0) reg_res(mid_res_[j / 2]); else reg_attn(mid_attn_[j / 2]); }
-        for (int bi = 0; bi < L_; ++bi) {
-            reg_res(up_res_[2 * bi]); reg_res(up_res_[2 * bi + 1]);
-            if (bi == 0) { reg_attn(up_attn_[0]); reg_attn(up_attn_[1]); }
-            if (bi < L_ - 1) reg_res(up_us_[bi]);
-        }
-        for (const char* k : {"last.0.weight", "last.0.bias", "last.2.weight", "last.2.bias"}) reg(p + k);
-        THA4_REQUIRE((long)param_off_.size() == (long)sd.size(), "unet: the state_dict has tensors outside the parameter layout");
+    time_t0_ = d_t0; time_t1_ = d_t1; time_t2_ = d_t2;
+    time_w3_ = dev_clone(sd_get(sd, p + "time_embed.3.weight"), s);
+    // the flat parameter-gradient layout: the reference's state_dict order (unet.py:438-529, registration order of the
+    // modules; per up level its ResBlocks, then its attention blocks, then the up-sampler)
+    auto reg = [&](const std::string& key) { param_off_[key] = param_total_; param_total_ += sd_get(sd, key).numel(); };
+    auto reg_res = [&](const ResBlockW& w) {
+        for (const char* k : {".norm0.weight", ".norm0.bias", ".conv0.weight", ".conv0.bias", ".cond0_layers.1.weight",
+                              ".cond0_layers.1.bias", ".norm1.weight", ".norm1.bias", ".conv1.weight", ".conv1.bias",
+                              ".cond1_layers.1.weight", ".cond1_layers.1.bias"})
+            reg(w.key + k);
+        if (w.has_skip) { reg(w.key + ".skip.weight"); reg(w.key + ".skip.bias"); }
+    };
+    auto reg_attn = [&](const AttnW& a) {
+        for (const char* k : {".norm.weight", ".norm.bias", ".qkv.weight", ".qkv.bias", ".conv.weight", ".conv.bias"}) reg(a.key + k);
+    };
+    for (const char* k : {"time_embed.1.weight", "time_embed.1.bias", "time_embed.3.weight", "time_embed.3.bias", "cond_embed.0.weight",
+                          "cond_embed.0.bias", "cond_embed.2.weight", "cond_embed.2.bias", "first_conv.weight", "first_conv.bias"})
+        reg(p + k);
+    for (int i = 0; i < L_; ++i) {
+        reg_res(down_res_[i]);
+        if (i == L_ - 1) reg_attn(down_attn_);
+        if (i < L_ - 1) reg_res(down_ds_[i]);
     }
+    for (int j = 0; j < 7; ++j) { if (j % 2 == 0) reg_res(mid_res_[j / 2]); else reg_attn(mid_attn_[j / 2]); }
+    for (int bi = 0; bi < L_; ++bi) {
+        reg_res(up_res_[2 * bi]); reg_res(up_res_[2 * bi + 1]);
+        if (bi == 0) { reg_attn(up_attn_[0]); reg_attn(up_attn_[1]); }
+        if (bi < L_ - 1) reg_res(up_us_[bi]);
+    }
+    for (const char* k : {"last.0.weight", "last.0.bias", "last.2.weight", "last.2.bias"}) reg(p + k);
+    if (upscaler_) { reg("coarse_image_conv.weight"); reg("coarse_image_conv.bias"); }     // Upscaler02's own, after the U-Net's
+    THA4_REQUIRE((long)param_off_.size() == (long)sd.size(), "unet: the state_dict has tensors outside the parameter layout");
     THA4_CUDA_CHECK(cudaStreamSynchronize(s));
-    if (upscaler_) { cudaFree(d_t0); cudaFree(d_t1); cudaFree(d_t2); }
     loaded_ = true;
 }
 

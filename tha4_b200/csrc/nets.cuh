@@ -162,8 +162,8 @@ struct UNetGrads {
     int d_pose_ld = 0;
     float* d_coarse_posed = nullptr;
     float* d_coarse_grid = nullptr;
-    // parameter gradients (the body morpher): a flat fp32 buffer of param_count() floats in state_dict order
-    // (UNetNet::param_offset); accumulate_params: add to what it holds (the second and later micro-batch chunks)
+    // parameter gradients: a flat fp32 buffer of param_count() floats in state_dict order (UNetNet::param_offset);
+    // accumulate_params: add to what it holds (the second and later micro-batch chunks)
     float* d_params = nullptr;
     int accumulate_params = 0;
 };
@@ -172,6 +172,10 @@ struct UNetGrads {
 // workspace pool per frame (measured on an H100 at B = 1 and 2, DESIGN.md section 4), and the pool keeps its peak: 6 frames
 // keep a pass under 16 GiB.
 constexpr int UPSCALER_BWD_MAX_BATCH = 6;
+// With parameter gradients the tape also keeps every conv's operand: a pass takes 3749 MiB at B = 1 and 3391 MiB per further
+// frame in strict mode, 2998 + 2635 MiB in the default mode (measured on an H100 as above, DESIGN.md section 3): 4 frames keep
+// a strict pass under 16 GiB (13.6 GiB), 5 would not.
+constexpr int UPSCALER_PARAM_BWD_MAX_BATCH = 4;
 
 // Morpher00 (morpher_00.py:35-72) and Upscaler02 (upscaler_02.py:37-102) on Unet / UnetWithFirstConvAddition
 // (unet.py:438-546,549-658).
@@ -183,14 +187,14 @@ public:
     // tape: keep what backward() reads (its tensors then live in rt.persist; normalisations write out of place).
     void forward(Runtime& rt, const ImgView& image, const float* coarse_posed, const float* coarse_grid, int coarse_size,
                  const float* pose, int pose_ld, float* const* outputs, UNetTape* tape = nullptr);
-    // Input gradients (unet_backward.cu): recomputes the forward (same inputs as forward()) in the context's precision mode
-    // with a tape, then runs the adjoint of every layer back to the inputs that were asked for.
+    // Input and parameter gradients (unet_backward.cu): recomputes the forward (same inputs as forward()) in the context's
+    // precision mode with a tape, then runs the adjoint of every layer back to the inputs that were asked for.
     void backward(Runtime& rt, const ImgView& image, const float* coarse_posed, const float* coarse_grid, int coarse_size,
                   const float* pose, int pose_ld, const UNetGrads& g);
     int size() const { return S_; }
     bool loaded() const { return loaded_; }
-    // floats of the network's parameters (the body morpher's state_dict; 0 for the upscaler, which has no parameter
-    // gradients), and the offset of a state_dict key's tensor in the flat state_dict-order buffer
+    // floats of the network's parameters (its state_dict; the upscaler's includes coarse_image_conv), and the offset of a
+    // state_dict key's tensor in the flat state_dict-order buffer
     long param_count() const { return param_total_; }
     long param_offset(const std::string& key) const;
 private:
@@ -221,8 +225,8 @@ private:
     float *cond_w0_ = nullptr, *cond_b0_ = nullptr, *cond_w2_ = nullptr, *cond_b2_ = nullptr;
     float *film1_w_ = nullptr, *film1_b_ = nullptr;
     int film1_total_ = 0;
-    // the t = 0 time embedding's intermediates and weights its parameter gradients need (the body morpher): t0 [mc], t1 =
-    // time_embed.1(t0), t2 = time_embed.3(SiLU(t1)) [256], time_embed.3's weight, the cond0 projections stacked like film1_w_
+    // the t = 0 time embedding's intermediates and weights its parameter gradients need: t0 [mc], t1 = time_embed.1(t0),
+    // t2 = time_embed.3(SiLU(t1)) [256], time_embed.3's weight, the cond0 projections stacked like film1_w_
     float *time_t0_ = nullptr, *time_t1_ = nullptr, *time_t2_ = nullptr, *time_w3_ = nullptr, *film0_w_ = nullptr;
     NormW last_n_;
     TailWeights tail_;

@@ -17,10 +17,11 @@
 //   pose:      d(film1) through the FiLM projection, cond_embed.2 and cond_embed.0 (fixed-order fp64 GEMVs);
 //   upscaler:  the fused 16-channel first conv's data gradient goes through the prologue's adjoint (image_ops.cu): identity
 //              and warp terms to the rest image (which the tail warps too), the posed / grid terms through the bilinear x2.
-// Parameter gradients (the body morpher), into a flat state_dict-order buffer:
+// Parameter gradients, into a flat state_dict-order buffer:
 //   conv weights: the weight-gradient convolution (conv_wgrad.cu) of each conv's taped operand, rebuilt as the forward
 //              multiplied it, against the dz its data gradient already reads; the default mode's folded conv1 + skip is two
-//              convs (conv1 on the normalised h0, skip on the raw x);
+//              convs (conv1 on the normalised h0, skip on the raw x), and so is the upscaler's fused first conv (first_conv
+//              and coarse_image_conv on channel views of the prologue's output);
 //   conv biases: fixed-order fp64 pixel sums of the same dz;
 //   GroupNorm weights / biases and the time FiLM: from the norm backward's per-(n, c) sums (gn_param_fold_kernel);
 //   pose and time MLPs: d(film1) / d(film0) against the layer inputs (linear_wgrad_kernel), then back through the MLPs.
@@ -603,7 +604,7 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
     const bool want_x0 = want_img || want_coarse;          // gradients that need the first conv's data gradient
     const bool want_par = g.d_params != nullptr;
     THA4_REQUIRE(want_x0 || want_pose || want_par, "unet backward: no gradient requested");
-    THA4_REQUIRE(!want_par || (!upscaler_ && param_total_ > 0), "unet backward: parameter gradients are the body morpher's");
+    THA4_REQUIRE(!want_par || param_total_ > 0, "unet backward: no parameter layout");
     if (!adj_ready_) pack_adjoints(rt);
     const int B = image.N, S = S_, NH = 2 * L_;
     cudaStream_t s = rt.stream;
@@ -793,9 +794,14 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
         const View e_ds = dhs(2 * i - 1);
         gk = res_bwd(down_ds_[i - 1], 2, g_in, &e_ds, true);
     }
-    if (want_par) {                  // first conv (the body morpher's: 4 input channels)
+    if (want_par && !upscaler_) {    // first conv (the body morpher's: 4 input channels)
         wgrad(p + "first_conv", CONV_3x3, operand(tape.x0), gk);
         bias(gk, p + "first_conv");
+    } else if (want_par) {           // the fused 16-channel first conv: body.first_conv on channels 0-3 of x0 (the rest image),
+                                     // coarse_image_conv on 4-13 (posed, warped, grid); its bias is the sum of both
+        wgrad(p + "first_conv", CONV_3x3, operand(tape.x0.slice(0, 4)), gk);
+        wgrad("coarse_image_conv", CONV_3x3, operand(tape.x0.slice(4, 10)), gk);
+        bias(gk, p + "first_conv", "coarse_image_conv");
     }
     if (want_x0 && !upscaler_) {     // first conv: its data gradient joins the warp's image term in the epilogue
         View dx0 = fresh(P, B, S, S, 4);

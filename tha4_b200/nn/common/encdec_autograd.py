@@ -4,13 +4,12 @@ the reference modules are (eyebrow_decomposer_00.py:46-64, eyebrow_morphing_comb
 morpher_00.py:42-66, upscaler_02.py:59-96).  This is what pose fitting on an arbitrary character (expression and body parameters), or training an
 image -> pose regressor with a teacher as a differentiable renderer, needs.
 
-Dispatch: the autograd path runs when grad mode is on and an input (image, layer or pose) requires grad, or -- for the three
-encoder-decoder networks and the body morpher -- when the module was made trainable (`module.trainable_(True)`) and any of its
-parameters requires grad; in every other case the forward is the plain inference call.  Trainability is an explicit opt-in, not the students'
-"any parameter requires grad" rule, because a freshly built teacher's parameters require grad (as every nn.Module's do) and
-its inference calls must stay plain calls without a graph.  A trainable module's backward returns the gradients of the
-parameters that require grad (flat d_params from the same library call as the input gradients); only the upscaler's
-parameters never receive gradients.
+Dispatch: the autograd path runs when grad mode is on and an input (image, layer or pose) requires grad, or when the module
+was made trainable (`module.trainable_(True)`) and any of its parameters requires grad; in every other case the forward is
+the plain inference call.  Trainability is an explicit opt-in, not the students' "any parameter requires grad" rule,
+because a freshly built teacher's parameters require grad (as every nn.Module's do) and its inference calls must stay plain
+calls without a graph.  A trainable module's backward returns the gradients of the parameters that require grad (flat
+d_params from the same library call as the input gradients).
 
 Forward: the inference call; the outputs are bit-identical to the no-grad path (each in its own allocation, so in-place ops
 on them work).  Inputs and parameters are saved, so an in-place write to either between forward and backward raises torch's
@@ -27,7 +26,7 @@ from tha4_b200.nn.common.native_module import contiguous_grads, refuse_double_ba
 
 class Trainable:
     """Opt-in parameter gradients of the teacher modules (mixed into EyebrowDecomposer00, EyebrowMorphingCombiner00,
-    FaceMorpher08, Morpher00)."""
+    FaceMorpher08, Morpher00, Upscaler02)."""
     _trainable = False
 
     def trainable_(self, mode: bool = True):
@@ -224,12 +223,18 @@ def _upscaler_backward(ctx, *grad_outputs):
     rest_image, coarse_posed_image, coarse_grid_change, pose, *params = ctx.saved_tensors
     none = (None,) * len(params)
     want = ctx.needs_input_grad[1:5]
-    if not any(want) or all(g is None for g in grad_outputs):
+    if not any(ctx.needs_input_grad[1:]) or all(g is None for g in grad_outputs):
+        return (None, None, None, None, None) + none
+    ctx.lib = ctx.module.sync_weights()
+    flat, dp = _param_grads(ctx, 5, rest_image.device)
+    if flat is None and not any(want):
         return (None, None, None, None, None) + none
     d = [_empty_like(t) if w else None for t, w in zip((rest_image, coarse_posed_image, coarse_grid_change, pose), want)]
-    ctx.module.sync_weights().upscaler_backward(rest_image, coarse_posed_image, coarse_grid_change, pose, contiguous_grads(grad_outputs),
-                                                d_rest_image=d[0], d_coarse_posed=d[1], d_coarse_grid=d[2], d_pose=d[3])
-    return (None, *d) + none
+    # d_params only from a trainable module: the plain one keeps the input-gradient call it always made
+    extra = {'d_params': flat} if ctx.module.is_trainable() else {}
+    ctx.lib.upscaler_backward(rest_image, coarse_posed_image, coarse_grid_change, pose, contiguous_grads(grad_outputs),
+                              d_rest_image=d[0], d_coarse_posed=d[1], d_coarse_grid=d[2], d_pose=d[3], **extra)
+    return (None, *d) + dp
 
 
 def eyebrow_decomposer(module, image: Tensor) -> List[Tensor]:

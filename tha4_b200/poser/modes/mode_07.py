@@ -107,11 +107,10 @@ class FiveStepPoserComputationProtocol(CachedComputationProtocol):
 
     @staticmethod
     def _trains_teacher(state: ComputationState) -> bool:
-        """A teacher module of the poser (an encoder-decoder or the body morpher) was made trainable (trainable_(True)) and has
-        parameters that require grad."""
+        """A teacher module of the poser was made trainable (trainable_(True)) and has parameters that require grad."""
         return any(state.modules[net.name].wants_autograd()
                    for net in (Network.eyebrow_decomposer, Network.eyebrow_morphing_combiner, Network.face_morpher,
-                               Network.body_morpher)
+                               Network.body_morpher, Network.upscaler)
                    if isinstance(state.modules.get(net.name), Trainable))
 
     def _differentiable(self, state: ComputationState) -> List[Tensor]:
