@@ -184,12 +184,27 @@ class Context:
         flat = torch.empty((total,), dtype=torch.float32, device=self.device)
         return [flat[o:o + n].view(B, c, s, s) for o, n, (c, s) in zip(offs, sizes, specs)]
 
+    def _empty_half(self, specs, B: int) -> List[Tensor]:
+        """fp16 output tensors for one call, packed back to back in one allocation."""
+        sizes = [B * c * s * s for c, s in specs]
+        flat = torch.empty((sum(sizes),), dtype=torch.float16, device=self.device)
+        return [t.view(B, c, s, s) for t, (c, s) in zip(flat.split(sizes), specs)]
+
     # ------------------------------------------------------------------ module level
+    # (channels, size) of each network's outputs, in output order
+    DECOMPOSER_SPECS = [(4, 128), (1, 128), (4, 128), (4, 128), (1, 128), (4, 128)]
+    COMBINER_SPECS = [(4, 128), (1, 128), (4, 128), (4, 128), (1, 128), (4, 128), (4, 128), (2, 128)]
+    FACE_MORPHER_SPECS = [(4, 192), (1, 192), (4, 192), (4, 192), (1, 192), (4, 192), (4, 192), (2, 192)]
+    MORPHER_SPECS = [(4, 256), (1, 256), (4, 256), (2, 256), (4, 256)]
+    UPSCALER_SPECS = [(4, 512), (1, 512), (4, 512), (2, 512), (4, 512)]
+    SIREN_MORPHER_SPECS = [(4, 512), (1, 512), (4, 512), (4, 512), (2, 512)]
+    STUDENT_SPECS = SIREN_MORPHER_SPECS + [(4, 128)]          # the body student's outputs, then the face student's
+
     def eyebrow_decomposer(self, image: Tensor) -> List[Tensor]:
         image = _check_input(image, self.device, 'image')
         assert image.shape[1:] == (4, 128, 128)
         B = image.shape[0]
-        outs = self._empty([(4, 128), (1, 128), (4, 128), (4, 128), (1, 128), (4, 128)], B)
+        outs = self._empty(self.DECOMPOSER_SPECS, B)
         self._call('tha4_eyebrow_decomposer_forward', _ptr(image), B, _ptr_array(outs), self._stream())
         return outs
 
@@ -200,7 +215,7 @@ class Context:
         B = background_layer.shape[0]
         assert background_layer.shape[1:] == (4, 128, 128) and eyebrow_layer.shape == background_layer.shape
         assert pose.shape == (B, 12)
-        outs = self._empty([(4, 128), (1, 128), (4, 128), (4, 128), (1, 128), (4, 128), (4, 128), (2, 128)], B)
+        outs = self._empty(self.COMBINER_SPECS, B)
         self._call('tha4_eyebrow_morphing_combiner_forward', _ptr(background_layer), _ptr(eyebrow_layer), _ptr(pose), 12, B,
                    _ptr_array(outs), self._stream())
         return outs
@@ -210,13 +225,9 @@ class Context:
         pose = _check_input(pose, self.device, 'pose')
         B = image.shape[0]
         assert image.shape[1:] == (4, 192, 192) and pose.shape == (B, 27)
-        outs = self._empty([(4, 192), (1, 192), (4, 192), (4, 192), (1, 192), (4, 192), (4, 192), (2, 192)], B)
+        outs = self._empty(self.FACE_MORPHER_SPECS, B)
         self._call('tha4_face_morpher_forward', _ptr(image), _ptr(pose), 27, B, _ptr_array(outs), self._stream())
         return outs
-
-    DECOMPOSER_SPECS = [(4, 128), (1, 128), (4, 128), (4, 128), (1, 128), (4, 128)]
-    COMBINER_SPECS = [(4, 128), (1, 128), (4, 128), (4, 128), (1, 128), (4, 128), (4, 128), (2, 128)]
-    FACE_MORPHER_SPECS = [(4, 192), (1, 192), (4, 192), (4, 192), (1, 192), (4, 192), (4, 192), (2, 192)]
 
     def _grads(self, specs, grad_outputs: Sequence[Optional[Tensor]], B: int) -> List[Optional[Tensor]]:
         assert len(grad_outputs) == len(specs)
@@ -286,8 +297,6 @@ class Context:
         self._call('tha4_face_morpher_backward', _ptr(image), _ptr(pose), 27, B, _ptr_array(gs), _ptr(d_image), _ptr(d_pose),
                    _ptr(d_params), self._stream())
 
-    MORPHER_SPECS = [(4, 256), (1, 256), (4, 256), (2, 256), (4, 256)]
-
     def morpher(self, image: Tensor, pose: Tensor) -> List[Tensor]:
         image = _check_input(image, self.device, 'image')
         pose = _check_input(pose, self.device, 'pose')
@@ -312,8 +321,6 @@ class Context:
         self._check_out(d_params, (self.param_count('body_morpher'),), 'd_params')
         self._call('tha4_morpher_backward', _ptr(image), _ptr(pose), 6, B, _ptr_array(gs), _ptr(d_image), _ptr(d_pose),
                    _ptr(d_params), self._stream())
-
-    UPSCALER_SPECS = [(4, 512), (1, 512), (4, 512), (2, 512), (4, 512)]
 
     def _upscaler_inputs(self, rest_image: Tensor, coarse_posed: Tensor, coarse_grid: Tensor, pose: Tensor):
         rest_image = _check_input(rest_image, self.device, 'rest_image')
@@ -361,8 +368,6 @@ class Context:
         self._call('tha4_siren_face_morpher_forward', _ptr(pose), 39, B, _ptr(out), self._stream())
         return out
 
-    SIREN_MORPHER_SPECS = [(4, 512), (1, 512), (4, 512), (4, 512), (2, 512)]
-
     def siren_morpher(self, image: Tensor, pose: Tensor) -> List[Tensor]:
         B = image.shape[0]
         return self.siren_morpher_into(image, pose, self._empty(self.SIREN_MORPHER_SPECS, B))
@@ -379,14 +384,9 @@ class Context:
         return outs
 
     # ------------------------------------------------------------------ poser level
-    TEACHER_SPECS = {
-        7: [(4, 512), (1, 512), (4, 512), (2, 512), (4, 512), (4, 512),
-            (4, 256), (1, 256), (4, 256), (2, 256), (4, 256)],
-        12: [],
-    }
-    FACE_COMB_DEC = [(4, 192), (1, 192), (4, 192), (4, 192), (1, 192), (4, 192), (4, 192), (2, 192),
-                     (4, 128), (1, 128), (4, 128), (4, 128), (1, 128), (4, 128), (4, 128), (2, 128),
-                     (4, 128), (1, 128), (4, 128), (4, 128), (1, 128), (4, 128)]
+    # mode 7: the upscaler's outputs, face_morphed_full, the body morpher's
+    TEACHER_SPECS = {7: UPSCALER_SPECS + [(4, 512)] + MORPHER_SPECS, 12: []}
+    FACE_COMB_DEC = FACE_MORPHER_SPECS + COMBINER_SPECS + DECOMPOSER_SPECS
 
     def teacher_forward(self, mode: int, image: Tensor, pose: Tensor, eyebrow_morphed_image_index: int = 2,
                         cached_decomposer: Optional[List[Tensor]] = None) -> List[Tensor]:
@@ -418,7 +418,7 @@ class Context:
         pose = _check_input(pose, self.device, 'pose')
         B = image.shape[0]
         assert image.shape[1:] == (4, 512, 512) and pose.shape == (B, 45)
-        outs = self._empty([(4, 512), (1, 512), (4, 512), (4, 512), (2, 512), (4, 128)], B)
+        outs = self._empty(self.STUDENT_SPECS, B)
         self._call('tha4_student_forward', _ptr(image), _ptr(pose), B, _ptr_array(outs), self._stream())
         return outs
 
@@ -430,13 +430,7 @@ class Context:
         pose = _check_input(pose, self.device, 'pose')
         B = image.shape[0]
         assert image.shape[1:] == (4, 512, 512) and pose.shape == (B, 45)
-        shapes = [(4, 512), (1, 512), (4, 512), (4, 512), (2, 512), (4, 128)]
-        flat = torch.empty(sum(B * c * r * r for c, r in shapes), dtype=torch.float16, device=self.device)
-        outs, o = [], 0
-        for c, r in shapes:
-            n = B * c * r * r
-            outs.append(flat[o:o + n].view(B, c, r, r))
-            o += n
+        outs = self._empty_half(self.STUDENT_SPECS, B)
         self._call('tha4_student_forward_io', _ptr(image), _ptr(pose), B, _ptr_array(outs), 1, self._stream())
         return outs
 
@@ -464,15 +458,7 @@ class Context:
         pose = _check_input(pose, self.device, 'pose')
         B = len(char_ids)
         assert B >= 1 and pose.shape == (B, 45)
-        specs = [(4, 512), (1, 512), (4, 512), (4, 512), (2, 512), (4, 128)]
-        if half:
-            flat = torch.empty(sum(B * c * r * r for c, r in specs), dtype=torch.float16, device=self.device)
-            outs, o = [], 0
-            for c, r in specs:
-                outs.append(flat[o:o + B * c * r * r].view(B, c, r, r))
-                o += B * c * r * r
-        else:
-            outs = self._empty(specs, B)
+        outs = self._empty_half(self.STUDENT_SPECS, B) if half else self._empty(self.STUDENT_SPECS, B)
         ids = (ctypes.c_int * B)(*[int(i) for i in char_ids])
         self._call('tha4_bank_forward', ids, _ptr(pose), B, _ptr_array(outs), 1 if half else 0, self._stream())
         return outs

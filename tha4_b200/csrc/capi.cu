@@ -188,6 +188,10 @@ void offset_outputs(float* const* outputs, const OutSpec* spec, int n0, float** 
     for (int i = 0; i < NOUT; ++i) dst[i] = outputs[i] + (size_t)n0 * spec[i].c * spec[i].s * spec[i].s;
 }
 
+// frame n0 of a batch whose frames are `frame` elements apart; null stays null (an input or output that is not given)
+template <typename T>
+T* at_frame(T* p, int n0, size_t frame) { return p ? p + (size_t)n0 * frame : nullptr; }
+
 // the upstream gradients of one micro-batch (an entry may be null)
 template <int NOUT>
 void offset_grads(const float* const* grads, const OutSpec* spec, int n0, const float** dst) {
@@ -323,7 +327,7 @@ int tha4_eyebrow_decomposer_forward(tha4_ctx* ctx, const float* image, int B, fl
         Runtime rt = make_rt(ctx, stream);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             float* o[6]; offset_outputs<6>(outputs, kEncDecDecomposer, n0, o);
-            ctx->decomposer->forward(rt, make_img(image + (size_t)n0 * 4 * 128 * 128, b, 4, 128, 128), ImgView{}, nullptr, 0, o);
+            ctx->decomposer->forward(rt, make_img(at_frame(image, n0, 4 * 128 * 128), b, 4, 128, 128), ImgView{}, nullptr, 0, o);
         });
     });
 }
@@ -334,9 +338,9 @@ int tha4_eyebrow_morphing_combiner_forward(tha4_ctx* ctx, const float* backgroun
         Runtime rt = make_rt(ctx, stream);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             float* o[8]; offset_outputs<8>(outputs, kCombiner, n0, o);
-            const size_t off = (size_t)n0 * 4 * 128 * 128;
-            ctx->combiner->forward(rt, make_img(eyebrow_layer + off, b, 4, 128, 128), make_img(background_layer + off, b, 4, 128, 128),
-                                   pose + (size_t)n0 * pose_ld, pose_ld, o);
+            const size_t layer = 4 * 128 * 128;
+            ctx->combiner->forward(rt, make_img(at_frame(eyebrow_layer, n0, layer), b, 4, 128, 128),
+                                   make_img(at_frame(background_layer, n0, layer), b, 4, 128, 128), at_frame(pose, n0, pose_ld), pose_ld, o);
         });
     });
 }
@@ -347,8 +351,8 @@ int tha4_face_morpher_forward(tha4_ctx* ctx, const float* image, const float* po
         Runtime rt = make_rt(ctx, stream);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             float* o[8]; offset_outputs<8>(outputs, kFace, n0, o);
-            ctx->face->forward(rt, make_img(image + (size_t)n0 * 4 * 192 * 192, b, 4, 192, 192), ImgView{},
-                               pose + (size_t)n0 * pose_ld, pose_ld, o);
+            ctx->face->forward(rt, make_img(at_frame(image, n0, 4 * 192 * 192), b, 4, 192, 192), ImgView{}, at_frame(pose, n0, pose_ld),
+                               pose_ld, o);
         });
     });
 }
@@ -380,9 +384,9 @@ int tha4_eyebrow_decomposer_backward(tha4_ctx* ctx, const float* image, int B, c
         Runtime rt = make_rt(ctx, stream);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             const float* g[6]; offset_grads<6>(grad_outputs, kEncDecDecomposer, n0, g);
-            EncDecGrads eg; eg.grad_outputs = g; eg.d_image0 = d_image ? d_image + (size_t)n0 * 4 * 128 * 128 : nullptr;
+            EncDecGrads eg; eg.grad_outputs = g; eg.d_image0 = at_frame(d_image, n0, 4 * 128 * 128);
             eg.d_params = d_params; eg.accumulate_params = n0 > 0;
-            ctx->decomposer->backward(rt, make_img(image + (size_t)n0 * 4 * 128 * 128, b, 4, 128, 128), ImgView{}, nullptr, 0, eg);
+            ctx->decomposer->backward(rt, make_img(at_frame(image, n0, 4 * 128 * 128), b, 4, 128, 128), ImgView{}, nullptr, 0, eg);
         });
     });
 }
@@ -397,14 +401,14 @@ int tha4_eyebrow_morphing_combiner_backward(tha4_ctx* ctx, const float* backgrou
         Runtime rt = make_rt(ctx, stream);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             const float* g[8]; offset_grads<8>(grad_outputs, kCombiner, n0, g);
-            const size_t off = (size_t)n0 * 4 * 128 * 128;
+            const size_t layer = 4 * 128 * 128;
             EncDecGrads eg; eg.grad_outputs = g;
-            eg.d_image0 = d_eyebrow_layer ? d_eyebrow_layer + off : nullptr;
-            eg.d_image1 = d_background_layer ? d_background_layer + off : nullptr;
-            eg.d_pose = d_pose ? d_pose + (size_t)n0 * 12 : nullptr; eg.d_pose_ld = 12;
+            eg.d_image0 = at_frame(d_eyebrow_layer, n0, layer);
+            eg.d_image1 = at_frame(d_background_layer, n0, layer);
+            eg.d_pose = at_frame(d_pose, n0, 12); eg.d_pose_ld = 12;
             eg.d_params = d_params; eg.accumulate_params = n0 > 0;
-            ctx->combiner->backward(rt, make_img(eyebrow_layer + off, b, 4, 128, 128), make_img(background_layer + off, b, 4, 128, 128),
-                                    pose + (size_t)n0 * pose_ld, pose_ld, eg);
+            ctx->combiner->backward(rt, make_img(at_frame(eyebrow_layer, n0, layer), b, 4, 128, 128),
+                                    make_img(at_frame(background_layer, n0, layer), b, 4, 128, 128), at_frame(pose, n0, pose_ld), pose_ld, eg);
         });
     });
 }
@@ -419,10 +423,10 @@ int tha4_face_morpher_backward(tha4_ctx* ctx, const float* image, const float* p
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             const float* g[8]; offset_grads<8>(grad_outputs, kFace, n0, g);
             EncDecGrads eg; eg.grad_outputs = g;
-            eg.d_image0 = d_image ? d_image + (size_t)n0 * 4 * 192 * 192 : nullptr;
-            eg.d_pose = d_pose ? d_pose + (size_t)n0 * 27 : nullptr; eg.d_pose_ld = 27;
+            eg.d_image0 = at_frame(d_image, n0, 4 * 192 * 192);
+            eg.d_pose = at_frame(d_pose, n0, 27); eg.d_pose_ld = 27;
             eg.d_params = d_params; eg.accumulate_params = n0 > 0;
-            ctx->face->backward(rt, make_img(image + (size_t)n0 * 4 * 192 * 192, b, 4, 192, 192), ImgView{}, pose + (size_t)n0 * pose_ld,
+            ctx->face->backward(rt, make_img(at_frame(image, n0, 4 * 192 * 192), b, 4, 192, 192), ImgView{}, at_frame(pose, n0, pose_ld),
                                 pose_ld, eg);
         });
     });
@@ -435,8 +439,8 @@ int tha4_morpher_forward(tha4_ctx* ctx, const float* image, const float* pose, i
         OutSpec spec[5]; fill_unet_spec(spec, 256);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             float* o[5]; offset_outputs<5>(outputs, spec, n0, o);
-            ctx->body->forward(rt, make_img(image + (size_t)n0 * 4 * 256 * 256, b, 4, 256, 256), nullptr, nullptr, 0,
-                               pose + (size_t)n0 * pose_ld, pose_ld, o);
+            ctx->body->forward(rt, make_img(at_frame(image, n0, 4 * 256 * 256), b, 4, 256, 256), nullptr, nullptr, 0,
+                               at_frame(pose, n0, pose_ld), pose_ld, o);
         });
     });
 }
@@ -452,11 +456,11 @@ int tha4_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, 
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             const float* g[5]; offset_grads<5>(grad_outputs, spec, n0, g);
             UNetGrads ug; ug.grad_outputs = g;
-            ug.d_image = d_image ? d_image + (size_t)n0 * 4 * 256 * 256 : nullptr;
-            ug.d_pose = d_pose ? d_pose + (size_t)n0 * 6 : nullptr; ug.d_pose_ld = 6;
+            ug.d_image = at_frame(d_image, n0, 4 * 256 * 256);
+            ug.d_pose = at_frame(d_pose, n0, 6); ug.d_pose_ld = 6;
             ug.d_params = d_params; ug.accumulate_params = n0 > 0;
-            ctx->body->backward(rt, make_img(image + (size_t)n0 * 4 * 256 * 256, b, 4, 256, 256), nullptr, nullptr, 0,
-                                pose + (size_t)n0 * pose_ld, pose_ld, ug);
+            ctx->body->backward(rt, make_img(at_frame(image, n0, 4 * 256 * 256), b, 4, 256, 256), nullptr, nullptr, 0,
+                                at_frame(pose, n0, pose_ld), pose_ld, ug);
         });
     });
 }
@@ -478,13 +482,13 @@ int tha4_upscaler_backward(tha4_ctx* ctx, const float* rest_image, const float* 
         for_chunks(ctx, B, std::min(ctx->opt.microbatch, max_batch), rt.stream, [&](int n0, int b) {
             const float* g[5]; offset_grads<5>(grad_outputs, spec, n0, g);
             UNetGrads ug; ug.grad_outputs = g;
-            ug.d_image = d_rest_image ? d_rest_image + (size_t)n0 * 4 * hw : nullptr;
-            ug.d_coarse_posed = d_coarse_posed_image ? d_coarse_posed_image + (size_t)n0 * 4 * chw : nullptr;
-            ug.d_coarse_grid = d_coarse_grid_change ? d_coarse_grid_change + (size_t)n0 * 2 * chw : nullptr;
-            ug.d_pose = d_pose ? d_pose + (size_t)n0 * 6 : nullptr; ug.d_pose_ld = 6;
+            ug.d_image = at_frame(d_rest_image, n0, 4 * hw);
+            ug.d_coarse_posed = at_frame(d_coarse_posed_image, n0, 4 * chw);
+            ug.d_coarse_grid = at_frame(d_coarse_grid_change, n0, 2 * chw);
+            ug.d_pose = at_frame(d_pose, n0, 6); ug.d_pose_ld = 6;
             ug.d_params = d_params; ug.accumulate_params = n0 > 0;
-            ctx->upscaler->backward(rt, make_img(rest_image + (size_t)n0 * 4 * hw, b, 4, 512, 512), coarse_posed_image + (size_t)n0 * 4 * chw,
-                                    coarse_grid_change + (size_t)n0 * 2 * chw, coarse_size, pose + (size_t)n0 * pose_ld, pose_ld, ug);
+            ctx->upscaler->backward(rt, make_img(at_frame(rest_image, n0, 4 * hw), b, 4, 512, 512), at_frame(coarse_posed_image, n0, 4 * chw),
+                                    at_frame(coarse_grid_change, n0, 2 * chw), coarse_size, at_frame(pose, n0, pose_ld), pose_ld, ug);
         });
     });
 }
@@ -495,11 +499,11 @@ int tha4_upscaler_forward(tha4_ctx* ctx, const float* rest_image, const float* c
     return guarded(ctx, [&] {
         Runtime rt = make_rt(ctx, stream);
         OutSpec spec[5]; fill_unet_spec(spec, 512);
+        const size_t hw = 512 * 512, chw = (size_t)coarse_size * coarse_size;
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
             float* o[5]; offset_outputs<5>(outputs, spec, n0, o);
-            ctx->upscaler->forward(rt, make_img(rest_image + (size_t)n0 * 4 * 512 * 512, b, 4, 512, 512),
-                                   coarse_posed_image + (size_t)n0 * 4 * coarse_size * coarse_size,
-                                   coarse_grid_change + (size_t)n0 * 2 * coarse_size * coarse_size, coarse_size, pose + (size_t)n0 * pose_ld, pose_ld, o);
+            ctx->upscaler->forward(rt, make_img(at_frame(rest_image, n0, 4 * hw), b, 4, 512, 512), at_frame(coarse_posed_image, n0, 4 * chw),
+                                   at_frame(coarse_grid_change, n0, 2 * chw), coarse_size, at_frame(pose, n0, pose_ld), pose_ld, o);
         });
     });
 }

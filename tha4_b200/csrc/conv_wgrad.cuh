@@ -30,6 +30,13 @@ struct WgradOperand {
     int coef_C = 0;
 };
 
+// The operand that reads View v as stored (no transform).
+inline WgradOperand wgrad_operand(const View& v) {
+    WgradOperand o;
+    o.p = v.p; o.f16 = v.f16; o.ld = v.ld; o.N = v.N; o.H = v.H; o.W = v.W; o.C = v.C;
+    return o;
+}
+
 // dW[d][c][tap] (+)= sum_p D[p][d] G[p * stride - pad + (ky, kx)][c], tap = ky * ksz + kx, written to out at
 // out_row[d] + c * ntaps + tap (n_map > 0: rows d >= n_map are dropped), else at (d * c_real + c) * ntaps + tap; channels
 // c >= c_real of G are not written.  accumulate: add to what out holds (later micro-batch chunks).

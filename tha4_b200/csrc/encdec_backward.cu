@@ -455,12 +455,6 @@ void EncDecNet::load_adjoints(const StateDict& sd, const std::string& p, cudaStr
     head_pack_adjoint(adj_head_, tail_, conv_pack_rounding(), s);
 }
 
-long EncDecNet::param_offset(const std::string& key) const {
-    auto it = param_off_.find(key);
-    THA4_REQUIRE(it != param_off_.end(), "parameter gradients: no tensor " + key);
-    return it->second;
-}
-
 void EncDecNet::backward(Runtime& rt, const ImgView& image0, const ImgView& image1, const float* pose, int pose_ld, const EncDecGrads& g) {
     THA4_REQUIRE(loaded_, "network weights not loaded");
     const bool want_img = g.d_image0 || g.d_image1, want_pose = g.d_pose != nullptr, want_par = g.d_params != nullptr;
@@ -494,8 +488,7 @@ void EncDecNet::backward(Runtime& rt, const ImgView& image0, const ImgView& imag
     // ---- weight gradients.  An operand as the forward conv multiplied it: the stored tensor, or (default mode) an f16 raw
     // conv output with the pending InstanceNorm + ReLU its consumer applied, rebuilt from `stats`' statistics
     auto operand = [&](const View& v, const NormW* nw = nullptr, const View* stats = nullptr) {
-        WgradOperand o;
-        o.p = v.p; o.f16 = v.f16; o.ld = v.ld; o.N = v.N; o.H = v.H; o.W = v.W; o.C = v.C;
+        WgradOperand o = wgrad_operand(v);
         if (nw && rt.f16) {
             float2* coef = reinterpret_cast<float2*>(P->alloc((size_t)v.N * nw->C * 2));
             wgrad_xf_coef(*stats, nw->gamma, nw->beta, nw->C, ACT_RELU, coef, s);
@@ -540,10 +533,10 @@ void EncDecNet::backward(Runtime& rt, const ImgView& image0, const ImgView& imag
         int ch = 0;
         for (size_t h = 0; h < head_key_.size(); ++h) {
             const long wo = param_offset(head_key_[h] + ".weight");
-            auto bi = param_off_.find(head_key_[h] + ".bias");
+            auto bi = params_.off.find(head_key_[h] + ".bias");
             for (int co = 0; co < head_cout_[h]; ++co, ++ch) {
                 a.out_row[ch] = wo + (long)co * f.C * 9;
-                hb.off[ch] = bi == param_off_.end() ? -1 : bi->second + co;
+                hb.off[ch] = bi == params_.off.end() ? -1 : bi->second + co;
             }
         }
         a.n_map = ch; d.C = ch;

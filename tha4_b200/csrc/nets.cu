@@ -278,9 +278,10 @@ void EncDecNet::load(const StateDict& sd, cudaStream_t s) {
     if (kind_ == TAIL_DECOMPOSER) head_key_ = {"background_layer_alpha.0", "background_layer_color_change.0", "eyebrow_layer_alpha.0", "eyebrow_layer_color_change.0"};
     else if (kind_ == TAIL_COMBINER) head_key_ = {"morphed_eyebrow_layer_grid_change", "morphed_eyebrow_layer_alpha.0", "morphed_eyebrow_layer_color_change.0", "combine_alpha.0"};
     else head_key_ = {"iris_mouth_grid_change", "iris_mouth_color_change.0", "iris_mouth_alpha.0", "eye_color_change.0", "eye_alpha.0"};
-    param_off_.clear(); param_total_ = 0;
-    auto reg = [&](const std::string& key) { param_off_[key] = param_total_; param_total_ += sd_get(sd, key).numel(); };
-    auto reg_block = [&](const std::string& conv, const std::string& norm) { reg(conv + ".weight"); reg(norm + ".weight"); reg(norm + ".bias"); };
+    params_ = ParamLayout();
+    auto reg_block = [&](const std::string& conv, const std::string& norm) {
+        params_.add(sd, conv + ".weight"); params_.add(sd, norm + ".weight"); params_.add(sd, norm + ".bias");
+    };
     for (int i = 0; i < 4; ++i) reg_block(p + "downsample_blocks." + std::to_string(i) + ".0", p + "downsample_blocks." + std::to_string(i) + ".1");
     reg_block(p + "bottleneck_blocks.0.0", p + "bottleneck_blocks.0.1");
     for (int i = 0; i < 5; ++i) {
@@ -290,9 +291,9 @@ void EncDecNet::load(const StateDict& sd, cudaStream_t s) {
     }
     for (int i = 0; i < 3; ++i) reg_block(p + "upsample_blocks." + std::to_string(i) + ".0", p + "upsample_blocks." + std::to_string(i) + ".1");
     for (const std::string& h : head_key_) {
-        reg(h + ".weight");
+        params_.add(sd, h + ".weight");
         head_cout_.push_back((int)sd_get(sd, h + ".weight").shape[0]);
-        if (sd.count(h + ".bias")) reg(h + ".bias");
+        if (sd.count(h + ".bias")) params_.add(sd, h + ".bias");
     }
     load_adjoints(sd, p, s);
     THA4_CUDA_CHECK(cudaStreamSynchronize(s));
@@ -589,25 +590,25 @@ void UNetNet::load(const StateDict& sd, cudaStream_t s) {
                                         2 * w->cout * sizeof(float), cudaMemcpyDeviceToDevice, s));
     }
     if (conv_pack_rounding()) tail_make_half(tail_, s);       // default mode: the wgmma tail's f16 head weights
-    param_off_.clear(); param_total_ = 0;
+    params_ = ParamLayout();
     time_t0_ = d_t0; time_t1_ = d_t1; time_t2_ = d_t2;
     time_w3_ = dev_clone(sd_get(sd, p + "time_embed.3.weight"), s);
     // the flat parameter-gradient layout: the reference's state_dict order (unet.py:438-529, registration order of the
     // modules; per up level its ResBlocks, then its attention blocks, then the up-sampler)
-    auto reg = [&](const std::string& key) { param_off_[key] = param_total_; param_total_ += sd_get(sd, key).numel(); };
     auto reg_res = [&](const ResBlockW& w) {
         for (const char* k : {".norm0.weight", ".norm0.bias", ".conv0.weight", ".conv0.bias", ".cond0_layers.1.weight",
                               ".cond0_layers.1.bias", ".norm1.weight", ".norm1.bias", ".conv1.weight", ".conv1.bias",
                               ".cond1_layers.1.weight", ".cond1_layers.1.bias"})
-            reg(w.key + k);
-        if (w.has_skip) { reg(w.key + ".skip.weight"); reg(w.key + ".skip.bias"); }
+            params_.add(sd, w.key + k);
+        if (w.has_skip) { params_.add(sd, w.key + ".skip.weight"); params_.add(sd, w.key + ".skip.bias"); }
     };
     auto reg_attn = [&](const AttnW& a) {
-        for (const char* k : {".norm.weight", ".norm.bias", ".qkv.weight", ".qkv.bias", ".conv.weight", ".conv.bias"}) reg(a.key + k);
+        for (const char* k : {".norm.weight", ".norm.bias", ".qkv.weight", ".qkv.bias", ".conv.weight", ".conv.bias"})
+            params_.add(sd, a.key + k);
     };
     for (const char* k : {"time_embed.1.weight", "time_embed.1.bias", "time_embed.3.weight", "time_embed.3.bias", "cond_embed.0.weight",
                           "cond_embed.0.bias", "cond_embed.2.weight", "cond_embed.2.bias", "first_conv.weight", "first_conv.bias"})
-        reg(p + k);
+        params_.add(sd, p + k);
     for (int i = 0; i < L_; ++i) {
         reg_res(down_res_[i]);
         if (i == L_ - 1) reg_attn(down_attn_);
@@ -619,16 +620,24 @@ void UNetNet::load(const StateDict& sd, cudaStream_t s) {
         if (bi == 0) { reg_attn(up_attn_[0]); reg_attn(up_attn_[1]); }
         if (bi < L_ - 1) reg_res(up_us_[bi]);
     }
-    for (const char* k : {"last.0.weight", "last.0.bias", "last.2.weight", "last.2.bias"}) reg(p + k);
-    if (upscaler_) { reg("coarse_image_conv.weight"); reg("coarse_image_conv.bias"); }     // Upscaler02's own, after the U-Net's
-    THA4_REQUIRE((long)param_off_.size() == (long)sd.size(), "unet: the state_dict has tensors outside the parameter layout");
+    for (const char* k : {"last.0.weight", "last.0.bias", "last.2.weight", "last.2.bias"}) params_.add(sd, p + k);
+    if (upscaler_) {      // Upscaler02's own, after the U-Net's
+        params_.add(sd, "coarse_image_conv.weight");
+        params_.add(sd, "coarse_image_conv.bias");
+    }
+    THA4_REQUIRE((long)params_.off.size() == (long)sd.size(), "unet: the state_dict has tensors outside the parameter layout");
     THA4_CUDA_CHECK(cudaStreamSynchronize(s));
     loaded_ = true;
 }
 
-long UNetNet::param_offset(const std::string& key) const {
-    auto it = param_off_.find(key);
-    THA4_REQUIRE(it != param_off_.end(), "parameter gradients: no tensor " + key);
+void ParamLayout::add(const StateDict& sd, const std::string& key) {
+    off[key] = total;
+    total += sd_get(sd, key).numel();
+}
+
+long ParamLayout::offset(const std::string& key) const {
+    auto it = off.find(key);
+    THA4_REQUIRE(it != off.end(), "parameter gradients: no tensor " + key);
     return it->second;
 }
 

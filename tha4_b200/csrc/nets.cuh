@@ -50,6 +50,22 @@ struct Runtime {                      // per-call execution context
     double* alloc_stats(size_t n);
 };
 
+// The flat parameter-gradient layout of a network: the offset of each state_dict tensor in a buffer of `total` floats, in
+// the order add() registered them (the reference's state_dict order).
+struct ParamLayout {
+    std::map<std::string, long> off;
+    long total = 0;
+    void add(const StateDict& sd, const std::string& key);     // appends the tensor sd[key]
+    long offset(const std::string& key) const;
+};
+
+// The parameter gradients a backward writes: a flat fp32 buffer of param_count() floats in state_dict order (null = not
+// computed); accumulate_params: add to what it holds (the second and later micro-batch chunks) instead of overwriting it.
+struct ParamGrads {
+    float* d_params = nullptr;
+    int accumulate_params = 0;
+};
+
 // ------------------------------------------------------------------ encoder-decoder networks
 // The activations a backward pass reads from the forward it recomputes: the NHWC network input and the RAW output of every
 // conv that is followed by an InstanceNorm (fp32 or f16 data, with the statistics the producing conv accumulated).
@@ -66,16 +82,12 @@ struct EncDecTape {
 // What EncDecNet::backward computes.  grad_outputs: the upstream gradients of the network's outputs (NCHW, an entry may be
 // null = zero).  Every other pointer is an output, null = not computed: d_image0 / d_image1 follow forward()'s image0 /
 // image1, d_pose is [N][d_pose_ld] (its first pose_ch entries per row are written).
-struct EncDecGrads {
+struct EncDecGrads : ParamGrads {
     const float* const* grad_outputs = nullptr;
     float* d_image0 = nullptr;
     float* d_image1 = nullptr;
     float* d_pose = nullptr;
     int d_pose_ld = 0;
-    // parameter gradients: a flat fp32 buffer of param_count() floats in state_dict order (EncDecNet::param_offset);
-    // accumulate_params: add to what it holds (the second and later micro-batch chunks) instead of overwriting it
-    float* d_params = nullptr;
-    int accumulate_params = 0;
 };
 
 // EyebrowDecomposer00 / EyebrowMorphingCombiner00 / FaceMorpher08 (poser_encoder_decoder_00.py:43-121,
@@ -95,8 +107,8 @@ public:
     int size() const { return S_; }
     int num_outputs() const { return kind_ == TAIL_DECOMPOSER ? 6 : 8; }
     // floats of the network's parameters, and the offset of a state_dict key's tensor in the flat state_dict-order buffer
-    long param_count() const { return param_total_; }
-    long param_offset(const std::string& key) const;
+    long param_count() const { return params_.total; }
+    long param_offset(const std::string& key) const { return params_.offset(key); }
     bool loaded() const { return loaded_; }
 private:
     void forward_fused(Runtime& rt, const View& x0, const ImgView& image0, const ImgView& image1, const float* pose, int pose_ld,
@@ -107,8 +119,7 @@ private:
     int S_, in_ch_, pose_ch_, pose_pad_;
     bool loaded_ = false;
     std::string prefix_;
-    std::map<std::string, long> param_off_;     // state_dict key -> offset in the flat parameter buffer
-    long param_total_ = 0;
+    ParamLayout params_;
     std::vector<int> head_cout_;                // output channels of each head, in the tail's packing order
     std::vector<std::string> head_key_;         //   and its state_dict prefix
     ConvWeights down_[4], bott0_, res_[5][2], up_[3];
@@ -155,17 +166,13 @@ struct UNetTape {
 // What UNetNet::backward computes: grad_outputs[5] (merged, alpha, warped, grid_change, direct; NCHW, null = zero);
 // d_image [N,4,S,S] (the upscaler: its rest image), d_pose [N][d_pose_ld] (first 6 entries per row) and, on the upscaler only,
 // d_coarse_posed [N,4,c,c] / d_coarse_grid [N,2,c,c] (c = coarse_size) are outputs, null = not computed.
-struct UNetGrads {
+struct UNetGrads : ParamGrads {
     const float* const* grad_outputs = nullptr;
     float* d_image = nullptr;
     float* d_pose = nullptr;
     int d_pose_ld = 0;
     float* d_coarse_posed = nullptr;
     float* d_coarse_grid = nullptr;
-    // parameter gradients: a flat fp32 buffer of param_count() floats in state_dict order (UNetNet::param_offset);
-    // accumulate_params: add to what it holds (the second and later micro-batch chunks)
-    float* d_params = nullptr;
-    int accumulate_params = 0;
 };
 
 // Frames per pass of the upscaler backward.  Its taped forward and gradient buffers at 512x512 take 2610 MiB of the context's
@@ -195,12 +202,11 @@ public:
     bool loaded() const { return loaded_; }
     // floats of the network's parameters (its state_dict; the upscaler's includes coarse_image_conv), and the offset of a
     // state_dict key's tensor in the flat state_dict-order buffer
-    long param_count() const { return param_total_; }
-    long param_offset(const std::string& key) const;
+    long param_count() const { return params_.total; }
+    long param_offset(const std::string& key) const { return params_.offset(key); }
 private:
     AllocSink owned_;          // every device allocation made by load()
-    std::map<std::string, long> param_off_;     // state_dict key -> offset in the flat parameter buffer
-    long param_total_ = 0;
+    ParamLayout params_;
     void forward_fused(Runtime& rt, const ImgView& image, const float* coarse_posed, const float* coarse_grid, int coarse_size,
                        const float* pose, int pose_ld, float* const* outputs, UNetTape* tape);
     void res_block(Runtime& rt, const ResBlockW& w, const View& x, int mode, const float* film1, const View& out, UNetTape* tape);

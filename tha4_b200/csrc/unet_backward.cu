@@ -604,7 +604,7 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
     const bool want_x0 = want_img || want_coarse;          // gradients that need the first conv's data gradient
     const bool want_par = g.d_params != nullptr;
     THA4_REQUIRE(want_x0 || want_pose || want_par, "unet backward: no gradient requested");
-    THA4_REQUIRE(!want_par || param_total_ > 0, "unet backward: no parameter layout");
+    THA4_REQUIRE(!want_par || params_.total > 0, "unet backward: no parameter layout");
     if (!adj_ready_) pack_adjoints(rt);
     const int B = image.N, S = S_, NH = 2 * L_;
     cudaStream_t s = rt.stream;
@@ -639,14 +639,9 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
     };
     // ---- parameter-gradient helpers ----
     const auto ws_alloc = [&](size_t n) { return rt.scratch->alloc(n); };
-    auto operand = [&](const View& v) {
-        WgradOperand o;
-        o.p = v.p; o.f16 = v.f16; o.ld = v.ld; o.N = v.N; o.H = v.H; o.W = v.W; o.C = v.C;
-        return o;
-    };
     // an f16 raw tensor with the pending GroupNorm (+FiLM) + act its consumer conv applied, coefficients from the forward's builder
     auto pending = [&](const View& raw, const NormW& nw, int act, const float* film0, const float* film1) {
-        WgradOperand o = operand(raw);
+        WgradOperand o = wgrad_operand(raw);
         float2* coef = reinterpret_cast<float2*>(P->alloc((size_t)B * nw.C * 2));
         wgrad_xf_coef(raw, nw.gamma, nw.beta, nw.C, act, coef, s, 32, film0, film1, film1_total_);
         o.xf = WG_XF_HALF; o.act = act; o.coef = coef; o.coef_C = nw.C;
@@ -655,7 +650,7 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
     auto wgrad = [&](const std::string& key, ConvKind kind, const WgradOperand& x, const View& dz) {
         WgradArgs a;
         a.accumulate = acc; a.out = par(key + ".weight");
-        conv_wgrad_layer(kind, x, operand(dz), a, rt.strict, 0, ws_alloc, s);
+        conv_wgrad_layer(kind, x, wgrad_operand(dz), a, rt.strict, 0, ws_alloc, s);
     };
     auto bias = [&](const View& dz, const std::string& key, const std::string& key2 = std::string()) {
         const long pixels = (long)dz.N * dz.H * dz.W;
@@ -686,11 +681,11 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
             // conv1 (and the skip, which the default mode folds into conv1's launch) against dout; conv0 against dh0.  The
             // operands: strict mode the normalised tensors the passes wrote; default mode the raw f16 tensors with the
             // normalisation the consumer conv applied (a down-sampling block's pooled operand comes from a pass)
-            const WgradOperand x1 = rt.f16 ? pending(t.h0, w.norm1, ACT_SILU_FAST, w.film0, f1) : operand(t.h2);
+            const WgradOperand x1 = rt.f16 ? pending(t.h0, w.norm1, ACT_SILU_FAST, w.film0, f1) : wgrad_operand(t.h2);
             wgrad(w.key + ".conv1", CONV_3x3, x1, dout);
-            if (w.has_skip) wgrad(w.key + ".skip", CONV_1x1, operand(t.x), dout);
+            if (w.has_skip) wgrad(w.key + ".skip", CONV_1x1, wgrad_operand(t.x), dout);
             bias(dout, w.key + ".conv1", w.has_skip ? w.key + ".skip" : std::string());
-            const WgradOperand x0 = (rt.f16 && mode != 2) ? pending(t.x, w.norm0, ACT_SILU_FAST, nullptr, nullptr) : operand(t.t0);
+            const WgradOperand x0 = (rt.f16 && mode != 2) ? pending(t.x, w.norm0, ACT_SILU_FAST, nullptr, nullptr) : wgrad_operand(t.t0);
             wgrad(w.key + ".conv0", mode == 1 ? CONV_UP2_3x3 : CONV_3x3, x0, dh0);
             bias(dh0, w.key + ".conv0");
         }
@@ -718,9 +713,9 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
         View dqkv = fresh(P, B, dout.H, dout.W, 3 * w.C);
         attention_backward(t.qkv, da, 8, dqkv, rt.scratch->alloc((size_t)B * 8 * 256 * 4), s);
         if (want_par) {
-            wgrad(w.key + ".conv", CONV_1x1, operand(t.a), dout);
+            wgrad(w.key + ".conv", CONV_1x1, wgrad_operand(t.a), dout);
             bias(dout, w.key + ".conv");
-            wgrad(w.key + ".qkv", CONV_1x1, rt.f16 ? pending(t.x, w.norm, ACT_NONE, nullptr, nullptr) : operand(t.t), dqkv);
+            wgrad(w.key + ".qkv", CONV_1x1, rt.f16 ? pending(t.x, w.norm, ACT_NONE, nullptr, nullptr) : wgrad_operand(t.t), dqkv);
             bias(dqkv, w.key + ".qkv");
         }
         View dn = fresh(P, B, dout.H, dout.W, w.C);
@@ -747,7 +742,7 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
         const View& f = tape.feat;
         float* coef = P->alloc((size_t)B * f.C * 2);
         norm_finalize(f, 32, last_n_.gamma, last_n_.beta, nullptr, nullptr, 0, coef, s);
-        WgradOperand x = operand(f);
+        WgradOperand x = wgrad_operand(f);
         x.xf = f.f16 ? WG_XF_FLOAT16 : WG_XF_FLOAT; x.act = f.f16 ? ACT_SILU_FAST : ACT_SILU;
         x.coef = reinterpret_cast<const float2*>(coef); x.coef_C = f.C;
         View dh7 = dh; dh7.C = 7;
@@ -795,12 +790,12 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
         gk = res_bwd(down_ds_[i - 1], 2, g_in, &e_ds, true);
     }
     if (want_par && !upscaler_) {    // first conv (the body morpher's: 4 input channels)
-        wgrad(p + "first_conv", CONV_3x3, operand(tape.x0), gk);
+        wgrad(p + "first_conv", CONV_3x3, wgrad_operand(tape.x0), gk);
         bias(gk, p + "first_conv");
     } else if (want_par) {           // the fused 16-channel first conv: body.first_conv on channels 0-3 of x0 (the rest image),
                                      // coarse_image_conv on 4-13 (posed, warped, grid); its bias is the sum of both
-        wgrad(p + "first_conv", CONV_3x3, operand(tape.x0.slice(0, 4)), gk);
-        wgrad("coarse_image_conv", CONV_3x3, operand(tape.x0.slice(4, 10)), gk);
+        wgrad(p + "first_conv", CONV_3x3, wgrad_operand(tape.x0.slice(0, 4)), gk);
+        wgrad("coarse_image_conv", CONV_3x3, wgrad_operand(tape.x0.slice(4, 10)), gk);
         bias(gk, p + "first_conv", "coarse_image_conv");
     }
     if (want_x0 && !upscaler_) {     // first conv: its data gradient joins the warp's image term in the epilogue

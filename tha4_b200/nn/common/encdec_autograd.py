@@ -26,7 +26,12 @@ from tha4_b200.nn.common.native_module import contiguous_grads, refuse_double_ba
 
 class Trainable:
     """Opt-in parameter gradients of the teacher modules (mixed into EyebrowDecomposer00, EyebrowMorphingCombiner00,
-    FaceMorpher08, Morpher00, Upscaler02)."""
+    FaceMorpher08, Morpher00, Upscaler02), and the dispatch of their forward.  Each module names its library calls once:
+    CTX_FORWARD / CTX_BACKWARD are its Context forward and backward methods, INPUT_GRADS the backward's keyword for the
+    gradient of each forward input, in input order."""
+    CTX_FORWARD = ''
+    CTX_BACKWARD = ''
+    INPUT_GRADS = ()
     _trainable = False
 
     def trainable_(self, mode: bool = True):
@@ -41,6 +46,13 @@ class Trainable:
         if not torch.is_grad_enabled():
             return False
         return any(t.requires_grad for t in inputs) or (self._trainable and any(p.requires_grad for p in self._params()))
+
+    def run_net(self, *inputs: Tensor) -> List[Tensor]:
+        """The network's outputs for its forward inputs: through _TeacherFunction when autograd needs a graph, otherwise the
+        plain library call."""
+        if self.wants_autograd(*inputs):
+            return list(_TeacherFunction.apply(self, *inputs, *self._params()))
+        return getattr(self.sync_weights(), self.CTX_FORWARD)(*inputs)
 
 
 def _param_grads(ctx, first: int, device):
@@ -73,185 +85,41 @@ def _empty_like(t: Tensor) -> Tensor:
     return torch.empty(t.shape, dtype=torch.float32, device=t.device)
 
 
-class _DecomposerFunction(torch.autograd.Function):
+class _TeacherFunction(torch.autograd.Function):
+    """apply(module, *inputs, *params): the module's forward inputs (len(module.INPUT_GRADS) of them), then its _params()."""
+
     @staticmethod
-    def forward(ctx, module, image: Tensor, *params: Tensor):
-        outs = module.sync_weights().eyebrow_decomposer(image)
+    def forward(ctx, module, *tensors: Tensor):
+        inputs = tensors[:len(module.INPUT_GRADS)]
+        outs = getattr(module.sync_weights(), module.CTX_FORWARD)(*inputs)
         ctx.set_materialize_grads(False)
         ctx.module = module
-        ctx.save_for_backward(image, *params)
+        ctx.save_for_backward(*tensors)
         return _own(outs)
 
     @staticmethod
     def backward(ctx, *grad_outputs):
-        refuse_double_backward('EyebrowDecomposer00')
-        return _decomposer_backward(ctx, *grad_outputs)
+        refuse_double_backward(type(ctx.module).__name__)
+        return _teacher_backward(ctx, *grad_outputs)
 
 
 @once_differentiable
-def _decomposer_backward(ctx, *grad_outputs):
-    image, *params = ctx.saved_tensors
-    none = (None,) * len(params)
+def _teacher_backward(ctx, *grad_outputs):
+    module = ctx.module
+    saved = ctx.saved_tensors
+    n = len(module.INPUT_GRADS)
+    inputs, want = saved[:n], ctx.needs_input_grad[1:1 + n]
+    nothing = (None,) * (1 + len(saved))
     if not any(ctx.needs_input_grad[1:]) or all(g is None for g in grad_outputs):
-        return (None, None) + none
-    ctx.lib = ctx.module.sync_weights()
-    flat, dp = _param_grads(ctx, 2, image.device)
-    if flat is None and not ctx.needs_input_grad[1]:
-        return (None, None) + none
-    d_image = _empty_like(image) if ctx.needs_input_grad[1] else None
-    ctx.lib.eyebrow_decomposer_backward(image, contiguous_grads(grad_outputs), d_image, d_params=flat)
-    return (None, d_image) + dp
-
-
-class _CombinerFunction(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, module, background_layer: Tensor, eyebrow_layer: Tensor, pose: Tensor, *params: Tensor):
-        outs = module.sync_weights().eyebrow_morphing_combiner(background_layer, eyebrow_layer, pose)
-        ctx.set_materialize_grads(False)
-        ctx.module = module
-        ctx.save_for_backward(background_layer, eyebrow_layer, pose, *params)
-        return _own(outs)
-
-    @staticmethod
-    def backward(ctx, *grad_outputs):
-        refuse_double_backward('EyebrowMorphingCombiner00')
-        return _combiner_backward(ctx, *grad_outputs)
-
-
-@once_differentiable
-def _combiner_backward(ctx, *grad_outputs):
-    background_layer, eyebrow_layer, pose, *params = ctx.saved_tensors
-    none = (None,) * len(params)
-    want = ctx.needs_input_grad[1:4]
-    if not any(ctx.needs_input_grad[1:]) or all(g is None for g in grad_outputs):
-        return (None, None, None, None) + none
-    ctx.lib = ctx.module.sync_weights()
-    flat, dp = _param_grads(ctx, 4, background_layer.device)
+        return nothing
+    ctx.lib = module.sync_weights()
+    flat, dp = _param_grads(ctx, 1 + n, inputs[0].device)
     if flat is None and not any(want):
-        return (None, None, None, None) + none
-    d_bg = _empty_like(background_layer) if want[0] else None
-    d_eb = _empty_like(eyebrow_layer) if want[1] else None
-    d_pose = _empty_like(pose) if want[2] else None
-    ctx.lib.eyebrow_morphing_combiner_backward(background_layer, eyebrow_layer, pose, contiguous_grads(grad_outputs),
-                                               d_background_layer=d_bg, d_eyebrow_layer=d_eb, d_pose=d_pose, d_params=flat)
-    return (None, d_bg, d_eb, d_pose) + dp
-
-
-class _FaceMorpherFunction(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, module, image: Tensor, pose: Tensor, *params: Tensor):
-        outs = module.sync_weights().face_morpher(image, pose)
-        ctx.set_materialize_grads(False)
-        ctx.module = module
-        ctx.save_for_backward(image, pose, *params)
-        return _own(outs)
-
-    @staticmethod
-    def backward(ctx, *grad_outputs):
-        refuse_double_backward('FaceMorpher08')
-        return _face_morpher_backward(ctx, *grad_outputs)
-
-
-@once_differentiable
-def _face_morpher_backward(ctx, *grad_outputs):
-    image, pose, *params = ctx.saved_tensors
-    none = (None,) * len(params)
-    want_image, want_pose = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
-    if not any(ctx.needs_input_grad[1:]) or all(g is None for g in grad_outputs):
-        return (None, None, None) + none
-    ctx.lib = ctx.module.sync_weights()
-    flat, dp = _param_grads(ctx, 3, image.device)
-    if flat is None and not (want_image or want_pose):
-        return (None, None, None) + none
-    d_image = _empty_like(image) if want_image else None
-    d_pose = _empty_like(pose) if want_pose else None
-    ctx.lib.face_morpher_backward(image, pose, contiguous_grads(grad_outputs), d_image=d_image, d_pose=d_pose, d_params=flat)
-    return (None, d_image, d_pose) + dp
-
-
-class _MorpherFunction(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, module, image: Tensor, pose: Tensor, *params: Tensor):
-        outs = module.sync_weights().morpher(image, pose)
-        ctx.set_materialize_grads(False)
-        ctx.module = module
-        ctx.save_for_backward(image, pose, *params)
-        return _own(outs)
-
-    @staticmethod
-    def backward(ctx, *grad_outputs):
-        refuse_double_backward('Morpher00')
-        return _morpher_backward(ctx, *grad_outputs)
-
-
-@once_differentiable
-def _morpher_backward(ctx, *grad_outputs):
-    image, pose, *params = ctx.saved_tensors
-    none = (None,) * len(params)
-    want_image, want_pose = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
-    if not any(ctx.needs_input_grad[1:]) or all(g is None for g in grad_outputs):
-        return (None, None, None) + none
-    ctx.lib = ctx.module.sync_weights()
-    flat, dp = _param_grads(ctx, 3, image.device)
-    if flat is None and not (want_image or want_pose):
-        return (None, None, None) + none
-    d_image = _empty_like(image) if want_image else None
-    d_pose = _empty_like(pose) if want_pose else None
+        return nothing
+    d = [_empty_like(t) if w else None for t, w in zip(inputs, want)]
+    grads = dict(zip(module.INPUT_GRADS, d))
     # d_params only from a trainable module: the plain one keeps the input-gradient call it always made
-    extra = {'d_params': flat} if ctx.module.is_trainable() else {}
-    ctx.lib.morpher_backward(image, pose, contiguous_grads(grad_outputs), d_image=d_image, d_pose=d_pose, **extra)
-    return (None, d_image, d_pose) + dp
-
-
-class _UpscalerFunction(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, module, rest_image: Tensor, coarse_posed_image: Tensor, coarse_grid_change: Tensor, pose: Tensor, *params: Tensor):
-        outs = module.sync_weights().upscaler(rest_image, coarse_posed_image, coarse_grid_change, pose)
-        ctx.set_materialize_grads(False)
-        ctx.module = module
-        ctx.save_for_backward(rest_image, coarse_posed_image, coarse_grid_change, pose, *params)
-        return _own(outs)
-
-    @staticmethod
-    def backward(ctx, *grad_outputs):
-        refuse_double_backward('Upscaler02')
-        return _upscaler_backward(ctx, *grad_outputs)
-
-
-@once_differentiable
-def _upscaler_backward(ctx, *grad_outputs):
-    rest_image, coarse_posed_image, coarse_grid_change, pose, *params = ctx.saved_tensors
-    none = (None,) * len(params)
-    want = ctx.needs_input_grad[1:5]
-    if not any(ctx.needs_input_grad[1:]) or all(g is None for g in grad_outputs):
-        return (None, None, None, None, None) + none
-    ctx.lib = ctx.module.sync_weights()
-    flat, dp = _param_grads(ctx, 5, rest_image.device)
-    if flat is None and not any(want):
-        return (None, None, None, None, None) + none
-    d = [_empty_like(t) if w else None for t, w in zip((rest_image, coarse_posed_image, coarse_grid_change, pose), want)]
-    # d_params only from a trainable module: the plain one keeps the input-gradient call it always made
-    extra = {'d_params': flat} if ctx.module.is_trainable() else {}
-    ctx.lib.upscaler_backward(rest_image, coarse_posed_image, coarse_grid_change, pose, contiguous_grads(grad_outputs),
-                              d_rest_image=d[0], d_coarse_posed=d[1], d_coarse_grid=d[2], d_pose=d[3], **extra)
+    if module.is_trainable():
+        grads['d_params'] = flat
+    getattr(ctx.lib, module.CTX_BACKWARD)(*inputs, contiguous_grads(grad_outputs), **grads)
     return (None, *d) + dp
-
-
-def eyebrow_decomposer(module, image: Tensor) -> List[Tensor]:
-    return list(_DecomposerFunction.apply(module, image, *module._params()))
-
-
-def eyebrow_morphing_combiner(module, background_layer: Tensor, eyebrow_layer: Tensor, pose: Tensor) -> List[Tensor]:
-    return list(_CombinerFunction.apply(module, background_layer, eyebrow_layer, pose, *module._params()))
-
-
-def face_morpher(module, image: Tensor, pose: Tensor) -> List[Tensor]:
-    return list(_FaceMorpherFunction.apply(module, image, pose, *module._params()))
-
-
-def morpher(module, image: Tensor, pose: Tensor) -> List[Tensor]:
-    return list(_MorpherFunction.apply(module, image, pose, *module._params()))
-
-
-def upscaler(module, rest_image: Tensor, coarse_posed_image: Tensor, coarse_grid_change: Tensor, pose: Tensor) -> List[Tensor]:
-    return list(_UpscalerFunction.apply(module, rest_image, coarse_posed_image, coarse_grid_change, pose, *module._params()))

@@ -11,15 +11,15 @@ from tha4_b200.nn.state_dict_spec import eyebrow_decomposer_spec
 
 class EyebrowDecomposer00(encdec_autograd.Trainable, NativeModule):
     NET_NAME = 'eyebrow_decomposer'
+    CTX_FORWARD, CTX_BACKWARD = 'eyebrow_decomposer', 'eyebrow_decomposer_backward'
+    INPUT_GRADS = ('d_image',)
 
     def __init__(self, args=None):
         super().__init__(eyebrow_decomposer_spec())
         self.args = args
 
     def forward(self, image: Tensor, *args) -> List[Tensor]:
-        if self.wants_autograd(image):
-            return encdec_autograd.eyebrow_decomposer(self, image)
-        return self.sync_weights().eyebrow_decomposer(image)
+        return self.run_net(image)
 
     EYEBROW_LAYER_INDEX = 0
     EYEBROW_LAYER_ALPHA_INDEX = 1

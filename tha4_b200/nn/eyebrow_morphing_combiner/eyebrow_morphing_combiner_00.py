@@ -11,15 +11,15 @@ from tha4_b200.nn.state_dict_spec import eyebrow_morphing_combiner_spec
 
 class EyebrowMorphingCombiner00(encdec_autograd.Trainable, NativeModule):
     NET_NAME = 'eyebrow_morphing_combiner'
+    CTX_FORWARD, CTX_BACKWARD = 'eyebrow_morphing_combiner', 'eyebrow_morphing_combiner_backward'
+    INPUT_GRADS = ('d_background_layer', 'd_eyebrow_layer', 'd_pose')
 
     def __init__(self, args=None):
         super().__init__(eyebrow_morphing_combiner_spec())
         self.args = args
 
     def forward(self, background_layer: Tensor, eyebrow_layer: Tensor, pose: Tensor, *args) -> List[Tensor]:
-        if self.wants_autograd(background_layer, eyebrow_layer, pose):
-            return encdec_autograd.eyebrow_morphing_combiner(self, background_layer, eyebrow_layer, pose)
-        return self.sync_weights().eyebrow_morphing_combiner(background_layer, eyebrow_layer, pose)
+        return self.run_net(background_layer, eyebrow_layer, pose)
 
     EYEBROW_IMAGE_INDEX = 0
     COMBINE_ALPHA_INDEX = 1

@@ -11,15 +11,15 @@ from tha4_b200.nn.state_dict_spec import face_morpher_spec
 
 class FaceMorpher08(encdec_autograd.Trainable, NativeModule):
     NET_NAME = 'face_morpher'
+    CTX_FORWARD, CTX_BACKWARD = 'face_morpher', 'face_morpher_backward'
+    INPUT_GRADS = ('d_image', 'd_pose')
 
     def __init__(self, args=None):
         super().__init__(face_morpher_spec())
         self.args = args
 
     def forward(self, image: Tensor, pose: Tensor, *args) -> List[Tensor]:
-        if self.wants_autograd(image, pose):
-            return encdec_autograd.face_morpher(self, image, pose)
-        return self.sync_weights().face_morpher(image, pose)
+        return self.run_net(image, pose)
 
     OUTPUT_IMAGE_INDEX = 0
     EYE_ALPHA_INDEX = 1

@@ -12,6 +12,8 @@ from tha4_b200.nn.state_dict_spec import body_morpher_spec
 
 class Morpher00(encdec_autograd.Trainable, NativeModule):
     NET_NAME = 'body_morpher'
+    CTX_FORWARD, CTX_BACKWARD = 'morpher', 'morpher_backward'
+    INPUT_GRADS = ('d_image', 'd_pose')
 
     def __init__(self, args=None):
         super().__init__(body_morpher_spec())
@@ -20,9 +22,7 @@ class Morpher00(encdec_autograd.Trainable, NativeModule):
     def forward(self, image: torch.Tensor, pose: torch.Tensor) -> List[Tensor]:
         assert len(image.shape) == 4 and image.shape[1:] == (4, 256, 256)     # morpher_00.py:43-49
         assert len(pose.shape) == 2 and image.shape[0] == pose.shape[0] and pose.shape[1] == 6
-        if self.wants_autograd(image, pose):
-            return encdec_autograd.morpher(self, image, pose)
-        return self.sync_weights().morpher(image, pose)
+        return self.run_net(image, pose)
 
     INDEX_MERGED = 0
     INDEX_ALPHA = 1

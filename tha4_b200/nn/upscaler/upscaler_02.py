@@ -17,6 +17,8 @@ from tha4_b200.nn.state_dict_spec import upscaler_spec
 
 class Upscaler02(encdec_autograd.Trainable, NativeModule):
     NET_NAME = 'upscaler'
+    CTX_FORWARD, CTX_BACKWARD = 'upscaler', 'upscaler_backward'
+    INPUT_GRADS = ('d_rest_image', 'd_coarse_posed', 'd_coarse_grid', 'd_pose')
 
     def __init__(self, args=None):
         super().__init__(upscaler_spec())
@@ -27,9 +29,7 @@ class Upscaler02(encdec_autograd.Trainable, NativeModule):
         assert len(rest_image.shape) == 4 and rest_image.shape[1:] == (4, 512, 512)       # upscaler_02.py:53-74
         assert coarse_posed_image.shape[0] == pose.shape[0] and coarse_grid_change.shape[1] == 2
         assert pose.shape[1] == 6
-        if self.wants_autograd(rest_image, coarse_posed_image, coarse_grid_change, pose):
-            return encdec_autograd.upscaler(self, rest_image, coarse_posed_image, coarse_grid_change, pose)
-        return self.sync_weights().upscaler(rest_image, coarse_posed_image, coarse_grid_change, pose)
+        return self.run_net(rest_image, coarse_posed_image, coarse_grid_change, pose)
 
     INDEX_MERGED = 0
     INDEX_ALPHA = 1
