@@ -403,6 +403,35 @@ int tha4_test_conv_backward_data_ex(tha4_ctx* ctx, int kind, const float* w, con
 /* linear_backward: dx[n][k] = SiLU'(pre[n][k]) sum_r dy[n][r] W[r][k] (pre NULL: no SiLU'), W [R][K] */
 int tha4_test_linear_backward(tha4_ctx* ctx, const float* dy, int dy_ld, int N, int R, const float* W, int K, const float* pre, int pre_ld,
                               float* dx, int dx_ld, void* stream);
+/* The parameter-gradient reductions of the network backwards, each through the launcher the networks call, on caller-owned
+ * device buffers.  accumulate = 1 adds to the outputs instead of overwriting them.
+ *
+ * group_norm_backward as tha4_test_group_norm_backward_ex, then the GroupNorm (+FiLM) parameter fold of its per-(n, c) sums:
+ * d_gamma / d_beta [C]; d_film0 (or NULL; needs film0): a row of d_film0_ld floats whose columns d_film0_off .. + 2C receive
+ * d(scale0) then d(shift0), written whatever accumulate says; no other column is touched. */
+int tha4_test_group_norm_param_grads(tha4_ctx* ctx, const void* x, int x_f16, int x_ld, int N, int C, int H, int W, int groups,
+                                     const double* stats, int stats_rep, int stats_ld, const float* gamma, const float* beta,
+                                     const float* film0, const float* film1, int film1_ld, int film1_off, int act, const float* dy,
+                                     int dy_ld, int dy_pool, const float* res, int res_ld, int res_mode, const float* add, int add_ld,
+                                     float* dx, int dx_ld, float* d_film, int d_film_ld, float* d_gamma, float* d_beta, float* d_film0,
+                                     int d_film0_ld, int d_film0_off, int accumulate, void* stream);
+/* norm_backward as tha4_test_norm_backward_ex, then the InstanceNorm parameter fold: d_gamma / d_beta [C]. */
+int tha4_test_norm_param_grads(tha4_ctx* ctx, const void* x, int x_f16, int x_ld, int N, int C, int H, int W, const double* stats,
+                               int stats_rep, int stats_ld, const float* gamma, const float* beta, int act, const float* dy, int dy_ld,
+                               float* dx, int dx_ld, float* d_gamma, float* d_beta, int accumulate, void* stream);
+/* Conv bias gradients: out[c] = sum over `pixels` rows of x [pixels][ld] of channel c < C; out2 (or NULL) gets the same. */
+int tha4_test_channel_sums(tha4_ctx* ctx, const float* x, int ld, int64_t pixels, int C, float* out, float* out2, int accumulate,
+                           void* stream);
+/* Dense layer weight gradients: dW [R][K] = sum_n dy[n][r] u(x[n][k]), db [R] = sum_n dy[n][r], u = SiLU if silu_x. */
+int tha4_test_linear_wgrad(tha4_ctx* ctx, const float* dy, int dy_ld, int N, int R, const float* x, int x_ld, int K, int silu_x,
+                           float* dW, float* db, int accumulate, void* stream);
+/* Encoder-decoder head biases: out[offsets[d]] = sum over the pixels of dh [pixels][16] of channel d < n <= 16; an offset
+ * below 0 skips its channel. */
+int tha4_test_head_bias(tha4_ctx* ctx, const float* dh, int64_t pixels, const int64_t* offsets, int n, float* out, int accumulate,
+                        void* stream);
+/* Encoder-decoder d(pose): dpose[n][k] = sum over the hw pixels of sample n < N of dbin [N][hw][ld] channel c0 + k, k < P. */
+int tha4_test_pose_sum(tha4_ctx* ctx, const float* dbin, int ld, int64_t hw, int c0, int P, int N, float* dpose, int dpose_ld,
+                       void* stream);
 /* The default-mode forward kernels in the layouts the networks run them, on caller-owned device buffers so that a test can
  * chain launches into one concatenation buffer.  Tensors are NHWC, given by a pointer to their channel 0 and a pixel stride;
  * statistics slots by a pointer to their first column, a per-sample column stride stats_ld, `rep` replicas and the replica

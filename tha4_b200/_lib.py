@@ -34,6 +34,8 @@ EXPORTED_SYMBOLS = [
     'tha4_test_conv_backward_data', 'tha4_test_norm_backward', 'tha4_test_tail_backward', 'tha4_test_upscaler_prologue_backward',
     'tha4_test_group_norm_backward', 'tha4_test_attention_backward',
     'tha4_test_group_norm_backward_ex', 'tha4_test_norm_backward_ex', 'tha4_test_conv_backward_data_ex', 'tha4_test_conv_wgrad', 'tha4_test_unet_wgrad', 'tha4_test_linear_backward',
+    'tha4_test_group_norm_param_grads', 'tha4_test_norm_param_grads', 'tha4_test_channel_sums', 'tha4_test_linear_wgrad',
+    'tha4_test_head_bias', 'tha4_test_pose_sum',
     'tha4_test_conv_forward_ex', 'tha4_test_tail_ex',
     'tha4_base_grid', 'tha4_test_conv', 'tha4_test_conv_norm', 'tha4_test_conv_norm_ex', 'tha4_test_conv_skip_fold', 'tha4_test_norm', 'tha4_test_tail', 'tha4_test_attention', 'tha4_test_linear',
     'tha4_test_siren_level', 'tha4_test_sine', 'tha4_test_siren_plan_check',

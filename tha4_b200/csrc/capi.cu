@@ -1463,6 +1463,84 @@ int tha4_test_linear_backward(tha4_ctx* ctx, const float* dy, int dy_ld, int N, 
     return guarded(ctx, [&] { linear_backward(dy, dy_ld, N, R, W, K, pre, pre_ld, dx, dx_ld, (cudaStream_t)stream); });
 }
 
+// ------------------------------------------------------------------------------------------------ parameter-gradient reductions
+// Each through the launcher the network backward calls, on the caller's buffers.
+int tha4_test_group_norm_param_grads(tha4_ctx* ctx, const void* x, int x_f16, int x_ld, int N, int C, int H, int W, int groups,
+                                     const double* stats, int stats_rep, int stats_ld, const float* gamma, const float* beta,
+                                     const float* film0, const float* film1, int film1_ld, int film1_off, int act, const float* dy,
+                                     int dy_ld, int dy_pool, const float* res, int res_ld, int res_mode, const float* add, int add_ld,
+                                     float* dx, int dx_ld, float* d_film, int d_film_ld, float* d_gamma, float* d_beta, float* d_film0,
+                                     int d_film0_ld, int d_film0_off, int accumulate, void* stream) {
+    return guarded(ctx, [&] {
+        cudaStream_t s = (cudaStream_t)stream;
+        THA4_REQUIRE(act == ACT_NONE || act == ACT_SILU, "test_group_norm_param_grads: act 0 or 2");
+        THA4_REQUIRE(res_mode >= RES_NONE && res_mode <= RES_DOWN2 && (res != nullptr) == (res_mode != RES_NONE),
+                     "test_group_norm_param_grads: res with res_mode 1..3, or neither");
+        THA4_REQUIRE(!d_film0 || (film0 && d_film0_off >= 0 && d_film0_off + 2 * C <= d_film0_ld),
+                     "test_group_norm_param_grads: d_film0 needs film0 and its 2C columns inside d_film0_ld");
+        begin_pass(ctx, s);
+        Runtime rt = make_rt(ctx, stream);
+        const View xin = stats_input(x, x_f16, x_ld, N, C, H, W, stats, stats_rep, stats_ld);
+        const View g = dy_pool ? nhwc_view(dy, N, H / 2, W / 2, C, dy_ld) : nhwc_view(dy, N, H, W, C, dy_ld);
+        const int rs = res_mode == RES_UP2 ? 2 : 1, rd = res_mode == RES_DOWN2 ? 2 : 1;
+        const View r = nhwc_view(res, N, H * rs / rd, W * rs / rd, C, res_ld);
+        const View a = nhwc_view(add, N, H, W, C, add_ld);
+        const float* f1 = film1 ? film1 + film1_off : nullptr;
+        double* sums = rt.alloc_stats((size_t)N * C * 2);
+        group_norm_backward(xin, groups, gamma, beta, film0, f1, film1_ld, act, g, dy_pool, nhwc_view(dx, N, H, W, C, dx_ld),
+                            d_film ? d_film + film1_off : nullptr, d_film_ld, res ? &r : nullptr, res_mode, add ? &a : nullptr, sums,
+                            ctx->persist.alloc((size_t)N * C * 8), s);
+        group_norm_param_fold(sums, N, C, gamma, beta, film0, f1, film1_ld, d_gamma, d_beta, d_film0 ? d_film0 + d_film0_off : nullptr,
+                              accumulate, s);
+    });
+}
+
+int tha4_test_norm_param_grads(tha4_ctx* ctx, const void* x, int x_f16, int x_ld, int N, int C, int H, int W, const double* stats,
+                               int stats_rep, int stats_ld, const float* gamma, const float* beta, int act, const float* dy, int dy_ld,
+                               float* dx, int dx_ld, float* d_gamma, float* d_beta, int accumulate, void* stream) {
+    return guarded(ctx, [&] {
+        cudaStream_t s = (cudaStream_t)stream;
+        THA4_REQUIRE(act == ACT_NONE || act == ACT_RELU, "test_norm_param_grads: act 0 or 1");
+        begin_pass(ctx, s);
+        Runtime rt = make_rt(ctx, stream);
+        double* sums = rt.alloc_stats((size_t)N * C * 2);
+        norm_backward(stats_input(x, x_f16, x_ld, N, C, H, W, stats, stats_rep, stats_ld), gamma, beta, act, nhwc_view(dy, N, H, W, C, dy_ld),
+                      nhwc_view(dx, N, H, W, C, dx_ld), sums, s);
+        norm_param_fold(sums, N, C, d_gamma, d_beta, accumulate, s);
+    });
+}
+
+int tha4_test_channel_sums(tha4_ctx* ctx, const float* x, int ld, int64_t pixels, int C, float* out, float* out2, int accumulate,
+                           void* stream) {
+    return guarded(ctx, [&] {
+        cudaStream_t s = (cudaStream_t)stream;
+        THA4_REQUIRE(pixels > 0 && C > 0 && ld >= C, "test_channel_sums: pixels > 0, 0 < C <= ld");
+        begin_pass(ctx, s);
+        double* part = reinterpret_cast<double*>(ctx->scratch.alloc((size_t)channel_sum_chunks(pixels) * C * 2));
+        channel_sums(x, ld, pixels, C, out, out2, accumulate, part, s);
+    });
+}
+
+int tha4_test_linear_wgrad(tha4_ctx* ctx, const float* dy, int dy_ld, int N, int R, const float* x, int x_ld, int K, int silu_x,
+                           float* dW, float* db, int accumulate, void* stream) {
+    return guarded(ctx, [&] { linear_wgrad(dy, dy_ld, N, R, x, x_ld, K, silu_x, dW, db, accumulate, (cudaStream_t)stream); });
+}
+
+int tha4_test_head_bias(tha4_ctx* ctx, const float* dh, int64_t pixels, const int64_t* offsets, int n, float* out, int accumulate,
+                        void* stream) {
+    return guarded(ctx, [&] {
+        THA4_REQUIRE(offsets != nullptr && n > 0 && n <= 16, "test_head_bias: 1..16 offsets");
+        long off[16];
+        for (int d = 0; d < n; ++d) off[d] = (long)offsets[d];
+        head_bias_sums(dh, pixels, off, n, out, accumulate, (cudaStream_t)stream);
+    });
+}
+
+int tha4_test_pose_sum(tha4_ctx* ctx, const float* dbin, int ld, int64_t hw, int c0, int P, int N, float* dpose, int dpose_ld,
+                       void* stream) {
+    return guarded(ctx, [&] { pose_sums(dbin, ld, hw, c0, P, N, dpose, dpose_ld, (cudaStream_t)stream); });
+}
+
 // One default-mode conv through conv_forward as run_conv_tc issues it, on the caller's own device buffers (views addressed by
 // a pointer to their channel 0, a pixel stride and, for statistics, a column stride and replicas).  Weights are packed as
 // the networks pack them: TF32-rounded, an f16 copy, and conv_make_fold when a 1x1 skip is given.

@@ -432,6 +432,25 @@ void tail_backward(TailKind kind, const float* const* outputs, const float* cons
     THA4_LAUNCH_CHECK();
 }
 
+void norm_param_fold(const double* sums, int N, int C, float* dgamma, float* dbeta, int accumulate, cudaStream_t s) {
+    norm_param_fold_kernel<<<ceil_div(C, 256), 256, 0, s>>>(sums, N, C, dgamma, dbeta, accumulate);
+    THA4_LAUNCH_CHECK();
+}
+
+void head_bias_sums(const float* dh, long pixels, const long* off, int n, float* out, int accumulate, cudaStream_t s) {
+    THA4_REQUIRE(n > 0 && n <= 16, "head bias: 1..16 head channels");
+    HeadBiasArgs hb;
+    hb.dh = dh; hb.pixels = pixels; hb.out = out; hb.accumulate = accumulate;
+    for (int d = 0; d < n; ++d) hb.off[d] = off[d];
+    head_bias_kernel<<<n, 256, 0, s>>>(hb);
+    THA4_LAUNCH_CHECK();
+}
+
+void pose_sums(const float* dbin, int ld, long hw, int c0, int P, int N, float* dpose, int dpose_ld, cudaStream_t s) {
+    pose_sum_kernel<<<N, round_up(P, 32), 0, s>>>(dbin, ld, hw, c0, P, dpose, dpose_ld);
+    THA4_LAUNCH_CHECK();
+}
+
 // ------------------------------------------------------------------------------------------------ EncDecNet
 void EncDecNet::load_adjoints(const StateDict& sd, const std::string& p, cudaStream_t s) {
     auto adj = [&](ConvWeights& cw, const std::string& key, ConvKind kind, int cout_kernel = 0) {
@@ -478,11 +497,9 @@ void EncDecNet::backward(Runtime& rt, const ImgView& image0, const ImgView& imag
         View dx = fresh(P, x.N, x.H, x.W, x.C);
         double* sums = rt.alloc_stats((size_t)x.N * x.C * 2);
         norm_backward(x, nw.gamma, nw.beta, act, dy, dx, sums, s);
-        if (want_par) {
-            norm_param_fold_kernel<<<ceil_div(x.C, 256), 256, 0, s>>>(sums, x.N, x.C, g.d_params + param_offset(key + ".weight"),
-                                                                      g.d_params + param_offset(key + ".bias"), g.accumulate_params);
-            THA4_LAUNCH_CHECK();
-        }
+        if (want_par)
+            norm_param_fold(sums, x.N, x.C, g.d_params + param_offset(key + ".weight"), g.d_params + param_offset(key + ".bias"),
+                            g.accumulate_params, s);
         return dx;
     };
     // ---- weight gradients.  An operand as the forward conv multiplied it: the stored tensor, or (default mode) an f16 raw
@@ -529,21 +546,20 @@ void EncDecNet::backward(Runtime& rt, const ImgView& image0, const ImgView& imag
         x.xf = f.f16 ? WG_XF_FLOAT16 : WG_XF_FLOAT; x.act = ACT_RELU; x.coef = coef; x.coef_C = f.C;
         WgradArgs a;
         WgradOperand d = operand(dh);
-        HeadBiasArgs hb; hb.dh = dh.p; hb.pixels = (long)B * S * S; hb.out = g.d_params; hb.accumulate = g.accumulate_params;
+        long bias_off[16];
         int ch = 0;
         for (size_t h = 0; h < head_key_.size(); ++h) {
             const long wo = param_offset(head_key_[h] + ".weight");
             auto bi = params_.off.find(head_key_[h] + ".bias");
             for (int co = 0; co < head_cout_[h]; ++co, ++ch) {
                 a.out_row[ch] = wo + (long)co * f.C * 9;
-                hb.off[ch] = bi == params_.off.end() ? -1 : bi->second + co;
+                bias_off[ch] = bi == params_.off.end() ? -1 : bi->second + co;
             }
         }
         a.n_map = ch; d.C = ch;
         a.out = g.d_params; a.accumulate = g.accumulate_params;
         conv_wgrad_layer(CONV_3x3, x, d, a, rt.strict, 0, ws_alloc, s);
-        head_bias_kernel<<<ch, 256, 0, s>>>(hb);
-        THA4_LAUNCH_CHECK();
+        head_bias_sums(dh.p, (long)B * S * S, bias_off, ch, g.d_params, g.accumulate_params, s);
     }
     // decoder
     View d = nbwd(tape.up[2], up_n_[2], ACT_RELU, df, blk("upsample_blocks.", 2, ".1"));
@@ -577,10 +593,7 @@ void EncDecNet::backward(Runtime& rt, const ImgView& image0, const ImgView& imag
         WgradOperand x = operand(tape.op_bott0, &down_n_[3], &tape.down[3]);     // pose planes pass through the transform
         wgrad(blk("bottleneck_blocks.", 0, ".0"), CONV_3x3, x, db, 512 + pose_ch_);
     }
-    if (want_pose) {
-        pose_sum_kernel<<<B, round_up(pose_ch_, 32), 0, s>>>(dbin.p, dbin.ld, (long)b * b, 512, pose_ch_, g.d_pose, g.d_pose_ld);
-        THA4_LAUNCH_CHECK();
-    }
+    if (want_pose) pose_sums(dbin.p, dbin.ld, (long)b * b, 512, pose_ch_, B, g.d_pose, g.d_pose_ld, s);
     if (!want_img && !want_par) return;
     // encoder (walked for its parameters also when no image gradient is wanted)
     d = nbwd(tape.down[3], down_n_[3], ACT_RELU, dbin.slice(0, 512), blk("downsample_blocks.", 3, ".1"));

@@ -248,4 +248,26 @@ void head_pack_adjoint(ConvWeights& cw, const TailWeights& tw, bool round_w, cud
 // cw.w with tracked_malloc; the values are those of fwd (TF32-rounded iff fwd's are).
 void conv_adjoint_from_packed(ConvWeights& cw, const ConvWeights& fwd, ConvKind kind, cudaStream_t s);
 
+// ------------------------------------------------------------------ parameter-gradient reductions (fp64, fixed order)
+// The launches the network backwards issue for their small parameter gradients.  accumulate: add to the outputs instead of
+// overwriting them.
+// GroupNorm (+FiLM) affine and time-FiLM gradients from group_norm_backward's per-(n, c) sums [N][C][2] (S1 = sum dz, S2 =
+// sum dz xhat): dgamma / dbeta [C]; dfilm0 (or null; needs film0): d(scale0) at [c], d(shift0) at [C + c], written, never
+// accumulated.  film1: row n at film1 + n * film1_ld, or null.
+void group_norm_param_fold(const double* sums, int N, int C, const float* gamma, const float* beta, const float* film0,
+                           const float* film1, int film1_ld, float* dgamma, float* dbeta, float* dfilm0, int accumulate, cudaStream_t s);
+// Per-channel sums of x [pixels][ld] (C channels) into out [C] and, if not null, the same values into out2 (conv biases);
+// part: channel_sum_chunks(pixels) * C doubles of workspace.
+int channel_sum_chunks(long pixels);
+void channel_sums(const float* x, int ld, long pixels, int C, float* out, float* out2, int accumulate, double* part, cudaStream_t s);
+// dW [R][K] = sum_n dy[n][r] u(x[n][k]), db [R] = sum_n dy[n][r]; u = SiLU when silu_x, else the identity.
+void linear_wgrad(const float* dy, int dy_ld, int N, int R, const float* x, int x_ld, int K, int silu_x, float* dW, float* db,
+                  int accumulate, cudaStream_t s);
+// InstanceNorm affine gradients from norm_backward's per-(n, c) sums: dgamma = sum_n S2, dbeta = sum_n S1.
+void norm_param_fold(const double* sums, int N, int C, float* dgamma, float* dbeta, int accumulate, cudaStream_t s);
+// Head biases: out[off[d]] = sum over the pixels of dh [pixels][16] channel d, for d < n <= 16; off[d] < 0 skips channel d.
+void head_bias_sums(const float* dh, long pixels, const long* off, int n, float* out, int accumulate, cudaStream_t s);
+// d(pose) of the encoder-decoders: dpose[n][k] = sum over the hw pixels of sample n of dbin[n][pixel][c0 + k], k < P, written.
+void pose_sums(const float* dbin, int ld, long hw, int c0, int P, int N, float* dpose, int dpose_ld, cudaStream_t s);
+
 }  // namespace tha4

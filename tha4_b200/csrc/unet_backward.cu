@@ -566,6 +566,28 @@ void linear_backward(const float* dy, int dy_ld, int N, int R, const float* W, i
     THA4_LAUNCH_CHECK();
 }
 
+void group_norm_param_fold(const double* sums, int N, int C, const float* gamma, const float* beta, const float* film0,
+                           const float* film1, int film1_ld, float* dgamma, float* dbeta, float* dfilm0, int accumulate, cudaStream_t s) {
+    gn_param_fold_kernel<<<ceil_div(C, 256), 256, 0, s>>>(sums, N, C, gamma, beta, film0, film1, film1_ld, dgamma, dbeta, dfilm0, accumulate);
+    THA4_LAUNCH_CHECK();
+}
+
+int channel_sum_chunks(long pixels) { return ceil_div(pixels, CS_CHUNK); }
+
+void channel_sums(const float* x, int ld, long pixels, int C, float* out, float* out2, int accumulate, double* part, cudaStream_t s) {
+    const int chunks = channel_sum_chunks(pixels);
+    channel_sum_partial_kernel<<<dim3(ceil_div(C, 32), chunks), 256, 0, s>>>(x, ld, pixels, C, part);
+    THA4_LAUNCH_CHECK();
+    channel_sum_finish_kernel<<<ceil_div(C, 256), 256, 0, s>>>(part, chunks, C, out, out2, accumulate);
+    THA4_LAUNCH_CHECK();
+}
+
+void linear_wgrad(const float* dy, int dy_ld, int N, int R, const float* x, int x_ld, int K, int silu_x, float* dW, float* db,
+                  int accumulate, cudaStream_t s) {
+    linear_wgrad_kernel<<<grid_for((long)R * K), 256, 0, s>>>(dy, dy_ld, N, R, x, x_ld, K, silu_x, dW, db, accumulate);
+    THA4_LAUNCH_CHECK();
+}
+
 // ------------------------------------------------------------------------------------------------ UNetNet
 void UNetNet::pack_adjoints(Runtime& rt) {
     SinkScope own(&owned_);
@@ -630,12 +652,9 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
         group_norm_backward(x, 32, nw.gamma, nw.beta, film0, film1, film1_total_, act, dy, dy_pool, dx,
                             film1 ? dfilm + (film1 - tape.film1) : nullptr, film1_total_, res, res_mode, add,
                             sums, rt.scratch->alloc((size_t)B * x.C * 8), s);
-        if (want_par) {
-            gn_param_fold_kernel<<<ceil_div(x.C, 256), 256, 0, s>>>(sums, B, x.C, nw.gamma, nw.beta, film0, film1, film1_total_,
-                                                                    par(key + ".weight"), par(key + ".bias"),
-                                                                    film0 ? dfilm0 + (film1 - tape.film1) : nullptr, acc);
-            THA4_LAUNCH_CHECK();
-        }
+        if (want_par)
+            group_norm_param_fold(sums, B, x.C, nw.gamma, nw.beta, film0, film1, film1_total_, par(key + ".weight"), par(key + ".bias"),
+                                  film0 ? dfilm0 + (film1 - tape.film1) : nullptr, acc, s);
     };
     // ---- parameter-gradient helpers ----
     const auto ws_alloc = [&](size_t n) { return rt.scratch->alloc(n); };
@@ -654,18 +673,11 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
     };
     auto bias = [&](const View& dz, const std::string& key, const std::string& key2 = std::string()) {
         const long pixels = (long)dz.N * dz.H * dz.W;
-        const int chunks = ceil_div(pixels, CS_CHUNK);
-        double* part = reinterpret_cast<double*>(rt.scratch->alloc((size_t)chunks * dz.C * 2));
-        channel_sum_partial_kernel<<<dim3(ceil_div(dz.C, 32), chunks), 256, 0, s>>>(dz.p, dz.ld, pixels, dz.C, part);
-        THA4_LAUNCH_CHECK();
-        channel_sum_finish_kernel<<<ceil_div(dz.C, 256), 256, 0, s>>>(part, chunks, dz.C, par(key + ".bias"),
-                                                                      key2.empty() ? nullptr : par(key2 + ".bias"), acc);
-        THA4_LAUNCH_CHECK();
+        double* part = reinterpret_cast<double*>(rt.scratch->alloc((size_t)channel_sum_chunks(pixels) * dz.C * 2));
+        channel_sums(dz.p, dz.ld, pixels, dz.C, par(key + ".bias"), key2.empty() ? nullptr : par(key2 + ".bias"), acc, part, s);
     };
     auto linear_wgrad = [&](const float* dy, int dy_ld, int N, int R, const float* x, int x_ld, int K, int silu_x, const std::string& key) {
-        linear_wgrad_kernel<<<grid_for((long)R * K), 256, 0, s>>>(dy, dy_ld, N, R, x, x_ld, K, silu_x, par(key + ".weight"),
-                                                                  par(key + ".bias"), acc);
-        THA4_LAUNCH_CHECK();
+        tha4::linear_wgrad(dy, dy_ld, N, R, x, x_ld, K, silu_x, par(key + ".weight"), par(key + ".bias"), acc, s);
     };
     // ResBlock: out = conv1(SiLU(FiLM(GN(h0)))) + skip(resample(x)),  h0 = conv0(resample(SiLU(GN(x)))).  Returns the gradient of x
     // (+ extra); with input_grad false it stops once the block's d(film1) is written.
