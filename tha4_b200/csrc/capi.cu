@@ -145,12 +145,26 @@ void teacher_chunk(tha4_ctx* ctx, Runtime& rt, int mode, const float* image, lon
 }
 
 struct OutSpec { int c, s; };
-const OutSpec kEncDecDecomposer[6] = {{4, 128}, {1, 128}, {4, 128}, {4, 128}, {1, 128}, {4, 128}};
-const OutSpec kCombiner[8] = {{4, 128}, {1, 128}, {4, 128}, {4, 128}, {1, 128}, {4, 128}, {4, 128}, {2, 128}};
-const OutSpec kFace[8] = {{4, 192}, {1, 192}, {4, 192}, {4, 192}, {1, 192}, {4, 192}, {4, 192}, {2, 192}};
 const OutSpec kSirenBody[5] = {{4, 512}, {1, 512}, {4, 512}, {4, 512}, {2, 512}};
 
-void fill_unet_spec(OutSpec* o, int S) { o[0] = {4, S}; o[1] = {1, S}; o[2] = {4, S}; o[3] = {2, S}; o[4] = {4, S}; }
+// The outputs of a teacher network, written at `spec`: its tail's (TAIL_OUTPUTS) at the network's resolution S.  Returns
+// their count.
+int teacher_spec(TailKind kind, int S, OutSpec* spec) {
+    const TailOutputs& t = TAIL_OUTPUTS[kind];
+    for (int i = 0; i < t.count; ++i) spec[i] = {t.ch[i], S};
+    return t.count;
+}
+
+// The teacher network of a THA4_NET_* id, without weights; other ids: nothing.
+void create_teacher(tha4_ctx* ctx, int net) {
+    switch (net) {
+        case THA4_NET_EYEBROW_DECOMPOSER: ctx->decomposer.reset(new EncDecNet(TAIL_DECOMPOSER, 128, 4, 0)); break;
+        case THA4_NET_EYEBROW_MORPHING_COMBINER: ctx->combiner.reset(new EncDecNet(TAIL_COMBINER, 128, 8, 12)); break;
+        case THA4_NET_FACE_MORPHER: ctx->face.reset(new EncDecNet(TAIL_FACE, 192, 4, 27)); break;
+        case THA4_NET_BODY_MORPHER: ctx->body.reset(new UNetNet(false, 256, 64, {1, 2, 4, 4, 4})); break;       // mode_07.py:210-226
+        case THA4_NET_UPSCALER: ctx->upscaler.reset(new UNetNet(true, 512, 32, {1, 2, 4, 8, 8, 8})); break;     // mode_07.py:241-257
+    }
+}
 
 StateDict make_sd(int n, const char* const* keys, const void* const* ptrs, const int64_t* shapes, const int* ndims) {
     StateDict sd;
@@ -183,9 +197,8 @@ void for_chunks(tha4_ctx* ctx, int B, int chunk, cudaStream_t stream, F&& fn) {
     }
 }
 
-template <int NOUT>
-void offset_outputs(float* const* outputs, const OutSpec* spec, int n0, float** dst) {
-    for (int i = 0; i < NOUT; ++i) dst[i] = outputs[i] + (size_t)n0 * spec[i].c * spec[i].s * spec[i].s;
+void offset_outputs(float* const* outputs, const OutSpec* spec, int n, int n0, float** dst) {
+    for (int i = 0; i < n; ++i) dst[i] = outputs[i] + (size_t)n0 * spec[i].c * spec[i].s * spec[i].s;
 }
 
 // frame n0 of a batch whose frames are `frame` elements apart; null stays null (an input or output that is not given)
@@ -193,9 +206,8 @@ template <typename T>
 T* at_frame(T* p, int n0, size_t frame) { return p ? p + (size_t)n0 * frame : nullptr; }
 
 // the upstream gradients of one micro-batch (an entry may be null)
-template <int NOUT>
-void offset_grads(const float* const* grads, const OutSpec* spec, int n0, const float** dst) {
-    for (int i = 0; i < NOUT; ++i) dst[i] = (grads && grads[i]) ? grads[i] + (size_t)n0 * spec[i].c * spec[i].s * spec[i].s : nullptr;
+void offset_grads(const float* const* grads, const OutSpec* spec, int n, int n0, const float** dst) {
+    for (int i = 0; i < n; ++i) dst[i] = (grads && grads[i]) ? grads[i] + (size_t)n0 * spec[i].c * spec[i].s * spec[i].s : nullptr;
 }
 
 
@@ -220,11 +232,7 @@ int tha4_ctx_create(int device, tha4_ctx** out) {
         ctx->stats_cap = (size_t)32 << 20;                      // 32 Mi doubles = 256 MB (enough for micro-batches of 32)
         THA4_CUDA_CHECK(cudaMalloc(&ctx->stats_base, ctx->stats_cap * sizeof(double)));
         THA4_CUDA_CHECK(cudaMemset(ctx->stats_base, 0, ctx->stats_cap * sizeof(double)));
-        ctx->decomposer.reset(new EncDecNet(TAIL_DECOMPOSER, 128, 4, 0));
-        ctx->combiner.reset(new EncDecNet(TAIL_COMBINER, 128, 8, 12));
-        ctx->face.reset(new EncDecNet(TAIL_FACE, 192, 4, 27));
-        ctx->body.reset(new UNetNet(false, 256, 64, {1, 2, 4, 4, 4}));           // mode_07.py:210-226
-        ctx->upscaler.reset(new UNetNet(true, 512, 32, {1, 2, 4, 8, 8, 8}));     // mode_07.py:241-257
+        for (int net = THA4_NET_EYEBROW_DECOMPOSER; net <= THA4_NET_UPSCALER; ++net) create_teacher(ctx, net);
         ctx->sface.reset(new SirenFaceNet());
         ctx->sbody.reset(new SirenBodyNet());
         *out = ctx;
@@ -308,12 +316,13 @@ int tha4_load_net(tha4_ctx* ctx, int net, int n_tensors, const char* const* keys
         cudaDeviceSynchronize();
         ctx->drop_graphs();                   // graphs hold pointers to the previous weights
         conv_set_pack_rounding(!ctx->opt.strict);     // non-strict: weights are rounded to TF32 once, at pack time
+        create_teacher(ctx, net);
         switch (net) {
-            case THA4_NET_EYEBROW_DECOMPOSER: ctx->decomposer.reset(new EncDecNet(TAIL_DECOMPOSER, 128, 4, 0)); ctx->decomposer->load(sd, s); break;
-            case THA4_NET_EYEBROW_MORPHING_COMBINER: ctx->combiner.reset(new EncDecNet(TAIL_COMBINER, 128, 8, 12)); ctx->combiner->load(sd, s); break;
-            case THA4_NET_FACE_MORPHER: ctx->face.reset(new EncDecNet(TAIL_FACE, 192, 4, 27)); ctx->face->load(sd, s); break;
-            case THA4_NET_BODY_MORPHER: ctx->body.reset(new UNetNet(false, 256, 64, {1, 2, 4, 4, 4})); ctx->body->load(sd, s); break;
-            case THA4_NET_UPSCALER: ctx->upscaler.reset(new UNetNet(true, 512, 32, {1, 2, 4, 8, 8, 8})); ctx->upscaler->load(sd, s); break;
+            case THA4_NET_EYEBROW_DECOMPOSER: ctx->decomposer->load(sd, s); break;
+            case THA4_NET_EYEBROW_MORPHING_COMBINER: ctx->combiner->load(sd, s); break;
+            case THA4_NET_FACE_MORPHER: ctx->face->load(sd, s); break;
+            case THA4_NET_BODY_MORPHER: ctx->body->load(sd, s); break;
+            case THA4_NET_UPSCALER: ctx->upscaler->load(sd, s); break;
             case THA4_NET_SIREN_FACE_MORPHER: ctx->sface.reset(new SirenFaceNet()); ctx->sface->load(sd, s); break;
             case THA4_NET_SIREN_BODY_MORPHER: ctx->sbody.reset(new SirenBodyNet()); ctx->sbody->load(sd, s); break;
             default: throw std::runtime_error("tha4: unknown network id");
@@ -325,8 +334,9 @@ int tha4_load_net(tha4_ctx* ctx, int net, int n_tensors, const char* const* keys
 int tha4_eyebrow_decomposer_forward(tha4_ctx* ctx, const float* image, int B, float* const* outputs, void* stream) {
     return guarded(ctx, [&] {
         Runtime rt = make_rt(ctx, stream);
+        OutSpec spec[TAIL_MAX_OUTPUTS]; const int nout = teacher_spec(TAIL_DECOMPOSER, 128, spec);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
-            float* o[6]; offset_outputs<6>(outputs, kEncDecDecomposer, n0, o);
+            float* o[TAIL_MAX_OUTPUTS]; offset_outputs(outputs, spec, nout, n0, o);
             ctx->decomposer->forward(rt, make_img(at_frame(image, n0, 4 * 128 * 128), b, 4, 128, 128), ImgView{}, nullptr, 0, o);
         });
     });
@@ -336,8 +346,9 @@ int tha4_eyebrow_morphing_combiner_forward(tha4_ctx* ctx, const float* backgroun
                                            const float* pose, int pose_ld, int B, float* const* outputs, void* stream) {
     return guarded(ctx, [&] {
         Runtime rt = make_rt(ctx, stream);
+        OutSpec spec[TAIL_MAX_OUTPUTS]; const int nout = teacher_spec(TAIL_COMBINER, 128, spec);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
-            float* o[8]; offset_outputs<8>(outputs, kCombiner, n0, o);
+            float* o[TAIL_MAX_OUTPUTS]; offset_outputs(outputs, spec, nout, n0, o);
             const size_t layer = 4 * 128 * 128;
             ctx->combiner->forward(rt, make_img(at_frame(eyebrow_layer, n0, layer), b, 4, 128, 128),
                                    make_img(at_frame(background_layer, n0, layer), b, 4, 128, 128), at_frame(pose, n0, pose_ld), pose_ld, o);
@@ -349,8 +360,9 @@ int tha4_face_morpher_forward(tha4_ctx* ctx, const float* image, const float* po
                               float* const* outputs, void* stream) {
     return guarded(ctx, [&] {
         Runtime rt = make_rt(ctx, stream);
+        OutSpec spec[TAIL_MAX_OUTPUTS]; const int nout = teacher_spec(TAIL_FACE, 192, spec);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
-            float* o[8]; offset_outputs<8>(outputs, kFace, n0, o);
+            float* o[TAIL_MAX_OUTPUTS]; offset_outputs(outputs, spec, nout, n0, o);
             ctx->face->forward(rt, make_img(at_frame(image, n0, 4 * 192 * 192), b, 4, 192, 192), ImgView{}, at_frame(pose, n0, pose_ld),
                                pose_ld, o);
         });
@@ -382,8 +394,9 @@ int tha4_eyebrow_decomposer_backward(tha4_ctx* ctx, const float* image, int B, c
         THA4_REQUIRE(d_image || d_params, "decomposer backward: no gradient requested");
         check_param_layout(d_params ? ctx->decomposer->param_count() : 0, THA4_NET_EYEBROW_DECOMPOSER, d_params);
         Runtime rt = make_rt(ctx, stream);
+        OutSpec spec[TAIL_MAX_OUTPUTS]; const int nout = teacher_spec(TAIL_DECOMPOSER, 128, spec);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
-            const float* g[6]; offset_grads<6>(grad_outputs, kEncDecDecomposer, n0, g);
+            const float* g[TAIL_MAX_OUTPUTS]; offset_grads(grad_outputs, spec, nout, n0, g);
             EncDecGrads eg; eg.grad_outputs = g; eg.d_image0 = at_frame(d_image, n0, 4 * 128 * 128);
             eg.d_params = d_params; eg.accumulate_params = n0 > 0;
             ctx->decomposer->backward(rt, make_img(at_frame(image, n0, 4 * 128 * 128), b, 4, 128, 128), ImgView{}, nullptr, 0, eg);
@@ -399,8 +412,9 @@ int tha4_eyebrow_morphing_combiner_backward(tha4_ctx* ctx, const float* backgrou
         check_param_layout(d_params ? ctx->combiner->param_count() : 0, THA4_NET_EYEBROW_MORPHING_COMBINER, d_params);
         THA4_REQUIRE(pose_ld >= 12, "combiner backward: pose rows need at least 12 entries");
         Runtime rt = make_rt(ctx, stream);
+        OutSpec spec[TAIL_MAX_OUTPUTS]; const int nout = teacher_spec(TAIL_COMBINER, 128, spec);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
-            const float* g[8]; offset_grads<8>(grad_outputs, kCombiner, n0, g);
+            const float* g[TAIL_MAX_OUTPUTS]; offset_grads(grad_outputs, spec, nout, n0, g);
             const size_t layer = 4 * 128 * 128;
             EncDecGrads eg; eg.grad_outputs = g;
             eg.d_image0 = at_frame(d_eyebrow_layer, n0, layer);
@@ -420,8 +434,9 @@ int tha4_face_morpher_backward(tha4_ctx* ctx, const float* image, const float* p
         check_param_layout(d_params ? ctx->face->param_count() : 0, THA4_NET_FACE_MORPHER, d_params);
         THA4_REQUIRE(pose_ld >= 27, "face morpher backward: pose rows need at least 27 entries");
         Runtime rt = make_rt(ctx, stream);
+        OutSpec spec[TAIL_MAX_OUTPUTS]; const int nout = teacher_spec(TAIL_FACE, 192, spec);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
-            const float* g[8]; offset_grads<8>(grad_outputs, kFace, n0, g);
+            const float* g[TAIL_MAX_OUTPUTS]; offset_grads(grad_outputs, spec, nout, n0, g);
             EncDecGrads eg; eg.grad_outputs = g;
             eg.d_image0 = at_frame(d_image, n0, 4 * 192 * 192);
             eg.d_pose = at_frame(d_pose, n0, 27); eg.d_pose_ld = 27;
@@ -436,9 +451,9 @@ int tha4_morpher_forward(tha4_ctx* ctx, const float* image, const float* pose, i
                          float* const* outputs, void* stream) {
     return guarded(ctx, [&] {
         Runtime rt = make_rt(ctx, stream);
-        OutSpec spec[5]; fill_unet_spec(spec, 256);
+        OutSpec spec[TAIL_MAX_OUTPUTS]; const int nout = teacher_spec(TAIL_UNET, 256, spec);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
-            float* o[5]; offset_outputs<5>(outputs, spec, n0, o);
+            float* o[TAIL_MAX_OUTPUTS]; offset_outputs(outputs, spec, nout, n0, o);
             ctx->body->forward(rt, make_img(at_frame(image, n0, 4 * 256 * 256), b, 4, 256, 256), nullptr, nullptr, 0,
                                at_frame(pose, n0, pose_ld), pose_ld, o);
         });
@@ -452,9 +467,9 @@ int tha4_morpher_backward(tha4_ctx* ctx, const float* image, const float* pose, 
         check_param_layout(d_params ? ctx->body->param_count() : 0, THA4_NET_BODY_MORPHER, d_params);
         THA4_REQUIRE(pose_ld >= 6, "morpher backward: pose rows need at least 6 entries");
         Runtime rt = make_rt(ctx, stream);
-        OutSpec spec[5]; fill_unet_spec(spec, 256);
+        OutSpec spec[TAIL_MAX_OUTPUTS]; const int nout = teacher_spec(TAIL_UNET, 256, spec);
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
-            const float* g[5]; offset_grads<5>(grad_outputs, spec, n0, g);
+            const float* g[TAIL_MAX_OUTPUTS]; offset_grads(grad_outputs, spec, nout, n0, g);
             UNetGrads ug; ug.grad_outputs = g;
             ug.d_image = at_frame(d_image, n0, 4 * 256 * 256);
             ug.d_pose = at_frame(d_pose, n0, 6); ug.d_pose_ld = 6;
@@ -476,11 +491,11 @@ int tha4_upscaler_backward(tha4_ctx* ctx, const float* rest_image, const float* 
         THA4_REQUIRE(coarse_size == 256 || coarse_size == 512, "upscaler backward: coarse_size must be 256 or 512");
         THA4_REQUIRE(pose_ld >= 6, "upscaler backward: pose rows need at least 6 entries");
         Runtime rt = make_rt(ctx, stream);
-        OutSpec spec[5]; fill_unet_spec(spec, 512);
+        OutSpec spec[TAIL_MAX_OUTPUTS]; const int nout = teacher_spec(TAIL_UNET, 512, spec);
         const size_t hw = 512 * 512, chw = (size_t)coarse_size * coarse_size;
         const int max_batch = d_params ? UPSCALER_PARAM_BWD_MAX_BATCH : UPSCALER_BWD_MAX_BATCH;
         for_chunks(ctx, B, std::min(ctx->opt.microbatch, max_batch), rt.stream, [&](int n0, int b) {
-            const float* g[5]; offset_grads<5>(grad_outputs, spec, n0, g);
+            const float* g[TAIL_MAX_OUTPUTS]; offset_grads(grad_outputs, spec, nout, n0, g);
             UNetGrads ug; ug.grad_outputs = g;
             ug.d_image = at_frame(d_rest_image, n0, 4 * hw);
             ug.d_coarse_posed = at_frame(d_coarse_posed_image, n0, 4 * chw);
@@ -498,10 +513,10 @@ int tha4_upscaler_forward(tha4_ctx* ctx, const float* rest_image, const float* c
                           float* const* outputs, void* stream) {
     return guarded(ctx, [&] {
         Runtime rt = make_rt(ctx, stream);
-        OutSpec spec[5]; fill_unet_spec(spec, 512);
+        OutSpec spec[TAIL_MAX_OUTPUTS]; const int nout = teacher_spec(TAIL_UNET, 512, spec);
         const size_t hw = 512 * 512, chw = (size_t)coarse_size * coarse_size;
         for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
-            float* o[5]; offset_outputs<5>(outputs, spec, n0, o);
+            float* o[TAIL_MAX_OUTPUTS]; offset_outputs(outputs, spec, nout, n0, o);
             ctx->upscaler->forward(rt, make_img(at_frame(rest_image, n0, 4 * hw), b, 4, 512, 512), at_frame(coarse_posed_image, n0, 4 * chw),
                                    at_frame(coarse_grid_change, n0, 2 * chw), coarse_size, at_frame(pose, n0, pose_ld), pose_ld, o);
         });
@@ -534,23 +549,22 @@ int tha4_teacher_forward(tha4_ctx* ctx, int mode, const float* image, int64_t im
         const long img_sn = (long)image_batch_stride;
         Runtime rt = make_rt(ctx, stream);
         OutSpec spec[33];
-        int n = 0;
+        int nout = 0;
         if (mode == 7) {
-            fill_unet_spec(spec, 512); n = 5;
-            spec[n++] = {4, 512};
-            fill_unet_spec(spec + n, 256); n += 5;
+            nout += teacher_spec(TAIL_UNET, 512, spec + nout);
+            spec[nout++] = {4, 512};                         // face_morphed_full
+            nout += teacher_spec(TAIL_UNET, 256, spec + nout);
         }
-        for (int i = 0; i < 8; ++i) spec[n++] = kFace[i];
-        for (int i = 0; i < 8; ++i) spec[n++] = kCombiner[i];
-        for (int i = 0; i < 6; ++i) spec[n++] = kEncDecDecomposer[i];
-        const int nout = n;
+        nout += teacher_spec(TAIL_FACE, 192, spec + nout);
+        nout += teacher_spec(TAIL_COMBINER, 128, spec + nout);
+        nout += teacher_spec(TAIL_DECOMPOSER, 128, spec + nout);
         auto run = [&](const float* img_p, const float* pose_p, float* const* outs, const float* const* cached_p) {
             for_chunks(ctx, B, ctx->opt.microbatch, rt.stream, [&](int n0, int b) {
                 float* o[33];
                 for (int i = 0; i < nout; ++i) o[i] = outs[i] ? outs[i] + (size_t)n0 * spec[i].c * spec[i].s * spec[i].s : nullptr;
                 const float* cd[6];
                 if (cached_p)
-                    for (int i = 0; i < 6; ++i) cd[i] = cached_p[i] + (size_t)n0 * kEncDecDecomposer[i].c * 128 * 128;
+                    for (int i = 0; i < 6; ++i) cd[i] = cached_p[i] + (size_t)n0 * TAIL_OUTPUTS[TAIL_DECOMPOSER].ch[i] * 128 * 128;
                 teacher_chunk(ctx, rt, mode, img_p + (size_t)n0 * img_sn, img_sn, pose_p + (size_t)n0 * 45, b, o,
                               eyebrow_morphed_image_index, cached_p ? cd : nullptr);
             });
@@ -773,7 +787,7 @@ int tha4_siren_morpher_backward(tha4_ctx* ctx, const float* image, const float* 
         if (grads) THA4_CUDA_CHECK(cudaMemsetAsync(grads, 0, siren_body_param_count() * sizeof(float), rt.stream));
         constexpr size_t hw = 512 * 512;
         for_chunks(ctx, B, SIREN_BODY_MAX_BATCH, rt.stream, [&](int n0, int b) {     // micro-batches accumulate into grads
-            const float* g[5]; offset_grads<5>(grad_outputs, kSirenBody, n0, g);
+            const float* g[5]; offset_grads(grad_outputs, kSirenBody, 5, n0, g);
             if (siren)
                 siren_body_backward(rt, make_img(image + (size_t)n0 * 4 * hw, b, 4, 512, 512), pose + (size_t)n0 * pose_ld, pose_ld, g,
                                     params, grads, d_pose ? d_pose + (size_t)n0 * 45 : nullptr);

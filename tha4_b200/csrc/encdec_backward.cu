@@ -336,14 +336,6 @@ __global__ void __launch_bounds__(256) tail_bwd_kernel(const TailBwdArgs a) {
     }
 }
 
-int grid_for(long n) { return (int)std::max<long>(1, std::min<long>((n + 255) / 256, 132L * 16)); }
-
-View fresh(Pool* P, int N, int H, int W, int C) {
-    View v; v.N = N; v.H = H; v.W = W; v.C = C; v.ld = C;
-    v.p = P->alloc((size_t)N * H * W * C);
-    return v;
-}
-
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------ shared entry points
@@ -361,7 +353,7 @@ void head_pack_adjoint(ConvWeights& cw, const TailWeights& tw, bool round_w, cud
     cw.w = reinterpret_cast<float*>(tracked_malloc(conv_packed_floats(cw) * sizeof(float)));
     THA4_CUDA_CHECK(cudaMemsetAsync(cw.w, 0, conv_packed_floats(cw) * sizeof(float), s));
     cw.tf32_rounded = round_w;
-    head_adjoint_pack_kernel<<<grid_for(9L * tw.C * tw.CO), 256, 0, s>>>(cw.w, tw.w, tw.C, tw.CO, cw.cin_pad, cw.cout_pad, round_w ? 1 : 0);
+    head_adjoint_pack_kernel<<<backward_grid(9L * tw.C * tw.CO), 256, 0, s>>>(cw.w, tw.w, tw.C, tw.CO, cw.cin_pad, cw.cout_pad, round_w ? 1 : 0);
     THA4_LAUNCH_CHECK();
 }
 
@@ -380,7 +372,7 @@ void conv_pack_adjoint(ConvWeights& cw, ConvKind kind, const float* w_ref, int c
         const size_t n = (size_t)oc * cout * 9;
         THA4_CUDA_CHECK(cudaMalloc(&tmp, n * sizeof(float)));
         THA4_CUDA_CHECK(cudaMemsetAsync(tmp, 0, n * sizeof(float), s));
-        adjoint3x3_kernel<<<grid_for((long)cout * cin * 9), 256, 0, s>>>(tmp, w_ref, cout, cin);
+        adjoint3x3_kernel<<<backward_grid((long)cout * cin * 9), 256, 0, s>>>(tmp, w_ref, cout, cin);
         THA4_LAUNCH_CHECK();
         conv_pack(cw, CONV_3x3, tmp, cout, 0, s);
         THA4_CUDA_CHECK(cudaStreamSynchronize(s));
@@ -407,11 +399,11 @@ void norm_backward(const View& x, const float* gamma, const float* beta, int act
     if (x.f16) {
         norm_bwd_reduce_kernel<true><<<g1, 256, 0, s>>>(a);
         THA4_LAUNCH_CHECK();
-        norm_bwd_apply_kernel<true><<<grid_for(total), 256, 0, s>>>(a, total);
+        norm_bwd_apply_kernel<true><<<backward_grid(total), 256, 0, s>>>(a, total);
     } else {
         norm_bwd_reduce_kernel<false><<<g1, 256, 0, s>>>(a);
         THA4_LAUNCH_CHECK();
-        norm_bwd_apply_kernel<false><<<grid_for(total), 256, 0, s>>>(a, total);
+        norm_bwd_apply_kernel<false><<<backward_grid(total), 256, 0, s>>>(a, total);
     }
     THA4_LAUNCH_CHECK();
 }
@@ -420,15 +412,15 @@ void tail_backward(TailKind kind, const float* const* outputs, const float* cons
                    const View& dh, float* d0, float* d1, int dld, cudaStream_t s) {
     THA4_REQUIRE(dh.C == 16 && dh.ld == 16 && dh.H == image0.H && dh.W == image0.W && image0.H == image0.W, "tail backward: dims");
     TailBwdArgs a;
-    const int nout = kind == TAIL_UNET ? 5 : (kind == TAIL_DECOMPOSER ? 6 : 8);
+    const int nout = TAIL_OUTPUTS[kind].count;
     for (int k = 0; k < 8; ++k) { a.out[k] = k < nout ? outputs[k] : nullptr; a.g[k] = (grads && k < nout) ? grads[k] : nullptr; }
     a.img0 = image0; a.img1 = image1; a.base = base_grid_table(image0.H);
     a.S = image0.H; a.N = dh.N; a.dh = dh.p; a.d0 = d0; a.d1 = d1; a.dld = dld;
     const long total = (long)a.N * a.S * a.S;
-    if (kind == TAIL_UNET) tail_bwd_kernel<TAIL_UNET><<<grid_for(total), 256, 0, s>>>(a);
-    else if (kind == TAIL_DECOMPOSER) tail_bwd_kernel<TAIL_DECOMPOSER><<<grid_for(total), 256, 0, s>>>(a);
-    else if (kind == TAIL_COMBINER) tail_bwd_kernel<TAIL_COMBINER><<<grid_for(total), 256, 0, s>>>(a);
-    else tail_bwd_kernel<TAIL_FACE><<<grid_for(total), 256, 0, s>>>(a);
+    if (kind == TAIL_UNET) tail_bwd_kernel<TAIL_UNET><<<backward_grid(total), 256, 0, s>>>(a);
+    else if (kind == TAIL_DECOMPOSER) tail_bwd_kernel<TAIL_DECOMPOSER><<<backward_grid(total), 256, 0, s>>>(a);
+    else if (kind == TAIL_COMBINER) tail_bwd_kernel<TAIL_COMBINER><<<backward_grid(total), 256, 0, s>>>(a);
+    else tail_bwd_kernel<TAIL_FACE><<<backward_grid(total), 256, 0, s>>>(a);
     THA4_LAUNCH_CHECK();
 }
 
@@ -485,10 +477,9 @@ void EncDecNet::backward(Runtime& rt, const ImgView& image0, const ImgView& imag
     Pool* P = rt.persist;
 
     // forward, keeping the activations (its outputs are what the tail backward differentiates through)
-    static const int kChDec[6] = {4, 1, 4, 4, 1, 4}, kCh8[8] = {4, 1, 4, 4, 1, 4, 4, 2};
-    const int* ch = kind_ == TAIL_DECOMPOSER ? kChDec : kCh8;
-    float* outs[8] = {};
-    for (int k = 0; k < num_outputs(); ++k) outs[k] = P->alloc((size_t)B * ch[k] * S * S);
+    const TailOutputs& to = TAIL_OUTPUTS[kind_];
+    float* outs[TAIL_MAX_OUTPUTS] = {};
+    for (int k = 0; k < to.count; ++k) outs[k] = P->alloc((size_t)B * to.ch[k] * S * S);
     EncDecTape tape;
     forward(rt, image0, image1, pose, pose_ld, outs, &tape);
 

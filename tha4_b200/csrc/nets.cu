@@ -102,21 +102,34 @@ int stats_rep_cap() {
     return cap;
 }
 
-// rt != nullptr: the view also gets a (zeroed) statistics slot, to be filled by the conv that produces the tensor
-View make_view(Pool* pool, int N, int H, int W, int C, Runtime* rt = nullptr) {
+// gives `v` (its geometry set) a zeroed statistics slot: replicas ~ tiles/16 (128-pixel conv tiles per sample), a power of
+// two in [1, stats_rep_cap()]
+void add_stats(View& v, Runtime& rt) {
+    const int tiles = ((v.W + 15) / 16) * ((v.H + 7) / 8);
+    int rep = 1;
+    while (rep < stats_rep_cap() && rep * 32 <= tiles) rep *= 2;
+    v.stats_rep = rep;
+    v.stats_rep_stride = (long)v.N * v.C * 2;
+    v.stats = rt.alloc_stats((size_t)rep * v.N * v.C * 2);
+    v.stats_ld = v.C;
+}
+
+// `data` with the statistics slot of `slot`, another view of the same tensor
+View with_stats(View data, const View& slot) {
+    data.stats = slot.stats; data.stats_ld = slot.stats_ld; data.stats_rep = slot.stats_rep; data.stats_rep_stride = slot.stats_rep_stride;
+    return data;
+}
+
+}  // namespace
+
+View make_view(Pool* pool, int N, int H, int W, int C, Runtime* rt) {
     View v; v.N = N; v.H = H; v.W = W; v.C = C; v.ld = C;
     v.p = pool->alloc((size_t)N * H * W * C);
-    if (rt) {   // replicas ~ tiles/16 (128-pixel conv tiles per sample), power of two in [1, 16]
-        const int tiles = ((W + 15) / 16) * ((H + 7) / 8);
-        int rep = 1;
-        while (rep < stats_rep_cap() && rep * 32 <= tiles) rep *= 2;
-        v.stats_rep = rep;
-        v.stats_rep_stride = (long)N * C * 2;
-        v.stats = rt->alloc_stats((size_t)rep * N * C * 2);
-        v.stats_ld = C;
-    }
+    if (rt) add_stats(v, *rt);
     return v;
 }
+
+namespace {
 
 // f16 activation tensor (conv operand produced by a normalisation layer; see View::f16)
 View make_view16(Pool* pool, int N, int H, int W, int C) {
@@ -162,18 +175,9 @@ struct Tens { View f; View h; };
 
 Tens make_act(Pool* pool, Runtime& rt, int N, int H, int W, int C, bool want_f32, bool want_f16, bool stats = true) {
     Tens a;
-    if (want_f32) a.f = make_view(pool, N, H, W, C, stats ? &rt : nullptr);
-    else {
-        View v; v.N = N; v.H = H; v.W = W; v.C = C; v.ld = C;
-        if (stats) {   // same replica rule as make_view
-            const int tiles = ((W + 15) / 16) * ((H + 7) / 8);
-            int rep = 1;
-            while (rep < stats_rep_cap() && rep * 32 <= tiles) rep *= 2;
-            v.stats_rep = rep; v.stats_rep_stride = (long)N * C * 2;
-            v.stats = rt.alloc_stats((size_t)rep * N * C * 2); v.stats_ld = C;
-        }
-        a.f = v;
-    }
+    if (want_f32) a.f = make_view(pool, N, H, W, C);
+    else { a.f.N = N; a.f.H = H; a.f.W = W; a.f.C = C; a.f.ld = C; }
+    if (stats) add_stats(a.f, rt);
     if (want_f16) a.h = make_view16(pool, N, H, W, C);
     return a;
 }
@@ -189,12 +193,7 @@ Tens slice_act(const Tens& a, int c0, int c) {
 }
 
 // the data (fp32 copy if there is one, else the f16 copy) and the statistics slot of a raw conv output
-View raw_view(const Tens& a) {
-    if (a.f.p) return a.f;
-    View v = a.h;
-    v.stats = a.f.stats; v.stats_ld = a.f.stats_ld; v.stats_rep = a.f.stats_rep; v.stats_rep_stride = a.f.stats_rep_stride;
-    return v;
-}
+View raw_view(const Tens& a) { return a.f.p ? a.f : with_stats(a.h, a.f); }
 
 // pending normalisation of `src` (its statistics) with the weights of the layer that follows it in the reference graph
 ConvNormIn norm_in(const View& src_stats, const NormW& nw, int groups, int act, const float* film0 = nullptr,
@@ -318,55 +317,50 @@ void EncDecNet::forward(Runtime& rt, const ImgView& image0, const ImgView& image
     }
     if (tape) tape->x0 = x0;
     if (rt.f16) { forward_fused(rt, x0, image0, image1, pose, pose_ld, outputs, tape); return; }
-    // conv -> InstanceNorm -> ReLU; the activated tensor goes to `dst`, or to a fresh f16 tensor when its only consumer is
-    // a wgmma conv (to16), or back in place (out of place when a backward keeps the raw output: `keep`)
-    const bool h16 = false;
-    auto conv_in_relu = [&](const ConvWeights& cw, const NormW& nw, const View& in, int oh, const View* dst, bool to16,
-                            View* keep = nullptr) -> View {
+    // conv -> InstanceNorm -> ReLU; the activated tensor goes to `dst`, or back in place (out of place when a backward keeps
+    // the raw output: `keep`)
+    auto conv_in_relu = [&](const ConvWeights& cw, const NormW& nw, const View& in, int oh, const View* dst, View* keep) -> View {
         View raw = make_view(P, B, oh, oh, cw.cout, &rt);
         run_conv(rt, cw, in, raw);
-        const View y = dst ? *dst : (to16 ? make_view16(P, B, oh, oh, cw.cout) : (keep ? make_view(P, B, oh, oh, cw.cout) : raw));
+        const View y = dst ? *dst : (keep ? make_view(P, B, oh, oh, cw.cout) : raw);
         run_norm(rt, raw, nw, 0, nullptr, nullptr, 0, ACT_RELU, 0, nullptr, y);
         if (keep) *keep = raw;
         return y;
     };
-    View f = conv_in_relu(down_[0], down_n_[0], x0, S_, nullptr, false, tape ? &tape->down[0] : nullptr);       // the stride-2 convs read fp32
+    View f = conv_in_relu(down_[0], down_n_[0], x0, S_, nullptr, tape ? &tape->down[0] : nullptr);
     if (tape) { tape->op_down[0] = x0; tape->op_down[1] = f; }
-    f = conv_in_relu(down_[1], down_n_[1], f, S_ / 2, nullptr, false, tape ? &tape->down[1] : nullptr);
+    f = conv_in_relu(down_[1], down_n_[1], f, S_ / 2, nullptr, tape ? &tape->down[1] : nullptr);
     if (tape) tape->op_down[2] = f;
-    f = conv_in_relu(down_[2], down_n_[2], f, S_ / 4, nullptr, false, tape ? &tape->down[2] : nullptr);
+    f = conv_in_relu(down_[2], down_n_[2], f, S_ / 4, nullptr, tape ? &tape->down[2] : nullptr);
     if (tape) tape->op_down[3] = f;
     const int b = S_ / 8;
-    View bin = h16 ? make_view16(P, B, b, b, 512 + pose_pad_) : make_view(P, B, b, b, 512 + pose_pad_);
+    View bin = make_view(P, B, b, b, 512 + pose_pad_);
     View bfeat = bin.slice(0, 512);
-    conv_in_relu(down_[3], down_n_[3], f, b, &bfeat, false, tape ? &tape->down[3] : nullptr);
+    conv_in_relu(down_[3], down_n_[3], f, b, &bfeat, tape ? &tape->down[3] : nullptr);
     if (pose_pad_ > 0) tile_vector(pose, pose_ld, pose_ch_, bin.slice(512, pose_pad_), s);   // poser_encoder_decoder_00.py:110-113
-    // the bottleneck stream x is both a residual (fp32) and a conv operand (f16 copy x16)
-    View x = make_view(P, B, b, b, bott0_.cout, &rt), x16;
+    View x = make_view(P, B, b, b, bott0_.cout, &rt);
     run_conv(rt, bott0_, bin, x);
     if (tape) tape->op_bott0 = bin;
-    if (h16) x16 = make_view16(P, B, b, b, bott0_.cout);
     {
         const View y = tape ? make_view(P, B, b, b, bott0_.cout) : x;
-        run_norm(rt, x, bott0_n_, 0, nullptr, nullptr, 0, ACT_RELU, 0, nullptr, y, h16 ? &x16 : nullptr);
+        run_norm(rt, x, bott0_n_, 0, nullptr, nullptr, 0, ACT_RELU, 0, nullptr, y);
         if (tape) tape->bott0 = x;
         x = y;
     }
     for (int i = 0; i < 5; ++i) {   // ResnetBlock: x + IN(conv(relu(IN(conv(x)))))  (resnet_block.py:52-67)
-        View h = conv_in_relu(res_[i][0], res_n_[i][0], h16 ? x16 : x, b, nullptr, h16, tape ? &tape->res[i][0] : nullptr);
+        View h = conv_in_relu(res_[i][0], res_n_[i][0], x, b, nullptr, tape ? &tape->res[i][0] : nullptr);
         if (tape) { tape->op_res[i][0] = x; tape->op_res[i][1] = h; }
         View raw = make_view(P, B, b, b, 512, &rt);
         run_conv(rt, res_[i][1], h, raw);
-        View n16; if (h16) n16 = make_view16(P, B, b, b, 512);
         const View y = tape ? make_view(P, B, b, b, 512) : raw;
-        run_norm(rt, raw, res_n_[i][1], 0, nullptr, nullptr, 0, ACT_NONE, 0, &x, y, h16 ? &n16 : nullptr);
+        run_norm(rt, raw, res_n_[i][1], 0, nullptr, nullptr, 0, ACT_NONE, 0, &x, y);
         if (tape) tape->res[i][1] = raw;
-        x = y; x16 = n16;
+        x = y;
     }
     if (tape) tape->op_up[0] = x;
-    x = conv_in_relu(up_[0], up_n_[0], h16 ? x16 : x, b * 2, nullptr, h16, tape ? &tape->up[0] : nullptr);
+    x = conv_in_relu(up_[0], up_n_[0], x, b * 2, nullptr, tape ? &tape->up[0] : nullptr);
     if (tape) tape->op_up[1] = x;
-    x = conv_in_relu(up_[1], up_n_[1], x, b * 4, nullptr, h16, tape ? &tape->up[1] : nullptr);
+    x = conv_in_relu(up_[1], up_n_[1], x, b * 4, nullptr, tape ? &tape->up[1] : nullptr);
     if (tape) tape->op_up[2] = x;
     // last block: leave InstanceNorm + ReLU pending; the tail kernel applies them while staging its halo tile
     View raw = make_view(P, B, S_, S_, 64, &rt);
@@ -448,8 +442,7 @@ void EncDecNet::forward_fused(Runtime& rt, const View& x0, const ImgView& image0
     }
     if (tape) tape->up[2] = raw_view(feat);
     if (tc_tail) {
-        View fv = feat.h;                                 // f16 data + the statistics slot of the tensor
-        fv.stats = feat.f.stats; fv.stats_ld = feat.f.stats_ld; fv.stats_rep = feat.f.stats_rep; fv.stats_rep_stride = feat.f.stats_rep_stride;
+        const View fv = with_stats(feat.h, feat.f);       // f16 data + the statistics slot of the tensor
         NormSpecTail ns; ns.groups = 0; ns.act = ACT_RELU; ns.gamma = up_n_[2].gamma; ns.beta = up_n_[2].beta;
         // the network's own NHWC input holds interleaved copies of the image(s) the tail samples (combiner: [background | eyebrow])
         const View g0 = kind_ == TAIL_COMBINER ? x0.slice(4, 4) : x0.slice(0, 4);
@@ -463,7 +456,22 @@ void EncDecNet::forward_fused(Runtime& rt, const View& x0, const ImgView& image0
 
 // ------------------------------------------------------------------------------------------------ UNetNet
 UNetNet::UNetNet(bool upscaler, int size, int model_channels, std::vector<int> mults)
-    : upscaler_(upscaler), S_(size), mc_(model_channels), L_((int)mults.size()), mults_(std::move(mults)) {}
+    : upscaler_(upscaler), S_(size), mc_(model_channels), L_((int)mults.size()), mults_(std::move(mults)), cat_h_(2 * L_),
+      cat_skip_(2 * L_) {
+    // the skip tensors hs[k] in down-path order: the first conv's output, then per level its ResBlock's and (but on the last
+    // level) its down-sampler's
+    std::vector<int> hs_ch(2 * L_);
+    hs_ch[0] = mc_;
+    for (int i = 0; i < L_; ++i) {
+        hs_ch[2 * i + 1] = mc_ * mults_[i];
+        if (i < L_ - 1) hs_ch[2 * i + 2] = mc_ * mults_[i];
+    }
+    for (int j = 0; j < 2 * L_; ++j) {
+        const int lvl = L_ - 1 - j / 2;
+        cat_h_[j] = (j == 0) ? mc_ * mults_[L_ - 1] : ((j & 1) ? mc_ * mults_[lvl] : mc_ * mults_[lvl + 1]);
+        cat_skip_[j] = hs_ch[2 * L_ - 1 - j];
+    }
+}
 
 namespace {
 
@@ -548,6 +556,10 @@ void UNetNet::load(const StateDict& sd, cudaStream_t s) {
             up_us_[bi] = load_res_block(sd, bp + ".upsample", s, true);
             all_blocks.push_back({&up_us_[bi], bp + ".upsample"});
         }
+    }
+    for (int j = 0; j < 2 * L_; ++j) {
+        THA4_REQUIRE(cat_h_[j] + cat_skip_[j] == up_res_[j].cin, "unet: concat plan does not match weights");
+        THA4_REQUIRE(up_res_[j].has_skip, "unet: an up ResBlock reads its concatenation through a 1x1 skip (no fp32 residual)");
     }
     last_n_ = load_norm(sd, p + "last.0", s);
     tail_init(tail_, mc_, s);
@@ -649,15 +661,14 @@ void UNetNet::res_block(Runtime& rt, const ResBlockW& w, const View& x, int mode
     const int B = x.N;
     // norm0 -> SiLU -> (avg-pool) ; the nearest-upsample is folded into conv0's gather
     const int th = (mode == 2) ? x.H / 2 : x.H;
-    const bool h16 = rt.f16 != 0;
     const bool ops = tape && tape->ops;          // the normalised operands stay for the weight gradients
     Pool* op_pool = ops ? rt.persist : rt.scratch;
-    View t0 = h16 ? make_view16(op_pool, B, th, th, w.cin) : make_view(op_pool, B, th, th, w.cin);
+    View t0 = make_view(op_pool, B, th, th, w.cin);
     run_norm(rt, x, w.norm0, 32, nullptr, nullptr, 0, rt.strict ? ACT_SILU : ACT_SILU_FAST, mode == 2 ? 1 : 0, nullptr, t0);
     View h = make_view(tape ? rt.persist : rt.scratch, B, out.H, out.W, w.cout, &rt);
     run_conv(rt, w.conv0, t0, h);      // mode 1: conv0 was packed as CONV_UP2_3x3 (upsample folded into 4 phases)
     // norm1 -> FiLM(time) -> FiLM(pose) -> SiLU, folded into one per-(n,c) affine
-    const View h2 = h16 ? make_view16(op_pool, B, out.H, out.W, w.cout) : (tape ? make_view(op_pool, B, out.H, out.W, w.cout) : h);
+    const View h2 = tape ? make_view(op_pool, B, out.H, out.W, w.cout) : h;
     if (tape) tape->res[&w] = {x, h, ops ? t0 : View{}, ops ? h2 : View{}};
     run_norm(rt, h, w.norm1, 32, w.film0, film1 + w.film1_off, film1_total_, rt.strict ? ACT_SILU : ACT_SILU_FAST, 0, nullptr, h2);
     if (w.has_skip) {
@@ -676,7 +687,7 @@ void UNetNet::attn_block(Runtime& rt, const AttnW& w, const View& x, const View&
     rt.scratch->reset();
     const bool ops = tape && tape->ops;
     Pool* op_pool = ops ? rt.persist : rt.scratch;
-    View t = rt.f16 ? make_view16(op_pool, x.N, x.H, x.W, x.C) : make_view(op_pool, x.N, x.H, x.W, x.C);
+    View t = make_view(op_pool, x.N, x.H, x.W, x.C);
     run_norm(rt, x, w.norm, 32, nullptr, nullptr, 0, ACT_NONE, 0, nullptr, t);
     View qkv = make_view(tape ? rt.persist : rt.scratch, x.N, x.H, x.W, 3 * x.C);
     run_conv(rt, w.qkv, t, qkv);
@@ -715,24 +726,13 @@ void UNetNet::forward(Runtime& rt, const ImgView& image, const float* coarse_pos
     }
     if (tape) tape->x0 = x0;
 
-    // ---- plan the skip concatenations: up res-block j reads cat(h_j, hs[2L-1-j]) from one buffer ----
+    // ---- the skip concatenations: up res-block j reads cat(h_j, hs[2L-1-j]) from one buffer ----
     const int NH = 2 * L_;
-    std::vector<int> hs_ch(NH);
-    hs_ch[0] = mc_;
-    for (int i = 0; i < L_; ++i) {
-        hs_ch[2 * i + 1] = mc_ * mults_[i];
-        if (i < L_ - 1) hs_ch[2 * i + 2] = mc_ * mults_[i];
-    }
     std::vector<View> cat(NH), hs(NH);
-    std::vector<int> ch_h(NH);
     for (int j = 0; j < NH; ++j) {
-        const int lvl = L_ - 1 - j / 2;
-        const int sp = S_ >> lvl;
-        ch_h[j] = (j == 0) ? mc_ * mults_[L_ - 1] : ((j & 1) ? mc_ * mults_[lvl] : mc_ * mults_[lvl + 1]);
-        const int cs = hs_ch[NH - 1 - j];
-        THA4_REQUIRE(ch_h[j] + cs == up_res_[j].cin, "unet: concat plan does not match weights");
-        cat[j] = make_view(P, B, sp, sp, ch_h[j] + cs, &rt);
-        hs[NH - 1 - j] = cat[j].slice(ch_h[j], cs);
+        const int sp = S_ >> (L_ - 1 - j / 2);
+        cat[j] = make_view(P, B, sp, sp, cat_h_[j] + cat_skip_[j], &rt);
+        hs[NH - 1 - j] = cat[j].slice(cat_h_[j], cat_skip_[j]);
     }
 
     // ---- down path (unet.py:534-536) ----
@@ -755,7 +755,7 @@ void UNetNet::forward(Runtime& rt, const ImgView& image, const float* coarse_pos
     // ---- middle: Res, Attn, Res, Attn, Res, Attn, Res (unet.py:481-498) ----
     for (int j = 0; j < 4; ++j) {
         const bool last = (j == 3);
-        View r = last ? cat[0].slice(0, ch_h[0]) : make_view(P, B, cur.H, cur.W, cur.C, &rt);
+        View r = last ? cat[0].slice(0, cat_h_[0]) : make_view(P, B, cur.H, cur.W, cur.C, &rt);
         res_block(rt, mid_res_[j], cur, 0, film1, r, tape);
         cur = r;
         if (!last) {
@@ -771,7 +771,7 @@ void UNetNet::forward(Runtime& rt, const ImgView& image, const float* coarse_pos
         const bool second = (j & 1);
         const int co = up_res_[j].cout;
         View dst;
-        if (!second) dst = cat[j + 1].slice(0, ch_h[j + 1]);
+        if (!second) dst = cat[j + 1].slice(0, cat_h_[j + 1]);
         else dst = make_view(P, B, cat[j].H, cat[j].W, co, &rt);      // goes to the upsampler or is the final feature
         if (lvl == L_ - 1) {
             View tmp = make_view(P, B, cat[j].H, cat[j].W, co, &rt);
@@ -781,7 +781,7 @@ void UNetNet::forward(Runtime& rt, const ImgView& image, const float* coarse_pos
             res_block(rt, up_res_[j], cat[j], 0, film1, dst, tape);
         }
         if (second) {
-            if (lvl > 0) res_block(rt, up_us_[L_ - 1 - lvl], dst, 1, film1, cat[j + 1].slice(0, ch_h[j + 1]), tape);
+            if (lvl > 0) res_block(rt, up_us_[L_ - 1 - lvl], dst, 1, film1, cat[j + 1].slice(0, cat_h_[j + 1]), tape);
             else feat = dst;
         }
     }
@@ -800,12 +800,7 @@ void UNetNet::forward(Runtime& rt, const ImgView& image, const float* coarse_pos
 namespace {
 
 // a normalisation's input as the fused consumer conv reads it: the f16 operand copy when there is one, with the statistics
-View op_view(const Tens& a) {
-    if (!a.h.p) return a.f;
-    View v = a.h;
-    v.stats = a.f.stats; v.stats_ld = a.f.stats_ld; v.stats_rep = a.f.stats_rep; v.stats_rep_stride = a.f.stats_rep_stride;
-    return v;
-}
+View op_view(const Tens& a) { return a.h.p ? with_stats(a.h, a.f) : a.f; }
 
 struct UNetFused {
     Runtime& rt;
@@ -921,25 +916,13 @@ void UNetNet::forward_fused(Runtime& rt, const ImgView& image, const float* coar
     }
     if (tape) tape->x0 = x0;
 
-    // ---- plan the skip concatenations: up res-block j reads cat(h_j, hs[2L-1-j]) from one buffer (both precisions) ----
+    // ---- the skip concatenations: up res-block j reads cat(h_j, hs[2L-1-j]) from one buffer (both precisions) ----
     const int NH = 2 * L_;
-    std::vector<int> hs_ch(NH);
-    hs_ch[0] = mc_;
-    for (int i = 0; i < L_; ++i) {
-        hs_ch[2 * i + 1] = mc_ * mults_[i];
-        if (i < L_ - 1) hs_ch[2 * i + 2] = mc_ * mults_[i];
-    }
     std::vector<Tens> cat(NH), hs(NH);
-    std::vector<int> ch_h(NH);
     for (int j = 0; j < NH; ++j) {
-        const int lvl = L_ - 1 - j / 2;
-        const int sp = S_ >> lvl;
-        ch_h[j] = (j == 0) ? mc_ * mults_[L_ - 1] : ((j & 1) ? mc_ * mults_[lvl] : mc_ * mults_[lvl + 1]);
-        const int cs = hs_ch[NH - 1 - j];
-        THA4_REQUIRE(ch_h[j] + cs == up_res_[j].cin, "unet: concat plan does not match weights");
-        THA4_REQUIRE(up_res_[j].has_skip, "unet: an up ResBlock reads its concatenation through a 1x1 skip (no fp32 residual)");
-        cat[j] = make_act(P, rt, B, sp, sp, ch_h[j] + cs, true, true);
-        hs[NH - 1 - j] = slice_act(cat[j], ch_h[j], cs);
+        const int sp = S_ >> (L_ - 1 - j / 2);
+        cat[j] = make_act(P, rt, B, sp, sp, cat_h_[j] + cat_skip_[j], true, true);
+        hs[NH - 1 - j] = slice_act(cat[j], cat_h_[j], cat_skip_[j]);
     }
 
     // ---- down path (unet.py:534-536) ----
@@ -964,7 +947,7 @@ void UNetNet::forward_fused(Runtime& rt, const ImgView& image, const float* coar
     // ---- middle: Res, Attn, Res, Attn, Res, Attn, Res (unet.py:481-498) ----
     for (int j = 0; j < 4; ++j) {
         const bool last = (j == 3);
-        Tens r = last ? f16_only(slice_act(cat[0], 0, ch_h[0])) : make_act(P, rt, B, cur.f.H, cur.f.W, cur.f.C, true, true);
+        Tens r = last ? f16_only(slice_act(cat[0], 0, cat_h_[0])) : make_act(P, rt, B, cur.f.H, cur.f.W, cur.f.C, true, true);
         F.res_block(mid_res_[j], cur, 0, r);
         cur = r;
         if (!last) {
@@ -983,7 +966,7 @@ void UNetNet::forward_fused(Runtime& rt, const ImgView& image, const float* coar
         const bool second = (j & 1);
         const int co = up_res_[j].cout;
         Tens dst;
-        if (!second) dst = f16_only(slice_act(cat[j + 1], 0, ch_h[j + 1]));
+        if (!second) dst = f16_only(slice_act(cat[j + 1], 0, cat_h_[j + 1]));
         else dst = make_act(P, rt, B, cat[j].f.H, cat[j].f.W, co, lvl > 0 || !tc_tail, true);   // goes to the upsampler or is the final feature
         if (lvl == L_ - 1) {
             Tens tmp = make_act(P, rt, B, cat[j].f.H, cat[j].f.W, co, true, true);
@@ -993,7 +976,7 @@ void UNetNet::forward_fused(Runtime& rt, const ImgView& image, const float* coar
             F.res_block(up_res_[j], cat[j], 0, dst);
         }
         if (second) {
-            if (lvl > 0) F.res_block(up_us_[L_ - 1 - lvl], dst, 1, f16_only(slice_act(cat[j + 1], 0, ch_h[j + 1])));
+            if (lvl > 0) F.res_block(up_us_[L_ - 1 - lvl], dst, 1, f16_only(slice_act(cat[j + 1], 0, cat_h_[j + 1])));
             else feat = dst;
         }
     }
@@ -1001,8 +984,7 @@ void UNetNet::forward_fused(Runtime& rt, const ImgView& image, const float* coar
     rt.scratch->reset();
     ImgView none{};
     if (tc_tail) {
-        View fv = feat.h;
-        fv.stats = feat.f.stats; fv.stats_ld = feat.f.stats_ld; fv.stats_rep = feat.f.stats_rep; fv.stats_rep_stride = feat.f.stats_rep_stride;
+        const View fv = with_stats(feat.h, feat.f);
         NormSpecTail ns; ns.groups = 32; ns.act = ACT_SILU_FAST; ns.gamma = last_n_.gamma; ns.beta = last_n_.beta;
         if (tape) tape->feat = fv;
         const View g0 = x0.slice(0, 4);       // channels 0-3 of the network input are the image the tail warps (Upscaler02: the rest image)

@@ -50,6 +50,10 @@ struct Runtime {                      // per-call execution context
     double* alloc_stats(size_t n);
 };
 
+// An NHWC fp32 tensor from `pool`.  rt != nullptr: it also gets a zeroed statistics slot (View::stats), to be filled by the
+// conv that produces the tensor.
+View make_view(Pool* pool, int N, int H, int W, int C, Runtime* rt = nullptr);
+
 // The flat parameter-gradient layout of a network: the offset of each state_dict tensor in a buffer of `total` floats, in
 // the order add() registered them (the reference's state_dict order).
 struct ParamLayout {
@@ -105,7 +109,6 @@ public:
     // then runs the adjoint of every layer back to the inputs that were asked for.
     void backward(Runtime& rt, const ImgView& image0, const ImgView& image1, const float* pose, int pose_ld, const EncDecGrads& g);
     int size() const { return S_; }
-    int num_outputs() const { return kind_ == TAIL_DECOMPOSER ? 6 : 8; }
     // floats of the network's parameters, and the offset of a state_dict key's tensor in the flat state_dict-order buffer
     long param_count() const { return params_.total; }
     long param_offset(const std::string& key) const { return params_.offset(key); }
@@ -223,6 +226,8 @@ private:
     bool upscaler_;
     int S_, mc_, L_;
     std::vector<int> mults_;
+    // the skip concatenations: up ResBlock j reads cat(h_j, hs[2L-1-j]) from one buffer of cat_h_[j] + cat_skip_[j] channels
+    std::vector<int> cat_h_, cat_skip_;
     bool loaded_ = false;
     ConvWeights first_;
     std::vector<ResBlockW> down_res_, down_ds_, mid_res_, up_res_, up_us_;   // up_res_: 2 per level
@@ -239,6 +244,10 @@ private:
 };
 
 // ------------------------------------------------------------------ backward helpers shared by the networks
+// A gradient tensor: an NHWC fp32 tensor without a statistics slot.
+inline View fresh(Pool* P, int N, int H, int W, int C) { return make_view(P, N, H, W, C); }
+// CTAs of 256 threads for a grid-stride loop over n elements: at most 16 per SM of an H100 (132 SMs).
+inline int backward_grid(long n) { return (int)std::max<long>(1, std::min<long>((n + 255) / 256, 132L * 16)); }
 // Data gradient of a conv on the conv kernels: dx = conv(dy) with adjoint-packed weights (+ add, same resolution).
 void run_dgrad(Runtime& rt, const ConvWeights& cw, const View& dy, const View& dx, const View* add = nullptr);
 // The fused tail's head conv (tw.w) as one packed 3x3 conv from its 16-channel head-gradient tensor to the tw.C features.

@@ -76,6 +76,20 @@ void base_grid_host(int W, float* out);
 
 // ---------------------------------------------------------------- fused decoder tails (tail.cu)
 enum TailKind { TAIL_UNET = 0, TAIL_DECOMPOSER = 1, TAIL_COMBINER = 2, TAIL_FACE = 3 };
+// What each kind's tail returns, indexed by TailKind: the count of its outputs and the channels of each, in the order the
+// tail writes them (NCHW, at the network's resolution).
+constexpr int TAIL_MAX_OUTPUTS = 8;
+struct TailOutputs {
+    int count;
+    int ch[TAIL_MAX_OUTPUTS];
+    constexpr int channels() const { int c = 0; for (int i = 0; i < count; ++i) c += ch[i]; return c; }
+};
+constexpr TailOutputs TAIL_OUTPUTS[4] = {
+    {5, {4, 1, 4, 2, 4}},                 // TAIL_UNET
+    {6, {4, 1, 4, 4, 1, 4}},              // TAIL_DECOMPOSER
+    {8, {4, 1, 4, 4, 1, 4, 4, 2}},        // TAIL_COMBINER
+    {8, {4, 1, 4, 4, 1, 4, 4, 2}},        // TAIL_FACE
+};
 struct TailWeights {
     float* w = nullptr;      // [9][C][CO_PAD] fp32
     float* bias = nullptr;   // [CO_PAD]

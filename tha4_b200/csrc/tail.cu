@@ -178,19 +178,18 @@ __global__ void __launch_bounds__(TAIL_THREADS) tail_kernel(const float* __restr
 
 template <int KIND, int NT, bool STRICT>
 void launch_tail(const TailWeights& tw, const View& f, const float* coef, int act, const ImgView& i0, const ImgView& i1,
-                 float* const* o, int nout, cudaStream_t s) {
+                 float* const* o, cudaStream_t s) {
     THA4_REQUIRE(tw.C % 8 == 0 && tw.CO <= NT * 8, "tail: head channel layout");
     const size_t halo = (size_t)HALO_H * HALO * (tw.C + 4), outs = (size_t)TILE * TILE_H * OPITCH;
     const size_t smem = ((size_t)9 * tw.C * wpitch(NT) + std::max(halo, outs)) * sizeof(float);
     THA4_ENSURE_SMEM((tail_kernel<KIND, NT, STRICT>), smem);
     float* op[8];
-    for (int i = 0; i < 8; ++i) op[i] = i < nout ? o[i] : nullptr;
+    for (int i = 0; i < 8; ++i) op[i] = i < TAIL_OUTPUTS[KIND].count ? o[i] : nullptr;
     dim3 grid(f.W / TILE, f.H / TILE_H, f.N);
     ProfScope prof(PROF_TAIL, s);
     {   // compulsory traffic: feature map + 4-channel image(s) read once, every returned tensor written once (SURVEY 8d)
-        const int out_ch[4] = {15, 18, 24, 24};
         const int img_ch = (KIND == TAIL_COMBINER) ? 8 : 4;
-        prof_add_work(PROF_TAIL, 2.0 * f.pixels() * 9 * tw.C * tw.CO, (double)f.pixels() * (f.C + img_ch + out_ch[KIND]) * 4);
+        prof_add_work(PROF_TAIL, 2.0 * f.pixels() * 9 * tw.C * tw.CO, (double)f.pixels() * (f.C + img_ch + TAIL_OUTPUTS[KIND].channels()) * 4);
     }
     tail_kernel<KIND, NT, STRICT><<<grid, TAIL_THREADS, smem, s>>>(f.p, f.H, f.C, f.ld, coef, act, tw.w, tw.bias, i0, i1,
                                              base_grid_table(f.H), op[0], op[1], op[2], op[3], op[4], op[5], op[6], op[7]);
@@ -231,20 +230,20 @@ void tail_forward(TailKind kind, const TailWeights& tw, const View& feature, con
     THA4_REQUIRE(image0.H == feature.H && image0.W == feature.W && image0.C == 4, "tail: image dims");
     switch (kind) {
         case TAIL_UNET:
-            if (strict) launch_tail<TAIL_UNET, 1, true>(tw, feature, coef, act, image0, image1, outputs, 5, s);
-            else launch_tail<TAIL_UNET, 1, false>(tw, feature, coef, act, image0, image1, outputs, 5, s);
+            if (strict) launch_tail<TAIL_UNET, 1, true>(tw, feature, coef, act, image0, image1, outputs, s);
+            else launch_tail<TAIL_UNET, 1, false>(tw, feature, coef, act, image0, image1, outputs, s);
             break;
         case TAIL_DECOMPOSER:
-            if (strict) launch_tail<TAIL_DECOMPOSER, 2, true>(tw, feature, coef, act, image0, image1, outputs, 6, s);
-            else launch_tail<TAIL_DECOMPOSER, 2, false>(tw, feature, coef, act, image0, image1, outputs, 6, s);
+            if (strict) launch_tail<TAIL_DECOMPOSER, 2, true>(tw, feature, coef, act, image0, image1, outputs, s);
+            else launch_tail<TAIL_DECOMPOSER, 2, false>(tw, feature, coef, act, image0, image1, outputs, s);
             break;
         case TAIL_COMBINER:
-            if (strict) launch_tail<TAIL_COMBINER, 1, true>(tw, feature, coef, act, image0, image1, outputs, 8, s);
-            else launch_tail<TAIL_COMBINER, 1, false>(tw, feature, coef, act, image0, image1, outputs, 8, s);
+            if (strict) launch_tail<TAIL_COMBINER, 1, true>(tw, feature, coef, act, image0, image1, outputs, s);
+            else launch_tail<TAIL_COMBINER, 1, false>(tw, feature, coef, act, image0, image1, outputs, s);
             break;
         case TAIL_FACE:
-            if (strict) launch_tail<TAIL_FACE, 2, true>(tw, feature, coef, act, image0, image1, outputs, 8, s);
-            else launch_tail<TAIL_FACE, 2, false>(tw, feature, coef, act, image0, image1, outputs, 8, s);
+            if (strict) launch_tail<TAIL_FACE, 2, true>(tw, feature, coef, act, image0, image1, outputs, s);
+            else launch_tail<TAIL_FACE, 2, false>(tw, feature, coef, act, image0, image1, outputs, s);
             break;
     }
 }

@@ -556,7 +556,7 @@ __global__ void tail_absmax_kernel(const float* __restrict__ w, int n, unsigned*
 }
 
 template <int KIND, int C>
-void launch_tail_tc(const TailWeights& tw, const View& f, const NormSpecTail& ns, const ImgView& i0, const ImgView& i1, float* const* o, int nout,
+void launch_tail_tc(const TailWeights& tw, const View& f, const NormSpecTail& ns, const ImgView& i0, const ImgView& i1, float* const* o,
                     cudaStream_t s) {
     using Cfg = TailCfg<C>;
     TailTcParams p{};
@@ -565,21 +565,20 @@ void launch_tail_tc(const TailWeights& tw, const View& f, const NormSpecTail& ns
     p.groups = ns.groups; p.act = ns.act; p.gamma = ns.gamma; p.beta = ns.beta;
     p.bias = tw.bias; p.acc_scale = 1.0f / tw.w16_scale;
     p.img0 = i0; p.img1 = i1; p.base = base_grid_table(f.H);
-    for (int i = 0; i < 8; ++i) p.o[i] = i < nout ? o[i] : nullptr;
+    for (int i = 0; i < 8; ++i) p.o[i] = i < TAIL_OUTPUTS[KIND].count ? o[i] : nullptr;
     THA4_ENSURE_SMEM((tail_tc_kernel<KIND, C>), Cfg::SMEM);
     dim3 grid(ceil_div(f.W, TT_W), f.H / Cfg::TR, f.N);
     ProfScope prof(PROF_TAIL, s);
     {   // compulsory traffic as SURVEY 8d defines it (fp32 element size): feature map + image(s) read once, every returned tensor written once
-        const int out_ch[4] = {15, 18, 24, 24};
         const int img_ch = (KIND == TAIL_COMBINER) ? 8 : 4;
-        prof_add_work(PROF_TAIL, 2.0 * f.pixels() * 9 * tw.C * tw.CO, (double)f.pixels() * (f.C + img_ch + out_ch[KIND]) * 4);
+        prof_add_work(PROF_TAIL, 2.0 * f.pixels() * 9 * tw.C * tw.CO, (double)f.pixels() * (f.C + img_ch + TAIL_OUTPUTS[KIND].channels()) * 4);
     }
     launch_pdl(tail_tc_kernel<KIND, C>, grid, dim3(TT_THREADS), Cfg::SMEM, s, 1, feature_map(f, Cfg::TR), head_weight_map(tw), p);
     THA4_LAUNCH_CHECK();
 }
 
 template <int KIND, int C, int TR>
-void launch_tail_persist(const TailWeights& tw, const View& f, const NormSpecTail& ns, const ImgView& i0, const ImgView& i1, float* const* o, int nout,
+void launch_tail_persist(const TailWeights& tw, const View& f, const NormSpecTail& ns, const ImgView& i0, const ImgView& i1, float* const* o,
                          cudaStream_t s, const View* g0, const View* g1) {
     using Cfg = TailPCfg<C, TR>;
     TailTcParams p{};
@@ -594,35 +593,34 @@ void launch_tail_persist(const TailWeights& tw, const View& f, const NormSpecTai
     };
     if (gather_ok(g0)) { p.g0 = g0->p; p.g0_ld = g0->ld; }
     if (gather_ok(g1)) { p.g1 = g1->p; p.g1_ld = g1->ld; }
-    for (int i = 0; i < 8; ++i) p.o[i] = i < nout ? o[i] : nullptr;
+    for (int i = 0; i < 8; ++i) p.o[i] = i < TAIL_OUTPUTS[KIND].count ? o[i] : nullptr;
     THA4_REQUIRE(f.H <= Cfg::MAX_S, "tail_tc: image size");
     THA4_ENSURE_SMEM((tail_tc_persist_kernel<KIND, C, TR>), Cfg::SMEM);
     const long total = (long)ceil_div(f.W, TT_W) * (f.H / TR) * f.N;
     dim3 grid((unsigned)std::min<long>(total, num_sms()));
     ProfScope prof(PROF_TAIL, s);
     {   // compulsory traffic as SURVEY 8d defines it (fp32 element size): feature map + image(s) read once, every returned tensor written once
-        const int out_ch[4] = {15, 18, 24, 24};
         const int img_ch = (KIND == TAIL_COMBINER) ? 8 : 4;
-        prof_add_work(PROF_TAIL, 2.0 * f.pixels() * 9 * tw.C * tw.CO, (double)f.pixels() * (f.C + img_ch + out_ch[KIND]) * 4);
+        prof_add_work(PROF_TAIL, 2.0 * f.pixels() * 9 * tw.C * tw.CO, (double)f.pixels() * (f.C + img_ch + TAIL_OUTPUTS[KIND].channels()) * 4);
     }
     launch_pdl(tail_tc_persist_kernel<KIND, C, TR>, grid, dim3(Cfg::THREADS), Cfg::SMEM, s, 1, feature_map(f, TR), head_weight_map(tw), p);
     THA4_LAUNCH_CHECK();
 }
 
 template <int KIND>
-void launch_tail_tc_c(const TailWeights& tw, const View& f, const NormSpecTail& ns, const ImgView& i0, const ImgView& i1, float* const* o, int nout,
+void launch_tail_tc_c(const TailWeights& tw, const View& f, const NormSpecTail& ns, const ImgView& i0, const ImgView& i1, float* const* o,
                       cudaStream_t s, const View* g0, const View* g1) {
     if (opts().tail_persist) {
         // tile rows per step (32-channel sites): 4 when that still gives every SM two tiles or more, else 2 (more, smaller tiles:
         // the small sites at B = 1 are one latency chain per CTA)
         const long tiles4 = (long)ceil_div(f.W, TT_W) * (f.H / 4) * f.N;
         const bool tr4 = tiles4 >= 2L * num_sms();
-        if (tw.C == 32) { if (tr4) launch_tail_persist<KIND, 32, 4>(tw, f, ns, i0, i1, o, nout, s, g0, g1); else launch_tail_persist<KIND, 32, 2>(tw, f, ns, i0, i1, o, nout, s, g0, g1); }
-        else            launch_tail_persist<KIND, 64, 2>(tw, f, ns, i0, i1, o, nout, s, g0, g1);        // two halo slots of 66 KB
+        if (tw.C == 32) { if (tr4) launch_tail_persist<KIND, 32, 4>(tw, f, ns, i0, i1, o, s, g0, g1); else launch_tail_persist<KIND, 32, 2>(tw, f, ns, i0, i1, o, s, g0, g1); }
+        else            launch_tail_persist<KIND, 64, 2>(tw, f, ns, i0, i1, o, s, g0, g1);        // two halo slots of 66 KB
         return;
     }
-    if (tw.C == 32) launch_tail_tc<KIND, 32>(tw, f, ns, i0, i1, o, nout, s);
-    else launch_tail_tc<KIND, 64>(tw, f, ns, i0, i1, o, nout, s);
+    if (tw.C == 32) launch_tail_tc<KIND, 32>(tw, f, ns, i0, i1, o, s);
+    else launch_tail_tc<KIND, 64>(tw, f, ns, i0, i1, o, s);
 }
 
 }  // namespace
@@ -661,10 +659,10 @@ void tail_tc_forward(TailKind kind, const TailWeights& tw, const View& feature, 
     THA4_REQUIRE(image0.H == feature.H && image0.W == feature.W && image0.C == 4, "tail_tc: image dims");
     THA4_REQUIRE(ns.groups == 0 || tw.C % ns.groups == 0, "tail_tc: groups");
     switch (kind) {
-        case TAIL_UNET: launch_tail_tc_c<TAIL_UNET>(tw, feature, ns, image0, image1, outputs, 5, s, g0, g1); break;
-        case TAIL_DECOMPOSER: launch_tail_tc_c<TAIL_DECOMPOSER>(tw, feature, ns, image0, image1, outputs, 6, s, g0, g1); break;
-        case TAIL_COMBINER: launch_tail_tc_c<TAIL_COMBINER>(tw, feature, ns, image0, image1, outputs, 8, s, g0, g1); break;
-        case TAIL_FACE: launch_tail_tc_c<TAIL_FACE>(tw, feature, ns, image0, image1, outputs, 8, s, g0, g1); break;
+        case TAIL_UNET: launch_tail_tc_c<TAIL_UNET>(tw, feature, ns, image0, image1, outputs, s, g0, g1); break;
+        case TAIL_DECOMPOSER: launch_tail_tc_c<TAIL_DECOMPOSER>(tw, feature, ns, image0, image1, outputs, s, g0, g1); break;
+        case TAIL_COMBINER: launch_tail_tc_c<TAIL_COMBINER>(tw, feature, ns, image0, image1, outputs, s, g0, g1); break;
+        case TAIL_FACE: launch_tail_tc_c<TAIL_FACE>(tw, feature, ns, image0, image1, outputs, s, g0, g1); break;
     }
 }
 

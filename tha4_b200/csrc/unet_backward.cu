@@ -32,14 +32,6 @@ namespace tha4 {
 
 namespace {
 
-int grid_for(long n) { return (int)std::max<long>(1, std::min<long>((n + 255) / 256, 132L * 16)); }
-
-View fresh(Pool* P, int N, int H, int W, int C) {
-    View v; v.N = N; v.H = H; v.W = W; v.C = C; v.ld = C;
-    v.p = P->alloc((size_t)N * H * W * C);
-    return v;
-}
-
 // ------------------------------------------------------------------------------------------------ adjoint packing
 struct TapMap { int src[CONV_MAX_TAPS]; };    // adjoint tap -> forward (phase * ntaps + tap)
 
@@ -501,7 +493,7 @@ void conv_adjoint_from_packed(ConvWeights& cw, const ConvWeights& fwd, ConvKind 
     THA4_CUDA_CHECK(cudaMemsetAsync(cw.w, 0, conv_packed_floats(cw) * sizeof(float), s));
     cw.tf32_rounded = fwd.tf32_rounded;
     const long total = (long)cw.ntaps * cw.cout * cw.cin;
-    adjoint_from_packed_kernel<<<grid_for(total), 256, 0, s>>>(cw.w, fwd.w, m, cw.ntaps, cw.cout, cw.cin, cw.cout_pad, cw.cin_pad,
+    adjoint_from_packed_kernel<<<backward_grid(total), 256, 0, s>>>(cw.w, fwd.w, m, cw.ntaps, cw.cout, cw.cin, cw.cout_pad, cw.cin_pad,
                                                               fwd.cout_pad, fwd.cin_pad);
     THA4_LAUNCH_CHECK();
 }
@@ -540,8 +532,8 @@ void group_norm_backward(const View& x, int groups, const float* gamma, const fl
     THA4_LAUNCH_CHECK();
     gn_bwd_finalize_kernel<<<x.N, 256, 0, s>>>(a);
     THA4_LAUNCH_CHECK();
-    if (x.f16) gn_bwd_apply_kernel<true><<<grid_for(total), 256, 0, s>>>(a, total);
-    else gn_bwd_apply_kernel<false><<<grid_for(total), 256, 0, s>>>(a, total);
+    if (x.f16) gn_bwd_apply_kernel<true><<<backward_grid(total), 256, 0, s>>>(a, total);
+    else gn_bwd_apply_kernel<false><<<backward_grid(total), 256, 0, s>>>(a, total);
     THA4_LAUNCH_CHECK();
 }
 
@@ -584,7 +576,7 @@ void channel_sums(const float* x, int ld, long pixels, int C, float* out, float*
 
 void linear_wgrad(const float* dy, int dy_ld, int N, int R, const float* x, int x_ld, int K, int silu_x, float* dW, float* db,
                   int accumulate, cudaStream_t s) {
-    linear_wgrad_kernel<<<grid_for((long)R * K), 256, 0, s>>>(dy, dy_ld, N, R, x, x_ld, K, silu_x, dW, db, accumulate);
+    linear_wgrad_kernel<<<backward_grid((long)R * K), 256, 0, s>>>(dy, dy_ld, N, R, x, x_ld, K, silu_x, dW, db, accumulate);
     THA4_LAUNCH_CHECK();
 }
 
@@ -633,9 +625,9 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
     Pool* P = rt.persist;
 
     // forward with a tape; its outputs are what the tail backward differentiates through
-    static const int kCh[5] = {4, 1, 4, 2, 4};
-    float* outs[5];
-    for (int k = 0; k < 5; ++k) outs[k] = P->alloc((size_t)B * kCh[k] * S * S);
+    const TailOutputs& to = TAIL_OUTPUTS[TAIL_UNET];
+    float* outs[TAIL_MAX_OUTPUTS];
+    for (int k = 0; k < to.count; ++k) outs[k] = P->alloc((size_t)B * to.ch[k] * S * S);
     UNetTape tape;
     tape.ops = want_par;
     forward(rt, image, coarse_posed, coarse_grid, coarse_size, pose, pose_ld, outs, &tape);
@@ -765,27 +757,22 @@ void UNetNet::backward(Runtime& rt, const ImgView& image, const float* coarse_po
     gn(tape.feat, last_n_, nullptr, nullptr, ACT_SILU, df, 0, dfeat, nullptr, RES_NONE, nullptr, p + "last.0");
 
     // ---- up path in reverse: dcat[j] = gradient of up ResBlock j's input cat(h_j, hs[NH-1-j]) ----
-    std::vector<int> ch_h(NH);
-    for (int j = 0; j < NH; ++j) {
-        const int lvl = L_ - 1 - j / 2;
-        ch_h[j] = (j == 0) ? mc_ * mults_[L_ - 1] : ((j & 1) ? mc_ * mults_[lvl] : mc_ * mults_[lvl + 1]);
-    }
     std::vector<View> dcat(NH);
     for (int j = NH - 1; j >= 0; --j) {
         const int lvl = L_ - 1 - j / 2;
         const bool second = (j & 1);
         View d_dst;
-        if (!second) d_dst = dcat[j + 1].slice(0, ch_h[j + 1]);
-        else if (lvl > 0) d_dst = res_bwd(up_us_[L_ - 1 - lvl], 1, dcat[j + 1].slice(0, ch_h[j + 1]), nullptr, true);
+        if (!second) d_dst = dcat[j + 1].slice(0, cat_h_[j + 1]);
+        else if (lvl > 0) d_dst = res_bwd(up_us_[L_ - 1 - lvl], 1, dcat[j + 1].slice(0, cat_h_[j + 1]), nullptr, true);
         else d_dst = dfeat;
         if (lvl == L_ - 1) d_dst = attn_bwd(up_attn_[second ? 1 : 0], d_dst);
         dcat[j] = res_bwd(up_res_[j], 0, d_dst, nullptr, true);
     }
     // the cat half of the gradient of skip tensor hs[k] (joined in its down-path consumer's last adjoint)
-    auto dhs = [&](int k) { const View& d = dcat[NH - 1 - k]; return d.slice(ch_h[NH - 1 - k], d.C - ch_h[NH - 1 - k]); };
+    auto dhs = [&](int k) { const int j = NH - 1 - k; return dcat[j].slice(cat_h_[j], cat_skip_[j]); };
 
     // ---- middle in reverse: Res, Attn, Res, Attn, Res, Attn, Res ----
-    View dm = dcat[0].slice(0, ch_h[0]);
+    View dm = dcat[0].slice(0, cat_h_[0]);
     for (int j = 3; j >= 0; --j) {
         const View extra = dhs(NH - 1);
         dm = res_bwd(mid_res_[j], 0, dm, j == 0 ? &extra : nullptr, true);
